@@ -38,13 +38,13 @@ def workload_config(n_gpus, precision="split", input_dtype="float32"):
             "frame": [H, W, 3], "batch_per_gpu": BATCH, "global_batch": BATCH * n_gpus, "num_class": 15,
             "rpn_topk": 300, "precision": precision, "input_dtype": input_dtype,
             "weights": "seeded synthetic (synth.py, seed 1234)",
-            "l2": "inputs rotate over distinct batches larger than the 126 MB L2 (4 x 88 MB float32 / 8 x 22 MB uint8) "
+            "l2": "inputs rotate over distinct batches larger than the 50 MB L2 (4 x 88 MB float32 / 8 x 22 MB uint8) "
                   "and the per-step activation footprint (> 2 GB) exceeds L2",
             "parallelism": "replicas x%d" % n_gpus}
 
 
 class ClockSampler(threading.Thread):
-    """Samples SM clock / throttle reasons during the timed region (B200_PROFILING.md): NVML every 10 ms
+    """Samples SM clock / throttle reasons during the timed region: NVML every 10 ms
     (nvidia-smi every 200 ms as a fallback when the NVML binding is unavailable)."""
 
     REASONS = {0x4: "sw_power_cap", 0x8: "hw_slowdown", 0x20: "sw_thermal_slowdown", 0x40: "hw_thermal_slowdown"}
@@ -116,20 +116,16 @@ def measured_peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return d, "measured (MEASURED_PEAKS.json)"
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}, "fallback (B200_PROFILING.md)"
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0}, "NVIDIA H100 SXM data sheet (dense, 700 W board limit)"
 
 
-def ncu_traffic(precision):
-    """dram__bytes_read.sum + dram__bytes_write.sum per conv_tc_kernel launch (average over the launches of one
-    pass) from the committed ncu capture of the same workload, or None when no capture is committed."""
-    p = os.path.join(ROOT, "profiles", "r2_conv_tc_dram_%s_b8.json" % precision)     # this round's capture first
-    if not os.path.exists(p):
-        p = os.path.join(ROOT, "profiles", "r1_conv_tc_dram_%s_b8.json" % precision)
-    if not os.path.exists(p):
-        return None
-    d = json.load(open(p))
-    return {"bytes_per_launch_avg": d["dram_bytes_total"] / d["launches"], "launches": d["launches"],
-            "source": "profiles/" + os.path.basename(p)}
+def dump_outputs(det, out_dir):
+    """Writes what the last pass left in the detector -- what detect_device hands its caller: final boxes / probs /
+    labels, the per-image detection count and the [B*R, 256, 7, 7] ROI box features -- as float32 DIR/<name>.npy
+    (about 40 MB at the bench size)."""
+    os.makedirs(out_dir, exist_ok=True)
+    for name in ("final_boxes", "final_probs", "final_labels", "final_count", "fpn_box_feat"):
+        np.save(os.path.join(out_dir, name + ".npy"), det.get_stage(name).astype(np.float32))
 
 
 def usable_cores():
@@ -279,6 +275,9 @@ def main():
     ap.add_argument("--single-semantics", action="store_true", help="batch of 8 through the single-image graph semantics")
     ap.add_argument("--sustained-seconds", type=float, default=5.0, help="length of the sustained replay record (0 = skip)")
     ap.add_argument("--no-stream", action="store_true", help="skip the config-1 detect+track stream record")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="write the outputs of the last timed step as DIR/<name>.npy (rank 0; inputs are seeded, so two "
+                         "builds can be compared output for output)")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl == "b200" else args.warmup
     rank = int(os.environ.get("RANK", "0"))
@@ -296,7 +295,7 @@ def main():
     from object_detection_tracking_b200.synth import synth_frame, synth_weights
 
     if not torch.cuda.is_available():
-        raise RuntimeError("bench.py needs a B200: no CUDA device (there is no CPU fallback for the product path)")
+        raise RuntimeError("bench.py needs an H100: no CUDA device (there is no CPU fallback for the product path)")
     torch.cuda.set_device(local_rank)
     if world > 1:
         dist.init_process_group("nccl", device_id=torch.device("cuda", local_rank))
@@ -313,7 +312,7 @@ def main():
     det.load_weights(synth_weights(cfg, 1234))
     # 4 distinct batches of synthetic frames (seeded per rank), resident on device and in pinned host memory
     np_dt = np.float32 if args.input_dtype == "float32" else np.uint8
-    nb = 4 if args.input_dtype == "float32" else 8            # rotating input set larger than the 126 MB L2
+    nb = 4 if args.input_dtype == "float32" else 8            # rotating input set larger than the 50 MB L2
     host = [torch.from_numpy(np.stack([synth_frame(H, W, seed=1000 * rank + 8 * j + i) for i in range(BATCH)])
                              .astype(np_dt)).pin_memory() for j in range(nb)]
     dev = [h.cuda(local_rank) for h in host]
@@ -334,6 +333,8 @@ def main():
     barrier()
     sampler.stop.set()
     sampler.join(timeout=2)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(det, args.dump_outputs)
     # ---------------- sustained: the same graph replayed for >= 5 s (what the board settles at under its power cap) ----------------
     sustained = None
     if args.sustained_seconds > 0:
@@ -403,7 +404,7 @@ def main():
     d2h = sum(v.numel() * v.element_size() for v in outs.values())
 
     if rank == 0:
-        # ---------------- roofline of the dominant kernel (tcgen05 conv), live CUDA-event timing ----------------
+        # ---------------- roofline of the dominant kernel (wgmma conv), live CUDA-event timing ----------------
         prof = det.profile_steps(reps=3)
         conv = [p for p in prof if p["kind"] == 0]
         conv_ms = sum(p["ms"] for p in conv)
@@ -412,14 +413,13 @@ def main():
         peaks, peak_src = measured_peaks()
         peak_tf = float(peaks.get("bf16_tflops_sustained", peaks.get("bf16_tflops", 1400.0)))
         achieved_tf = conv_flops / (conv_ms * 1e-3) / 1e12
-        roofline = {"bound": "tensor", "kernel": "conv_tc_kernel (tcgen05 implicit GEMM, %d launches/step)" % len(conv),
+        roofline = {"bound": "tensor", "kernel": "conv_tc_kernel (wgmma implicit GEMM, %d launches/step)" % len(conv),
                     "achieved": achieved_tf, "peak": peak_tf, "unit": "TFLOP/s", "frac": achieved_tf / peak_tf,
-                    "peak_source": peak_src + ", fp16/bf16 dense sustained",
+                    "peak_source": peak_src + ", fp16/bf16 dense",
                     "algorithmic_gflop_per_launch_avg": conv_flops / len(conv) / 1e9,
                     "avg_launch_ms": conv_ms / len(conv), "share_of_step": conv_ms / total_ms,
                     "mma_flop_multiplier": 3 if args.precision == "split" else 1,
                     "tensor_pipe_work_frac": achieved_tf * (3 if args.precision == "split" else 1) / peak_tf,
-                    "traffic": ncu_traffic(args.precision),
                     # the timed pass forks the backbone / FPN / RPN-head phases over two streams (half-batch launches
                     # that overlap each other's tails); avg_launch_ms above is the serial full-batch launch
                     "conv_tflops_over_whole_step": conv_flops / (dt / args.steps) / 1e12}

@@ -1,4 +1,4 @@
-/* libb200det -- C ABI of the B200-native detect -> embed -> associate hot path.
+/* libb200det -- C ABI of the H100-native detect -> embed -> associate hot path.
  *
  * Drop-in boundary for JunweiLiang/Object_Detection_Tracking: the entry points below are what the
  * reference's Python call surface binds for this path (the reference has no native code of its own;
@@ -44,7 +44,7 @@ typedef struct b2_config {
   int32_t fpn_num_channel;    /* 256 */
   int32_t fc_head_dim;        /* 1024 */
   int32_t precision;          /* 0 = fp16 operands / fp32 accumulate; 1 = split fp16 pair (~fp32 products) */
-  int32_t conv_impl;          /* 0 = tcgen05 tensor-core kernel, 1 = CUDA-core cross-check kernel */
+  int32_t conv_impl;          /* 0 = tensor-core (wgmma) kernel, named "tcgen05" in Python, 1 = CUDA-core cross-check kernel */
   int32_t use_cuda_graph;     /* replay the frame as one CUDA graph */
   float max_size;             /* rounded up to a multiple of 32 by the caller */
   float rpn_min_size, rpn_nms_thres, fastrcnn_nms_iou_thres, result_score_thres;
@@ -308,10 +308,6 @@ int b2_track_spatial_dist(const int32_t* frames1, const double* pts1, const int3
 int b2_op_conv2d(int device, const float* x, const float* w, const float* bias, const float* res, int B, int H, int W,
                  int Cin, int R, int S, int Cout, int stride, int dil, int pad_t, int pad_b, int pad_l, int pad_r,
                  int relu, int res_shift, int impl, int split, int a_mode, float* out);
-
-/* Number of conv launches of this process that ran on CTA pairs (tcgen05 cta_group::2; opt-in through the environment
- * variable B2_PAIR=<min K-blocks>, DESIGN.md 4.3b): lets the tests assert that the hook is live. */
-long long b2_conv_pair_launches(void);
 
 #ifdef __cplusplus
 }

@@ -111,7 +111,6 @@ SYMBOLS = [
     ("b2_gallery_free", c_int, [c_int, c_void_p]),
     ("b2_track_spatial_dist", c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, ctypes.c_double, c_void_p]),
     ("b2_op_conv2d", c_int, [c_int, c_void_p, c_void_p, c_void_p, c_void_p] + [c_int] * 18 + [c_void_p]),
-    ("b2_conv_pair_launches", c_int64, []),
 ]
 
 PHASES = dict(BACKBONE=1, FPN=2, RPN_HEAD=4, PROPOSALS=8, ROI=16, HEAD_FC=32, POST=64, BOX_FEAT=128, ALL=255)

@@ -14,7 +14,7 @@ models.py:196-263).  This module provides the same surface on top of libb200det:
 
 Outputs follow the reference conventions: fresh, writable numpy arrays owned by the caller; boxes are
 x1,y1,x2,y2 in resized-image pixels; labels are 1-based (int64 single image, float32 batch).
-There is no CPU fallback: without the CUDA library or a B200 the calls raise.
+There is no CPU fallback: without the CUDA library or an H100 the calls raise.
 """
 from __future__ import annotations
 

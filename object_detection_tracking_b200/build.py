@@ -1,4 +1,4 @@
-"""Builds libb200det.so in-tree with nvcc for sm_100a (no JIT cache: the .so travels with the repo)."""
+"""Builds libb200det.so in-tree with nvcc for sm_90a (H100; no JIT cache: the .so sits next to this file)."""
 from __future__ import annotations
 
 import hashlib
@@ -11,7 +11,7 @@ CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libb200det.so")
 SOURCES = ["engine.cu", "conv_tc.cu", "conv_simt.cu", "stem.cu", "rpn.cu", "roialign.cu", "head.cu", "cosine.cu", "reid.cu",
            "reid_engine.cu", "effdet.cu", "effnet.cu", "effdet_engine.cu", "tracker.cpp", "tmot.cpp", "pairmatch.cu"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "--expt-relaxed-constexpr", "-Xcompiler", "-fPIC", "-Xcompiler", "-O2",
               "-Xcompiler", "-Wno-attributes"]
 
@@ -61,7 +61,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
             sys.stderr.write(out)
     if failed:
         raise RuntimeError("libb200det build failed")
-    link = [_nvcc(), "-shared", "-o", OUT, *objs, "-gencode", "arch=compute_100a,code=sm_100a", "-cudart", "static"]
+    link = [_nvcc(), "-shared", "-o", OUT, *objs, "-gencode", "arch=compute_90a,code=sm_90a", "-cudart", "static"]
     r = subprocess.run(link, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
     if r.returncode != 0:
         raise RuntimeError("link failed:\n" + r.stdout)

@@ -51,7 +51,6 @@ struct ConvDesc {
   int in_pitch_H = 0, in_pitch_W = 0;       // buffer dims used for strides (>= view dims)
   int in_ld = 0;                            // pixel stride in elements (0 => Cin)
   int force_a_mode = -1;                    // tests: -1 auto, 0 tiled-2D A operand, 1 im2col TMA
-  int force_epi_mode = -1;                  // tests: -1 auto, 0 direct per-thread epilogue
   int acc_kb = 0;                           // split precision: K-blocks per accumulation restart (0 default, <0 off)
   int R = 1, S = 1, stride = 1, dil = 1;
   int pad_t = 0, pad_b = 0, pad_l = 0, pad_r = 0;   // zero padding (pad_b/pad_r may be negative = crop)
@@ -92,7 +91,6 @@ struct ConvPlan;
 ConvPlan* conv_tc_plan_create(const ConvDesc& d, const ConvWeights& w, const ConvIO& io, bool split, int num_sms);
 void conv_tc_plan_destroy(ConvPlan*);
 int conv_tc_launch(const ConvPlan*, cudaStream_t);
-long long conv_tc_pair_launches();   // conv launches of this process that used CTA pairs (B2_PAIR)
 int conv_tc_init();   // resolves the driver entry point for cuTensorMapEncode*
 
 // CUDA-core reference implementation of exactly the same contract (validation + odd shapes).

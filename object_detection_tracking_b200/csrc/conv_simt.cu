@@ -1,5 +1,5 @@
 // CUDA-core implementation of the ConvDesc contract (same operands, same hi/lo arithmetic, fp32
-// accumulate) -- the on-device cross-check for the tcgen05 kernel and the path for shapes the
+// accumulate) -- the on-device cross-check for the tensor-core kernel and the path for shapes the
 // tensor-core kernel does not take (Cin % 64 != 0).  One thread per (pixel, 4 output channels).
 #include "common.h"
 
@@ -81,7 +81,7 @@ int conv_simt_launch(const ConvDesc& d, const ConvWeights& w, const ConvIO& io, 
   const size_t total = static_cast<size_t>(d.B) * Ho * Wo * (w.Cout_pad / 4);
   const int threads = 256;
   size_t blocks = (total + threads - 1) / threads;
-  if (blocks > 148 * 64) blocks = 148 * 64;
+  if (blocks > 132 * 64) blocks = 132 * 64;
   if (split)
     conv_simt_kernel<true><<<static_cast<unsigned>(blocks), threads, 0, stream>>>(d, w, io, Ho, Wo);
   else

@@ -1,6 +1,6 @@
 // DeepSORT appearance cost: L2-normalise gallery / detection rows into tensor-core operands, and the
 // segmented row-min that turns the [S, N] similarity GEMM into the [T, N] cost matrix.
-// The GEMM itself runs on the tcgen05 conv kernel (1x1 conv, split precision).
+// The GEMM itself runs on the wgmma conv kernel (1x1 conv, split precision).
 //
 // Reference ops replaced: nn_matching._cosine_distance (deep_sort/nn_matching.py:31-54),
 // _nn_cosine_distance (:78-96), NearestNeighborDistanceMetric.distance (:156-177).

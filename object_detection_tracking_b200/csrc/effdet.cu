@@ -1,5 +1,5 @@
 // Non-GEMM kernels of the EfficientDet feature network (BiFPN), heads and post-processing.  The pointwise
-// halves of every separable conv and the 1x1 resampling convs run on the tcgen05 implicit-GEMM kernel.
+// halves of every separable conv and the 1x1 resampling convs run on the wgmma implicit-GEMM kernel.
 //
 // Reference ops replaced: resample_feature_map (efficientdet_arch.py:105-200: max_pooling2d SAME / nearest
 // upsampling), the node combine + swish of build_bifpn_layer (:594-682), the depthwise half of
@@ -343,9 +343,9 @@ __global__ void __launch_bounds__(32, 1) nms_scan_kernel(const __grid_constant__
 
 __global__ void topk_seed_kernel(uint32_t* state, uint32_t need) { state[2] = need; }
 
-constexpr unsigned kTopkMaxBlocks = 148 * 8;
+constexpr unsigned kTopkMaxBlocks = 132 * 8;
 
-inline unsigned grid_for(size_t total, int threads, unsigned cap = 148 * 16) {
+inline unsigned grid_for(size_t total, int threads, unsigned cap = 132 * 16) {
   size_t b = (total + threads - 1) / threads;
   if (b > cap) b = cap;
   if (b == 0) b = 1;
@@ -363,7 +363,7 @@ int next_pow2(int v) {
 int bifpn_combine_launch(const BifpnCombineParams& p, cudaStream_t s) {
   B2_CHECK(p.C % 8 == 0 && p.n_in >= 1 && p.n_in <= 3, "bifpn_combine: bad parameters");
   const size_t total = static_cast<size_t>(p.B) * p.Ho * p.Wo * (p.C / 8);
-  bifpn_combine_kernel<<<grid_for(total, 256, 148 * 32), 256, 0, s>>>(p);
+  bifpn_combine_kernel<<<grid_for(total, 256, 132 * 32), 256, 0, s>>>(p);
   B2_CUDA(cudaGetLastError());
   return 0;
 }

@@ -7,7 +7,7 @@
 // efficientdet_wrapper.py add_metric_fn_inputs (:367-474), anchors.py _generate_detections_tf (:399-487) and the
 // wrapper's own-level ROIAlign box feature (:265-301).
 //
-// Every separable conv = depthwise 3x3 kernel (effdet.cu) + pointwise GEMM on the tcgen05 conv kernel with bias,
+// Every separable conv = depthwise 3x3 kernel (effdet.cu) + pointwise GEMM on the wgmma conv kernel with bias,
 // folded BatchNorm (eps 1e-3) and swish in the epilogue.  The class/box nets share conv weights across levels but
 // not BatchNorm statistics, so each level gets its own folded copy of the pointwise weights.
 #include <math.h>
@@ -88,7 +88,7 @@ int pad16(int c) { return (c + 15) / 16 * 16; }
 
 struct b2_effdet {
   b2_effdet_config cfg;
-  int device = 0, num_sms = 148;
+  int device = 0, num_sms = 132;
   bool split = true;
   int F = 0, Fp = 0, nlev = 0, na = 0;
   int fh[8] = {0}, fw[8] = {0};               // feature size per level (index = level)
@@ -588,7 +588,7 @@ int b2_effdet_create(b2_effdet** out, const b2_effdet_config* cfg, int device) {
   c->cfg = *cfg; c->device = device; c->split = cfg->precision == 1;
   cudaDeviceProp prop;
   B2_CUDA(cudaGetDeviceProperties(&prop, device));
-  B2_CHECK(prop.major == 10, "b2_effdet_create: this library is built for sm_100a (B200) only");
+  B2_CHECK(prop.major == 9 && prop.minor == 0, "b2_effdet_create: this library is built for sm_90a (H100) only");
   c->num_sms = prop.multiProcessorCount;
   B2_CUDA(cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking));
   if (build(c.get())) { b2_effdet_destroy(c.release()); return -1; }

@@ -1,5 +1,5 @@
 // Non-GEMM kernels of the EfficientNet backbone (EfficientDet config) and of the wrapper's input pre-processing.
-// The 1x1 expand / project convolutions and the (im2col-packed) stem run on the tcgen05 conv kernel.
+// The 1x1 expand / project convolutions and the (im2col-packed) stem run on the wgmma conv kernel.
 //
 // Reference ops replaced: EfficientDet.build_preprocess (efficientdet_wrapper.py:40-61) + InputProcessor
 // (efficientdet/dataloader.py:56-123: convert_image_dtype, mean/std, tf.image.resize_images BILINEAR,
@@ -328,7 +328,7 @@ template <int K, int S>
 int dw_strip_launch(const DwConvParams& p, bool act, cudaStream_t s) {
   constexpr int TX = S == 2 ? 2 : 4;
   const size_t total = static_cast<size_t>(p.Ho) * ((p.Wo + TX - 1) / TX) * (p.C / 8);
-  const unsigned grid = grid_for(total, 128, 148 * 64);
+  const unsigned grid = grid_for(total, 128, 132 * 64);
   if (act) dw_strip_kernel<K, S, TX, true><<<grid, 128, 0, s>>>(p);
   else dw_strip_kernel<K, S, TX, false><<<grid, 128, 0, s>>>(p);
   B2_CUDA(cudaGetLastError());

@@ -131,7 +131,7 @@ using namespace b2;
 
 struct b2_ctx {
   b2_config cfg;
-  int device = 0, num_sms = 148;
+  int device = 0, num_sms = 132;
   bool split = false;
   cudaStream_t stream = nullptr;
   std::vector<void*> allocs;
@@ -670,7 +670,7 @@ int run_step(b2_ctx* c, const b2_ctx::Step& s) {
       return roialign_launch(c->roi3, st);
     case 9: {
       const size_t total = static_cast<size_t>(cfg.batch) * cfg.result_per_im * 784;
-      mask_select_kernel<<<static_cast<unsigned>(std::min<size_t>((total + 255) / 256, 148 * 32)), 256, 0, st>>>(
+      mask_select_kernel<<<static_cast<unsigned>(std::min<size_t>((total + 255) / 256, 132 * 32)), 256, 0, st>>>(
           c->mask_logits, c->mask_ld, c->post.final_labels, c->post.final_count, cfg.batch, cfg.result_per_im,
           c->final_masks);
       B2_CUDA(cudaGetLastError());
@@ -915,7 +915,7 @@ int b2_create(b2_ctx** out, int device, const b2_config* cfg) {
   c->split = cfg->precision == 1;
   cudaDeviceProp prop;
   B2_CUDA(cudaGetDeviceProperties(&prop, device));
-  B2_CHECK(prop.major == 10, "b2_create: this library is built for sm_100a (B200) only");
+  B2_CHECK(prop.major == 9 && prop.minor == 0, "b2_create: this library is built for sm_90a (H100) only");
   c->num_sms = prop.multiProcessorCount;
   B2_CUDA(cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking));
   for (int i = 0; i <= NPHASE; ++i) B2_CUDA(cudaEventCreate(&c->ev[i]));
@@ -1436,8 +1436,8 @@ int b2_set_stage(b2_ctx* c, const char* name, const void* src, int64_t bytes) {
 // ---- workspace for the small per-frame GEMM calls ------------------------------------------------------------------
 // b2_cosine_cost / b2_distance_matrix are called once per frame (per cascade level) by the trackers.  They run out of ONE
 // grow-only workspace per device with the GEMM plans cached per padded shape: a call is three uploads, four launches and
-// one download on a private stream (round 1 allocated ~12 device buffers, encoded the tensor maps and freed everything
-// again on every call: 48 ms per JDE frame against 1.7 ms for numpy, profiles/r2_widen_timing_before_ws.jsonl).  Operands
+// one download on a private stream (allocating device buffers and encoding the tensor maps on every call instead costs
+// more than the numpy computation it replaces).  Operands
 // are padded to the plan's shape with whatever the buffers hold (finite leftovers of earlier calls): padded rows / columns
 // only produce outputs nobody reads.  B2_NO_WS=1 (test hook) runs every call in a private workspace that is released
 // when the call returns -- same code, no reuse; tests compare the two bit for bit.
@@ -1449,7 +1449,7 @@ struct DistWs {
   int* d_off = nullptr;
   __half *a_hi = nullptr, *a_lo = nullptr, *b_hi = nullptr, *b_lo = nullptr;
   std::map<std::vector<int>, ConvPlan*> plans;   // key: Sp, Np, Dp, split
-  int num_sms = 148;
+  int num_sms = 132;
   bool transient = false;   // B2_NO_WS: owned by one call
   DistWs() = default;
   DistWs(const DistWs&) = delete;
@@ -1622,7 +1622,6 @@ int b2_distance_matrix(int device, const float* a, int na, const float* b, int n
 }
 
 // ---- single conv op for kernel parity tests ---------------------------------------------------
-long long b2_conv_pair_launches(void) { return b2::conv_tc_pair_launches(); }
 
 int b2_op_conv2d(int device, const float* x, const float* w, const float* bias, const float* res, int B, int H, int W,
                  int Cin, int R, int S, int Cout, int stride, int dil, int pad_t, int pad_b, int pad_l, int pad_r,

@@ -1,5 +1,5 @@
 // Non-GEMM kernels of the OSNet ReID embedding (HBM-bound byte/element work; the 1x1 convolutions and
-// the fc run on the tcgen05 implicit-GEMM kernel).
+// the fc run on the wgmma implicit-GEMM kernel).
 //
 // Reference ops replaced (torchreid/models/osnet.py): LightConv3x3's depthwise 3x3 + BN + ReLU (:128-156),
 // ChannelGate (:162-220: global avg-pool -> fc1 -> ReLU -> fc2 -> sigmoid -> scale), the 4-stream gated sum
@@ -221,7 +221,7 @@ __global__ void avgpool2_kernel(const __half* __restrict__ in_hi, const __half* 
   }
 }
 
-inline unsigned grid_for(size_t total, int threads, unsigned cap = 148 * 32) {
+inline unsigned grid_for(size_t total, int threads, unsigned cap = 132 * 32) {
   size_t b = (total + threads - 1) / threads;
   if (b > cap) b = cap;
   if (b == 0) b = 1;

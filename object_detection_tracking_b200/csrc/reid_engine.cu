@@ -13,7 +13,7 @@
 // single_video_reid.py:410-415 with image_size (128, 256):  conv1 7x7/2 + BN + ReLU -> maxpool 3/2 pad 1 ->
 // layer1..4 of Bottleneck blocks (1x1 -> 3x3 carrying the stride -> 1x1, BN folded, ReLU / residual in the epilogue,
 // 1x1 strided downsample on the first block of a layer) -> global avg-pool = the 2048-d feature (eval mode).
-// Every conv runs on conv_tc_kernel (tcgen05); max-pool / global-average kernels are shared with OSNet.
+// Every conv runs on conv_tc_kernel (wgmma); max-pool / global-average kernels are shared with OSNet.
 #include <math.h>
 #include <stdlib.h>
 #include <string.h>
@@ -73,7 +73,7 @@ struct RStep {
 }  // namespace
 
 struct b2_reid {
-  int device = 0, num_sms = 148, B = 0;
+  int device = 0, num_sms = 132, B = 0;
   int model = 0;                     // 0 osnet_x1_0, 1 resnet101
   int in_h = 256, in_w = 128;        // crop size (h, w) the extractor resizes to
   int feat_dim = 512;
@@ -424,7 +424,7 @@ int b2_reid_create_model(b2_reid** out, int device, int batch, int precision, in
   if (model == 1) { c->in_h = 128; c->in_w = 256; c->feat_dim = 2048; }   // single_video_reid.py:410-415
   cudaDeviceProp prop;
   B2_CUDA(cudaGetDeviceProperties(&prop, device));
-  B2_CHECK(prop.major == 10, "b2_reid_create: this library is built for sm_100a (B200) only");
+  B2_CHECK(prop.major == 9 && prop.minor == 0, "b2_reid_create: this library is built for sm_90a (H100) only");
   c->num_sms = prop.multiProcessorCount;
   B2_CUDA(cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking));
   if ((model == 1 ? build_resnet101(c.get()) : build(c.get()))) { b2_reid_destroy(c.release()); return -1; }

@@ -32,7 +32,7 @@ __global__ void planes_to_f32_kernel(const __half* __restrict__ hi, const __half
 
 // Stem operand pack.  The 7x7 stride-2 conv on 3 channels is not a tensor-core shape, so the frame is
 // re-laid out once per pass so that it becomes a 4x1 stride-1 conv on 64 channels (K = 256) that the
-// tcgen05 implicit-GEMM kernel takes unchanged:
+// wgmma implicit-GEMM kernel takes unchanged:
 //   P  = normalised frame, zero padded [3 top/left, 2 + pad-to-32 bottom/right]        (nn.py:871-877)
 //   U[b][y][q][s*12 + ry*6 + sx*3 + c] = P[b][2y + ry][2(q + s) + sx][c]   s in 0..3, ry,sx in 0..1, c in 0..2
 //   conv0[p][q][o] = sum_{r<4} sum_{ch<64} U[p + r][q][ch] * W'[o][r][ch],  W'[o][r][ch] = W[2r+ry][2s+sx][c][o]
@@ -197,7 +197,7 @@ __global__ void resize_u8_to_f32_kernel(const uint8_t* __restrict__ src, int B, 
   }
 }
 
-inline unsigned grid_for(size_t total, int threads, unsigned cap = 148 * 32) {
+inline unsigned grid_for(size_t total, int threads, unsigned cap = 132 * 32) {
   size_t b = (total + threads - 1) / threads;
   if (b > cap) b = cap;
   if (b == 0) b = 1;
@@ -220,7 +220,7 @@ int planes_to_f32(const __half* hi, const __half* lo, float* dst, size_t n, cuda
 int stem_pack_launch(const void* img, int is_u8, int B, int H, int W, __half* out_hi, __half* out_lo, int Hu, int Wu,
                      int norm_mode, cudaStream_t s) {
   const size_t total = static_cast<size_t>(B) * Hu * Wu * 8;
-  const unsigned grid = grid_for(total, 256, 148 * 32);
+  const unsigned grid = grid_for(total, 256, 132 * 32);
   if (is_u8)
     stem_pack_kernel<uint8_t><<<grid, 256, 0, s>>>(static_cast<const uint8_t*>(img), B, H, W, out_hi, out_lo, Hu, Wu, norm_mode);
   else
@@ -232,7 +232,7 @@ int stem_pack_launch(const void* img, int is_u8, int B, int H, int W, __half* ou
 int stem_pack16_launch(const void* img, int is_u8, int B, int H, int W, __half* out_hi, __half* out_lo, int Hu, int Wv,
                        cudaStream_t s) {
   const size_t total = static_cast<size_t>(B) * Hu * Wv;
-  const unsigned grid = grid_for(total, 256, 148 * 32);
+  const unsigned grid = grid_for(total, 256, 132 * 32);
   if (is_u8)
     stem_pack16_kernel<uint8_t><<<grid, 256, 0, s>>>(static_cast<const uint8_t*>(img), B, H, W, out_hi, out_lo, Hu, Wv);
   else

@@ -1,6 +1,6 @@
 // DeepSORT association loop in native host code (float64 state, as the reference): Kalman predict / project /
 // update / gating, matching cascade, IoU matching, rectangular linear assignment, track life cycle, per-track
-// appearance gallery -- with the appearance cost matrix computed on the GPU by b2_cosine_cost (one tcgen05 GEMM)
+// appearance gallery -- with the appearance cost matrix computed on the GPU by b2_cosine_cost (one tensor-core GEMM)
 // unless the caller installs another cost function.
 //
 // Reference (Python, per-track loops): deep_sort/tracker.py:10-138, track.py:19-166, kalman_filter.py:23-232,

@@ -1,4 +1,4 @@
-"""EfficientDet BiFPN + heads + post-processing on the B200 (config 3 of the reference,
+"""EfficientDet BiFPN + heads + post-processing on the H100 (config 3 of the reference,
 efficientdet_wrapper.py:160-474).  Thin host mirror over the C ABI (include/b200det.h, b2_effdet_*); no CPU path."""
 from __future__ import annotations
 

@@ -94,7 +94,7 @@ class FeatureExtractor(object):
                  pixel_mean=(0.485, 0.456, 0.406), pixel_std=(0.229, 0.224, 0.225), pixel_norm=True,
                  device="cuda", verbose=False, batch=32, precision="split", state_dict=None):
         if model_name not in ReidEngine.MODELS:
-            raise NotImplementedError("the B200 path implements osnet_x1_0 (person) and resnet101 (vehicle), the two "
+            raise NotImplementedError("the GPU path implements osnet_x1_0 (person) and resnet101 (vehicle), the two "
                                       "extractors the drivers build (single_video_reid.py:404-415)")
         if tuple(image_size) != ReidEngine.MODELS[model_name][1] or not pixel_norm \
                 or tuple(pixel_mean) != (0.485, 0.456, 0.406) or tuple(pixel_std) != (0.229, 0.224, 0.225):

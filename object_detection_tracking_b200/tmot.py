@@ -1,6 +1,6 @@
 """Drop-ins for the reference's TMOT tracker (tmot/multitracker.py, tmot/matching.py) over libb200det's native
 association code (csrc/tmot.cpp).  The per-frame embedding distance is one tensor-core GEMM on the GPU; everything else is
-float64 host code, as in the reference.  No CPU fallback for the embedding distance: without a B200 only the `cost_fn` hook
+float64 host code, as in the reference.  No CPU fallback for the embedding distance: without an H100 only the `cost_fn` hook
 (used by the CPU parity tests with the oracle) can supply it."""
 from __future__ import annotations
 

@@ -143,7 +143,7 @@ class Tracker(object):
     `metric` supplies the parameters exactly as in the reference: an object with `matching_threshold` and `budget`
     (nn_matching.NearestNeighborDistanceMetric or GpuNearestNeighborDistanceMetric); its own sample store is not used --
     the native tracker keeps the per-track galleries.  `cost_fn(gallery, seg_offsets, dets) -> [T,N]` replaces the GPU
-    appearance cost (tests pass the CPU oracle there); without it a B200 is required.
+    appearance cost (tests pass the CPU oracle there); without it an H100 is required.
     Detections need `.tlwh`, `.confidence`, `.feature` (deep_sort/detection.py:27-42)."""
 
     def __init__(self, metric, max_iou_distance=0.5, max_age=60, n_init=1, device=0, precision="split", cost_fn=None):

@@ -178,8 +178,8 @@ def osnet():
     resized = np.stack([np.asarray(ext.to_pil(c).resize((128, 256), 2)) for c in crops])   # 2 = PIL BILINEAR
     d_cos = distance.compute_distance_matrix(torch.from_numpy(feats[:4]), torch.from_numpy(feats[2:]), "cosine").numpy()
     d_euc = distance.compute_distance_matrix(torch.from_numpy(feats[:4]), torch.from_numpy(feats[2:]), "euclidean").numpy()
-    np.savez_compressed(os.path.join(HERE, "osnet.npz"), feats=feats, resized=resized, d_cos=d_cos, d_euc=d_euc,
-                        **{"crop%d" % i: c for i, c in enumerate(crops)})
+    # the crops are not stored: tests/test_reid_gpu.py draws them from the same seed
+    np.savez_compressed(os.path.join(HERE, "osnet.npz"), feats=feats, resized=resized, d_cos=d_cos, d_euc=d_euc)
 
 
 def effdet_numpy():
@@ -225,6 +225,20 @@ def effdet_numpy():
     np.savez_compressed(os.path.join(HERE, "effdet_numpy.npz"), **out)
 
 
+def torchreid_state_shapes():
+    """Parameter / buffer shapes of the reference's torchreid osnet_x1_0 and resnet101 (1-class models, classifier and
+    BN step counters left out): what the synthetic state dicts of object_detection_tracking_b200.synth must match."""
+    import json
+    from torchreid.models import build_model
+    out = {}
+    for name in ("osnet_x1_0", "resnet101"):
+        sd = build_model(name, num_classes=1, pretrained=False, use_gpu=False).state_dict()
+        out[name] = {k: list(v.shape) for k, v in sd.items()
+                     if not k.startswith("classifier") and not k.endswith("num_batches_tracked")}
+    with open(os.path.join(HERE, "torchreid_state_shapes.json"), "w") as f:
+        json.dump(out, f, indent=0, sort_keys=True)
+
+
 if __name__ == "__main__":
     anchors()
     cosine()
@@ -233,4 +247,5 @@ if __name__ == "__main__":
     track_nms()
     osnet()
     effdet_numpy()
+    torchreid_state_shapes()
     print("golden fixtures written to", HERE)

@@ -8,7 +8,7 @@
   C3  EfficientDet-D7 1536x1536 on one frame is in tests/test_effdet_gpu.py::test_d7_full_size_matches_oracle
 
 Bars (north_star): counts and class ids bit-exact, box coordinates and probabilities within 1e-3 absolute; feature
-maps relative.  Every test also appends its measured margins to gpurun_out/baseline_parity.jsonl (copied to profiles/).
+maps relative.  Every test also appends its measured margins to a baseline_parity.jsonl record (log_margins).
 
 What "within 1e-3 of the reference" can mean at this depth.  Coordinates reach 1280 px (float32 ulp 1.2e-4 px) after 105
 conv layers, so two float32 evaluations of the SAME graph already differ at the 1e-3 level: the float32 oracle is

@@ -85,30 +85,30 @@ def _gpu_count():
         return 0
 
 
-if _gpu_count() >= 2:
-    # NCCL cannot place two ranks on one GPU, so this test exists only on multi-GPU boxes (`gpurun --gpus 2`); the
-    # single-GPU suite covers the same pair-cost kernels through the p2p form above and tests/test_widen_gpu.py.
-    def test_two_cameras_nccl_allgather_device_resident(golden_dir):
-        """Device-resident form of config 5: galleries in HBM, ONE all_gather_into_tensor over NCCL, pair cost on the
-        gathered device pointers; ids pinned by the reference-generated reid_pairs.npz (multi_video_reid.py:260-324,512)."""
-        import torch.multiprocessing as mp
-        s = socket.socket()
-        s.bind(("127.0.0.1", 0))
-        port = s.getsockname()[1]
-        s.close()
-        path = os.path.join(golden_dir, "reid_pairs.npz")
-        ctx = mp.get_context("spawn")
-        q = ctx.Queue()
-        procs = [ctx.Process(target=_worker_allgather, args=(r, 2, port, q, path)) for r in range(2)]
-        for p in procs:
-            p.start()
-        got = [q.get(timeout=300) for _ in range(2)]
-        for p in procs:
-            p.join(timeout=60)
-            assert p.exitcode == 0
-        out = {r: m for r, m, _ in got}
-        g = np.load(path)
-        ids1, ids2 = sorted(int(t) for t in g["c1_ids"]), sorted(int(t) for t in g["c2_ids"])
-        ref = [(ids1[i], ids2[int(j)]) for i, j in enumerate(g["x"]) if j >= 0]
-        assert out[0] == {(0, 1): ref} and out[1] == {}
-        assert all(t["allgather_ms"] > 0 for _, _, t in got)
+# NCCL cannot place two ranks on one GPU, so this test runs only on multi-GPU machines; the single-GPU suite covers the
+# same pair-cost kernels through the p2p form above and tests/test_widen_gpu.py.
+@pytest.mark.skipif(_gpu_count() < 2, reason="needs two GPUs (NCCL cannot place two ranks on one GPU)")
+def test_two_cameras_nccl_allgather_device_resident(golden_dir):
+    """Device-resident form of config 5: galleries in HBM, ONE all_gather_into_tensor over NCCL, pair cost on the
+    gathered device pointers; ids pinned by the reference-generated reid_pairs.npz (multi_video_reid.py:260-324,512)."""
+    import torch.multiprocessing as mp
+    s = socket.socket()
+    s.bind(("127.0.0.1", 0))
+    port = s.getsockname()[1]
+    s.close()
+    path = os.path.join(golden_dir, "reid_pairs.npz")
+    ctx = mp.get_context("spawn")
+    q = ctx.Queue()
+    procs = [ctx.Process(target=_worker_allgather, args=(r, 2, port, q, path)) for r in range(2)]
+    for p in procs:
+        p.start()
+    got = [q.get(timeout=300) for _ in range(2)]
+    for p in procs:
+        p.join(timeout=60)
+        assert p.exitcode == 0
+    out = {r: m for r, m, _ in got}
+    g = np.load(path)
+    ids1, ids2 = sorted(int(t) for t in g["c1_ids"]), sorted(int(t) for t in g["c2_ids"])
+    ref = [(ids1[i], ids2[int(j)]) for i, j in enumerate(g["x"]) if j >= 0]
+    assert out[0] == {(0, 1): ref} and out[1] == {}
+    assert all(t["allgather_ms"] > 0 for _, _, t in got)

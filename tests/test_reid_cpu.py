@@ -1,4 +1,5 @@
 """CPU-side checks of the ReID layer: synthetic state_dict layout, all-gather exchange (gloo, world 2)."""
+import json
 import os
 import socket
 
@@ -22,14 +23,14 @@ def test_osnet_state_layout_and_param_count():
     np.testing.assert_array_equal(st["fc.0.weight"], synth_osnet_state(1)["fc.0.weight"])
 
 
-@pytest.mark.skipif(not os.path.isdir("/root/reference/torchreid"), reason="reference checkout not present")
-def test_state_layout_matches_reference_model():
-    import sys
-    sys.path.insert(0, "/root/reference")
-    from torchreid.models import build_model
-    sd = build_model("osnet_x1_0", num_classes=1, pretrained=False, use_gpu=False).state_dict()
-    ref = {k: tuple(v.shape) for k, v in sd.items() if not k.startswith("classifier") and not k.endswith("num_batches_tracked")}
-    assert ref == {k: tuple(v) for k, v in osnet_param_shapes().items()}
+def _reference_shapes(golden_dir, model):
+    """State-dict shapes of the reference's torchreid model (tests/golden/make_golden.py: torchreid_state_shapes)."""
+    with open(os.path.join(golden_dir, "torchreid_state_shapes.json")) as f:
+        return {k: tuple(v) for k, v in json.load(f)[model].items()}
+
+
+def test_state_layout_matches_reference_model(golden_dir):
+    assert _reference_shapes(golden_dir, "osnet_x1_0") == {k: tuple(v) for k, v in osnet_param_shapes().items()}
 
 
 def _free_port():
@@ -78,12 +79,6 @@ def test_resnet101_reid_state_layout_and_param_count():
     assert a.dtype == np.float32 and a.shape == (2048, 512, 1, 1)
 
 
-@pytest.mark.skipif(not os.path.isdir("/root/reference/torchreid"), reason="reference checkout not present")
-def test_resnet101_state_layout_matches_reference_model():
-    import sys
-    sys.path.insert(0, "/root/reference")
-    from torchreid.models import build_model
+def test_resnet101_state_layout_matches_reference_model(golden_dir):
     from object_detection_tracking_b200.synth import resnet101_reid_param_shapes
-    sd = build_model("resnet101", num_classes=1, pretrained=False, use_gpu=False).state_dict()
-    ref = {k: tuple(v.shape) for k, v in sd.items() if not k.startswith("classifier") and not k.endswith("num_batches_tracked")}
-    assert ref == {k: tuple(v) for k, v in resnet101_reid_param_shapes().items()}
+    assert _reference_shapes(golden_dir, "resnet101") == {k: tuple(v) for k, v in resnet101_reid_param_shapes().items()}

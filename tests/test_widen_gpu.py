@@ -1,7 +1,7 @@
 """GPU parity of the section-8f widening that composes already-verified kernels (the tensor-core GEMM behind
 b2_distance_matrix) with small new ones: TMOT embedding distance, the JDE tracker with its embedding cost on the GPU, and
 the multi-camera track-pair cost (b2_track_pair_cost), device-side frame resize, given-box features, the detect -> track
-loop.  First B200 run: round 2, 12/12 green (gpurun_out/widen_tests.log -> profiles/r2_first_gpu_call.txt)."""
+loop."""
 import os
 
 import numpy as np

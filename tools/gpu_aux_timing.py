@@ -1,6 +1,6 @@
 """Wall-clock timings of the two other engines through their host-facing calls (host buffers in, host results out):
 EfficientDet-D7 1536x1536 single-frame detect (BASELINE configs[2]) and OSNet-x1.0 ReID embedding (configs[4]).
-Prints one JSON line per engine; redirect into profiles/."""
+Prints one JSON line per engine; redirect it to a file."""
 import json
 import os
 import sys

@@ -1,7 +1,7 @@
 """Host-side timing of the TMOT association loop (no GPU involved): the native JDE tracker (csrc/tmot.cpp) against the
 reference's tmot.multitracker.JDETracker on the same synthetic sequence, both with a CPU embedding distance (the native
 one through the cost_fn hook with scipy's cdist -- what the reference calls).  Shows what moving the per-track Python loops
-into native code buys on its own; on a B200 the embedding distance additionally moves to the tensor cores.
+into native code buys on its own; on the GPU the embedding distance additionally moves to the tensor cores.
 Needs /root/reference (authoring container only).  Usage: python tools/host_jde_bench.py [n_objects] [frames]"""
 import json
 import os
