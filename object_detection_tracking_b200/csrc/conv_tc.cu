@@ -236,54 +236,76 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
 #pragma unroll
       for (int i = 0; i < kAcc; ++i) sums[i] = 0.0f;
     }
+    // The wait structure is the same on every K-block: no wgmma_wait sits on a run-time branch.  A wait whose count
+    // depends on a divergent path makes ptxas serialise every wgmma of the loop (C7518) or insert waits of its own
+    // (C7517); tests/test_conv_ptxas_cpu.py keeps both out.
     int kq = 0;       // ACC: K-block inside the current chunk
-    int held = -1;    // stage the last commit group may still be reading (released after the next wait)
+    int held = -1;    // stage the newest commit group may still be reading (released after the next wait)
     for (int kb = 0; kb < p.num_kb; ++kb) {
       mbar_wait(&full_bar[stage], phase);
       const uint32_t st = tiles_u32 + static_cast<uint32_t>(stage) * p.stage_bytes;
       const uint32_t a_hi = st + cwg * (kWgRows * kBlockK * 2);
       const uint32_t b_hi = st + b_hi_off;
+      const uint32_t first = kb > 0 ? 1u : 0u;
       wgmma_fence();
+      if constexpr (ACC) {
+        // two commit groups: the four hi*hi MMAs of the chunk accumulator, then the eight cross terms.
 #pragma unroll
-      for (int k = 0; k < kBlockK / kWgmmaK; ++k) {
-        const uint32_t ko = k * kWgmmaK * 2;   // 32 bytes along K inside the 128-byte swizzle row
-        const uint64_t da_hi = make_smem_desc_sw128(a_hi + ko);
-        const uint64_t db_hi = make_smem_desc_sw128(b_hi + ko);
-        const uint32_t first = (kb > 0 || k > 0) ? 1u : 0u;
-        wgmma_f16<BN>(acc0, da_hi, db_hi, ACC ? ((kq > 0 || k > 0) ? 1u : 0u) : first);
-        if constexpr (SPLIT) {
-          const uint64_t da_lo = make_smem_desc_sw128(a_hi + a_lo_off + ko);
-          const uint64_t db_lo = make_smem_desc_sw128(st + b_lo_off + ko);
-          wgmma_f16<BN>(acc1, da_hi, db_lo, first);
-          wgmma_f16<BN>(acc1, da_lo, db_hi, 1u);
+        for (int k = 0; k < kBlockK / kWgmmaK; ++k) {
+          const uint32_t ko = k * kWgmmaK * 2;   // 32 bytes along K inside the 128-byte swizzle row
+          wgmma_f16<BN>(acc0, make_smem_desc_sw128(a_hi + ko), make_smem_desc_sw128(b_hi + ko),
+                        (kq > 0 || k > 0) ? 1u : 0u);
         }
-      }
-      wgmma_commit();
-      if (ACC && (kq + 1 == p.acc_kb || kb == p.num_kb - 1)) {
-        // chunk complete: fold it into the running sums with round-to-nearest adds
-        wgmma_wait<0>();
-        fence_regs(acc0);
-#pragma unroll
-        for (int i = 0; i < kAcc; ++i) sums[i] = __fadd_rn(sums[i], acc0[i]);
+        wgmma_commit();
+        // all but the newest group done: the previous K-block's cross terms have finished with their stage, which
+        // goes back to the producer while this K-block's hi*hi MMAs run
+        wgmma_wait<1>();
         if (held >= 0) release(held);
-        release(stage);
-        held = -1;
-        kq = 0;
+#pragma unroll
+        for (int k = 0; k < kBlockK / kWgmmaK; ++k) {
+          const uint32_t ko = k * kWgmmaK * 2;
+          const uint64_t da_hi = make_smem_desc_sw128(a_hi + ko);
+          const uint64_t db_hi = make_smem_desc_sw128(b_hi + ko);
+          wgmma_f16<BN>(acc1, da_hi, make_smem_desc_sw128(st + b_lo_off + ko), (first | k) ? 1u : 0u);
+          wgmma_f16<BN>(acc1, make_smem_desc_sw128(a_hi + a_lo_off + ko), db_hi, 1u);
+        }
+        wgmma_commit();
+        // acc0 is final: at the end of a chunk it is folded into the running sums with round-to-nearest adds (a
+        // select, not a branch) while the cross terms -- two thirds of the K-block's MMAs -- are still on the tensor
+        // cores
+        wgmma_wait<1>();
+        fence_regs(acc0);
+        const bool fold = kq + 1 == p.acc_kb || kb == p.num_kb - 1;
+#pragma unroll
+        for (int i = 0; i < kAcc; ++i) sums[i] = fold ? __fadd_rn(sums[i], acc0[i]) : sums[i];
+        kq = fold ? 0 : kq + 1;
       } else {
+#pragma unroll
+        for (int k = 0; k < kBlockK / kWgmmaK; ++k) {
+          const uint32_t ko = k * kWgmmaK * 2;
+          const uint64_t da_hi = make_smem_desc_sw128(a_hi + ko);
+          const uint64_t db_hi = make_smem_desc_sw128(b_hi + ko);
+          const uint32_t acc = (first | k) ? 1u : 0u;
+          wgmma_f16<BN>(acc0, da_hi, db_hi, acc);
+          if constexpr (SPLIT) {
+            const uint64_t da_lo = make_smem_desc_sw128(a_hi + a_lo_off + ko);
+            const uint64_t db_lo = make_smem_desc_sw128(st + b_lo_off + ko);
+            wgmma_f16<BN>(acc1, da_hi, db_lo, acc);
+            wgmma_f16<BN>(acc1, da_lo, db_hi, 1u);
+          }
+        }
+        wgmma_commit();
         wgmma_wait<1>();   // the previous K-block's MMAs are done with their stage
         if (held >= 0) release(held);
-        held = stage;
-        ++kq;
       }
+      held = stage;
       if (++stage == p.num_stages) {
         stage = 0;
         phase ^= 1;
       }
     }
-    if (held >= 0) {
-      wgmma_wait<0>();
-      release(held);
-    }
+    wgmma_wait<0>();   // num_kb >= 1: held is a stage here
+    release(held);
     fence_regs(acc0);
     if constexpr (SPLIT) fence_regs(acc1);
 
