@@ -8,11 +8,19 @@
 //   image rows / batch images are all resolved by the tensor map (zero fill outside the image).
 // * W is pre-packed [Cout][R][S][Cin] (K-major); a 2D tiled TMA load brings block_n x 64 per K-block.
 // * Both land in shared memory in the 128-byte-swizzled K-major layout wgmma reads directly.
-// * Warpgroup roles (384 threads): warpgroup 0 = TMA producer (one warp issues, the others retire at once and hand
-//   their registers to the consumers), warpgroups 1 and 2 = consumers: each issues wgmma.m64n{64,128}k16 for its 64
-//   rows of the 128-row tile, keeps the accumulators in registers and runs the epilogue of those rows
-//   (bias / residual / activation -> HBM).  The two consumers interleave on the tensor cores, so one's waits and
-//   epilogue overlap the other's MMAs.
+// * Warpgroup roles (384 threads): warpgroup 0 = TMA producer (warp 0 issues the operand loads, warp 1 is the output
+//   warp of the staged epilogue, the others retire at once and hand their registers to the consumers), warpgroups 1 and
+//   2 = consumers: each issues wgmma.m64n{64,128}k16 for its 64 rows of the 128-row tile, keeps the accumulators in
+//   registers and runs the epilogue of those rows (bias / residual / activation).  The two consumers interleave their
+//   MMAs on the tensor cores; they own halves of the same tile and reach its epilogue together.
+// * Epilogue, two paths chosen by the plan (p.epi_slots):
+//   - staged (fp16-plane outputs that are dense [M][Cout_pad] matrices, with no residual or an unshifted one of the
+//     same size): results go through 64 x 64 shared-memory slots, one ring per consumer warpgroup, and leave by TMA
+//     store.  The output warp loads the residual into the slots by TMA, running up to kResSlots chunks ahead of the
+//     consumers across tile boundaries, so the consumers never wait on a DRAM round trip; they add the residual in place,
+//     write the result into the slot and move on.
+//   - direct (fp32 outputs, outputs at a placement offset, 2x-upsampled residuals): loads and stores straight from and to
+//     global memory.
 // * Persistent: grid = min(#tiles, #SMs), static round-robin tile schedule; the producer runs ahead into the next
 //   tile while the consumers are in the epilogue of the current one.
 // * SPLIT precision: every operand is an fp16 pair (hi, lo') with x = hi + lo'/2048.  Three MMAs per
@@ -40,8 +48,14 @@ constexpr int kWgRows = 64;                 // tile rows per consumer warpgroup 
 constexpr int kWgmmaK = 16;
 constexpr int kThreads = 384;               // producer warpgroup + two consumer warpgroups
 constexpr int kMaxStages = 8;
-constexpr int kSmemBudget = 224 * 1024;     // pipeline stages (alignment slack and barriers on top, 227 KB in all)
+constexpr int kSmemBudget = 224 * 1024;     // stages + epilogue slots (alignment slack and barriers on top, 227 KB in all)
 constexpr int kSmemLimit = 227 * 1024;
+// staged epilogue: a slot holds one consumer warpgroup's 64 rows x 64 columns (one 128-byte swizzle row), per plane
+constexpr int kChunkN = 64;
+constexpr uint32_t kSlotPlaneBytes = kWgRows * kChunkN * 2;   // 8 KB
+constexpr int kMaxSlots = 4;                // per consumer warpgroup
+constexpr int kResSlots = 3;                // slots per warpgroup with a residual (the ring the residual is loaded ahead in)
+constexpr int kOutSlots = 1;                // slots per warpgroup without one
 
 struct ConvTcParams {
   int M, Ho, Wo, HoWo;
@@ -66,7 +80,32 @@ struct ConvTcParams {
   int acc_kb;        // ACC: K-blocks per tensor-core accumulation chunk
   float acc_delta;   // SPLIT: relative compensation of the tensor-core accumulator's truncation (kAccDelta)
   unsigned int* range_flag;   // ORed with 1 when a plane output exceeds the fp16 range (nullptr = not monitored)
+  int epi_slots;     // 0 = direct epilogue (registers -> global); > 0 = staged epilogue with this many slots per warpgroup
+  uint32_t slot_bytes;     // one slot: kSlotPlaneBytes per plane (hi, and lo' in split precision)
 };
+
+template <bool SWISH>
+__device__ __forceinline__ void activate(int relu, float& v0, float& v1) {
+  if (relu == 1) {
+    v0 = fmaxf(v0, 0.0f);
+    v1 = fmaxf(v1, 0.0f);
+  } else if (SWISH && relu == 2) {   // swish: x * sigmoid(x) -- only in the SWISH instantiations (EfficientDet)
+    v0 = __fmul_rn(v0, 1.f / (1.f + expf(-v0)));   // x * sigmoid(x) as the other kernels compute it
+    v1 = __fmul_rn(v1, 1.f / (1.f + expf(-v1)));
+  }
+}
+
+// fp16 (hi, lo') planes of two adjacent outputs; lo == nullptr stores the hi plane only
+template <bool SPLIT>
+__device__ __forceinline__ void store_planes(float v0, float v1, __half2* hi_dst, __half2* lo_dst, float& amax) {
+  amax = fmaxf(amax, fmaxf(fabsf(v0), fabsf(v1)));
+  const __half2 hi = __floats2half2_rn(v0, v1);
+  *hi_dst = hi;
+  if (SPLIT && lo_dst != nullptr) {
+    const float2 h = __half22float2(hi);
+    *lo_dst = __floats2half2_rn((v0 - h.x) * kLoScale, (v1 - h.y) * kLoScale);
+  }
+}
 
 // Two adjacent output channels (n, n + 1) of one pixel: bias, residual, activation, store (fp16 hi/lo planes or fp32)
 // straight to global memory.
@@ -86,24 +125,35 @@ __device__ __forceinline__ void epilogue_pair(const ConvTcParams& p, float v0, f
       v1 = fmaf(l.y, kLoInv, v1);
     }
   }
-  if (p.relu == 1) {
-    v0 = fmaxf(v0, 0.0f);
-    v1 = fmaxf(v1, 0.0f);
-  } else if (SWISH && p.relu == 2) {   // swish: x * sigmoid(x) -- only in the SWISH instantiations (EfficientDet)
-    v0 = __fmul_rn(v0, 1.f / (1.f + expf(-v0)));   // x * sigmoid(x) as the other kernels compute it
-    v1 = __fmul_rn(v1, 1.f / (1.f + expf(-v1)));
-  }
+  activate<SWISH>(p.relu, v0, v1);
   if (p.out_f32 != nullptr) {
     *reinterpret_cast<float2*>(p.out_f32 + opix * p.ldc + n) = make_float2(v0, v1);
     return;
   }
-  amax = fmaxf(amax, fmaxf(fabsf(v0), fabsf(v1)));
-  const __half2 hi = __floats2half2_rn(v0, v1);
-  *reinterpret_cast<__half2*>(p.out_hi + opix * p.ldc + n) = hi;
-  if (SPLIT && p.out_lo != nullptr) {
-    const float2 h = __half22float2(hi);
-    *reinterpret_cast<__half2*>(p.out_lo + opix * p.ldc + n) = __floats2half2_rn((v0 - h.x) * kLoScale, (v1 - h.y) * kLoScale);
+  store_planes<SPLIT>(v0, v1, reinterpret_cast<__half2*>(p.out_hi + opix * p.ldc + n),
+                      p.out_lo != nullptr ? reinterpret_cast<__half2*>(p.out_lo + opix * p.ldc + n) : nullptr, amax);
+}
+
+// The same arithmetic in a staged-epilogue slot: the residual (when there is one) was loaded into the slot by TMA, and
+// the result overwrites it in place (hi at s_hi, lo' at s_lo), to leave by TMA store.
+template <bool SPLIT, bool SWISH>
+__device__ __forceinline__ void epilogue_pair_slot(const ConvTcParams& p, float v0, float v1, int n, __half2* s_hi,
+                                                   __half2* s_lo, float& amax) {
+  const float2 b = __ldg(reinterpret_cast<const float2*>(p.bias + n));
+  v0 += b.x;
+  v1 += b.y;
+  if (p.res_hi != nullptr) {
+    const float2 r = __half22float2(*s_hi);
+    v0 += r.x;
+    v1 += r.y;
+    if (SPLIT && p.res_lo != nullptr) {
+      const float2 l = __half22float2(*s_lo);
+      v0 = fmaf(l.x, kLoInv, v0);
+      v1 = fmaf(l.y, kLoInv, v1);
+    }
   }
+  activate<SWISH>(p.relu, v0, v1);
+  store_planes<SPLIT>(v0, v1, s_hi, p.out_lo != nullptr ? s_lo : nullptr, amax);
 }
 
 // ACC (split precision only): the tensor core adds into its fp32 accumulator with truncation (round
@@ -124,12 +174,19 @@ template <int BN, bool SPLIT, bool ACC, bool SWISH>
 __global__ void __launch_bounds__(kThreads, 1)
 conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant__ CUtensorMap tmA_lo,
                const __grid_constant__ CUtensorMap tmB_hi, const __grid_constant__ CUtensorMap tmB_lo,
+               const __grid_constant__ CUtensorMap tmO_hi, const __grid_constant__ CUtensorMap tmO_lo,
+               const __grid_constant__ CUtensorMap tmR_hi, const __grid_constant__ CUtensorMap tmR_lo,
                const __grid_constant__ ConvTcParams p) {
   extern __shared__ uint8_t smem_raw[];
-  // 128B swizzle atoms need 1024-byte aligned tiles
-  uint8_t* tiles = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(tiles + static_cast<size_t>(p.num_stages) * p.stage_bytes);
+  // 128B swizzle atoms need 1024-byte aligned tiles (an offset from smem_raw, so that the compiler knows the pointers
+  // below are shared memory and accesses through them are LDS / STS)
+  uint8_t* tiles = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+  // staged epilogue: slot s of consumer warpgroup w at slots + (w * epi_slots + s) * slot_bytes
+  uint8_t* slots = tiles + static_cast<size_t>(p.num_stages) * p.stage_bytes;
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(slots + static_cast<size_t>(2 * p.epi_slots) * p.slot_bytes);
   uint64_t* empty_bar = full_bar + kMaxStages;
+  uint64_t* slot_full = empty_bar + kMaxStages;        // [w * kMaxSlots + s]: residual landed / slot free to write
+  uint64_t* slot_written = slot_full + 2 * kMaxSlots;  // [w * kMaxSlots + s]: the warpgroup's result is in the slot
 
   // broadcast from lane 0 so that the compiler treats the warp index (and everything derived from it) as warp-uniform
   const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0);
@@ -147,6 +204,16 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
       mbar_init(&full_bar[i], 1);
       mbar_init(&empty_bar[i], 8);   // one arrive per consumer warp
     }
+    if (p.epi_slots > 0) {
+      tma_prefetch_desc(&tmO_hi);
+      if (SPLIT && p.out_lo != nullptr) tma_prefetch_desc(&tmO_lo);
+      if (p.res_hi != nullptr) tma_prefetch_desc(&tmR_hi);
+      if (SPLIT && p.res_lo != nullptr) tma_prefetch_desc(&tmR_lo);
+      for (int i = 0; i < 2 * kMaxSlots; ++i) {
+        mbar_init(&slot_full[i], 1);
+        mbar_init(&slot_written[i], 4);   // one arrive per warp of the consumer warpgroup
+      }
+    }
     fence_mbar_init();
   }
   __syncthreads();
@@ -158,6 +225,70 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
   if (wg == 0) {
     // ===================== TMA producer =====================
     setmaxnreg_dec<40>();
+    if (warp == 1 && p.epi_slots > 0) {
+      // ===================== output warp (staged epilogue), one lane =====================
+      // Walks this CTA's (tile, 64-column chunk) sequence twice: arming slots (residual TMA load, or a plain arrive)
+      // epi_slots chunks ahead of the consumers, across tile boundaries, and storing each chunk once both
+      // warpgroups have written it.  A slot is re-armed when the store has finished reading it.
+      if (lane != 0) return;
+      constexpr int kChunks = BN / kChunkN;
+      const bool res = p.res_hi != nullptr;
+      const bool res_lo = SPLIT && p.res_lo != nullptr;
+      const bool out_lo = SPLIT && p.out_lo != nullptr;
+      const uint32_t res_tx = kSlotPlaneBytes * (res_lo ? 2 : 1);
+      int arm_tile = blockIdx.x, arm_chunk = 0;
+      auto arm = [&](int s) {   // slot s of both warpgroups <- chunk (arm_tile, arm_chunk)
+        const int m_blk = arm_tile / p.num_n_blocks;
+        const int n = (arm_tile - m_blk * p.num_n_blocks) * BN + arm_chunk * kChunkN;
+#pragma unroll
+        for (int w = 0; w < 2; ++w) {
+          uint64_t* bar = &slot_full[w * kMaxSlots + s];
+          const int m = m_blk * kBlockM + w * kWgRows;
+          if (res && m < p.M) {
+            uint8_t* dst = slots + static_cast<size_t>(w * p.epi_slots + s) * p.slot_bytes;
+            mbar_expect_tx(bar, res_tx);
+            tma_load_2d(dst, &tmR_hi, bar, n, m);
+            if (res_lo) tma_load_2d(dst + kSlotPlaneBytes, &tmR_lo, bar, n, m);
+          } else {
+            mbar_arrive(bar);
+          }
+        }
+        if (++arm_chunk == kChunks) {
+          arm_chunk = 0;
+          arm_tile += gridDim.x;
+        }
+      };
+      for (int s = 0; s < p.epi_slots && arm_tile < p.num_tiles; ++s) arm(s);
+      int slot = 0;
+      uint32_t phase = 0;
+      for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
+        const int m_blk = tile / p.num_n_blocks;
+        const int n0 = (tile - m_blk * p.num_n_blocks) * BN;
+        for (int c = 0; c < kChunks; ++c) {
+#pragma unroll
+          for (int w = 0; w < 2; ++w) {
+            mbar_wait(&slot_written[w * kMaxSlots + slot], phase);
+            const int m = m_blk * kBlockM + w * kWgRows;
+            if (m < p.M) {
+              const uint8_t* src = slots + static_cast<size_t>(w * p.epi_slots + slot) * p.slot_bytes;
+              tma_store_2d(&tmO_hi, src, n0 + c * kChunkN, m);
+              if (out_lo) tma_store_2d(&tmO_lo, src + kSlotPlaneBytes, n0 + c * kChunkN, m);
+            }
+          }
+          bulk_commit();
+          if (arm_tile < p.num_tiles) {
+            bulk_wait_read<0>();
+            arm(slot);
+          }
+          if (++slot == p.epi_slots) {
+            slot = 0;
+            phase ^= 1;
+          }
+        }
+      }
+      bulk_wait<0>();   // the shared-memory sources must outlive the stores
+      return;
+    }
     if (warp != 0) return;
     // converged warp, one elected lane issues
     int stage = 0;
@@ -217,8 +348,11 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
   const int cwg = wg - 1;        // rows cwg * 64 .. of the tile
   // wgmma accumulator layout: warp q of the warpgroup holds rows 16q..16q+15; lane l holds rows l/4 and l/4 + 8 of
   // those, columns 8j + 2(l%4) + {0, 1} of every 8-column block j in registers 4j + {0, 1} (first row) / 4j + {2, 3}
-  const int row0 = cwg * kWgRows + (warp & 3) * 16 + (lane >> 2);
+  const int wg_row = (warp & 3) * 16 + (lane >> 2);   // first row inside the warpgroup's 64 (the other is + 8)
+  const int row0 = cwg * kWgRows + wg_row;
   const int col0 = 2 * (lane & 3);
+  int eslot = 0;         // staged epilogue: slot of this warpgroup's next chunk
+  uint32_t ephase = 0;
   const uint32_t tiles_u32 = smem_u32(tiles);
   float acc0[kAcc];
   float acc1[SPLIT ? kAcc : 1];
@@ -310,44 +444,76 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
     if constexpr (SPLIT) fence_regs(acc1);
 
     // ---- epilogue: this thread's two rows
-    size_t opix[2] = {0, 0}, rpix[2] = {0, 0};
+    auto out_value = [&](int i) -> float {   // accumulator register i -> conv output before bias
+      if constexpr (!SPLIT) {
+        return acc0[i];
+      } else if constexpr (ACC) {
+        const float s = fmaf(acc1[i], kLoInv, sums[i]);
+        return fmaf(s, p.acc_delta, s);
+      } else {   // single-chunk (K <= 64) split layers: the same compensation
+        const float v = fmaf(acc0[i], p.acc_delta, acc0[i]);
+        return fmaf(acc1[i], kLoInv, v);
+      }
+    };
     bool valid[2];
 #pragma unroll
-    for (int h = 0; h < 2; ++h) {
-      const int m = m_blk * kBlockM + row0 + 8 * h;
-      valid[h] = m < p.M;
-      if (valid[h]) {
-        const int img = m / p.HoWo;
-        const int rem = m - img * p.HoWo;
-        const int pp = rem / p.Wo + p.off_h;
-        const int qq = rem - (rem / p.Wo) * p.Wo + p.off_w;
-        opix[h] = (static_cast<size_t>(img) * p.out_H + pp) * p.out_W + qq;
-        rpix[h] = (static_cast<size_t>(img) * p.res_H + (pp >> p.res_shift)) * p.res_W + (qq >> p.res_shift);
-      }
-    }
+    for (int h = 0; h < 2; ++h) valid[h] = m_blk * kBlockM + row0 + 8 * h < p.M;
     float amax = 0.f;   // largest |output| this thread writes in this tile (range monitor)
-#pragma unroll
-    for (int j = 0; j < BN / 8; ++j) {
-      const int n = n0 + 8 * j + col0;
-      if (n >= p.n_cols) continue;
+    if (p.epi_slots == 0) {
+      size_t opix[2] = {0, 0}, rpix[2] = {0, 0};
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
-        if (!valid[h]) continue;
-        float v[2];
+        const int m = m_blk * kBlockM + row0 + 8 * h;
+        if (valid[h]) {
+          const int img = m / p.HoWo;
+          const int rem = m - img * p.HoWo;
+          const int pp = rem / p.Wo + p.off_h;
+          const int qq = rem - (rem / p.Wo) * p.Wo + p.off_w;
+          opix[h] = (static_cast<size_t>(img) * p.out_H + pp) * p.out_W + qq;
+          rpix[h] = (static_cast<size_t>(img) * p.res_H + (pp >> p.res_shift)) * p.res_W + (qq >> p.res_shift);
+        }
+      }
 #pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          const int i = 4 * j + 2 * h + e;
-          if constexpr (!SPLIT) {
-            v[e] = acc0[i];
-          } else if constexpr (ACC) {
-            const float s = fmaf(acc1[i], kLoInv, sums[i]);
-            v[e] = fmaf(s, p.acc_delta, s);
-          } else {   // single-chunk (K <= 64) split layers: the same compensation
-            v[e] = fmaf(acc0[i], p.acc_delta, acc0[i]);
-            v[e] = fmaf(acc1[i], kLoInv, v[e]);
+      for (int j = 0; j < BN / 8; ++j) {
+        const int n = n0 + 8 * j + col0;
+        if (n >= p.n_cols) continue;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          if (!valid[h]) continue;
+          const int i = 4 * j + 2 * h;
+          epilogue_pair<SPLIT, SWISH>(p, out_value(i), out_value(i + 1), opix[h], rpix[h], n, amax);
+        }
+      }
+    } else {
+      // staged: one 64-column chunk at a time through this warpgroup's slot ring.  Slot layout = the TMA box with
+      // 128-byte swizzle: row r at r * 128, 16-byte unit u at (u ^ (r % 8)) * 16.  The 8 rows a warp's lanes hold
+      // have distinct r % 8, so every 4-byte access of the warp hits 32 distinct banks.
+#pragma unroll
+      for (int c = 0; c < BN / kChunkN; ++c) {
+        mbar_wait(&slot_full[cwg * kMaxSlots + eslot], ephase);
+        uint8_t* s_hi = slots + static_cast<size_t>(cwg * p.epi_slots + eslot) * p.slot_bytes;
+#pragma unroll
+        for (int u = 0; u < kChunkN / 8; ++u) {
+          const int j = c * (kChunkN / 8) + u;
+          const int n = n0 + 8 * j + col0;
+          if (n >= p.n_cols) continue;
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            if (!valid[h]) continue;
+            const int i = 4 * j + 2 * h;
+            const uint32_t off = (wg_row + 8 * h) * 128 + ((u ^ (lane >> 2)) << 4) + col0 * 2;
+            epilogue_pair_slot<SPLIT, SWISH>(p, out_value(i), out_value(i + 1), n,
+                                             reinterpret_cast<__half2*>(s_hi + off),
+                                             reinterpret_cast<__half2*>(s_hi + kSlotPlaneBytes + off), amax);
           }
         }
-        epilogue_pair<SPLIT, SWISH>(p, v[0], v[1], opix[h], rpix[h], n, amax);
+        fence_proxy_async_smem();   // the TMA store reads what this thread wrote
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&slot_written[cwg * kMaxSlots + eslot]);
+        if (++eslot == p.epi_slots) {
+          eslot = 0;
+          ephase ^= 1;
+        }
       }
     }
     // inf included; a NaN can only follow an inf, which an earlier launch has flagged
@@ -391,7 +557,8 @@ int encode_2d(CUtensorMap* m, const void* base, uint64_t inner, uint64_t outer, 
 }
 
 
-typedef void (*ConvKernel)(CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, ConvTcParams);
+typedef void (*ConvKernel)(CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap, CUtensorMap,
+                           CUtensorMap, ConvTcParams);
 
 template <int BN>
 ConvKernel kernel_for(bool split, bool acc, bool swish) {
@@ -408,6 +575,7 @@ ConvKernel kernel_for(int block_n, bool split, bool acc, bool swish) {
 
 struct ConvPlan {
   CUtensorMap tmA_hi, tmA_lo, tmB_hi, tmB_lo;
+  CUtensorMap tmO_hi, tmO_lo, tmR_hi, tmR_lo;   // staged epilogue: output / residual planes as [M][Cout_pad]
   ConvTcParams p;
   ConvKernel kernel;
   int grid;
@@ -471,7 +639,19 @@ static int plan_build(ConvPlan* pl, const ConvDesc& d, const ConvWeights& w, con
   p.b_slot_bytes = static_cast<uint32_t>(block_n) * kBlockK * 2;
   p.stage_bytes = (kABytes + p.b_slot_bytes) * (split ? 2 : 1);
   p.tx_bytes = (kABytes + static_cast<uint32_t>(b_rows) * kBlockK * 2) * (split ? 2 : 1);
-  p.num_stages = kSmemBudget / static_cast<int>(p.stage_bytes);
+  // Staged epilogue (results leave by TMA store, the residual arrives by TMA load) when output and residual are dense
+  // [M][Cout_pad] row-major matrices the tensor maps can describe: fp16 planes written without a placement offset, an
+  // unshifted residual of the same size, 16-byte aligned bases and row strides.
+  auto aligned16 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; };
+  const bool staged =
+      io.out_f32 == nullptr && d.off_h == 0 && d.off_w == 0 && d.out_H == Ho && d.out_W == Wo && aligned16(io.out_hi) &&
+      (!split || aligned16(io.out_lo)) &&
+      (io.res_hi == nullptr || (d.res_shift == 0 && d.res_H == Ho && d.res_W == Wo && d.ldr % 8 == 0 &&
+                                aligned16(io.res_hi) && (!split || aligned16(io.res_lo))));
+  p.epi_slots = !staged ? 0 : io.res_hi != nullptr ? kResSlots : kOutSlots;
+  p.slot_bytes = kSlotPlaneBytes * (split ? 2 : 1);
+  const int slot_total = 2 * p.epi_slots * static_cast<int>(p.slot_bytes);
+  p.num_stages = (kSmemBudget - slot_total) / static_cast<int>(p.stage_bytes);
   if (p.num_stages > kMaxStages) p.num_stages = kMaxStages;
   B2_CHECK(p.num_stages >= 2, "conv_tc: tile too large for shared memory");
   p.out_hi = io.out_hi;
@@ -502,7 +682,8 @@ static int plan_build(ConvPlan* pl, const ConvDesc& d, const ConvWeights& w, con
   if (p.acc_kb >= 2) p.acc_delta = getenv("B2_ACC_DELTA2") ? static_cast<float>(atof(getenv("B2_ACC_DELTA2"))) : kAccDelta2;
   pl->kernel = kernel_for(block_n, split, acc, d.relu == 2);
   pl->grid = p.num_tiles < num_sms ? p.num_tiles : num_sms;
-  pl->smem_bytes = static_cast<size_t>(p.num_stages) * p.stage_bytes + 1024 /*align*/ + 2 * kMaxStages * 8 /*barriers*/;
+  pl->smem_bytes = static_cast<size_t>(p.num_stages) * p.stage_bytes + slot_total + 1024 /*align*/ +
+                   (2 * kMaxStages + 4 * kMaxSlots) * 8 /*barriers*/;
   const int in_ld = d.in_ld > 0 ? d.in_ld : d.Cin;
   const bool plain = (d.R == 1 && d.S == 1 && d.stride == 1 && d.pad_t == 0 && d.pad_b == 0 && d.pad_l == 0 &&
                       d.pad_r == 0 && d.in_H == d.in_pitch_H && d.in_W == d.in_pitch_W);
@@ -548,6 +729,21 @@ static int plan_build(ConvPlan* pl, const ConvDesc& d, const ConvWeights& w, con
     pl->tmA_lo = pl->tmA_hi;
     pl->tmB_lo = pl->tmB_hi;
   }
+  // staged epilogue: 64 x 64 boxes of [M][Cout_pad]; stores clip the ragged last m- and n-blocks, loads zero-fill them
+  pl->tmO_hi = pl->tmO_lo = pl->tmR_hi = pl->tmR_lo = pl->tmB_hi;   // unused maps: any valid map
+  if (p.epi_slots > 0) {
+    const int planes = split ? 2 : 1;
+    for (int plane = 0; plane < planes; ++plane) {
+      const __half* o = plane == 0 ? io.out_hi : io.out_lo;
+      if (o && encode_2d(plane == 0 ? &pl->tmO_hi : &pl->tmO_lo, o, w.Cout_pad, p.M, static_cast<uint64_t>(d.ldc) * 2,
+                         kChunkN, kWgRows))
+        return -1;
+      const __half* r = plane == 0 ? io.res_hi : io.res_lo;
+      if (r && encode_2d(plane == 0 ? &pl->tmR_hi : &pl->tmR_lo, r, w.Cout_pad, p.M, static_cast<uint64_t>(d.ldr) * 2,
+                         kChunkN, kWgRows))
+        return -1;
+    }
+  }
   return 0;
 }
 
@@ -563,7 +759,8 @@ ConvPlan* conv_tc_plan_create(const ConvDesc& d, const ConvWeights& w, const Con
 void conv_tc_plan_destroy(ConvPlan* p) { delete p; }
 
 int conv_tc_launch(const ConvPlan* pl, cudaStream_t stream) {
-  pl->kernel<<<pl->grid, kThreads, pl->smem_bytes, stream>>>(pl->tmA_hi, pl->tmA_lo, pl->tmB_hi, pl->tmB_lo, pl->p);
+  pl->kernel<<<pl->grid, kThreads, pl->smem_bytes, stream>>>(pl->tmA_hi, pl->tmA_lo, pl->tmB_hi, pl->tmB_lo, pl->tmO_hi,
+                                                             pl->tmO_lo, pl->tmR_hi, pl->tmR_lo, pl->p);
   B2_CUDA(cudaGetLastError());
   return 0;
 }
