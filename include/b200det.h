@@ -57,6 +57,10 @@ typedef struct b2_config {
   int32_t add_mask;           /* --add_mask: mask head on the final boxes (models.py:934-961, 1173-1199; mrcnn_head_dim 256):
                                  ROIAlign 14x14 -> 4 x conv3x3 -> 2x2/2 transposed conv -> conv1x1 -> sigmoid of the box's own
                                  class; results through b2_get_masks */
+  int32_t use_gn;             /* --use_gn: GroupNorm (32 groups, statistics per image at run time, nn.py:81-108) instead of
+                                 folded BatchNorm in the backbone, and after every FPN lateral / post-hoc conv (nn.py:987-1009) */
+  int32_t conv_head_dim;      /* 0 = 2fc head; > 0: --use_conv_frcnn_head with conv_frcnn_head_dim channels (models.py:1110-1125):
+                                 4 x conv3x3 + ReLU (+ GroupNorm per ROI with use_gn) -> fc, replacing fc6 / fc7 */
 } b2_config;
 
 const char* b2_last_error(void);
@@ -308,6 +312,13 @@ int b2_track_spatial_dist(const int32_t* frames1, const double* pts1, const int3
 int b2_op_conv2d(int device, const float* x, const float* w, const float* bias, const float* res, int B, int H, int W,
                  int Cin, int R, int S, int Cout, int stride, int dil, int pad_t, int pad_b, int pad_l, int pad_r,
                  int relu, int res_shift, int impl, int split, int a_mode, float* out);
+/* GroupNorm (32 groups, eps 1e-5) of the view H x W at (off_h, off_w) of x [B][pitch_H][pitch_W][C] (host, fp32, converted to
+ * the engine's planes), then + res [B][res_H][res_W][C] read at (y >> res_shift, x >> res_shift) (res may be NULL), then ReLU.
+ * per_roi = 1: the box head's one-kernel form (statistics and apply per sample).  out [B][pitch_H][pitch_W][C]: the buffer
+ * after the op when in_place, else a zero-initialised output buffer of which only the view is written. */
+int b2_op_group_norm(int device, const float* x, const float* res, const float* gamma, const float* beta, int B,
+                     int pitch_H, int pitch_W, int C, int H, int W, int off_h, int off_w, int res_H, int res_W, int res_shift,
+                     int relu, int per_roi, int split, int in_place, float* out);
 
 #ifdef __cplusplus
 }

@@ -38,6 +38,9 @@ _DEFAULTS = dict(
     is_train=False,
     add_mask=False,
     mrcnn_head_dim=256,                # obj_detect_tracking.py:324
+    use_gn=False,                      # --use_gn (obj_detect_tracking.py:101-102): GroupNorm backbone + FPN
+    use_conv_frcnn_head=False,         # --use_conv_frcnn_head (:103-104): 4-conv box head
+    conv_frcnn_head_dim=256,           # only main.py:250 sets it (default 256); the inference drivers never do
     use_partial_classes=False,
     is_efficientdet=False,
 )

@@ -115,6 +115,12 @@ struct Layer {
                            // 5 stem, 6 mask-head transposed conv 2x2/2 (as a 1x1 conv onto 4 taps x C outputs)
 };
 
+// One GroupNorm of the plan (use_gn backbone / FPN, conv box head): normalises a conv output in place.
+struct GnOp {
+  std::string name;        // reference variable scope, e.g. "group1/block0/conv1/gn", "fpn/gn_c2", "fastrcnn/gn0"
+  GnParams p;              // full-batch launch; the half-batch launches offset it per image
+};
+
 struct StageRef {
   int kind;                // 0 planes, 1 f32, 2 i32
   Planes pl;
@@ -162,6 +168,8 @@ struct b2_ctx {
   RoiAlignParams roi1, roi2, roi3;
   HeadPostParams post;
   Planes roi_feat, fc6, fc7;
+  Planes head_a, head_b;           // conv box head (cfg.conv_head_dim > 0): [M][7][7][conv_head_dim] ping-pong
+  std::vector<std::unique_ptr<GnOp>> gns;
   float* head_logits = nullptr;
   float* box_feat = nullptr;
   float* box_feat_pooled = nullptr;
@@ -179,8 +187,10 @@ struct b2_ctx {
   struct Step {
     int phase;
     int kind;   // 0 conv layer, 1 stem, 2 maxpool, 3 subsample p6, 4 proposals, 5 roialign1, 6 post, 7 roialign2,
-                // 8 roialign 14x14 of the final boxes (mask head), 9 mask select + sigmoid
+                // 8 roialign 14x14 of the final boxes (mask head), 9 mask select + sigmoid,
+                // 10 GroupNorm statistics, 11 GroupNorm apply (+ residual, ReLU), 12 per-ROI GroupNorm (box head)
     Layer* layer;
+    GnOp* gn = nullptr;
   };
   std::vector<Step> steps;
   cudaGraphExec_t graph = nullptr;
@@ -270,6 +280,45 @@ Layer* add_conv(b2_ctx* c, int phase, const std::string& name, const Planes& in,
   return raw;
 }
 
+// GroupNorm `name` of the view (view_h x view_w at (off_h, off_w)) of `buf`, in place, then + `res` (read at
+// (y >> res_shift, x >> res_shift)) and ReLU: a statistics step and an apply step, or with per_roi one step that
+// normalises each [7][7][C] sample of the box head on chip.  Statistics scratch is allocated here, so capture works.
+int add_gn(b2_ctx* c, int phase, const std::string& name, const Planes& buf, int view_h, int view_w, int off_h, int off_w,
+           const Planes* res, int res_shift, bool relu, bool per_roi = false) {
+  std::unique_ptr<GnOp> G(new GnOp());
+  G->name = name;
+  GnParams& p = G->p;
+  memset(&p, 0, sizeof(p));
+  p.x_hi = buf.hi; p.x_lo = buf.lo; p.y_hi = buf.hi; p.y_lo = buf.lo;
+  p.B = buf.B; p.H = view_h; p.W = view_w; p.C = buf.C;
+  p.pitch_H = buf.H; p.pitch_W = buf.W; p.ld = buf.C; p.off_h = off_h; p.off_w = off_w;
+  if (res) {
+    p.r_hi = res->hi; p.r_lo = res->lo;
+    p.res_H = res->H; p.res_W = res->W; p.res_ld = res->C; p.res_shift = res_shift;
+  }
+  p.relu = relu ? 1 : 0;
+  p.gamma = c->alloc<float>(buf.C);
+  p.beta = c->alloc<float>(buf.C);
+  p.range_flag = c->range_flag;
+  B2_CHECK(p.gamma && p.beta, "out of device memory (GroupNorm " + name + ")");
+  if (!per_roi) {
+    p.chunks = gn_chunks(view_h, view_w, buf.C);
+    p.partial = c->alloc<float>(static_cast<size_t>(buf.B) * p.chunks * 32 * 3);
+    p.stats = c->alloc<float>(static_cast<size_t>(buf.B) * 32 * 2);
+    p.counter = c->alloc<unsigned int>(buf.B);
+    B2_CHECK(p.partial && p.stats && p.counter, "out of device memory (GroupNorm " + name + " statistics)");
+  }
+  GnOp* raw = G.get();
+  c->gns.push_back(std::move(G));
+  if (per_roi) {
+    c->steps.push_back({phase, 12, nullptr, raw});
+  } else {
+    c->steps.push_back({phase, 10, nullptr, raw});
+    c->steps.push_back({phase, 11, nullptr, raw});
+  }
+  return 0;
+}
+
 int log2i(int v) { int r = 0; while ((1 << r) < v) ++r; return r; }
 
 // generate_anchors.py:42-109 restated for one (stride, size): the 3 ratio anchors of a cell.
@@ -335,13 +384,17 @@ int build_plan(b2_ctx* c) {
   B2_CHECK(c->alloc_planes(c->c1, B, c->c1h, c->c1w, 64), "alloc c1");
   B2_CHECK(c->alloc_planes(c->pool, B, c->ch[0], c->cw[0], 64), "alloc pool");
   c->steps.push_back({0, 1, nullptr});
+  // use_gn (nn.py:859-862, 474-477): every backbone conv is a plain conv followed by GroupNorm steps that carry the ReLU
+  // and the residual; with BatchNorm the norm, ReLU and residual are in the conv epilogue
+  const bool gn = cfg.use_gn != 0;
   // conv0 as a 4x1 VALID conv over the packed operand (see stem.cu), BN + ReLU in the epilogue
   {
     Planes view = c->stem_u;
     view.C = 64;                       // one GEMM pixel = 4 consecutive operand pixels
-    Layer* L0 = add_conv(c, 0, "conv0", view, c->c1h + 3, c->c1w, 4, 1, 1, 0, 0, 0, 0, 64, true, false, true, c->c1, 0, 0,
+    Layer* L0 = add_conv(c, 0, "conv0", view, c->c1h + 3, c->c1w, 4, 1, 1, 0, 0, 0, 0, 64, !gn, false, !gn, c->c1, 0, 0,
                          nullptr, 0, nullptr, 0, 5, 1);
     L0->d.in_ld = 16;
+    if (gn && add_gn(c, 0, "conv0/gn", c->c1, c->c1h, c->c1w, 0, 0, nullptr, 0, true)) return -1;
   }
   c->steps.push_back({0, 2, nullptr});
   reg_planes(c, "c1", c->c1);
@@ -368,33 +421,41 @@ int build_plan(b2_ctx* c) {
       const int dil = (g == 3 && cfg.use_dilations && in_last3) ? 2 : 1;
       const Planes& x = cur;
       const Planes& a1 = (i == 0) ? t1_first : t1;
-      add_conv(c, 0, p + "/conv1", x, x.H, x.W, 1, 1, 1, 0, 0, 0, 0, feat, true, false, true, a1, 0, 0, nullptr, 0);
+      add_conv(c, 0, p + "/conv1", x, x.H, x.W, 1, 1, 1, 0, 0, 0, 0, feat, !gn, false, !gn, a1, 0, 0, nullptr, 0);
+      if (gn && add_gn(c, 0, p + "/conv1/gn", a1, a1.H, a1.W, 0, 0, nullptr, 0, true)) return -1;
       const Planes* a2 = &t2;
       if (stride == 2) {
         // pad [1,0] + 3x3 stride-2 VALID (nn.py:487-492); with dilation the output is padded [1,0] again
-        // (nn.py:493-497): written at offset (1,1) of a buffer whose first row/col stay zero.
+        // (nn.py:493-497): written at offset (1,1) of a buffer whose first row/col stay zero.  GroupNorm + ReLU run
+        // before that pad (nn.py:490-497): their view is the conv output, so the pad row / column stay out of the
+        // statistics and stay 0.
         a2 = &t2_first;
         const int off = dil != 1 ? 1 : 0;
-        add_conv(c, 0, p + "/conv2", a1, a1.H, a1.W, 3, 2, dil, 1, 0, 1, 0, feat, true, false, true, *a2, off, off,
-                 nullptr, 0);
+        Layer* L2 = add_conv(c, 0, p + "/conv2", a1, a1.H, a1.W, 3, 2, dil, 1, 0, 1, 0, feat, !gn, false, !gn, *a2, off,
+                             off, nullptr, 0);
+        if (gn && add_gn(c, 0, p + "/conv2/gn", *a2, L2->d.Ho(), L2->d.Wo(), off, off, nullptr, 0, true)) return -1;
       } else {
-        add_conv(c, 0, p + "/conv2", a1, a1.H, a1.W, 3, 1, dil, dil, dil, dil, dil, feat, true, false, true, *a2, 0,
+        add_conv(c, 0, p + "/conv2", a1, a1.H, a1.W, 3, 1, dil, dil, dil, dil, dil, feat, !gn, false, !gn, *a2, 0,
                  0, nullptr, 0);
+        if (gn && add_gn(c, 0, p + "/conv2/gn", *a2, a2->H, a2->W, 0, 0, nullptr, 0, true)) return -1;
       }
       const Planes* resid = &x;
       if (x.C != feat * 4) {
         // resnet_shortcut (nn.py:551-566): stride 2 => drop last row/col, 1x1 stride-2 VALID
         if (stride == 2)
-          add_conv(c, 0, p + "/convshortcut", x, x.H, x.W, 1, 2, 1, 0, -1, 0, -1, feat * 4, true, false, false, sc, 0,
+          add_conv(c, 0, p + "/convshortcut", x, x.H, x.W, 1, 2, 1, 0, -1, 0, -1, feat * 4, !gn, false, false, sc, 0,
                    0, nullptr, 0);
         else
-          add_conv(c, 0, p + "/convshortcut", x, x.H, x.W, 1, 1, 1, 0, 0, 0, 0, feat * 4, true, false, false, sc, 0,
+          add_conv(c, 0, p + "/convshortcut", x, x.H, x.W, 1, 1, 1, 0, 0, 0, 0, feat * 4, !gn, false, false, sc, 0,
                    0, nullptr, 0);
+        if (gn && add_gn(c, 0, p + "/convshortcut/gn", sc, sc.H, sc.W, 0, 0, nullptr, 0, false)) return -1;
         resid = &sc;
       }
       const Planes& out = pingpong[i & 1];
-      add_conv(c, 0, p + "/conv3", *a2, a2->H, a2->W, 1, 1, 1, 0, 0, 0, 0, feat * 4, true, false, true, out, 0, 0,
-               resid, 0);
+      add_conv(c, 0, p + "/conv3", *a2, a2->H, a2->W, 1, 1, 1, 0, 0, 0, 0, feat * 4, !gn, false, !gn, out, 0, 0,
+               gn ? nullptr : resid, 0);
+      // relu(gn(conv3) + shortcut) (nn.py:512-521, 586-587)
+      if (gn && add_gn(c, 0, p + "/conv3/gn", out, out.H, out.W, 0, 0, resid, 0, true)) return -1;
       cur = out;
     }
     c->cfeat[g] = cur;
@@ -406,14 +467,22 @@ int build_plan(b2_ctx* c) {
   for (int i = 3; i >= 0; --i) {
     B2_CHECK(c->alloc_planes(c->lat[i], B, c->ch[i], c->cw[i], nc), "alloc lateral");
     const std::string nm = "fpn/lateral_1x1_c" + std::to_string(i + 2);
+    // use_gn: GroupNorm of the lateral before the top-down sum (gn_c*, nn.py:987-990); its apply step does the
+    // nearest-2x upsample-add that the conv epilogue does otherwise
+    const Planes* up = i < 3 ? &c->lat[i + 1] : nullptr;
     add_conv(c, 1, nm, c->cfeat[i], c->ch[i], c->cw[i], 1, 1, 1, 0, 0, 0, 0, nc, false, true, false, c->lat[i], 0, 0,
-             i < 3 ? &c->lat[i + 1] : nullptr, 1);
+             gn ? nullptr : up, 1);
+    if (gn && add_gn(c, 1, "fpn/gn_c" + std::to_string(i + 2), c->lat[i], c->ch[i], c->cw[i], 0, 0, up, 1, false))
+      return -1;
   }
   for (int i = 0; i < 4; ++i) {
     B2_CHECK(c->alloc_planes(c->pfeat[i], B, c->pfh[i], c->pfw[i], nc), "alloc p");
     const std::string nm = "fpn/posthoc_3x3_p" + std::to_string(i + 2);
     add_conv(c, 1, nm, c->lat[i], c->ch[i], c->cw[i], 3, 1, 1, 1, 1, 1, 1, nc, false, true, false, c->pfeat[i], 0, 0,
              nullptr, 0);
+    // gn_p* (nn.py:1007-1009) over the whole, uncropped level; p6 below subsamples the normalised p5
+    if (gn && add_gn(c, 1, "fpn/gn_p" + std::to_string(i + 2), c->pfeat[i], c->pfh[i], c->pfw[i], 0, 0, nullptr, 0, false))
+      return -1;
     reg_planes(c, "p" + std::to_string(i + 2), c->pfeat[i]);
   }
   B2_CHECK(c->alloc_planes(c->pfeat[4], B, c->pfh[4], c->pfw[4], nc), "alloc p6");
@@ -489,22 +558,53 @@ int build_plan(b2_ctx* c) {
   // ---- box head (models.py:1030-1108), phase 5: fc6, fc7, class+box outputs fused (N = 5*num_class) ----
   const int dim = cfg.fc_head_dim;
   B2_CHECK(dim % 64 == 0, "b2_create: fc_head_dim must be a multiple of 64");
-  B2_CHECK(c->alloc_planes(c->fc6, 1, 1, Mpad, dim), "alloc fc6");
-  B2_CHECK(c->alloc_planes(c->fc7, 1, 1, Mpad, dim), "alloc fc7");
+  const int hd = cfg.conv_head_dim;
+  if (hd <= 0) {
+    B2_CHECK(c->alloc_planes(c->fc6, 1, 1, Mpad, dim), "alloc fc6");
+    B2_CHECK(c->alloc_planes(c->fc7, 1, 1, Mpad, dim), "alloc fc7");
+  }
   const int nout = cfg.num_class + (cfg.class_agnostic ? 4 : cfg.num_class * 4);
   const int ldo = (nout + 15) / 16 * 16;
   c->head_logits = c->alloc<float>(static_cast<size_t>(Mpad) * ldo);
   Planes rf = c->roi_feat; rf.W = M;
-  Planes f6 = c->fc6; f6.W = M;
-  Planes f7 = c->fc7; f7.W = M;
-  add_conv(c, 5, "fastrcnn/fc6", rf, 1, M, 1, 1, 1, 0, 0, 0, 0, dim, false, true, true, f6, 0, 0, nullptr, 0, nullptr,
-           0, 1);
-  add_conv(c, 5, "fastrcnn/fc7", f6, 1, M, 1, 1, 1, 0, 0, 0, 0, dim, false, true, true, f7, 0, 0, nullptr, 0, nullptr,
-           0, 2);
-  add_conv(c, 5, "fastrcnn/outputs", f7, 1, M, 1, 1, 1, 0, 0, 0, 0, nout, false, true, false, Planes(), 0, 0, nullptr,
-           0, c->head_logits, ldo, 4);
-  reg_planes(c, "fc6", f6);
-  reg_planes(c, "fc7", f7);
+  if (hd > 0) {
+    // conv_frcnn_head (models.py:1110-1125), use_conv_frcnn_head: 4 x [conv 3x3 SAME + bias + ReLU, then GroupNorm per ROI
+    // if use_gn] on the [M][7][7] ROI maps (the ROIAlign rows are already (y*7+x)*256+c per ROI: M small images, as in the
+    // mask head), then dense "fc" + ReLU over the NCHW flatten (fc6's row permutation with conv_head_dim channels)
+    B2_CHECK(hd % 64 == 0 && hd <= 2048 && (!gn || 2048 % hd == 0),
+             "b2_create: conv_head_dim must be a multiple of 64 (a power of two from 64 to 2048 with use_gn)");
+    B2_CHECK(c->alloc_planes(c->head_a, Mpad, 7, 7, hd) && c->alloc_planes(c->head_b, Mpad, 7, 7, hd), "alloc conv head");
+    B2_CHECK(c->alloc_planes(c->fc6, 1, 1, Mpad, dim), "alloc fc");
+    Planes rf7 = c->roi_feat; rf7.B = M; rf7.H = 7; rf7.W = 7; rf7.C = nc;
+    Planes ha = c->head_a; ha.B = M;
+    Planes hb = c->head_b; hb.B = M;
+    Planes cur_h = rf7;
+    for (int k = 0; k < 4; ++k) {
+      const Planes& o = (k & 1) ? hb : ha;
+      add_conv(c, 5, "fastrcnn/conv" + std::to_string(k), cur_h, 7, 7, 3, 1, 1, 1, 1, 1, 1, hd, false, true, true, o, 0, 0,
+               nullptr, 0);
+      if (gn && add_gn(c, 5, "fastrcnn/gn" + std::to_string(k), o, 7, 7, 0, 0, nullptr, 0, false, true)) return -1;
+      cur_h = o;
+    }
+    Planes flat = cur_h; flat.B = 1; flat.H = 1; flat.W = M; flat.C = 49 * hd;
+    Planes f = c->fc6; f.W = M;
+    add_conv(c, 5, "fastrcnn/fc", flat, 1, M, 1, 1, 1, 0, 0, 0, 0, dim, false, true, true, f, 0, 0, nullptr, 0, nullptr,
+             0, 1);
+    add_conv(c, 5, "fastrcnn/outputs", f, 1, M, 1, 1, 1, 0, 0, 0, 0, nout, false, true, false, Planes(), 0, 0, nullptr,
+             0, c->head_logits, ldo, 4);
+    reg_planes(c, "fc", f);
+  } else {
+    Planes f6 = c->fc6; f6.W = M;
+    Planes f7 = c->fc7; f7.W = M;
+    add_conv(c, 5, "fastrcnn/fc6", rf, 1, M, 1, 1, 1, 0, 0, 0, 0, dim, false, true, true, f6, 0, 0, nullptr, 0, nullptr,
+             0, 1);
+    add_conv(c, 5, "fastrcnn/fc7", f6, 1, M, 1, 1, 1, 0, 0, 0, 0, dim, false, true, true, f7, 0, 0, nullptr, 0, nullptr,
+             0, 2);
+    add_conv(c, 5, "fastrcnn/outputs", f7, 1, M, 1, 1, 1, 0, 0, 0, 0, nout, false, true, false, Planes(), 0, 0, nullptr,
+             0, c->head_logits, ldo, 4);
+    reg_planes(c, "fc6", f6);
+    reg_planes(c, "fc7", f7);
+  }
   reg_raw(c, "head_logits", c->head_logits, 1, B, K, ldo, 1);
 
   // ---- post-processing (phase 6) ----
@@ -676,8 +776,32 @@ int run_step(b2_ctx* c, const b2_ctx::Step& s) {
       B2_CUDA(cudaGetLastError());
       return 0;
     }
+    case 10:
+      return gn_stats_launch(s.gn->p, st);
+    case 11:
+      return gn_apply_launch(s.gn->p, st);
+    case 12:
+      return gn_roi_launch(s.gn->p, st);
   }
   return -1;
+}
+
+// The launch of GroupNorm `p` restricted to images [h * hb, (h + 1) * hb).
+GnParams gn_part(GnParams p, int h, int hb) {
+  const size_t xo = static_cast<size_t>(h) * hb * p.pitch_H * p.pitch_W * p.ld;
+  p.x_hi += xo; p.y_hi += xo;
+  if (p.x_lo) p.x_lo += xo;
+  if (p.y_lo) p.y_lo += xo;
+  if (p.r_hi) {
+    const size_t ro = static_cast<size_t>(h) * hb * p.res_H * p.res_W * p.res_ld;
+    p.r_hi += ro;
+    if (p.r_lo) p.r_lo += ro;
+  }
+  p.partial += static_cast<size_t>(h) * hb * p.chunks * 32 * 3;
+  p.stats += static_cast<size_t>(h) * hb * 32 * 2;
+  p.counter += static_cast<size_t>(h) * hb;
+  p.B = hb;
+  return p;
 }
 
 // One step of phases 0-2 over part `h` (of nsplit) of the batch, on stream `st`.
@@ -705,6 +829,10 @@ int run_step_half(b2_ctx* c, const b2_ctx::Step& s, int h, cudaStream_t st) {
       B2_CUDA(cudaGetLastError());
       return 0;
     }
+    case 10:
+      return gn_stats_launch(gn_part(s.gn->p, h, hb), st);
+    case 11:
+      return gn_apply_launch(gn_part(s.gn->p, h, hb), st);
   }
   return -1;
 }
@@ -714,6 +842,7 @@ int step_launches(const b2_ctx::Step& s) {
     case 4: return 2;
     case 6: return 3;
     case 7: return 2;
+    case 10: case 11: case 12: return 1;   // GroupNorm statistics / apply / per-ROI
     default: return 1;
   }
 }
@@ -845,7 +974,7 @@ int load_layer(b2_ctx* c, Layer* L, const WeightSet& ws) {
     // stem: reference HWIO [7,7,3,64] re-indexed for the packed operand (stem.cu):
     // W'[o][r][s*16 + ry*6 + sx*3 + c] = W[2r+ry][2s+sx][c][o]   (12 real + 4 zero channels per width tap s)
     const float* w = ws.get(L->name + "/W", 7 * 7 * 3 * 64);
-    if (!w || bn_fold(ws, L->name, Cout, scale, shift)) return -1;
+    if (!w || (L->has_bn && bn_fold(ws, L->name, Cout, scale, shift))) return -1;
     for (int r = 0; r < 4; ++r)
       for (int ch = 0; ch < 64; ++ch) {
         const int s4 = ch / 16, r12 = ch % 16, ry = r12 / 6, sx = (r12 % 6) / 3, cc = r12 % 3;
@@ -856,9 +985,9 @@ int load_layer(b2_ctx* c, Layer* L, const WeightSet& ws) {
           packed[static_cast<size_t>(o) * K + static_cast<size_t>(r) * Cin + ch] = static_cast<float>(src[o] * scale[o]);
       }
   } else if (L->kind == 1) {
-    // fc6: reference flattens NCHW (index c*49 + y*7 + x, models.py:1056 + nn.py:738-740);
+    // fc6 (and the conv head's fc): reference flattens NCHW (index c*49 + y*7 + x, models.py:1056 + nn.py:738-740);
     // our ROI features are [y][x][c], so permute the rows of W [in, out].
-    const int C = c->cfg.fpn_num_channel;
+    const int C = Cin / 49;
     const float* w = ws.get(L->name + "/W", static_cast<int64_t>(Cin) * Cout);
     const float* b = ws.get(L->name + "/b", Cout);
     if (!w || !b) return -1;
@@ -895,6 +1024,20 @@ int load_layer(b2_ctx* c, Layer* L, const WeightSet& ws) {
   }
   for (int o = 0; o < Cout; ++o) bias[o] = static_cast<float>(shift[o]);
   return upload_layer(c, L, packed, bias);
+}
+
+// group_norm's "<scope>/gamma" and "<scope>/beta" (nn.py:97-102), [C] each
+int load_gn(b2_ctx* c, GnOp* G, const WeightSet& ws) {
+  const int C = G->p.C;
+  const float* g = ws.get(G->name + "/gamma", C);
+  const float* b = ws.get(G->name + "/beta", C);
+  if (!g || !b) return -1;
+  for (int i = 0; i < C; ++i)
+    B2_CHECK(std::isfinite(g[i]) && std::isfinite(b[i]), "GroupNorm " + G->name + ": gamma / beta not finite");
+  B2_CUDA(cudaMemcpyAsync(const_cast<float*>(G->p.gamma), g, C * sizeof(float), cudaMemcpyHostToDevice, c->stream));
+  B2_CUDA(cudaMemcpyAsync(const_cast<float*>(G->p.beta), b, C * sizeof(float), cudaMemcpyHostToDevice, c->stream));
+  B2_CUDA(cudaStreamSynchronize(c->stream));
+  return 0;
 }
 
 }  // namespace
@@ -978,6 +1121,8 @@ int b2_load_weights(b2_ctx* c, const char* const* names, const float* const* dat
   // shared RPN weights: packed once, every level's layer gets its own copy of the (small) operand
   for (auto& L : c->layers)
     if (load_layer(c, L.get(), ws)) return -1;
+  for (auto& G : c->gns)
+    if (load_gn(c, G.get(), ws)) return -1;
   c->weights_loaded = true;
   return 0;
 }
@@ -1049,7 +1194,8 @@ int b2_step_info(b2_ctx* c, int idx, char* name, int name_cap, double* flops, do
   B2_CHECK(idx >= 0 && idx < static_cast<int>(c->steps.size()), "b2_step_info: index out of range");
   const b2_ctx::Step& s = c->steps[idx];
   static const char* kKindNames[] = {"conv", "stem_pack", "maxpool", "p6_subsample", "rpn_proposals", "roialign_proposals",
-                                     "head_post", "roialign_final", "roialign_mask", "mask_select"};
+                                     "head_post", "roialign_final", "roialign_mask", "mask_select", "gn_stats", "gn_apply",
+                                     "gn_roi"};
   std::string nm = s.kind == 0 ? s.layer->name : kKindNames[s.kind];
   *kind = s.kind;
   *flops = 0;
@@ -1070,6 +1216,15 @@ int b2_step_info(b2_ctx* c, int idx, char* name, int name_cap, double* flops, do
     *bytes = static_cast<double>(c->img_bytes) + static_cast<double>(c->stem_u.elems()) * esz;
   } else if (s.kind == 2) {
     *bytes = (static_cast<double>(c->c1.elems()) + c->pool.elems()) * esz;
+  } else if (s.kind >= 10 && s.kind <= 12) {
+    // GroupNorm: statistics read the view once; apply / per-ROI read it, write it and read the residual (a quarter of
+    // the view's size when it is upsampled)
+    const GnParams& p = s.gn->p;
+    const double n = static_cast<double>(p.B) * p.H * p.W * p.C;
+    *bytes = s.kind == 10 ? n * esz : 2.0 * n * esz + (p.r_hi ? n * esz / (p.res_shift ? 4.0 : 1.0) : 0.0);
+    nm = s.gn->name + (s.kind == 10 ? " stats" : s.kind == 11 ? " apply" : " per-roi") + " [" + std::to_string(p.H) +
+         "x" + std::to_string(p.W) + "x" + std::to_string(p.C) +
+         (s.kind != 10 && p.r_hi ? (p.res_shift ? " +up2" : " +res") : "") + (s.kind != 10 && p.relu ? " relu" : "") + "]";
   }
   snprintf(name, name_cap, "%s", nm.c_str());
   return 0;
@@ -1705,6 +1860,78 @@ int b2_op_conv2d(int device, const float* x, const float* w, const float* bias, 
   cudaFree(dx); cudaFree(dw); cudaFree(dof); cudaFree(xh); cudaFree(xl); cudaFree(cw.w_hi); cudaFree(cw.w_lo);
   cudaFree(oh); cudaFree(ol); cudaFree(cw.bias);
   if (res) { cudaFree(dr); cudaFree(rh); cudaFree(rl); }
+  return 0;
+}
+
+// ---- single GroupNorm op for kernel parity tests ------------------------------------------------
+
+int b2_op_group_norm(int device, const float* x, const float* res, const float* gamma, const float* beta, int B,
+                     int pitch_H, int pitch_W, int C, int H, int W, int off_h, int off_w, int res_H, int res_W, int res_shift,
+                     int relu, int per_roi, int split, int in_place, float* out) {
+  B2_CHECK(x && gamma && beta && out, "b2_op_group_norm: null argument");
+  B2_CHECK(B >= 1 && H >= 1 && W >= 1 && off_h >= 0 && off_w >= 0 && off_h + H <= pitch_H && off_w + W <= pitch_W,
+           "b2_op_group_norm: view outside the buffer");
+  B2_CHECK(!res || (res_shift >= 0 && ((H - 1) >> res_shift) < res_H && ((W - 1) >> res_shift) < res_W),
+           "b2_op_group_norm: residual smaller than the view");
+  B2_CUDA(cudaSetDevice(device));
+  const size_t n = static_cast<size_t>(B) * pitch_H * pitch_W * C, nr = res ? static_cast<size_t>(B) * res_H * res_W * C : 0;
+  std::vector<void*> bufs;
+  auto dalloc = [&](size_t bytes) -> void* {
+    void* p = nullptr;
+    if (cudaMalloc(&p, bytes + 256) != cudaSuccess) return nullptr;
+    cudaMemset(p, 0, bytes + 256);
+    bufs.push_back(p);
+    return p;
+  };
+  auto release = [&]() { for (void* p : bufs) cudaFree(p); };
+  float* f32 = static_cast<float*>(dalloc(std::max(n, nr) * 4));
+  __half* xh = static_cast<__half*>(dalloc(n * 2));
+  __half* xl = split ? static_cast<__half*>(dalloc(n * 2)) : nullptr;
+  __half* yh = in_place ? xh : static_cast<__half*>(dalloc(n * 2));
+  __half* yl = in_place ? xl : (split ? static_cast<__half*>(dalloc(n * 2)) : nullptr);
+  __half* rh = res ? static_cast<__half*>(dalloc(nr * 2)) : nullptr;
+  __half* rl = res && split ? static_cast<__half*>(dalloc(nr * 2)) : nullptr;
+  float* dg = static_cast<float*>(dalloc(C * 4));
+  float* db = static_cast<float*>(dalloc(C * 4));
+  GnParams p;
+  memset(&p, 0, sizeof(p));
+  p.chunks = gn_chunks(H, W, C);
+  p.partial = static_cast<float*>(dalloc(static_cast<size_t>(B) * p.chunks * 32 * 3 * 4));
+  p.stats = static_cast<float*>(dalloc(static_cast<size_t>(B) * 32 * 2 * 4));
+  p.counter = static_cast<unsigned int*>(dalloc(static_cast<size_t>(B) * 4));
+  for (void* q : bufs)
+    if (!q) { release(); B2_CHECK(false, "b2_op_group_norm: out of device memory"); }
+  int rc = 0;
+  cudaError_t e = cudaMemcpy(f32, x, n * 4, cudaMemcpyHostToDevice);
+  if (e == cudaSuccess) rc = f32_to_planes(f32, xh, xl, n, nullptr);
+  if (e == cudaSuccess && !rc && res) {
+    e = cudaMemcpy(f32, res, nr * 4, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) rc = f32_to_planes(f32, rh, rl, nr, nullptr);
+  }
+  if (e == cudaSuccess) e = cudaMemcpy(dg, gamma, C * 4, cudaMemcpyHostToDevice);
+  if (e == cudaSuccess) e = cudaMemcpy(db, beta, C * 4, cudaMemcpyHostToDevice);
+  p.x_hi = xh; p.x_lo = xl; p.y_hi = yh; p.y_lo = yl;
+  p.B = B; p.H = H; p.W = W; p.C = C;
+  p.pitch_H = pitch_H; p.pitch_W = pitch_W; p.ld = C; p.off_h = off_h; p.off_w = off_w;
+  if (res) {
+    p.r_hi = rh; p.r_lo = rl; p.res_H = res_H; p.res_W = res_W; p.res_ld = C; p.res_shift = res_shift;
+  }
+  p.relu = relu;
+  p.gamma = dg; p.beta = db;
+  if (e == cudaSuccess && !rc) {
+    if (per_roi) {
+      rc = gn_roi_launch(p, nullptr);
+    } else {
+      rc = gn_stats_launch(p, nullptr);
+      if (!rc) rc = gn_apply_launch(p, nullptr);
+    }
+  }
+  if (e == cudaSuccess && !rc) e = cudaDeviceSynchronize();
+  if (e == cudaSuccess && !rc) rc = planes_to_f32(yh, yl, f32, n, nullptr);
+  if (e == cudaSuccess && !rc) e = cudaMemcpy(out, f32, n * 4, cudaMemcpyDeviceToHost);
+  release();
+  if (rc) return -1;
+  B2_CUDA(e);
   return 0;
 }
 

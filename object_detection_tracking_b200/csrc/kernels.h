@@ -77,6 +77,31 @@ struct HeadPostParams {
 };
 int head_post_launch(const HeadPostParams& p, cudaStream_t s);
 
+// groupnorm.cu -- GroupNorm of a conv output at run time (nn.py:81-108), 32 groups, eps 1e-5
+struct GnParams {
+  const __half* x_hi;         // input planes (NHWC); the view is H x W at (off_h, off_w) of a pitch_H x pitch_W buffer
+  const __half* x_lo;         // nullptr in fp16 precision
+  __half* y_hi;               // output planes, same geometry as x (may be x: in place); only the view is written
+  __half* y_lo;
+  int B, H, W, C;             // images (ROIs for gn_roi), view extents, channels
+  int pitch_H, pitch_W, ld, off_h, off_w;
+  const __half* r_hi;         // optional residual added after the normalisation: pixel (y >> res_shift, x >> res_shift)
+  const __half* r_lo;         // of a res_H x res_W buffer with pixel stride res_ld (res_shift 1 = nearest 2x upsample)
+  int res_H, res_W, res_ld, res_shift;
+  int relu;                   // ReLU after the (normalise, residual) sum
+  const float* gamma;         // [C]
+  const float* beta;          // [C]
+  int chunks;                 // pixel chunks per image (gn_chunks): blocks per image of gn_stats / gn_apply
+  float* partial;             // [B][chunks][32][3] (count, mean, M2) per chunk and group
+  float* stats;               // [B][32][2] (mean, var) per image and group
+  unsigned int* counter;      // [B] finished-chunk tickets, zero between launches
+  unsigned int* range_flag;   // ORed with 1 when an output leaves the fp16 range (nullptr = not monitored)
+};
+int gn_chunks(int H, int W, int C);
+int gn_stats_launch(const GnParams& p, cudaStream_t s);
+int gn_apply_launch(const GnParams& p, cudaStream_t s);
+int gn_roi_launch(const GnParams& p, cudaStream_t s);   // per sample statistics + apply in one kernel (7x7 ROI maps)
+
 // reid.cu
 int dwconv3x3_launch(const __half* in_hi, const __half* in_lo, int B, int H, int W, int C, const float* w,
                      const float* bias, __half* out_hi, __half* out_lo, cudaStream_t s);

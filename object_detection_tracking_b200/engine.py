@@ -239,6 +239,26 @@ def op_conv2d(x, w, bias=None, res=None, stride=1, dil=1, pad=(0, 0, 0, 0), relu
     return out
 
 
+def op_group_norm(x, gamma, beta, view=None, res=None, res_shift=0, relu=False, per_roi=False, split=True,
+                  in_place=True, device=0) -> np.ndarray:
+    """GroupNorm (32 groups) of a NHWC buffer x [B, pitch_H, pitch_W, C] through the C ABI -- used by the kernel tests.
+    view = (off_h, off_w, H, W) restricts it to a window (default: the whole buffer); res [B, rH, rW, C] is added after
+    the normalisation at (y >> res_shift, x >> res_shift), then ReLU.  Returns the buffer after the op (in_place) or a
+    zero-initialised output buffer of which only the view is written."""
+    lib = _lib.load()
+    x = np.ascontiguousarray(x, dtype=np.float32)
+    B, PH, PW, C = x.shape
+    oh, ow, H, W = view if view is not None else (0, 0, PH, PW)
+    r = None if res is None else np.ascontiguousarray(res, dtype=np.float32)
+    rH, rW = (0, 0) if r is None else r.shape[1:3]
+    out = np.zeros_like(x)
+    _lib.check(lib.b2_op_group_norm(device, _lib.ptr(x), _lib.ptr(r), _lib.ptr(np.ascontiguousarray(gamma, np.float32)),
+                                    _lib.ptr(np.ascontiguousarray(beta, np.float32)), B, PH, PW, C, H, W, oh, ow, rH, rW,
+                                    int(res_shift), int(relu), int(per_roi), int(split), int(in_place), _lib.ptr(out)),
+               "b2_op_group_norm")
+    return out
+
+
 def get_new_hw(h, w, size, max_size):
     """nn.py:1548-1560: (neww, newh) of resizeImage for an h x w frame."""
     scale = size * 1.0 / min(h, w)

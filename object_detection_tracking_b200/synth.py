@@ -11,6 +11,8 @@ weights.  Names follow the Tensorpack-npz convention the reference loads
   fpn/lateral_1x1_c{2..5}/{W,b}, fpn/posthoc_3x3_p{2..5}/{W,b}
   rpn/conv0/{W,b}, rpn/class/{W,b}, rpn/box/{W,b}
   fastrcnn/fc6/{W,b}, fastrcnn/fc7/{W,b}, fastrcnn/outputs/{class,box}/{W,b}
+  use_gn: <conv scope>/gn/{gamma,beta} instead of bn/..., fpn/gn_c{2..5}/.., fpn/gn_p{2..5}/..
+  use_conv_frcnn_head: fastrcnn/conv{0..3}/{W,b} (+ fastrcnn/gn{0..3}/.. with use_gn), fastrcnn/fc/{W,b}
 
 Conv kernels are HWIO (`nn.py:350,367`), dense kernels [in,out] (`nn.py:753`).
 The distributions are chosen so activations stay O(1) through 33 residual blocks
@@ -88,7 +90,49 @@ def synth_weights(cfg, seed: int = 1234) -> dict:
         w["maskrcnn/deconv/b"] = (rng.standard_normal(md) * 0.02).astype(np.float32)
         w["maskrcnn/conv/W"] = (rng.standard_normal((1, 1, md, ncls - 1)) * np.sqrt(4.0 / md)).astype(np.float32)
         w["maskrcnn/conv/b"] = (rng.standard_normal(ncls - 1) * 0.5).astype(np.float32)
+    # The GroupNorm and conv-head variables are drawn after everything above, and the BatchNorm / fc6 / fc7 values they
+    # replace are still drawn (then dropped): every weight a seed shares between the model families stays the same.
+    if getattr(cfg, "use_gn", False):                # group_norm (nn.py:81-108) instead of every backbone BatchNorm
+        for k in [k for k in w if "/bn/" in k]:
+            del w[k]
+        for scope, c, last in _backbone_norm_scopes(cfg):
+            # residual-branch last GN: small gamma keeps the running sum bounded (as for BN above)
+            _gn(rng, w, scope + "/gn", c, 0.1 if last else 0.8, 0.3 if last else 1.2)
+        for i in range(4):
+            _gn(rng, w, "fpn/gn_c%d" % (i + 2), nc)
+            _gn(rng, w, "fpn/gn_p%d" % (i + 2), nc)
+    if getattr(cfg, "use_conv_frcnn_head", False):   # conv_frcnn_head (models.py:1110-1125) instead of fc6 / fc7
+        hd = int(getattr(cfg, "conv_frcnn_head_dim", 256))
+        for k in ("fastrcnn/fc6/W", "fastrcnn/fc6/b", "fastrcnn/fc7/W", "fastrcnn/fc7/b"):
+            del w[k]
+        for k in range(4):
+            w["fastrcnn/conv%d/W" % k] = _conv_w(rng, 3, nc if k == 0 else hd, hd)
+            w["fastrcnn/conv%d/b" % k] = (rng.standard_normal(hd) * 0.02).astype(np.float32)
+            if getattr(cfg, "use_gn", False):
+                _gn(rng, w, "fastrcnn/gn%d" % k, hd)
+        fin = hd * 7 * 7
+        w["fastrcnn/fc/W"] = (rng.standard_normal((fin, dim)) * np.sqrt(2.0 / fin)).astype(np.float32)
+        w["fastrcnn/fc/b"] = (rng.standard_normal(dim) * 0.02).astype(np.float32)
     return w
+
+
+def _gn(rng, w, name, c, gamma_lo=0.8, gamma_hi=1.2):
+    w[name + "/gamma"] = rng.uniform(gamma_lo, gamma_hi, c).astype(np.float32)
+    w[name + "/beta"] = (rng.standard_normal(c) * 0.05).astype(np.float32)
+
+
+def _backbone_norm_scopes(cfg):
+    """(conv scope, channels, is the residual branch's last conv) of every normalised backbone conv, in graph order."""
+    out = [("conv0", 64, False)]
+    cin = 64
+    for g, (feat, count) in enumerate(zip((64, 128, 256, 512), cfg.resnet_num_block)):
+        for i in range(count):
+            p = "group%d/block%d" % (g, i)
+            out += [(p + "/conv1", feat, False), (p + "/conv2", feat, False), (p + "/conv3", feat * 4, True)]
+            if cin != feat * 4:
+                out.append((p + "/convshortcut", feat * 4, False))
+            cin = feat * 4
+    return out
 
 
 def frcnn_weight_shapes(cfg) -> dict:
@@ -103,7 +147,13 @@ def frcnn_weight_shapes(cfg) -> dict:
         if bias:
             sh[name + "/b"] = (cout,)
 
+    gn = getattr(cfg, "use_gn", False)
+
     def bn(name, c):
+        if gn:                                       # group_norm "<scope>/gn/{gamma,beta}" (nn.py:97-102, 591-603)
+            for k in ("gamma", "beta"):
+                sh["%s/gn/%s" % (name, k)] = (c,)
+            return
         for k in ("gamma", "beta", "mean/EMA", "variance/EMA"):
             sh["%s/bn/%s" % (name, k)] = (c,)
 
@@ -124,14 +174,27 @@ def frcnn_weight_shapes(cfg) -> dict:
     for i, c in enumerate((256, 512, 1024, 2048)):
         conv("fpn/lateral_1x1_c%d" % (i + 2), 1, c, nc, bias=True)
         conv("fpn/posthoc_3x3_p%d" % (i + 2), 3, nc, nc, bias=True)
+        if gn:                                       # gn_c* / gn_p* (nn.py:987-990, 1007-1009)
+            for s in ("gn_c%d" % (i + 2), "gn_p%d" % (i + 2)):
+                sh["fpn/%s/gamma" % s] = (nc,)
+                sh["fpn/%s/beta" % s] = (nc,)
     na = len(cfg.anchor_ratios)
     conv("rpn/conv0", 3, nc, nc, bias=True)
     conv("rpn/class", 1, nc, na, bias=True)
     conv("rpn/box", 1, nc, 4 * na, bias=True)
     dim = cfg.fpn_frcnn_fc_head_dim
     nbox = 1 if cfg.use_frcnn_class_agnostic else cfg.num_class
-    for name, fin, fout in (("fastrcnn/fc6", nc * 49, dim), ("fastrcnn/fc7", dim, dim),
-                            ("fastrcnn/outputs/class", dim, cfg.num_class), ("fastrcnn/outputs/box", dim, nbox * 4)):
+    if getattr(cfg, "use_conv_frcnn_head", False):   # conv_frcnn_head (models.py:1110-1125)
+        hd = int(getattr(cfg, "conv_frcnn_head_dim", 256))
+        for k in range(4):
+            conv("fastrcnn/conv%d" % k, 3, nc if k == 0 else hd, hd, bias=True)
+            if gn:
+                sh["fastrcnn/gn%d/gamma" % k] = (hd,)
+                sh["fastrcnn/gn%d/beta" % k] = (hd,)
+        hidden = (("fastrcnn/fc", hd * 49, dim),)
+    else:
+        hidden = (("fastrcnn/fc6", nc * 49, dim), ("fastrcnn/fc7", dim, dim))
+    for name, fin, fout in hidden + (("fastrcnn/outputs/class", dim, cfg.num_class), ("fastrcnn/outputs/box", dim, nbox * 4)):
         sh[name + "/W"] = (fin, fout)
         sh[name + "/b"] = (fout,)
     if getattr(cfg, "add_mask", False):              # models.py:1173-1199; Conv2DTranspose kernel is [kh, kw, out, in]

@@ -1,0 +1,115 @@
+"""Throughput of the GroupNorm model family: R50-GN-FPN with the GroupNorm 4-conv box head (--use_gn
+--use_conv_frcnn_head, conv_frcnn_head_dim 256), COCO 81 classes, version 2 (no dilation), 1280x720, rpn300, batch 8,
+batch-graph semantics, CUDA graph -- the same loop and clock record as bench.py's device-resident leg.
+
+  python tools/bench_gn.py [--steps 50 --warmup 5 --precision split --sustained-seconds 5 --profile-json FILE]
+
+Prints one JSON line: frames/s (host clock around synchronised graph replays), a sustained record, SM clocks, the board's
+name and power limit, and from one eager per-step profile (CUDA events, three passes averaged) the share of the pass spent
+in GroupNorm steps and the achieved bandwidth of every GN step from b2_step_info's byte counts."""
+import argparse
+import json
+import os
+import sys
+import time
+
+import numpy as np
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+
+H, W, BATCH = 720, 1280, 8
+MODEL = dict(resnet_num_block=(3, 4, 6, 3), num_class=81, use_dilations=False, version=2, use_gn=True,
+             use_conv_frcnn_head=True)
+GN_KINDS = {10: "stats", 11: "apply", 12: "per_roi"}
+
+
+def board(index):
+    out = {"name": None, "power_limit_w": None}
+    try:
+        import pynvml
+        pynvml.nvmlInit()
+        h = pynvml.nvmlDeviceGetHandleByIndex(index)
+        name = pynvml.nvmlDeviceGetName(h)
+        out["name"] = name.decode() if isinstance(name, bytes) else name
+        out["power_limit_w"] = pynvml.nvmlDeviceGetPowerManagementLimit(h) / 1000.0
+    except Exception:
+        import torch
+        out["name"] = torch.cuda.get_device_name(index)
+    return out
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--steps", type=int, default=50)
+    ap.add_argument("--warmup", type=int, default=5)
+    ap.add_argument("--precision", default="split", choices=["split", "fp16"])
+    ap.add_argument("--sustained-seconds", type=float, default=5.0)
+    ap.add_argument("--profile-json", default="", help="write the per-step profile here")
+    args = ap.parse_args()
+
+    import torch
+    from bench import ClockSampler
+    from object_detection_tracking_b200.config import make_config
+    from object_detection_tracking_b200.engine import Detector
+    from object_detection_tracking_b200.synth import synth_frame, synth_weights
+    if not torch.cuda.is_available():
+        raise RuntimeError("bench_gn.py needs an H100: no CUDA device")
+    torch.cuda.set_device(0)
+    cfg = make_config(**MODEL)
+    det = Detector(cfg, BATCH, H, W, device=0, precision=args.precision, use_cuda_graph=True, multi_semantics=True)
+    det.load_weights(synth_weights(cfg, 1234))
+    dev = [torch.from_numpy(np.stack([synth_frame(H, W, seed=8 * j + i) for i in range(BATCH)]).astype(np.float32)).cuda()
+           for j in range(4)]                    # 4 x 88 MB: the rotating input set exceeds the 50 MB L2
+
+    for i in range(max(args.warmup, 3)):
+        det.detect_device(dev[i % 4], None, sync=True)
+    sampler = ClockSampler(0)
+    sampler.start()
+    torch.cuda.synchronize()
+    t0 = time.perf_counter()
+    for i in range(args.steps):
+        det.detect_device(dev[i % 4], None, sync=(i == args.steps - 1))
+    torch.cuda.synchronize()
+    dt = time.perf_counter() - t0
+    sampler.stop.set()
+    sampler.join(timeout=2)
+
+    sustained = None
+    if args.sustained_seconds > 0:
+        s2 = ClockSampler(0)
+        s2.start()
+        n, ts = 0, time.perf_counter()
+        while time.perf_counter() - ts < args.sustained_seconds:
+            for _ in range(16):
+                det.detect_device(dev[n % 4], None, sync=False)
+                n += 1
+            det.detect_device(dev[n % 4], None, sync=True)
+            n += 1
+        dts = time.perf_counter() - ts
+        s2.stop.set()
+        s2.join(timeout=2)
+        sustained = {"value": n * BATCH / dts, "unit": "frames/s", "seconds": dts, "clocks": s2.summary()}
+
+    prof = det.profile_steps(reps=3)
+    if args.profile_json:
+        with open(args.profile_json, "w") as f:
+            json.dump({"precision": args.precision, "batch": BATCH, "model": MODEL, "steps": prof}, f, indent=1)
+    total = sum(p["ms"] for p in prof)
+    gn = [p for p in prof if p["kind"] in GN_KINDS]
+    by_kind = {GN_KINDS[k]: {"steps": sum(1 for p in gn if p["kind"] == k),
+                             "ms": sum(p["ms"] for p in gn if p["kind"] == k),
+                             "gb": sum(p["bytes"] for p in gn if p["kind"] == k) / 1e9} for k in GN_KINDS}
+    line = {"metric": "detector FPS @1280x720 rpn300 (ResNet-50-GN-FPN Faster-RCNN, GN conv head, COCO 81)",
+            "value": args.steps * BATCH / dt, "unit": "frames/s", "steps": args.steps, "ms_per_step": dt / args.steps * 1e3,
+            "batch": BATCH, "precision": args.precision, "weights": "seeded synthetic (synth.py, seed 1234)",
+            "board": board(0), "clocks": sampler.summary(), "sustained": sustained,
+            "profile": {"total_ms": total, "gn_ms": sum(p["ms"] for p in gn), "gn_share": sum(p["ms"] for p in gn) / total,
+                        "gn_by_kind": by_kind,
+                        "gn_steps_gbs": [{"name": p["name"], "ms": p["ms"], "gb": p["bytes"] / 1e9,
+                                          "gbs": p["bytes"] / (p["ms"] * 1e-3) / 1e9} for p in gn]}}
+    print(json.dumps(line), flush=True)
+
+
+if __name__ == "__main__":
+    main()
