@@ -1,4 +1,4 @@
-// Shared host-side declarations for libb200det: error plumbing, activation tensors, kernel launchers.
+// Shared host-side declarations for libb200det: error plumbing, the conv description and its launchers.
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -29,17 +29,6 @@ const char* last_error();
       return -1;                                                                     \
     }                                                                                \
   } while (0)
-
-// Activation tensor in HBM: NHWC, fp16 "hi" plane plus (in split precision) an fp16 "lo" plane that
-// holds (x - hi) * 2048, so x ~= hi + lo / 2048 to ~22 significant bits.  `ld` = channel stride of a
-// pixel in elements (>= C).
-struct Act {
-  __half* hi = nullptr;
-  __half* lo = nullptr;   // nullptr when precision == fp16
-  int N = 0, H = 0, W = 0, C = 0;
-  size_t pixels() const { return static_cast<size_t>(N) * H * W; }
-  size_t elems() const { return pixels() * C; }
-};
 
 constexpr float kLoScale = 2048.0f;
 constexpr float kLoInv = 1.0f / 2048.0f;

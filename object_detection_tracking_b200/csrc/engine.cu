@@ -1,4 +1,4 @@
-// libb200det engine: context, weight folding/packing, the static per-frame launch plan, C ABI.
+// libb200det detector engine: context, weight packing, the static per-frame launch plan, C ABI.
 //
 // The plan is built once per (batch, H, W): every activation buffer, every TMA tensor map and every
 // kernel parameter block is fixed, so one frame is a fixed sequence of ~150 launches that is captured
@@ -9,22 +9,16 @@
 #include <string.h>
 
 #include <algorithm>
-#include <map>
+#include <functional>
 #include <memory>
-#include <mutex>
 #include <string>
 #include <vector>
 
 #include "../../include/b200det.h"
-#include "common.h"
+#include "engine_core.h"
 #include "kernels.h"
 
 namespace b2 {
-
-static thread_local std::string g_err;
-void set_error(const std::string& msg) { g_err = msg; }
-const char* last_error() { return g_err.c_str(); }
-
 namespace {
 
 __global__ void subsample2_kernel(const __half* __restrict__ in_hi, const __half* __restrict__ in_lo, int B, int H,
@@ -96,36 +90,21 @@ __global__ void mask_select_kernel(const float* __restrict__ logits, int ld, con
   }
 }
 
-struct Planes {
-  __half* hi = nullptr;
-  __half* lo = nullptr;
-  int B = 0, H = 0, W = 0, C = 0;
-  size_t elems() const { return static_cast<size_t>(B) * H * W * C; }
-};
-
-struct Layer {
-  std::string name;        // reference variable scope, e.g. "group1/block0/conv2"
-  ConvDesc d;
-  ConvWeights w;
-  ConvIO io;
-  ConvPlan* plan = nullptr;
-  std::vector<ConvPlan*> part_plan;              // the same layer over each 1/nsplit of the batch (multi-stream passes)
-  bool has_bn = false, has_bias = false;
-  int kind = 0;            // 0 conv HWIO, 1 fc6 (NCHW-flatten permute), 2 dense, 3 rpn class+box, 4 head outputs,
-                           // 5 stem, 6 mask-head transposed conv 2x2/2 (as a 1x1 conv onto 4 taps x C outputs)
-};
-
 // One GroupNorm of the plan (use_gn backbone / FPN, conv box head): normalises a conv output in place.
 struct GnOp {
   std::string name;        // reference variable scope, e.g. "group1/block0/conv1/gn", "fpn/gn_c2", "fastrcnn/gn0"
-  GnParams p;              // full-batch launch; the half-batch launches offset it per image
+  GnParams p;              // full-batch launch (its gamma / beta are loaded with the weights)
 };
 
-struct StageRef {
-  int kind;                // 0 planes, 1 f32, 2 i32
-  Planes pl;
-  void* ptr = nullptr;
-  int64_t shape[4] = {1, 1, 1, 1};
+// Packing of a checkpoint weight into the [Cout_pad][K] operand (ConvLayer::layout).
+enum Layout {
+  kHwio = 0,     // conv HWIO
+  kFc6 = 1,      // dense over the NCHW flatten of [7][7][C] ROI features
+  kDense = 2,
+  kRpnOut = 3,   // rpn/{class,box} fused along N
+  kHeadOut = 4,  // fastrcnn/outputs/{class,box} fused along N
+  kStem = 5,     // 7x7 stem re-indexed for the packed operand
+  kDeconv = 6,   // mask-head transposed conv 2x2/2 as a 1x1 conv onto 4 taps x C outputs
 };
 
 enum { NPHASE = 8 };
@@ -136,14 +115,16 @@ enum { NPHASE = 8 };
 using namespace b2;
 
 struct b2_ctx {
+  Arena arena;             // first member: freed after everything that refers to it
   b2_config cfg;
   int device = 0, num_sms = 132;
   bool split = false;
   cudaStream_t stream = nullptr;
-  std::vector<void*> allocs;
-  std::vector<std::unique_ptr<Layer>> layers;
-  std::vector<Layer*> phase_layers[NPHASE];   // conv layers per phase, in launch order (phases with only convs)
-  std::map<std::string, StageRef> stages;
+  std::vector<std::unique_ptr<ConvLayer>> layers;
+  std::vector<ConvLayer*> part_layers;        // layers of the forked phases 0-2 (they get per-part plans)
+  std::vector<std::unique_ptr<GnOp>> gns;
+  std::vector<Step> steps;
+  StageMap stages;
   // geometry
   int c1h = 0, c1w = 0, ch[4], cw[4], ph[5], pw[5], pfh[5], pfw[5];
   // buffers
@@ -169,7 +150,6 @@ struct b2_ctx {
   HeadPostParams post;
   Planes roi_feat, fc6, fc7;
   Planes head_a, head_b;           // conv box head (cfg.conv_head_dim > 0): [M][7][7][conv_head_dim] ping-pong
-  std::vector<std::unique_ptr<GnOp>> gns;
   float* head_logits = nullptr;
   float* box_feat = nullptr;
   float* box_feat_pooled = nullptr;
@@ -183,19 +163,9 @@ struct b2_ctx {
   float* mask_logits = nullptr;
   int mask_ld = 0;
   float* final_masks = nullptr;    // [B][R][28][28]
-  // launch bookkeeping
-  struct Step {
-    int phase;
-    int kind;   // 0 conv layer, 1 stem, 2 maxpool, 3 subsample p6, 4 proposals, 5 roialign1, 6 post, 7 roialign2,
-                // 8 roialign 14x14 of the final boxes (mask head), 9 mask select + sigmoid,
-                // 10 GroupNorm statistics, 11 GroupNorm apply (+ residual, ReLU), 12 per-ROI GroupNorm (box head)
-    Layer* layer;
-    GnOp* gn = nullptr;
-  };
-  std::vector<Step> steps;
   cudaGraphExec_t graph = nullptr;
-  // dual-stream pass: the backbone / FPN / RPN-head phases run as two half-batches on two streams, so that the tail of
-  // one layer's persistent kernel (tiles % SMs != 0, no SM busy in the last round) overlaps the other half's kernels
+  // dual-stream pass: the backbone / FPN / RPN-head phases run as nsplit batch parts on as many streams, so that the tail
+  // of one layer's persistent kernel (tiles % SMs != 0, no SM busy in the last round) overlaps the other parts' kernels
   bool dual = false;
   int nsplit = 1;                                  // batch parts (= streams) of the forked phases
   cudaStream_t side_stream[7] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
@@ -203,80 +173,91 @@ struct b2_ctx {
   bool weights_loaded = false;
   cudaEvent_t ev[NPHASE + 1];
   float phase_ms[NPHASE];
-  int launches = 0;
 
-  template <typename T>
-  T* alloc(size_t n, bool zero = true) {
-    void* p = nullptr;
-    if (cudaMalloc(&p, n * sizeof(T) + 256) != cudaSuccess) return nullptr;
-    if (zero) cudaMemset(p, 0, n * sizeof(T) + 256);
-    allocs.push_back(p);
-    return static_cast<T*>(p);
-  }
   bool alloc_planes(Planes& p, int B, int H, int W, int C) {
-    p.B = B; p.H = H; p.W = W; p.C = C;
-    p.hi = alloc<__half>(p.elems());
-    p.lo = split ? alloc<__half>(p.elems()) : nullptr;
-    return p.hi != nullptr && (!split || p.lo != nullptr);
+    p = arena.planes(B, H, W, C, split);
+    return p.hi != nullptr;
   }
 };
 
 namespace {
 
-void reg_planes(b2_ctx* c, const std::string& name, const Planes& p) {
-  StageRef s;
-  s.kind = 0;
-  s.pl = p;
-  s.shape[0] = p.B; s.shape[1] = p.H; s.shape[2] = p.W; s.shape[3] = p.C;
-  c->stages[name] = s;
-}
-void reg_raw(b2_ctx* c, const std::string& name, void* ptr, int kind, int64_t a, int64_t b, int64_t cc, int64_t d) {
-  StageRef s;
-  s.kind = kind;
-  s.ptr = ptr;
-  s.shape[0] = a; s.shape[1] = b; s.shape[2] = cc; s.shape[3] = d;
-  c->stages[name] = s;
+// Adds step `kind` of `phase`.  `launch(b0, n, st)` enqueues it over images [b0, b0 + n); in the forked phases 0-2 the
+// step gets one launch per batch part.
+Step& add_batch_step(b2_ctx* c, int phase, int kind, const std::string& name,
+                     const std::function<int(int, int, cudaStream_t)>& launch, int launches = 1) {
+  static const char* kKindNames[] = {"conv", "stem_pack", "maxpool", "p6_subsample", "rpn_proposals", "roialign_proposals",
+                                     "head_post", "roialign_final", "roialign_mask", "mask_select", "gn_stats", "gn_apply",
+                                     "gn_roi"};
+  const int B = c->cfg.batch;
+  Step& s = add_step(c->steps, phase, kind, name.empty() ? kKindNames[kind] : name,
+                     [launch, B](cudaStream_t st) { return launch(0, B, st); }, 0, 0, launches);
+  if (c->dual && phase <= 2) {
+    const int hb = B / c->nsplit;
+    for (int h = 0; h < c->nsplit; ++h) s.parts.push_back([launch, h, hb](cudaStream_t st) { return launch(h * hb, hb, st); });
+  }
+  return s;
 }
 
-// Adds one conv layer reading `in` (view in_H x in_W of the buffer) and writing `out`.
-Layer* add_conv(b2_ctx* c, int phase, const std::string& name, const Planes& in, int view_h, int view_w, int R,
-                int stride, int dil, int pt, int pb, int pl, int pr, int Cout, bool bn, bool bias, bool relu,
-                const Planes& out, int off_h, int off_w, const Planes* res, int res_shift, float* out_f32 = nullptr,
-                int ldc_f32 = 0, int kind = 0, int S = 0) {
-  std::unique_ptr<Layer> L(new Layer());
-  L->name = name;
-  L->has_bn = bn;
-  L->has_bias = bias;
-  L->kind = kind;
-  ConvDesc& d = L->d;
-  d.B = in.B; d.in_H = view_h; d.in_W = view_w; d.Cin = in.C;
-  d.in_pitch_H = in.H; d.in_pitch_W = in.W; d.in_ld = in.C;
+// The operands of layer L over images [b0, ...): each offset by whole images of its own buffer (a view's pixel stride
+// and pitch, not the view's extent)
+ConvIO images(const ConvLayer& L, int b0) {
+  const ConvDesc& d = L.d;
+  auto at = [b0](auto* p, int H, int W, int C) { return p ? p + static_cast<size_t>(b0) * H * W * C : p; };
+  ConvIO io = L.io;
+  io.in_hi = at(io.in_hi, d.in_pitch_H, d.in_pitch_W, d.in_ld);
+  io.in_lo = at(io.in_lo, d.in_pitch_H, d.in_pitch_W, d.in_ld);
+  io.out_hi = at(io.out_hi, d.out_H, d.out_W, d.ldc);
+  io.out_lo = at(io.out_lo, d.out_H, d.out_W, d.ldc);
+  io.out_f32 = at(io.out_f32, d.out_H, d.out_W, d.ldc);
+  io.res_hi = at(io.res_hi, d.res_H, d.res_W, d.ldr);
+  io.res_lo = at(io.res_lo, d.res_H, d.res_W, d.ldr);
+  return io;
+}
+
+// Adds one conv layer reading `in` (view in_H x in_W of the buffer, pixel stride in_ld, 0 = in.C) and writing `out`.
+ConvLayer* add_conv(b2_ctx* c, int phase, const std::string& name, const Planes& in, int view_h, int view_w, int R,
+                    int stride, int dil, int pt, int pb, int pl, int pr, int Cout, bool bn, bool bias, bool relu,
+                    const Planes& out, int off_h, int off_w, const Planes* res, int res_shift, float* out_f32 = nullptr,
+                    int ldc_f32 = 0, int layout = kHwio, int S = 0, int in_ld = 0) {
+  ConvDesc d;
+  d.in_H = view_h; d.in_W = view_w; d.in_ld = in_ld;
   d.R = R; d.S = S > 0 ? S : R; d.stride = stride; d.dil = dil;
   d.pad_t = pt; d.pad_b = pb; d.pad_l = pl; d.pad_r = pr;
   d.Cout = Cout;
   d.relu = relu ? 1 : 0;
   d.acc_kb = c->cfg.accum_chunk;
   d.off_h = off_h; d.off_w = off_w;
-  if (out_f32) {
-    d.out_H = d.Ho(); d.out_W = d.Wo(); d.ldc = ldc_f32;
-  } else {
-    d.out_H = out.H; d.out_W = out.W; d.ldc = out.C;
-  }
-  if (res) {
-    d.res_H = res->H; d.res_W = res->W; d.ldr = res->C; d.res_shift = res_shift;
-  }
-  L->w.Cout_pad = (Cout + 15) / 16 * 16;
-  L->w.K = d.R * d.S * in.C;
-  L->w.w_hi = c->alloc<__half>(static_cast<size_t>(L->w.Cout_pad) * L->w.K);
-  L->w.w_lo = c->split ? c->alloc<__half>(static_cast<size_t>(L->w.Cout_pad) * L->w.K) : nullptr;
-  L->w.bias = c->alloc<float>(L->w.Cout_pad);
-  L->io.in_hi = in.hi; L->io.in_lo = in.lo;
-  L->io.out_hi = out.hi; L->io.out_lo = out.lo; L->io.out_f32 = out_f32;
-  if (res) { L->io.res_hi = res->hi; L->io.res_lo = res->lo; }
+  d.res_shift = res ? res_shift : 0;
+  std::unique_ptr<ConvLayer> L = make_conv(c->arena, c->split, name, d, in, out, res, out_f32, ldc_f32);
+  L->bn = bn ? name + "/bn" : "";
+  L->bias = bias ? name + "/b" : "";
+  L->layout = layout;
   L->io.range_flag = c->range_flag;
-  Layer* raw = L.get();
+  ConvLayer* raw = L.get();
   c->layers.push_back(std::move(L));
-  c->steps.push_back({phase, 0, raw});
+  if (phase <= 2) c->part_layers.push_back(raw);
+  // algorithmic FLOPs and HBM bytes (each operand read once, output written once, at the stored precision)
+  const ConvDesc& e = raw->d;
+  const double esz = c->split ? 4.0 : 2.0;
+  const double M = static_cast<double>(e.B) * e.Ho() * e.Wo();
+  const double K = static_cast<double>(e.R) * e.S * e.Cin;
+  const double in_px = static_cast<double>(e.B) * e.in_H * e.in_W;
+  const int conv_impl = c->cfg.conv_impl;
+  const bool split = c->split;
+  Step& s = add_batch_step(c, phase, 0,
+                           name + " [" + std::to_string(e.in_H) + "x" + std::to_string(e.in_W) + "x" + std::to_string(e.Cin) + " " +
+                               std::to_string(e.R) + "x" + std::to_string(e.S) + "/" + std::to_string(e.stride) + " d" +
+                               std::to_string(e.dil) + " ->" + std::to_string(e.Cout) + "]",
+                           [raw, conv_impl, split](int, int, cudaStream_t st) {
+                             if (conv_impl == 0) return conv_tc_launch(raw->plan.get(), st);
+                             return conv_simt_launch(raw->d, raw->w, raw->io, split, st);
+                           });
+  for (size_t h = 0; h < s.parts.size(); ++h)
+    s.parts[h] = [raw, h](cudaStream_t st) { return conv_tc_launch(raw->part_plan[h].get(), st); };
+  s.flops = 2.0 * M * K * e.Cout;
+  s.bytes = in_px * (e.in_ld > 0 && e.in_ld < e.Cin ? e.in_ld : e.Cin) * esz + K * e.Cout * esz +
+            M * e.Cout * (raw->io.out_f32 ? 4.0 : esz) + (raw->io.res_hi ? M * e.Cout * esz / (e.res_shift ? 4.0 : 1.0) : 0.0);
   return raw;
 }
 
@@ -287,39 +268,60 @@ int add_gn(b2_ctx* c, int phase, const std::string& name, const Planes& buf, int
            const Planes* res, int res_shift, bool relu, bool per_roi = false) {
   std::unique_ptr<GnOp> G(new GnOp());
   G->name = name;
-  GnParams& p = G->p;
-  memset(&p, 0, sizeof(p));
-  p.x_hi = buf.hi; p.x_lo = buf.lo; p.y_hi = buf.hi; p.y_lo = buf.lo;
-  p.B = buf.B; p.H = view_h; p.W = view_w; p.C = buf.C;
-  p.pitch_H = buf.H; p.pitch_W = buf.W; p.ld = buf.C; p.off_h = off_h; p.off_w = off_w;
-  if (res) {
-    p.r_hi = res->hi; p.r_lo = res->lo;
-    p.res_H = res->H; p.res_W = res->W; p.res_ld = res->C; p.res_shift = res_shift;
-  }
-  p.relu = relu ? 1 : 0;
-  p.gamma = c->alloc<float>(buf.C);
-  p.beta = c->alloc<float>(buf.C);
-  p.range_flag = c->range_flag;
-  B2_CHECK(p.gamma && p.beta, "out of device memory (GroupNorm " + name + ")");
+  GnParams base;
+  memset(&base, 0, sizeof(base));
+  base.H = view_h; base.W = view_w; base.C = buf.C;
+  base.pitch_H = buf.H; base.pitch_W = buf.W; base.ld = buf.C; base.off_h = off_h; base.off_w = off_w;
+  if (res) { base.res_H = res->H; base.res_W = res->W; base.res_ld = res->C; base.res_shift = res_shift; }
+  base.relu = relu ? 1 : 0;
+  base.gamma = c->arena.alloc<float>(buf.C);
+  base.beta = c->arena.alloc<float>(buf.C);
+  base.range_flag = c->range_flag;
+  B2_CHECK(base.gamma && base.beta, "out of device memory (GroupNorm " + name + ")");
   if (!per_roi) {
-    p.chunks = gn_chunks(view_h, view_w, buf.C);
-    p.partial = c->alloc<float>(static_cast<size_t>(buf.B) * p.chunks * 32 * 3);
-    p.stats = c->alloc<float>(static_cast<size_t>(buf.B) * 32 * 2);
-    p.counter = c->alloc<unsigned int>(buf.B);
-    B2_CHECK(p.partial && p.stats && p.counter, "out of device memory (GroupNorm " + name + " statistics)");
+    base.chunks = gn_chunks(view_h, view_w, buf.C);
+    base.partial = c->arena.alloc<float>(static_cast<size_t>(buf.B) * base.chunks * 32 * 3);
+    base.stats = c->arena.alloc<float>(static_cast<size_t>(buf.B) * 32 * 2);
+    base.counter = c->arena.alloc<unsigned int>(buf.B);
+    B2_CHECK(base.partial && base.stats && base.counter, "out of device memory (GroupNorm " + name + " statistics)");
   }
-  GnOp* raw = G.get();
+  // the launch over images [b0, b0 + n): planes and per-image scratch offset by b0
+  const Planes x = buf;
+  const Planes r = res ? *res : Planes();
+  auto params = [base, x, r, per_roi](int b0, int n) {
+    GnParams p = base;
+    const Planes xs = x.images(b0, n), rs = r.images(b0, n);
+    p.x_hi = xs.hi; p.x_lo = xs.lo; p.y_hi = xs.hi; p.y_lo = xs.lo;
+    p.r_hi = rs.hi; p.r_lo = rs.lo;
+    if (!per_roi) {
+      p.partial += static_cast<size_t>(b0) * p.chunks * 32 * 3;
+      p.stats += static_cast<size_t>(b0) * 32 * 2;
+      p.counter += b0;
+    }
+    p.B = n;
+    return p;
+  };
+  G->p = params(0, buf.B);
   c->gns.push_back(std::move(G));
-  if (per_roi) {
-    c->steps.push_back({phase, 12, nullptr, raw});
+  // bytes: statistics read the view once; apply / per-ROI read it, write it and read the residual (a quarter of the view's
+  // size when it is upsampled)
+  const GnParams& p = c->gns.back()->p;
+  const double esz = c->split ? 4.0 : 2.0;
+  const double n = static_cast<double>(p.B) * p.H * p.W * p.C;
+  const double apply_bytes = 2.0 * n * esz + (p.r_hi ? n * esz / (p.res_shift ? 4.0 : 1.0) : 0.0);
+  const std::string dims = " [" + std::to_string(p.H) + "x" + std::to_string(p.W) + "x" + std::to_string(p.C);
+  const std::string epi = std::string(p.r_hi ? (p.res_shift ? " +up2" : " +res") : "") + (p.relu ? " relu" : "") + "]";
+  if (per_roi) {   // the box head's samples are ROIs, not images: always the whole buffer
+    add_batch_step(c, phase, 12, name + " per-roi" + dims + epi,
+                   [p](int, int, cudaStream_t st) { return gn_roi_launch(p, st); }).bytes = apply_bytes;
   } else {
-    c->steps.push_back({phase, 10, nullptr, raw});
-    c->steps.push_back({phase, 11, nullptr, raw});
+    add_batch_step(c, phase, 10, name + " stats" + dims + "]",
+                   [params](int b0, int nb, cudaStream_t st) { return gn_stats_launch(params(b0, nb), st); }).bytes = n * esz;
+    add_batch_step(c, phase, 11, name + " apply" + dims + epi,
+                   [params](int b0, int nb, cudaStream_t st) { return gn_apply_launch(params(b0, nb), st); }).bytes = apply_bytes;
   }
   return 0;
 }
-
-int log2i(int v) { int r = 0; while ((1 << r) < v) ++r; return r; }
 
 // generate_anchors.py:42-109 restated for one (stride, size): the 3 ratio anchors of a cell.
 void cell_anchors(float stride, float size, const float* ratios, float out[3][4]) {
@@ -349,6 +351,14 @@ int build_plan(b2_ctx* c) {
   B2_CHECK(B >= 1 && H >= 32 && W >= 32, "b2_create: bad frame geometry");
   B2_CHECK(cfg.fpn_num_channel == 256, "b2_create: fpn_num_channel must be 256");
   B2_CHECK(cfg.rpn_topk >= 1 && cfg.rpn_topk <= 1024, "b2_create: rpn_topk must be in [1,1024]");
+  // Images are independent through phases 0-2 (stem, ResNet, FPN, RPN head): their steps also get one launch per part of
+  // the batch, each with its own plans (same tiles per image, so the results are bit-identical to the full-batch plan).
+  if (cfg.conv_impl == 0) {
+    c->nsplit = 2;
+    if (const char* e = getenv("B2_SPLIT")) c->nsplit = atoi(e);   // experiment hook: 1, 2, 4, 8 batch parts
+    if (c->nsplit < 1 || c->nsplit > 8 || B % c->nsplit != 0) c->nsplit = 1;
+    c->dual = c->nsplit > 1;
+  }
   // ---- geometry (nn.py:843-944, tf_pad_reverse=True) ----
   const int PH = (H + 31) / 32 * 32, PW = (W + 31) / 32 * 32;
   c->c1h = (PH + 5 - 7) / 2 + 1;
@@ -374,8 +384,8 @@ int build_plan(b2_ctx* c) {
 
   // ---- input + stem + pool (phase 0) ----
   c->img_bytes = static_cast<size_t>(B) * H * W * 3 * (cfg.input_dtype == 1 ? 1 : 4);
-  c->img = c->alloc<uint8_t>(c->img_bytes);
-  c->range_flag = c->alloc<unsigned int>(1);
+  c->img = c->arena.alloc<uint8_t>(c->img_bytes);
+  c->range_flag = c->arena.alloc<unsigned int>(1);
   B2_CHECK(c->range_flag != nullptr, "out of device memory (range flag)");
   B2_CUDA(cudaMallocHost(&c->h_range, 3 * sizeof(unsigned int)));
   c->h_range[0] = c->h_range[1] = c->h_range[2] = 0;
@@ -383,7 +393,12 @@ int build_plan(b2_ctx* c) {
   B2_CHECK(c->alloc_planes(c->stem_u, B, c->c1h + 3, c->c1w + 3, 16), "alloc stem operand");
   B2_CHECK(c->alloc_planes(c->c1, B, c->c1h, c->c1w, 64), "alloc c1");
   B2_CHECK(c->alloc_planes(c->pool, B, c->ch[0], c->cw[0], 64), "alloc pool");
-  c->steps.push_back({0, 1, nullptr});
+  const double esz = c->split ? 4.0 : 2.0;
+  add_batch_step(c, 0, 1, "", [c](int b0, int n, cudaStream_t st) {
+    const Planes u = c->stem_u.images(b0, n);
+    return stem_pack16_launch(static_cast<const uint8_t*>(c->img) + static_cast<size_t>(b0) * (c->img_bytes / c->cfg.batch),
+                              c->cfg.input_dtype == 1, n, c->cfg.height, c->cfg.width, u.hi, u.lo, u.H, u.W, st);
+  }).bytes = static_cast<double>(c->img_bytes) + static_cast<double>(c->stem_u.elems()) * esz;
   // use_gn (nn.py:859-862, 474-477): every backbone conv is a plain conv followed by GroupNorm steps that carry the ReLU
   // and the residual; with BatchNorm the norm, ReLU and residual are in the conv epilogue
   const bool gn = cfg.use_gn != 0;
@@ -391,14 +406,16 @@ int build_plan(b2_ctx* c) {
   {
     Planes view = c->stem_u;
     view.C = 64;                       // one GEMM pixel = 4 consecutive operand pixels
-    Layer* L0 = add_conv(c, 0, "conv0", view, c->c1h + 3, c->c1w, 4, 1, 1, 0, 0, 0, 0, 64, !gn, false, !gn, c->c1, 0, 0,
-                         nullptr, 0, nullptr, 0, 5, 1);
-    L0->d.in_ld = 16;
+    add_conv(c, 0, "conv0", view, c->c1h + 3, c->c1w, 4, 1, 1, 0, 0, 0, 0, 64, !gn, false, !gn, c->c1, 0, 0, nullptr, 0,
+             nullptr, 0, kStem, 1, 16);
     if (gn && add_gn(c, 0, "conv0/gn", c->c1, c->c1h, c->c1w, 0, 0, nullptr, 0, true)) return -1;
   }
-  c->steps.push_back({0, 2, nullptr});
-  reg_planes(c, "c1", c->c1);
-  reg_planes(c, "pool", c->pool);
+  add_batch_step(c, 0, 2, "", [c](int b0, int n, cudaStream_t st) {
+    const Planes a = c->c1.images(b0, n), p = c->pool.images(b0, n);
+    return maxpool_launch(a.hi, a.lo, n, c->c1h, c->c1w, 64, p.hi, p.lo, c->ch[0], c->cw[0], st);
+  }).bytes = (static_cast<double>(c->c1.elems()) + c->pool.elems()) * esz;
+  c->stages.planes("c1", c->c1);
+  c->stages.planes("pool", c->pool);
 
   // ---- ResNet groups (nn.py:459-588) ----
   Planes cur = c->pool;
@@ -431,7 +448,7 @@ int build_plan(b2_ctx* c) {
         // statistics and stay 0.
         a2 = &t2_first;
         const int off = dil != 1 ? 1 : 0;
-        Layer* L2 = add_conv(c, 0, p + "/conv2", a1, a1.H, a1.W, 3, 2, dil, 1, 0, 1, 0, feat, !gn, false, !gn, *a2, off,
+        ConvLayer* L2 = add_conv(c, 0, p + "/conv2", a1, a1.H, a1.W, 3, 2, dil, 1, 0, 1, 0, feat, !gn, false, !gn, *a2, off,
                              off, nullptr, 0);
         if (gn && add_gn(c, 0, p + "/conv2/gn", *a2, L2->d.Ho(), L2->d.Wo(), off, off, nullptr, 0, true)) return -1;
       } else {
@@ -459,7 +476,7 @@ int build_plan(b2_ctx* c) {
       cur = out;
     }
     c->cfeat[g] = cur;
-    reg_planes(c, "c" + std::to_string(g + 2), cur);
+    c->stages.planes("c" + std::to_string(g + 2), cur);
   }
 
   // ---- FPN (nn.py:947-1014), phase 1 ----
@@ -483,22 +500,29 @@ int build_plan(b2_ctx* c) {
     // gn_p* (nn.py:1007-1009) over the whole, uncropped level; p6 below subsamples the normalised p5
     if (gn && add_gn(c, 1, "fpn/gn_p" + std::to_string(i + 2), c->pfeat[i], c->pfh[i], c->pfw[i], 0, 0, nullptr, 0, false))
       return -1;
-    reg_planes(c, "p" + std::to_string(i + 2), c->pfeat[i]);
+    c->stages.planes("p" + std::to_string(i + 2), c->pfeat[i]);
   }
   B2_CHECK(c->alloc_planes(c->pfeat[4], B, c->pfh[4], c->pfw[4], nc), "alloc p6");
-  c->steps.push_back({1, 3, nullptr});
-  reg_planes(c, "p6", c->pfeat[4]);
+  add_batch_step(c, 1, 3, "", [c](int b0, int n, cudaStream_t st) {
+    const Planes p5 = c->pfeat[3].images(b0, n), p6 = c->pfeat[4].images(b0, n);
+    const size_t total = static_cast<size_t>(n) * p6.H * p6.W * (p6.C / 8);
+    subsample2_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, st>>>(p5.hi, p5.lo, n, p5.H, p5.W, p5.C, p6.hi,
+                                                                                   p6.lo, p6.H, p6.W);
+    B2_CUDA(cudaGetLastError());
+    return 0;
+  });
+  c->stages.planes("p6", c->pfeat[4]);
 
   // ---- RPN head (models.py:979-1009), phase 2; class+box 1x1 fused into one N=15 GEMM ----
   for (int i = 0; i < 5; ++i) {
     B2_CHECK(c->alloc_planes(c->rpn_h[i], B, c->ph[i], c->pw[i], nc), "alloc rpn hidden");
-    Layer* L0 = add_conv(c, 2, "rpn/conv0", c->pfeat[i], c->ph[i], c->pw[i], 3, 1, 1, 1, 1, 1, 1, nc, false, true,
+    ConvLayer* L0 = add_conv(c, 2, "rpn/conv0", c->pfeat[i], c->ph[i], c->pw[i], 3, 1, 1, 1, 1, 1, 1, nc, false, true,
                          true, c->rpn_h[i], 0, 0, nullptr, 0);
     (void)L0;
-    c->rpn_out[i] = c->alloc<float>(static_cast<size_t>(B) * c->ph[i] * c->pw[i] * 16 + 16 * 128);
+    c->rpn_out[i] = c->arena.alloc<float>(static_cast<size_t>(B) * c->ph[i] * c->pw[i] * 16 + 16 * 128);
     add_conv(c, 2, "rpn/classbox", c->rpn_h[i], c->ph[i], c->pw[i], 1, 1, 1, 0, 0, 0, 0, 15, false, true, false,
-             Planes(), 0, 0, nullptr, 0, c->rpn_out[i], 16, 3);
-    reg_raw(c, "rpn_l" + std::to_string(i), c->rpn_out[i], 1, B, c->ph[i], c->pw[i], 16);
+             Planes(), 0, 0, nullptr, 0, c->rpn_out[i], 16, kRpnOut);
+    c->stages.raw("rpn_l" + std::to_string(i), c->rpn_out[i], Stage::kF32, B, c->ph[i], c->pw[i], 16);
   }
 
   // ---- proposals (phase 3) ----
@@ -522,19 +546,19 @@ int build_plan(b2_ctx* c) {
   rp.min_size = cfg.rpn_min_size;
   rp.multi = cfg.multi_semantics;
   rp.nms_thr = cfg.rpn_nms_thres;
-  rp.lvl_boxes = c->alloc<float>(static_cast<size_t>(B) * 5 * K * 4);
-  rp.lvl_scores = c->alloc<float>(static_cast<size_t>(B) * 5 * K);
-  rp.lvl_count = c->alloc<int>(B * 5);
-  rp.prop_boxes = c->alloc<float>(static_cast<size_t>(B) * K * 4);
-  rp.prop_scores = c->alloc<float>(static_cast<size_t>(B) * K);
-  rp.prop_count = c->alloc<int>(B);
-  c->steps.push_back({3, 4, nullptr});
-  reg_raw(c, "lvl_boxes", rp.lvl_boxes, 1, B, 5, K, 4);
-  reg_raw(c, "lvl_scores", rp.lvl_scores, 1, B, 5, K, 1);
-  reg_raw(c, "lvl_count", rp.lvl_count, 2, B, 5, 1, 1);
-  reg_raw(c, "proposal_boxes", rp.prop_boxes, 1, B, K, 4, 1);
-  reg_raw(c, "proposal_scores", rp.prop_scores, 1, B, K, 1, 1);
-  reg_raw(c, "proposal_count", rp.prop_count, 2, B, 1, 1, 1);
+  rp.lvl_boxes = c->arena.alloc<float>(static_cast<size_t>(B) * 5 * K * 4);
+  rp.lvl_scores = c->arena.alloc<float>(static_cast<size_t>(B) * 5 * K);
+  rp.lvl_count = c->arena.alloc<int>(B * 5);
+  rp.prop_boxes = c->arena.alloc<float>(static_cast<size_t>(B) * K * 4);
+  rp.prop_scores = c->arena.alloc<float>(static_cast<size_t>(B) * K);
+  rp.prop_count = c->arena.alloc<int>(B);
+  add_batch_step(c, 3, 4, "", [c](int, int, cudaStream_t st) { return rpn_proposals_launch(c->rpn, st); }, 2);
+  c->stages.raw("lvl_boxes", rp.lvl_boxes, Stage::kF32, B, 5, K, 4);
+  c->stages.raw("lvl_scores", rp.lvl_scores, Stage::kF32, B, 5, K, 1);
+  c->stages.raw("lvl_count", rp.lvl_count, Stage::kI32, B, 5, 1, 1);
+  c->stages.raw("proposal_boxes", rp.prop_boxes, Stage::kF32, B, K, 4, 1);
+  c->stages.raw("proposal_scores", rp.prop_scores, Stage::kF32, B, K, 1, 1);
+  c->stages.raw("proposal_count", rp.prop_count, Stage::kI32, B, 1, 1, 1);
 
   // ---- ROIAlign of the proposals (phase 4) ----
   const int M = B * K;
@@ -552,8 +576,8 @@ int build_plan(b2_ctx* c) {
   r1.C = nc; r1.B = B; r1.rois_per_image = K;
   r1.boxes = rp.prop_boxes; r1.count = rp.prop_count;
   r1.out_hi = c->roi_feat.hi; r1.out_lo = c->roi_feat.lo; r1.out_nchw = nullptr;
-  c->steps.push_back({4, 5, nullptr});
-  reg_planes(c, "roi_feat", c->roi_feat);
+  add_batch_step(c, 4, 5, "", [c](int, int, cudaStream_t st) { return roialign_launch(c->roi1, st); });
+  c->stages.planes("roi_feat", c->roi_feat);
 
   // ---- box head (models.py:1030-1108), phase 5: fc6, fc7, class+box outputs fused (N = 5*num_class) ----
   const int dim = cfg.fc_head_dim;
@@ -565,7 +589,7 @@ int build_plan(b2_ctx* c) {
   }
   const int nout = cfg.num_class + (cfg.class_agnostic ? 4 : cfg.num_class * 4);
   const int ldo = (nout + 15) / 16 * 16;
-  c->head_logits = c->alloc<float>(static_cast<size_t>(Mpad) * ldo);
+  c->head_logits = c->arena.alloc<float>(static_cast<size_t>(Mpad) * ldo);
   Planes rf = c->roi_feat; rf.W = M;
   if (hd > 0) {
     // conv_frcnn_head (models.py:1110-1125), use_conv_frcnn_head: 4 x [conv 3x3 SAME + bias + ReLU, then GroupNorm per ROI
@@ -589,23 +613,23 @@ int build_plan(b2_ctx* c) {
     Planes flat = cur_h; flat.B = 1; flat.H = 1; flat.W = M; flat.C = 49 * hd;
     Planes f = c->fc6; f.W = M;
     add_conv(c, 5, "fastrcnn/fc", flat, 1, M, 1, 1, 1, 0, 0, 0, 0, dim, false, true, true, f, 0, 0, nullptr, 0, nullptr,
-             0, 1);
+             0, kFc6);
     add_conv(c, 5, "fastrcnn/outputs", f, 1, M, 1, 1, 1, 0, 0, 0, 0, nout, false, true, false, Planes(), 0, 0, nullptr,
-             0, c->head_logits, ldo, 4);
-    reg_planes(c, "fc", f);
+             0, c->head_logits, ldo, kHeadOut);
+    c->stages.planes("fc", f);
   } else {
     Planes f6 = c->fc6; f6.W = M;
     Planes f7 = c->fc7; f7.W = M;
     add_conv(c, 5, "fastrcnn/fc6", rf, 1, M, 1, 1, 1, 0, 0, 0, 0, dim, false, true, true, f6, 0, 0, nullptr, 0, nullptr,
-             0, 1);
+             0, kFc6);
     add_conv(c, 5, "fastrcnn/fc7", f6, 1, M, 1, 1, 1, 0, 0, 0, 0, dim, false, true, true, f7, 0, 0, nullptr, 0, nullptr,
-             0, 2);
+             0, kDense);
     add_conv(c, 5, "fastrcnn/outputs", f7, 1, M, 1, 1, 1, 0, 0, 0, 0, nout, false, true, false, Planes(), 0, 0, nullptr,
-             0, c->head_logits, ldo, 4);
-    reg_planes(c, "fc6", f6);
-    reg_planes(c, "fc7", f7);
+             0, c->head_logits, ldo, kHeadOut);
+    c->stages.planes("fc6", f6);
+    c->stages.planes("fc7", f7);
   }
-  reg_raw(c, "head_logits", c->head_logits, 1, B, K, ldo, 1);
+  c->stages.raw("head_logits", c->head_logits, Stage::kF32, B, K, ldo, 1);
 
   // ---- post-processing (phase 6) ----
   HeadPostParams& hp = c->post;
@@ -621,32 +645,39 @@ int build_plan(b2_ctx* c) {
   hp.score_thresh = cfg.multi_semantics ? -INFINITY : cfg.result_score_thres;
   hp.nms_thr = cfg.fastrcnn_nms_iou_thres;
   hp.max_per_class = R; hp.max_total = R;
-  hp.probs = c->alloc<float>(static_cast<size_t>(M) * cfg.num_class);
-  hp.dec_boxes = c->alloc<float>(static_cast<size_t>(M) * nc1 * 4);
-  hp.cls_keep = c->alloc<int>(static_cast<size_t>(B) * nc1 * R);
-  hp.cls_count = c->alloc<int>(B * nc1);
-  hp.final_boxes = c->alloc<float>(static_cast<size_t>(B) * R * 4);
-  hp.final_probs = c->alloc<float>(static_cast<size_t>(B) * R);
-  hp.final_labels = c->alloc<int>(static_cast<size_t>(B) * R);
-  hp.final_count = c->alloc<int>(B);
-  c->steps.push_back({6, 6, nullptr});
-  reg_raw(c, "probs", hp.probs, 1, B, K, cfg.num_class, 1);
-  reg_raw(c, "dec_boxes", hp.dec_boxes, 1, B, K, nc1, 4);
-  reg_raw(c, "final_boxes", hp.final_boxes, 1, B, R, 4, 1);
-  reg_raw(c, "final_probs", hp.final_probs, 1, B, R, 1, 1);
-  reg_raw(c, "final_labels", hp.final_labels, 2, B, R, 1, 1);
-  reg_raw(c, "final_count", hp.final_count, 2, B, 1, 1, 1);
+  hp.probs = c->arena.alloc<float>(static_cast<size_t>(M) * cfg.num_class);
+  hp.dec_boxes = c->arena.alloc<float>(static_cast<size_t>(M) * nc1 * 4);
+  hp.cls_keep = c->arena.alloc<int>(static_cast<size_t>(B) * nc1 * R);
+  hp.cls_count = c->arena.alloc<int>(B * nc1);
+  hp.final_boxes = c->arena.alloc<float>(static_cast<size_t>(B) * R * 4);
+  hp.final_probs = c->arena.alloc<float>(static_cast<size_t>(B) * R);
+  hp.final_labels = c->arena.alloc<int>(static_cast<size_t>(B) * R);
+  hp.final_count = c->arena.alloc<int>(B);
+  add_batch_step(c, 6, 6, "", [c](int, int, cudaStream_t st) { return head_post_launch(c->post, st); }, 3);
+  c->stages.raw("probs", hp.probs, Stage::kF32, B, K, cfg.num_class, 1);
+  c->stages.raw("dec_boxes", hp.dec_boxes, Stage::kF32, B, K, nc1, 4);
+  c->stages.raw("final_boxes", hp.final_boxes, Stage::kF32, B, R, 4, 1);
+  c->stages.raw("final_probs", hp.final_probs, Stage::kF32, B, R, 1, 1);
+  c->stages.raw("final_labels", hp.final_labels, Stage::kI32, B, R, 1, 1);
+  c->stages.raw("final_count", hp.final_count, Stage::kI32, B, 1, 1, 1);
 
   // ---- fpn_box_feat: ROIAlign of the final boxes (models.py:972-973), phase 7 ----
-  c->box_feat = c->alloc<float>(static_cast<size_t>(B) * R * nc * 49);
-  c->box_feat_pooled = c->alloc<float>(static_cast<size_t>(B) * R * nc);
+  c->box_feat = c->arena.alloc<float>(static_cast<size_t>(B) * R * nc * 49);
+  c->box_feat_pooled = c->arena.alloc<float>(static_cast<size_t>(B) * R * nc);
   RoiAlignParams& r2 = c->roi2;
   r2 = r1;
   r2.rois_per_image = R;
   r2.boxes = hp.final_boxes; r2.count = hp.final_count;
   r2.out_hi = nullptr; r2.out_lo = nullptr; r2.out_nchw = c->box_feat;
-  c->steps.push_back({7, 7, nullptr});
-  reg_raw(c, "fpn_box_feat", c->box_feat, 1, static_cast<int64_t>(B) * R, nc, 7, 7);
+  add_batch_step(c, 7, 7, "", [c](int, int, cudaStream_t st) {
+    if (roialign_launch(c->roi2, st)) return -1;
+    const int rows = c->cfg.batch * c->cfg.result_per_im;
+    pool_feat_kernel<<<(rows * c->cfg.fpn_num_channel + 255) / 256, 256, 0, st>>>(c->box_feat, rows, c->cfg.fpn_num_channel,
+                                                                                   c->box_feat_pooled);
+    B2_CUDA(cudaGetLastError());
+    return 0;
+  }, 2);
+  c->stages.raw("fpn_box_feat", c->box_feat, Stage::kF32, static_cast<int64_t>(B) * R, nc, 7, 7);
 
   // ---- mask head (models.py:934-961, 1173-1199), phase 7, only with cfg.add_mask ----
   if (cfg.add_mask) {
@@ -660,68 +691,50 @@ int build_plan(b2_ctx* c) {
     r3.rois_per_image = R;
     r3.boxes = hp.final_boxes; r3.count = hp.final_count;
     r3.out_hi = c->mask_a.hi; r3.out_lo = c->mask_a.lo; r3.out_nchw = nullptr; r3.out_res = 14;
-    c->steps.push_back({7, 8, nullptr});
+    add_batch_step(c, 7, 8, "", [c](int, int, cudaStream_t st) { return roialign_launch(c->roi3, st); });
     const Planes* pp[2] = {&c->mask_a, &c->mask_b};
     for (int k = 0; k < 4; ++k)                      // conv2d 3x3 SAME + bias + ReLU
       add_conv(c, 7, "maskrcnn/fcn" + std::to_string(k), *pp[k & 1], 14, 14, 3, 1, 1, 1, 1, 1, 1, md, false, true, true,
                *pp[(k + 1) & 1], 0, 0, nullptr, 0);
     // Conv2DTranspose 2x2 stride 2: no overlap between taps, so it is a 1x1 conv onto (tap, channel) outputs
     add_conv(c, 7, "maskrcnn/deconv", c->mask_a, 14, 14, 1, 1, 1, 0, 0, 0, 0, 4 * md, false, true, true, c->mask_up, 0, 0,
-             nullptr, 0, nullptr, 0, 6);
+             nullptr, 0, nullptr, 0, kDeconv);
     // the 1x1 class conv commutes with the pixel shuffle: apply it to the (pixel, tap) rows directly
     const int rows = MR * 196 * 4, rows_pad = (rows + 127) / 128 * 128;
     c->mask_ld = (cfg.num_class - 1 + 15) / 16 * 16;
-    c->mask_logits = c->alloc<float>(static_cast<size_t>(rows_pad) * c->mask_ld);
+    c->mask_logits = c->arena.alloc<float>(static_cast<size_t>(rows_pad) * c->mask_ld);
     Planes up_rows = c->mask_up;
     up_rows.B = 1; up_rows.H = 1; up_rows.W = rows; up_rows.C = md;
     add_conv(c, 7, "maskrcnn/conv", up_rows, 1, rows, 1, 1, 1, 0, 0, 0, 0, cfg.num_class - 1, false, true, false, Planes(),
              0, 0, nullptr, 0, c->mask_logits, c->mask_ld);
-    c->final_masks = c->alloc<float>(static_cast<size_t>(MR) * 784);
-    c->steps.push_back({7, 9, nullptr});
-    reg_planes(c, "mask_roi_feat", c->mask_a);       // valid right after step 8 only (ping-pong buffer)
-    reg_raw(c, "mask_logits", c->mask_logits, 1, MR, 196 * 4, c->mask_ld, 1);
-    reg_raw(c, "final_masks", c->final_masks, 1, B, R, 28, 28);
+    c->final_masks = c->arena.alloc<float>(static_cast<size_t>(MR) * 784);
+    add_batch_step(c, 7, 9, "", [c](int, int, cudaStream_t st) {
+      const size_t total = static_cast<size_t>(c->cfg.batch) * c->cfg.result_per_im * 784;
+      mask_select_kernel<<<static_cast<unsigned>(std::min<size_t>((total + 255) / 256, 132 * 32)), 256, 0, st>>>(
+          c->mask_logits, c->mask_ld, c->post.final_labels, c->post.final_count, c->cfg.batch, c->cfg.result_per_im,
+          c->final_masks);
+      B2_CUDA(cudaGetLastError());
+      return 0;
+    });
+    c->stages.planes("mask_roi_feat", c->mask_a);       // valid right after step 8 only (ping-pong buffer)
+    c->stages.raw("mask_logits", c->mask_logits, Stage::kF32, MR, 196 * 4, c->mask_ld, 1);
+    c->stages.raw("final_masks", c->final_masks, Stage::kF32, B, R, 28, 28);
   }
+
 
   // ---- tensor-core plans ----
   if (cfg.conv_impl == 0) {
-    for (auto& L : c->layers) {
-      L->plan = conv_tc_plan_create(L->d, L->w, L->io, c->split, c->num_sms);
-      if (!L->plan) {
-        set_error(std::string("plan for ") + L->name + ": " + last_error());
-        return -1;
-      }
-    }
-    // Images are independent through phases 0-2 (stem, ResNet, FPN, RPN head): a second set of plans covers each
-    // half of the batch by itself (same tiles per image, so the results are bit-identical to the full-batch plan).
-    c->nsplit = 2;
-    if (const char* e = getenv("B2_SPLIT")) c->nsplit = atoi(e);   // experiment hook: 1, 2, 4, 8 batch parts
-    if (c->nsplit < 1 || c->nsplit > 8 || B % c->nsplit != 0) c->nsplit = 1;
-    c->dual = c->nsplit > 1 && getenv("B2_NO_DUAL") == nullptr;
-    if (c->dual) {
-      for (const auto& s : c->steps) {
-        if (s.kind != 0 || s.phase > 2) continue;
-        Layer* L = s.layer;
-        L->part_plan.assign(c->nsplit, nullptr);
-        for (int h = 0; h < c->nsplit; ++h) {
-          ConvDesc d = L->d;
-          ConvIO io = L->io;
-          d.B = B / c->nsplit;
-          const size_t in_off = static_cast<size_t>(h) * d.B * d.in_pitch_H * d.in_pitch_W * (d.in_ld > 0 ? d.in_ld : d.Cin);
-          const size_t out_off = static_cast<size_t>(h) * d.B * d.out_H * d.out_W * d.ldc;
-          const size_t res_off = static_cast<size_t>(h) * d.B * d.res_H * d.res_W * d.ldr;
-          io.in_hi += in_off;
-          if (io.in_lo) io.in_lo += in_off;
-          if (io.out_hi) io.out_hi += out_off;
-          if (io.out_lo) io.out_lo += out_off;
-          if (io.out_f32) io.out_f32 += out_off;
-          if (io.res_hi) io.res_hi += res_off;
-          if (io.res_lo) io.res_lo += res_off;
-          L->part_plan[h] = conv_tc_plan_create(d, L->w, io, c->split, c->num_sms);
-          if (!L->part_plan[h]) {
-            set_error(std::string("half-batch plan for ") + L->name + ": " + last_error());
-            return -1;
-          }
+    if (plan_convs(c->layers, c->split, c->num_sms)) return -1;
+    // the forked layers over each part of the batch: operands offset by whole images of their own buffers
+    for (ConvLayer* L : c->part_layers) {
+      if (!c->dual) break;
+      for (int h = 0; h < c->nsplit; ++h) {
+        ConvDesc d = L->d;
+        d.B = B / c->nsplit;
+        L->part_plan.emplace_back(conv_tc_plan_create(d, L->w, images(*L, h * d.B), c->split, c->num_sms));
+        if (!L->part_plan.back()) {
+          set_error(std::string("half-batch plan for ") + L->name + ": " + last_error());
+          return -1;
         }
       }
     }
@@ -729,252 +742,74 @@ int build_plan(b2_ctx* c) {
   return 0;
 }
 
-int run_step(b2_ctx* c, const b2_ctx::Step& s) {
-  const b2_config& cfg = c->cfg;
-  cudaStream_t st = c->stream;
-  switch (s.kind) {
-    case 0:
-      if (cfg.conv_impl == 0) return conv_tc_launch(s.layer->plan, st);
-      return conv_simt_launch(s.layer->d, s.layer->w, s.layer->io, c->split, st);
-    case 1:
-      return stem_pack16_launch(c->img, cfg.input_dtype == 1, cfg.batch, cfg.height, cfg.width, c->stem_u.hi,
-                                c->stem_u.lo, c->stem_u.H, c->stem_u.W, st);
-    case 2:
-      return maxpool_launch(c->c1.hi, c->c1.lo, cfg.batch, c->c1h, c->c1w, 64, c->pool.hi, c->pool.lo, c->ch[0],
-                            c->cw[0], st);
-    case 3: {
-      const Planes& p5 = c->pfeat[3];
-      const Planes& p6 = c->pfeat[4];
-      const size_t total = static_cast<size_t>(p6.B) * p6.H * p6.W * (p6.C / 8);
-      subsample2_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, st>>>(p5.hi, p5.lo, p5.B, p5.H, p5.W,
-                                                                                     p5.C, p6.hi, p6.lo, p6.H, p6.W);
-      B2_CUDA(cudaGetLastError());
-      return 0;
-    }
-    case 4:
-      return rpn_proposals_launch(c->rpn, st);
-    case 5:
-      return roialign_launch(c->roi1, st);
-    case 6:
-      return head_post_launch(c->post, st);
-    case 7: {
-      if (roialign_launch(c->roi2, st)) return -1;
-      const int rows = cfg.batch * cfg.result_per_im;
-      pool_feat_kernel<<<(rows * cfg.fpn_num_channel + 255) / 256, 256, 0, st>>>(c->box_feat, rows,
-                                                                                 cfg.fpn_num_channel,
-                                                                                 c->box_feat_pooled);
-      B2_CUDA(cudaGetLastError());
-      return 0;
-    }
-    case 8:
-      return roialign_launch(c->roi3, st);
-    case 9: {
-      const size_t total = static_cast<size_t>(cfg.batch) * cfg.result_per_im * 784;
-      mask_select_kernel<<<static_cast<unsigned>(std::min<size_t>((total + 255) / 256, 132 * 32)), 256, 0, st>>>(
-          c->mask_logits, c->mask_ld, c->post.final_labels, c->post.final_count, cfg.batch, cfg.result_per_im,
-          c->final_masks);
-      B2_CUDA(cudaGetLastError());
-      return 0;
-    }
-    case 10:
-      return gn_stats_launch(s.gn->p, st);
-    case 11:
-      return gn_apply_launch(s.gn->p, st);
-    case 12:
-      return gn_roi_launch(s.gn->p, st);
-  }
-  return -1;
-}
-
-// The launch of GroupNorm `p` restricted to images [h * hb, (h + 1) * hb).
-GnParams gn_part(GnParams p, int h, int hb) {
-  const size_t xo = static_cast<size_t>(h) * hb * p.pitch_H * p.pitch_W * p.ld;
-  p.x_hi += xo; p.y_hi += xo;
-  if (p.x_lo) p.x_lo += xo;
-  if (p.y_lo) p.y_lo += xo;
-  if (p.r_hi) {
-    const size_t ro = static_cast<size_t>(h) * hb * p.res_H * p.res_W * p.res_ld;
-    p.r_hi += ro;
-    if (p.r_lo) p.r_lo += ro;
-  }
-  p.partial += static_cast<size_t>(h) * hb * p.chunks * 32 * 3;
-  p.stats += static_cast<size_t>(h) * hb * 32 * 2;
-  p.counter += static_cast<size_t>(h) * hb;
-  p.B = hb;
-  return p;
-}
-
-// One step of phases 0-2 over part `h` (of nsplit) of the batch, on stream `st`.
-int run_step_half(b2_ctx* c, const b2_ctx::Step& s, int h, cudaStream_t st) {
-  const b2_config& cfg = c->cfg;
-  const int hb = cfg.batch / c->nsplit;
-  auto off = [&](const Planes& p) { return static_cast<size_t>(h) * hb * p.H * p.W * p.C; };
-  auto lo = [&](const Planes& p) { return p.lo ? p.lo + off(p) : nullptr; };
-  switch (s.kind) {
-    case 0:
-      return conv_tc_launch(s.layer->part_plan[h], st);
-    case 1:
-      return stem_pack16_launch(static_cast<const uint8_t*>(c->img) + static_cast<size_t>(h) * (c->img_bytes / c->nsplit),
-                                cfg.input_dtype == 1, hb, cfg.height, cfg.width, c->stem_u.hi + off(c->stem_u),
-                                lo(c->stem_u), c->stem_u.H, c->stem_u.W, st);
-    case 2:
-      return maxpool_launch(c->c1.hi + off(c->c1), lo(c->c1), hb, c->c1h, c->c1w, 64, c->pool.hi + off(c->pool),
-                            lo(c->pool), c->ch[0], c->cw[0], st);
-    case 3: {
-      const Planes& p5 = c->pfeat[3];
-      const Planes& p6 = c->pfeat[4];
-      const size_t total = static_cast<size_t>(hb) * p6.H * p6.W * (p6.C / 8);
-      subsample2_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, st>>>(
-          p5.hi + off(p5), lo(p5), hb, p5.H, p5.W, p5.C, p6.hi + off(p6), lo(p6), p6.H, p6.W);
-      B2_CUDA(cudaGetLastError());
-      return 0;
-    }
-    case 10:
-      return gn_stats_launch(gn_part(s.gn->p, h, hb), st);
-    case 11:
-      return gn_apply_launch(gn_part(s.gn->p, h, hb), st);
-  }
-  return -1;
-}
-
-int step_launches(const b2_ctx::Step& s) {
-  switch (s.kind) {
-    case 4: return 2;
-    case 6: return 3;
-    case 7: return 2;
-    case 10: case 11: case 12: return 1;   // GroupNorm statistics / apply / per-ROI
-    default: return 1;
-  }
-}
-
-// The whole pass with phases 0-2 forked over two streams (also valid inside a stream capture: the second stream joins
-// the capture through the fork event and rejoins before the proposals).
+// The whole pass with phases 0-2 forked over nsplit streams (also valid inside a stream capture: the side streams join
+// the capture through the fork event and rejoin before the proposals).
 int enqueue_dual(b2_ctx* c) {
   B2_CUDA(cudaEventRecord(c->fork_ev, c->stream));
   for (int h = 1; h < c->nsplit; ++h) B2_CUDA(cudaStreamWaitEvent(c->side_stream[h - 1], c->fork_ev, 0));
-  for (const auto& s : c->steps) {
+  for (const Step& s : c->steps) {
     if (s.phase > 2) continue;
     for (int h = 0; h < c->nsplit; ++h)
-      if (run_step_half(c, s, h, h == 0 ? c->stream : c->side_stream[h - 1])) return -1;
+      if (s.parts[h](h == 0 ? c->stream : c->side_stream[h - 1])) return -1;
   }
   for (int h = 1; h < c->nsplit; ++h) {
     B2_CUDA(cudaEventRecord(c->join_ev[h - 1], c->side_stream[h - 1]));
     B2_CUDA(cudaStreamWaitEvent(c->stream, c->join_ev[h - 1], 0));
   }
-  for (const auto& s : c->steps)
-    if (s.phase > 2 && run_step(c, s)) return -1;
-  return 0;
+  return run_steps(c->steps, ~0x7u, c->stream);
 }
 
 int enqueue(b2_ctx* c, int mask, bool with_events) {
   if (c->dual && !with_events && mask == B2_PHASE_ALL) return enqueue_dual(c);
-  if (with_events) B2_CUDA(cudaEventRecord(c->ev[0], c->stream));
+  if (!with_events) return run_steps(c->steps, mask, c->stream);
+  B2_CUDA(cudaEventRecord(c->ev[0], c->stream));
   int last = -1;
-  for (const auto& s : c->steps) {
+  for (const Step& s : c->steps) {
     if (!(mask & (1 << s.phase))) continue;
-    if (with_events && last >= 0 && s.phase != last) B2_CUDA(cudaEventRecord(c->ev[last + 1], c->stream));
-    if (run_step(c, s)) return -1;
+    if (last >= 0 && s.phase != last) B2_CUDA(cudaEventRecord(c->ev[last + 1], c->stream));
+    if (s.run(c->stream)) return -1;
     last = s.phase;
   }
-  if (with_events && last >= 0) B2_CUDA(cudaEventRecord(c->ev[last + 1], c->stream));
+  if (last >= 0) B2_CUDA(cudaEventRecord(c->ev[last + 1], c->stream));
   return 0;
 }
 
 // ---- weight loading -------------------------------------------------------------------------
-struct WeightSet {
-  std::map<std::string, std::pair<const float*, int64_t>> m;
-  const float* get(const std::string& n, int64_t expect) const {
-    auto it = m.find(n);
-    if (it == m.end()) { set_error("missing weight: " + n); return nullptr; }
-    if (it->second.second != expect) {
-      set_error("weight " + n + ": expected " + std::to_string(expect) + " values, got " +
-                std::to_string(it->second.second));
-      return nullptr;
-    }
-    return it->second.first;
-  }
-  bool has(const std::string& n) const { return m.count(n) != 0; }
-};
-
-// BatchNorm inference folded into a per-output-channel scale/shift (nn.py:1771-1774, eps 1e-5)
-int bn_fold(const WeightSet& ws, const std::string& scope, int C, std::vector<double>& scale,
-            std::vector<double>& shift) {
-  const float* g = ws.get(scope + "/bn/gamma", C);
-  const float* b = ws.get(scope + "/bn/beta", C);
-  const float* m = ws.get(scope + "/bn/mean/EMA", C);
-  const float* v = ws.get(scope + "/bn/variance/EMA", C);
-  if (!g || !b || !m || !v) return -1;
-  scale.resize(C);
-  shift.resize(C);
-  for (int i = 0; i < C; ++i) {
-    const double inv = static_cast<double>(g[i]) / sqrt(static_cast<double>(v[i]) + 1e-5);
-    scale[i] = inv;
-    shift[i] = static_cast<double>(b[i]) - static_cast<double>(m[i]) * inv;
-  }
-  return 0;
-}
-
-int upload_layer(b2_ctx* c, Layer* L, const std::vector<float>& packed, const std::vector<float>& bias) {
-  const size_t n = packed.size();
-  // the (hi, lo) operand planes are fp16: a folded weight beyond +-65504 (or a non-finite one) would become inf here and
-  // NaN inside the MMA (inf * 0) -- refuse it at load time; activations are watched by the kernel's range monitor
-  for (size_t i = 0; i < n; ++i)
-    if (!(fabsf(packed[i]) <= 65504.f)) {
-      set_error("weight of layer '" + L->name + "' outside the fp16-plane range (|w| > 65504 after BatchNorm folding, or not "
-                "finite): this checkpoint is not representable in the (hi, lo) fp16 operand format");
-      return -1;
-    }
-  for (size_t i = 0; i < bias.size(); ++i)
-    if (!std::isfinite(bias[i])) {
-      set_error("bias / folded BatchNorm shift of layer '" + L->name + "' is not finite");
-      return -1;
-    }
-  float* tmp = nullptr;
-  B2_CUDA(cudaMalloc(&tmp, n * sizeof(float)));
-  B2_CUDA(cudaMemcpyAsync(tmp, packed.data(), n * sizeof(float), cudaMemcpyHostToDevice, c->stream));
-  if (f32_to_planes(tmp, L->w.w_hi, L->w.w_lo, n, c->stream)) return -1;
-  B2_CUDA(cudaMemcpyAsync(L->w.bias, bias.data(), bias.size() * sizeof(float), cudaMemcpyHostToDevice, c->stream));
-  B2_CUDA(cudaStreamSynchronize(c->stream));
-  B2_CUDA(cudaFree(tmp));
-  return 0;
-}
-
-int load_layer(b2_ctx* c, Layer* L, const WeightSet& ws) {
+int load_layer(b2_ctx* c, const ConvLayer* L, const WeightSet& ws) {
   const int Cin = L->d.Cin, R = L->d.R, S = L->d.S, Cout = L->d.Cout, K = L->w.K, Cp = L->w.Cout_pad;
-  std::vector<float> packed(static_cast<size_t>(Cp) * K, 0.f), bias(Cp, 0.f);
-  std::vector<double> scale(Cout, 1.0), shift(Cout, 0.0);
-  if (L->kind == 0) {
+  std::vector<float> packed(static_cast<size_t>(Cp) * K, 0.f);
+  std::vector<double> scale, shift;
+  // BatchNorm inference (nn.py:1771-1774, eps 1e-5)
+  if (fold_bn(ws, L->bn, kTensorpackBn, 1e-5, Cout, scale, shift)) return -1;
+  std::vector<float> b(Cout, 0.f);   // the layer's bias, when it has one
+  bool has_b = !L->bias.empty();
+  if (L->layout == kHwio) {
     const float* w = ws.get(L->name + "/W", static_cast<int64_t>(R) * S * Cin * Cout);   // HWIO
     if (!w) return -1;
-    if (L->has_bn && bn_fold(ws, L->name, Cout, scale, shift)) return -1;
-    if (L->has_bias) {
-      const float* b = ws.get(L->name + "/b", Cout);
-      if (!b) return -1;
-      for (int o = 0; o < Cout; ++o) shift[o] = b[o];
-    }
     for (int t = 0; t < R * S; ++t)
       for (int ci = 0; ci < Cin; ++ci) {
         const float* src = w + (static_cast<size_t>(t) * Cin + ci) * Cout;
         for (int o = 0; o < Cout; ++o)
           packed[static_cast<size_t>(o) * K + static_cast<size_t>(t) * Cin + ci] = static_cast<float>(src[o] * scale[o]);
       }
-  } else if (L->kind == 6) {
+  } else if (L->layout == kDeconv) {
     // tf.layers.Conv2DTranspose kernel [kh=2, kw=2, out, in] (nn.py:402-412): output row (dy*2+dx)*out + o of the 1x1 conv
     const int co = Cout / 4;
     const float* w = ws.get(L->name + "/W", static_cast<int64_t>(4) * co * Cin);
-    const float* b = ws.get(L->name + "/b", co);
-    if (!w || !b) return -1;
+    const float* bb = ws.get(L->bias, co);
+    if (!w || !bb) return -1;
     for (int t = 0; t < 4; ++t)
       for (int o = 0; o < co; ++o) {
         const float* src = w + (static_cast<size_t>(t) * co + o) * Cin;
         for (int ci = 0; ci < Cin; ++ci) packed[static_cast<size_t>(t * co + o) * K + ci] = src[ci];
-        shift[t * co + o] = b[o];
+        b[t * co + o] = bb[o];
       }
-  } else if (L->kind == 5) {
+    has_b = false;
+  } else if (L->layout == kStem) {
     // stem: reference HWIO [7,7,3,64] re-indexed for the packed operand (stem.cu):
     // W'[o][r][s*16 + ry*6 + sx*3 + c] = W[2r+ry][2s+sx][c][o]   (12 real + 4 zero channels per width tap s)
     const float* w = ws.get(L->name + "/W", 7 * 7 * 3 * 64);
-    if (!w || (L->has_bn && bn_fold(ws, L->name, Cout, scale, shift))) return -1;
+    if (!w) return -1;
     for (int r = 0; r < 4; ++r)
       for (int ch = 0; ch < 64; ++ch) {
         const int s4 = ch / 16, r12 = ch % 16, ry = r12 / 6, sx = (r12 % 6) / 3, cc = r12 % 3;
@@ -984,31 +819,27 @@ int load_layer(b2_ctx* c, Layer* L, const WeightSet& ws) {
         for (int o = 0; o < Cout; ++o)
           packed[static_cast<size_t>(o) * K + static_cast<size_t>(r) * Cin + ch] = static_cast<float>(src[o] * scale[o]);
       }
-  } else if (L->kind == 1) {
+  } else if (L->layout == kFc6) {
     // fc6 (and the conv head's fc): reference flattens NCHW (index c*49 + y*7 + x, models.py:1056 + nn.py:738-740);
     // our ROI features are [y][x][c], so permute the rows of W [in, out].
     const int C = Cin / 49;
     const float* w = ws.get(L->name + "/W", static_cast<int64_t>(Cin) * Cout);
-    const float* b = ws.get(L->name + "/b", Cout);
-    if (!w || !b) return -1;
+    if (!w) return -1;
     for (int ch = 0; ch < C; ++ch)
       for (int s = 0; s < 49; ++s) {
         const float* src = w + (static_cast<size_t>(ch) * 49 + s) * Cout;
         const size_t k = static_cast<size_t>(s) * C + ch;
         for (int o = 0; o < Cout; ++o) packed[static_cast<size_t>(o) * K + k] = src[o];
       }
-    for (int o = 0; o < Cout; ++o) shift[o] = b[o];
-  } else if (L->kind == 2) {
+  } else if (L->layout == kDense) {
     const float* w = ws.get(L->name + "/W", static_cast<int64_t>(Cin) * Cout);
-    const float* b = ws.get(L->name + "/b", Cout);
-    if (!w || !b) return -1;
+    if (!w) return -1;
     for (int k = 0; k < Cin; ++k)
       for (int o = 0; o < Cout; ++o) packed[static_cast<size_t>(o) * K + k] = w[static_cast<size_t>(k) * Cout + o];
-    for (int o = 0; o < Cout; ++o) shift[o] = b[o];
-  } else if (L->kind == 3 || L->kind == 4) {
+  } else {
     // two reference layers fused along N: rpn/{class,box} or fastrcnn/outputs/{class,box}
-    const std::string base = L->kind == 3 ? "rpn" : "fastrcnn/outputs";
-    const int n0 = L->kind == 3 ? 3 : c->cfg.num_class;
+    const std::string base = L->layout == kRpnOut ? "rpn" : "fastrcnn/outputs";
+    const int n0 = L->layout == kRpnOut ? 3 : c->cfg.num_class;
     const int n1 = Cout - n0;
     const float* w0 = ws.get(base + "/class/W", static_cast<int64_t>(Cin) * n0);
     const float* b0 = ws.get(base + "/class/b", n0);
@@ -1019,11 +850,16 @@ int load_layer(b2_ctx* c, Layer* L, const WeightSet& ws) {
       for (int o = 0; o < n0; ++o) packed[static_cast<size_t>(o) * K + k] = w0[static_cast<size_t>(k) * n0 + o];
       for (int o = 0; o < n1; ++o) packed[static_cast<size_t>(n0 + o) * K + k] = w1[static_cast<size_t>(k) * n1 + o];
     }
-    for (int o = 0; o < n0; ++o) shift[o] = b0[o];
-    for (int o = 0; o < n1; ++o) shift[n0 + o] = b1[o];
+    for (int o = 0; o < n0; ++o) b[o] = b0[o];
+    for (int o = 0; o < n1; ++o) b[n0 + o] = b1[o];
+    has_b = false;
   }
-  for (int o = 0; o < Cout; ++o) bias[o] = static_cast<float>(shift[o]);
-  return upload_layer(c, L, packed, bias);
+  if (has_b) {
+    const float* bb = ws.get(L->bias, Cout);
+    if (!bb) return -1;
+    b.assign(bb, bb + Cout);
+  }
+  return upload_conv(*L, packed, fold_bias(scale, shift, L->bias.empty() ? nullptr : b.data(), Cout, Cp), c->stream);
 }
 
 // group_norm's "<scope>/gamma" and "<scope>/beta" (nn.py:97-102), [C] each
@@ -1045,22 +881,14 @@ int load_gn(b2_ctx* c, GnOp* G, const WeightSet& ws) {
 // =================================================================================================
 extern "C" {
 
-const char* b2_last_error(void) { return b2::last_error(); }
-int b2_version(void) { return 1; }
-
 int b2_create(b2_ctx** out, int device, const b2_config* cfg) {
   B2_CHECK(out && cfg, "b2_create: null argument");
   *out = nullptr;
-  B2_CUDA(cudaSetDevice(device));
   std::unique_ptr<b2_ctx> c(new b2_ctx());
   c->cfg = *cfg;
   c->device = device;
   c->split = cfg->precision == 1;
-  cudaDeviceProp prop;
-  B2_CUDA(cudaGetDeviceProperties(&prop, device));
-  B2_CHECK(prop.major == 9 && prop.minor == 0, "b2_create: this library is built for sm_90a (H100) only");
-  c->num_sms = prop.multiProcessorCount;
-  B2_CUDA(cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking));
+  if (open_device(device, "b2_create", &c->num_sms, &c->stream)) return -1;
   for (int i = 0; i <= NPHASE; ++i) B2_CUDA(cudaEventCreate(&c->ev[i]));
   memset(c->phase_ms, 0, sizeof(c->phase_ms));
   if (build_plan(c.get())) {
@@ -1074,8 +902,6 @@ int b2_create(b2_ctx** out, int device, const b2_config* cfg) {
       B2_CUDA(cudaEventCreateWithFlags(&c->join_ev[h - 1], cudaEventDisableTiming));
     }
   }
-  c->launches = 0;
-  for (const auto& s : c->steps) c->launches += step_launches(s) * ((c->dual && s.phase <= 2) ? c->nsplit : 1);
   B2_CUDA(cudaDeviceSynchronize());
   *out = c.release();
   return 0;
@@ -1086,11 +912,6 @@ void b2_destroy(b2_ctx* c) {
   cudaSetDevice(c->device);
   cudaDeviceSynchronize();
   if (c->graph) cudaGraphExecDestroy(c->graph);
-  for (auto& L : c->layers) {
-    if (L->plan) conv_tc_plan_destroy(L->plan);
-    for (ConvPlan* pp : L->part_plan)
-      if (pp) conv_tc_plan_destroy(pp);
-  }
   if (c->fork_ev) cudaEventDestroy(c->fork_ev);
   for (int h = 0; h < 7; ++h) {
     if (c->join_ev[h]) cudaEventDestroy(c->join_ev[h]);
@@ -1098,7 +919,6 @@ void b2_destroy(b2_ctx* c) {
   }
   if (c->raw_frames) cudaFree(c->raw_frames);
   if (c->h_range) cudaFreeHost(c->h_range);
-  for (void* p : c->allocs) cudaFree(p);
   for (int i = 0; i <= NPHASE; ++i)
     if (c->ev[i]) cudaEventDestroy(c->ev[i]);
   for (int i = 0; i < 2; ++i) {
@@ -1110,14 +930,13 @@ void b2_destroy(b2_ctx* c) {
   if (c->copy_stream) cudaStreamDestroy(c->copy_stream);
   if (c->down_stream) cudaStreamDestroy(c->down_stream);
   if (c->stream) cudaStreamDestroy(c->stream);
-  delete c;
+  delete c;   // plans, then the arena's device memory
 }
 
 int b2_load_weights(b2_ctx* c, const char* const* names, const float* const* data, const int64_t* numel, int n) {
   B2_CHECK(c && names && data && numel, "b2_load_weights: null argument");
   B2_CUDA(cudaSetDevice(c->device));
-  WeightSet ws;
-  for (int i = 0; i < n; ++i) ws.m[names[i]] = std::make_pair(data[i], numel[i]);
+  const WeightSet ws(names, data, numel, n);
   // shared RPN weights: packed once, every level's layer gets its own copy of the (small) operand
   for (auto& L : c->layers)
     if (load_layer(c, L.get(), ws)) return -1;
@@ -1129,14 +948,18 @@ int b2_load_weights(b2_ctx* c, const char* const* names, const float* const* dat
 
 static int range_failed(b2_ctx* c, int idx);
 
+// Waits for the stream and fails when the pass left the fp16-plane range (synchronous calls).
+static int sync_range(b2_ctx* c) {
+  B2_CUDA(cudaMemcpyAsync(&c->h_range[2], c->range_flag, sizeof(unsigned int), cudaMemcpyDeviceToHost, c->stream));
+  B2_CUDA(cudaStreamSynchronize(c->stream));
+  return range_failed(c, 2);
+}
+
 int b2_run_phases(b2_ctx* c, int mask) {
   B2_CHECK(c, "b2_run_phases: null ctx");
   B2_CUDA(cudaSetDevice(c->device));
   B2_CHECK(c->weights_loaded, "b2_run_phases: weights not loaded");
-  if (enqueue(c, mask, true)) return -1;
-  B2_CUDA(cudaMemcpyAsync(&c->h_range[2], c->range_flag, sizeof(unsigned int), cudaMemcpyDeviceToHost, c->stream));
-  B2_CUDA(cudaStreamSynchronize(c->stream));
-  if (range_failed(c, 2)) return -1;
+  if (enqueue(c, mask, true) || sync_range(c)) return -1;
   int last = -1;
   for (int ph = 0; ph < NPHASE; ++ph) {
     c->phase_ms[ph] = 0.f;
@@ -1156,95 +979,27 @@ int b2_phase_times(b2_ctx* c, float ms[8]) {
   return 0;
 }
 
-int b2_kernel_launches(b2_ctx* c) { return c ? c->launches : -1; }
+int b2_kernel_launches(b2_ctx* c) { return c ? total_launches(c->steps) : -1; }
 
 // Per-step device timing (CUDA events around every launch group, eager mode), averaged over `reps`.
 int b2_profile_steps(b2_ctx* c, int reps, float* ms_out, int cap, int* n_out) {
   B2_CHECK(c && ms_out && n_out, "b2_profile_steps: null argument");
   B2_CUDA(cudaSetDevice(c->device));
   B2_CHECK(c->weights_loaded, "b2_profile_steps: weights not loaded");
-  const int n = static_cast<int>(c->steps.size());
-  B2_CHECK(cap >= n, "b2_profile_steps: buffer too small");
-  std::vector<cudaEvent_t> ev(2 * n);
-  for (auto& e : ev) B2_CUDA(cudaEventCreate(&e));
-  std::vector<double> acc(n, 0.0);
-  for (int r = 0; r < reps; ++r) {
-    for (int i = 0; i < n; ++i) {
-      B2_CUDA(cudaEventRecord(ev[2 * i], c->stream));
-      if (run_step(c, c->steps[i])) return -1;
-      B2_CUDA(cudaEventRecord(ev[2 * i + 1], c->stream));
-    }
-    B2_CUDA(cudaStreamSynchronize(c->stream));
-    for (int i = 0; i < n; ++i) {
-      float ms = 0.f;
-      B2_CUDA(cudaEventElapsedTime(&ms, ev[2 * i], ev[2 * i + 1]));
-      acc[i] += ms;
-    }
-  }
-  for (int i = 0; i < n; ++i) ms_out[i] = static_cast<float>(acc[i] / reps);
-  for (auto& e : ev) cudaEventDestroy(e);
-  *n_out = n;
-  return 0;
+  return profile_steps(c->steps, c->stream, reps, ms_out, cap, n_out);
 }
 
 // Describes step `idx`: name, kind (0 = tensor-core conv/dense), algorithmic FLOPs and HBM bytes
 // (each operand read once, output written once, at the stored precision).
 int b2_step_info(b2_ctx* c, int idx, char* name, int name_cap, double* flops, double* bytes, int* kind) {
-  B2_CHECK(c && name && flops && bytes && kind, "b2_step_info: null argument");
-  B2_CHECK(idx >= 0 && idx < static_cast<int>(c->steps.size()), "b2_step_info: index out of range");
-  const b2_ctx::Step& s = c->steps[idx];
-  static const char* kKindNames[] = {"conv", "stem_pack", "maxpool", "p6_subsample", "rpn_proposals", "roialign_proposals",
-                                     "head_post", "roialign_final", "roialign_mask", "mask_select", "gn_stats", "gn_apply",
-                                     "gn_roi"};
-  std::string nm = s.kind == 0 ? s.layer->name : kKindNames[s.kind];
-  *kind = s.kind;
-  *flops = 0;
-  *bytes = 0;
-  const double esz = c->split ? 4.0 : 2.0;
-  if (s.kind == 0) {
-    const ConvDesc& d = s.layer->d;
-    const double M = static_cast<double>(d.B) * d.Ho() * d.Wo();
-    const double K = static_cast<double>(d.R) * d.S * d.Cin;
-    *flops = 2.0 * M * K * d.Cout;
-    const double in_px = static_cast<double>(d.B) * d.in_H * d.in_W;
-    *bytes = in_px * (d.in_ld > 0 && d.in_ld < d.Cin ? d.in_ld : d.Cin) * esz + K * d.Cout * esz + M * d.Cout * (s.layer->io.out_f32 ? 4.0 : esz) +
-             (s.layer->io.res_hi ? M * d.Cout * esz / (d.res_shift ? 4.0 : 1.0) : 0.0);
-    nm += " [" + std::to_string(d.in_H) + "x" + std::to_string(d.in_W) + "x" + std::to_string(d.Cin) + " " +
-          std::to_string(d.R) + "x" + std::to_string(d.S) + "/" + std::to_string(d.stride) + " d" +
-          std::to_string(d.dil) + " ->" + std::to_string(d.Cout) + "]";
-  } else if (s.kind == 1) {
-    *bytes = static_cast<double>(c->img_bytes) + static_cast<double>(c->stem_u.elems()) * esz;
-  } else if (s.kind == 2) {
-    *bytes = (static_cast<double>(c->c1.elems()) + c->pool.elems()) * esz;
-  } else if (s.kind >= 10 && s.kind <= 12) {
-    // GroupNorm: statistics read the view once; apply / per-ROI read it, write it and read the residual (a quarter of
-    // the view's size when it is upsampled)
-    const GnParams& p = s.gn->p;
-    const double n = static_cast<double>(p.B) * p.H * p.W * p.C;
-    *bytes = s.kind == 10 ? n * esz : 2.0 * n * esz + (p.r_hi ? n * esz / (p.res_shift ? 4.0 : 1.0) : 0.0);
-    nm = s.gn->name + (s.kind == 10 ? " stats" : s.kind == 11 ? " apply" : " per-roi") + " [" + std::to_string(p.H) +
-         "x" + std::to_string(p.W) + "x" + std::to_string(p.C) +
-         (s.kind != 10 && p.r_hi ? (p.res_shift ? " +up2" : " +res") : "") + (s.kind != 10 && p.relu ? " relu" : "") + "]";
-  }
-  snprintf(name, name_cap, "%s", nm.c_str());
-  return 0;
+  B2_CHECK(c, "b2_step_info: null argument");
+  return step_info(c->steps, idx, name, name_cap, flops, bytes, kind);
 }
 int b2_num_steps(b2_ctx* c) { return c ? static_cast<int>(c->steps.size()) : -1; }
 
 static int ensure_graph(b2_ctx* c) {
   if (c->graph || !c->cfg.use_cuda_graph) return 0;
-  cudaGraph_t g = nullptr;
-  // one eager pass first: lazy one-time attribute setup must not happen inside the capture
-  if (enqueue(c, B2_PHASE_ALL, false)) return -1;
-  B2_CUDA(cudaStreamSynchronize(c->stream));
-  B2_CUDA(cudaStreamBeginCapture(c->stream, cudaStreamCaptureModeThreadLocal));
-  const int rc = enqueue(c, B2_PHASE_ALL, false);
-  cudaError_t e = cudaStreamEndCapture(c->stream, &g);
-  if (rc) return -1;
-  B2_CUDA(e);
-  B2_CUDA(cudaGraphInstantiate(&c->graph, g, 0));
-  B2_CUDA(cudaGraphDestroy(g));
-  return 0;
+  return capture_graph(c->stream, [c] { return enqueue(c, B2_PHASE_ALL, false); }, &c->graph);
 }
 
 static int run_all(b2_ctx* c) {
@@ -1282,7 +1037,7 @@ static int copy_outputs(b2_ctx* c, float* boxes, float* probs, int32_t* labels, 
     } else if (feat_mode >= 2) {
       const int rows = B * R, n = feat_mode == 2 ? rows * C : rows * 49;
       if (!c->box_feat_agg) {
-        c->box_feat_agg = c->alloc<float>(static_cast<size_t>(rows) * (C > 49 ? C : 49), /*zero=*/false);   // fully overwritten
+        c->box_feat_agg = c->arena.alloc<float>(static_cast<size_t>(rows) * (C > 49 ? C : 49), /*zero=*/false);   // fully overwritten
         B2_CHECK(c->box_feat_agg != nullptr, "out of device memory (feature aggregation scratch)");
       }
       agg_feat_kernel<<<(n + 255) / 256, 256, 0, st>>>(c->box_feat, rows, C, feat_mode, c->box_feat_agg);
@@ -1304,12 +1059,7 @@ int b2_detect(b2_ctx* c, const void* frames_dev, float* boxes, float* probs, int
     B2_CUDA(cudaMemcpyAsync(c->img, frames_dev, c->img_bytes, cudaMemcpyDeviceToDevice, c->stream));
   if (run_all(c)) return -1;
   if (copy_outputs(c, boxes, probs, labels, valid, box_feat, feat_mode, cudaMemcpyDeviceToDevice)) return -1;
-  if (sync) {
-    B2_CUDA(cudaMemcpyAsync(&c->h_range[2], c->range_flag, sizeof(unsigned int), cudaMemcpyDeviceToHost, c->stream));
-    B2_CUDA(cudaStreamSynchronize(c->stream));
-    return range_failed(c, 2);
-  }
-  return 0;
+  return sync ? sync_range(c) : 0;
 }
 
 int b2_detect_host(b2_ctx* c, const void* frames_host, float* boxes, float* probs, int32_t* labels, int32_t* valid,
@@ -1320,9 +1070,7 @@ int b2_detect_host(b2_ctx* c, const void* frames_host, float* boxes, float* prob
   B2_CUDA(cudaMemcpyAsync(c->img, frames_host, c->img_bytes, cudaMemcpyHostToDevice, c->stream));
   if (run_all(c)) return -1;
   if (copy_outputs(c, boxes, probs, labels, valid, box_feat, feat_mode, cudaMemcpyDeviceToHost)) return -1;
-  B2_CUDA(cudaMemcpyAsync(&c->h_range[2], c->range_flag, sizeof(unsigned int), cudaMemcpyDeviceToHost, c->stream));
-  B2_CUDA(cudaStreamSynchronize(c->stream));
-  return range_failed(c, 2);
+  return sync_range(c);
 }
 
 // Frame ingest with the resize on the device (SURVEY 8f rank 1; reference host path: frame.astype("float32") ->
@@ -1351,30 +1099,7 @@ int b2_detect_host_resize(b2_ctx* c, const uint8_t* frames_u8, int src_h, int sr
                        c->stream)) return -1;
   if (run_all(c)) return -1;
   if (copy_outputs(c, boxes, probs, labels, valid, box_feat, feat_mode, cudaMemcpyDeviceToHost)) return -1;
-  B2_CUDA(cudaMemcpyAsync(&c->h_range[2], c->range_flag, sizeof(unsigned int), cudaMemcpyDeviceToHost, c->stream));
-  B2_CUDA(cudaStreamSynchronize(c->stream));
-  return range_failed(c, 2);
-}
-
-// The resize alone (parity tests): host uint8 [n, src_h, src_w, 3] -> host float32 [n, dst_h, dst_w, 3].
-int b2_resize_frames(int device, const uint8_t* frames_u8, int n, int src_h, int src_w, int dst_h, int dst_w,
-                     float* out_host) {
-  B2_CHECK(frames_u8 && out_host && n > 0 && src_h > 0 && src_w > 0 && dst_h > 0 && dst_w > 0, "b2_resize_frames: bad argument");
-  B2_CUDA(cudaSetDevice(device));
-  uint8_t* d_src = nullptr;
-  float* d_dst = nullptr;
-  const size_t nb_src = static_cast<size_t>(n) * src_h * src_w * 3, nb_dst = static_cast<size_t>(n) * dst_h * dst_w * 3 * sizeof(float);
-  B2_CUDA(cudaMalloc(&d_src, nb_src));
-  cudaError_t e = cudaMalloc(&d_dst, nb_dst);
-  if (e == cudaSuccess) e = cudaMemcpy(d_src, frames_u8, nb_src, cudaMemcpyHostToDevice);
-  int rc = 0;
-  if (e == cudaSuccess) rc = resize_u8_launch(d_src, n, src_h, src_w, d_dst, dst_h, dst_w, nullptr);
-  if (e == cudaSuccess && !rc) e = cudaMemcpy(out_host, d_dst, nb_dst, cudaMemcpyDeviceToHost);
-  cudaFree(d_src);
-  cudaFree(d_dst);
-  if (rc) return -1;
-  B2_CUDA(e);
-  return 0;
+  return sync_range(c);
 }
 
 // Pipelined ingest for streaming drivers (the reference's queue-fed loop, obj_detect_tracking_multi_queuer.py:386-480):
@@ -1398,10 +1123,9 @@ static int submit_impl(b2_ctx* c, const void* frames_host, int src_h, int src_w,
     B2_CUDA(cudaStreamCreateWithFlags(&c->copy_stream, cudaStreamNonBlocking));
     B2_CUDA(cudaStreamCreateWithFlags(&c->down_stream, cudaStreamNonBlocking));
     for (int i = 0; i < 2; ++i) {
-      B2_CUDA(cudaMalloc(&c->stage_in[i], c->img_bytes));
-      c->allocs.push_back(c->stage_in[i]);
-      B2_CUDA(cudaMalloc(&c->stage_out[i], nb_boxes + nb_probs + nb_labels + nb_valid + nb_feat));
-      c->allocs.push_back(c->stage_out[i]);
+      c->stage_in[i] = c->arena.alloc<uint8_t>(c->img_bytes, false);
+      c->stage_out[i] = c->arena.alloc<uint8_t>(nb_boxes + nb_probs + nb_labels + nb_valid + nb_feat, false);
+      B2_CHECK(c->stage_in[i] && c->stage_out[i], "out of device memory (submit staging buffers)");
       B2_CUDA(cudaEventCreateWithFlags(&c->h2d_done[i], cudaEventDisableTiming));
       B2_CUDA(cudaEventCreateWithFlags(&c->staged_free[i], cudaEventDisableTiming));
       B2_CUDA(cudaEventCreateWithFlags(&c->out_done[i], cudaEventDisableTiming));
@@ -1486,10 +1210,10 @@ int b2_box_features(b2_ctx* c, const void* frame_host, const float* boxes_host, 
   B2_CHECK(c->weights_loaded, "b2_box_features: weights not loaded");
   const int R = c->cfg.result_per_im, C = c->cfg.fpn_num_channel;
   if (!c->given_boxes) {
-    c->given_boxes = c->alloc<float>(static_cast<size_t>(R) * 4);
-    c->given_count = c->alloc<int>(1);
-    c->given_feat = c->alloc<float>(static_cast<size_t>(R) * C * 49);
-    c->given_pooled = c->alloc<float>(static_cast<size_t>(R) * C);
+    c->given_boxes = c->arena.alloc<float>(static_cast<size_t>(R) * 4);
+    c->given_count = c->arena.alloc<int>(1);
+    c->given_feat = c->arena.alloc<float>(static_cast<size_t>(R) * C * 49);
+    c->given_pooled = c->arena.alloc<float>(static_cast<size_t>(R) * C);
     B2_CHECK(c->given_boxes && c->given_count && c->given_feat && c->given_pooled, "out of device memory (given-box buffers)");
     B2_CUDA(cudaDeviceSynchronize());   // the zero fills of alloc() run on the legacy stream
   }
@@ -1530,33 +1254,20 @@ int b2_get_masks(b2_ctx* c, float* masks_host, int64_t capacity_bytes) {
 
 int b2_stage_shape(b2_ctx* c, const char* name, int64_t shape[4], int32_t* dtype) {
   B2_CHECK(c && name && shape, "b2_stage_shape: null argument");
-  auto it = c->stages.find(name);
-  B2_CHECK(it != c->stages.end(), std::string("unknown stage: ") + name);
-  for (int i = 0; i < 4; ++i) shape[i] = it->second.shape[i];
-  if (dtype) *dtype = it->second.kind == 2 ? 1 : 0;
+  const Stage* s = c->stages.find(name);
+  if (!s) return -1;
+  for (int i = 0; i < 4; ++i) shape[i] = s->shape[i];
+  if (dtype) *dtype = s->kind == Stage::kI32 ? 1 : 0;
   return 0;
 }
 
 int b2_get_stage(b2_ctx* c, const char* name, void* dst, int64_t capacity) {
   B2_CHECK(c && name && dst, "b2_get_stage: null argument");
   B2_CUDA(cudaSetDevice(c->device));
-  auto it = c->stages.find(name);
-  B2_CHECK(it != c->stages.end(), std::string("unknown stage: ") + name);
-  const StageRef& s = it->second;
-  const int64_t n = s.shape[0] * s.shape[1] * s.shape[2] * s.shape[3];
-  B2_CHECK(capacity >= n * 4, "b2_get_stage: buffer too small");
-  B2_CUDA(cudaStreamSynchronize(c->stream));
-  if (s.kind == 0) {
-    float* tmp = nullptr;
-    B2_CUDA(cudaMalloc(&tmp, n * 4));
-    if (planes_to_f32(s.pl.hi, s.pl.lo, tmp, n, c->stream)) return -1;
-    B2_CUDA(cudaMemcpyAsync(dst, tmp, n * 4, cudaMemcpyDeviceToHost, c->stream));
-    B2_CUDA(cudaStreamSynchronize(c->stream));
-    B2_CUDA(cudaFree(tmp));
-  } else {
-    B2_CUDA(cudaMemcpy(dst, s.ptr, n * 4, cudaMemcpyDeviceToHost));
-  }
-  return 0;
+  const Stage* s = c->stages.find(name);
+  if (!s) return -1;
+  B2_CHECK(capacity >= s->numel() * 4, "b2_get_stage: buffer too small");
+  return stage_read(*s, c->stream, dst);
 }
 
 int b2_set_stage(b2_ctx* c, const char* name, const void* src, int64_t bytes) {
@@ -1568,371 +1279,10 @@ int b2_set_stage(b2_ctx* c, const char* name, const void* src, int64_t bytes) {
     B2_CUDA(cudaStreamSynchronize(c->stream));
     return 0;
   }
-  auto it = c->stages.find(name);
-  B2_CHECK(it != c->stages.end(), std::string("unknown stage: ") + name);
-  const StageRef& s = it->second;
-  const int64_t n = s.shape[0] * s.shape[1] * s.shape[2] * s.shape[3];
-  B2_CHECK(bytes == n * 4, "b2_set_stage: size mismatch");
-  B2_CUDA(cudaStreamSynchronize(c->stream));
-  if (s.kind == 0) {
-    float* tmp = nullptr;
-    B2_CUDA(cudaMalloc(&tmp, n * 4));
-    B2_CUDA(cudaMemcpyAsync(tmp, src, n * 4, cudaMemcpyHostToDevice, c->stream));   // same stream as the kernel
-    if (f32_to_planes(tmp, s.pl.hi, s.pl.lo, n, c->stream)) return -1;
-    B2_CUDA(cudaStreamSynchronize(c->stream));
-    B2_CUDA(cudaFree(tmp));
-  } else {
-    B2_CUDA(cudaMemcpyAsync(s.ptr, src, n * 4, cudaMemcpyHostToDevice, c->stream));
-    B2_CUDA(cudaStreamSynchronize(c->stream));
-  }
-  return 0;
-}
-
-// ---- workspace for the small per-frame GEMM calls ------------------------------------------------------------------
-// b2_cosine_cost / b2_distance_matrix are called once per frame (per cascade level) by the trackers.  They run out of ONE
-// grow-only workspace per device with the GEMM plans cached per padded shape: a call is three uploads, four launches and
-// one download on a private stream (allocating device buffers and encoding the tensor maps on every call instead costs
-// more than the numpy computation it replaces).  Operands
-// are padded to the plan's shape with whatever the buffers hold (finite leftovers of earlier calls): padded rows / columns
-// only produce outputs nobody reads.  B2_NO_WS=1 (test hook) runs every call in a private workspace that is released
-// when the call returns -- same code, no reuse; tests compare the two bit for bit.
-struct DistWs {
-  int device = -1;
-  cudaStream_t stream = nullptr;
-  size_t cap_a = 0, cap_b = 0, cap_rows = 0, cap_cols = 0, cap_dp = 0;
-  float *d_a = nullptr, *d_b = nullptr, *d_dots = nullptr, *d_out = nullptr, *d_bias = nullptr, *d_na2 = nullptr, *d_nb2 = nullptr;
-  int* d_off = nullptr;
-  __half *a_hi = nullptr, *a_lo = nullptr, *b_hi = nullptr, *b_lo = nullptr;
-  std::map<std::vector<int>, ConvPlan*> plans;   // key: Sp, Np, Dp, split
-  int num_sms = 132;
-  bool transient = false;   // B2_NO_WS: owned by one call
-  DistWs() = default;
-  DistWs(const DistWs&) = delete;
-  DistWs& operator=(const DistWs&) = delete;
-  void release() {
-    for (auto& kv : plans) conv_tc_plan_destroy(kv.second);
-    plans.clear();
-    void* ptrs[] = {d_a, d_b, d_dots, d_out, d_bias, d_na2, d_nb2, d_off, a_hi, a_lo, b_hi, b_lo};
-    for (void* q : ptrs) if (q) cudaFree(q);
-    d_a = d_b = d_dots = d_out = d_bias = d_na2 = d_nb2 = nullptr;
-    d_off = nullptr;
-    a_hi = a_lo = b_hi = b_lo = nullptr;
-    cap_a = cap_b = cap_rows = cap_cols = cap_dp = 0;
-  }
-  ~DistWs() {
-    if (!transient) return;   // the per-device workspaces live as long as the process (no CUDA calls at exit)
-    release();
-    if (stream) cudaStreamDestroy(stream);
-  }
-};
-static std::map<int, DistWs> g_dist_ws;
-static std::map<int, int> g_num_sms;
-static std::mutex g_dist_ws_mutex;   // one call at a time per process (the trackers are single-threaded per stream)
-
-// Makes `w` (on `device`) hold S x D / N x D raw rows, Sp x Dp / Np x Dp operand planes, Sp x Np products, `aux` ints.
-static int dist_ws_reserve(DistWs& w, int device, int S, int N, int D, int Sp, int Np, int Dp, int aux) {
-  if (w.device < 0) {
-    w.device = device;
-    auto it = g_num_sms.find(device);
-    if (it == g_num_sms.end()) {
-      int n = 0;
-      B2_CUDA(cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, device));
-      it = g_num_sms.emplace(device, n).first;
-    }
-    w.num_sms = it->second;
-    B2_CUDA(cudaStreamCreateWithFlags(&w.stream, cudaStreamNonBlocking));
-  }
-  const size_t need_a = static_cast<size_t>(S) * D, need_b = static_cast<size_t>(N) * D;
-  if (need_a > w.cap_a || need_b > w.cap_b || static_cast<size_t>(Sp) > w.cap_rows || static_cast<size_t>(Np) > w.cap_cols ||
-      static_cast<size_t>(Dp) > w.cap_dp || static_cast<size_t>(aux) > w.cap_rows + w.cap_cols) {
-    B2_CUDA(cudaStreamSynchronize(w.stream));
-    const size_t o_a = w.cap_a, o_b = w.cap_b, o_r = w.cap_rows, o_c = w.cap_cols, o_d = w.cap_dp;
-    w.release();                                          // the plans hold the old addresses
-    const size_t head = w.transient ? 1 : 2;              // only the dimension that overflowed grows (x2 head room)
-    auto grow = [head](size_t cap, size_t need, size_t floor_) {
-      return need > cap ? std::max(need * head, floor_) : std::max(cap, floor_);
-    };
-    w.cap_a = grow(o_a, need_a, 1);
-    w.cap_b = grow(o_b, need_b, 1);
-    w.cap_rows = grow(o_r, static_cast<size_t>(Sp), w.transient ? 128 : 256);
-    w.cap_cols = grow(o_c, static_cast<size_t>(Np), w.transient ? 16 : 256);
-    if (static_cast<size_t>(aux) > w.cap_rows + w.cap_cols) w.cap_rows = static_cast<size_t>(aux);
-    w.cap_dp = std::max(o_d, static_cast<size_t>(Dp));
-    B2_CUDA(cudaMalloc(&w.d_a, w.cap_a * 4));
-    B2_CUDA(cudaMalloc(&w.d_b, w.cap_b * 4));
-    B2_CUDA(cudaMalloc(&w.d_dots, w.cap_rows * w.cap_cols * 4));
-    B2_CUDA(cudaMalloc(&w.d_out, w.cap_rows * w.cap_cols * 4));
-    B2_CUDA(cudaMalloc(&w.d_bias, w.cap_cols * 4));
-    B2_CUDA(cudaMalloc(&w.d_na2, w.cap_rows * 4));
-    B2_CUDA(cudaMalloc(&w.d_nb2, w.cap_cols * 4));
-    B2_CUDA(cudaMalloc(&w.d_off, (w.cap_rows + w.cap_cols + 1) * 4));
-    B2_CUDA(cudaMalloc(&w.a_hi, w.cap_rows * w.cap_dp * 2));
-    B2_CUDA(cudaMalloc(&w.a_lo, w.cap_rows * w.cap_dp * 2));
-    B2_CUDA(cudaMalloc(&w.b_hi, w.cap_cols * w.cap_dp * 2));
-    B2_CUDA(cudaMalloc(&w.b_lo, w.cap_cols * w.cap_dp * 2));
-    B2_CUDA(cudaMemsetAsync(w.d_bias, 0, w.cap_cols * 4, w.stream));
-    B2_CUDA(cudaMemsetAsync(w.a_hi, 0, w.cap_rows * w.cap_dp * 2, w.stream));
-    B2_CUDA(cudaMemsetAsync(w.a_lo, 0, w.cap_rows * w.cap_dp * 2, w.stream));
-    B2_CUDA(cudaMemsetAsync(w.b_hi, 0, w.cap_cols * w.cap_dp * 2, w.stream));
-    B2_CUDA(cudaMemsetAsync(w.b_lo, 0, w.cap_cols * w.cap_dp * 2, w.stream));
-    B2_CUDA(cudaStreamSynchronize(w.stream));
-  }
-  return 0;
-}
-
-// the [Sp rows] x [Np columns] GEMM over K = Dp on the workspace operand planes (row stride Dp)
-static int dist_ws_gemm(DistWs& w, int Sp, int Np, int Dp, bool split) {
-  const std::vector<int> key = {Sp, Np, Dp, split ? 1 : 0};
-  auto it = w.plans.find(key);
-  if (it == w.plans.end()) {
-    ConvDesc d;
-    d.B = 1; d.in_H = 1; d.in_W = Sp; d.Cin = Dp; d.in_pitch_H = 1; d.in_pitch_W = Sp; d.in_ld = Dp;
-    d.Cout = Np; d.out_H = 1; d.out_W = Sp; d.ldc = Np;
-    ConvWeights cw;
-    cw.w_hi = w.b_hi; cw.w_lo = split ? w.b_lo : nullptr; cw.bias = w.d_bias; cw.Cout_pad = Np; cw.K = Dp;
-    ConvIO io;
-    io.in_hi = w.a_hi; io.in_lo = split ? w.a_lo : nullptr; io.out_f32 = w.d_dots;
-    ConvPlan* plan = conv_tc_plan_create(d, cw, io, split, w.num_sms);
-    B2_CHECK(plan != nullptr, std::string("distance workspace plan: ") + last_error());
-    it = w.plans.emplace(key, plan).first;
-  }
-  return conv_tc_launch(it->second, w.stream);
-}
-
-static int cosine_cost_run(DistWs& w, int device, const float* gallery, const int32_t* seg_offsets, int T, const float* dets,
-                           int N, int D, bool split, float* cost) {
-  const int S = seg_offsets[T];
-  const int Dp = (D + 63) / 64 * 64, Np = (N + 15) / 16 * 16, Sp = (S + 127) / 128 * 128;
-  if (dist_ws_reserve(w, device, S, N, D, Sp, Np, Dp, T + 1)) return -1;
-  cudaStream_t st = w.stream;
-  B2_CUDA(cudaMemcpyAsync(w.d_a, gallery, sizeof(float) * S * D, cudaMemcpyHostToDevice, st));
-  B2_CUDA(cudaMemcpyAsync(w.d_b, dets, sizeof(float) * N * D, cudaMemcpyHostToDevice, st));
-  B2_CUDA(cudaMemcpyAsync(w.d_off, seg_offsets, sizeof(int) * (T + 1), cudaMemcpyHostToDevice, st));
-  if (cosine_normalize_rows(w.d_a, S, D, w.a_hi, w.a_lo, Dp, st) || cosine_normalize_rows(w.d_b, N, D, w.b_hi, w.b_lo, Dp, st))
-    return -1;
-  if (dist_ws_gemm(w, Sp, Np, Dp, split)) return -1;
-  if (cosine_segmin(w.d_dots, Np, w.d_off, T, N, w.d_out, st)) return -1;
-  B2_CUDA(cudaMemcpyAsync(cost, w.d_out, sizeof(float) * T * N, cudaMemcpyDeviceToHost, st));
-  B2_CUDA(cudaStreamSynchronize(st));
-  return 0;
-}
-
-static int distance_matrix_run(DistWs& w, int device, const float* a, int na, const float* b, int nb, int D, int metric,
-                               bool split, float* out) {
-  const int Dp = (D + 63) / 64 * 64, Np = (nb + 15) / 16 * 16, Sp = (na + 127) / 128 * 128;
-  if (dist_ws_reserve(w, device, na, nb, D, Sp, Np, Dp, 0)) return -1;
-  cudaStream_t st = w.stream;
-  B2_CUDA(cudaMemcpyAsync(w.d_a, a, sizeof(float) * na * D, cudaMemcpyHostToDevice, st));
-  B2_CUDA(cudaMemcpyAsync(w.d_b, b, sizeof(float) * nb * D, cudaMemcpyHostToDevice, st));
-  if (metric == 0) {
-    if (cosine_normalize_rows(w.d_a, na, D, w.a_hi, w.a_lo, Dp, st) || cosine_normalize_rows(w.d_b, nb, D, w.b_hi, w.b_lo, Dp, st))
-      return -1;
-  } else {
-    if (rows_to_planes(w.d_a, na, D, w.a_hi, w.a_lo, Dp, w.d_na2, st) || rows_to_planes(w.d_b, nb, D, w.b_hi, w.b_lo, Dp, w.d_nb2, st))
-      return -1;
-  }
-  if (dist_ws_gemm(w, Sp, Np, Dp, split)) return -1;
-  if (distance_finish(w.d_dots, Np, na, nb, metric, w.d_na2, w.d_nb2, w.d_out, st)) return -1;
-  B2_CUDA(cudaMemcpyAsync(out, w.d_out, sizeof(float) * na * nb, cudaMemcpyDeviceToHost, st));
-  B2_CUDA(cudaStreamSynchronize(st));
-  return 0;
-}
-
-// ---- DeepSORT appearance cost ---------------------------------------------------------------
-int b2_cosine_cost(int device, const float* gallery, const int32_t* seg_offsets, int T, const float* dets, int N,
-                   int D, int precision, float* cost) {
-  B2_CHECK(gallery && seg_offsets && dets && cost, "b2_cosine_cost: null argument");
-  if (T <= 0 || N <= 0) return 0;
-  B2_CHECK(D > 0 && seg_offsets[0] == 0, "b2_cosine_cost: seg_offsets must start at 0");
-  for (int t = 0; t < T; ++t)
-    B2_CHECK(seg_offsets[t + 1] >= seg_offsets[t], "b2_cosine_cost: seg_offsets must be non-decreasing");
-  B2_CHECK(seg_offsets[T] > 0, "b2_cosine_cost: empty gallery");
-  B2_CUDA(cudaSetDevice(device));
-  const bool split = precision == 1;
-  std::lock_guard<std::mutex> lock(g_dist_ws_mutex);
-  if (getenv("B2_NO_WS") != nullptr) {
-    DistWs w;
-    w.transient = true;
-    return cosine_cost_run(w, device, gallery, seg_offsets, T, dets, N, D, split, cost);
-  }
-  return cosine_cost_run(g_dist_ws[device], device, gallery, seg_offsets, T, dets, N, D, split, cost);
-}
-
-// ---- distance matrix (torchreid/distance.py:6-80) ------------------------------------------------
-int b2_distance_matrix(int device, const float* a, int na, const float* b, int nb, int D, int metric, int precision,
-                       float* out) {
-  B2_CHECK(a && b && out, "b2_distance_matrix: null argument");
-  B2_CHECK(metric == 0 || metric == 1, "b2_distance_matrix: metric must be 0 (cosine) or 1 (squared euclidean)");
-  if (na <= 0 || nb <= 0) return 0;
-  B2_CHECK(D > 0, "b2_distance_matrix: D must be positive");
-  B2_CUDA(cudaSetDevice(device));
-  const bool split = precision == 1;
-  std::lock_guard<std::mutex> lock(g_dist_ws_mutex);
-  if (getenv("B2_NO_WS") != nullptr) {
-    DistWs w;
-    w.transient = true;
-    return distance_matrix_run(w, device, a, na, b, nb, D, metric, split, out);
-  }
-  return distance_matrix_run(g_dist_ws[device], device, a, na, b, nb, D, metric, split, out);
-}
-
-// ---- single conv op for kernel parity tests ---------------------------------------------------
-
-int b2_op_conv2d(int device, const float* x, const float* w, const float* bias, const float* res, int B, int H, int W,
-                 int Cin, int R, int S, int Cout, int stride, int dil, int pad_t, int pad_b, int pad_l, int pad_r,
-                 int relu, int res_shift, int impl, int split, int a_mode, float* out) {
-  B2_CHECK(x && w && out, "b2_op_conv2d: null argument");
-  B2_CUDA(cudaSetDevice(device));
-  ConvDesc d;
-  d.B = B; d.in_H = H; d.in_W = W; d.Cin = Cin; d.in_pitch_H = H; d.in_pitch_W = W; d.in_ld = Cin;
-  d.R = R; d.S = S; d.stride = stride; d.dil = dil;
-  d.pad_t = pad_t; d.pad_b = pad_b; d.pad_l = pad_l; d.pad_r = pad_r;
-  d.Cout = Cout; d.relu = relu; d.force_a_mode = a_mode;
-  const int Ho = d.Ho(), Wo = d.Wo();
-  B2_CHECK(Ho > 0 && Wo > 0, "b2_op_conv2d: empty output");
-  const int Cp = (Cout + 15) / 16 * 16;
-  d.out_H = Ho; d.out_W = Wo; d.ldc = Cp;
-  const int rH = res_shift ? (Ho + 1) / 2 : Ho, rW = res_shift ? (Wo + 1) / 2 : Wo;
-  d.res_H = rH; d.res_W = rW; d.ldr = Cp; d.res_shift = res_shift;
-  const size_t nx = static_cast<size_t>(B) * H * W * Cin, K = static_cast<size_t>(R) * S * Cin;
-  const size_t nw = static_cast<size_t>(Cp) * K, no = static_cast<size_t>(B) * Ho * Wo * Cp;
-  const size_t nr = static_cast<size_t>(B) * rH * rW * Cp;
-  // pack HWIO -> [Cout_pad][R*S*Cin]
-  std::vector<float> pw(nw, 0.f), pb(Cp, 0.f);
-  for (size_t k = 0; k < K; ++k)
-    for (int o = 0; o < Cout; ++o) pw[static_cast<size_t>(o) * K + k] = w[k * Cout + o];
-  if (bias) for (int o = 0; o < Cout; ++o) pb[o] = bias[o];
-  std::vector<float> pr;
-  if (res) {
-    pr.assign(nr, 0.f);
-    for (size_t p = 0; p < static_cast<size_t>(B) * rH * rW; ++p)
-      for (int o = 0; o < Cout; ++o) pr[p * Cp + o] = res[p * Cout + o];
-  }
-  float *dx = nullptr, *dw = nullptr, *dr = nullptr, *dof = nullptr;
-  ConvWeights cw; ConvIO io;
-  __half *xh, *xl, *oh, *ol, *rh = nullptr, *rl = nullptr;
-  B2_CUDA(cudaMalloc(&dx, nx * 4));
-  B2_CUDA(cudaMalloc(&dw, nw * 4));
-  B2_CUDA(cudaMalloc(&dof, no * 4));
-  B2_CUDA(cudaMalloc(&xh, nx * 2 + 256)); B2_CUDA(cudaMalloc(&xl, nx * 2 + 256));
-  B2_CUDA(cudaMalloc(&cw.w_hi, nw * 2 + 256)); B2_CUDA(cudaMalloc(&cw.w_lo, nw * 2 + 256));
-  B2_CUDA(cudaMalloc(&oh, no * 2 + 256)); B2_CUDA(cudaMalloc(&ol, no * 2 + 256));
-  B2_CUDA(cudaMalloc(&cw.bias, Cp * 4));
-  B2_CUDA(cudaMemset(oh, 0, no * 2)); B2_CUDA(cudaMemset(ol, 0, no * 2));
-  B2_CUDA(cudaMemcpy(dx, x, nx * 4, cudaMemcpyHostToDevice));
-  B2_CUDA(cudaMemcpy(dw, pw.data(), nw * 4, cudaMemcpyHostToDevice));
-  B2_CUDA(cudaMemcpy(cw.bias, pb.data(), Cp * 4, cudaMemcpyHostToDevice));
-  cudaStream_t st = nullptr;
-  if (f32_to_planes(dx, xh, xl, nx, st) || f32_to_planes(dw, cw.w_hi, cw.w_lo, nw, st)) return -1;
-  if (res) {
-    B2_CUDA(cudaMalloc(&dr, nr * 4));
-    B2_CUDA(cudaMalloc(&rh, nr * 2 + 256)); B2_CUDA(cudaMalloc(&rl, nr * 2 + 256));
-    B2_CUDA(cudaMemcpy(dr, pr.data(), nr * 4, cudaMemcpyHostToDevice));
-    if (f32_to_planes(dr, rh, rl, nr, st)) return -1;
-  }
-  cw.Cout_pad = Cp; cw.K = static_cast<int>(K);
-  if (!split) { /* keep lo planes allocated but unused */ }
-  io.in_hi = xh; io.in_lo = split ? xl : nullptr;
-  io.out_hi = oh; io.out_lo = split ? ol : nullptr;
-  io.res_hi = rh; io.res_lo = split ? rl : nullptr;
-  ConvWeights cw_use = cw;
-  if (!split) cw_use.w_lo = nullptr;
-  int rc = 0;
-  if (impl == 0) {
-    cudaDeviceProp prop;
-    B2_CUDA(cudaGetDeviceProperties(&prop, device));
-    ConvPlan* plan = conv_tc_plan_create(d, cw_use, io, split != 0, prop.multiProcessorCount);
-    B2_CHECK(plan != nullptr, std::string("b2_op_conv2d: ") + last_error());
-    rc = conv_tc_launch(plan, st);
-    cudaError_t e = cudaDeviceSynchronize();
-    conv_tc_plan_destroy(plan);
-    if (!rc) B2_CUDA(e);
-  } else {
-    rc = conv_simt_launch(d, cw_use, io, split != 0, st);
-    if (!rc) B2_CUDA(cudaDeviceSynchronize());
-  }
-  if (rc) return -1;
-  if (planes_to_f32(oh, split ? ol : nullptr, dof, no, st)) return -1;
-  std::vector<float> ho(no);
-  B2_CUDA(cudaMemcpy(ho.data(), dof, no * 4, cudaMemcpyDeviceToHost));
-  for (size_t p = 0; p < static_cast<size_t>(B) * Ho * Wo; ++p)
-    for (int o = 0; o < Cout; ++o) out[p * Cout + o] = ho[p * Cp + o];
-  cudaFree(dx); cudaFree(dw); cudaFree(dof); cudaFree(xh); cudaFree(xl); cudaFree(cw.w_hi); cudaFree(cw.w_lo);
-  cudaFree(oh); cudaFree(ol); cudaFree(cw.bias);
-  if (res) { cudaFree(dr); cudaFree(rh); cudaFree(rl); }
-  return 0;
-}
-
-// ---- single GroupNorm op for kernel parity tests ------------------------------------------------
-
-int b2_op_group_norm(int device, const float* x, const float* res, const float* gamma, const float* beta, int B,
-                     int pitch_H, int pitch_W, int C, int H, int W, int off_h, int off_w, int res_H, int res_W, int res_shift,
-                     int relu, int per_roi, int split, int in_place, float* out) {
-  B2_CHECK(x && gamma && beta && out, "b2_op_group_norm: null argument");
-  B2_CHECK(B >= 1 && H >= 1 && W >= 1 && off_h >= 0 && off_w >= 0 && off_h + H <= pitch_H && off_w + W <= pitch_W,
-           "b2_op_group_norm: view outside the buffer");
-  B2_CHECK(!res || (res_shift >= 0 && ((H - 1) >> res_shift) < res_H && ((W - 1) >> res_shift) < res_W),
-           "b2_op_group_norm: residual smaller than the view");
-  B2_CUDA(cudaSetDevice(device));
-  const size_t n = static_cast<size_t>(B) * pitch_H * pitch_W * C, nr = res ? static_cast<size_t>(B) * res_H * res_W * C : 0;
-  std::vector<void*> bufs;
-  auto dalloc = [&](size_t bytes) -> void* {
-    void* p = nullptr;
-    if (cudaMalloc(&p, bytes + 256) != cudaSuccess) return nullptr;
-    cudaMemset(p, 0, bytes + 256);
-    bufs.push_back(p);
-    return p;
-  };
-  auto release = [&]() { for (void* p : bufs) cudaFree(p); };
-  float* f32 = static_cast<float*>(dalloc(std::max(n, nr) * 4));
-  __half* xh = static_cast<__half*>(dalloc(n * 2));
-  __half* xl = split ? static_cast<__half*>(dalloc(n * 2)) : nullptr;
-  __half* yh = in_place ? xh : static_cast<__half*>(dalloc(n * 2));
-  __half* yl = in_place ? xl : (split ? static_cast<__half*>(dalloc(n * 2)) : nullptr);
-  __half* rh = res ? static_cast<__half*>(dalloc(nr * 2)) : nullptr;
-  __half* rl = res && split ? static_cast<__half*>(dalloc(nr * 2)) : nullptr;
-  float* dg = static_cast<float*>(dalloc(C * 4));
-  float* db = static_cast<float*>(dalloc(C * 4));
-  GnParams p;
-  memset(&p, 0, sizeof(p));
-  p.chunks = gn_chunks(H, W, C);
-  p.partial = static_cast<float*>(dalloc(static_cast<size_t>(B) * p.chunks * 32 * 3 * 4));
-  p.stats = static_cast<float*>(dalloc(static_cast<size_t>(B) * 32 * 2 * 4));
-  p.counter = static_cast<unsigned int*>(dalloc(static_cast<size_t>(B) * 4));
-  for (void* q : bufs)
-    if (!q) { release(); B2_CHECK(false, "b2_op_group_norm: out of device memory"); }
-  int rc = 0;
-  cudaError_t e = cudaMemcpy(f32, x, n * 4, cudaMemcpyHostToDevice);
-  if (e == cudaSuccess) rc = f32_to_planes(f32, xh, xl, n, nullptr);
-  if (e == cudaSuccess && !rc && res) {
-    e = cudaMemcpy(f32, res, nr * 4, cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) rc = f32_to_planes(f32, rh, rl, nr, nullptr);
-  }
-  if (e == cudaSuccess) e = cudaMemcpy(dg, gamma, C * 4, cudaMemcpyHostToDevice);
-  if (e == cudaSuccess) e = cudaMemcpy(db, beta, C * 4, cudaMemcpyHostToDevice);
-  p.x_hi = xh; p.x_lo = xl; p.y_hi = yh; p.y_lo = yl;
-  p.B = B; p.H = H; p.W = W; p.C = C;
-  p.pitch_H = pitch_H; p.pitch_W = pitch_W; p.ld = C; p.off_h = off_h; p.off_w = off_w;
-  if (res) {
-    p.r_hi = rh; p.r_lo = rl; p.res_H = res_H; p.res_W = res_W; p.res_ld = C; p.res_shift = res_shift;
-  }
-  p.relu = relu;
-  p.gamma = dg; p.beta = db;
-  if (e == cudaSuccess && !rc) {
-    if (per_roi) {
-      rc = gn_roi_launch(p, nullptr);
-    } else {
-      rc = gn_stats_launch(p, nullptr);
-      if (!rc) rc = gn_apply_launch(p, nullptr);
-    }
-  }
-  if (e == cudaSuccess && !rc) e = cudaDeviceSynchronize();
-  if (e == cudaSuccess && !rc) rc = planes_to_f32(yh, yl, f32, n, nullptr);
-  if (e == cudaSuccess && !rc) e = cudaMemcpy(out, f32, n * 4, cudaMemcpyDeviceToHost);
-  release();
-  if (rc) return -1;
-  B2_CUDA(e);
-  return 0;
+  const Stage* s = c->stages.find(name);
+  if (!s) return -1;
+  B2_CHECK(bytes == s->numel() * 4, "b2_set_stage: size mismatch");
+  return stage_write(*s, c->stream, src);
 }
 
 }  // extern "C"

@@ -1,0 +1,145 @@
+// Single-kernel entry points for parity tests and host tools: one conv, one GroupNorm, the frame resize.  Each call owns
+// its device buffers in an Arena, so every return path frees them.
+#include <string.h>
+
+#include <algorithm>
+#include <vector>
+
+#include "../../include/b200det.h"
+#include "engine_core.h"
+#include "kernels.h"
+
+using namespace b2;
+
+extern "C" {
+
+int b2_op_conv2d(int device, const float* x, const float* w, const float* bias, const float* res, int B, int H, int W,
+                 int Cin, int R, int S, int Cout, int stride, int dil, int pad_t, int pad_b, int pad_l, int pad_r,
+                 int relu, int res_shift, int impl, int split, int a_mode, float* out) {
+  B2_CHECK(x && w && out, "b2_op_conv2d: null argument");
+  B2_CUDA(cudaSetDevice(device));
+  ConvDesc d;
+  d.B = B; d.in_H = H; d.in_W = W; d.Cin = Cin; d.in_pitch_H = H; d.in_pitch_W = W; d.in_ld = Cin;
+  d.R = R; d.S = S; d.stride = stride; d.dil = dil;
+  d.pad_t = pad_t; d.pad_b = pad_b; d.pad_l = pad_l; d.pad_r = pad_r;
+  d.Cout = Cout; d.relu = relu; d.force_a_mode = a_mode;
+  const int Ho = d.Ho(), Wo = d.Wo();
+  B2_CHECK(Ho > 0 && Wo > 0, "b2_op_conv2d: empty output");
+  const int Cp = (Cout + 15) / 16 * 16;
+  d.out_H = Ho; d.out_W = Wo; d.ldc = Cp;
+  const int rH = res_shift ? (Ho + 1) / 2 : Ho, rW = res_shift ? (Wo + 1) / 2 : Wo;
+  d.res_H = rH; d.res_W = rW; d.ldr = Cp; d.res_shift = res_shift;
+  const size_t nx = static_cast<size_t>(B) * H * W * Cin, K = static_cast<size_t>(R) * S * Cin;
+  const size_t nw = static_cast<size_t>(Cp) * K, no = static_cast<size_t>(B) * Ho * Wo * Cp;
+  const size_t nr = static_cast<size_t>(B) * rH * rW * Cp;
+  // pack HWIO -> [Cout_pad][R*S*Cin]
+  std::vector<float> pw(nw, 0.f), pb(Cp, 0.f);
+  for (size_t k = 0; k < K; ++k)
+    for (int o = 0; o < Cout; ++o) pw[static_cast<size_t>(o) * K + k] = w[k * Cout + o];
+  if (bias) for (int o = 0; o < Cout; ++o) pb[o] = bias[o];
+  std::vector<float> pr;
+  if (res) {
+    pr.assign(nr, 0.f);
+    for (size_t p = 0; p < static_cast<size_t>(B) * rH * rW; ++p)
+      for (int o = 0; o < Cout; ++o) pr[p * Cp + o] = res[p * Cout + o];
+  }
+  // every operand is converted to both planes; fp16 precision leaves the lo planes unused
+  Arena a;
+  __half *xh = a.alloc<__half>(nx), *xl = a.alloc<__half>(nx), *oh = a.alloc<__half>(no), *ol = a.alloc<__half>(no);
+  __half *rh = res ? a.alloc<__half>(nr) : nullptr, *rl = res ? a.alloc<__half>(nr) : nullptr;
+  ConvWeights cw;
+  cw.w_hi = a.alloc<__half>(nw);
+  cw.w_lo = a.alloc<__half>(nw);
+  cw.bias = a.alloc<float>(Cp);
+  B2_CHECK(xh && xl && oh && ol && (!res || (rh && rl)) && cw.w_hi && cw.w_lo && cw.bias, "b2_op_conv2d: out of device memory");
+  cudaStream_t st = nullptr;
+  if (upload_planes(x, xh, xl, nx, st) || upload_planes(pw.data(), cw.w_hi, cw.w_lo, nw, st)) return -1;
+  if (res && upload_planes(pr.data(), rh, rl, nr, st)) return -1;
+  B2_CUDA(cudaMemcpy(cw.bias, pb.data(), Cp * 4, cudaMemcpyHostToDevice));
+  cw.Cout_pad = Cp; cw.K = static_cast<int>(K);
+  ConvIO io;
+  io.in_hi = xh; io.in_lo = split ? xl : nullptr;
+  io.out_hi = oh; io.out_lo = split ? ol : nullptr;
+  io.res_hi = rh; io.res_lo = split ? rl : nullptr;
+  if (!split) cw.w_lo = nullptr;
+  if (impl == 0) {
+    cudaDeviceProp prop;
+    B2_CUDA(cudaGetDeviceProperties(&prop, device));
+    PlanPtr plan(conv_tc_plan_create(d, cw, io, split != 0, prop.multiProcessorCount));
+    B2_CHECK(plan != nullptr, std::string("b2_op_conv2d: ") + last_error());
+    const int rc = conv_tc_launch(plan.get(), st);
+    const cudaError_t e = cudaDeviceSynchronize();   // the kernel is done before its plan goes away
+    if (rc) return -1;
+    B2_CUDA(e);
+  } else {
+    if (conv_simt_launch(d, cw, io, split != 0, st)) return -1;
+    B2_CUDA(cudaDeviceSynchronize());
+  }
+  std::vector<float> ho(no);
+  if (download_planes(oh, split ? ol : nullptr, no, ho.data(), st)) return -1;
+  for (size_t p = 0; p < static_cast<size_t>(B) * Ho * Wo; ++p)
+    for (int o = 0; o < Cout; ++o) out[p * Cout + o] = ho[p * Cp + o];
+  return 0;
+}
+
+int b2_op_group_norm(int device, const float* x, const float* res, const float* gamma, const float* beta, int B,
+                     int pitch_H, int pitch_W, int C, int H, int W, int off_h, int off_w, int res_H, int res_W, int res_shift,
+                     int relu, int per_roi, int split, int in_place, float* out) {
+  B2_CHECK(x && gamma && beta && out, "b2_op_group_norm: null argument");
+  B2_CHECK(B >= 1 && H >= 1 && W >= 1 && off_h >= 0 && off_w >= 0 && off_h + H <= pitch_H && off_w + W <= pitch_W,
+           "b2_op_group_norm: view outside the buffer");
+  B2_CHECK(!res || (res_shift >= 0 && ((H - 1) >> res_shift) < res_H && ((W - 1) >> res_shift) < res_W),
+           "b2_op_group_norm: residual smaller than the view");
+  B2_CUDA(cudaSetDevice(device));
+  const size_t n = static_cast<size_t>(B) * pitch_H * pitch_W * C, nr = res ? static_cast<size_t>(B) * res_H * res_W * C : 0;
+  Arena a;
+  const Planes xp = a.planes(B, pitch_H, pitch_W, C, split != 0);
+  const Planes yp = in_place ? xp : a.planes(B, pitch_H, pitch_W, C, split != 0);
+  const Planes rp = res ? a.planes(B, res_H, res_W, C, split != 0) : Planes();
+  GnParams p;
+  memset(&p, 0, sizeof(p));
+  p.chunks = gn_chunks(H, W, C);
+  p.gamma = a.alloc<float>(C);
+  p.beta = a.alloc<float>(C);
+  p.partial = a.alloc<float>(static_cast<size_t>(B) * p.chunks * 32 * 3);
+  p.stats = a.alloc<float>(static_cast<size_t>(B) * 32 * 2);
+  p.counter = a.alloc<unsigned int>(B);
+  B2_CHECK(xp.hi && yp.hi && (!res || rp.hi) && p.gamma && p.beta && p.partial && p.stats && p.counter,
+           "b2_op_group_norm: out of device memory");
+  if (upload_planes(x, xp.hi, xp.lo, n, nullptr)) return -1;
+  if (res && upload_planes(res, rp.hi, rp.lo, nr, nullptr)) return -1;
+  B2_CUDA(cudaMemcpy(const_cast<float*>(p.gamma), gamma, C * 4, cudaMemcpyHostToDevice));
+  B2_CUDA(cudaMemcpy(const_cast<float*>(p.beta), beta, C * 4, cudaMemcpyHostToDevice));
+  p.x_hi = xp.hi; p.x_lo = xp.lo; p.y_hi = yp.hi; p.y_lo = yp.lo;
+  p.B = B; p.H = H; p.W = W; p.C = C;
+  p.pitch_H = pitch_H; p.pitch_W = pitch_W; p.ld = C; p.off_h = off_h; p.off_w = off_w;
+  if (res) {
+    p.r_hi = rp.hi; p.r_lo = rp.lo; p.res_H = res_H; p.res_W = res_W; p.res_ld = C; p.res_shift = res_shift;
+  }
+  p.relu = relu;
+  if (per_roi) {
+    if (gn_roi_launch(p, nullptr)) return -1;
+  } else {
+    if (gn_stats_launch(p, nullptr) || gn_apply_launch(p, nullptr)) return -1;
+  }
+  B2_CUDA(cudaDeviceSynchronize());
+  return download_planes(yp.hi, yp.lo, n, out, nullptr);
+}
+
+// The resize alone (parity tests): host uint8 [n, src_h, src_w, 3] -> host float32 [n, dst_h, dst_w, 3].
+int b2_resize_frames(int device, const uint8_t* frames_u8, int n, int src_h, int src_w, int dst_h, int dst_w,
+                     float* out_host) {
+  B2_CHECK(frames_u8 && out_host && n > 0 && src_h > 0 && src_w > 0 && dst_h > 0 && dst_w > 0, "b2_resize_frames: bad argument");
+  B2_CUDA(cudaSetDevice(device));
+  const size_t nb_src = static_cast<size_t>(n) * src_h * src_w * 3, nb_dst = static_cast<size_t>(n) * dst_h * dst_w * 3 * sizeof(float);
+  Arena a;
+  uint8_t* d_src = a.alloc<uint8_t>(nb_src, false);
+  float* d_dst = a.alloc<float>(nb_dst / sizeof(float), false);
+  B2_CHECK(d_src && d_dst, "b2_resize_frames: out of device memory");
+  B2_CUDA(cudaMemcpy(d_src, frames_u8, nb_src, cudaMemcpyHostToDevice));
+  if (resize_u8_launch(d_src, n, src_h, src_w, d_dst, dst_h, dst_w, nullptr)) return -1;
+  B2_CUDA(cudaMemcpy(out_host, d_dst, nb_dst, cudaMemcpyDeviceToHost));
+  return 0;
+}
+
+}  // extern "C"

@@ -11,86 +11,20 @@
 
 #include <algorithm>
 #include <map>
+#include <mutex>
 #include <vector>
 
 #include "../../include/b200det.h"
-#include "common.h"
+#include "gemm_ws.h"
 #include "kernels.h"
-
-#include <mutex>
 
 namespace b2 {
 namespace {
 
-// Grow-only workspace per device (the pair costs of config 5 are computed pair after pair with similar shapes): operand
-// planes, products, norms, segment tables, gate and the GEMM plans cached per padded shape.  Round 1 allocated 13 buffers,
-// queried the device properties and encoded the tensor maps on every call (13.7 ms per camera pair on an 8-GPU box, of
-// which the GEMM + segmented min are well under a millisecond).
-struct PairWs {
-  int num_sms = 0;
-  cudaStream_t stream = nullptr;
-  size_t cap_a = 0, cap_b = 0, cap_sp = 0, cap_np = 0, cap_dp = 0, cap_seg = 0, cap_nm = 0;
-  float *d_a = nullptr, *d_b = nullptr, *d_dots = nullptr, *d_out = nullptr, *d_bias = nullptr, *d_na2 = nullptr, *d_nb2 = nullptr;
-  int *d_sa = nullptr, *d_sb = nullptr;
-  unsigned char* d_gate = nullptr;
-  __half *a_hi = nullptr, *a_lo = nullptr, *b_hi = nullptr, *b_lo = nullptr;
-  std::map<std::vector<int>, ConvPlan*> plans;
-  void release() {
-    for (auto& kv : plans) conv_tc_plan_destroy(kv.second);
-    plans.clear();
-    void* ptrs[] = {d_a, d_b, d_dots, d_out, d_bias, d_na2, d_nb2, d_sa, d_sb, d_gate, a_hi, a_lo, b_hi, b_lo};
-    for (void* q : ptrs) if (q) cudaFree(q);
-    d_a = d_b = d_dots = d_out = d_bias = d_na2 = d_nb2 = nullptr;
-    d_sa = d_sb = nullptr;
-    d_gate = nullptr;
-    a_hi = a_lo = b_hi = b_lo = nullptr;
-  }
-};
-std::map<int, PairWs> g_pair_ws;
+// One workspace per device (the pair costs of config 5 are computed pair after pair with similar shapes), apart from the
+// trackers' so that the two kinds of callers do not wait on each other.
+std::map<int, GemmWs> g_pair_ws;
 std::mutex g_pair_mutex;
-
-int pair_ws_reserve(PairWs& w, int device, size_t need_a, size_t need_b, int Sp, int Np, int Dp, int nseg, size_t nm) {
-  if (!w.stream) {
-    B2_CUDA(cudaDeviceGetAttribute(&w.num_sms, cudaDevAttrMultiProcessorCount, device));
-    B2_CUDA(cudaStreamCreateWithFlags(&w.stream, cudaStreamNonBlocking));
-  }
-  if (need_a <= w.cap_a && need_b <= w.cap_b && static_cast<size_t>(Sp) <= w.cap_sp && static_cast<size_t>(Np) <= w.cap_np &&
-      static_cast<size_t>(Dp) <= w.cap_dp && static_cast<size_t>(nseg) <= w.cap_seg && nm <= w.cap_nm)
-    return 0;
-  B2_CUDA(cudaStreamSynchronize(w.stream));
-  w.release();                                            // the plans hold the old addresses
-  auto grow = [](size_t cap, size_t need) { return need > cap ? need + need / 2 : cap; };
-  w.cap_a = grow(w.cap_a, std::max<size_t>(need_a, 1));
-  w.cap_b = grow(w.cap_b, std::max<size_t>(need_b, 1));
-  w.cap_sp = grow(w.cap_sp, static_cast<size_t>(Sp));
-  w.cap_np = grow(w.cap_np, static_cast<size_t>(Np));
-  w.cap_dp = std::max(w.cap_dp, static_cast<size_t>(Dp));
-  w.cap_seg = grow(w.cap_seg, static_cast<size_t>(nseg));
-  w.cap_nm = grow(w.cap_nm, std::max<size_t>(nm, 1));
-  B2_CUDA(cudaMalloc(&w.d_a, w.cap_a * 4));
-  B2_CUDA(cudaMalloc(&w.d_b, w.cap_b * 4));
-  B2_CUDA(cudaMalloc(&w.d_dots, w.cap_sp * w.cap_np * 4));
-  B2_CUDA(cudaMalloc(&w.d_out, w.cap_nm * 4));
-  B2_CUDA(cudaMalloc(&w.d_bias, w.cap_np * 4));
-  B2_CUDA(cudaMalloc(&w.d_na2, w.cap_sp * 4));
-  B2_CUDA(cudaMalloc(&w.d_nb2, w.cap_np * 4));
-  B2_CUDA(cudaMalloc(&w.d_sa, w.cap_seg * 4));
-  B2_CUDA(cudaMalloc(&w.d_sb, w.cap_seg * 4));
-  B2_CUDA(cudaMalloc(&w.d_gate, w.cap_nm));
-  B2_CUDA(cudaMalloc(&w.a_hi, w.cap_sp * w.cap_dp * 2));
-  B2_CUDA(cudaMalloc(&w.a_lo, w.cap_sp * w.cap_dp * 2));
-  B2_CUDA(cudaMalloc(&w.b_hi, w.cap_np * w.cap_dp * 2));
-  B2_CUDA(cudaMalloc(&w.b_lo, w.cap_np * w.cap_dp * 2));
-  B2_CUDA(cudaMemsetAsync(w.d_bias, 0, w.cap_np * 4, w.stream));
-  B2_CUDA(cudaMemsetAsync(w.d_na2, 0, w.cap_sp * 4, w.stream));
-  B2_CUDA(cudaMemsetAsync(w.d_nb2, 0, w.cap_np * 4, w.stream));
-  B2_CUDA(cudaMemsetAsync(w.a_hi, 0, w.cap_sp * w.cap_dp * 2, w.stream));
-  B2_CUDA(cudaMemsetAsync(w.a_lo, 0, w.cap_sp * w.cap_dp * 2, w.stream));
-  B2_CUDA(cudaMemsetAsync(w.b_hi, 0, w.cap_np * w.cap_dp * 2, w.stream));
-  B2_CUDA(cudaMemsetAsync(w.b_lo, 0, w.cap_np * w.cap_dp * 2, w.stream));
-  B2_CUDA(cudaStreamSynchronize(w.stream));
-  return 0;
-}
 
 }  // namespace
 }  // namespace b2
@@ -121,10 +55,15 @@ static int pair_cost_impl(int device, const float* a, bool a_dev, const int32_t*
   const bool split = precision == 1;
   const int Dp = (D + 63) / 64 * 64, Np = (Sb + 15) / 16 * 16, Sp = (Sa + 127) / 128 * 128;
   std::lock_guard<std::mutex> lock(g_pair_mutex);
-  PairWs& w = g_pair_ws[device];
-  if (pair_ws_reserve(w, device, a_dev ? 0 : static_cast<size_t>(Sa) * D, b_dev ? 0 : static_cast<size_t>(Sb) * D, Sp, Np, Dp,
-                      std::max(N, M) + 1, static_cast<size_t>(N) * M))
-    return -1;
+  GemmWs& w = g_pair_ws[device];
+  GemmNeed need;
+  need.a = a_dev ? 0 : static_cast<size_t>(Sa) * D;
+  need.b = b_dev ? 0 : static_cast<size_t>(Sb) * D;
+  need.Sp = Sp; need.Np = Np; need.Dp = Dp;
+  need.out = static_cast<size_t>(N) * M;
+  need.ints = static_cast<size_t>(N) + M + 2;
+  need.gate = static_cast<size_t>(N) * M;
+  if (w.reserve(device, need)) return -1;
   cudaStream_t st = w.stream;
   const float* d_a = a;
   const float* d_b = b;
@@ -136,27 +75,15 @@ static int pair_cost_impl(int device, const float* a, bool a_dev, const int32_t*
     B2_CUDA(cudaMemcpyAsync(w.d_b, b, sizeof(float) * Sb * D, cudaMemcpyHostToDevice, st));
     d_b = w.d_b;
   }
-  B2_CUDA(cudaMemcpyAsync(w.d_sa, seg_a, sizeof(int) * (N + 1), cudaMemcpyHostToDevice, st));
-  B2_CUDA(cudaMemcpyAsync(w.d_sb, seg_b, sizeof(int) * (M + 1), cudaMemcpyHostToDevice, st));
+  int* d_sa = w.d_int;
+  int* d_sb = w.d_int + N + 1;
+  B2_CUDA(cudaMemcpyAsync(d_sa, seg_a, sizeof(int) * (N + 1), cudaMemcpyHostToDevice, st));
+  B2_CUDA(cudaMemcpyAsync(d_sb, seg_b, sizeof(int) * (M + 1), cudaMemcpyHostToDevice, st));
   if (gate) B2_CUDA(cudaMemcpyAsync(w.d_gate, gate, static_cast<size_t>(N) * M, cudaMemcpyHostToDevice, st));
   if (rows_to_planes(d_a, Sa, D, w.a_hi, w.a_lo, Dp, w.d_na2, st) || rows_to_planes(d_b, Sb, D, w.b_hi, w.b_lo, Dp, w.d_nb2, st))
     return -1;
-  const std::vector<int> key = {Sp, Np, Dp, split ? 1 : 0};
-  auto it = w.plans.find(key);
-  if (it == w.plans.end()) {
-    ConvDesc d;
-    d.B = 1; d.in_H = 1; d.in_W = Sp; d.Cin = Dp; d.in_pitch_H = 1; d.in_pitch_W = Sp; d.in_ld = Dp;
-    d.Cout = Np; d.out_H = 1; d.out_W = Sp; d.ldc = Np;
-    ConvWeights cw;
-    cw.w_hi = w.b_hi; cw.w_lo = split ? w.b_lo : nullptr; cw.bias = w.d_bias; cw.Cout_pad = Np; cw.K = Dp;
-    ConvIO io;
-    io.in_hi = w.a_hi; io.in_lo = split ? w.a_lo : nullptr; io.out_f32 = w.d_dots;
-    ConvPlan* plan = conv_tc_plan_create(d, cw, io, split, w.num_sms);
-    B2_CHECK(plan != nullptr, std::string("b2_track_pair_cost: ") + last_error());
-    it = w.plans.emplace(key, plan).first;
-  }
-  if (conv_tc_launch(it->second, st)) return -1;
-  if (pair_segmin(w.d_dots, Np, w.d_na2, w.d_nb2, w.d_sa, N, w.d_sb, M, gate ? w.d_gate : nullptr, fill, w.d_out, st)) return -1;
+  if (w.gemm(Sp, Np, Dp, split)) return -1;
+  if (pair_segmin(w.d_dots, Np, w.d_na2, w.d_nb2, d_sa, N, d_sb, M, gate ? w.d_gate : nullptr, fill, w.d_out, st)) return -1;
   B2_CUDA(cudaMemcpyAsync(out, w.d_out, sizeof(float) * N * M, cudaMemcpyDeviceToHost, st));
   B2_CUDA(cudaStreamSynchronize(st));
   return 0;

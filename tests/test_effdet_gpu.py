@@ -331,3 +331,17 @@ def test_efficientdet_model_object_drop_in():
     np.testing.assert_array_equal(labels, ref["final_labels"])
     assert np.abs(boxes - ref["final_boxes"]).max() <= 1e-3
     assert np.abs(probs - ref["final_probs"]).max() <= 5e-6
+
+
+def test_weight_outside_fp16_range_is_refused():
+    """A folded weight beyond +-65504 has no fp16 operand-plane representation: loading it fails instead of computing
+    on inf."""
+    from object_detection_tracking_b200.effdet import EffdetEngine
+    from object_detection_tracking_b200.effdet_config import make_effdet_config
+    from object_detection_tracking_b200.synth import synth_effdet_weights
+    cfg = make_effdet_config("efficientdet-d0", 256, 384, fpn_cell_repeats=1, box_class_repeats=1)
+    W = dict(synth_effdet_weights(cfg))
+    k = sorted(n for n in W if n.endswith("pointwise_kernel"))[0]
+    W[k] = W[k] * np.float32(1e9)
+    with pytest.raises(RuntimeError, match="outside the fp16-plane range"):
+        EffdetEngine(cfg, W)
