@@ -30,9 +30,6 @@ const char* last_error();
     }                                                                                \
   } while (0)
 
-constexpr float kLoScale = 2048.0f;
-constexpr float kLoInv = 1.0f / 2048.0f;
-
 // Geometry + epilogue description of one implicit-GEMM convolution (also dense layers, as 1x1).
 struct ConvDesc {
   // input view (may be a crop of a larger buffer: in_H/in_W are the view, pitch_* the buffer)

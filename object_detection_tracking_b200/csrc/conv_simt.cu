@@ -2,6 +2,7 @@
 // accumulate) -- the on-device cross-check for the tensor-core kernel and the path for shapes the
 // tensor-core kernel does not take (Cin % 64 != 0).  One thread per (pixel, 4 output channels).
 #include "common.h"
+#include "planes.cuh"
 
 namespace b2 {
 namespace {
@@ -57,17 +58,12 @@ __global__ void conv_simt_kernel(ConvDesc d, ConvWeights w, ConvIO io, int Ho, i
       v += w.bias[n];
       if (io.res_hi) {
         v += __half2float(io.res_hi[rpix * d.ldr + n]);
-        if (SPLIT && io.res_lo) v = fmaf(__half2float(io.res_lo[rpix * d.ldr + n]), kLoInv, v);
+        if (SPLIT && io.res_lo) v = join(v, io.res_lo[rpix * d.ldr + n]);
       }
       if (d.relu == 1) v = fmaxf(v, 0.f);
       else if (d.relu == 2) v = __fmul_rn(v, 1.f / (1.f + expf(-v)));
-      if (io.out_f32) {
-        io.out_f32[opix * d.ldc + n] = v;
-      } else {
-        const __half h = __float2half_rn(v);
-        io.out_hi[opix * d.ldc + n] = h;
-        if (SPLIT && io.out_lo) io.out_lo[opix * d.ldc + n] = __float2half_rn((v - __half2float(h)) * kLoScale);
-      }
+      if (io.out_f32) io.out_f32[opix * d.ldc + n] = v;
+      else store1(io.out_hi, SPLIT ? io.out_lo : nullptr, opix * d.ldc + n, v);
     }
   }
 }
@@ -79,13 +75,11 @@ int conv_simt_launch(const ConvDesc& d, const ConvWeights& w, const ConvIO& io, 
   B2_CHECK(Ho > 0 && Wo > 0, "conv_simt: empty output");
   B2_CHECK(w.Cout_pad % 4 == 0 && d.ldc >= w.Cout_pad, "conv_simt: bad Cout_pad/ldc");
   const size_t total = static_cast<size_t>(d.B) * Ho * Wo * (w.Cout_pad / 4);
-  const int threads = 256;
-  size_t blocks = (total + threads - 1) / threads;
-  if (blocks > 132 * 64) blocks = 132 * 64;
+  const unsigned blocks = grid_for(total, 256, 132 * 64);
   if (split)
-    conv_simt_kernel<true><<<static_cast<unsigned>(blocks), threads, 0, stream>>>(d, w, io, Ho, Wo);
+    conv_simt_kernel<true><<<blocks, 256, 0, stream>>>(d, w, io, Ho, Wo);
   else
-    conv_simt_kernel<false><<<static_cast<unsigned>(blocks), threads, 0, stream>>>(d, w, io, Ho, Wo);
+    conv_simt_kernel<false><<<blocks, 256, 0, stream>>>(d, w, io, Ho, Wo);
   B2_CUDA(cudaGetLastError());
   return 0;
 }

@@ -35,6 +35,7 @@
 #include <vector>
 
 #include "common.h"
+#include "planes.cuh"
 #include "ptx.cuh"
 
 namespace b2 {
@@ -99,12 +100,10 @@ __device__ __forceinline__ void activate(int relu, float& v0, float& v1) {
 template <bool SPLIT>
 __device__ __forceinline__ void store_planes(float v0, float v1, __half2* hi_dst, __half2* lo_dst, float& amax) {
   amax = fmaxf(amax, fmaxf(fabsf(v0), fabsf(v1)));
-  const __half2 hi = __floats2half2_rn(v0, v1);
+  __half2 hi, lo;
+  split2(v0, v1, hi, lo);
   *hi_dst = hi;
-  if (SPLIT && lo_dst != nullptr) {
-    const float2 h = __half22float2(hi);
-    *lo_dst = __floats2half2_rn((v0 - h.x) * kLoScale, (v1 - h.y) * kLoScale);
-  }
+  if (SPLIT && lo_dst != nullptr) *lo_dst = lo;
 }
 
 // Two adjacent output channels (n, n + 1) of one pixel: bias, residual, activation, store (fp16 hi/lo planes or fp32)
@@ -120,9 +119,9 @@ __device__ __forceinline__ void epilogue_pair(const ConvTcParams& p, float v0, f
     v0 += r.x;
     v1 += r.y;
     if (SPLIT && p.res_lo != nullptr) {
-      const float2 l = __half22float2(__ldg(reinterpret_cast<const __half2*>(p.res_lo + rpix * p.ldr + n)));
-      v0 = fmaf(l.x, kLoInv, v0);
-      v1 = fmaf(l.y, kLoInv, v1);
+      const float2 s = join2(make_float2(v0, v1), __ldg(reinterpret_cast<const __half2*>(p.res_lo + rpix * p.ldr + n)));
+      v0 = s.x;
+      v1 = s.y;
     }
   }
   activate<SWISH>(p.relu, v0, v1);
@@ -147,9 +146,9 @@ __device__ __forceinline__ void epilogue_pair_slot(const ConvTcParams& p, float 
     v0 += r.x;
     v1 += r.y;
     if (SPLIT && p.res_lo != nullptr) {
-      const float2 l = __half22float2(*s_lo);
-      v0 = fmaf(l.x, kLoInv, v0);
-      v1 = fmaf(l.y, kLoInv, v1);
+      const float2 s = join2(make_float2(v0, v1), *s_lo);
+      v0 = s.x;
+      v1 = s.y;
     }
   }
   activate<SWISH>(p.relu, v0, v1);

@@ -6,6 +6,7 @@
 // _nn_cosine_distance (:78-96), NearestNeighborDistanceMetric.distance (:156-177).
 #include "common.h"
 #include "kernels.h"
+#include "planes.cuh"
 
 namespace b2 {
 namespace {
@@ -22,12 +23,8 @@ __global__ void cosine_normalize_kernel(const float* __restrict__ src, int rows,
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, o);
   const float nrm = sqrtf(ss);
-  for (int c = lane; c < ld; c += 32) {
-    const float v = c < D ? __fdiv_rn(x[c], nrm) : 0.f;
-    const __half h = __float2half_rn(v);
-    hi[static_cast<size_t>(row) * ld + c] = h;
-    if (lo) lo[static_cast<size_t>(row) * ld + c] = __float2half_rn((v - __half2float(h)) * kLoScale);
-  }
+  for (int c = lane; c < ld; c += 32)
+    store1(hi, lo, static_cast<size_t>(row) * ld + c, c < D ? __fdiv_rn(x[c], nrm) : 0.f);
 }
 
 // cost[t][n] = min over gallery rows s in [off[t], off[t+1]) of (1 - dots[s][n])
@@ -52,9 +49,7 @@ __global__ void rows_to_planes_kernel(const float* __restrict__ src, int rows, i
   for (int c = lane; c < ld; c += 32) {
     const float v = c < D ? x[c] : 0.f;
     ss = fmaf(v, v, ss);
-    const __half h = __float2half_rn(v);
-    hi[static_cast<size_t>(row) * ld + c] = h;
-    if (lo) lo[static_cast<size_t>(row) * ld + c] = __float2half_rn((v - __half2float(h)) * kLoScale);
+    store1(hi, lo, static_cast<size_t>(row) * ld + c, v);
   }
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, o);

@@ -9,44 +9,10 @@
 #include "common.h"
 #include "devutil.cuh"
 #include "kernels.h"
+#include "planes.cuh"
 
 namespace b2 {
 namespace {
-
-__device__ __forceinline__ void ld8(const __half* hi, const __half* lo, size_t off, float (&v)[8]) {
-  const uint4 h = __ldg(reinterpret_cast<const uint4*>(hi + off));
-  const __half2* hh = reinterpret_cast<const __half2*>(&h);
-#pragma unroll
-  for (int t = 0; t < 4; ++t) {
-    const float2 f = __half22float2(hh[t]);
-    v[2 * t] = f.x;
-    v[2 * t + 1] = f.y;
-  }
-  if (lo) {
-    const uint4 l = __ldg(reinterpret_cast<const uint4*>(lo + off));
-    const __half2* ll = reinterpret_cast<const __half2*>(&l);
-#pragma unroll
-    for (int t = 0; t < 4; ++t) {
-      const float2 f = __half22float2(ll[t]);
-      v[2 * t] = fmaf(f.x, kLoInv, v[2 * t]);
-      v[2 * t + 1] = fmaf(f.y, kLoInv, v[2 * t + 1]);
-    }
-  }
-}
-
-__device__ __forceinline__ void st8(__half* hi, __half* lo, size_t off, const float (&v)[8]) {
-  uint4 oh, ol;
-  __half2* hh = reinterpret_cast<__half2*>(&oh);
-  __half2* ll = reinterpret_cast<__half2*>(&ol);
-#pragma unroll
-  for (int t = 0; t < 4; ++t) {
-    hh[t] = __floats2half2_rn(v[2 * t], v[2 * t + 1]);
-    const float2 f = __half22float2(hh[t]);
-    ll[t] = __floats2half2_rn((v[2 * t] - f.x) * kLoScale, (v[2 * t + 1] - f.y) * kLoScale);
-  }
-  *reinterpret_cast<uint4*>(hi + off) = oh;
-  if (lo) *reinterpret_cast<uint4*>(lo + off) = ol;
-}
 
 // One BiFPN node input resampled on the fly to the node resolution (Ho x Wo):
 //   mode 0: same size; mode 1: 3x3 stride-2 max-pool with TF SAME padding from a 2x finer map;
@@ -54,9 +20,9 @@ __device__ __forceinline__ void st8(__half* hi, __half* lo, size_t off, const fl
 __device__ __forceinline__ void fetch_resampled(const BifpnInput& in, int b, int y, int x, int C, int cv,
                                                 float (&v)[8]) {
   if (in.mode == 0) {
-    ld8(in.hi, in.lo, ((static_cast<size_t>(b) * in.H + y) * in.W + x) * C + cv * 8, v);
+    load8(in.hi, in.lo, ((static_cast<size_t>(b) * in.H + y) * in.W + x) * C + cv * 8, v);
   } else if (in.mode == 2) {
-    ld8(in.hi, in.lo, ((static_cast<size_t>(b) * in.H + (y >> 1)) * in.W + (x >> 1)) * C + cv * 8, v);
+    load8(in.hi, in.lo, ((static_cast<size_t>(b) * in.H + (y >> 1)) * in.W + (x >> 1)) * C + cv * 8, v);
   } else {
     // SAME padding for k=3, s=2: pad_total = max((out-1)*2 + 3 - in, 0), pad_before = pad_total / 2
     const int y0 = 2 * y - in.pad_t, x0 = 2 * x - in.pad_l;
@@ -69,7 +35,7 @@ __device__ __forceinline__ void fetch_resampled(const BifpnInput& in, int b, int
         const int ix = x0 + s;
         if (ix < 0 || ix >= in.W) continue;
         float t[8];
-        ld8(in.hi, in.lo, ((static_cast<size_t>(b) * in.H + iy) * in.W + ix) * C + cv * 8, t);
+        load8(in.hi, in.lo, ((static_cast<size_t>(b) * in.H + iy) * in.W + ix) * C + cv * 8, t);
 #pragma unroll
         for (int j = 0; j < 8; ++j) v[j] = fmaxf(v[j], t[j]);
       }
@@ -102,7 +68,7 @@ __global__ void bifpn_combine_kernel(const __grid_constant__ BifpnCombineParams 
 #pragma unroll
       for (int j = 0; j < 8; ++j) acc[j] = __fmul_rn(acc[j], 1.f / (1.f + expf(-acc[j])));
     }
-    st8(p.out_hi, p.out_lo, pix * p.C + cv * 8, acc);
+    store8(p.out_hi, p.out_lo, pix * p.C + cv * 8, acc);
   }
 }
 
@@ -344,13 +310,6 @@ __global__ void __launch_bounds__(32, 1) nms_scan_kernel(const __grid_constant__
 __global__ void topk_seed_kernel(uint32_t* state, uint32_t need) { state[2] = need; }
 
 constexpr unsigned kTopkMaxBlocks = 132 * 8;
-
-inline unsigned grid_for(size_t total, int threads, unsigned cap = 132 * 16) {
-  size_t b = (total + threads - 1) / threads;
-  if (b > cap) b = cap;
-  if (b == 0) b = 1;
-  return static_cast<unsigned>(b);
-}
 
 int next_pow2(int v) {
   int p = 1;

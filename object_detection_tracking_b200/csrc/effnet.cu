@@ -7,44 +7,10 @@
 // squeeze-excite (_call_se :300-326); Model's stem Conv2D 3x3/2 SAME (:519-531).
 #include "common.h"
 #include "kernels.h"
+#include "planes.cuh"
 
 namespace b2 {
 namespace {
-
-__device__ __forceinline__ void ld8(const __half* hi, const __half* lo, size_t off, float (&v)[8]) {
-  const uint4 h = __ldg(reinterpret_cast<const uint4*>(hi + off));
-  const __half2* hh = reinterpret_cast<const __half2*>(&h);
-#pragma unroll
-  for (int t = 0; t < 4; ++t) {
-    const float2 f = __half22float2(hh[t]);
-    v[2 * t] = f.x;
-    v[2 * t + 1] = f.y;
-  }
-  if (lo) {
-    const uint4 l = __ldg(reinterpret_cast<const uint4*>(lo + off));
-    const __half2* ll = reinterpret_cast<const __half2*>(&l);
-#pragma unroll
-    for (int t = 0; t < 4; ++t) {
-      const float2 f = __half22float2(ll[t]);
-      v[2 * t] = fmaf(f.x, kLoInv, v[2 * t]);
-      v[2 * t + 1] = fmaf(f.y, kLoInv, v[2 * t + 1]);
-    }
-  }
-}
-
-__device__ __forceinline__ void st8(__half* hi, __half* lo, size_t off, const float (&v)[8]) {
-  uint4 oh, ol;
-  __half2* hh = reinterpret_cast<__half2*>(&oh);
-  __half2* ll = reinterpret_cast<__half2*>(&ol);
-#pragma unroll
-  for (int t = 0; t < 4; ++t) {
-    hh[t] = __floats2half2_rn(v[2 * t], v[2 * t + 1]);
-    const float2 f = __half22float2(hh[t]);
-    ll[t] = __floats2half2_rn((v[2 * t] - f.x) * kLoScale, (v[2 * t + 1] - f.y) * kLoScale);
-  }
-  *reinterpret_cast<uint4*>(hi + off) = oh;
-  if (lo) *reinterpret_cast<uint4*>(lo + off) = ol;
-}
 
 // uint8 BGR frame -> RGB, * 1/255, (x - mean) / std, legacy bilinear resize (align_corners=False, no half-pixel
 // centres) to (sh, sw), zero-padded bottom/right to [H, W, 3] fp32.  The reference normalises first and resizes the
@@ -99,7 +65,7 @@ __global__ void stem_im2col_kernel(const float* __restrict__ img, int H, int W, 
     }
     v[j] = t;
   }
-  st8(out_hi, out_lo, pix * 64 + oct * 8, v);
+  store8(out_hi, out_lo, pix * 64 + oct * 8, v);
 }
 
 // depthwise KxK, stride 1/2, TF SAME padding, optional bias (folded BatchNorm shift) and swish.
@@ -143,7 +109,7 @@ __global__ void __launch_bounds__(128) dw_strip_kernel(const __grid_constant__ D
         const int ix = ix0 + i;
         const bool ok = oky && ix >= 0 && ix < p.W;
         const int cx = min(max(ix, 0), p.W - 1);
-        ld8(p.in_hi, p.in_lo, (static_cast<size_t>(cy) * p.W + cx) * p.C + cv * 8, col[i]);
+        load8(p.in_hi, p.in_lo, (static_cast<size_t>(cy) * p.W + cx) * p.C + cv * 8, col[i]);
         if (!ok) {
 #pragma unroll
           for (int j = 0; j < 8; ++j) col[i][j] = 0.f;
@@ -167,7 +133,7 @@ __global__ void __launch_bounds__(128) dw_strip_kernel(const __grid_constant__ D
 #pragma unroll
         for (int j = 0; j < 8; ++j) acc[t][j] = __fmul_rn(acc[t][j], 1.f / (1.f + expf(-acc[t][j])));
       }
-      st8(p.out_hi, p.out_lo, (static_cast<size_t>(y) * p.Wo + x0 + t) * p.C + cv * 8, acc[t]);
+      store8(p.out_hi, p.out_lo, (static_cast<size_t>(y) * p.Wo + x0 + t) * p.C + cv * 8, acc[t]);
     }
   }
 }
@@ -188,7 +154,7 @@ __global__ void __launch_bounds__(256) se_partial_kernel(const __half* __restric
     for (int u = 0; u < 4; ++u) {
       const int pp = p + 32 * u;
       if (pp < p1) {
-        ld8(in_hi, in_lo, static_cast<size_t>(pp) * C + cg * 64 + cv * 8, v[u]);
+        load8(in_hi, in_lo, static_cast<size_t>(pp) * C + cg * 64 + cv * 8, v[u]);
       } else {
 #pragma unroll
         for (int j = 0; j < 8; ++j) v[u][j] = 0.f;
@@ -292,18 +258,8 @@ __global__ void __launch_bounds__(256) se_fc2_scale_kernel(const float* __restri
   const float g = gate[cc];
   for (int o = threadIdx.x >> 6; o < rows; o += 4) {
     const size_t idx = static_cast<size_t>(o) * K + c0 + cc;
-    const float v = __fmul_rn(w[idx], g);
-    const __half h = __float2half_rn(v);
-    hi[idx] = h;
-    if (lo) lo[idx] = __float2half_rn((v - __half2float(h)) * kLoScale);
+    store1(hi, lo, idx, __fmul_rn(w[idx], g));
   }
-}
-
-inline unsigned grid_for(size_t total, int threads, unsigned cap) {
-  size_t b = (total + threads - 1) / threads;
-  if (b > cap) b = cap;
-  if (b == 0) b = 1;
-  return static_cast<unsigned>(b);
 }
 
 }  // namespace

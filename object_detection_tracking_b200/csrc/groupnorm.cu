@@ -19,6 +19,7 @@
 
 #include "common.h"
 #include "kernels.h"
+#include "planes.cuh"
 
 namespace b2 {
 namespace {
@@ -61,28 +62,6 @@ __device__ __forceinline__ Moments warp_merge(Moments m, int lane) {
   return m;
 }
 
-// eight channels of one pixel as fp32: hi + lo / 2048
-__device__ __forceinline__ void load8(const __half* hi, const __half* lo, size_t off, float v[8]) {
-  const uint4 h = *reinterpret_cast<const uint4*>(hi + off);
-  const __half2* h2 = reinterpret_cast<const __half2*>(&h);
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const float2 f = __half22float2(h2[i]);
-    v[2 * i] = f.x;
-    v[2 * i + 1] = f.y;
-  }
-  if (lo != nullptr) {
-    const uint4 l = *reinterpret_cast<const uint4*>(lo + off);
-    const __half2* l2 = reinterpret_cast<const __half2*>(&l);
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      const float2 f = __half22float2(l2[i]);
-      v[2 * i] = fmaf(f.x, kLoInv, v[2 * i]);
-      v[2 * i + 1] = fmaf(f.y, kLoInv, v[2 * i + 1]);
-    }
-  }
-}
-
 __device__ __forceinline__ size_t view_offset(const GnParams& p, int b, long long q, int vec) {
   const int y = static_cast<int>(q / p.W), x = static_cast<int>(q % p.W);
   return ((static_cast<size_t>(b) * p.pitch_H + y + p.off_h) * p.pitch_W + x + p.off_w) * p.ld + vec * 8;
@@ -103,7 +82,7 @@ __device__ void block_moments(const GnParams& p, int b, long long q0, long long 
     float v[4][8];
 #pragma unroll
     for (int u = 0; u < 4; ++u)
-      if (q + u * lanes < q1) load8(p.x_hi, p.x_lo, view_offset(p, b, q + u * lanes, vec), v[u]);
+      if (q + u * lanes < q1) load8_coherent(p.x_hi, p.x_lo, view_offset(p, b, q + u * lanes, vec), v[u]);
 #pragma unroll
     for (int u = 0; u < 4; ++u) {
       if (q + u * lanes >= q1) continue;
@@ -157,14 +136,14 @@ __device__ void apply_range(const GnParams& p, int b, long long q0, long long q1
   for (long long q = q0 + pl; q < q1; q += lanes) {
     const size_t off = view_offset(p, b, q, vec);
     float v[8];
-    load8(p.x_hi, p.x_lo, off, v);
+    load8_coherent(p.x_hi, p.x_lo, off, v);
 #pragma unroll
     for (int i = 0; i < 8; ++i) v[i] = v[i] * s_inv[vec * 8 + i] + s_shift[vec * 8 + i];
     if (p.r_hi != nullptr) {
       const int y = static_cast<int>(q / p.W) >> p.res_shift, x = static_cast<int>(q % p.W) >> p.res_shift;
       const size_t roff = ((static_cast<size_t>(b) * p.res_H + y) * p.res_W + x) * p.res_ld + vec * 8;
       float r[8];
-      load8(p.r_hi, p.r_lo, roff, r);
+      load8_coherent(p.r_hi, p.r_lo, roff, r);
 #pragma unroll
       for (int i = 0; i < 8; ++i) v[i] += r[i];
     }
@@ -172,18 +151,9 @@ __device__ void apply_range(const GnParams& p, int b, long long q0, long long q1
 #pragma unroll
       for (int i = 0; i < 8; ++i) v[i] = fmaxf(v[i], 0.f);
     }
-    uint4 h, l;
-    __half2* h2 = reinterpret_cast<__half2*>(&h);
-    __half2* l2 = reinterpret_cast<__half2*>(&l);
 #pragma unroll
-    for (int i = 0; i < 4; ++i) {
-      amax = fmaxf(amax, fmaxf(fabsf(v[2 * i]), fabsf(v[2 * i + 1])));
-      h2[i] = __floats2half2_rn(v[2 * i], v[2 * i + 1]);
-      const float2 hf = __half22float2(h2[i]);
-      l2[i] = __floats2half2_rn((v[2 * i] - hf.x) * kLoScale, (v[2 * i + 1] - hf.y) * kLoScale);
-    }
-    *reinterpret_cast<uint4*>(p.y_hi + off) = h;
-    if (p.y_lo != nullptr) *reinterpret_cast<uint4*>(p.y_lo + off) = l;
+    for (int i = 0; i < 8; ++i) amax = fmaxf(amax, fabsf(v[i]));
+    store8(p.y_hi, p.y_lo, off, v);
   }
   // same monitor as conv_tc_kernel: inf included, a NaN can only follow an inf an earlier launch has flagged
   if (p.range_flag != nullptr && amax > 65504.f) atomicOr(p.range_flag, 1u);

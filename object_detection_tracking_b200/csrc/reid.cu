@@ -6,36 +6,10 @@
 // of OSBlock.forward (:262-268), AvgPool2d(2) of the transitions (:375-381), AdaptiveAvgPool2d(1) (:428).
 #include "common.h"
 #include "kernels.h"
+#include "planes.cuh"
 
 namespace b2 {
 namespace {
-
-__device__ __forceinline__ void unpack8(const uint4& h, const uint4& l, bool has_lo, float (&v)[8]) {
-  const __half2* hh = reinterpret_cast<const __half2*>(&h);
-  const __half2* ll = reinterpret_cast<const __half2*>(&l);
-#pragma unroll
-  for (int t = 0; t < 4; ++t) {
-    float2 f = __half22float2(hh[t]);
-    if (has_lo) {
-      const float2 g = __half22float2(ll[t]);
-      f.x = fmaf(g.x, kLoInv, f.x);
-      f.y = fmaf(g.y, kLoInv, f.y);
-    }
-    v[2 * t] = f.x;
-    v[2 * t + 1] = f.y;
-  }
-}
-
-__device__ __forceinline__ void pack8(const float (&v)[8], uint4& h, uint4& l) {
-  __half2* hh = reinterpret_cast<__half2*>(&h);
-  __half2* ll = reinterpret_cast<__half2*>(&l);
-#pragma unroll
-  for (int t = 0; t < 4; ++t) {
-    hh[t] = __floats2half2_rn(v[2 * t], v[2 * t + 1]);
-    const float2 f = __half22float2(hh[t]);
-    ll[t] = __floats2half2_rn((v[2 * t] - f.x) * kLoScale, (v[2 * t + 1] - f.y) * kLoScale);
-  }
-}
 
 // depthwise 3x3, stride 1, pad 1, + folded BN + ReLU.  w: [9][C] fp32 (BN scale folded), bias [C].
 __global__ void dwconv3x3_kernel(const __half* __restrict__ in_hi, const __half* __restrict__ in_lo, int B, int H, int W,
@@ -61,12 +35,8 @@ __global__ void dwconv3x3_kernel(const __half* __restrict__ in_hi, const __half*
       for (int s = 0; s < 3; ++s) {
         const int ix = x + s - 1;
         if (ix < 0 || ix >= W) continue;
-        const size_t off = ((static_cast<size_t>(b) * H + iy) * W + ix) * C + cv * 8;
-        const uint4 h = __ldg(reinterpret_cast<const uint4*>(in_hi + off));
-        uint4 l = make_uint4(0, 0, 0, 0);
-        if (in_lo) l = __ldg(reinterpret_cast<const uint4*>(in_lo + off));
         float v[8];
-        unpack8(h, l, in_lo != nullptr, v);
+        load8_early(in_hi, in_lo, ((static_cast<size_t>(b) * H + iy) * W + ix) * C + cv * 8, v);
         const float4* wp = reinterpret_cast<const float4*>(w + static_cast<size_t>(r * 3 + s) * C + cv * 8);
         const float4 w0 = __ldg(wp), w1 = __ldg(wp + 1);
         acc[0] = fmaf(v[0], w0.x, acc[0]); acc[1] = fmaf(v[1], w0.y, acc[1]);
@@ -80,11 +50,7 @@ __global__ void dwconv3x3_kernel(const __half* __restrict__ in_hi, const __half*
     const float bb[8] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
 #pragma unroll
     for (int j = 0; j < 8; ++j) acc[j] = fmaxf(acc[j] + bb[j], 0.f);
-    uint4 oh, ol;
-    pack8(acc, oh, ol);
-    const size_t o = pix * C + cv * 8;
-    *reinterpret_cast<uint4*>(out_hi + o) = oh;
-    if (out_lo) *reinterpret_cast<uint4*>(out_lo + o) = ol;
+    store8(out_hi, out_lo, pix * C + cv * 8, acc);
   }
 }
 
@@ -97,12 +63,8 @@ __global__ void __launch_bounds__(256) gap_kernel(const __half* __restrict__ in_
 #pragma unroll
   for (int j = 0; j < 8; ++j) acc[j] = 0.f;
   for (int p = pl; p < HW; p += 32) {
-    const size_t off = (static_cast<size_t>(b) * HW + p) * C + cg * 64 + cv * 8;
-    const uint4 h = __ldg(reinterpret_cast<const uint4*>(in_hi + off));
-    uint4 l = make_uint4(0, 0, 0, 0);
-    if (in_lo) l = __ldg(reinterpret_cast<const uint4*>(in_lo + off));
     float v[8];
-    unpack8(h, l, in_lo != nullptr, v);
+    load8_early(in_hi, in_lo, (static_cast<size_t>(b) * HW + p) * C + cg * 64 + cv * 8, v);
 #pragma unroll
     for (int j = 0; j < 8; ++j) acc[j] += v[j];
   }
@@ -167,19 +129,13 @@ __global__ void gated_sum4_kernel(const __half* __restrict__ a_hi, const __half*
     for (int j = 0; j < 8; ++j) acc[j] = 0.f;
 #pragma unroll
     for (int s = 0; s < 4; ++s) {
-      const uint4 h = __ldg(reinterpret_cast<const uint4*>(his[s] + off));
-      uint4 l = make_uint4(0, 0, 0, 0);
-      if (los[s]) l = __ldg(reinterpret_cast<const uint4*>(los[s] + off));
       float v[8];
-      unpack8(h, l, los[s] != nullptr, v);
+      load8_early(his[s], los[s], off, v);
       const float* gp = gates + (static_cast<size_t>(b) * 4 + s) * C + cv * 8;
 #pragma unroll
       for (int j = 0; j < 8; ++j) acc[j] = __fadd_rn(acc[j], __fmul_rn(v[j], __ldg(gp + j)));
     }
-    uint4 oh, ol;
-    pack8(acc, oh, ol);
-    *reinterpret_cast<uint4*>(out_hi + off) = oh;
-    if (out_lo) *reinterpret_cast<uint4*>(out_lo + off) = ol;
+    store8(out_hi, out_lo, off, acc);
   }
 }
 
@@ -202,30 +158,15 @@ __global__ void avgpool2_kernel(const __half* __restrict__ in_hi, const __half* 
     for (int dy = 0; dy < 2; ++dy)
 #pragma unroll
       for (int dx = 0; dx < 2; ++dx) {
-        const size_t off = ((static_cast<size_t>(b) * H + 2 * y + dy) * W + 2 * x + dx) * C + cv * 8;
-        const uint4 h = __ldg(reinterpret_cast<const uint4*>(in_hi + off));
-        uint4 l = make_uint4(0, 0, 0, 0);
-        if (in_lo) l = __ldg(reinterpret_cast<const uint4*>(in_lo + off));
         float v[8];
-        unpack8(h, l, in_lo != nullptr, v);
+        load8_early(in_hi, in_lo, ((static_cast<size_t>(b) * H + 2 * y + dy) * W + 2 * x + dx) * C + cv * 8, v);
 #pragma unroll
         for (int j = 0; j < 8; ++j) acc[j] += v[j];
       }
 #pragma unroll
     for (int j = 0; j < 8; ++j) acc[j] *= 0.25f;
-    uint4 oh, ol;
-    pack8(acc, oh, ol);
-    const size_t o = pix * C + cv * 8;
-    *reinterpret_cast<uint4*>(out_hi + o) = oh;
-    if (out_lo) *reinterpret_cast<uint4*>(out_lo + o) = ol;
+    store8(out_hi, out_lo, pix * C + cv * 8, acc);
   }
-}
-
-inline unsigned grid_for(size_t total, int threads, unsigned cap = 132 * 32) {
-  size_t b = (total + threads - 1) / threads;
-  if (b > cap) b = cap;
-  if (b == 0) b = 1;
-  return static_cast<unsigned>(b);
 }
 
 }  // namespace
@@ -233,7 +174,7 @@ inline unsigned grid_for(size_t total, int threads, unsigned cap = 132 * 32) {
 int dwconv3x3_launch(const __half* in_hi, const __half* in_lo, int B, int H, int W, int C, const float* w,
                      const float* bias, __half* out_hi, __half* out_lo, cudaStream_t s) {
   const size_t total = static_cast<size_t>(B) * H * W * (C / 8);
-  dwconv3x3_kernel<<<grid_for(total, 256), 256, 0, s>>>(in_hi, in_lo, B, H, W, C, w, bias, out_hi, out_lo);
+  dwconv3x3_kernel<<<grid_for(total, 256, 132 * 32), 256, 0, s>>>(in_hi, in_lo, B, H, W, C, w, bias, out_hi, out_lo);
   B2_CUDA(cudaGetLastError());
   return 0;
 }
@@ -256,8 +197,8 @@ int gate_mlp_launch(const float* g, int rows, int C, int Creal, int Cr, const fl
 int gated_sum4_launch(const __half* const hi[4], const __half* const lo[4], const float* gates, int B, int HW, int C,
                       __half* out_hi, __half* out_lo, cudaStream_t s) {
   const size_t total = static_cast<size_t>(B) * HW * (C / 8);
-  gated_sum4_kernel<<<grid_for(total, 256), 256, 0, s>>>(hi[0], lo[0], hi[1], lo[1], hi[2], lo[2], hi[3], lo[3], gates,
-                                                           B, HW, C, out_hi, out_lo);
+  gated_sum4_kernel<<<grid_for(total, 256, 132 * 32), 256, 0, s>>>(hi[0], lo[0], hi[1], lo[1], hi[2], lo[2], hi[3], lo[3],
+                                                                     gates, B, HW, C, out_hi, out_lo);
   B2_CUDA(cudaGetLastError());
   return 0;
 }
@@ -265,7 +206,7 @@ int gated_sum4_launch(const __half* const hi[4], const __half* const lo[4], cons
 int avgpool2_launch(const __half* in_hi, const __half* in_lo, int B, int H, int W, int C, __half* out_hi,
                     __half* out_lo, cudaStream_t s) {
   const size_t total = static_cast<size_t>(B) * (H / 2) * (W / 2) * (C / 8);
-  avgpool2_kernel<<<grid_for(total, 256), 256, 0, s>>>(in_hi, in_lo, B, H, W, C, out_hi, out_lo);
+  avgpool2_kernel<<<grid_for(total, 256, 132 * 32), 256, 0, s>>>(in_hi, in_lo, B, H, W, C, out_hi, out_lo);
   B2_CUDA(cudaGetLastError());
   return 0;
 }

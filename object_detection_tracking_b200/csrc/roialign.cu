@@ -8,6 +8,7 @@
 // op for op, with explicit round-to-nearest intrinsics so no FMA contraction changes the sample grid.
 #include "common.h"
 #include "kernels.h"
+#include "planes.cuh"
 
 namespace b2 {
 namespace {
@@ -43,27 +44,6 @@ __device__ __forceinline__ Axis make_axis(float c0, float c1, int dim, int bin) 
     a.lerp[t] = __fsub_rn(inc, fl);
   }
   return a;
-}
-
-__device__ __forceinline__ void load8(const __half* hi, const __half* lo, size_t off, float (&v)[8]) {
-  const uint4 h = __ldg(reinterpret_cast<const uint4*>(hi + off));
-  const __half2* hh = reinterpret_cast<const __half2*>(&h);
-#pragma unroll
-  for (int t = 0; t < 4; ++t) {
-    const float2 f = __half22float2(hh[t]);
-    v[2 * t] = f.x;
-    v[2 * t + 1] = f.y;
-  }
-  if (lo) {
-    const uint4 l = __ldg(reinterpret_cast<const uint4*>(lo + off));
-    const __half2* ll = reinterpret_cast<const __half2*>(&l);
-#pragma unroll
-    for (int t = 0; t < 4; ++t) {
-      const float2 f = __half22float2(ll[t]);
-      v[2 * t] = fmaf(f.x, kLoInv, v[2 * t]);
-      v[2 * t + 1] = fmaf(f.y, kLoInv, v[2 * t + 1]);
-    }
-  }
 }
 
 template <int kOut>
@@ -127,18 +107,7 @@ __global__ void __launch_bounds__(256) roialign_kernel(const __grid_constant__ R
 #pragma unroll
     for (int t = 0; t < 8; ++t) o[static_cast<size_t>(t) * kOut * kOut] = acc[t];
   }
-  if (p.out_hi) {
-    __align__(16) __half hb[8];
-    __align__(16) __half lb[8];
-#pragma unroll
-    for (int t = 0; t < 8; ++t) {
-      hb[t] = __float2half_rn(acc[t]);
-      lb[t] = __float2half_rn((acc[t] - __half2float(hb[t])) * kLoScale);
-    }
-    const size_t o = (roi * (kOut * kOut) + bin) * p.C + c0;
-    *reinterpret_cast<uint4*>(p.out_hi + o) = *reinterpret_cast<uint4*>(hb);
-    if (p.out_lo) *reinterpret_cast<uint4*>(p.out_lo + o) = *reinterpret_cast<uint4*>(lb);
-  }
+  if (p.out_hi) store8(p.out_hi, p.out_lo, (roi * (kOut * kOut) + bin) * p.C + c0, acc);
 }
 
 // EfficientDet box feature: ROIAlign 7x7 on the detection's own pyramid level, then the mean of the 49 bins.

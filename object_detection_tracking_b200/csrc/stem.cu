@@ -4,6 +4,7 @@
 // Reference ops replaced: build_preprocess (models.py:337-357), resnet_fpn_backbone stem
 // (nn.py:871-900: pad [3, 2+pad32], conv0 7x7 s2 VALID + BN + ReLU, pad [1,0], MaxPooling 3x3 s2 VALID).
 #include "common.h"
+#include "planes.cuh"
 #include "resize_math.h"
 
 namespace b2 {
@@ -12,12 +13,8 @@ namespace {
 __global__ void f32_to_planes_kernel(const float* __restrict__ src, __half* __restrict__ hi, __half* __restrict__ lo,
                                      size_t n) {
   for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < n;
-       i += static_cast<size_t>(gridDim.x) * blockDim.x) {
-    const float v = src[i];
-    const __half h = __float2half_rn(v);
-    hi[i] = h;
-    if (lo) lo[i] = __float2half_rn((v - __half2float(h)) * kLoScale);
-  }
+       i += static_cast<size_t>(gridDim.x) * blockDim.x)
+    store1(hi, lo, i, src[i]);
 }
 
 __global__ void planes_to_f32_kernel(const __half* __restrict__ hi, const __half* __restrict__ lo,
@@ -25,7 +22,7 @@ __global__ void planes_to_f32_kernel(const __half* __restrict__ hi, const __half
   for (size_t i = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; i < n;
        i += static_cast<size_t>(gridDim.x) * blockDim.x) {
     float v = __half2float(hi[i]);
-    if (lo) v = fmaf(__half2float(lo[i]), kLoInv, v);
+    if (lo) v = join(v, lo[i]);
     dst[i] = v;
   }
 }
@@ -70,8 +67,7 @@ __global__ void __launch_bounds__(256) stem_pack_kernel(const TIn* __restrict__ 
           v = __fdiv_rn(x, stdv[c]);
         }
       }
-      hb[j] = __float2half_rn(v);
-      lb[j] = __float2half_rn((v - __half2float(hb[j])) * kLoScale);
+      split(v, hb[j], lb[j]);
     }
     *reinterpret_cast<uint4*>(out_hi + pix * 64 + cg * 8) = *reinterpret_cast<uint4*>(hb);
     if (out_lo) *reinterpret_cast<uint4*>(out_lo + pix * 64 + cg * 8) = *reinterpret_cast<uint4*>(lb);
@@ -110,8 +106,7 @@ __global__ void __launch_bounds__(256) stem_pack16_kernel(const TIn* __restrict_
           v = __fdiv_rn(t, stdv[c]);
         }
       }
-      hb[j] = __float2half_rn(v);
-      lb[j] = __float2half_rn((v - __half2float(hb[j])) * kLoScale);
+      split(v, hb[j], lb[j]);
     }
     uint4* oh = reinterpret_cast<uint4*>(out_hi + pix * 16);
     oh[0] = reinterpret_cast<uint4*>(hb)[0];
@@ -159,7 +154,7 @@ __global__ void maxpool_kernel(const __half* __restrict__ in_hi, const __half* _
         const __half* l = reinterpret_cast<const __half*>(&vl);
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
-          const float v = fmaf(__half2float(l[j]), kLoInv, __half2float(h[j]));
+          const float v = join(__half2float(h[j]), l[j]);
           if (v > best[j]) {
             best[j] = v;
             bh[j] = h[j];
@@ -197,22 +192,15 @@ __global__ void resize_u8_to_f32_kernel(const uint8_t* __restrict__ src, int B, 
   }
 }
 
-inline unsigned grid_for(size_t total, int threads, unsigned cap = 132 * 32) {
-  size_t b = (total + threads - 1) / threads;
-  if (b > cap) b = cap;
-  if (b == 0) b = 1;
-  return static_cast<unsigned>(b);
-}
-
 }  // namespace
 
 int f32_to_planes(const float* src, __half* hi, __half* lo, size_t n, cudaStream_t s) {
-  f32_to_planes_kernel<<<grid_for(n, 256), 256, 0, s>>>(src, hi, lo, n);
+  f32_to_planes_kernel<<<grid_for(n, 256, 132 * 32), 256, 0, s>>>(src, hi, lo, n);
   B2_CUDA(cudaGetLastError());
   return 0;
 }
 int planes_to_f32(const __half* hi, const __half* lo, float* dst, size_t n, cudaStream_t s) {
-  planes_to_f32_kernel<<<grid_for(n, 256), 256, 0, s>>>(hi, lo, dst, n);
+  planes_to_f32_kernel<<<grid_for(n, 256, 132 * 32), 256, 0, s>>>(hi, lo, dst, n);
   B2_CUDA(cudaGetLastError());
   return 0;
 }
@@ -243,7 +231,7 @@ int stem_pack16_launch(const void* img, int is_u8, int B, int H, int W, __half* 
 
 int resize_u8_launch(const uint8_t* src, int B, int sh, int sw, float* dst, int dh, int dw, cudaStream_t s) {
   const size_t total = static_cast<size_t>(B) * dh * dw;
-  resize_u8_to_f32_kernel<<<grid_for(total, 256), 256, 0, s>>>(src, B, sh, sw, dst, dh, dw);
+  resize_u8_to_f32_kernel<<<grid_for(total, 256, 132 * 32), 256, 0, s>>>(src, B, sh, sw, dst, dh, dw);
   B2_CUDA(cudaGetLastError());
   return 0;
 }
@@ -251,7 +239,7 @@ int resize_u8_launch(const uint8_t* src, int B, int sh, int sw, float* dst, int 
 int maxpool_launch(const __half* in_hi, const __half* in_lo, int B, int H, int W, int C, __half* out_hi,
                    __half* out_lo, int Ho, int Wo, cudaStream_t s) {
   const size_t total = static_cast<size_t>(B) * Ho * Wo * (C / 8);
-  maxpool_kernel<<<grid_for(total, 256), 256, 0, s>>>(in_hi, in_lo, B, H, W, C, out_hi, out_lo, Ho, Wo);
+  maxpool_kernel<<<grid_for(total, 256, 132 * 32), 256, 0, s>>>(in_hi, in_lo, B, H, W, C, out_hi, out_lo, Ho, Wo);
   B2_CUDA(cudaGetLastError());
   return 0;
 }
