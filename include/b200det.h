@@ -61,6 +61,9 @@ typedef struct b2_config {
                                  folded BatchNorm in the backbone, and after every FPN lateral / post-hoc conv (nn.py:987-1009) */
   int32_t conv_head_dim;      /* 0 = 2fc head; > 0: --use_conv_frcnn_head with conv_frcnn_head_dim channels (models.py:1110-1125):
                                  4 x conv3x3 + ReLU (+ GroupNorm per ROI with use_gn) -> fc, replacing fc6 / fc7 */
+  int32_t use_se;             /* --use_se (--version 6): squeeze-excite in every bottleneck (nn.py:506-519), per image:
+                                 relu(conv3 * sigmoid(fc2(relu(fc1(mean_hw(conv3))))) + shortcut), weights
+                                 "<block>/fc1/{W,b}" [4*ch, ch/4] and "<block>/fc2/{W,b}" [ch/4, 4*ch] */
 } b2_config;
 
 const char* b2_last_error(void);
@@ -319,6 +322,11 @@ int b2_op_conv2d(int device, const float* x, const float* w, const float* bias, 
 int b2_op_group_norm(int device, const float* x, const float* res, const float* gamma, const float* beta, int B,
                      int pitch_H, int pitch_W, int C, int H, int W, int off_h, int off_w, int res_H, int res_W, int res_shift,
                      int relu, int per_roi, int split, int in_place, float* out);
+/* The SE-ResNet bottleneck's squeeze-excite (nn.py:506-519) as the engine runs it: x [B][H][W][C] (host, fp32, converted to
+ * the engine's planes), gate[b] = sigmoid(relu(mean_hw(x[b]) @ w1 + b1) @ w2 + b2) with w1 [C][nr], w2 [nr][C], then
+ * out = relu(x * gate[b][c] + res) in place (res [B][H][W][C], may be NULL).  gate_out [B][C] may be NULL. */
+int b2_op_squeeze_excite(int device, const float* x, const float* res, const float* w1, const float* b1, const float* w2,
+                         const float* b2, int B, int H, int W, int C, int nr, int split, float* out, float* gate_out);
 
 #ifdef __cplusplus
 }

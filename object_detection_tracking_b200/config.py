@@ -41,6 +41,8 @@ _DEFAULTS = dict(
     use_gn=False,                      # --use_gn (obj_detect_tracking.py:101-102): GroupNorm backbone + FPN
     use_conv_frcnn_head=False,         # --use_conv_frcnn_head (:103-104): 4-conv box head
     conv_frcnn_head_dim=256,           # only main.py:250 sets it (default 256); the inference drivers never do
+    use_se=False,                      # --use_se (obj_detect_tracking.py:192-193; set by --version 6, :278-280):
+                                       # squeeze-excite in every bottleneck (nn.py:506-519)
     use_partial_classes=False,
     is_efficientdet=False,
 )

@@ -138,10 +138,19 @@ __global__ void __launch_bounds__(128) dw_strip_kernel(const __grid_constant__ D
   }
 }
 
-// squeeze: per-channel partial sums over a pixel chunk.  grid (C/64, nchunks); partial [nchunks][C]
+// Squeeze-excite, shared by EfficientNet's MBConv blocks and the SE-ResNet bottleneck.  Every kernel takes the image from
+// blockIdx.z / blockIdx.y and touches only that image's scratch: input [B][HW][C], partial [B][nchunks][C],
+// r_part [B][kSeFc1Blocks][kSeMaxNr], gate [B][C].  The chunking depends on HW alone, so an image's gate does not depend
+// on the batch it is in.
+//
+// squeeze: per-channel partial sums over a pixel chunk.  grid (C/64, nchunks, B)
 __global__ void __launch_bounds__(256) se_partial_kernel(const __half* __restrict__ in_hi, const __half* __restrict__ in_lo,
                                                          int HW, int C, int chunk, float* __restrict__ partial) {
   const int cg = blockIdx.x, ch = blockIdx.y;
+  const size_t img = static_cast<size_t>(blockIdx.z) * HW * C;
+  in_hi += img;
+  if (in_lo != nullptr) in_lo += img;
+  partial += static_cast<size_t>(blockIdx.z) * gridDim.y * C;
   const int cv = threadIdx.x & 7, pl = threadIdx.x >> 3;
   const int p0 = ch * chunk, p1 = min(p0 + chunk, HW);
   float acc[8];
@@ -175,13 +184,16 @@ __global__ void __launch_bounds__(256) se_partial_kernel(const __half* __restric
 }
 
 // excite, stage 1: each block owns a channel slice: mean of its channels, then its share of the 1x1 reduce
-//   r_part[b][j] = sum_{c in slice b} mean[c] * w1[c][j]        (w1 = HWIO of [1,1,C,nr]: row c is contiguous in j)
+//   r_part[b][j] = sum_{c in slice b} mean[c] * w1[c][j]        (w1 = HWIO of [1,1,C,nr] or dense [C, nr]: row c is
+//   contiguous in j).  grid (kSeFc1Blocks, B)
 constexpr int kSeFc1Blocks = 32;
 constexpr int kSeMaxNr = 192;
 
 __global__ void __launch_bounds__(256) se_fc1_kernel(const float* __restrict__ partial, int nchunks, int Cpad, int C, int nr,
                                                      float inv_hw, const float* __restrict__ w1, float* __restrict__ r_part) {
   __shared__ float red[8][kSeMaxNr];
+  partial += static_cast<size_t>(blockIdx.y) * nchunks * Cpad;
+  r_part += static_cast<size_t>(blockIdx.y) * gridDim.x * kSeMaxNr;
   const int cs = (C + gridDim.x - 1) / gridDim.x;
   const int c0 = blockIdx.x * cs, c1 = min(c0 + cs, C);
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
@@ -214,9 +226,14 @@ __global__ void __launch_bounds__(256) se_fc1_kernel(const float* __restrict__ p
   }
 }
 
-// excite, stage 2 + weight fold: each block owns 64 channels: r = swish(sum_b r_part + b1) (recomputed per block, tiny),
-// gate_c = sigmoid(b2[c] + sum_j r_j w2[j][c]), then w'[o][c] = w[o][c] * gate_c for every output row o of the
-// projection conv, written as (hi, lo) operand planes.
+// excite, stage 2 + optional weight fold: each block owns 64 channels of one image: r = act(sum_b r_part + b1)
+// (recomputed per block, tiny; ACT = swish for MBConv, ReLU for the SE-ResNet bottleneck),
+// gate_c = sigmoid(b2[c] + sum_j r_j w2[j][c]) into gate_out [B][K]; then, when w is given (MBConv, batch 1),
+// w'[o][c] = w[o][c] * gate_c for every output row o of the projection conv, written as (hi, lo) operand planes.
+// grid (K/64, B)
+enum class SeAct { kSwish, kRelu };
+
+template <SeAct ACT>
 __global__ void __launch_bounds__(256) se_fc2_scale_kernel(const float* __restrict__ r_part, int nparts, int C, int nr,
                                                            const float* __restrict__ b1, const float* __restrict__ w2,
                                                            const float* __restrict__ b2, float* __restrict__ gate_out,
@@ -225,11 +242,13 @@ __global__ void __launch_bounds__(256) se_fc2_scale_kernel(const float* __restri
   __shared__ float r[kSeMaxNr];
   __shared__ float part[4][64];
   __shared__ float gate[64];
+  r_part += static_cast<size_t>(blockIdx.y) * nparts * kSeMaxNr;
+  gate_out += static_cast<size_t>(blockIdx.y) * K;
   for (int j = threadIdx.x; j < nr; j += blockDim.x) {
     float a = b1[j];
 #pragma unroll 8
     for (int b = 0; b < nparts; ++b) a += __ldg(r_part + static_cast<size_t>(b) * kSeMaxNr + j);
-    r[j] = a * (1.f / (1.f + expf(-a)));
+    r[j] = ACT == SeAct::kSwish ? a * (1.f / (1.f + expf(-a))) : fmaxf(a, 0.f);
   }
   __syncthreads();
   const int c0 = blockIdx.x * 64;
@@ -253,6 +272,7 @@ __global__ void __launch_bounds__(256) se_fc2_scale_kernel(const float* __restri
     gate[threadIdx.x] = a;
     gate_out[c] = a;
   }
+  if (w == nullptr) return;   // gate only (uniform across the block)
   __syncthreads();
   const int cc = threadIdx.x & 63;
   const float g = gate[cc];
@@ -311,17 +331,38 @@ int se_chunks(int HW) {
 int se_fc1_parts() { return kSeFc1Blocks; }
 int se_max_nr() { return kSeMaxNr; }
 
+int se_squeeze_launch(const __half* in_hi, const __half* in_lo, int B, int HW, int Cpad, float* partial, cudaStream_t s) {
+  B2_CHECK(Cpad % 64 == 0 && B >= 1 && HW >= 1, "se squeeze: bad geometry");
+  const int nch = se_chunks(HW), chunk = (HW + nch - 1) / nch;
+  se_partial_kernel<<<dim3(Cpad / 64, nch, B), 256, 0, s>>>(in_hi, in_lo, HW, Cpad, chunk, partial);
+  B2_CUDA(cudaGetLastError());
+  return 0;
+}
+
+int se_excite_launch(const float* partial, int B, int HW, int Cpad, int C, int nr, float* r_part, const float* w1,
+                     const float* b1, const float* w2, const float* b2, int relu, float* gate, const float* w, int rows,
+                     __half* w_hi, __half* w_lo, cudaStream_t s) {
+  B2_CHECK(Cpad % 64 == 0 && nr >= 1 && nr <= kSeMaxNr, "se excite: channel count out of range");
+  B2_CHECK(w == nullptr || B == 1, "se excite: the weight fold takes one image");
+  se_fc1_kernel<<<dim3(kSeFc1Blocks, B), 256, 0, s>>>(partial, se_chunks(HW), Cpad, C, nr, 1.0f / static_cast<float>(HW),
+                                                       w1, r_part);
+  const dim3 grid(Cpad / 64, B);
+  if (relu)
+    se_fc2_scale_kernel<SeAct::kRelu><<<grid, 256, 0, s>>>(r_part, kSeFc1Blocks, C, nr, b1, w2, b2, gate, w, rows, Cpad,
+                                                           w_hi, w_lo);
+  else
+    se_fc2_scale_kernel<SeAct::kSwish><<<grid, 256, 0, s>>>(r_part, kSeFc1Blocks, C, nr, b1, w2, b2, gate, w, rows, Cpad,
+                                                            w_hi, w_lo);
+  B2_CUDA(cudaGetLastError());
+  return 0;
+}
+
 // squeeze-excite of one MBConv block, gate folded into the projection weights (w [rows][K=Cpad] fp32 master copy)
 int se_gate_launch(const __half* in_hi, const __half* in_lo, int HW, int Cpad, int C, int nr, float* partial, float* r_part,
                    const float* w1, const float* b1, const float* w2, const float* b2, float* gate, const float* w, int rows,
                    __half* w_hi, __half* w_lo, cudaStream_t s) {
-  B2_CHECK(Cpad % 64 == 0 && nr >= 1 && nr <= kSeMaxNr, "se gate: channel count out of range");
-  const int nch = se_chunks(HW), chunk = (HW + nch - 1) / nch;
-  se_partial_kernel<<<dim3(Cpad / 64, nch), 256, 0, s>>>(in_hi, in_lo, HW, Cpad, chunk, partial);
-  se_fc1_kernel<<<kSeFc1Blocks, 256, 0, s>>>(partial, nch, Cpad, C, nr, 1.0f / static_cast<float>(HW), w1, r_part);
-  se_fc2_scale_kernel<<<Cpad / 64, 256, 0, s>>>(r_part, kSeFc1Blocks, C, nr, b1, w2, b2, gate, w, rows, Cpad, w_hi, w_lo);
-  B2_CUDA(cudaGetLastError());
-  return 0;
+  if (se_squeeze_launch(in_hi, in_lo, 1, HW, Cpad, partial, s)) return -1;
+  return se_excite_launch(partial, 1, HW, Cpad, C, nr, r_part, w1, b1, w2, b2, 0, gate, w, rows, w_hi, w_lo, s);
 }
 
 }  // namespace b2

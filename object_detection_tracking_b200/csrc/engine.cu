@@ -96,6 +96,13 @@ struct GnOp {
   GnParams p;              // full-batch launch (its gamma / beta are loaded with the weights)
 };
 
+// The squeeze-excite of one SE-ResNet bottleneck (use_se): the dense weights "<name>/fc1/{W,b}" and "<name>/fc2/{W,b}".
+struct SeOp {
+  std::string name;        // block scope, e.g. "group1/block0"
+  int C = 0, nr = 0;       // 4 * ch_out gated channels, ch_out / 4 hidden units
+  float *w1 = nullptr, *b1 = nullptr, *w2 = nullptr, *b2 = nullptr;   // [C][nr], [nr], [nr][C], [C]
+};
+
 // Packing of a checkpoint weight into the [Cout_pad][K] operand (ConvLayer::layout).
 enum Layout {
   kHwio = 0,     // conv HWIO
@@ -123,6 +130,7 @@ struct b2_ctx {
   std::vector<std::unique_ptr<ConvLayer>> layers;
   std::vector<ConvLayer*> part_layers;        // layers of the forked phases 0-2 (they get per-part plans)
   std::vector<std::unique_ptr<GnOp>> gns;
+  std::vector<std::unique_ptr<SeOp>> ses;
   std::vector<Step> steps;
   StageMap stages;
   // geometry
@@ -188,7 +196,7 @@ Step& add_batch_step(b2_ctx* c, int phase, int kind, const std::string& name,
                      const std::function<int(int, int, cudaStream_t)>& launch, int launches = 1) {
   static const char* kKindNames[] = {"conv", "stem_pack", "maxpool", "p6_subsample", "rpn_proposals", "roialign_proposals",
                                      "head_post", "roialign_final", "roialign_mask", "mask_select", "gn_stats", "gn_apply",
-                                     "gn_roi"};
+                                     "gn_roi", "se_squeeze", "se_excite", "se_apply"};
   const int B = c->cfg.batch;
   Step& s = add_step(c->steps, phase, kind, name.empty() ? kKindNames[kind] : name,
                      [launch, B](cudaStream_t st) { return launch(0, B, st); }, 0, 0, launches);
@@ -323,6 +331,66 @@ int add_gn(b2_ctx* c, int phase, const std::string& name, const Planes& buf, int
   return 0;
 }
 
+// Squeeze-excite of the bottleneck `name` (nn.py:506-519) on its conv3 output `buf`, then relu(buf * gate + res) in place
+// (nn.py:520-521, 586-587): a squeeze step (per-image channel sums), an excite step (fc1 + ReLU, fc2 + sigmoid -> gate
+// [B][C]) and an apply step through GroupNorm's apply path.  Every image has its own scratch, so the per-part launches of
+// the forked phases never share a buffer and an image's gate does not depend on its batch.
+int add_se(b2_ctx* c, int phase, const std::string& name, const Planes& buf, const Planes& res) {
+  std::unique_ptr<SeOp> S(new SeOp());
+  S->name = name;
+  S->C = buf.C;
+  S->nr = buf.C / 16;                                 // ch_out // 4 with C = 4 * ch_out
+  const int B = buf.B, C = S->C, nr = S->nr, HW = buf.H * buf.W, nch = se_chunks(HW);
+  B2_CHECK(nr >= 1 && nr <= se_max_nr(), "b2_create: squeeze-excite width out of range (" + name + ")");
+  S->w1 = c->arena.alloc<float>(static_cast<size_t>(C) * nr);
+  S->b1 = c->arena.alloc<float>(nr);
+  S->w2 = c->arena.alloc<float>(static_cast<size_t>(nr) * C);
+  S->b2 = c->arena.alloc<float>(C);
+  float* partial = c->arena.alloc<float>(static_cast<size_t>(B) * nch * C);
+  float* r_part = c->arena.alloc<float>(static_cast<size_t>(B) * se_fc1_parts() * se_max_nr());
+  float* gate = c->arena.alloc<float>(static_cast<size_t>(B) * C);
+  B2_CHECK(S->w1 && S->b1 && S->w2 && S->b2 && partial && r_part && gate, "out of device memory (squeeze-excite " + name + ")");
+  GnParams base;
+  memset(&base, 0, sizeof(base));
+  base.H = buf.H; base.W = buf.W; base.C = C;
+  base.pitch_H = buf.H; base.pitch_W = buf.W; base.ld = C;
+  base.res_H = res.H; base.res_W = res.W; base.res_ld = res.C;
+  base.relu = 1;
+  base.chunks = gn_chunks(buf.H, buf.W, C);
+  base.range_flag = c->range_flag;
+  const SeOp* se = S.get();
+  c->ses.push_back(std::move(S));
+  const Planes x = buf, r = res;
+  const double esz = c->split ? 4.0 : 2.0;
+  const double n = static_cast<double>(B) * HW * C;
+  const std::string dims = " [" + std::to_string(buf.H) + "x" + std::to_string(buf.W) + "x" + std::to_string(C);
+  add_batch_step(c, phase, 13, name + "/se squeeze" + dims + "]", [x, partial, nch, C](int b0, int nb, cudaStream_t st) {
+    const Planes xs = x.images(b0, nb);
+    return se_squeeze_launch(xs.hi, xs.lo, nb, xs.H * xs.W, C, partial + static_cast<size_t>(b0) * nch * C, st);
+  }).bytes = n * esz;
+  c->steps.back().flops = n;
+  const size_t rp_img = static_cast<size_t>(se_fc1_parts()) * se_max_nr();
+  add_batch_step(c, phase, 14, name + "/se excite [" + std::to_string(C) + "->" + std::to_string(nr) + "->" +
+                                   std::to_string(C) + "]",
+                 [se, partial, r_part, gate, nch, HW, rp_img](int b0, int nb, cudaStream_t st) {
+                   return se_excite_launch(partial + static_cast<size_t>(b0) * nch * se->C, nb, HW, se->C, se->C, se->nr,
+                                           r_part + b0 * rp_img, se->w1, se->b1, se->w2, se->b2, 1,
+                                           gate + static_cast<size_t>(b0) * se->C, nullptr, 0, nullptr, nullptr, st);
+                 }, 2).bytes = B * (static_cast<double>(nch) * C + 2.0 * C * nr + C) * 4.0;
+  c->steps.back().flops = B * (static_cast<double>(nch) * C + 4.0 * C * nr);
+  add_batch_step(c, phase, 15, name + "/se apply" + dims + " +res relu]", [base, x, r, gate](int b0, int nb, cudaStream_t st) {
+    GnParams p = base;
+    const Planes xs = x.images(b0, nb), rs = r.images(b0, nb);
+    p.x_hi = xs.hi; p.x_lo = xs.lo; p.y_hi = xs.hi; p.y_lo = xs.lo;
+    p.r_hi = rs.hi; p.r_lo = rs.lo;
+    p.gate = gate + static_cast<size_t>(b0) * p.C;
+    p.B = nb;
+    return se_apply_launch(p, st);
+  }).bytes = 3.0 * n * esz;
+  c->steps.back().flops = 3.0 * n;
+  return 0;
+}
+
 // generate_anchors.py:42-109 restated for one (stride, size): the 3 ratio anchors of a cell.
 void cell_anchors(float stride, float size, const float* ratios, float out[3][4]) {
   const double base = stride;
@@ -402,6 +470,7 @@ int build_plan(b2_ctx* c) {
   // use_gn (nn.py:859-862, 474-477): every backbone conv is a plain conv followed by GroupNorm steps that carry the ReLU
   // and the residual; with BatchNorm the norm, ReLU and residual are in the conv epilogue
   const bool gn = cfg.use_gn != 0;
+  const bool se = cfg.use_se != 0;   // squeeze-excite bottlenecks (nn.py:506-519)
   // conv0 as a 4x1 VALID conv over the packed operand (see stem.cu), BN + ReLU in the epilogue
   {
     Planes view = c->stem_u;
@@ -469,10 +538,13 @@ int build_plan(b2_ctx* c) {
         resid = &sc;
       }
       const Planes& out = pingpong[i & 1];
-      add_conv(c, 0, p + "/conv3", *a2, a2->H, a2->W, 1, 1, 1, 0, 0, 0, 0, feat * 4, !gn, false, !gn, out, 0, 0,
-               gn ? nullptr : resid, 0);
-      // relu(gn(conv3) + shortcut) (nn.py:512-521, 586-587)
-      if (gn && add_gn(c, 0, p + "/conv3/gn", out, out.H, out.W, 0, 0, resid, 0, true)) return -1;
+      // relu(norm(conv3) + shortcut) (nn.py:512-521, 586-587): with BatchNorm in the conv epilogue, with GroupNorm in its
+      // apply step; with use_se the norm alone, then the gate, the shortcut and the ReLU in the SE apply step
+      const bool epi = !gn && !se;
+      add_conv(c, 0, p + "/conv3", *a2, a2->H, a2->W, 1, 1, 1, 0, 0, 0, 0, feat * 4, !gn, false, epi, out, 0, 0,
+               epi ? resid : nullptr, 0);
+      if (gn && add_gn(c, 0, p + "/conv3/gn", out, out.H, out.W, 0, 0, se ? nullptr : resid, 0, !se)) return -1;
+      if (se && add_se(c, 0, p, out, *resid)) return -1;
       cur = out;
     }
     c->cfeat[g] = cur;
@@ -876,6 +948,23 @@ int load_gn(b2_ctx* c, GnOp* G, const WeightSet& ws) {
   return 0;
 }
 
+// dense "<block>/fc1" and "<block>/fc2" (nn.py:509-514, dense nn.py:730-774): W [in, out] row-contiguous, b [out]
+int load_se(b2_ctx* c, SeOp* S, const WeightSet& ws) {
+  const int C = S->C, nr = S->nr;
+  const struct { const char* suffix; int64_t n; float* dst; } parts[] = {
+      {"/fc1/W", static_cast<int64_t>(C) * nr, S->w1}, {"/fc1/b", nr, S->b1},
+      {"/fc2/W", static_cast<int64_t>(nr) * C, S->w2}, {"/fc2/b", C, S->b2}};
+  for (const auto& e : parts) {
+    const float* h = ws.get(S->name + e.suffix, e.n);
+    if (!h) return -1;
+    for (int64_t i = 0; i < e.n; ++i)
+      B2_CHECK(std::isfinite(h[i]), "squeeze-excite " + S->name + e.suffix + ": not finite");
+    B2_CUDA(cudaMemcpyAsync(e.dst, h, e.n * sizeof(float), cudaMemcpyHostToDevice, c->stream));
+  }
+  B2_CUDA(cudaStreamSynchronize(c->stream));
+  return 0;
+}
+
 }  // namespace
 
 // =================================================================================================
@@ -942,6 +1031,8 @@ int b2_load_weights(b2_ctx* c, const char* const* names, const float* const* dat
     if (load_layer(c, L.get(), ws)) return -1;
   for (auto& G : c->gns)
     if (load_gn(c, G.get(), ws)) return -1;
+  for (auto& S : c->ses)
+    if (load_se(c, S.get(), ws)) return -1;
   c->weights_loaded = true;
   return 0;
 }

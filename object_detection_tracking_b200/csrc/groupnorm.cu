@@ -13,6 +13,8 @@
 //                    only, in place or not, with the conv kernel's fp16 range monitor.
 //   gn_roi_kernel    grid (rois).  The box head's per-ROI GroupNorm: one 7x7xC sample fits on chip, so statistics and
 //                    apply run in one block.
+//   se_apply_kernel  grid (chunks, B).  The SE-ResNet bottleneck's gate (use_se) through the same apply: the table is
+//                    inv = gate[b][c] (from effnet.cu's squeeze-excite kernels), shift = 0.
 // The chunking of an image depends only on its geometry (gn_chunks), and chunks and threads are merged in a fixed order, so
 // the result for an image does not depend on the batch it is in: half-batch launches are bit-identical to full ones.
 #include <algorithm>
@@ -219,6 +221,21 @@ __global__ void __launch_bounds__(kGnThreads) gn_apply_kernel(GnParams p) {
   apply_range(p, b, HW * chunk / p.chunks, HW * (chunk + 1) / p.chunks, s_inv, s_shift);
 }
 
+// squeeze-excite gate of the SE-ResNet bottleneck (nn.py:506-519): the apply with inv = gate[b], shift = 0
+__global__ void __launch_bounds__(kGnThreads) se_apply_kernel(GnParams p) {
+  extern __shared__ float s_tab[];
+  float* s_inv = s_tab;
+  float* s_shift = s_tab + p.C;
+  const int b = blockIdx.y, chunk = blockIdx.x;
+  for (int c = threadIdx.x; c < p.C; c += kGnThreads) {
+    s_inv[c] = p.gate[static_cast<size_t>(b) * p.C + c];
+    s_shift[c] = 0.f;
+  }
+  __syncthreads();
+  const long long HW = static_cast<long long>(p.H) * p.W;
+  apply_range(p, b, HW * chunk / p.chunks, HW * (chunk + 1) / p.chunks, s_inv, s_shift);
+}
+
 template <int NSUB>
 __global__ void __launch_bounds__(kGnThreads) gn_roi_kernel(GnParams p) {
   __shared__ Moments s_part[kGnThreads * NSUB];
@@ -249,7 +266,7 @@ int check(const GnParams& p, const char* what) {
            std::string(what) + ": GroupNorm needs C in {64, 128, 256, 512, 1024, 2048} (32 groups, 16-byte loads)");
   B2_CHECK(p.ld % 8 == 0 && p.ld >= p.C && (p.r_hi == nullptr || p.res_ld % 8 == 0),
            std::string(what) + ": GroupNorm needs 16-byte aligned pixel strides");
-  B2_CHECK(p.B >= 1 && p.H >= 1 && p.W >= 1 && p.gamma && p.beta, std::string(what) + ": bad GroupNorm view");
+  B2_CHECK(p.B >= 1 && p.H >= 1 && p.W >= 1 && (p.gate || (p.gamma && p.beta)), std::string(what) + ": bad GroupNorm view");
   return 0;
 }
 
@@ -279,6 +296,14 @@ int gn_apply_launch(const GnParams& p, cudaStream_t s) {
   if (check(p, "gn_apply")) return -1;
   B2_CHECK(p.stats && p.chunks >= 1, "gn_apply: missing statistics");
   gn_apply_kernel<<<dim3(p.chunks, p.B), kGnThreads, 2 * p.C * sizeof(float), s>>>(p);
+  B2_CUDA(cudaGetLastError());
+  return 0;
+}
+
+int se_apply_launch(const GnParams& p, cudaStream_t s) {
+  if (check(p, "se_apply")) return -1;
+  B2_CHECK(p.gate && p.chunks >= 1, "se_apply: missing gate");
+  se_apply_kernel<<<dim3(p.chunks, p.B), kGnThreads, 2 * p.C * sizeof(float), s>>>(p);
   B2_CUDA(cudaGetLastError());
   return 0;
 }

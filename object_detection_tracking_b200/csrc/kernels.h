@@ -91,7 +91,8 @@ struct GnParams {
   int relu;                   // ReLU after the (normalise, residual) sum
   const float* gamma;         // [C]
   const float* beta;          // [C]
-  int chunks;                 // pixel chunks per image (gn_chunks): blocks per image of gn_stats / gn_apply
+  const float* gate;          // se_apply only: [B][C] per-image channel gate, y = x * gate[b][c] (+ residual) (ReLU)
+  int chunks;                 // pixel chunks per image (gn_chunks): blocks per image of gn_stats / gn_apply / se_apply
   float* partial;             // [B][chunks][32][3] (count, mean, M2) per chunk and group
   float* stats;               // [B][32][2] (mean, var) per image and group
   unsigned int* counter;      // [B] finished-chunk tickets, zero between launches
@@ -101,6 +102,9 @@ int gn_chunks(int H, int W, int C);
 int gn_stats_launch(const GnParams& p, cudaStream_t s);
 int gn_apply_launch(const GnParams& p, cudaStream_t s);
 int gn_roi_launch(const GnParams& p, cudaStream_t s);   // per sample statistics + apply in one kernel (7x7 ROI maps)
+// The squeeze-excite gate of the SE-ResNet bottleneck through GroupNorm's apply path (scale = p.gate[b], shift 0);
+// p.gamma / p.beta unused
+int se_apply_launch(const GnParams& p, cudaStream_t s);
 
 // reid.cu
 int dwconv3x3_launch(const __half* in_hi, const __half* in_lo, int B, int H, int W, int C, const float* w,
@@ -189,6 +193,13 @@ int se_max_nr();
 int se_gate_launch(const __half* in_hi, const __half* in_lo, int HW, int Cpad, int C, int nr, float* partial, float* r_part,
                    const float* w1, const float* b1, const float* w2, const float* b2, float* gate, const float* w, int rows,
                    __half* w_hi, __half* w_lo, cudaStream_t s);
+// The two halves of squeeze-excite over B images [B][HW][Cpad], every image with its own scratch: partial
+// [B][se_chunks(HW)][Cpad], r_part [B][se_fc1_parts()][se_max_nr()], gate [B][Cpad].  relu selects the hidden activation
+// (1 ReLU for the SE-ResNet bottleneck, 0 swish for MBConv); w == nullptr writes the gate only (no weight fold).
+int se_squeeze_launch(const __half* in_hi, const __half* in_lo, int B, int HW, int Cpad, float* partial, cudaStream_t s);
+int se_excite_launch(const float* partial, int B, int HW, int Cpad, int C, int nr, float* r_part, const float* w1,
+                     const float* b1, const float* w2, const float* b2, int relu, float* gate, const float* w, int rows,
+                     __half* w_hi, __half* w_lo, cudaStream_t s);
 
 // roialign.cu -- ROIAlign 7x7 on the detection's own level + mean over the 49 bins (efficientdet_wrapper.py:265-301)
 struct LevelRoiFeatParams {

@@ -1,4 +1,4 @@
-// Single-kernel entry points for parity tests and host tools: one conv, one GroupNorm, the frame resize.  Each call owns
+// Single-kernel entry points for parity tests and host tools: one conv, one GroupNorm, one squeeze-excite, the frame resize.  Each call owns
 // its device buffers in an Arena, so every return path frees them.
 #include <string.h>
 
@@ -124,6 +124,50 @@ int b2_op_group_norm(int device, const float* x, const float* res, const float* 
   }
   B2_CUDA(cudaDeviceSynchronize());
   return download_planes(yp.hi, yp.lo, n, out, nullptr);
+}
+
+int b2_op_squeeze_excite(int device, const float* x, const float* res, const float* w1, const float* b1, const float* w2,
+                         const float* b2, int B, int H, int W, int C, int nr, int split, float* out, float* gate_out) {
+  B2_CHECK(x && w1 && b1 && w2 && b2 && out, "b2_op_squeeze_excite: null argument");
+  B2_CHECK(B >= 1 && H >= 1 && W >= 1 && nr >= 1 && nr <= se_max_nr() && C >= 64 && C <= 2048 && (C & (C - 1)) == 0,
+           "b2_op_squeeze_excite: C must be a power of two from 64 to 2048 and nr at most se_max_nr()");
+  B2_CUDA(cudaSetDevice(device));
+  const size_t n = static_cast<size_t>(B) * H * W * C;
+  Arena a;
+  const Planes xp = a.planes(B, H, W, C, split != 0);
+  const Planes rp = res ? a.planes(B, H, W, C, split != 0) : Planes();
+  float* partial = a.alloc<float>(static_cast<size_t>(B) * se_chunks(H * W) * C);
+  float* r_part = a.alloc<float>(static_cast<size_t>(B) * se_fc1_parts() * se_max_nr());
+  float* gate = a.alloc<float>(static_cast<size_t>(B) * C);
+  float* dw1 = a.alloc<float>(static_cast<size_t>(C) * nr);
+  float* db1 = a.alloc<float>(nr);
+  float* dw2 = a.alloc<float>(static_cast<size_t>(nr) * C);
+  float* db2 = a.alloc<float>(C);
+  B2_CHECK(xp.hi && (!res || rp.hi) && partial && r_part && gate && dw1 && db1 && dw2 && db2,
+           "b2_op_squeeze_excite: out of device memory");
+  if (upload_planes(x, xp.hi, xp.lo, n, nullptr)) return -1;
+  if (res && upload_planes(res, rp.hi, rp.lo, n, nullptr)) return -1;
+  B2_CUDA(cudaMemcpy(dw1, w1, static_cast<size_t>(C) * nr * 4, cudaMemcpyHostToDevice));
+  B2_CUDA(cudaMemcpy(db1, b1, nr * 4, cudaMemcpyHostToDevice));
+  B2_CUDA(cudaMemcpy(dw2, w2, static_cast<size_t>(nr) * C * 4, cudaMemcpyHostToDevice));
+  B2_CUDA(cudaMemcpy(db2, b2, C * 4, cudaMemcpyHostToDevice));
+  GnParams p;
+  memset(&p, 0, sizeof(p));
+  p.x_hi = xp.hi; p.x_lo = xp.lo; p.y_hi = xp.hi; p.y_lo = xp.lo;
+  p.B = B; p.H = H; p.W = W; p.C = C;
+  p.pitch_H = H; p.pitch_W = W; p.ld = C;
+  if (res) { p.r_hi = rp.hi; p.r_lo = rp.lo; p.res_H = H; p.res_W = W; p.res_ld = C; }
+  p.relu = 1;
+  p.gate = gate;
+  p.chunks = gn_chunks(H, W, C);
+  if (se_squeeze_launch(xp.hi, xp.lo, B, H * W, C, partial, nullptr) ||
+      se_excite_launch(partial, B, H * W, C, C, nr, r_part, dw1, db1, dw2, db2, 1, gate, nullptr, 0, nullptr, nullptr,
+                       nullptr) ||
+      se_apply_launch(p, nullptr))
+    return -1;
+  B2_CUDA(cudaDeviceSynchronize());
+  if (gate_out) B2_CUDA(cudaMemcpy(gate_out, gate, static_cast<size_t>(B) * C * 4, cudaMemcpyDeviceToHost));
+  return download_planes(xp.hi, xp.lo, n, out, nullptr);
 }
 
 // The resize alone (parity tests): host uint8 [n, src_h, src_w, 3] -> host float32 [n, dst_h, dst_w, 3].

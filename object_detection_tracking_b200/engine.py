@@ -259,6 +259,28 @@ def op_group_norm(x, gamma, beta, view=None, res=None, res_shift=0, relu=False, 
     return out
 
 
+def op_squeeze_excite(x, w1, b1, w2, b2, res=None, split=True, device=0):
+    """The SE-ResNet bottleneck's squeeze-excite through the C ABI -- used by the kernel tests: x [B, H, W, C] NHWC,
+    dense w1 [C, nr], w2 [nr, C].  Returns (relu(x * gate[b] + res), gate [B, C])."""
+    lib = _lib.load()
+    x = np.ascontiguousarray(x, dtype=np.float32)
+    B, H, W, C = x.shape
+    w1 = np.ascontiguousarray(w1, dtype=np.float32)
+    nr = w1.shape[1]
+    assert w1.shape == (C, nr) and np.shape(w2) == (nr, C), (w1.shape, np.shape(w2))
+    r = None if res is None else np.ascontiguousarray(res, dtype=np.float32)
+    assert r is None or r.shape == x.shape, r.shape
+    out = np.empty_like(x)
+    gate = np.empty((B, C), dtype=np.float32)
+    _lib.check(lib.b2_op_squeeze_excite(device, _lib.ptr(x), _lib.ptr(r), _lib.ptr(w1),
+                                        _lib.ptr(np.ascontiguousarray(b1, np.float32)),
+                                        _lib.ptr(np.ascontiguousarray(w2, np.float32)),
+                                        _lib.ptr(np.ascontiguousarray(b2, np.float32)), B, H, W, C, nr, int(split),
+                                        _lib.ptr(out), _lib.ptr(gate)),
+               "b2_op_squeeze_excite")
+    return out, gate
+
+
 def get_new_hw(h, w, size, max_size):
     """nn.py:1548-1560: (neww, newh) of resizeImage for an h x w frame."""
     scale = size * 1.0 / min(h, w)

@@ -13,6 +13,7 @@ weights.  Names follow the Tensorpack-npz convention the reference loads
   fastrcnn/fc6/{W,b}, fastrcnn/fc7/{W,b}, fastrcnn/outputs/{class,box}/{W,b}
   use_gn: <conv scope>/gn/{gamma,beta} instead of bn/..., fpn/gn_c{2..5}/.., fpn/gn_p{2..5}/..
   use_conv_frcnn_head: fastrcnn/conv{0..3}/{W,b} (+ fastrcnn/gn{0..3}/.. with use_gn), fastrcnn/fc/{W,b}
+  use_se: group{0..3}/block{i}/fc1/{W,b}, fc2/{W,b} (squeeze-excite dense layers)
 
 Conv kernels are HWIO (`nn.py:350,367`), dense kernels [in,out] (`nn.py:753`).
 The distributions are chosen so activations stay O(1) through 33 residual blocks
@@ -113,7 +114,23 @@ def synth_weights(cfg, seed: int = 1234) -> dict:
         fin = hd * 7 * 7
         w["fastrcnn/fc/W"] = (rng.standard_normal((fin, dim)) * np.sqrt(2.0 / fin)).astype(np.float32)
         w["fastrcnn/fc/b"] = (rng.standard_normal(dim) * 0.02).astype(np.float32)
+    # The squeeze-excite variables come last, so every other array of a seed is the same with and without use_se.
+    if getattr(cfg, "use_se", False):                # resnet_bottleneck's fc1 / fc2 (nn.py:506-519)
+        for p, c in _se_blocks(cfg):
+            # channel means of conv3's BN output are O(0.1): fc1's gain and bias keep most hidden units live and
+            # image-dependent; fc2's bias spread puts the gates around 0.2-0.8 (saturated gates would make parity vacuous)
+            nr = c // 16
+            w[p + "/fc1/W"] = (rng.standard_normal((c, nr)) * np.sqrt(8.0 / c)).astype(np.float32)
+            w[p + "/fc1/b"] = rng.uniform(0.0, 0.1, nr).astype(np.float32)
+            w[p + "/fc2/W"] = (rng.standard_normal((nr, c)) * np.sqrt(2.0 / nr)).astype(np.float32)
+            w[p + "/fc2/b"] = (rng.standard_normal(c) * 0.4).astype(np.float32)
     return w
+
+
+def _se_blocks(cfg):
+    """(block scope, gated channels 4 * ch_out) of every bottleneck, in graph order."""
+    return [("group%d/block%d" % (g, i), feat * 4)
+            for g, (feat, count) in enumerate(zip((64, 128, 256, 512), cfg.resnet_num_block)) for i in range(count)]
 
 
 def _gn(rng, w, name, c, gamma_lo=0.8, gamma_hi=1.2):
@@ -170,6 +187,12 @@ def frcnn_weight_shapes(cfg) -> dict:
                 conv(p + "/convshortcut", 1, cin, feat * 4)
                 bn(p + "/convshortcut", feat * 4)
             cin = feat * 4
+    if getattr(cfg, "use_se", False):                # dense fc1 / fc2 of every bottleneck (nn.py:509-514, 762)
+        for p, c in _se_blocks(cfg):
+            sh[p + "/fc1/W"] = (c, c // 16)
+            sh[p + "/fc1/b"] = (c // 16,)
+            sh[p + "/fc2/W"] = (c // 16, c)
+            sh[p + "/fc2/b"] = (c,)
     nc = cfg.fpn_num_channel
     for i, c in enumerate((256, 512, 1024, 2048)):
         conv("fpn/lateral_1x1_c%d" % (i + 2), 1, c, nc, bias=True)
