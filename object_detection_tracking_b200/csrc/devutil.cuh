@@ -5,9 +5,10 @@
 
 namespace b2 {
 
-// Monotone map float -> uint32 (larger float => larger key); -0.0 < +0.0 is harmless here.
+// Monotone map float -> uint32 (larger float => larger key).  -0.0 and +0.0 give one key, so that equal scores of either
+// sign tie by index as in tf.nn.top_k (a bare f + 0.f could be folded away, so the select is explicit).
 __device__ __forceinline__ uint32_t float_key(float f) {
-  const uint32_t u = __float_as_uint(f);
+  const uint32_t u = f == 0.f ? 0u : __float_as_uint(f);
   return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
 }
 

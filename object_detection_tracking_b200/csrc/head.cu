@@ -144,7 +144,9 @@ int head_post_launch(const HeadPostParams& p, cudaStream_t s) {
   const int total = p.B * R;
   head_decode_kernel<<<(total + 127) / 128, 128, 0, s>>>(p);
   B2_CUDA(cudaGetLastError());
-  const int KP = next_pow2(R);
+  // at least 2 keys, so that the float4 boxes after the 8-byte keys start 16-byte aligned (one ROI per image would put
+  // them at 8)
+  const int KP = next_pow2(R) < 2 ? 2 : next_pow2(R);
   const size_t smem1 = static_cast<size_t>(KP) * (8 + 16 + 4 + 4) + static_cast<size_t>(R) * ((R + 31) / 32) * 4;
   const int KP2 = next_pow2(nc1 * p.max_per_class);
   const size_t smem2 = static_cast<size_t>(KP2) * 8;

@@ -307,7 +307,8 @@ int next_pow2(int v) {
 
 int rpn_proposals_launch(const RpnParams& p, cudaStream_t s) {
   B2_CHECK(p.topk >= 1 && p.topk <= 1024, "rpn: post-NMS top-k must be in [1, 1024]");
-  const int KP = next_pow2(p.topk);
+  // at least 2 keys, so that the float4 boxes after the 8-byte keys start 16-byte aligned (top-k 1 would put them at 8)
+  const int KP = std::max(2, next_pow2(p.topk));
   const int words = (p.topk + 31) / 32;
   const size_t smem1 = static_cast<size_t>(KP) * (8 + 16 + 4 + 4) + static_cast<size_t>(p.topk) * words * 4;
   const int KP2 = next_pow2(5 * p.topk);

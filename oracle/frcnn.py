@@ -182,6 +182,44 @@ def generate_rpn_proposals(boxes, scores, hw, cfg, topk):
     return b[keep], sc[keep]
 
 
+def level_proposals(cfg, level, cls, box, hw, multi=False):
+    """The proposals of one FPN level from its RPN outputs cls [fh,fw,A], box [fh,fw,A,4]: anchors, decode, then
+    generate_rpn_proposals (single-image graph) or, with `multi`, the batch graph's top-k + clip + hard NMS without the
+    min-size filter (nn.py:1431-1474).  Returns the kept (boxes [n,4], scores [n]) in selection order."""
+    fh, fw = cls.shape[:2]
+    anchors = get_all_anchors(cfg.anchor_strides[level], [cfg.anchor_sizes[level]], cfg.anchor_ratios,
+                              cfg.max_size)[:fh, :fw]
+    dec = decode_bbox_target(box, anchors, cfg.bbox_decode_clip).reshape(-1, 4)     # nn.py:1486-1514
+    K = cfg.rpn_test_post_nms_topk
+    if not multi:
+        return generate_rpn_proposals(dec, cls.reshape(-1), hw, cfg, K)
+    sc, idx = tf_ops.top_k(cls.reshape(-1), min(K, cls.size))                        # nn.py:1431
+    bx = clip_boxes(dec[idx], hw)                                                      # no min-size filter (:1441-1455)
+    ob, os_, n = combined_nms_single_class(bx, sc, K, cfg.rpn_proposal_nms_thres)
+    return ob[:n], os_[:n]
+
+
+def merge_level_proposals(levels, topk):
+    """generate_fpn_proposals (models.py:425-434), single-image graph: concatenate the levels' (boxes, scores) in level
+    order and keep the top-k by score (ties -> lower concatenated position)."""
+    pb = np.concatenate([b for b, _ in levels], 0); ps = np.concatenate([s for _, s in levels], 0)
+    ps, ti = tf_ops.top_k(ps, min(ps.shape[0], topk))
+    return pb[ti], ps
+
+
+def merge_level_proposals_multi(levels, topk):
+    """The batch graph's merge (models.py:2490-2520): every level zero-padded to topk (box 0, score 0), top-k by score --
+    so the padding outranks negative logits --, then zero-area boxes dropped."""
+    cb = np.zeros((len(levels) * topk, 4), np.float32); cs = np.zeros((len(levels) * topk,), np.float32)
+    for i, (b, s) in enumerate(levels):
+        cb[i * topk:i * topk + len(s)] = b; cs[i * topk:i * topk + len(s)] = s
+    ps, ti = tf_ops.top_k(cs, min(cs.shape[0], topk))
+    pb = cb[ti]
+    area = ((pb[:, 3] - pb[:, 1]) * (pb[:, 2] - pb[:, 0])).astype(np.float32)
+    keep = area > 0                                                                    # models.py:2516-2520
+    return pb[keep], ps[keep]
+
+
 def fpn_map_rois_to_levels(boxes):
     """models.py:439-461: level = floor(4 + log(sqrt(area)/224 + 1e-6)/log 2), clamp 2..5."""
     f32 = np.float32
@@ -270,6 +308,37 @@ def fastrcnn_predictions(boxes, probs, cfg):
     return sel[ti][:, ::-1].copy(), tp
 
 
+def fastrcnn_predictions_multi(boxes, probs, cfg):
+    """The batch graph's combined NMS over classes (models.py:2924-2976): per class hard NMS (<= result_per_im), no score
+    threshold, merge, sort by score, keep result_per_im.  Canonical tie order: (class, selection order).  Same returns
+    as fastrcnn_predictions."""
+    R = cfg.result_per_im
+    cand = []
+    for c in range(boxes.shape[1]):
+        keep = tf_ops.non_max_suppression(boxes[:, c], probs[:, c + 1], R, cfg.fastrcnn_nms_iou_thres)
+        cand += [(int(k), c) for k in keep]
+    if not cand:
+        return np.zeros((0, 2), np.int64), np.zeros((0,), np.float32)
+    cand = np.asarray(cand, dtype=np.int64)
+    sc = probs[cand[:, 0], cand[:, 1] + 1].astype(np.float32)
+    tp, ti = tf_ops.top_k(sc, min(R, len(cand)))
+    return cand[ti], tp
+
+
+def head_postprocess(cls_logits, box_logits, proposals, hw, cfg, multi=False):
+    """Inference decode of the box head (models.py:830-843) + fastrcnn_predictions (or, with `multi`, the batch graph's
+    combined NMS).  box_logits [K, num_class-1, 4] (class-agnostic already tiled).  Returns (decoded boxes [K,C-1,4],
+    probs [K,C], pred_indices [R,2] = (box_id, class_id), final probs [R])."""
+    nc1 = box_logits.shape[1]
+    anchors = np.tile(proposals[:, None, :], (1, nc1, 1))
+    rw = np.asarray(cfg.fastrcnn_bbox_reg_weights, dtype=np.float32)
+    dec = decode_bbox_target((box_logits / rw).astype(np.float32), anchors)   # default clip log(1333/16)
+    dec = clip_boxes(dec, hw)
+    probs = softmax(cls_logits)
+    pred, fprobs = (fastrcnn_predictions_multi if multi else fastrcnn_predictions)(dec, probs, cfg)
+    return dec, probs, pred, fprobs
+
+
 def maskrcnn_head(feat, W, num_class):
     """maskrcnn_up4conv_head (models.py:1173-1199): 4 x [conv3x3 SAME + bias + ReLU] on the [R,256,14,14] ROI features,
     Conv2DTranspose 2x2 stride 2 + bias + ReLU (nn.deconv2d, nn.py:383-413; TF kernel layout [kh, kw, out, in]),
@@ -312,32 +381,19 @@ def forward(cfg, W, img_hwc_f32: np.ndarray, stages: bool = True) -> dict:
             th = int(math.ceil(H * (1.0 / s))); tw = int(math.ceil(W_ * (1.0 / s)))
             p23456[i] = p23456[i][:, :, :th, :tw]
     na = len(cfg.anchor_ratios)
-    all_b, all_s, lvl_props = [], [], []
+    lvl_props = []
     rpn_out = []
-    for i, (s, size) in enumerate(zip(cfg.anchor_strides, cfg.anchor_sizes)):
+    for i in range(len(cfg.anchor_strides)):
         with torch.no_grad():
             cls, box = rpn_head(p23456[i], W, na)
-        fh, fw = cls.shape[:2]
-        anchors = get_all_anchors(s, [size], cfg.anchor_ratios, cfg.max_size)[:fh, :fw]
-        dec = decode_bbox_target(box, anchors, cfg.bbox_decode_clip)
-        b, sc = generate_rpn_proposals(dec.reshape(-1, 4), cls.reshape(-1), hw, cfg,
-                                       cfg.rpn_test_post_nms_topk)
-        all_b.append(b); all_s.append(sc); lvl_props.append((b, sc))
+        lvl_props.append(level_proposals(cfg, i, cls, box, hw))
         rpn_out.append((cls, box))
-    pb = np.concatenate(all_b, 0); ps = np.concatenate(all_s, 0)
-    ps, ti = tf_ops.top_k(ps, min(ps.shape[0], cfg.rpn_test_post_nms_topk))   # models.py:429-433
-    pb = pb[ti]
+    pb, ps = merge_level_proposals(lvl_props, cfg.rpn_test_post_nms_topk)
     feats = [_np(p[0]) for p in p23456[:4]]
     roi, roi_lvl = multilevel_roi_align(feats, pb, 7, cfg.anchor_strides)
     with torch.no_grad():
         cls_logits, box_logits, hidden = fastrcnn_head(roi, W, cfg)
-    nc1 = box_logits.shape[1]
-    anchors = np.tile(pb[:, None, :], (1, nc1, 1))
-    rw = np.asarray(cfg.fastrcnn_bbox_reg_weights, dtype=np.float32)
-    dec = decode_bbox_target((box_logits / rw).astype(np.float32), anchors)   # default clip log(1333/16)
-    dec = clip_boxes(dec, hw)
-    probs = softmax(cls_logits)
-    pred, fprobs = fastrcnn_predictions(dec, probs, cfg)
+    dec, probs, pred, fprobs = head_postprocess(cls_logits, box_logits, pb, hw, cfg)
     fboxes = dec[pred[:, 0], pred[:, 1]] if len(pred) else np.zeros((0, 4), np.float32)
     flabels = (pred[:, 1] + 1).astype(np.int64)
     if len(fboxes):
@@ -389,7 +445,6 @@ def forward_multi(cfg, W, imgs, stages=False):
     sized frames.  Returns zero-padded [B,100,...] outputs + valid counts + concatenated box features."""
     B = len(imgs)
     K, R = cfg.rpn_test_post_nms_topk, cfg.result_per_im
-    nc1 = cfg.num_class - 1
     out_boxes = np.zeros((B, R, 4), np.float32); out_probs = np.zeros((B, R), np.float32)
     out_labels = np.zeros((B, R), np.float32); valid = np.zeros((B,), np.int32)
     feats_all, per_image = [], []
@@ -403,42 +458,20 @@ def forward_multi(cfg, W, imgs, stages=False):
         for i, s in enumerate(cfg.anchor_strides):
             if i < 3:
                 p23456[i] = p23456[i][:, :, :int(math.ceil(H / float(s))), :int(math.ceil(W_ / float(s)))]
-        lvl_b, lvl_s = [], []
-        for i, (s, size) in enumerate(zip(cfg.anchor_strides, cfg.anchor_sizes)):
+        lvl = []
+        for i in range(len(cfg.anchor_strides)):
             with torch.no_grad():
                 cls, box = rpn_head(p23456[i], W, na)
-            fh, fw = cls.shape[:2]
-            anchors = get_all_anchors(s, [size], cfg.anchor_ratios, cfg.max_size)[:fh, :fw]
-            dec = decode_bbox_target(box, anchors, cfg.bbox_decode_clip).reshape(-1, 4)   # nn.py:1486-1514
-            sc, idx = tf_ops.top_k(cls.reshape(-1), min(K, cls.size))                      # nn.py:1431
-            bx = clip_boxes(dec[idx], hw)                                                  # no min-size filter (:1441-1455)
-            ob, os_, _ = combined_nms_single_class(bx, sc, K, cfg.rpn_proposal_nms_thres)
-            lvl_b.append(ob); lvl_s.append(os_)
-        cb = np.concatenate(lvl_b, 0); cs = np.concatenate(lvl_s, 0)                       # zero padded (models.py:2490-2496)
-        ps, ti = tf_ops.top_k(cs, min(cs.shape[0], K))
-        pb = cb[ti]
-        area = ((pb[:, 3] - pb[:, 1]) * (pb[:, 2] - pb[:, 0])).astype(np.float32)
-        keep = area > 0                                                                    # models.py:2516-2520
-        pb, ps = pb[keep], ps[keep]
+            lvl.append(level_proposals(cfg, i, cls, box, hw, multi=True))
+        pb, ps = merge_level_proposals_multi(lvl, K)
         fmaps = [_np(p[0]) for p in p23456[:4]]
         roi, _ = multilevel_roi_align(fmaps, pb, 7, cfg.anchor_strides)
         with torch.no_grad():
             cls_logits, box_logits, _ = fastrcnn_head(roi, W, cfg)
-        rw = np.asarray(cfg.fastrcnn_bbox_reg_weights, dtype=np.float32)
-        dec = clip_boxes(decode_bbox_target((box_logits / rw).astype(np.float32), np.tile(pb[:, None, :], (1, nc1, 1))), hw)
-        probs = softmax(cls_logits)
-        # combined NMS over classes (models.py:2924-2976): per class hard NMS (<= R), no score threshold,
-        # merge, sort by score, keep R.  Canonical tie order: (class, selection order).
-        cand = []
-        for c in range(nc1):
-            keep = tf_ops.non_max_suppression(dec[:, c], probs[:, c + 1], R, cfg.fastrcnn_nms_iou_thres)
-            cand += [(c, int(k)) for k in keep]
-        sc = np.array([probs[k, c + 1] for c, k in cand], np.float32)
-        tp, ti = tf_ops.top_k(sc, min(R, len(cand)))
-        n = len(ti)
+        dec, probs, pred, _ = head_postprocess(cls_logits, box_logits, pb, hw, cfg, multi=True)
+        n = len(pred)
         valid[b] = n
-        for j, t in enumerate(ti):
-            c, k = cand[t]
+        for j, (k, c) in enumerate(pred):
             out_boxes[b, j] = dec[k, c]; out_probs[b, j] = probs[k, c + 1]; out_labels[b, j] = c + 1
         bf, _ = multilevel_roi_align(fmaps, out_boxes[b, :n], 7, cfg.anchor_strides) if n else (np.zeros((0, 256, 7, 7), np.float32), None)
         feats_all.append(bf)
