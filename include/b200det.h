@@ -64,6 +64,9 @@ typedef struct b2_config {
   int32_t use_se;             /* --use_se (--version 6): squeeze-excite in every bottleneck (nn.py:506-519), per image:
                                  relu(conv3 * sigmoid(fc2(relu(fc1(mean_hw(conv3))))) + shortcut), weights
                                  "<block>/fc1/{W,b}" [4*ch, ch/4] and "<block>/fc2/{W,b}" [ch/4, 4*ch] */
+  int32_t use_resnext;        /* --use_resnext: ResNeXt 32x4d blocks (nn.py:524-549): conv1 1x1 -> 2*ch, conv2 3x3 2*ch -> 2*ch in
+                                 32 groups with SAME padding (weight [3,3,2*ch/32,2*ch]), conv3 1x1 -> 4*ch; no squeeze-excite
+                                 (use_se is ignored) */
 } b2_config;
 
 const char* b2_last_error(void);
@@ -327,6 +330,12 @@ int b2_op_group_norm(int device, const float* x, const float* res, const float* 
  * out = relu(x * gate[b][c] + res) in place (res [B][H][W][C], may be NULL).  gate_out [B][C] may be NULL. */
 int b2_op_squeeze_excite(int device, const float* x, const float* res, const float* w1, const float* b1, const float* w2,
                          const float* b2, int B, int H, int W, int C, int nr, int split, float* out, float* gate_out);
+/* Grouped conv (TF conv2d with C / groups input channels per filter, nn.py:352-355) of x [B][H][W][C] with the HWIO
+ * weight w [R][S][C/groups][C]: output channel o reads the input channels of its group o / (C/groups).  bias [C] and
+ * res [B][Ho][Wo][C] may be NULL; impl 0 = tensor cores (64-channel windows), 1 = CUDA cores (dense block-diagonal). */
+int b2_op_group_conv2d(int device, const float* x, const float* w, const float* bias, const float* res, int B, int H, int W,
+                       int C, int R, int S, int groups, int stride, int dil, int pad_t, int pad_b, int pad_l, int pad_r,
+                       int relu, int impl, int split, float* out);
 
 #ifdef __cplusplus
 }

@@ -43,6 +43,8 @@ _DEFAULTS = dict(
     conv_frcnn_head_dim=256,           # only main.py:250 sets it (default 256); the inference drivers never do
     use_se=False,                      # --use_se (obj_detect_tracking.py:192-193; set by --version 6, :278-280):
                                        # squeeze-excite in every bottleneck (nn.py:506-519)
+    use_resnext=False,                 # --use_resnext (obj_detect_tracking.py:196): ResNeXt 32x4d blocks with grouped
+                                       # 3x3 convs (nn.py:524-549, 864-868); the block has no SE branch
     use_partial_classes=False,
     is_efficientdet=False,
 )

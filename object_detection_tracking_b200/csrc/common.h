@@ -46,11 +46,20 @@ struct ConvDesc {
   int relu = 0;        // 0 none, 1 ReLU, 2 swish (x * sigmoid(x))
   int res_shift = 0;   // residual pixel = (p >> shift, q >> shift) in a res_H x res_W buffer
   int res_H = 0, res_W = 0, ldr = 0;
+  // grouped conv (ResNeXt's conv2, nn.py:352-355): groups > 1 splits Cin and Cout into that many equal ranges, output
+  // range g reading input range g only.  conv_tc takes Cin == Cout, Cin % 64 == 0 and groups of at most 64 channels that
+  // tile 64: output columns [n0, n0 + 64) then read input channels [n0, n0 + 64) only, and the weights are packed per
+  // 64-channel window, [Cout_pad][R*S*kGroupWindow] with the group blocks on each window's diagonal.  conv_simt reads the
+  // dense block-diagonal expansion [Cout_pad][R*S*Cin] and ignores `groups`.
+  int groups = 1;
   int Ho() const { return (in_H + pad_t + pad_b - ((R - 1) * dil + 1)) / stride + 1; }
   int Wo() const { return (in_W + pad_l + pad_r - ((S - 1) * dil + 1)) / stride + 1; }
 };
 
-// Packed weights of one conv: [Cout_pad][R*S*Cin] fp16 hi (+lo), fp32 bias[Cout_pad].
+constexpr int kGroupWindow = 64;   // input channels a grouped conv_tc layer's 64 output columns read (ConvDesc::groups)
+
+// Packed weights of one conv: [Cout_pad][R*S*Cin] fp16 hi (+lo) ([Cout_pad][R*S*kGroupWindow] for a grouped conv_tc
+// layer), fp32 bias[Cout_pad].
 struct ConvWeights {
   __half* w_hi = nullptr;
   __half* w_lo = nullptr;

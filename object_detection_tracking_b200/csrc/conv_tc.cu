@@ -65,6 +65,7 @@ struct ConvTcParams {
   int n_cols;        // Cout_pad: columns at or past it (the ragged last n-block) are not stored
   int num_n_blocks, num_tiles;
   int a_mode;        // 0 = A is a plain [M][Cin] matrix (2D tiled TMA), 1 = im2col TMA
+  int a_window;      // grouped conv (64-column tiles, one 64-channel block per tap): A reads input channels [n0, n0 + 64)
   uint32_t b_slot_bytes;   // one B plane of a stage in shared memory (block_n rows)
   uint32_t stage_bytes;    // shared-memory footprint of a stage
   uint32_t tx_bytes;       // bytes the TMA loads of a stage deliver (B boxes are clipped to Cout_pad rows)
@@ -306,6 +307,7 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
         cw = p.lower_w + qq * p.stride;
       }
       int tap = 0, cb = 0;   // K-block = (filter tap, 64-channel block)
+      const int c0 = p.a_window ? n0 : 0;   // first input channel of the K-blocks
       for (int kb = 0; kb < p.num_kb; ++kb) {
         mbar_wait(&empty_bar[stage], phase ^ 1);
         uint8_t* st = tiles + static_cast<size_t>(stage) * p.stage_bytes;
@@ -316,11 +318,11 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
             const int s = tap - r * p.S;
             const uint16_t ow = static_cast<uint16_t>(s * p.dil);
             const uint16_t oh = static_cast<uint16_t>(r * p.dil);
-            tma_load_im2col_4d(st, &tmA_hi, &full_bar[stage], cb * kBlockK, cw, ch, img, ow, oh);
-            if (SPLIT) tma_load_im2col_4d(st + a_lo_off, &tmA_lo, &full_bar[stage], cb * kBlockK, cw, ch, img, ow, oh);
+            tma_load_im2col_4d(st, &tmA_hi, &full_bar[stage], c0 + cb * kBlockK, cw, ch, img, ow, oh);
+            if (SPLIT) tma_load_im2col_4d(st + a_lo_off, &tmA_lo, &full_bar[stage], c0 + cb * kBlockK, cw, ch, img, ow, oh);
           } else {
-            tma_load_2d(st, &tmA_hi, &full_bar[stage], cb * kBlockK, m0);
-            if (SPLIT) tma_load_2d(st + a_lo_off, &tmA_lo, &full_bar[stage], cb * kBlockK, m0);
+            tma_load_2d(st, &tmA_hi, &full_bar[stage], c0 + cb * kBlockK, m0);
+            if (SPLIT) tma_load_2d(st + a_lo_off, &tmA_lo, &full_bar[stage], c0 + cb * kBlockK, m0);
           }
           tma_load_2d(st + b_hi_off, &tmB_hi, &full_bar[stage], kb * kBlockK, n0);
           if (SPLIT) tma_load_2d(st + b_lo_off, &tmB_lo, &full_bar[stage], kb * kBlockK, n0);
@@ -613,7 +615,11 @@ static int plan_build(ConvPlan* pl, const ConvDesc& d, const ConvWeights& w, con
   B2_CHECK(conv_tc_init() == 0, "conv_tc_init failed");
   B2_CHECK(d.Cin % kBlockK == 0, "conv_tc: Cin must be a multiple of 64");
   B2_CHECK(w.Cout_pad % 16 == 0, "conv_tc: Cout_pad must be a multiple of 16");
-  B2_CHECK(w.K == d.R * d.S * d.Cin, "conv_tc: packed weight K mismatch");
+  // grouped conv as block-diagonal 64-channel windows: a 64-column tile's outputs read only the same 64 input channels
+  const bool grouped = d.groups > 1;
+  B2_CHECK(!grouped || (d.Cin % d.groups == 0 && d.Cout == d.Cin && kGroupWindow % (d.Cin / d.groups) == 0),
+           "conv_tc: a grouped conv needs Cout == Cin and groups whose channel count divides 64");
+  B2_CHECK(w.K == d.R * d.S * (grouped ? kGroupWindow : d.Cin), "conv_tc: packed weight K mismatch");
   B2_CHECK(!split || (io.in_lo && w.w_lo), "conv_tc: split precision needs lo planes");
   ConvTcParams& p = pl->p;
   const int Ho = d.Ho(), Wo = d.Wo();
@@ -627,9 +633,10 @@ static int plan_build(ConvPlan* pl, const ConvDesc& d, const ConvWeights& w, con
   p.lower_h = -d.pad_t;
   p.lower_w = -d.pad_l;
   p.S = d.S;
-  p.cin_blocks = d.Cin / kBlockK;
+  p.cin_blocks = grouped ? 1 : d.Cin / kBlockK;
   p.num_kb = d.R * d.S * p.cin_blocks;
-  const int block_n = pick_block_n(w.Cout_pad);
+  p.a_window = grouped ? 1 : 0;
+  const int block_n = grouped ? kGroupWindow : pick_block_n(w.Cout_pad);
   const int b_rows = w.Cout_pad < block_n ? w.Cout_pad : block_n;   // rows of the B box (<= the tensor's)
   p.n_cols = w.Cout_pad;
   p.num_n_blocks = (w.Cout_pad + block_n - 1) / block_n;

@@ -112,6 +112,7 @@ enum Layout {
   kHeadOut = 4,  // fastrcnn/outputs/{class,box} fused along N
   kStem = 5,     // 7x7 stem re-indexed for the packed operand
   kDeconv = 6,   // mask-head transposed conv 2x2/2 as a 1x1 conv onto 4 taps x C outputs
+  kGrouped = 7,  // grouped conv HWIO [R][S][Cin/groups][Cout] (pack_grouped)
 };
 
 enum { NPHASE = 8 };
@@ -227,7 +228,7 @@ ConvIO images(const ConvLayer& L, int b0) {
 ConvLayer* add_conv(b2_ctx* c, int phase, const std::string& name, const Planes& in, int view_h, int view_w, int R,
                     int stride, int dil, int pt, int pb, int pl, int pr, int Cout, bool bn, bool bias, bool relu,
                     const Planes& out, int off_h, int off_w, const Planes* res, int res_shift, float* out_f32 = nullptr,
-                    int ldc_f32 = 0, int layout = kHwio, int S = 0, int in_ld = 0) {
+                    int ldc_f32 = 0, int layout = kHwio, int S = 0, int in_ld = 0, int groups = 1) {
   ConvDesc d;
   d.in_H = view_h; d.in_W = view_w; d.in_ld = in_ld;
   d.R = R; d.S = S > 0 ? S : R; d.stride = stride; d.dil = dil;
@@ -237,7 +238,10 @@ ConvLayer* add_conv(b2_ctx* c, int phase, const std::string& name, const Planes&
   d.acc_kb = c->cfg.accum_chunk;
   d.off_h = off_h; d.off_w = off_w;
   d.res_shift = res ? res_shift : 0;
-  std::unique_ptr<ConvLayer> L = make_conv(c->arena, c->split, name, d, in, out, res, out_f32, ldc_f32);
+  d.groups = groups;
+  // the CUDA-core kernel runs a grouped conv as the dense conv with block-diagonal weights
+  std::unique_ptr<ConvLayer> L =
+      make_conv(c->arena, c->split, name, d, in, out, res, out_f32, ldc_f32, c->cfg.conv_impl != 0);
   L->bn = bn ? name + "/bn" : "";
   L->bias = bias ? name + "/b" : "";
   L->layout = layout;
@@ -245,11 +249,12 @@ ConvLayer* add_conv(b2_ctx* c, int phase, const std::string& name, const Planes&
   ConvLayer* raw = L.get();
   c->layers.push_back(std::move(L));
   if (phase <= 2) c->part_layers.push_back(raw);
-  // algorithmic FLOPs and HBM bytes (each operand read once, output written once, at the stored precision)
+  // algorithmic FLOPs (a grouped conv's output reads Cin / groups channels per tap) and HBM bytes (each operand read
+  // once -- the weights as packed --, output written once, at the stored precision)
   const ConvDesc& e = raw->d;
   const double esz = c->split ? 4.0 : 2.0;
   const double M = static_cast<double>(e.B) * e.Ho() * e.Wo();
-  const double K = static_cast<double>(e.R) * e.S * e.Cin;
+  const double K = static_cast<double>(e.R) * e.S * e.Cin / e.groups;
   const double in_px = static_cast<double>(e.B) * e.in_H * e.in_W;
   const int conv_impl = c->cfg.conv_impl;
   const bool split = c->split;
@@ -264,7 +269,7 @@ ConvLayer* add_conv(b2_ctx* c, int phase, const std::string& name, const Planes&
   for (size_t h = 0; h < s.parts.size(); ++h)
     s.parts[h] = [raw, h](cudaStream_t st) { return conv_tc_launch(raw->part_plan[h].get(), st); };
   s.flops = 2.0 * M * K * e.Cout;
-  s.bytes = in_px * (e.in_ld > 0 && e.in_ld < e.Cin ? e.in_ld : e.Cin) * esz + K * e.Cout * esz +
+  s.bytes = in_px * (e.in_ld > 0 && e.in_ld < e.Cin ? e.in_ld : e.Cin) * esz + static_cast<double>(raw->w.K) * e.Cout * esz +
             M * e.Cout * (raw->io.out_f32 ? 4.0 : esz) + (raw->io.res_hi ? M * e.Cout * esz / (e.res_shift ? 4.0 : 1.0) : 0.0);
   return raw;
 }
@@ -470,7 +475,10 @@ int build_plan(b2_ctx* c) {
   // use_gn (nn.py:859-862, 474-477): every backbone conv is a plain conv followed by GroupNorm steps that carry the ReLU
   // and the residual; with BatchNorm the norm, ReLU and residual are in the conv epilogue
   const bool gn = cfg.use_gn != 0;
-  const bool se = cfg.use_se != 0;   // squeeze-excite bottlenecks (nn.py:506-519)
+  // ResNeXt 32x4d blocks (nn.py:524-549, chosen at :864-868): conv1 / conv2 at twice the width, conv2 grouped; the block
+  // has no squeeze-excite branch, so use_resnext overrides use_se
+  const bool rx = cfg.use_resnext != 0;
+  const bool se = cfg.use_se != 0 && !rx;   // squeeze-excite bottlenecks (nn.py:506-519)
   // conv0 as a 4x1 VALID conv over the packed operand (see stem.cu), BN + ReLU in the epilogue
   {
     Planes view = c->stem_u;
@@ -490,15 +498,16 @@ int build_plan(b2_ctx* c) {
   Planes cur = c->pool;
   for (int g = 0; g < 4; ++g) {
     const int feat = 64 << g, count = cfg.resnet_blocks[g];
+    const int mid = rx ? 2 * feat : feat;   // width of conv1 / conv2
     const int gh = c->ch[g], gw = c->cw[g];
     Planes pingpong[2];
     B2_CHECK(c->alloc_planes(pingpong[0], B, gh, gw, feat * 4), "alloc group out");
     B2_CHECK(c->alloc_planes(pingpong[1], B, gh, gw, feat * 4), "alloc group out");
     Planes t1_first, t1, t2, t2_first, sc;
-    B2_CHECK(c->alloc_planes(t1_first, B, cur.H, cur.W, feat), "alloc t1");
-    B2_CHECK(c->alloc_planes(t1, B, gh, gw, feat), "alloc t1");
-    B2_CHECK(c->alloc_planes(t2, B, gh, gw, feat), "alloc t2");
-    B2_CHECK(c->alloc_planes(t2_first, B, gh, gw, feat), "alloc t2");
+    B2_CHECK(c->alloc_planes(t1_first, B, cur.H, cur.W, mid), "alloc t1");
+    B2_CHECK(c->alloc_planes(t1, B, gh, gw, mid), "alloc t1");
+    B2_CHECK(c->alloc_planes(t2, B, gh, gw, mid), "alloc t2");
+    B2_CHECK(c->alloc_planes(t2_first, B, gh, gw, mid), "alloc t2");
     B2_CHECK(c->alloc_planes(sc, B, gh, gw, feat * 4), "alloc shortcut");
     for (int i = 0; i < count; ++i) {
       const std::string p = "group" + std::to_string(g) + "/block" + std::to_string(i);
@@ -507,21 +516,37 @@ int build_plan(b2_ctx* c) {
       const int dil = (g == 3 && cfg.use_dilations && in_last3) ? 2 : 1;
       const Planes& x = cur;
       const Planes& a1 = (i == 0) ? t1_first : t1;
-      add_conv(c, 0, p + "/conv1", x, x.H, x.W, 1, 1, 1, 0, 0, 0, 0, feat, !gn, false, !gn, a1, 0, 0, nullptr, 0);
+      add_conv(c, 0, p + "/conv1", x, x.H, x.W, 1, 1, 1, 0, 0, 0, 0, mid, !gn, false, !gn, a1, 0, 0, nullptr, 0);
       if (gn && add_gn(c, 0, p + "/conv1/gn", a1, a1.H, a1.W, 0, 0, nullptr, 0, true)) return -1;
       const Planes* a2 = &t2;
-      if (stride == 2) {
+      if (rx) {
+        // 3x3 split=32, padding SAME (nn.py:537-540): TF pads the total (out - 1) * stride + (3 - 1) * dil + 1 - in
+        // with the odd element at the bottom / right (SURVEY Appendix B) -- at stride 2 on the even sizes here 0 / 1,
+        // with dilation 2 then 1 / 2 -- and nothing follows the conv (no [1,0] pad, no output offset)
+        if (stride == 2) a2 = &t2_first;
+        int pad[4];   // top, bottom, left, right
+        for (int k = 0; k < 2; ++k) {
+          const int n = k == 0 ? a1.H : a1.W, o = (n + stride - 1) / stride;
+          const int total = std::max((o - 1) * stride + 2 * dil + 1 - n, 0);
+          pad[2 * k] = total / 2;
+          pad[2 * k + 1] = total - total / 2;
+        }
+        ConvLayer* L2 = add_conv(c, 0, p + "/conv2", a1, a1.H, a1.W, 3, stride, dil, pad[0], pad[1], pad[2], pad[3], mid,
+                                 !gn, false, !gn, *a2, 0, 0, nullptr, 0, nullptr, 0, kGrouped, 0, 0, 32);
+        B2_CHECK(L2->d.Ho() == a2->H && L2->d.Wo() == a2->W, "b2_create: ResNeXt conv2 output does not match its group");
+        if (gn && add_gn(c, 0, p + "/conv2/gn", *a2, a2->H, a2->W, 0, 0, nullptr, 0, true)) return -1;
+      } else if (stride == 2) {
         // pad [1,0] + 3x3 stride-2 VALID (nn.py:487-492); with dilation the output is padded [1,0] again
         // (nn.py:493-497): written at offset (1,1) of a buffer whose first row/col stay zero.  GroupNorm + ReLU run
         // before that pad (nn.py:490-497): their view is the conv output, so the pad row / column stay out of the
         // statistics and stay 0.
         a2 = &t2_first;
         const int off = dil != 1 ? 1 : 0;
-        ConvLayer* L2 = add_conv(c, 0, p + "/conv2", a1, a1.H, a1.W, 3, 2, dil, 1, 0, 1, 0, feat, !gn, false, !gn, *a2, off,
+        ConvLayer* L2 = add_conv(c, 0, p + "/conv2", a1, a1.H, a1.W, 3, 2, dil, 1, 0, 1, 0, mid, !gn, false, !gn, *a2, off,
                              off, nullptr, 0);
         if (gn && add_gn(c, 0, p + "/conv2/gn", *a2, L2->d.Ho(), L2->d.Wo(), off, off, nullptr, 0, true)) return -1;
       } else {
-        add_conv(c, 0, p + "/conv2", a1, a1.H, a1.W, 3, 1, dil, dil, dil, dil, dil, feat, !gn, false, !gn, *a2, 0,
+        add_conv(c, 0, p + "/conv2", a1, a1.H, a1.W, 3, 1, dil, dil, dil, dil, dil, mid, !gn, false, !gn, *a2, 0,
                  0, nullptr, 0);
         if (gn && add_gn(c, 0, p + "/conv2/gn", *a2, a2->H, a2->W, 0, 0, nullptr, 0, true)) return -1;
       }
@@ -864,6 +889,11 @@ int load_layer(b2_ctx* c, const ConvLayer* L, const WeightSet& ws) {
         for (int o = 0; o < Cout; ++o)
           packed[static_cast<size_t>(o) * K + static_cast<size_t>(t) * Cin + ci] = static_cast<float>(src[o] * scale[o]);
       }
+  } else if (L->layout == kGrouped) {
+    // ResNeXt conv2 (split=32): HWIO [R][S][Cin/groups][Cout], output o reading the input channels of its group
+    const float* w = ws.get(L->name + "/W", static_cast<int64_t>(R) * S * (Cin / L->d.groups) * Cout);
+    if (!w) return -1;
+    pack_grouped(w, R * S, Cin, Cout, L->d.groups, scale.data(), K, packed);
   } else if (L->layout == kDeconv) {
     // tf.layers.Conv2DTranspose kernel [kh=2, kw=2, out, in] (nn.py:402-412): output row (dy*2+dx)*out + o of the 1x1 conv
     const int co = Cout / 4;

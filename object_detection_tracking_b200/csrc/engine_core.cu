@@ -34,7 +34,8 @@ Planes Arena::planes(int B, int H, int W, int C, bool split, int creal) {
 }
 
 std::unique_ptr<ConvLayer> make_conv(Arena& a, bool split, const std::string& name, ConvDesc d, const Planes& in,
-                                     const Planes& out, const Planes* res, float* out_f32, int ldc_f32) {
+                                     const Planes& out, const Planes* res, float* out_f32, int ldc_f32,
+                                     bool dense_groups) {
   std::unique_ptr<ConvLayer> L(new ConvLayer());
   L->name = name;
   d.B = in.B; d.Cin = in.C;
@@ -49,7 +50,7 @@ std::unique_ptr<ConvLayer> make_conv(Arena& a, bool split, const std::string& na
   if (res) { d.res_H = res->H; d.res_W = res->W; d.ldr = res->C; }
   L->d = d;
   L->w.Cout_pad = (d.Cout + 15) / 16 * 16;
-  L->w.K = d.R * d.S * in.C;
+  L->w.K = d.R * d.S * (d.groups > 1 && !dense_groups ? kGroupWindow : in.C);
   L->w.w_hi = a.alloc<__half>(static_cast<size_t>(L->w.Cout_pad) * L->w.K);
   L->w.w_lo = split ? a.alloc<__half>(static_cast<size_t>(L->w.Cout_pad) * L->w.K) : nullptr;
   L->w.bias = a.alloc<float>(L->w.Cout_pad);
@@ -108,6 +109,23 @@ std::vector<float> fold_bias(const std::vector<double>& scale, const std::vector
   for (int o = 0; o < Cout; ++o)
     bias[o] = static_cast<float>(b ? shift[o] + static_cast<double>(b[o]) * scale[o] : shift[o]);
   return bias;
+}
+
+void pack_grouped(const float* w, int RS, int Cin, int Cout, int groups, const double* scale, int K,
+                  std::vector<float>& packed) {
+  const int cg = Cin / groups, cgo = Cout / groups;
+  const bool windowed = K != RS * Cin;
+  const int kc = windowed ? kGroupWindow : Cin;   // input channels per tap in the packed row
+  for (int o = 0; o < Cout; ++o) {
+    // first input channel of o's group, relative to the channels o's packed row covers
+    const int c0 = (o / cgo) * cg - (windowed ? o / kGroupWindow * kGroupWindow : 0);
+    for (int t = 0; t < RS; ++t)
+      for (int ci = 0; ci < cg; ++ci) {
+        const float v = w[(static_cast<size_t>(t) * cg + ci) * Cout + o];
+        packed[static_cast<size_t>(o) * K + static_cast<size_t>(t) * kc + c0 + ci] =
+            scale ? static_cast<float>(v * scale[o]) : v;
+      }
+  }
 }
 
 namespace {

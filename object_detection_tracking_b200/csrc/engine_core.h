@@ -75,10 +75,12 @@ struct ConvLayer {
 
 // Completes `d` for input `in` (d.in_H / d.in_W are the view, 0 = the whole buffer; d.in_ld 0 = in.C) writing `out`
 // planes, or fp32 rows of stride `ldc_f32` into `out_f32` when that is set, plus `res` when given, and allocates the packed
-// weights [Cout_pad][R*S*Cin].  Caller fills R, S, stride, dilation, pads, Cout, epilogue and placement in `d`.
+// weights [Cout_pad][R*S*Cin] (a grouped conv: [Cout_pad][R*S*kGroupWindow], or with `dense_groups` the dense
+// block-diagonal expansion the CUDA-core kernel reads).  Caller fills R, S, stride, dilation, pads, Cout, groups,
+// epilogue and placement in `d`.
 std::unique_ptr<ConvLayer> make_conv(Arena& a, bool split, const std::string& name, ConvDesc d, const Planes& in,
                                      const Planes& out, const Planes* res = nullptr, float* out_f32 = nullptr,
-                                     int ldc_f32 = 0);
+                                     int ldc_f32 = 0, bool dense_groups = false);
 // Creates the full-batch plan of every layer.
 int plan_convs(const std::vector<std::unique_ptr<ConvLayer>>& layers, bool split, int num_sms);
 
@@ -104,6 +106,12 @@ int fold_bn(const WeightSet& ws, const std::string& scope, const BnNames& nm, do
 // The epilogue bias of a conv whose output is BN(Wx + b): shift + b * scale (b may be null), Cout_pad entries.
 std::vector<float> fold_bias(const std::vector<double>& scale, const std::vector<double>& shift, const float* b, int Cout,
                              int Cout_pad);
+
+// A grouped conv's HWIO weight [R*S][Cin/groups][Cout], each output column o times scale[o] (scale may be null), into
+// `packed` [Cout_pad][K] (zero elsewhere): K = R*S*kGroupWindow packs each 64-column window's diagonal group blocks
+// (conv_tc), K = R*S*Cin the dense block-diagonal expansion (conv_simt).
+void pack_grouped(const float* w, int RS, int Cin, int Cout, int groups, const double* scale, int K,
+                  std::vector<float>& packed);
 
 // Packed fp32 weights [Cout_pad][K] -> the layer's operand planes (and w_master), bias -> the layer's bias.  Refuses a
 // weight the fp16 planes cannot represent and a non-finite bias.

@@ -1,5 +1,5 @@
-// Single-kernel entry points for parity tests and host tools: one conv, one GroupNorm, one squeeze-excite, the frame resize.  Each call owns
-// its device buffers in an Arena, so every return path frees them.
+// Single-kernel entry points for parity tests and host tools: one conv, one grouped conv, one GroupNorm, one squeeze-excite,
+// the frame resize.  Each call owns its device buffers in an Arena, so every return path frees them.
 #include <string.h>
 
 #include <algorithm>
@@ -10,6 +10,68 @@
 #include "kernels.h"
 
 using namespace b2;
+
+namespace {
+
+// Runs the conv `d` (input, geometry, epilogue and residual size filled in; output placement and strides set here) on
+// host x [B][H][W][Cin] with the packed weights pw [Cout_pad][K] and bias pb [Cout_pad]; res [B][res_H][res_W][Cout]
+// may be null.  Writes out [B][Ho][Wo][Cout].
+int run_conv(int device, ConvDesc d, const float* x, const std::vector<float>& pw, int K, const std::vector<float>& pb,
+             const float* res, int impl, int split, float* out, const char* who) {
+  const int Ho = d.Ho(), Wo = d.Wo(), Cout = d.Cout;
+  const int Cp = (Cout + 15) / 16 * 16;
+  d.out_H = Ho; d.out_W = Wo; d.ldc = Cp;
+  d.ldr = Cp;
+  const size_t nx = static_cast<size_t>(d.B) * d.in_H * d.in_W * d.Cin;
+  const size_t nw = static_cast<size_t>(Cp) * K, no = static_cast<size_t>(d.B) * Ho * Wo * Cp;
+  const size_t nr = static_cast<size_t>(d.B) * d.res_H * d.res_W * Cp;
+  std::vector<float> pr;
+  if (res) {
+    pr.assign(nr, 0.f);
+    for (size_t p = 0; p < static_cast<size_t>(d.B) * d.res_H * d.res_W; ++p)
+      for (int o = 0; o < Cout; ++o) pr[p * Cp + o] = res[p * Cout + o];
+  }
+  // every operand is converted to both planes; fp16 precision leaves the lo planes unused
+  Arena a;
+  __half *xh = a.alloc<__half>(nx), *xl = a.alloc<__half>(nx), *oh = a.alloc<__half>(no), *ol = a.alloc<__half>(no);
+  __half *rh = res ? a.alloc<__half>(nr) : nullptr, *rl = res ? a.alloc<__half>(nr) : nullptr;
+  ConvWeights cw;
+  cw.w_hi = a.alloc<__half>(nw);
+  cw.w_lo = a.alloc<__half>(nw);
+  cw.bias = a.alloc<float>(Cp);
+  B2_CHECK(xh && xl && oh && ol && (!res || (rh && rl)) && cw.w_hi && cw.w_lo && cw.bias,
+           std::string(who) + ": out of device memory");
+  cudaStream_t st = nullptr;
+  if (upload_planes(x, xh, xl, nx, st) || upload_planes(pw.data(), cw.w_hi, cw.w_lo, nw, st)) return -1;
+  if (res && upload_planes(pr.data(), rh, rl, nr, st)) return -1;
+  B2_CUDA(cudaMemcpy(cw.bias, pb.data(), Cp * 4, cudaMemcpyHostToDevice));
+  cw.Cout_pad = Cp; cw.K = K;
+  ConvIO io;
+  io.in_hi = xh; io.in_lo = split ? xl : nullptr;
+  io.out_hi = oh; io.out_lo = split ? ol : nullptr;
+  io.res_hi = rh; io.res_lo = split ? rl : nullptr;
+  if (!split) cw.w_lo = nullptr;
+  if (impl == 0) {
+    cudaDeviceProp prop;
+    B2_CUDA(cudaGetDeviceProperties(&prop, device));
+    PlanPtr plan(conv_tc_plan_create(d, cw, io, split != 0, prop.multiProcessorCount));
+    B2_CHECK(plan != nullptr, std::string(who) + ": " + last_error());
+    const int rc = conv_tc_launch(plan.get(), st);
+    const cudaError_t e = cudaDeviceSynchronize();   // the kernel is done before its plan goes away
+    if (rc) return -1;
+    B2_CUDA(e);
+  } else {
+    if (conv_simt_launch(d, cw, io, split != 0, st)) return -1;
+    B2_CUDA(cudaDeviceSynchronize());
+  }
+  std::vector<float> ho(no);
+  if (download_planes(oh, split ? ol : nullptr, no, ho.data(), st)) return -1;
+  for (size_t p = 0; p < static_cast<size_t>(d.B) * Ho * Wo; ++p)
+    for (int o = 0; o < Cout; ++o) out[p * Cout + o] = ho[p * Cp + o];
+  return 0;
+}
+
+}  // namespace
 
 extern "C" {
 
@@ -26,60 +88,39 @@ int b2_op_conv2d(int device, const float* x, const float* w, const float* bias, 
   const int Ho = d.Ho(), Wo = d.Wo();
   B2_CHECK(Ho > 0 && Wo > 0, "b2_op_conv2d: empty output");
   const int Cp = (Cout + 15) / 16 * 16;
-  d.out_H = Ho; d.out_W = Wo; d.ldc = Cp;
-  const int rH = res_shift ? (Ho + 1) / 2 : Ho, rW = res_shift ? (Wo + 1) / 2 : Wo;
-  d.res_H = rH; d.res_W = rW; d.ldr = Cp; d.res_shift = res_shift;
-  const size_t nx = static_cast<size_t>(B) * H * W * Cin, K = static_cast<size_t>(R) * S * Cin;
-  const size_t nw = static_cast<size_t>(Cp) * K, no = static_cast<size_t>(B) * Ho * Wo * Cp;
-  const size_t nr = static_cast<size_t>(B) * rH * rW * Cp;
+  d.res_H = res_shift ? (Ho + 1) / 2 : Ho; d.res_W = res_shift ? (Wo + 1) / 2 : Wo; d.res_shift = res_shift;
+  const size_t K = static_cast<size_t>(R) * S * Cin;
   // pack HWIO -> [Cout_pad][R*S*Cin]
-  std::vector<float> pw(nw, 0.f), pb(Cp, 0.f);
+  std::vector<float> pw(static_cast<size_t>(Cp) * K, 0.f), pb(Cp, 0.f);
   for (size_t k = 0; k < K; ++k)
     for (int o = 0; o < Cout; ++o) pw[static_cast<size_t>(o) * K + k] = w[k * Cout + o];
   if (bias) for (int o = 0; o < Cout; ++o) pb[o] = bias[o];
-  std::vector<float> pr;
-  if (res) {
-    pr.assign(nr, 0.f);
-    for (size_t p = 0; p < static_cast<size_t>(B) * rH * rW; ++p)
-      for (int o = 0; o < Cout; ++o) pr[p * Cp + o] = res[p * Cout + o];
-  }
-  // every operand is converted to both planes; fp16 precision leaves the lo planes unused
-  Arena a;
-  __half *xh = a.alloc<__half>(nx), *xl = a.alloc<__half>(nx), *oh = a.alloc<__half>(no), *ol = a.alloc<__half>(no);
-  __half *rh = res ? a.alloc<__half>(nr) : nullptr, *rl = res ? a.alloc<__half>(nr) : nullptr;
-  ConvWeights cw;
-  cw.w_hi = a.alloc<__half>(nw);
-  cw.w_lo = a.alloc<__half>(nw);
-  cw.bias = a.alloc<float>(Cp);
-  B2_CHECK(xh && xl && oh && ol && (!res || (rh && rl)) && cw.w_hi && cw.w_lo && cw.bias, "b2_op_conv2d: out of device memory");
-  cudaStream_t st = nullptr;
-  if (upload_planes(x, xh, xl, nx, st) || upload_planes(pw.data(), cw.w_hi, cw.w_lo, nw, st)) return -1;
-  if (res && upload_planes(pr.data(), rh, rl, nr, st)) return -1;
-  B2_CUDA(cudaMemcpy(cw.bias, pb.data(), Cp * 4, cudaMemcpyHostToDevice));
-  cw.Cout_pad = Cp; cw.K = static_cast<int>(K);
-  ConvIO io;
-  io.in_hi = xh; io.in_lo = split ? xl : nullptr;
-  io.out_hi = oh; io.out_lo = split ? ol : nullptr;
-  io.res_hi = rh; io.res_lo = split ? rl : nullptr;
-  if (!split) cw.w_lo = nullptr;
-  if (impl == 0) {
-    cudaDeviceProp prop;
-    B2_CUDA(cudaGetDeviceProperties(&prop, device));
-    PlanPtr plan(conv_tc_plan_create(d, cw, io, split != 0, prop.multiProcessorCount));
-    B2_CHECK(plan != nullptr, std::string("b2_op_conv2d: ") + last_error());
-    const int rc = conv_tc_launch(plan.get(), st);
-    const cudaError_t e = cudaDeviceSynchronize();   // the kernel is done before its plan goes away
-    if (rc) return -1;
-    B2_CUDA(e);
-  } else {
-    if (conv_simt_launch(d, cw, io, split != 0, st)) return -1;
-    B2_CUDA(cudaDeviceSynchronize());
-  }
-  std::vector<float> ho(no);
-  if (download_planes(oh, split ? ol : nullptr, no, ho.data(), st)) return -1;
-  for (size_t p = 0; p < static_cast<size_t>(B) * Ho * Wo; ++p)
-    for (int o = 0; o < Cout; ++o) out[p * Cout + o] = ho[p * Cp + o];
-  return 0;
+  return run_conv(device, d, x, pw, static_cast<int>(K), pb, res, impl, split, out, "b2_op_conv2d");
+}
+
+int b2_op_group_conv2d(int device, const float* x, const float* w, const float* bias, const float* res, int B, int H, int W,
+                       int C, int R, int S, int groups, int stride, int dil, int pad_t, int pad_b, int pad_l, int pad_r,
+                       int relu, int impl, int split, float* out) {
+  B2_CHECK(x && w && out, "b2_op_group_conv2d: null argument");
+  B2_CHECK(B >= 1 && C >= 1 && groups >= 1 && C % groups == 0, "b2_op_group_conv2d: groups must divide C");
+  B2_CHECK(impl != 0 || (C % kGroupWindow == 0 && kGroupWindow % (C / groups) == 0),
+           "b2_op_group_conv2d: the tensor-core windows need C % 64 == 0 and C / groups dividing 64");
+  B2_CUDA(cudaSetDevice(device));
+  ConvDesc d;
+  d.B = B; d.in_H = H; d.in_W = W; d.Cin = C; d.in_pitch_H = H; d.in_pitch_W = W; d.in_ld = C;
+  d.R = R; d.S = S; d.stride = stride; d.dil = dil;
+  d.pad_t = pad_t; d.pad_b = pad_b; d.pad_l = pad_l; d.pad_r = pad_r;
+  d.Cout = C; d.relu = relu; d.groups = groups;
+  const int Ho = d.Ho(), Wo = d.Wo();
+  B2_CHECK(Ho > 0 && Wo > 0, "b2_op_group_conv2d: empty output");
+  d.res_H = Ho; d.res_W = Wo;
+  const int Cp = (C + 15) / 16 * 16;
+  // the tensor-core kernel reads 64-channel windows, the CUDA-core kernel the dense block-diagonal expansion
+  const int K = R * S * (impl == 0 ? kGroupWindow : C);
+  std::vector<float> pw(static_cast<size_t>(Cp) * K, 0.f), pb(Cp, 0.f);
+  pack_grouped(w, R * S, C, C, groups, nullptr, K, pw);
+  if (bias) for (int o = 0; o < C; ++o) pb[o] = bias[o];
+  return run_conv(device, d, x, pw, K, pb, res, impl, split, out, "b2_op_group_conv2d");
 }
 
 int b2_op_group_norm(int device, const float* x, const float* res, const float* gamma, const float* beta, int B,

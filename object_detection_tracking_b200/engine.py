@@ -239,6 +239,30 @@ def op_conv2d(x, w, bias=None, res=None, stride=1, dil=1, pad=(0, 0, 0, 0), relu
     return out
 
 
+def op_group_conv2d(x, w, bias=None, res=None, stride=1, dil=1, pad=(0, 0, 0, 0), relu=False, impl="tcgen05",
+                    split=True, device=0) -> np.ndarray:
+    """Grouped convolution through the C ABI -- used by the kernel tests: x [B, H, W, C] NHWC, HWIO kernel
+    w [R, S, C / groups, C] (TF's grouped conv2d, nn.py:352-355), res [B, Ho, Wo, C]."""
+    lib = _lib.load()
+    x = np.ascontiguousarray(x, dtype=np.float32)
+    w = np.ascontiguousarray(w, dtype=np.float32)
+    B, H, W, C = x.shape
+    R, S, cg, Cout = w.shape
+    assert Cout == C and C % cg == 0, (w.shape, C)
+    pt, pb, pl, pr = pad
+    Ho = (H + pt + pb - ((R - 1) * dil + 1)) // stride + 1
+    Wo = (W + pl + pr - ((S - 1) * dil + 1)) // stride + 1
+    out = np.zeros((B, Ho, Wo, C), dtype=np.float32)
+    b = None if bias is None else np.ascontiguousarray(bias, dtype=np.float32)
+    r = None if res is None else np.ascontiguousarray(res, dtype=np.float32)
+    assert r is None or r.shape == out.shape, r.shape
+    _lib.check(lib.b2_op_group_conv2d(device, _lib.ptr(x), _lib.ptr(w), _lib.ptr(b), _lib.ptr(r), B, H, W, C, R, S,
+                                      C // cg, stride, dil, pt, pb, pl, pr, int(relu), {"tcgen05": 0, "simt": 1}[impl],
+                                      int(split), _lib.ptr(out)),
+               "b2_op_group_conv2d")
+    return out
+
+
 def op_group_norm(x, gamma, beta, view=None, res=None, res_shift=0, relu=False, per_roi=False, split=True,
                   in_place=True, device=0) -> np.ndarray:
     """GroupNorm (32 groups) of a NHWC buffer x [B, pitch_H, pitch_W, C] through the C ABI -- used by the kernel tests.

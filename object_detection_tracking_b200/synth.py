@@ -14,6 +14,7 @@ weights.  Names follow the Tensorpack-npz convention the reference loads
   use_gn: <conv scope>/gn/{gamma,beta} instead of bn/..., fpn/gn_c{2..5}/.., fpn/gn_p{2..5}/..
   use_conv_frcnn_head: fastrcnn/conv{0..3}/{W,b} (+ fastrcnn/gn{0..3}/.. with use_gn), fastrcnn/fc/{W,b}
   use_se: group{0..3}/block{i}/fc1/{W,b}, fc2/{W,b} (squeeze-excite dense layers)
+  use_resnext: conv1 / conv2 at twice the width, conv2/W [3, 3, 2*ch/32, 2*ch] (32 groups), no fc1 / fc2
 
 Conv kernels are HWIO (`nn.py:350,367`), dense kernels [in,out] (`nn.py:753`).
 The distributions are chosen so activations stay O(1) through 33 residual blocks
@@ -44,13 +45,14 @@ def synth_weights(cfg, seed: int = 1234) -> dict:
     _bn(rng, w, "conv0", 64)
     cin = 64
     for g, (feat, count) in enumerate(zip((64, 128, 256, 512), cfg.resnet_num_block)):
+        mid, cg = _block_widths(cfg, feat)
         for i in range(count):
             p = "group%d/block%d" % (g, i)
-            w[p + "/conv1/W"] = _conv_w(rng, 1, cin, feat)
-            _bn(rng, w, p + "/conv1", feat)
-            w[p + "/conv2/W"] = _conv_w(rng, 3, feat, feat)
-            _bn(rng, w, p + "/conv2", feat)
-            w[p + "/conv3/W"] = _conv_w(rng, 1, feat, feat * 4)
+            w[p + "/conv1/W"] = _conv_w(rng, 1, cin, mid)
+            _bn(rng, w, p + "/conv1", mid)
+            w[p + "/conv2/W"] = _conv_w(rng, 3, cg, mid)            # fan-in 9 * cg: a grouped filter sees cg channels
+            _bn(rng, w, p + "/conv2", mid)
+            w[p + "/conv3/W"] = _conv_w(rng, 1, mid, feat * 4)
             # residual-branch last BN: small gamma keeps the running sum bounded
             _bn(rng, w, p + "/conv3", feat * 4, 0.1, 0.3)
             if cin != feat * 4:
@@ -115,7 +117,7 @@ def synth_weights(cfg, seed: int = 1234) -> dict:
         w["fastrcnn/fc/W"] = (rng.standard_normal((fin, dim)) * np.sqrt(2.0 / fin)).astype(np.float32)
         w["fastrcnn/fc/b"] = (rng.standard_normal(dim) * 0.02).astype(np.float32)
     # The squeeze-excite variables come last, so every other array of a seed is the same with and without use_se.
-    if getattr(cfg, "use_se", False):                # resnet_bottleneck's fc1 / fc2 (nn.py:506-519)
+    if _use_se(cfg):                                 # resnet_bottleneck's fc1 / fc2 (nn.py:506-519)
         for p, c in _se_blocks(cfg):
             # channel means of conv3's BN output are O(0.1): fc1's gain and bias keep most hidden units live and
             # image-dependent; fc2's bias spread puts the gates around 0.2-0.8 (saturated gates would make parity vacuous)
@@ -125,6 +127,19 @@ def synth_weights(cfg, seed: int = 1234) -> dict:
             w[p + "/fc2/W"] = (rng.standard_normal((nr, c)) * np.sqrt(2.0 / nr)).astype(np.float32)
             w[p + "/fc2/b"] = (rng.standard_normal(c) * 0.4).astype(np.float32)
     return w
+
+
+def _block_widths(cfg, feat):
+    """(conv1 / conv2 width, input channels per conv2 filter) of a block with ch_out = feat: the ResNet bottleneck's
+    (feat, feat) (nn.py:478-497), or ResNeXt 32x4d's (2 * feat, 2 * feat / 32) (nn.py:532-540)."""
+    if getattr(cfg, "use_resnext", False):
+        return 2 * feat, 2 * feat // 32
+    return feat, feat
+
+
+def _use_se(cfg):
+    """use_se selects squeeze-excite in resnet_bottleneck only: the ResNeXt block has no SE branch (nn.py:524-549)."""
+    return getattr(cfg, "use_se", False) and not getattr(cfg, "use_resnext", False)
 
 
 def _se_blocks(cfg):
@@ -143,9 +158,10 @@ def _backbone_norm_scopes(cfg):
     out = [("conv0", 64, False)]
     cin = 64
     for g, (feat, count) in enumerate(zip((64, 128, 256, 512), cfg.resnet_num_block)):
+        mid = _block_widths(cfg, feat)[0]
         for i in range(count):
             p = "group%d/block%d" % (g, i)
-            out += [(p + "/conv1", feat, False), (p + "/conv2", feat, False), (p + "/conv3", feat * 4, True)]
+            out += [(p + "/conv1", mid, False), (p + "/conv2", mid, False), (p + "/conv3", feat * 4, True)]
             if cin != feat * 4:
                 out.append((p + "/convshortcut", feat * 4, False))
             cin = feat * 4
@@ -178,16 +194,17 @@ def frcnn_weight_shapes(cfg) -> dict:
     bn("conv0", 64)
     cin = 64
     for g, (feat, count) in enumerate(zip((64, 128, 256, 512), cfg.resnet_num_block)):
+        mid, cg = _block_widths(cfg, feat)
         for i in range(count):
             p = "group%d/block%d" % (g, i)
-            for name, k, ci, co in (("conv1", 1, cin, feat), ("conv2", 3, feat, feat), ("conv3", 1, feat, feat * 4)):
+            for name, k, ci, co in (("conv1", 1, cin, mid), ("conv2", 3, cg, mid), ("conv3", 1, mid, feat * 4)):
                 conv("%s/%s" % (p, name), k, ci, co)
                 bn("%s/%s" % (p, name), co)
             if cin != feat * 4:
                 conv(p + "/convshortcut", 1, cin, feat * 4)
                 bn(p + "/convshortcut", feat * 4)
             cin = feat * 4
-    if getattr(cfg, "use_se", False):                # dense fc1 / fc2 of every bottleneck (nn.py:509-514, 762)
+    if _use_se(cfg):                                 # dense fc1 / fc2 of every bottleneck (nn.py:509-514, 762)
         for p, c in _se_blocks(cfg):
             sh[p + "/fc1/W"] = (c, c // 16)
             sh[p + "/fc1/b"] = (c // 16,)
