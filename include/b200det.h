@@ -67,6 +67,10 @@ typedef struct b2_config {
   int32_t use_resnext;        /* --use_resnext: ResNeXt 32x4d blocks (nn.py:524-549): conv1 1x1 -> 2*ch, conv2 3x3 2*ch -> 2*ch in
                                  32 groups with SAME padding (weight [3,3,2*ch/32,2*ch]), conv3 1x1 -> 4*ch; no squeeze-excite
                                  (use_se is ignored) */
+  int32_t add_relation_nn;    /* --add_relation_nn: relation modules RM_r1 / RM_r2 in the 2fc box head (models.py:1044-1054,
+                                 nn.py:115-190): h1 = relu(fc6) + RM_r1(relu(fc6), proposals), h2 = relu(fc7(h1)) +
+                                 RM_r2(relu(fc7(h1)), proposals), each image's ROIs attending to its own proposals only;
+                                 ignored with conv_head_dim > 0 */
 } b2_config;
 
 const char* b2_last_error(void);
@@ -336,6 +340,14 @@ int b2_op_squeeze_excite(int device, const float* x, const float* res, const flo
 int b2_op_group_conv2d(int device, const float* x, const float* w, const float* bias, const float* res, int B, int H, int W,
                        int C, int R, int S, int groups, int stride, int dil, int pad_t, int pad_b, int pad_l, int pad_r,
                        int relu, int impl, int split, float* out);
+/* One relation module (relation_network nn.py:115-190, group 16, geo_feat_dim 64) as the box head runs it, per image:
+ * h [B][K][D] (host, fp32, converted to the engine's planes), boxes [B][K][4] (x1 y1 x2 y2), count [B] valid rows per
+ * image (0..K; rows j >= count[b] take no part), weights geo_emb W [4][64], b [64], geo_conv W [64][16] (the [1,1,64,16]
+ * kernel), b [16], query_linear W [D][D], key_linear W [D][D], output_linear W [16*D][D].
+ * out [B][K][D] = h + output_linear(softmax_j(log(max(wg, 1e-6)) + q.k / sqrt(D/16)) . h); rows i >= count[b] are h. */
+int b2_op_relation(int device, const float* h, const float* boxes, const int32_t* count, const float* geo_emb_w,
+                   const float* geo_emb_b, const float* geo_conv_w, const float* geo_conv_b, const float* query_w,
+                   const float* key_w, const float* output_w, int B, int K, int D, int split, float* out);
 
 #ifdef __cplusplus
 }

@@ -45,6 +45,8 @@ _DEFAULTS = dict(
                                        # squeeze-excite in every bottleneck (nn.py:506-519)
     use_resnext=False,                 # --use_resnext (obj_detect_tracking.py:196): ResNeXt 32x4d blocks with grouped
                                        # 3x3 convs (nn.py:524-549, 864-868); the block has no SE branch
+    add_relation_nn=False,             # --add_relation_nn (obj_detect_tracking.py:226): relation modules RM_r1 / RM_r2 in
+                                       # the 2fc box head (models.py:1044-1054, nn.py:115-190); not with the conv head
     use_partial_classes=False,
     is_efficientdet=False,
 )

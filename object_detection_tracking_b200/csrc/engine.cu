@@ -103,6 +103,12 @@ struct SeOp {
   float *w1 = nullptr, *b1 = nullptr, *w2 = nullptr, *b2 = nullptr;   // [C][nr], [nr], [nr][C], [C]
 };
 
+// The geometry weights of one relation module (add_relation_nn): "<scope>/geo_emb/{W,b}", "<scope>/geo_conv/{W,b}".
+struct RelOp {
+  std::string name;        // module scope, "fastrcnn/RM_r1" or "fastrcnn/RM_r2"
+  float* geo = nullptr;    // kRelGeoWeights (relation_upload_geo)
+};
+
 // Packing of a checkpoint weight into the [Cout_pad][K] operand (ConvLayer::layout).
 enum Layout {
   kHwio = 0,     // conv HWIO
@@ -113,6 +119,8 @@ enum Layout {
   kStem = 5,     // 7x7 stem re-indexed for the packed operand
   kDeconv = 6,   // mask-head transposed conv 2x2/2 as a 1x1 conv onto 4 taps x C outputs
   kGrouped = 7,  // grouped conv HWIO [R][S][Cin/groups][Cout] (pack_grouped)
+  kRelQK = 8,    // relation module: <scope>/query_linear/W | <scope>/key_linear/W fused along N (relation_pack_qk)
+  kRuntime = 9,  // relation module P.V: the weights are the image's V^T, written by the attention step every pass
 };
 
 enum { NPHASE = 8 };
@@ -132,6 +140,7 @@ struct b2_ctx {
   std::vector<ConvLayer*> part_layers;        // layers of the forked phases 0-2 (they get per-part plans)
   std::vector<std::unique_ptr<GnOp>> gns;
   std::vector<std::unique_ptr<SeOp>> ses;
+  std::vector<std::unique_ptr<RelOp>> rels;
   std::vector<Step> steps;
   StageMap stages;
   // geometry
@@ -159,6 +168,10 @@ struct b2_ctx {
   HeadPostParams post;
   Planes roi_feat, fc6, fc7;
   Planes head_a, head_b;           // conv box head (cfg.conv_head_dim > 0): [M][7][7][conv_head_dim] ping-pong
+  // relation modules (cfg.add_relation_nn): their sums, and the scratch both modules share -- query|key [Mpad][2D] fp32,
+  // P [B][16K][Kp], P.V = the output_linear operand [Mpad][16D]
+  Planes rm1, rm2, rel_p, rel_o;
+  float* rel_qk = nullptr;
   float* head_logits = nullptr;
   float* box_feat = nullptr;
   float* box_feat_pooled = nullptr;
@@ -197,7 +210,7 @@ Step& add_batch_step(b2_ctx* c, int phase, int kind, const std::string& name,
                      const std::function<int(int, int, cudaStream_t)>& launch, int launches = 1) {
   static const char* kKindNames[] = {"conv", "stem_pack", "maxpool", "p6_subsample", "rpn_proposals", "roialign_proposals",
                                      "head_post", "roialign_final", "roialign_mask", "mask_select", "gn_stats", "gn_apply",
-                                     "gn_roi", "se_squeeze", "se_excite", "se_apply"};
+                                     "gn_roi", "se_squeeze", "se_excite", "se_apply", "relation_attend"};
   const int B = c->cfg.batch;
   Step& s = add_step(c->steps, phase, kind, name.empty() ? kKindNames[kind] : name,
                      [launch, B](cudaStream_t st) { return launch(0, B, st); }, 0, 0, launches);
@@ -393,6 +406,65 @@ int add_se(b2_ctx* c, int phase, const std::string& name, const Planes& buf, con
     return se_apply_launch(p, st);
   }).bytes = 3.0 * n * esz;
   c->steps.back().flops = 3.0 * n;
+  return 0;
+}
+
+// The relation module `name` (relation_network nn.py:115-190) over the M = B*K head rows h (image b's rows at b*K), with
+// out = h + output_linear(P . h) (models.py:1044-1054: the module's output plus its own input).  Steps:
+//   query_key          one N = 2D layer (query_linear | key_linear), fp32 output
+//   attend             per image: V^T into the image's P.V weights, then geometry + logits + masked softmax -> P
+//   attention_value    per image, one layer of 16K rows: P (rows i * 16 + g) times V^T, landing as the [K][16D] flatten
+//   output_linear      dense 16D -> D over the flatten, h added in the epilogue, no ReLU
+// An image's ROIs attend to its own proposals only (DESIGN 4, Relation head).
+int add_relation(b2_ctx* c, const std::string& name, const Planes& h, const Planes& out) {
+  const int B = c->cfg.batch, K = c->cfg.rpn_topk, D = c->cfg.fc_head_dim, M = B * K;
+  const int Kp = (K + 63) / 64 * 64, Mpad = (M + 127) / 128 * 128, G = kRelGroups;
+  if (!c->rel_qk) {
+    c->rel_qk = c->arena.alloc<float>(static_cast<size_t>(Mpad) * 2 * D);
+    B2_CHECK(c->rel_qk && c->alloc_planes(c->rel_p, B, 1, G * K, Kp) && c->alloc_planes(c->rel_o, 1, 1, Mpad, G * D),
+             "out of device memory (relation module scratch)");
+  }
+  std::unique_ptr<RelOp> R(new RelOp());
+  R->name = name;
+  R->geo = c->arena.alloc<float>(kRelGeoWeights);
+  __half** vt = c->arena.alloc<__half*>(2 * B);
+  B2_CHECK(R->geo && vt, "out of device memory (relation module " + name + ")");
+  add_conv(c, 5, name + "/query_key", h, 1, M, 1, 1, 1, 0, 0, 0, 0, 2 * D, false, false, false, Planes(), 0, 0, nullptr, 0,
+           c->rel_qk, 2 * D, kRelQK);
+  RelationParams p;
+  memset(&p, 0, sizeof(p));
+  p.boxes = c->rpn.prop_boxes; p.count = c->rpn.prop_count;
+  p.qk = c->rel_qk; p.ldqk = 2 * D; p.D = D; p.K = K; p.Kp = Kp;
+  p.rows = relation_rows_per_block(Kp, D);
+  p.geo = R->geo;
+  p.h_hi = h.hi; p.h_lo = h.lo;
+  p.p_hi = c->rel_p.hi; p.p_lo = c->rel_p.lo;
+  p.vt_hi = vt; p.vt_lo = c->split ? vt + B : nullptr;
+  c->rels.push_back(std::move(R));
+  const double esz = c->split ? 4.0 : 2.0;
+  Step& s = add_batch_step(c, 5, 16, name + "/attend [" + std::to_string(K) + "x" + std::to_string(K) + "x" +
+                                         std::to_string(G) + "]",
+                           [p](int b0, int nb, cudaStream_t st) { return relation_attend_launch(p, b0, nb, st); }, 2);
+  // at full K: per pair the 4 -> 64 -> 16 geometry net and 16 head dots; query / key read once, V^T and P written once
+  s.flops = 2.0 * B * K * K * (4.0 * kRelGeoDim + kRelGeoDim * G + D);
+  s.bytes = B * (static_cast<double>(K) * 2 * D * 4 + 2.0 * D * Kp * esz + static_cast<double>(G) * K * Kp * esz);
+  std::vector<__half*> tab(2 * B, nullptr);
+  for (int b = 0; b < B; ++b) {
+    Planes o = c->rel_o;   // image b's 16K rows of D: rows b*K .. b*K + K - 1 of the [Mpad][16D] operand
+    const size_t off = static_cast<size_t>(b) * G * K * D;
+    o.W = G * K; o.C = D;
+    o.hi += off;
+    if (o.lo) o.lo += off;
+    ConvLayer* L = add_conv(c, 5, name + "/attention_value [image " + std::to_string(b) + "]", c->rel_p.images(b, 1), 1,
+                            G * K, 1, 1, 1, 0, 0, 0, 0, D, false, false, false, o, 0, 0, nullptr, 0, nullptr, 0, kRuntime);
+    tab[b] = L->w.w_hi;
+    tab[B + b] = L->w.w_lo;
+  }
+  B2_CUDA(cudaMemcpy(vt, tab.data(), tab.size() * sizeof(__half*), cudaMemcpyHostToDevice));
+  Planes o = c->rel_o;
+  o.W = M;
+  add_conv(c, 5, name + "/output_linear", o, 1, M, 1, 1, 1, 0, 0, 0, 0, D, false, false, false, out, 0, 0, &h, 0, nullptr, 0,
+           kDense);
   return 0;
 }
 
@@ -717,14 +789,29 @@ int build_plan(b2_ctx* c) {
   } else {
     Planes f6 = c->fc6; f6.W = M;
     Planes f7 = c->fc7; f7.W = M;
+    // add_relation_nn (models.py:1044-1054): fc7 reads relu(fc6) + RM_r1, the outputs read relu(fc7) + RM_r2
+    const bool rel = cfg.add_relation_nn != 0;
+    Planes h1 = f6, h2 = f7;
+    if (rel) {
+      B2_CHECK(dim % 64 == 0, "b2_create: add_relation_nn needs fc_head_dim a multiple of 64");
+      B2_CHECK(c->alloc_planes(c->rm1, 1, 1, Mpad, dim) && c->alloc_planes(c->rm2, 1, 1, Mpad, dim), "alloc relation sums");
+      h1 = c->rm1; h1.W = M;
+      h2 = c->rm2; h2.W = M;
+    }
     add_conv(c, 5, "fastrcnn/fc6", rf, 1, M, 1, 1, 1, 0, 0, 0, 0, dim, false, true, true, f6, 0, 0, nullptr, 0, nullptr,
              0, kFc6);
-    add_conv(c, 5, "fastrcnn/fc7", f6, 1, M, 1, 1, 1, 0, 0, 0, 0, dim, false, true, true, f7, 0, 0, nullptr, 0, nullptr,
+    if (rel && add_relation(c, "fastrcnn/RM_r1", f6, h1)) return -1;
+    add_conv(c, 5, "fastrcnn/fc7", h1, 1, M, 1, 1, 1, 0, 0, 0, 0, dim, false, true, true, f7, 0, 0, nullptr, 0, nullptr,
              0, kDense);
-    add_conv(c, 5, "fastrcnn/outputs", f7, 1, M, 1, 1, 1, 0, 0, 0, 0, nout, false, true, false, Planes(), 0, 0, nullptr,
+    if (rel && add_relation(c, "fastrcnn/RM_r2", f7, h2)) return -1;
+    add_conv(c, 5, "fastrcnn/outputs", h2, 1, M, 1, 1, 1, 0, 0, 0, 0, nout, false, true, false, Planes(), 0, 0, nullptr,
              0, c->head_logits, ldo, kHeadOut);
     c->stages.planes("fc6", f6);
     c->stages.planes("fc7", f7);
+    if (rel) {
+      c->stages.planes("rm_r1", h1);
+      c->stages.planes("rm_r2", h2);
+    }
   }
   c->stages.raw("head_logits", c->head_logits, Stage::kF32, B, K, ldo, 1);
 
@@ -872,7 +959,18 @@ int enqueue(b2_ctx* c, int mask, bool with_events) {
 }
 
 // ---- weight loading -------------------------------------------------------------------------
+// geo_emb (dense 4 -> 64, nn.py:125-127) and geo_conv (1x1 conv 64 -> 16, nn.py:133-135) of a relation module
+int load_rel(b2_ctx* c, RelOp* R, const WeightSet& ws) {
+  const float* ew = ws.get(R->name + "/geo_emb/W", 4 * kRelGeoDim);
+  const float* eb = ws.get(R->name + "/geo_emb/b", kRelGeoDim);
+  const float* cw = ws.get(R->name + "/geo_conv/W", kRelGeoDim * kRelGroups);
+  const float* cb = ws.get(R->name + "/geo_conv/b", kRelGroups);
+  if (!ew || !eb || !cw || !cb) return -1;
+  return relation_upload_geo(ew, eb, cw, cb, R->geo, c->stream);
+}
+
 int load_layer(b2_ctx* c, const ConvLayer* L, const WeightSet& ws) {
+  if (L->layout == kRuntime) return 0;   // written by the pass itself
   const int Cin = L->d.Cin, R = L->d.R, S = L->d.S, Cout = L->d.Cout, K = L->w.K, Cp = L->w.Cout_pad;
   std::vector<float> packed(static_cast<size_t>(Cp) * K, 0.f);
   std::vector<double> scale, shift;
@@ -933,6 +1031,13 @@ int load_layer(b2_ctx* c, const ConvLayer* L, const WeightSet& ws) {
         const size_t k = static_cast<size_t>(s) * C + ch;
         for (int o = 0; o < Cout; ++o) packed[static_cast<size_t>(o) * K + k] = src[o];
       }
+  } else if (L->layout == kRelQK) {
+    // relation module query_linear / key_linear (nn.py:146-156): dense D -> D each, no bias, one N = 2D layer
+    const std::string scope = L->name.substr(0, L->name.rfind('/'));
+    const float* wq = ws.get(scope + "/query_linear/W", static_cast<int64_t>(Cin) * Cin);
+    const float* wk = ws.get(scope + "/key_linear/W", static_cast<int64_t>(Cin) * Cin);
+    if (!wq || !wk) return -1;
+    relation_pack_qk(wq, wk, Cin, packed);
   } else if (L->layout == kDense) {
     const float* w = ws.get(L->name + "/W", static_cast<int64_t>(Cin) * Cout);
     if (!w) return -1;
@@ -1063,6 +1168,8 @@ int b2_load_weights(b2_ctx* c, const char* const* names, const float* const* dat
     if (load_gn(c, G.get(), ws)) return -1;
   for (auto& S : c->ses)
     if (load_se(c, S.get(), ws)) return -1;
+  for (auto& R : c->rels)
+    if (load_rel(c, R.get(), ws)) return -1;
   c->weights_loaded = true;
   return 0;
 }

@@ -1,6 +1,8 @@
 // Parameter blocks and launchers of the non-GEMM kernels (proposals, ROIAlign, detection post-process,
 // appearance cost).  All launches are asynchronous on the given stream; nothing syncs with the host.
 #pragma once
+#include <vector>
+
 #include "common.h"
 
 namespace b2 {
@@ -214,6 +216,33 @@ struct LevelRoiFeatParams {
   float* out;               // [max_out][Creal]
 };
 int level_roi_feat_launch(const LevelRoiFeatParams& p, cudaStream_t s);
+
+// relation.cu -- the box head's relation module (add_relation_nn, nn.py:115-190): the geometry + attention softmax and
+// the V^T operand of the per-image P.V layer; query / key, P.V and output_linear run on conv_tc_kernel
+constexpr int kRelGroups = 16, kRelGeoDim = 64;
+constexpr int kRelGeoWeights = 4 * kRelGeoDim + kRelGeoDim + kRelGeoDim * kRelGroups + kRelGroups;
+struct RelationParams {
+  const float* boxes;       // [B][K][4] proposals x1 y1 x2 y2
+  const int* count;         // [B] proposals per image (rows j >= count are padding)
+  const float* qk;          // [B*K][ldqk] fp32: query in columns [0, D), key in [D, 2D)
+  int ldqk, D, K, Kp;       // Kp: K rounded up to 64 (columns of P, rows of V^T)
+  int rows;                 // query rows per block (relation_rows_per_block)
+  const float* geo;         // kRelGeoWeights: geo_emb W [4][64], b [64], geo_conv W [64][16], b [16]
+  const __half* h_hi;       // h [B*K][D] planes: the value
+  const __half* h_lo;
+  __half* p_hi;             // P [B][K*16][Kp] planes, row i * 16 + g
+  __half* p_lo;
+  __half* const* vt_hi;     // device table of B pointers: image b's V^T [D][Kp] planes (the P.V layer's weights)
+  __half* const* vt_lo;
+};
+int relation_rows_per_block(int Kp, int D);
+// V^T and P of images [b0, b0 + n)
+int relation_attend_launch(const RelationParams& p, int b0, int n, cudaStream_t s);
+// query_linear / key_linear W [D][D] ([in, out]) -> the fused layer's [2D][D] operand
+void relation_pack_qk(const float* wq, const float* wk, int D, std::vector<float>& packed);
+// geo_emb W [4, 64], b [64], geo_conv W [1, 1, 64, 16], b [16] -> dst (kRelGeoWeights floats on the device)
+int relation_upload_geo(const float* emb_w, const float* emb_b, const float* conv_w, const float* conv_b, float* dst,
+                        cudaStream_t s);
 
 // cosine.cu
 int cosine_normalize_rows(const float* src, int rows, int D, __half* hi, __half* lo, int ld, cudaStream_t s);

@@ -1,5 +1,5 @@
 // Single-kernel entry points for parity tests and host tools: one conv, one grouped conv, one GroupNorm, one squeeze-excite,
-// the frame resize.  Each call owns its device buffers in an Arena, so every return path frees them.
+// one relation module, the frame resize.  Each call owns its device buffers in an Arena, so every return path frees them.
 #include <string.h>
 
 #include <algorithm>
@@ -209,6 +209,87 @@ int b2_op_squeeze_excite(int device, const float* x, const float* res, const flo
   B2_CUDA(cudaDeviceSynchronize());
   if (gate_out) B2_CUDA(cudaMemcpy(gate_out, gate, static_cast<size_t>(B) * C * 4, cudaMemcpyDeviceToHost));
   return download_planes(xp.hi, xp.lo, n, out, nullptr);
+}
+
+// One relation module with the engine's steps and operands (engine.cu add_relation): query|key layer, V^T + attention,
+// one P.V layer per image, output_linear + h.
+int b2_op_relation(int device, const float* h, const float* boxes, const int32_t* count, const float* geo_emb_w,
+                   const float* geo_emb_b, const float* geo_conv_w, const float* geo_conv_b, const float* query_w,
+                   const float* key_w, const float* output_w, int B, int K, int D, int split, float* out) {
+  B2_CHECK(h && boxes && count && geo_emb_w && geo_emb_b && geo_conv_w && geo_conv_b && query_w && key_w && output_w && out,
+           "b2_op_relation: null argument");
+  B2_CHECK(B >= 1 && K >= 1 && K <= 1024 && D >= 64 && D % 64 == 0,
+           "b2_op_relation: needs B >= 1, 1 <= K <= 1024 and D a multiple of 64");
+  for (int b = 0; b < B; ++b) B2_CHECK(count[b] >= 0 && count[b] <= K, "b2_op_relation: count outside [0, K]");
+  B2_CUDA(cudaSetDevice(device));
+  cudaDeviceProp prop;
+  B2_CUDA(cudaGetDeviceProperties(&prop, device));
+  const bool sp = split != 0;
+  const int G = kRelGroups, M = B * K, Mpad = (M + 127) / 128 * 128, Kp = (K + 63) / 64 * 64;
+  Arena a;
+  const Planes hp = a.planes(1, 1, Mpad, D, sp), op = a.planes(1, 1, Mpad, D, sp);
+  const Planes pp = a.planes(B, 1, G * K, Kp, sp), vp = a.planes(1, 1, Mpad, G * D, sp);
+  float* qk = a.alloc<float>(static_cast<size_t>(Mpad) * 2 * D);
+  float* dbox = a.alloc<float>(static_cast<size_t>(M) * 4);
+  int* dcount = a.alloc<int>(B);
+  float* geo = a.alloc<float>(kRelGeoWeights);
+  __half** vt = a.alloc<__half*>(2 * B);
+  B2_CHECK(hp.hi && op.hi && pp.hi && vp.hi && qk && dbox && dcount && geo && vt, "b2_op_relation: out of device memory");
+  if (upload_planes(h, hp.hi, hp.lo, static_cast<size_t>(M) * D, nullptr)) return -1;
+  B2_CUDA(cudaMemcpy(dbox, boxes, static_cast<size_t>(M) * 4 * sizeof(float), cudaMemcpyHostToDevice));
+  B2_CUDA(cudaMemcpy(dcount, count, B * sizeof(int), cudaMemcpyHostToDevice));
+  if (relation_upload_geo(geo_emb_w, geo_emb_b, geo_conv_w, geo_conv_b, geo, nullptr)) return -1;
+
+  std::vector<std::unique_ptr<ConvLayer>> layers;
+  auto dense = [&](const char* name, const Planes& in, int rows, int Cout, const Planes& o, const Planes* res, float* f32,
+                   int ldc) {
+    ConvDesc d;
+    d.in_H = 1; d.in_W = rows; d.Cout = Cout;
+    layers.push_back(make_conv(a, sp, name, d, in, o, res, f32, ldc));
+    return layers.back().get();
+  };
+  Planes hv = hp, ov = op, vv = vp;
+  hv.W = M; ov.W = M; vv.W = M;
+  ConvLayer* Lqk = dense("query_key", hv, M, 2 * D, Planes(), nullptr, qk, 2 * D);
+  std::vector<__half*> tab(2 * B, nullptr);
+  for (int b = 0; b < B; ++b) {
+    Planes o = vp;
+    const size_t off = static_cast<size_t>(b) * G * K * D;
+    o.W = G * K; o.C = D;
+    o.hi += off;
+    if (o.lo) o.lo += off;
+    ConvLayer* L = dense("attention_value", pp.images(b, 1), G * K, D, o, nullptr, nullptr, 0);
+    tab[b] = L->w.w_hi;
+    tab[B + b] = L->w.w_lo;
+  }
+  ConvLayer* Lout = dense("output_linear", vv, M, D, ov, &hv, nullptr, 0);
+  B2_CUDA(cudaMemcpy(vt, tab.data(), tab.size() * sizeof(__half*), cudaMemcpyHostToDevice));
+  std::vector<float> packed;
+  relation_pack_qk(query_w, key_w, D, packed);
+  if (upload_conv(*Lqk, packed, std::vector<float>(2 * D, 0.f), nullptr)) return -1;
+  packed.assign(static_cast<size_t>(D) * G * D, 0.f);
+  for (size_t k = 0; k < static_cast<size_t>(G) * D; ++k)
+    for (int o = 0; o < D; ++o) packed[static_cast<size_t>(o) * G * D + k] = output_w[k * D + o];
+  if (upload_conv(*Lout, packed, std::vector<float>(D, 0.f), nullptr)) return -1;
+  if (plan_convs(layers, sp, prop.multiProcessorCount)) return -1;
+
+  RelationParams p;
+  memset(&p, 0, sizeof(p));
+  p.boxes = dbox; p.count = dcount;
+  p.qk = qk; p.ldqk = 2 * D; p.D = D; p.K = K; p.Kp = Kp;
+  p.rows = relation_rows_per_block(Kp, D);
+  p.geo = geo;
+  p.h_hi = hp.hi; p.h_lo = hp.lo;
+  p.p_hi = pp.hi; p.p_lo = pp.lo;
+  p.vt_hi = vt; p.vt_lo = sp ? vt + B : nullptr;
+  int rc = conv_tc_launch(Lqk->plan.get(), nullptr);
+  if (!rc) rc = relation_attend_launch(p, 0, B, nullptr);
+  for (size_t i = 1; i + 1 < layers.size() && !rc; ++i) rc = conv_tc_launch(layers[i]->plan.get(), nullptr);
+  if (!rc) rc = conv_tc_launch(Lout->plan.get(), nullptr);
+  const cudaError_t e = cudaDeviceSynchronize();   // the kernels are done before their plans go away
+  if (rc) return -1;
+  B2_CUDA(e);
+  return download_planes(op.hi, op.lo, static_cast<size_t>(M) * D, out, nullptr);
 }
 
 // The resize alone (parity tests): host uint8 [n, src_h, src_w, 3] -> host float32 [n, dst_h, dst_w, 3].

@@ -305,6 +305,29 @@ def op_squeeze_excite(x, w1, b1, w2, b2, res=None, split=True, device=0):
     return out, gate
 
 
+def op_relation(h, boxes, count, weights, split=True, device=0) -> np.ndarray:
+    """One relation module of the box head (relation_network nn.py:115-190) through the C ABI -- used by the kernel tests:
+    h [B, K, D] head rows, boxes [B, K, 4] proposals (x1, y1, x2, y2), count [B] valid rows per image, `weights` the
+    module's arrays keyed by their names under the module scope (geo_emb/W, geo_emb/b, geo_conv/W, geo_conv/b,
+    query_linear/W, key_linear/W, output_linear/W).  Returns h + RM(h, boxes) [B, K, D]; rows i >= count[b] are h."""
+    lib = _lib.load()
+    h = np.ascontiguousarray(h, dtype=np.float32)
+    B, K, D = h.shape
+    boxes = np.ascontiguousarray(boxes, dtype=np.float32)
+    count = np.ascontiguousarray(count, dtype=np.int32)
+    assert boxes.shape == (B, K, 4) and count.shape == (B,), (boxes.shape, count.shape)
+    shapes = {"geo_emb/W": (4, 64), "geo_emb/b": (64,), "geo_conv/W": (1, 1, 64, 16), "geo_conv/b": (16,),
+              "query_linear/W": (D, D), "key_linear/W": (D, D), "output_linear/W": (16 * D, D)}
+    w = {k: np.ascontiguousarray(weights[k], dtype=np.float32) for k in shapes}
+    for k, s in shapes.items():
+        assert w[k].size == int(np.prod(s)), (k, w[k].shape, s)
+    out = np.empty_like(h)
+    _lib.check(lib.b2_op_relation(device, _lib.ptr(h), _lib.ptr(boxes), _lib.ptr(count),
+                                  *[_lib.ptr(w[k]) for k in shapes], B, K, D, int(split), _lib.ptr(out)),
+               "b2_op_relation")
+    return out
+
+
 def get_new_hw(h, w, size, max_size):
     """nn.py:1548-1560: (neww, newh) of resizeImage for an h x w frame."""
     scale = size * 1.0 / min(h, w)

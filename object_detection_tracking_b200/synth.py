@@ -15,6 +15,7 @@ weights.  Names follow the Tensorpack-npz convention the reference loads
   use_conv_frcnn_head: fastrcnn/conv{0..3}/{W,b} (+ fastrcnn/gn{0..3}/.. with use_gn), fastrcnn/fc/{W,b}
   use_se: group{0..3}/block{i}/fc1/{W,b}, fc2/{W,b} (squeeze-excite dense layers)
   use_resnext: conv1 / conv2 at twice the width, conv2/W [3, 3, 2*ch/32, 2*ch] (32 groups), no fc1 / fc2
+  add_relation_nn: fastrcnn/RM_r{1,2}/{geo_emb/{W,b}, geo_conv/{W,b}, query_linear/W, key_linear/W, output_linear/W}
 
 Conv kernels are HWIO (`nn.py:350,367`), dense kernels [in,out] (`nn.py:753`).
 The distributions are chosen so activations stay O(1) through 33 residual blocks
@@ -126,6 +127,18 @@ def synth_weights(cfg, seed: int = 1234) -> dict:
             w[p + "/fc1/b"] = rng.uniform(0.0, 0.1, nr).astype(np.float32)
             w[p + "/fc2/W"] = (rng.standard_normal((nr, c)) * np.sqrt(2.0 / nr)).astype(np.float32)
             w[p + "/fc2/b"] = (rng.standard_normal(c) * 0.4).astype(np.float32)
+    # The relation modules come after everything else, so every other array of a seed is the same with and without them.
+    if _use_relation(cfg):                           # relation_network (nn.py:115-190) of RM_r1 / RM_r2
+        for name, shape in _relation_shapes(cfg).items():
+            fan_in = int(np.prod(shape[:-1]))
+            # geo_emb: the log-ratio features span ~[-7, 3], so a gain well under 1 keeps tanh off its rails; geo_conv
+            # without a bias offset puts about half of the (i, g, j) weights under the 1e-6 clamp and the rest in
+            # ~[1e-3, 2]; query / key give per-head logits of a few units (peaked, not one-hot rows); output_linear's
+            # unit gain over the 16 averaged heads makes the module's output the size of h
+            std = {"geo_emb/W": 0.3, "geo_emb/b": 0.1, "geo_conv/W": np.sqrt(1.0 / 64), "geo_conv/b": 0.05,
+                   "query_linear/W": np.sqrt(2.0 / fan_in), "key_linear/W": np.sqrt(2.0 / fan_in),
+                   "output_linear/W": np.sqrt(1.0 / fan_in)}[name.split("/", 2)[2]]
+            w[name] = (rng.standard_normal(shape) * std).astype(np.float32)
     return w
 
 
@@ -140,6 +153,23 @@ def _block_widths(cfg, feat):
 def _use_se(cfg):
     """use_se selects squeeze-excite in resnet_bottleneck only: the ResNeXt block has no SE branch (nn.py:524-549)."""
     return getattr(cfg, "use_se", False) and not getattr(cfg, "use_resnext", False)
+
+
+def _use_relation(cfg):
+    """add_relation_nn builds RM_r1 / RM_r2 in the 2fc head only: use_conv_frcnn_head takes precedence (models.py:1038-1041)."""
+    return getattr(cfg, "add_relation_nn", False) and not getattr(cfg, "use_conv_frcnn_head", False)
+
+
+def _relation_shapes(cfg):
+    """Name -> shape of the relation modules' variables (nn.py:115-190, group 16, geo_feat_dim 64), in graph order."""
+    dim = cfg.fpn_frcnn_fc_head_dim
+    sh = {}
+    for m in ("RM_r1", "RM_r2"):
+        p = "fastrcnn/%s/" % m
+        sh.update({p + "geo_emb/W": (4, 64), p + "geo_emb/b": (64,), p + "geo_conv/W": (1, 1, 64, 16),
+                   p + "geo_conv/b": (16,), p + "query_linear/W": (dim, dim), p + "key_linear/W": (dim, dim),
+                   p + "output_linear/W": (16 * dim, dim)})
+    return sh
 
 
 def _se_blocks(cfg):
@@ -237,6 +267,8 @@ def frcnn_weight_shapes(cfg) -> dict:
     for name, fin, fout in hidden + (("fastrcnn/outputs/class", dim, cfg.num_class), ("fastrcnn/outputs/box", dim, nbox * 4)):
         sh[name + "/W"] = (fin, fout)
         sh[name + "/b"] = (fout,)
+    if _use_relation(cfg):                           # fastrcnn_2fc_head(_class_agnostic) (models.py:1044-1054, 1139-1148)
+        sh.update(_relation_shapes(cfg))
     if getattr(cfg, "add_mask", False):              # models.py:1173-1199; Conv2DTranspose kernel is [kh, kw, out, in]
         md = getattr(cfg, "mrcnn_head_dim", 256)
         for k in range(4):
