@@ -71,6 +71,11 @@ typedef struct b2_config {
                                  nn.py:115-190): h1 = relu(fc6) + RM_r1(relu(fc6), proposals), h2 = relu(fc7(h1)) +
                                  RM_r2(relu(fc7(h1)), proposals), each image's ROIs attending to its own proposals only;
                                  ignored with conv_head_dim > 0 */
+  int32_t use_deformable;     /* --use_deformable: a bottleneck block is deformable when it has stride 2 and is among the last
+                                 3 blocks of its group (nn.py:459-521, 568-588): res5 block 0 for R50 / R101 / R152.  Its
+                                 conv2 samples conv1's output bilinearly at learned offsets ("<block>/conv2_offset/{W,b}",
+                                 [3,3,C,18], [18]) and has no norm and no ReLU.  Each image uses its own offsets.  Ignored
+                                 with use_resnext; refused with use_dilations, where the reference's residual sum fails */
 } b2_config;
 
 const char* b2_last_error(void);
@@ -348,6 +353,17 @@ int b2_op_group_conv2d(int device, const float* x, const float* w, const float* 
 int b2_op_relation(int device, const float* h, const float* boxes, const int32_t* count, const float* geo_emb_w,
                    const float* geo_emb_b, const float* geo_conv_w, const float* geo_conv_b, const float* query_w,
                    const float* key_w, const float* output_w, int B, int K, int D, int split, float* out);
+/* The deformable conv's bilinear sampler (deformable_conv2d nn.py:1642-1712, deformable_helper.py:42-137) as the engine runs
+ * it: x [B][H][W][C] (host, fp32, converted to the engine's planes), offsets [B][ceil(H/2)][ceil(W/2)][18] (channel 2k the
+ * y and 2k+1 the x offset of tap k, per image).  out [B][ceil(H/2)][ceil(W/2)][9][C]: the sampled operand read back from
+ * its planes.  C a multiple of 64. */
+int b2_op_deform_sample(int device, const float* x, const float* offsets, int B, int H, int W, int C, int split, float* out);
+/* The whole deformable conv2 as the engine runs it: offsets = 3x3 stride-2 conv of x with offset_w [3][3][C][18] and
+ * offset_b [18] (pads 1 top / left), the sampler, then the conv w [3][3][C][Cout] over the sampled operand with no bias,
+ * norm or activation.  out [B][ceil(H/2)][ceil(W/2)][Cout]; offsets_out (may be NULL) [B][ceil(H/2)][ceil(W/2)][18].
+ * impl 0 = tensor cores, 1 = CUDA cores (both for the offset conv and conv2). */
+int b2_op_deform_conv2d(int device, const float* x, const float* offset_w, const float* offset_b, const float* w, int B,
+                        int H, int W, int C, int Cout, int impl, int split, float* out, float* offsets_out);
 
 #ifdef __cplusplus
 }

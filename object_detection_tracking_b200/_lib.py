@@ -24,7 +24,7 @@ class B2Config(ctypes.Structure):
         ("anchor_strides", c_float * 5), ("anchor_sizes", c_float * 5), ("anchor_ratios", c_float * 3),
         ("bbox_reg_weights", c_float * 4), ("accum_chunk", c_int32), ("multi_semantics", c_int32),
         ("add_mask", c_int32), ("use_gn", c_int32), ("conv_head_dim", c_int32), ("use_se", c_int32),
-        ("use_resnext", c_int32), ("add_relation_nn", c_int32),
+        ("use_resnext", c_int32), ("add_relation_nn", c_int32), ("use_deformable", c_int32),
     ]
 
 
@@ -116,6 +116,8 @@ SYMBOLS = [
     ("b2_op_squeeze_excite", c_int, [c_int] + [c_void_p] * 6 + [c_int] * 6 + [c_void_p, c_void_p]),
     ("b2_op_group_conv2d", c_int, [c_int, c_void_p, c_void_p, c_void_p, c_void_p] + [c_int] * 16 + [c_void_p]),
     ("b2_op_relation", c_int, [c_int] + [c_void_p] * 10 + [c_int] * 4 + [c_void_p]),
+    ("b2_op_deform_sample", c_int, [c_int, c_void_p, c_void_p] + [c_int] * 5 + [c_void_p]),
+    ("b2_op_deform_conv2d", c_int, [c_int] + [c_void_p] * 4 + [c_int] * 7 + [c_void_p, c_void_p]),
 ]
 
 PHASES = dict(BACKBONE=1, FPN=2, RPN_HEAD=4, PROPOSALS=8, ROI=16, HEAD_FC=32, POST=64, BOX_FEAT=128, ALL=255)
@@ -197,4 +199,5 @@ def make_config(cfg, batch: int, height: int, width: int, input_dtype: str = "fl
     c.use_se = int(bool(getattr(cfg, "use_se", False)))
     c.use_resnext = int(bool(getattr(cfg, "use_resnext", False)))
     c.add_relation_nn = int(bool(getattr(cfg, "add_relation_nn", False)))
+    c.use_deformable = int(bool(getattr(cfg, "use_deformable", False)))
     return c

@@ -47,6 +47,9 @@ _DEFAULTS = dict(
                                        # 3x3 convs (nn.py:524-549, 864-868); the block has no SE branch
     add_relation_nn=False,             # --add_relation_nn (obj_detect_tracking.py:226): relation modules RM_r1 / RM_r2 in
                                        # the 2fc box head (models.py:1044-1054, nn.py:115-190); not with the conv head
+    use_deformable=False,              # --use_deformable (obj_detect_tracking.py:215): deformable conv2 in the stride-2
+                                       # blocks among the last 3 of a group (nn.py:459-521, 568-588): res5 block 0 of
+                                       # R50 / R101; ignored with use_resnext, refused with use_dilations
     use_partial_classes=False,
     is_efficientdet=False,
 )

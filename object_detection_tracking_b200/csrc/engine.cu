@@ -210,7 +210,8 @@ Step& add_batch_step(b2_ctx* c, int phase, int kind, const std::string& name,
                      const std::function<int(int, int, cudaStream_t)>& launch, int launches = 1) {
   static const char* kKindNames[] = {"conv", "stem_pack", "maxpool", "p6_subsample", "rpn_proposals", "roialign_proposals",
                                      "head_post", "roialign_final", "roialign_mask", "mask_select", "gn_stats", "gn_apply",
-                                     "gn_roi", "se_squeeze", "se_excite", "se_apply", "relation_attend"};
+                                     "gn_roi", "se_squeeze", "se_excite", "se_apply", "relation_attend",
+                                     "deform_sample"};
   const int B = c->cfg.batch;
   Step& s = add_step(c->steps, phase, kind, name.empty() ? kKindNames[kind] : name,
                      [launch, B](cudaStream_t st) { return launch(0, B, st); }, 0, 0, launches);
@@ -468,6 +469,44 @@ int add_relation(b2_ctx* c, const std::string& name, const Planes& h, const Plan
   return 0;
 }
 
+// The deformable conv2 of block `name` (nn.py:470-486, deformable_conv2d nn.py:1642-1712) from conv1's output `in` into
+// `out`.  Steps:
+//   conv2_offset   the offsets, fp32 [B][Ho][Wo][kDeformOffsetLd]: the reference's 3x3 SAME stride-1 conv (bias, no norm,
+//                  no activation) is read at the even centres only, so it runs as a 3x3 stride-2 conv with pad 1 top / left
+//                  and 2 * Ho - H bottom (2 * Wo - W right): the same value at each centre, a quarter of the work
+//   conv2_sample   the bilinear sampler (deform.cu) -> the operand [B][Ho][Wo][9][C]
+//   conv2          a 1x1 conv with K = 9 * C over the operand: the [3,3,C,Cout] kernel packed as a 3x3 conv ([Cout][3][3][C])
+//                  lines tap k = ky * 3 + kx up with the operand's tap-major K; no bias, norm or ReLU (activation tf.identity)
+// Each image is sampled at its own offsets (DESIGN 4, Deformable conv).
+int add_deform(b2_ctx* c, const std::string& name, const Planes& in, const Planes& out) {
+  const int B = c->cfg.batch, H = in.H, W = in.W, C = in.C, Ho = (H + 1) / 2, Wo = (W + 1) / 2;
+  B2_CHECK(out.H == Ho && out.W == Wo && out.C == C, "b2_create: deformable conv2 output does not match its group");
+  float* off = c->arena.alloc<float>(static_cast<size_t>(B) * Ho * Wo * kDeformOffsetLd);
+  Planes smp;
+  B2_CHECK(off && c->alloc_planes(smp, B, Ho, Wo, 9 * C), "alloc deformable operand");
+  add_conv(c, 0, name + "/conv2_offset", in, H, W, 3, 2, 1, 1, 2 * Ho - H, 1, 2 * Wo - W, 18, false, true, false, Planes(),
+           0, 0, nullptr, 0, off, kDeformOffsetLd);
+  DeformParams dp;
+  dp.in_hi = in.hi; dp.in_lo = in.lo;
+  dp.offset = off; dp.ld_off = kDeformOffsetLd;
+  dp.H = H; dp.W = W; dp.C = C; dp.Ho = Ho; dp.Wo = Wo;
+  dp.out_hi = smp.hi; dp.out_lo = smp.lo;
+  const double esz = c->split ? 4.0 : 2.0;
+  const double taps = 9.0 * B * Ho * Wo;
+  Step& s = add_batch_step(c, 0, 17, name + "/conv2_sample [" + std::to_string(H) + "x" + std::to_string(W) + "x" +
+                                         std::to_string(C) + " ->" + std::to_string(Ho) + "x" + std::to_string(Wo) + "x9x" +
+                                         std::to_string(C) + "]",
+                           [dp](int b0, int n, cudaStream_t st) { return deform_sample_launch(dp, b0, n, st); });
+  // the input read once (the four corners of every sample are mostly L2 hits), the offsets once, the operand written once;
+  // three lerps of three operations per sample
+  s.bytes = static_cast<double>(B) * H * W * C * esz + B * static_cast<double>(Ho) * Wo * 18 * 4.0 + taps * C * esz;
+  s.flops = 9.0 * taps * C;
+  add_conv(c, 0, name + "/conv2", smp, Ho, Wo, 1, 1, 1, 0, 0, 0, 0, C, false, false, false, out, 0, 0, nullptr, 0);
+  c->stages.raw(name + "/conv2_offset", off, Stage::kF32, B, Ho, Wo, kDeformOffsetLd);
+  c->stages.planes(name + "/conv2_sample", smp);
+  return 0;
+}
+
 // generate_anchors.py:42-109 restated for one (stride, size): the 3 ratio anchors of a cell.
 void cell_anchors(float stride, float size, const float* ratios, float out[3][4]) {
   const double base = stride;
@@ -591,7 +630,16 @@ int build_plan(b2_ctx* c) {
       add_conv(c, 0, p + "/conv1", x, x.H, x.W, 1, 1, 1, 0, 0, 0, 0, mid, !gn, false, !gn, a1, 0, 0, nullptr, 0);
       if (gn && add_gn(c, 0, p + "/conv1/gn", a1, a1.H, a1.W, 0, 0, nullptr, 0, true)) return -1;
       const Planes* a2 = &t2;
-      if (rx) {
+      // use_deformable (nn.py:470-486, 577-581): a stride-2 block among the last 3 of its group; the ResNeXt block has no
+      // deformable branch
+      const bool deform = cfg.use_deformable != 0 && !rx && stride == 2 && in_last3;
+      if (deform) {
+        B2_CHECK(dil == 1, "b2_create: use_deformable cannot be combined with use_dilations: " + p + " pads its deformable "
+                           "conv2 output [1, 0] (nn.py:493-497), but that output is ceil(h/2), not the dilated conv's h/2 - 1, "
+                           "so the reference's residual sum fails (24x41 against 23x40 at 720x1280)");
+        a2 = &t2_first;
+        if (add_deform(c, p, a1, *a2)) return -1;
+      } else if (rx) {
         // 3x3 split=32, padding SAME (nn.py:537-540): TF pads the total (out - 1) * stride + (3 - 1) * dil + 1 - in
         // with the odd element at the bottom / right (SURVEY Appendix B) -- at stride 2 on the even sizes here 0 / 1,
         // with dilation 2 then 1 / 2 -- and nothing follows the conv (no [1,0] pad, no output offset)

@@ -244,6 +244,21 @@ void relation_pack_qk(const float* wq, const float* wk, int D, std::vector<float
 int relation_upload_geo(const float* emb_w, const float* emb_b, const float* conv_w, const float* conv_b, float* dst,
                         cudaStream_t s);
 
+// deform.cu -- the bilinear sampler of a deformable conv2 (use_deformable, deformable_helper.py:42-137): conv1's output
+// sampled at tap k's base + offset around (2i, 2j), clamped to the map, into the operand of a 1x1 conv with K = 9 * C
+constexpr int kDeformOffsetLd = 32;   // row stride of the fp32 offsets: the offset conv's 18 outputs padded to Cout_pad
+struct DeformParams {
+  const __half* in_hi;      // conv1 output [B][H][W][C] planes
+  const __half* in_lo;
+  const float* offset;      // [B][Ho][Wo][ld_off] fp32: column 2k the y, 2k + 1 the x offset of tap k
+  int ld_off;
+  int H, W, C, Ho, Wo;      // Ho = ceil(H / 2), Wo = ceil(W / 2); C a multiple of 8
+  __half* out_hi;           // [B][Ho][Wo][9][C] planes: tap-major, then channel
+  __half* out_lo;
+};
+// images [b0, b0 + n)
+int deform_sample_launch(const DeformParams& p, int b0, int n, cudaStream_t s);
+
 // cosine.cu
 int cosine_normalize_rows(const float* src, int rows, int D, __half* hi, __half* lo, int ld, cudaStream_t s);
 int rows_to_planes(const float* src, int rows, int D, __half* hi, __half* lo, int ld, float* sqnorm, cudaStream_t s);

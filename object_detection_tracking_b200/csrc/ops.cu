@@ -1,5 +1,5 @@
 // Single-kernel entry points for parity tests and host tools: one conv, one grouped conv, one GroupNorm, one squeeze-excite,
-// one relation module, the frame resize.  Each call owns its device buffers in an Arena, so every return path frees them.
+// one relation module, the deformable sampler and conv, the frame resize.  Each call owns its device buffers in an Arena, so every return path frees them.
 #include <string.h>
 
 #include <algorithm>
@@ -290,6 +290,94 @@ int b2_op_relation(int device, const float* h, const float* boxes, const int32_t
   if (rc) return -1;
   B2_CUDA(e);
   return download_planes(op.hi, op.lo, static_cast<size_t>(M) * D, out, nullptr);
+}
+
+// The deformable sampler alone: fp32 x and offsets in, the sampled operand's planes joined to fp32 out.
+int b2_op_deform_sample(int device, const float* x, const float* offsets, int B, int H, int W, int C, int split, float* out) {
+  B2_CHECK(x && offsets && out, "b2_op_deform_sample: null argument");
+  B2_CHECK(B >= 1 && H >= 1 && W >= 1 && C >= 64 && C % 64 == 0, "b2_op_deform_sample: needs C a multiple of 64");
+  B2_CUDA(cudaSetDevice(device));
+  const bool sp = split != 0;
+  const int Ho = (H + 1) / 2, Wo = (W + 1) / 2;
+  const size_t nx = static_cast<size_t>(B) * H * W * C, noff = static_cast<size_t>(B) * Ho * Wo * 18;
+  Arena a;
+  const Planes xp = a.planes(B, H, W, C, sp), op = a.planes(B, Ho, Wo, 9 * C, sp);
+  float* off = a.alloc<float>(noff);
+  B2_CHECK(xp.hi && op.hi && off, "b2_op_deform_sample: out of device memory");
+  if (upload_planes(x, xp.hi, xp.lo, nx, nullptr)) return -1;
+  B2_CUDA(cudaMemcpy(off, offsets, noff * sizeof(float), cudaMemcpyHostToDevice));
+  DeformParams p;
+  p.in_hi = xp.hi; p.in_lo = xp.lo;
+  p.offset = off; p.ld_off = 18;
+  p.H = H; p.W = W; p.C = C; p.Ho = Ho; p.Wo = Wo;
+  p.out_hi = op.hi; p.out_lo = op.lo;
+  if (deform_sample_launch(p, 0, B, nullptr)) return -1;
+  B2_CUDA(cudaDeviceSynchronize());
+  return download_planes(op.hi, op.lo, op.elems(), out, nullptr);
+}
+
+// The deformable conv2 with the engine's steps and operands (engine.cu add_deform): offset conv, sampler, 1x1 conv over
+// the operand.
+int b2_op_deform_conv2d(int device, const float* x, const float* offset_w, const float* offset_b, const float* w, int B,
+                        int H, int W, int C, int Cout, int impl, int split, float* out, float* offsets_out) {
+  B2_CHECK(x && offset_w && offset_b && w && out, "b2_op_deform_conv2d: null argument");
+  B2_CHECK(B >= 1 && H >= 2 && W >= 2 && C >= 64 && C % 64 == 0 && Cout >= 1,
+           "b2_op_deform_conv2d: needs C a multiple of 64");
+  B2_CUDA(cudaSetDevice(device));
+  cudaDeviceProp prop;
+  B2_CUDA(cudaGetDeviceProperties(&prop, device));
+  const bool sp = split != 0;
+  const int Ho = (H + 1) / 2, Wo = (W + 1) / 2, Cp = (Cout + 15) / 16 * 16;
+  const size_t npix = static_cast<size_t>(B) * Ho * Wo;
+  Arena a;
+  const Planes xp = a.planes(B, H, W, C, sp), smp = a.planes(B, Ho, Wo, 9 * C, sp), op = a.planes(B, Ho, Wo, Cp, sp);
+  float* off = a.alloc<float>(npix * kDeformOffsetLd);
+  B2_CHECK(xp.hi && smp.hi && op.hi && off, "b2_op_deform_conv2d: out of device memory");
+  if (upload_planes(x, xp.hi, xp.lo, xp.elems(), nullptr)) return -1;
+  std::vector<std::unique_ptr<ConvLayer>> layers;
+  ConvDesc d;
+  d.R = 3; d.S = 3; d.stride = 2;
+  d.pad_t = 1; d.pad_b = 2 * Ho - H; d.pad_l = 1; d.pad_r = 2 * Wo - W;
+  d.Cout = 18;
+  layers.push_back(make_conv(a, sp, "conv2_offset", d, xp, Planes(), nullptr, off, kDeformOffsetLd));
+  ConvDesc d2;
+  d2.Cout = Cout;
+  layers.push_back(make_conv(a, sp, "conv2", d2, smp, op));
+  // HWIO -> [Cout_pad][K]: the offset conv's K = 9 * C, and conv2's [3,3,C,Cout] kernel as a 1x1 conv over 9 * C inputs
+  for (int l = 0; l < 2; ++l) {
+    const ConvLayer& L = *layers[l];
+    const int n = l == 0 ? 18 : Cout, K = L.w.K;
+    const float* src = l == 0 ? offset_w : w;
+    std::vector<float> packed(static_cast<size_t>(L.w.Cout_pad) * K, 0.f), bias(L.w.Cout_pad, 0.f);
+    for (int k = 0; k < K; ++k)
+      for (int o = 0; o < n; ++o) packed[static_cast<size_t>(o) * K + k] = src[static_cast<size_t>(k) * n + o];
+    if (l == 0) std::copy(offset_b, offset_b + 18, bias.begin());
+    if (upload_conv(L, packed, bias, nullptr)) return -1;
+  }
+  if (impl == 0 && plan_convs(layers, sp, prop.multiProcessorCount)) return -1;
+  auto conv = [&](const ConvLayer& L) {
+    return impl == 0 ? conv_tc_launch(L.plan.get(), nullptr) : conv_simt_launch(L.d, L.w, L.io, sp, nullptr);
+  };
+  DeformParams p;
+  p.in_hi = xp.hi; p.in_lo = xp.lo;
+  p.offset = off; p.ld_off = kDeformOffsetLd;
+  p.H = H; p.W = W; p.C = C; p.Ho = Ho; p.Wo = Wo;
+  p.out_hi = smp.hi; p.out_lo = smp.lo;
+  int rc = conv(*layers[0]);
+  if (!rc) rc = deform_sample_launch(p, 0, B, nullptr);
+  if (!rc) rc = conv(*layers[1]);
+  const cudaError_t e = cudaDeviceSynchronize();   // the kernels are done before their plans go away
+  if (rc) return -1;
+  B2_CUDA(e);
+  std::vector<float> o(npix * Cp);
+  if (download_planes(op.hi, op.lo, o.size(), o.data(), nullptr)) return -1;
+  for (size_t q = 0; q < npix; ++q) std::copy(&o[q * Cp], &o[q * Cp] + Cout, out + q * Cout);
+  if (offsets_out) {
+    std::vector<float> f(npix * kDeformOffsetLd);
+    B2_CUDA(cudaMemcpy(f.data(), off, f.size() * sizeof(float), cudaMemcpyDeviceToHost));
+    for (size_t q = 0; q < npix; ++q) std::copy(&f[q * kDeformOffsetLd], &f[q * kDeformOffsetLd] + 18, offsets_out + q * 18);
+  }
+  return 0;
 }
 
 // The resize alone (parity tests): host uint8 [n, src_h, src_w, 3] -> host float32 [n, dst_h, dst_w, 3].

@@ -328,6 +328,43 @@ def op_relation(h, boxes, count, weights, split=True, device=0) -> np.ndarray:
     return out
 
 
+def op_deform_sample(x, offsets, split=True, device=0) -> np.ndarray:
+    """The deformable conv's bilinear sampler through the C ABI -- used by the kernel tests: x [B, H, W, C] NHWC,
+    offsets [B, ceil(H/2), ceil(W/2), 18] (channel 2k the y, 2k + 1 the x offset of tap k).  Returns the sampled operand
+    [B, ceil(H/2), ceil(W/2), 9, C] as its planes store it."""
+    lib = _lib.load()
+    x = np.ascontiguousarray(x, dtype=np.float32)
+    B, H, W, C = x.shape
+    Ho, Wo = (H + 1) // 2, (W + 1) // 2
+    off = np.ascontiguousarray(offsets, dtype=np.float32)
+    assert off.shape == (B, Ho, Wo, 18), off.shape
+    out = np.empty((B, Ho, Wo, 9, C), dtype=np.float32)
+    _lib.check(lib.b2_op_deform_sample(device, _lib.ptr(x), _lib.ptr(off), B, H, W, C, int(split), _lib.ptr(out)),
+               "b2_op_deform_sample")
+    return out
+
+
+def op_deform_conv2d(x, offset_w, offset_b, w, impl="tcgen05", split=True, return_offsets=False, device=0):
+    """A deformable conv2 (deformable_conv2d nn.py:1642-1712 with its conv2_offset, nn.py:470-486) through the C ABI --
+    used by the kernel tests: x [B, H, W, C] NHWC, offset_w [3, 3, C, 18], offset_b [18], w [3, 3, C, Cout].  Returns
+    out [B, ceil(H/2), ceil(W/2), Cout], and the offsets [B, ceil(H/2), ceil(W/2), 18] with return_offsets."""
+    lib = _lib.load()
+    x = np.ascontiguousarray(x, dtype=np.float32)
+    B, H, W, C = x.shape
+    ow = np.ascontiguousarray(offset_w, dtype=np.float32)
+    ob = np.ascontiguousarray(offset_b, dtype=np.float32)
+    w = np.ascontiguousarray(w, dtype=np.float32)
+    Cout = w.shape[3]
+    assert ow.shape == (3, 3, C, 18) and ob.shape == (18,) and w.shape == (3, 3, C, Cout), (ow.shape, ob.shape, w.shape)
+    Ho, Wo = (H + 1) // 2, (W + 1) // 2
+    out = np.empty((B, Ho, Wo, Cout), dtype=np.float32)
+    off = np.empty((B, Ho, Wo, 18), dtype=np.float32)
+    _lib.check(lib.b2_op_deform_conv2d(device, _lib.ptr(x), _lib.ptr(ow), _lib.ptr(ob), _lib.ptr(w), B, H, W, C, Cout,
+                                       {"tcgen05": 0, "simt": 1}[impl], int(split), _lib.ptr(out), _lib.ptr(off)),
+               "b2_op_deform_conv2d")
+    return (out, off) if return_offsets else out
+
+
 def get_new_hw(h, w, size, max_size):
     """nn.py:1548-1560: (neww, newh) of resizeImage for an h x w frame."""
     scale = size * 1.0 / min(h, w)

@@ -16,6 +16,7 @@ weights.  Names follow the Tensorpack-npz convention the reference loads
   use_se: group{0..3}/block{i}/fc1/{W,b}, fc2/{W,b} (squeeze-excite dense layers)
   use_resnext: conv1 / conv2 at twice the width, conv2/W [3, 3, 2*ch/32, 2*ch] (32 groups), no fc1 / fc2
   add_relation_nn: fastrcnn/RM_r{1,2}/{geo_emb/{W,b}, geo_conv/{W,b}, query_linear/W, key_linear/W, output_linear/W}
+  use_deformable: <deformable block>/conv2_offset/{W,b} [3, 3, C, 18], [18]; that block's conv2 has no bn / gn
 
 Conv kernels are HWIO (`nn.py:350,367`), dense kernels [in,out] (`nn.py:753`).
 The distributions are chosen so activations stay O(1) through 33 residual blocks
@@ -139,6 +140,16 @@ def synth_weights(cfg, seed: int = 1234) -> dict:
                    "query_linear/W": np.sqrt(2.0 / fan_in), "key_linear/W": np.sqrt(2.0 / fan_in),
                    "output_linear/W": np.sqrt(1.0 / fan_in)}[name.split("/", 2)[2]]
             w[name] = (rng.standard_normal(shape) * std).astype(np.float32)
+    # The deformable blocks' conv2 norm is drawn above and dropped here, and their offset convs are drawn last: every array
+    # a seed shares with the plain model is the same with and without use_deformable.
+    for p, c in deformable_blocks(cfg):              # resnet_bottleneck's deformable branch (nn.py:470-486)
+        for k in [k for k in w if k.startswith(p + "/conv2/bn/") or k.startswith(p + "/conv2/gn/")]:
+            del w[k]
+        # conv1's output is ReLU'd BN output: a fan-in gain of 2 and a bias spread of 0.5 give offsets of one to a few
+        # pixels -- nearly every sample fractional, a fifth to two thirds of the offsets beyond one pixel, the border
+        # taps clamped (test_deform_cpu states the thresholds)
+        w[p + "/conv2_offset/W"] = _conv_w(rng, 3, c, 18)
+        w[p + "/conv2_offset/b"] = (rng.standard_normal(18) * 0.5).astype(np.float32)
     return w
 
 
@@ -170,6 +181,17 @@ def _relation_shapes(cfg):
                    p + "geo_conv/b": (16,), p + "query_linear/W": (dim, dim), p + "key_linear/W": (dim, dim),
                    p + "output_linear/W": (16 * dim, dim)})
     return sh
+
+
+def deformable_blocks(cfg):
+    """(block scope, conv2 channels) of every deformable block, in graph order.  resnet_group passes deformable to the last
+    3 blocks of a group (nn.py:577-581) and resnet_bottleneck uses it at stride 2 only (nn.py:470), so a group qualifies
+    when its block 0 has stride 2 (groups 1-3) and the group has at most 3 blocks.  The ResNeXt block has no deformable
+    branch."""
+    if not getattr(cfg, "use_deformable", False) or getattr(cfg, "use_resnext", False):
+        return []
+    return [("group%d/block0" % g, feat) for g, (feat, count) in enumerate(zip((64, 128, 256, 512), cfg.resnet_num_block))
+            if g > 0 and count <= 3]
 
 
 def _se_blocks(cfg):
@@ -222,6 +244,7 @@ def frcnn_weight_shapes(cfg) -> dict:
 
     conv("conv0", 7, 3, 64)
     bn("conv0", 64)
+    deform = dict(deformable_blocks(cfg))
     cin = 64
     for g, (feat, count) in enumerate(zip((64, 128, 256, 512), cfg.resnet_num_block)):
         mid, cg = _block_widths(cfg, feat)
@@ -229,7 +252,10 @@ def frcnn_weight_shapes(cfg) -> dict:
             p = "group%d/block%d" % (g, i)
             for name, k, ci, co in (("conv1", 1, cin, mid), ("conv2", 3, cg, mid), ("conv3", 1, mid, feat * 4)):
                 conv("%s/%s" % (p, name), k, ci, co)
-                bn("%s/%s" % (p, name), co)
+                if not (name == "conv2" and p in deform):    # deformable_conv2d: no norm (nn.py:483-485)
+                    bn("%s/%s" % (p, name), co)
+            if p in deform:                          # conv2_offset: 3x3 SAME with bias (nn.py:474-476)
+                conv(p + "/conv2_offset", 3, mid, 18, bias=True)
             if cin != feat * 4:
                 conv(p + "/convshortcut", 1, cin, feat * 4)
                 bn(p + "/convshortcut", feat * 4)
