@@ -327,6 +327,31 @@ int b2_track_spatial_dist(const int32_t* frames1, const double* pts1, const int3
 int b2_op_conv2d(int device, const float* x, const float* w, const float* bias, const float* res, int B, int H, int W,
                  int Cin, int R, int S, int Cout, int stride, int dil, int pad_t, int pad_b, int pad_l, int pad_r,
                  int relu, int res_shift, int impl, int split, int a_mode, float* out);
+/* One conv with the whole conv-kernel contract (the engines' ConvDesc): an input view, a pixel stride, an output placed in
+ * a larger buffer, fp32 or plane outputs, an upsampled residual, the epilogue and accumulation options. */
+typedef struct b2_conv_view {
+  int B, pitch_H, pitch_W, in_ld; /* input buffer x [B][pitch_H][pitch_W][in_ld] */
+  int in_H, in_W, Cin;            /* the view: in_H x in_W pixels of Cin channels at the buffer origin (in_ld < Cin:
+                                     overlapping windows of consecutive pixels) */
+  int R, S, stride, dil, pad_t, pad_b, pad_l, pad_r; /* negative pad_b / pad_r crop */
+  int Cout;
+  int out_H, out_W, off_h, off_w, ldc; /* output buffer [B][out_H][out_W][ldc]; the Ho x Wo result at (off_h, off_w) */
+  int out_f32;                         /* 1: fp32 output, 0: fp16 planes */
+  int res_H, res_W, ldr, res_shift;    /* residual [B][res_H][res_W][ldr] read at (y >> res_shift, x >> res_shift) */
+  int relu;                            /* 0 none, 1 ReLU, 2 swish */
+  int acc_kb, a_mode, force_epi;       /* ConvDesc's accumulation chunk and test knobs (0 / -1 / -1 = the defaults) */
+  int impl, split;                     /* impl 0 tensor cores, 1 CUDA cores; split 1 = (hi, lo) planes, 0 = fp16 */
+  int b0, nb;                          /* launch over images [b0, b0 + nb) only (nb 0 = all), operands offset by whole
+                                          images of their own buffers */
+} b2_conv_view;
+/* x as above, w HWIO [R][S][Cin][Cout], bias [Cout] and res [B][res_H][res_W][ldr] may be NULL.  out_init
+ * [B][out_H][out_W][ldc] is the output buffer's content before the launch (converted to planes for a plane output).  out
+ * receives the whole buffer after it (planes joined to fp32); out_hi / out_lo (may be NULL) the raw fp16 planes (out_lo
+ * only in split precision); range_flag (may be NULL) the range-monitor word.  Every view, placement and stride is checked
+ * against its buffer before any device work. */
+int b2_op_conv2d_view(int device, const b2_conv_view* a, const float* x, const float* w, const float* bias,
+                      const float* res, const float* out_init, float* out, uint16_t* out_hi, uint16_t* out_lo,
+                      uint32_t* range_flag);
 /* GroupNorm (32 groups, eps 1e-5) of the view H x W at (off_h, off_w) of x [B][pitch_H][pitch_W][C] (host, fp32, converted to
  * the engine's planes), then + res [B][res_H][res_W][C] read at (y >> res_shift, x >> res_shift) (res may be NULL), then ReLU.
  * per_roi = 1: the box head's one-kernel form (statistics and apply per sample).  out [B][pitch_H][pitch_W][C]: the buffer

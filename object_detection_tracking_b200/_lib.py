@@ -39,6 +39,13 @@ class B2EffdetConfig(ctypes.Structure):
     ]
 
 
+class B2ConvView(ctypes.Structure):
+    _fields_ = [(name, c_int32) for name in (
+        "B", "pitch_H", "pitch_W", "in_ld", "in_H", "in_W", "Cin", "R", "S", "stride", "dil", "pad_t", "pad_b", "pad_l",
+        "pad_r", "Cout", "out_H", "out_W", "off_h", "off_w", "ldc", "out_f32", "res_H", "res_W", "ldr", "res_shift", "relu",
+        "acc_kb", "a_mode", "force_epi", "impl", "split", "b0", "nb")]
+
+
 # every symbol include/b200det.h declares: (name, restype, argtypes)
 SYMBOLS = [
     ("b2_last_error", c_char_p, []),
@@ -112,6 +119,7 @@ SYMBOLS = [
     ("b2_gallery_free", c_int, [c_int, c_void_p]),
     ("b2_track_spatial_dist", c_int, [c_void_p, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_void_p, c_int, c_int, ctypes.c_double, c_void_p]),
     ("b2_op_conv2d", c_int, [c_int, c_void_p, c_void_p, c_void_p, c_void_p] + [c_int] * 18 + [c_void_p]),
+    ("b2_op_conv2d_view", c_int, [c_int, POINTER(B2ConvView)] + [c_void_p] * 9),
     ("b2_op_group_norm", c_int, [c_int, c_void_p, c_void_p, c_void_p, c_void_p] + [c_int] * 15 + [c_void_p]),
     ("b2_op_squeeze_excite", c_int, [c_int] + [c_void_p] * 6 + [c_int] * 6 + [c_void_p, c_void_p]),
     ("b2_op_group_conv2d", c_int, [c_int, c_void_p, c_void_p, c_void_p, c_void_p] + [c_int] * 16 + [c_void_p]),

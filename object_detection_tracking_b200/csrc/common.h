@@ -37,6 +37,7 @@ struct ConvDesc {
   int in_pitch_H = 0, in_pitch_W = 0;       // buffer dims used for strides (>= view dims)
   int in_ld = 0;                            // pixel stride in elements (0 => Cin)
   int force_a_mode = -1;                    // tests: -1 auto, 0 tiled-2D A operand, 1 im2col TMA
+  int force_epi = -1;                       // tests: -1 auto, 0 direct epilogue, 1 staged (refused where not eligible)
   int acc_kb = 0;                           // split precision: K-blocks per accumulation restart (0 default, <0 off)
   int R = 1, S = 1, stride = 1, dil = 1;
   int pad_t = 0, pad_b = 0, pad_l = 0, pad_r = 0;   // zero padding (pad_b/pad_r may be negative = crop)

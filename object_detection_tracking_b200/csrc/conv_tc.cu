@@ -649,11 +649,20 @@ static int plan_build(ConvPlan* pl, const ConvDesc& d, const ConvWeights& w, con
   // [M][Cout_pad] row-major matrices the tensor maps can describe: fp16 planes written without a placement offset, an
   // unshifted residual of the same size, 16-byte aligned bases and row strides.
   auto aligned16 = [](const void* q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; };
-  const bool staged =
-      io.out_f32 == nullptr && d.off_h == 0 && d.off_w == 0 && d.out_H == Ho && d.out_W == Wo && aligned16(io.out_hi) &&
-      (!split || aligned16(io.out_lo)) &&
-      (io.res_hi == nullptr || (d.res_shift == 0 && d.res_H == Ho && d.res_W == Wo && d.ldr % 8 == 0 &&
-                                aligned16(io.res_hi) && (!split || aligned16(io.res_lo))));
+  const char* not_staged = nullptr;   // why the staged epilogue cannot take this layer (nullptr: it can)
+  if (io.out_f32 != nullptr)
+    not_staged = "the output is fp32";
+  else if (d.off_h != 0 || d.off_w != 0 || d.out_H != Ho || d.out_W != Wo)
+    not_staged = "the output is placed inside a larger buffer";
+  else if (!aligned16(io.out_hi) || (split && !aligned16(io.out_lo)))
+    not_staged = "the output planes are not 16-byte aligned";
+  else if (io.res_hi != nullptr && (d.res_shift != 0 || d.res_H != Ho || d.res_W != Wo))
+    not_staged = "the residual is upsampled or not the output's size";
+  else if (io.res_hi != nullptr && (d.ldr % 8 != 0 || !aligned16(io.res_hi) || (split && !aligned16(io.res_lo))))
+    not_staged = "the residual rows or planes are not 16-byte aligned";
+  B2_CHECK(d.force_epi != 1 || not_staged == nullptr,
+           std::string("conv_tc: force_epi = 1 asks for the staged epilogue, but ") + (not_staged ? not_staged : ""));
+  const bool staged = not_staged == nullptr && d.force_epi != 0;
   p.epi_slots = !staged ? 0 : io.res_hi != nullptr ? kResSlots : kOutSlots;
   p.slot_bytes = kSlotPlaneBytes * (split ? 2 : 1);
   const int slot_total = 2 * p.epi_slots * static_cast<int>(p.slot_bytes);
@@ -674,7 +683,8 @@ static int plan_build(ConvPlan* pl, const ConvDesc& d, const ConvWeights& w, con
   p.res_hi = io.res_hi;
   p.res_lo = io.res_lo;
   p.ldr = d.ldr;
-  B2_CHECK(io.res_hi == nullptr || d.ldr % 2 == 0, "conv_tc: ldr must be even");
+  // both epilogues read residual columns [0, Cout_pad) of every row
+  B2_CHECK(io.res_hi == nullptr || (d.ldr % 2 == 0 && d.ldr >= w.Cout_pad), "conv_tc: ldr must be even and cover Cout_pad");
   p.res_H = d.res_H;
   p.res_W = d.res_W;
   p.res_shift = d.res_shift;

@@ -98,6 +98,122 @@ int b2_op_conv2d(int device, const float* x, const float* w, const float* bias, 
   return run_conv(device, d, x, pw, static_cast<int>(K), pb, res, impl, split, out, "b2_op_conv2d");
 }
 
+int b2_op_conv2d_view(int device, const b2_conv_view* a, const float* x, const float* w, const float* bias,
+                      const float* res, const float* out_init, float* out, uint16_t* out_hi, uint16_t* out_lo,
+                      uint32_t* range_flag) {
+  B2_CHECK(a && x && w && out_init && out, "b2_op_conv2d_view: null argument");
+  const b2_conv_view& v = *a;
+  B2_CHECK(v.B >= 1 && v.in_H >= 1 && v.in_W >= 1 && v.Cin >= 1 && v.Cout >= 1 && v.in_ld >= 1 && v.R >= 1 && v.S >= 1 &&
+               v.stride >= 1 && v.dil >= 1 && v.pad_t >= 0 && v.pad_l >= 0,
+           "b2_op_conv2d_view: sizes, strides and dilation must be positive, pad_t / pad_l not negative");
+  B2_CHECK(v.in_H <= v.pitch_H && v.in_W <= v.pitch_W, "b2_op_conv2d_view: the view lies outside the input buffer");
+  // the last pixel of the view reads Cin channels from its first element on (past its own in_ld when in_ld < Cin)
+  const size_t n_in = static_cast<size_t>(v.B) * v.pitch_H * v.pitch_W * v.in_ld;
+  const size_t last_px = (static_cast<size_t>(v.B - 1) * v.pitch_H + v.in_H - 1) * v.pitch_W + v.in_W - 1;
+  B2_CHECK(last_px * v.in_ld + v.Cin <= n_in, "b2_op_conv2d_view: the last pixel's Cin channels run past the input buffer");
+  ConvDesc d;
+  d.B = v.B; d.in_H = v.in_H; d.in_W = v.in_W; d.Cin = v.Cin;
+  d.in_pitch_H = v.pitch_H; d.in_pitch_W = v.pitch_W; d.in_ld = v.in_ld;
+  d.force_a_mode = v.a_mode; d.force_epi = v.force_epi; d.acc_kb = v.acc_kb;
+  d.R = v.R; d.S = v.S; d.stride = v.stride; d.dil = v.dil;
+  d.pad_t = v.pad_t; d.pad_b = v.pad_b; d.pad_l = v.pad_l; d.pad_r = v.pad_r;
+  d.Cout = v.Cout;
+  d.out_H = v.out_H; d.out_W = v.out_W; d.off_h = v.off_h; d.off_w = v.off_w; d.ldc = v.ldc;
+  d.relu = v.relu;
+  const int Ho = d.Ho(), Wo = d.Wo(), Cp = (v.Cout + 15) / 16 * 16;
+  B2_CHECK(Ho > 0 && Wo > 0, "b2_op_conv2d_view: empty output");
+  B2_CHECK(v.off_h >= 0 && v.off_w >= 0 && v.off_h + Ho <= v.out_H && v.off_w + Wo <= v.out_W,
+           "b2_op_conv2d_view: the placed output does not fit the output buffer");
+  B2_CHECK(v.ldc >= Cp, "b2_op_conv2d_view: ldc must cover Cout_pad");
+  if (res) {
+    B2_CHECK(v.ldr >= Cp, "b2_op_conv2d_view: ldr must cover Cout_pad");
+    B2_CHECK(v.res_shift >= 0 && v.res_shift < 16 && ((v.off_h + Ho - 1) >> v.res_shift) < v.res_H &&
+                 ((v.off_w + Wo - 1) >> v.res_shift) < v.res_W,
+             "b2_op_conv2d_view: the residual is smaller than the output coordinates index");
+    d.res_H = v.res_H; d.res_W = v.res_W; d.ldr = v.ldr; d.res_shift = v.res_shift;
+  }
+  const int b0 = v.b0, nb = v.nb > 0 ? v.nb : v.B - v.b0;
+  B2_CHECK(b0 >= 0 && nb >= 1 && b0 + nb <= v.B, "b2_op_conv2d_view: image range outside the batch");
+  B2_CUDA(cudaSetDevice(device));
+  const bool sp = v.split != 0;
+  const size_t K = static_cast<size_t>(v.R) * v.S * v.Cin;
+  const size_t n_out = static_cast<size_t>(v.B) * v.out_H * v.out_W * v.ldc;
+  const size_t n_res = res ? static_cast<size_t>(v.B) * v.res_H * v.res_W * v.ldr : 0;
+  // pack HWIO -> [Cout_pad][R*S*Cin]; columns [Cout, Cout_pad) have zero weights and bias
+  std::vector<float> pw(static_cast<size_t>(Cp) * K, 0.f), pb(Cp, 0.f);
+  for (size_t k = 0; k < K; ++k)
+    for (int o = 0; o < v.Cout; ++o) pw[static_cast<size_t>(o) * K + k] = w[k * v.Cout + o];
+  if (bias) std::copy(bias, bias + v.Cout, pb.begin());
+  Arena ar;
+  __half *xh = ar.alloc<__half>(n_in), *xl = sp ? ar.alloc<__half>(n_in) : nullptr;
+  __half *oh = nullptr, *ol = nullptr, *rh = nullptr, *rl = nullptr;
+  float* of = nullptr;
+  if (v.out_f32) {
+    of = ar.alloc<float>(n_out);
+  } else {
+    oh = ar.alloc<__half>(n_out);
+    ol = sp ? ar.alloc<__half>(n_out) : nullptr;
+  }
+  if (res) {
+    rh = ar.alloc<__half>(n_res);
+    rl = sp ? ar.alloc<__half>(n_res) : nullptr;
+  }
+  ConvWeights cw;
+  cw.w_hi = ar.alloc<__half>(pw.size());
+  cw.w_lo = sp ? ar.alloc<__half>(pw.size()) : nullptr;
+  cw.bias = ar.alloc<float>(Cp);
+  cw.Cout_pad = Cp;
+  cw.K = static_cast<int>(K);
+  unsigned int* flag = ar.alloc<unsigned int>(1);
+  B2_CHECK(xh && (!sp || xl) && (of || (oh && (!sp || ol))) && (!res || (rh && (!sp || rl))) && cw.w_hi &&
+               (!sp || cw.w_lo) && cw.bias && flag,
+           "b2_op_conv2d_view: out of device memory");
+  // fp16 precision: the lo planes of the operands are not allocated and the conversion skips them
+  cudaStream_t st = nullptr;
+  if (upload_planes(x, xh, xl, n_in, st) || upload_planes(pw.data(), cw.w_hi, cw.w_lo, pw.size(), st)) return -1;
+  if (res && upload_planes(res, rh, rl, n_res, st)) return -1;
+  if (of) {
+    B2_CUDA(cudaMemcpy(of, out_init, n_out * sizeof(float), cudaMemcpyHostToDevice));
+  } else if (upload_planes(out_init, oh, ol, n_out, st)) {
+    return -1;
+  }
+  B2_CUDA(cudaMemcpy(cw.bias, pb.data(), Cp * sizeof(float), cudaMemcpyHostToDevice));
+  // images [b0, b0 + nb): every operand offset by whole images of its own buffer, as the engine's batch parts
+  auto at = [b0](auto* p, int H, int W, int C) { return p ? p + static_cast<size_t>(b0) * H * W * C : p; };
+  ConvIO io;
+  io.in_hi = at(xh, v.pitch_H, v.pitch_W, v.in_ld);
+  io.in_lo = at(xl, v.pitch_H, v.pitch_W, v.in_ld);
+  io.out_hi = at(oh, v.out_H, v.out_W, v.ldc);
+  io.out_lo = at(ol, v.out_H, v.out_W, v.ldc);
+  io.out_f32 = at(of, v.out_H, v.out_W, v.ldc);
+  io.res_hi = at(rh, v.res_H, v.res_W, v.ldr);
+  io.res_lo = at(rl, v.res_H, v.res_W, v.ldr);
+  io.range_flag = flag;
+  d.B = nb;
+  if (v.impl == 0) {
+    cudaDeviceProp prop;
+    B2_CUDA(cudaGetDeviceProperties(&prop, device));
+    PlanPtr plan(conv_tc_plan_create(d, cw, io, sp, prop.multiProcessorCount));
+    B2_CHECK(plan != nullptr, std::string("b2_op_conv2d_view: ") + last_error());
+    const int rc = conv_tc_launch(plan.get(), st);
+    const cudaError_t e = cudaDeviceSynchronize();   // the kernel is done before its plan goes away
+    if (rc) return -1;
+    B2_CUDA(e);
+  } else {
+    if (conv_simt_launch(d, cw, io, sp, st)) return -1;
+    B2_CUDA(cudaDeviceSynchronize());
+  }
+  if (of) {
+    B2_CUDA(cudaMemcpy(out, of, n_out * sizeof(float), cudaMemcpyDeviceToHost));
+  } else {
+    if (download_planes(oh, ol, n_out, out, st)) return -1;
+    if (out_hi) B2_CUDA(cudaMemcpy(out_hi, oh, n_out * sizeof(__half), cudaMemcpyDeviceToHost));
+    if (out_lo && ol) B2_CUDA(cudaMemcpy(out_lo, ol, n_out * sizeof(__half), cudaMemcpyDeviceToHost));
+  }
+  if (range_flag) B2_CUDA(cudaMemcpy(range_flag, flag, sizeof(unsigned int), cudaMemcpyDeviceToHost));
+  return 0;
+}
+
 int b2_op_group_conv2d(int device, const float* x, const float* w, const float* bias, const float* res, int B, int H, int W,
                        int C, int R, int S, int groups, int stride, int dil, int pad_t, int pad_b, int pad_l, int pad_r,
                        int relu, int impl, int split, float* out) {

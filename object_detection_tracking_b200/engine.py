@@ -239,6 +239,56 @@ def op_conv2d(x, w, bias=None, res=None, stride=1, dil=1, pad=(0, 0, 0, 0), relu
     return out
 
 
+def op_conv2d_view(x, w, bias=None, res=None, view=None, stride=1, dil=1, pad=(0, 0, 0, 0), out_init=None, off=(0, 0),
+                   out_f32=False, res_shift=0, relu=0, acc_kb=0, a_mode=-1, force_epi=-1, impl="tcgen05", split=True,
+                   images=None, device=0):
+    """Single convolution with the whole conv-kernel contract through the C ABI -- used by the kernel tests.
+
+    x [B, pitch_H, pitch_W, in_ld] is the whole input buffer and view = (in_H, in_W, Cin) the view at its origin (default:
+    all of it; in_ld < Cin reads overlapping windows).  w is HWIO [R, S, Cin, Cout]; res [B, res_H, res_W, ldr] is read at
+    the placed output coordinates >> res_shift.  out_init [B, out_H, out_W, ldc] is the output buffer before the launch
+    (default: zeros of [B, Ho, Wo, Cout_pad]); the Ho x Wo result lands at off = (off_h, off_w).  images = (b0, nb) launches
+    over those images only.  Returns (out, hi, lo, flag): the whole buffer after the launch as fp32, the raw fp16 planes
+    as uint16 (None for an fp32 output; lo None in fp16 precision) and the range-monitor word."""
+    lib = _lib.load()
+    x = np.ascontiguousarray(x, dtype=np.float32)
+    w = np.ascontiguousarray(w, dtype=np.float32)
+    B, PH, PW, ld = x.shape
+    in_H, in_W, Cin = view if view is not None else (PH, PW, ld)
+    R, S, _, Cout = w.shape
+    pt, pb, pl, pr = pad
+    if out_init is None:
+        Ho = (in_H + pt + pb - ((R - 1) * dil + 1)) // stride + 1
+        Wo = (in_W + pl + pr - ((S - 1) * dil + 1)) // stride + 1
+        out_init = np.zeros((B, max(Ho, 1), max(Wo, 1), (Cout + 15) // 16 * 16), dtype=np.float32)
+    out_init = np.ascontiguousarray(out_init, dtype=np.float32)
+    a = _lib.B2ConvView()
+    a.B, a.pitch_H, a.pitch_W, a.in_ld, a.in_H, a.in_W, a.Cin = B, PH, PW, ld, in_H, in_W, Cin
+    a.R, a.S, a.stride, a.dil, a.pad_t, a.pad_b, a.pad_l, a.pad_r = R, S, stride, dil, pt, pb, pl, pr
+    a.Cout = Cout
+    _, a.out_H, a.out_W, a.ldc = out_init.shape
+    a.off_h, a.off_w = off
+    a.out_f32 = int(bool(out_f32))
+    b = None if bias is None else np.ascontiguousarray(bias, dtype=np.float32)
+    r = None if res is None else np.ascontiguousarray(res, dtype=np.float32)
+    if r is not None:
+        _, a.res_H, a.res_W, a.ldr = r.shape
+        a.res_shift = res_shift
+    a.relu, a.acc_kb, a.a_mode, a.force_epi = int(relu), acc_kb, a_mode, force_epi
+    a.impl, a.split = {"tcgen05": 0, "simt": 1}[impl], int(bool(split))
+    a.b0, a.nb = images if images is not None else (0, 0)
+    out = np.empty_like(out_init)
+    hi = lo = None
+    if not out_f32:
+        hi = np.empty(out_init.shape, dtype=np.uint16)
+        lo = np.empty(out_init.shape, dtype=np.uint16) if split else None
+    flag = np.zeros(1, dtype=np.uint32)
+    _lib.check(lib.b2_op_conv2d_view(device, ctypes.byref(a), _lib.ptr(x), _lib.ptr(w), _lib.ptr(b), _lib.ptr(r),
+                                     _lib.ptr(out_init), _lib.ptr(out), _lib.ptr(hi), _lib.ptr(lo), _lib.ptr(flag)),
+               "b2_op_conv2d_view")
+    return out, hi, lo, int(flag[0])
+
+
 def op_group_conv2d(x, w, bias=None, res=None, stride=1, dil=1, pad=(0, 0, 0, 0), relu=False, impl="tcgen05",
                     split=True, device=0) -> np.ndarray:
     """Grouped convolution through the C ABI -- used by the kernel tests: x [B, H, W, C] NHWC, HWIO kernel

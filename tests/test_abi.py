@@ -46,6 +46,7 @@ def test_config_structs_match_header_size():
     import ctypes
     assert ctypes.sizeof(_lib.B2Config) == 4 * _header_struct_words("b2_config")
     assert ctypes.sizeof(_lib.B2EffdetConfig) == 4 * _header_struct_words("b2_effdet_config")
+    assert ctypes.sizeof(_lib.B2ConvView) == 4 * _header_struct_words("b2_conv_view")
 
 
 def test_compute_entry_points_fail_loudly_without_gpu():
