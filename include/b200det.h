@@ -78,10 +78,22 @@ typedef struct b2_config {
                                  with use_resnext; refused with use_dilations, where the reference's residual sum fails */
 } b2_config;
 
+/* Graph options added after b2_config's layout was fixed.  b2_create_ex takes them; b2_create builds the graph with
+ * every field 0.  New options are appended here, so a b2_config written against an older header stays valid. */
+typedef struct b2_config_ext {
+  int32_t use_basic_block;    /* --resnet34 / --resnet18: basic blocks (nn.py:439-456) instead of bottlenecks:
+                                 relu(norm(conv2(relu(norm(conv1(x))))) + shortcut), conv1 3x3 at the block's stride and conv2
+                                 3x3, both SAME padding and ch_out wide; c2..c5 have 64 / 128 / 256 / 512 channels, and group0
+                                 block0's shortcut is the identity.  The block ignores use_dilations, use_deformable and
+                                 use_se; use_resnext wins over it (nn.py:864-868) */
+} b2_config_ext;
+
 const char* b2_last_error(void);
 int b2_version(void);
 
 int b2_create(b2_ctx** out, int device, const b2_config* cfg);
+/* b2_create with the options of b2_config_ext; ext may be NULL (all 0) */
+int b2_create_ex(b2_ctx** out, int device, const b2_config* cfg, const b2_config_ext* ext);
 void b2_destroy(b2_ctx* ctx);
 
 /* Named fp32 host arrays in the reference's Tensorpack-npz naming ("conv0/W",

@@ -28,6 +28,10 @@ class B2Config(ctypes.Structure):
     ]
 
 
+class B2ConfigExt(ctypes.Structure):
+    _fields_ = [("use_basic_block", c_int32)]
+
+
 class B2EffdetConfig(ctypes.Structure):
     _fields_ = [
         ("image_h", c_int32), ("image_w", c_int32), ("min_level", c_int32), ("max_level", c_int32),
@@ -51,6 +55,7 @@ SYMBOLS = [
     ("b2_last_error", c_char_p, []),
     ("b2_version", c_int, []),
     ("b2_create", c_int, [POINTER(c_void_p), c_int, POINTER(B2Config)]),
+    ("b2_create_ex", c_int, [POINTER(c_void_p), c_int, POINTER(B2Config), POINTER(B2ConfigExt)]),
     ("b2_destroy", None, [c_void_p]),
     ("b2_load_weights", c_int, [c_void_p, POINTER(c_char_p), POINTER(c_void_p), POINTER(c_int64), c_int]),
     ("b2_detect", c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int]),
@@ -209,3 +214,10 @@ def make_config(cfg, batch: int, height: int, width: int, input_dtype: str = "fl
     c.add_relation_nn = int(bool(getattr(cfg, "add_relation_nn", False)))
     c.use_deformable = int(bool(getattr(cfg, "use_deformable", False)))
     return c
+
+
+def make_config_ext(cfg) -> B2ConfigExt:
+    """The options of the namespace that b2_config_ext carries."""
+    e = B2ConfigExt()
+    e.use_basic_block = int(bool(getattr(cfg, "use_basic_block", False)))
+    return e

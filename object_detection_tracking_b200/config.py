@@ -50,9 +50,16 @@ _DEFAULTS = dict(
     use_deformable=False,              # --use_deformable (obj_detect_tracking.py:215): deformable conv2 in the stride-2
                                        # blocks among the last 3 of a group (nn.py:459-521, 568-588): res5 block 0 of
                                        # R50 / R101; ignored with use_resnext, refused with use_dilations
+    use_basic_block=False,             # set by --resnet34 / --resnet18 (obj_detect_tracking.py:349-359): resnet_basicblock
+                                       # (nn.py:439-456) instead of the bottleneck; use_resnext wins (nn.py:864-868);
+                                       # the block ignores use_dilations, use_deformable and use_se
     use_partial_classes=False,
     is_efficientdet=False,
 )
+
+# (flag, resnet_num_block, use_basic_block) of the backbone flags, in the order obj_detect_tracking.py:350-359 applies them
+_BACKBONE_FLAGS = (("resnet152", (3, 8, 36, 3), False), ("resnet50", (3, 4, 6, 3), False),
+                   ("resnet34", (3, 4, 6, 3), True), ("resnet18", (2, 2, 2, 2), True))
 
 
 def make_config(**overrides) -> SimpleNamespace:
@@ -66,8 +73,12 @@ def normalize_config(cfg):
     for k, v in _DEFAULTS.items():
         if not hasattr(cfg, k):
             setattr(cfg, k, v)
-    if getattr(cfg, "resnet50", False):
-        cfg.resnet_num_block = (3, 4, 6, 3)          # :351-352
+    # :348-359: the flags apply in this order, so with several set the last one's blocks win, and the basic block is used
+    # iff --resnet34 or --resnet18 is set; without any flag the blocks and use_basic_block are what the caller gave
+    flags = [f for f in _BACKBONE_FLAGS if getattr(cfg, f[0], False)]
+    if flags:
+        cfg.resnet_num_block = flags[-1][1]
+        cfg.use_basic_block = any(basic for _, _, basic in flags)
     cfg.resnet_num_block = tuple(int(x) for x in cfg.resnet_num_block)
     cfg.fpn_resolution_requirement = float(cfg.anchor_strides[3])   # :323
     # :330-331  max_size rounded up to a multiple of 32

@@ -56,6 +56,7 @@ constexpr int kChunkN = 64;
 constexpr uint32_t kSlotPlaneBytes = kWgRows * kChunkN * 2;   // 8 KB
 constexpr int kMaxSlots = 4;                // per consumer warpgroup
 constexpr int kResSlots = 3;                // slots per warpgroup with a residual (the ring the residual is loaded ahead in)
+constexpr int kRes3x3Slots = 1;             // the same for a layer with R x S > 1
 constexpr int kOutSlots = 1;                // slots per warpgroup without one
 
 struct ConvTcParams {
@@ -663,7 +664,12 @@ static int plan_build(ConvPlan* pl, const ConvDesc& d, const ConvWeights& w, con
   B2_CHECK(d.force_epi != 1 || not_staged == nullptr,
            std::string("conv_tc: force_epi = 1 asks for the staged epilogue, but ") + (not_staged ? not_staged : ""));
   const bool staged = not_staged == nullptr && d.force_epi != 0;
-  p.epi_slots = !staged ? 0 : io.res_hi != nullptr ? kResSlots : kOutSlots;
+  // a 1x1 residual layer (1-4 K-blocks) loads its residual kResSlots chunks ahead; an R x S > 1 one (9-72 K-blocks) is
+  // mainloop-bound and gets one slot, so that its operand ring keeps a stage more (DESIGN 4, Basic block)
+  int res_slots = d.R * d.S > 1 ? kRes3x3Slots : kResSlots;
+  if (const char* e = getenv("B2_RES_SLOTS"))   // experiment hook: slots of the staged R x S > 1 residual layers
+    if (d.R * d.S > 1 && atoi(e) >= 1 && atoi(e) <= kMaxSlots) res_slots = atoi(e);
+  p.epi_slots = !staged ? 0 : io.res_hi != nullptr ? res_slots : kOutSlots;
   p.slot_bytes = kSlotPlaneBytes * (split ? 2 : 1);
   const int slot_total = 2 * p.epi_slots * static_cast<int>(p.slot_bytes);
   p.num_stages = (kSmemBudget - slot_total) / static_cast<int>(p.stage_bytes);

@@ -133,6 +133,7 @@ using namespace b2;
 struct b2_ctx {
   Arena arena;             // first member: freed after everything that refers to it
   b2_config cfg;
+  b2_config_ext ext;       // options appended after b2_config's layout was fixed (b2_create_ex)
   int device = 0, num_sms = 132;
   bool split = false;
   cudaStream_t stream = nullptr;
@@ -507,6 +508,47 @@ int add_deform(b2_ctx* c, const std::string& name, const Planes& in, const Plane
   return 0;
 }
 
+// TF padding SAME of a 3x3 conv (SURVEY Appendix B): pad[0..3] = top, bottom, left, right of an h x w input.  The total
+// (out - 1) * stride + 2 * dil + 1 - n puts its odd element at the bottom / right: at stride 2 on the even sizes of the
+// backbone 0 / 1, with dilation 2 then 1 / 2.
+void same_pads3(int h, int w, int stride, int dil, int pad[4]) {
+  for (int k = 0; k < 2; ++k) {
+    const int n = k == 0 ? h : w, o = (n + stride - 1) / stride;
+    const int total = std::max((o - 1) * stride + 2 * dil + 1 - n, 0);
+    pad[2 * k] = total / 2;
+    pad[2 * k + 1] = total - total / 2;
+  }
+}
+
+// The basic block `name` (resnet_basicblock nn.py:439-456, resnet_shortcut :551-566, the group's ReLU :586-587) from `x`
+// into `out` (feat channels): conv1 3x3 at `stride`, SAME, NormReLU into `t1`; the shortcut (`x` itself when it already
+// has feat channels, else convshortcut + norm into `sc`); conv2 3x3 stride 1 SAME, norm, + shortcut, ReLU.  With
+// BatchNorm the norm, shortcut and ReLU are conv epilogues; with GroupNorm the apply steps carry them.  The block has no
+// dilation, deformable or squeeze-excite branch.
+int add_basic_block(b2_ctx* c, const std::string& name, const Planes& x, int stride, const Planes& t1, const Planes& sc,
+                    const Planes& out, bool gn) {
+  const int feat = out.C;
+  int pad[4];
+  same_pads3(x.H, x.W, stride, 1, pad);
+  ConvLayer* L1 = add_conv(c, 0, name + "/conv1", x, x.H, x.W, 3, stride, 1, pad[0], pad[1], pad[2], pad[3], feat, !gn,
+                           false, !gn, t1, 0, 0, nullptr, 0);
+  B2_CHECK(L1->d.Ho() == t1.H && L1->d.Wo() == t1.W, "b2_create: basic-block conv1 output does not match its group");
+  if (gn && add_gn(c, 0, name + "/conv1/gn", t1, t1.H, t1.W, 0, 0, nullptr, 0, true)) return -1;
+  const Planes* resid = &x;
+  if (x.C != feat) {
+    // stride 2: drop the last row / column, 1x1 stride-2 VALID (nn.py:554-559)
+    ConvLayer* S = add_conv(c, 0, name + "/convshortcut", x, x.H, x.W, 1, stride, 1, 0, 1 - stride, 0, 1 - stride, feat,
+                            !gn, false, false, sc, 0, 0, nullptr, 0);
+    B2_CHECK(S->d.Ho() == sc.H && S->d.Wo() == sc.W, "b2_create: basic-block shortcut output does not match its group");
+    if (gn && add_gn(c, 0, name + "/convshortcut/gn", sc, sc.H, sc.W, 0, 0, nullptr, 0, false)) return -1;
+    resid = &sc;
+  }
+  add_conv(c, 0, name + "/conv2", t1, t1.H, t1.W, 3, 1, 1, 1, 1, 1, 1, feat, !gn, false, !gn, out, 0, 0,
+           gn ? nullptr : resid, 0);
+  if (gn && add_gn(c, 0, name + "/conv2/gn", out, out.H, out.W, 0, 0, resid, 0, true)) return -1;
+  return 0;
+}
+
 // generate_anchors.py:42-109 restated for one (stride, size): the 3 ratio anchors of a cell.
 void cell_anchors(float stride, float size, const float* ratios, float out[3][4]) {
   const double base = stride;
@@ -589,7 +631,10 @@ int build_plan(b2_ctx* c) {
   // ResNeXt 32x4d blocks (nn.py:524-549, chosen at :864-868): conv1 / conv2 at twice the width, conv2 grouped; the block
   // has no squeeze-excite branch, so use_resnext overrides use_se
   const bool rx = cfg.use_resnext != 0;
-  const bool se = cfg.use_se != 0 && !rx;   // squeeze-excite bottlenecks (nn.py:506-519)
+  // basic blocks (--resnet34 / --resnet18, nn.py:439-456): block_func is reassigned to ResNeXt after them, so use_resnext
+  // wins (nn.py:864-868)
+  const bool basic = c->ext.use_basic_block != 0 && !rx;
+  const bool se = cfg.use_se != 0 && !rx && !basic;   // squeeze-excite bottlenecks (nn.py:506-519)
   // conv0 as a 4x1 VALID conv over the packed operand (see stem.cu), BN + ReLU in the epilogue
   {
     Planes view = c->stem_u;
@@ -611,18 +656,26 @@ int build_plan(b2_ctx* c) {
     const int feat = 64 << g, count = cfg.resnet_blocks[g];
     const int mid = rx ? 2 * feat : feat;   // width of conv1 / conv2
     const int gh = c->ch[g], gw = c->cw[g];
+    const int out_c = basic ? feat : feat * 4;   // the blocks' output width (resnet_shortcut's n_out)
     Planes pingpong[2];
-    B2_CHECK(c->alloc_planes(pingpong[0], B, gh, gw, feat * 4), "alloc group out");
-    B2_CHECK(c->alloc_planes(pingpong[1], B, gh, gw, feat * 4), "alloc group out");
+    B2_CHECK(c->alloc_planes(pingpong[0], B, gh, gw, out_c), "alloc group out");
+    B2_CHECK(c->alloc_planes(pingpong[1], B, gh, gw, out_c), "alloc group out");
     Planes t1_first, t1, t2, t2_first, sc;
-    B2_CHECK(c->alloc_planes(t1_first, B, cur.H, cur.W, mid), "alloc t1");
-    B2_CHECK(c->alloc_planes(t1, B, gh, gw, mid), "alloc t1");
-    B2_CHECK(c->alloc_planes(t2, B, gh, gw, mid), "alloc t2");
-    B2_CHECK(c->alloc_planes(t2_first, B, gh, gw, mid), "alloc t2");
-    B2_CHECK(c->alloc_planes(sc, B, gh, gw, feat * 4), "alloc shortcut");
+    if (!basic) B2_CHECK(c->alloc_planes(t1_first, B, cur.H, cur.W, mid), "alloc t1");
+    B2_CHECK(c->alloc_planes(t1, B, gh, gw, mid), "alloc t1");   // a basic block's conv1 output is gh x gw at any stride
+    if (!basic) {
+      B2_CHECK(c->alloc_planes(t2, B, gh, gw, mid), "alloc t2");
+      B2_CHECK(c->alloc_planes(t2_first, B, gh, gw, mid), "alloc t2");
+    }
+    B2_CHECK(c->alloc_planes(sc, B, gh, gw, out_c), "alloc shortcut");
     for (int i = 0; i < count; ++i) {
       const std::string p = "group" + std::to_string(g) + "/block" + std::to_string(i);
       const int stride = (g > 0 && i == 0) ? 2 : 1;
+      if (basic) {
+        if (add_basic_block(c, p, cur, stride, t1, sc, pingpong[i & 1], gn)) return -1;
+        cur = pingpong[i & 1];
+        continue;
+      }
       const bool in_last3 = i >= count - 3;
       const int dil = (g == 3 && cfg.use_dilations && in_last3) ? 2 : 1;
       const Planes& x = cur;
@@ -645,12 +698,7 @@ int build_plan(b2_ctx* c) {
         // with dilation 2 then 1 / 2 -- and nothing follows the conv (no [1,0] pad, no output offset)
         if (stride == 2) a2 = &t2_first;
         int pad[4];   // top, bottom, left, right
-        for (int k = 0; k < 2; ++k) {
-          const int n = k == 0 ? a1.H : a1.W, o = (n + stride - 1) / stride;
-          const int total = std::max((o - 1) * stride + 2 * dil + 1 - n, 0);
-          pad[2 * k] = total / 2;
-          pad[2 * k + 1] = total - total / 2;
-        }
+        same_pads3(a1.H, a1.W, stride, dil, pad);
         ConvLayer* L2 = add_conv(c, 0, p + "/conv2", a1, a1.H, a1.W, 3, stride, dil, pad[0], pad[1], pad[2], pad[3], mid,
                                  !gn, false, !gn, *a2, 0, 0, nullptr, 0, nullptr, 0, kGrouped, 0, 0, 32);
         B2_CHECK(L2->d.Ho() == a2->H && L2->d.Wo() == a2->W, "b2_create: ResNeXt conv2 output does not match its group");
@@ -1153,11 +1201,15 @@ int load_se(b2_ctx* c, SeOp* S, const WeightSet& ws) {
 // =================================================================================================
 extern "C" {
 
-int b2_create(b2_ctx** out, int device, const b2_config* cfg) {
+int b2_create(b2_ctx** out, int device, const b2_config* cfg) { return b2_create_ex(out, device, cfg, nullptr); }
+
+int b2_create_ex(b2_ctx** out, int device, const b2_config* cfg, const b2_config_ext* ext) {
   B2_CHECK(out && cfg, "b2_create: null argument");
   *out = nullptr;
   std::unique_ptr<b2_ctx> c(new b2_ctx());
   c->cfg = *cfg;
+  memset(&c->ext, 0, sizeof(c->ext));
+  if (ext) c->ext = *ext;
   c->device = device;
   c->split = cfg->precision == 1;
   if (open_device(device, "b2_create", &c->num_sms, &c->stream)) return -1;

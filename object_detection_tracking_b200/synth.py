@@ -17,6 +17,8 @@ weights.  Names follow the Tensorpack-npz convention the reference loads
   use_resnext: conv1 / conv2 at twice the width, conv2/W [3, 3, 2*ch/32, 2*ch] (32 groups), no fc1 / fc2
   add_relation_nn: fastrcnn/RM_r{1,2}/{geo_emb/{W,b}, geo_conv/{W,b}, query_linear/W, key_linear/W, output_linear/W}
   use_deformable: <deformable block>/conv2_offset/{W,b} [3, 3, C, 18], [18]; that block's conv2 has no bn / gn
+  use_basic_block: conv1/W [3, 3, cin, ch], conv2/W [3, 3, ch, ch], no conv3; convshortcut [1, 1, cin, ch] where cin != ch;
+                   laterals read 64 / 128 / 256 / 512 channels
 
 Conv kernels are HWIO (`nn.py:350,367`), dense kernels [in,out] (`nn.py:753`).
 The distributions are chosen so activations stay O(1) through 33 residual blocks
@@ -50,6 +52,16 @@ def synth_weights(cfg, seed: int = 1234) -> dict:
         mid, cg = _block_widths(cfg, feat)
         for i in range(count):
             p = "group%d/block%d" % (g, i)
+            if _use_basic(cfg):                      # resnet_basicblock (nn.py:439-456)
+                w[p + "/conv1/W"] = _conv_w(rng, 3, cin, feat)
+                _bn(rng, w, p + "/conv1", feat)
+                w[p + "/conv2/W"] = _conv_w(rng, 3, feat, feat)
+                _bn(rng, w, p + "/conv2", feat, 0.1, 0.3)              # residual-branch last BN, as conv3's below
+                if cin != feat:
+                    w[p + "/convshortcut/W"] = _conv_w(rng, 1, cin, feat, gain=1.0)
+                    _bn(rng, w, p + "/convshortcut", feat)
+                cin = feat
+                continue
             w[p + "/conv1/W"] = _conv_w(rng, 1, cin, mid)
             _bn(rng, w, p + "/conv1", mid)
             w[p + "/conv2/W"] = _conv_w(rng, 3, cg, mid)            # fan-in 9 * cg: a grouped filter sees cg channels
@@ -62,7 +74,7 @@ def synth_weights(cfg, seed: int = 1234) -> dict:
                 _bn(rng, w, p + "/convshortcut", feat * 4)
             cin = feat * 4
     nc = cfg.fpn_num_channel
-    for i, c in enumerate((256, 512, 1024, 2048)):
+    for i, c in enumerate(_c_channels(cfg)):
         w["fpn/lateral_1x1_c%d/W" % (i + 2)] = _conv_w(rng, 1, c, nc, gain=0.25)
         w["fpn/lateral_1x1_c%d/b" % (i + 2)] = (rng.standard_normal(nc) * 0.02).astype(np.float32)
         w["fpn/posthoc_3x3_p%d/W" % (i + 2)] = _conv_w(rng, 3, nc, nc, gain=(0.12, 0.3, 0.8, 2.5)[i])
@@ -161,9 +173,21 @@ def _block_widths(cfg, feat):
     return feat, feat
 
 
+def _use_basic(cfg):
+    """use_basic_block (--resnet34 / --resnet18) selects resnet_basicblock, unless use_resnext reassigns block_func after it
+    (nn.py:864-868)."""
+    return getattr(cfg, "use_basic_block", False) and not getattr(cfg, "use_resnext", False)
+
+
+def _c_channels(cfg):
+    """Channels of c2..c5: the blocks' output width, ch_out for the basic block and 4 * ch_out for the bottlenecks."""
+    return (64, 128, 256, 512) if _use_basic(cfg) else (256, 512, 1024, 2048)
+
+
 def _use_se(cfg):
-    """use_se selects squeeze-excite in resnet_bottleneck only: the ResNeXt block has no SE branch (nn.py:524-549)."""
-    return getattr(cfg, "use_se", False) and not getattr(cfg, "use_resnext", False)
+    """use_se selects squeeze-excite in resnet_bottleneck only: the ResNeXt and basic blocks have no SE branch
+    (nn.py:439-456, 524-549)."""
+    return getattr(cfg, "use_se", False) and not getattr(cfg, "use_resnext", False) and not _use_basic(cfg)
 
 
 def _use_relation(cfg):
@@ -186,9 +210,9 @@ def _relation_shapes(cfg):
 def deformable_blocks(cfg):
     """(block scope, conv2 channels) of every deformable block, in graph order.  resnet_group passes deformable to the last
     3 blocks of a group (nn.py:577-581) and resnet_bottleneck uses it at stride 2 only (nn.py:470), so a group qualifies
-    when its block 0 has stride 2 (groups 1-3) and the group has at most 3 blocks.  The ResNeXt block has no deformable
-    branch."""
-    if not getattr(cfg, "use_deformable", False) or getattr(cfg, "use_resnext", False):
+    when its block 0 has stride 2 (groups 1-3) and the group has at most 3 blocks.  The ResNeXt and basic blocks have no
+    deformable branch."""
+    if not getattr(cfg, "use_deformable", False) or getattr(cfg, "use_resnext", False) or _use_basic(cfg):
         return []
     return [("group%d/block0" % g, feat) for g, (feat, count) in enumerate(zip((64, 128, 256, 512), cfg.resnet_num_block))
             if g > 0 and count <= 3]
@@ -213,10 +237,14 @@ def _backbone_norm_scopes(cfg):
         mid = _block_widths(cfg, feat)[0]
         for i in range(count):
             p = "group%d/block%d" % (g, i)
-            out += [(p + "/conv1", mid, False), (p + "/conv2", mid, False), (p + "/conv3", feat * 4, True)]
-            if cin != feat * 4:
-                out.append((p + "/convshortcut", feat * 4, False))
-            cin = feat * 4
+            if _use_basic(cfg):
+                out += [(p + "/conv1", feat, False), (p + "/conv2", feat, True)]
+            else:
+                out += [(p + "/conv1", mid, False), (p + "/conv2", mid, False), (p + "/conv3", feat * 4, True)]
+            cout = _c_channels(cfg)[g]
+            if cin != cout:
+                out.append((p + "/convshortcut", cout, False))
+            cin = cout
     return out
 
 
@@ -248,18 +276,23 @@ def frcnn_weight_shapes(cfg) -> dict:
     cin = 64
     for g, (feat, count) in enumerate(zip((64, 128, 256, 512), cfg.resnet_num_block)):
         mid, cg = _block_widths(cfg, feat)
+        cout = _c_channels(cfg)[g]
         for i in range(count):
             p = "group%d/block%d" % (g, i)
-            for name, k, ci, co in (("conv1", 1, cin, mid), ("conv2", 3, cg, mid), ("conv3", 1, mid, feat * 4)):
+            if _use_basic(cfg):                      # resnet_basicblock: two 3x3 convs (nn.py:443-450)
+                convs = (("conv1", 3, cin, feat), ("conv2", 3, feat, feat))
+            else:
+                convs = (("conv1", 1, cin, mid), ("conv2", 3, cg, mid), ("conv3", 1, mid, feat * 4))
+            for name, k, ci, co in convs:
                 conv("%s/%s" % (p, name), k, ci, co)
                 if not (name == "conv2" and p in deform):    # deformable_conv2d: no norm (nn.py:483-485)
                     bn("%s/%s" % (p, name), co)
             if p in deform:                          # conv2_offset: 3x3 SAME with bias (nn.py:474-476)
                 conv(p + "/conv2_offset", 3, mid, 18, bias=True)
-            if cin != feat * 4:
-                conv(p + "/convshortcut", 1, cin, feat * 4)
-                bn(p + "/convshortcut", feat * 4)
-            cin = feat * 4
+            if cin != cout:                          # resnet_shortcut (nn.py:551-566)
+                conv(p + "/convshortcut", 1, cin, cout)
+                bn(p + "/convshortcut", cout)
+            cin = cout
     if _use_se(cfg):                                 # dense fc1 / fc2 of every bottleneck (nn.py:509-514, 762)
         for p, c in _se_blocks(cfg):
             sh[p + "/fc1/W"] = (c, c // 16)
@@ -267,7 +300,7 @@ def frcnn_weight_shapes(cfg) -> dict:
             sh[p + "/fc2/W"] = (c // 16, c)
             sh[p + "/fc2/b"] = (c,)
     nc = cfg.fpn_num_channel
-    for i, c in enumerate((256, 512, 1024, 2048)):
+    for i, c in enumerate(_c_channels(cfg)):
         conv("fpn/lateral_1x1_c%d" % (i + 2), 1, c, nc, bias=True)
         conv("fpn/posthoc_3x3_p%d" % (i + 2), 3, nc, nc, bias=True)
         if gn:                                       # gn_c* / gn_p* (nn.py:987-990, 1007-1009)
