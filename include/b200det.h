@@ -372,8 +372,8 @@ int b2_op_group_norm(int device, const float* x, const float* res, const float* 
                      int pitch_H, int pitch_W, int C, int H, int W, int off_h, int off_w, int res_H, int res_W, int res_shift,
                      int relu, int per_roi, int split, int in_place, float* out);
 /* The SE-ResNet bottleneck's squeeze-excite (nn.py:506-519) as the engine runs it: x [B][H][W][C] (host, fp32, converted to
- * the engine's planes), gate[b] = sigmoid(relu(mean_hw(x[b]) @ w1 + b1) @ w2 + b2) with w1 [C][nr], w2 [nr][C], then
- * out = relu(x * gate[b][c] + res) in place (res [B][H][W][C], may be NULL).  gate_out [B][C] may be NULL. */
+ * the engine's planes), gate[b] = sigmoid(relu(mean_hw(x[b]) @ w1 + b1) @ w2 + b2) with w1 [C][nr], w2 [nr][C] (nr = C / 16),
+ * then out = relu(x * gate[b][c] + res) in place (res [B][H][W][C], may be NULL).  gate_out [B][C] may be NULL. */
 int b2_op_squeeze_excite(int device, const float* x, const float* res, const float* w1, const float* b1, const float* w2,
                          const float* b2, int B, int H, int W, int C, int nr, int split, float* out, float* gate_out);
 /* Grouped conv (TF conv2d with C / groups input channels per filter, nn.py:352-355) of x [B][H][W][C] with the HWIO
@@ -397,7 +397,8 @@ int b2_op_relation(int device, const float* h, const float* boxes, const int32_t
 int b2_op_deform_sample(int device, const float* x, const float* offsets, int B, int H, int W, int C, int split, float* out);
 /* The whole deformable conv2 as the engine runs it: offsets = 3x3 stride-2 conv of x with offset_w [3][3][C][18] and
  * offset_b [18] (pads 1 top / left), the sampler, then the conv w [3][3][C][Cout] over the sampled operand with no bias,
- * norm or activation.  out [B][ceil(H/2)][ceil(W/2)][Cout]; offsets_out (may be NULL) [B][ceil(H/2)][ceil(W/2)][18].
+ * norm or activation; Cout == C.  out [B][ceil(H/2)][ceil(W/2)][Cout]; offsets_out (may be NULL)
+ * [B][ceil(H/2)][ceil(W/2)][18].
  * impl 0 = tensor cores, 1 = CUDA cores (both for the offset conv and conv2). */
 int b2_op_deform_conv2d(int device, const float* x, const float* offset_w, const float* offset_b, const float* w, int B,
                         int H, int W, int C, int Cout, int impl, int split, float* out, float* offsets_out);

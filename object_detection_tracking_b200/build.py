@@ -9,7 +9,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libb200det.so")
-SOURCES = ["engine_core.cu", "engine.cu", "ops.cu", "gemm_ws.cu", "conv_tc.cu", "conv_simt.cu", "stem.cu", "rpn.cu",
+SOURCES = ["engine_core.cu", "detplan.cu", "engine.cu", "ops.cu", "gemm_ws.cu", "conv_tc.cu", "conv_simt.cu", "stem.cu", "rpn.cu",
            "roialign.cu", "head.cu", "cosine.cu", "reid.cu", "reid_engine.cu", "effdet.cu", "effnet.cu", "effdet_engine.cu",
            "tracker.cpp", "tmot.cpp", "pairmatch.cu", "groupnorm.cu", "relation.cu", "deform.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",

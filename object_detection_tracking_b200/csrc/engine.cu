@@ -15,8 +15,7 @@
 #include <vector>
 
 #include "../../include/b200det.h"
-#include "engine_core.h"
-#include "kernels.h"
+#include "detplan.h"
 
 namespace b2 {
 namespace {
@@ -90,39 +89,6 @@ __global__ void mask_select_kernel(const float* __restrict__ logits, int ld, con
   }
 }
 
-// One GroupNorm of the plan (use_gn backbone / FPN, conv box head): normalises a conv output in place.
-struct GnOp {
-  std::string name;        // reference variable scope, e.g. "group1/block0/conv1/gn", "fpn/gn_c2", "fastrcnn/gn0"
-  GnParams p;              // full-batch launch (its gamma / beta are loaded with the weights)
-};
-
-// The squeeze-excite of one SE-ResNet bottleneck (use_se): the dense weights "<name>/fc1/{W,b}" and "<name>/fc2/{W,b}".
-struct SeOp {
-  std::string name;        // block scope, e.g. "group1/block0"
-  int C = 0, nr = 0;       // 4 * ch_out gated channels, ch_out / 4 hidden units
-  float *w1 = nullptr, *b1 = nullptr, *w2 = nullptr, *b2 = nullptr;   // [C][nr], [nr], [nr][C], [C]
-};
-
-// The geometry weights of one relation module (add_relation_nn): "<scope>/geo_emb/{W,b}", "<scope>/geo_conv/{W,b}".
-struct RelOp {
-  std::string name;        // module scope, "fastrcnn/RM_r1" or "fastrcnn/RM_r2"
-  float* geo = nullptr;    // kRelGeoWeights (relation_upload_geo)
-};
-
-// Packing of a checkpoint weight into the [Cout_pad][K] operand (ConvLayer::layout).
-enum Layout {
-  kHwio = 0,     // conv HWIO
-  kFc6 = 1,      // dense over the NCHW flatten of [7][7][C] ROI features
-  kDense = 2,
-  kRpnOut = 3,   // rpn/{class,box} fused along N
-  kHeadOut = 4,  // fastrcnn/outputs/{class,box} fused along N
-  kStem = 5,     // 7x7 stem re-indexed for the packed operand
-  kDeconv = 6,   // mask-head transposed conv 2x2/2 as a 1x1 conv onto 4 taps x C outputs
-  kGrouped = 7,  // grouped conv HWIO [R][S][Cin/groups][Cout] (pack_grouped)
-  kRelQK = 8,    // relation module: <scope>/query_linear/W | <scope>/key_linear/W fused along N (relation_pack_qk)
-  kRuntime = 9,  // relation module P.V: the weights are the image's V^T, written by the attention step every pass
-};
-
 enum { NPHASE = 8 };
 
 }  // namespace
@@ -131,19 +97,11 @@ enum { NPHASE = 8 };
 using namespace b2;
 
 struct b2_ctx {
-  Arena arena;             // first member: freed after everything that refers to it
+  DetPlan plan;            // first member: its arena is freed after everything that refers to it
   b2_config cfg;
   b2_config_ext ext;       // options appended after b2_config's layout was fixed (b2_create_ex)
   int device = 0, num_sms = 132;
-  bool split = false;
   cudaStream_t stream = nullptr;
-  std::vector<std::unique_ptr<ConvLayer>> layers;
-  std::vector<ConvLayer*> part_layers;        // layers of the forked phases 0-2 (they get per-part plans)
-  std::vector<std::unique_ptr<GnOp>> gns;
-  std::vector<std::unique_ptr<SeOp>> ses;
-  std::vector<std::unique_ptr<RelOp>> rels;
-  std::vector<Step> steps;
-  StageMap stages;
   // geometry
   int c1h = 0, c1w = 0, ch[4], cw[4], ph[5], pw[5], pfh[5], pfw[5];
   // buffers
@@ -158,21 +116,17 @@ struct b2_ctx {
   cudaEvent_t pass_done[2] = {nullptr, nullptr};
   cudaEvent_t h2d_done[2] = {nullptr, nullptr}, staged_free[2] = {nullptr, nullptr}, out_done[2] = {nullptr, nullptr};
   bool slot_busy[2] = {false, false};
-  // range monitor: conv_tc_kernel ORs the device word when an fp16-plane output exceeds +-65504 (or is NaN); the word is
-  // read back with every host-facing result (h_range: [0], [1] = submit slots, [2] = synchronous calls)
-  unsigned int* range_flag = nullptr;
+  // range monitor: conv_tc_kernel ORs the device word plan.range_flag when an fp16-plane output exceeds +-65504 (or is
+  // NaN); the word is read back with every host-facing result (h_range: [0], [1] = submit slots, [2] = synchronous calls)
   unsigned int* h_range = nullptr;
   Planes stem_u, c1, pool, cfeat[4], lat[4], pfeat[5], rpn_h[5];
   float* rpn_out[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};
   RpnParams rpn;
   RoiAlignParams roi1, roi2, roi3;
   HeadPostParams post;
-  Planes roi_feat, fc6, fc7;
+  Planes roi_feat, fc6, fc7;        // fc6 / fc7: the M = B * rpn_topk head rows (DetPlan::alloc_rows)
   Planes head_a, head_b;           // conv box head (cfg.conv_head_dim > 0): [M][7][7][conv_head_dim] ping-pong
-  // relation modules (cfg.add_relation_nn): their sums, and the scratch both modules share -- query|key [Mpad][2D] fp32,
-  // P [B][16K][Kp], P.V = the output_linear operand [Mpad][16D]
-  Planes rm1, rm2, rel_p, rel_o;
-  float* rel_qk = nullptr;
+  Planes rm1, rm2;                 // relation modules (cfg.add_relation_nn): their sums
   float* head_logits = nullptr;
   float* box_feat = nullptr;
   float* box_feat_pooled = nullptr;
@@ -187,367 +141,17 @@ struct b2_ctx {
   int mask_ld = 0;
   float* final_masks = nullptr;    // [B][R][28][28]
   cudaGraphExec_t graph = nullptr;
-  // dual-stream pass: the backbone / FPN / RPN-head phases run as nsplit batch parts on as many streams, so that the tail
-  // of one layer's persistent kernel (tiles % SMs != 0, no SM busy in the last round) overlaps the other parts' kernels
-  bool dual = false;
-  int nsplit = 1;                                  // batch parts (= streams) of the forked phases
+  // dual-stream pass (plan.dual): the backbone / FPN / RPN-head phases run as plan.nsplit batch parts on as many streams,
+  // so that the tail of one layer's persistent kernel (tiles % SMs != 0, no SM busy in the last round) overlaps the other
+  // parts' kernels
   cudaStream_t side_stream[7] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
   cudaEvent_t fork_ev = nullptr, join_ev[7] = {nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr};
   bool weights_loaded = false;
   cudaEvent_t ev[NPHASE + 1];
   float phase_ms[NPHASE];
-
-  bool alloc_planes(Planes& p, int B, int H, int W, int C) {
-    p = arena.planes(B, H, W, C, split);
-    return p.hi != nullptr;
-  }
 };
 
 namespace {
-
-// Adds step `kind` of `phase`.  `launch(b0, n, st)` enqueues it over images [b0, b0 + n); in the forked phases 0-2 the
-// step gets one launch per batch part.
-Step& add_batch_step(b2_ctx* c, int phase, int kind, const std::string& name,
-                     const std::function<int(int, int, cudaStream_t)>& launch, int launches = 1) {
-  static const char* kKindNames[] = {"conv", "stem_pack", "maxpool", "p6_subsample", "rpn_proposals", "roialign_proposals",
-                                     "head_post", "roialign_final", "roialign_mask", "mask_select", "gn_stats", "gn_apply",
-                                     "gn_roi", "se_squeeze", "se_excite", "se_apply", "relation_attend",
-                                     "deform_sample"};
-  const int B = c->cfg.batch;
-  Step& s = add_step(c->steps, phase, kind, name.empty() ? kKindNames[kind] : name,
-                     [launch, B](cudaStream_t st) { return launch(0, B, st); }, 0, 0, launches);
-  if (c->dual && phase <= 2) {
-    const int hb = B / c->nsplit;
-    for (int h = 0; h < c->nsplit; ++h) s.parts.push_back([launch, h, hb](cudaStream_t st) { return launch(h * hb, hb, st); });
-  }
-  return s;
-}
-
-// The operands of layer L over images [b0, ...): each offset by whole images of its own buffer (a view's pixel stride
-// and pitch, not the view's extent)
-ConvIO images(const ConvLayer& L, int b0) {
-  const ConvDesc& d = L.d;
-  auto at = [b0](auto* p, int H, int W, int C) { return p ? p + static_cast<size_t>(b0) * H * W * C : p; };
-  ConvIO io = L.io;
-  io.in_hi = at(io.in_hi, d.in_pitch_H, d.in_pitch_W, d.in_ld);
-  io.in_lo = at(io.in_lo, d.in_pitch_H, d.in_pitch_W, d.in_ld);
-  io.out_hi = at(io.out_hi, d.out_H, d.out_W, d.ldc);
-  io.out_lo = at(io.out_lo, d.out_H, d.out_W, d.ldc);
-  io.out_f32 = at(io.out_f32, d.out_H, d.out_W, d.ldc);
-  io.res_hi = at(io.res_hi, d.res_H, d.res_W, d.ldr);
-  io.res_lo = at(io.res_lo, d.res_H, d.res_W, d.ldr);
-  return io;
-}
-
-// Adds one conv layer reading `in` (view in_H x in_W of the buffer, pixel stride in_ld, 0 = in.C) and writing `out`.
-ConvLayer* add_conv(b2_ctx* c, int phase, const std::string& name, const Planes& in, int view_h, int view_w, int R,
-                    int stride, int dil, int pt, int pb, int pl, int pr, int Cout, bool bn, bool bias, bool relu,
-                    const Planes& out, int off_h, int off_w, const Planes* res, int res_shift, float* out_f32 = nullptr,
-                    int ldc_f32 = 0, int layout = kHwio, int S = 0, int in_ld = 0, int groups = 1) {
-  ConvDesc d;
-  d.in_H = view_h; d.in_W = view_w; d.in_ld = in_ld;
-  d.R = R; d.S = S > 0 ? S : R; d.stride = stride; d.dil = dil;
-  d.pad_t = pt; d.pad_b = pb; d.pad_l = pl; d.pad_r = pr;
-  d.Cout = Cout;
-  d.relu = relu ? 1 : 0;
-  d.acc_kb = c->cfg.accum_chunk;
-  d.off_h = off_h; d.off_w = off_w;
-  d.res_shift = res ? res_shift : 0;
-  d.groups = groups;
-  // the CUDA-core kernel runs a grouped conv as the dense conv with block-diagonal weights
-  std::unique_ptr<ConvLayer> L =
-      make_conv(c->arena, c->split, name, d, in, out, res, out_f32, ldc_f32, c->cfg.conv_impl != 0);
-  L->bn = bn ? name + "/bn" : "";
-  L->bias = bias ? name + "/b" : "";
-  L->layout = layout;
-  L->io.range_flag = c->range_flag;
-  ConvLayer* raw = L.get();
-  c->layers.push_back(std::move(L));
-  if (phase <= 2) c->part_layers.push_back(raw);
-  // algorithmic FLOPs (a grouped conv's output reads Cin / groups channels per tap) and HBM bytes (each operand read
-  // once -- the weights as packed --, output written once, at the stored precision)
-  const ConvDesc& e = raw->d;
-  const double esz = c->split ? 4.0 : 2.0;
-  const double M = static_cast<double>(e.B) * e.Ho() * e.Wo();
-  const double K = static_cast<double>(e.R) * e.S * e.Cin / e.groups;
-  const double in_px = static_cast<double>(e.B) * e.in_H * e.in_W;
-  const int conv_impl = c->cfg.conv_impl;
-  const bool split = c->split;
-  Step& s = add_batch_step(c, phase, 0,
-                           name + " [" + std::to_string(e.in_H) + "x" + std::to_string(e.in_W) + "x" + std::to_string(e.Cin) + " " +
-                               std::to_string(e.R) + "x" + std::to_string(e.S) + "/" + std::to_string(e.stride) + " d" +
-                               std::to_string(e.dil) + " ->" + std::to_string(e.Cout) + "]",
-                           [raw, conv_impl, split](int, int, cudaStream_t st) {
-                             if (conv_impl == 0) return conv_tc_launch(raw->plan.get(), st);
-                             return conv_simt_launch(raw->d, raw->w, raw->io, split, st);
-                           });
-  for (size_t h = 0; h < s.parts.size(); ++h)
-    s.parts[h] = [raw, h](cudaStream_t st) { return conv_tc_launch(raw->part_plan[h].get(), st); };
-  s.flops = 2.0 * M * K * e.Cout;
-  s.bytes = in_px * (e.in_ld > 0 && e.in_ld < e.Cin ? e.in_ld : e.Cin) * esz + static_cast<double>(raw->w.K) * e.Cout * esz +
-            M * e.Cout * (raw->io.out_f32 ? 4.0 : esz) + (raw->io.res_hi ? M * e.Cout * esz / (e.res_shift ? 4.0 : 1.0) : 0.0);
-  return raw;
-}
-
-// GroupNorm `name` of the view (view_h x view_w at (off_h, off_w)) of `buf`, in place, then + `res` (read at
-// (y >> res_shift, x >> res_shift)) and ReLU: a statistics step and an apply step, or with per_roi one step that
-// normalises each [7][7][C] sample of the box head on chip.  Statistics scratch is allocated here, so capture works.
-int add_gn(b2_ctx* c, int phase, const std::string& name, const Planes& buf, int view_h, int view_w, int off_h, int off_w,
-           const Planes* res, int res_shift, bool relu, bool per_roi = false) {
-  std::unique_ptr<GnOp> G(new GnOp());
-  G->name = name;
-  GnParams base;
-  memset(&base, 0, sizeof(base));
-  base.H = view_h; base.W = view_w; base.C = buf.C;
-  base.pitch_H = buf.H; base.pitch_W = buf.W; base.ld = buf.C; base.off_h = off_h; base.off_w = off_w;
-  if (res) { base.res_H = res->H; base.res_W = res->W; base.res_ld = res->C; base.res_shift = res_shift; }
-  base.relu = relu ? 1 : 0;
-  base.gamma = c->arena.alloc<float>(buf.C);
-  base.beta = c->arena.alloc<float>(buf.C);
-  base.range_flag = c->range_flag;
-  B2_CHECK(base.gamma && base.beta, "out of device memory (GroupNorm " + name + ")");
-  if (!per_roi) {
-    base.chunks = gn_chunks(view_h, view_w, buf.C);
-    base.partial = c->arena.alloc<float>(static_cast<size_t>(buf.B) * base.chunks * 32 * 3);
-    base.stats = c->arena.alloc<float>(static_cast<size_t>(buf.B) * 32 * 2);
-    base.counter = c->arena.alloc<unsigned int>(buf.B);
-    B2_CHECK(base.partial && base.stats && base.counter, "out of device memory (GroupNorm " + name + " statistics)");
-  }
-  // the launch over images [b0, b0 + n): planes and per-image scratch offset by b0
-  const Planes x = buf;
-  const Planes r = res ? *res : Planes();
-  auto params = [base, x, r, per_roi](int b0, int n) {
-    GnParams p = base;
-    const Planes xs = x.images(b0, n), rs = r.images(b0, n);
-    p.x_hi = xs.hi; p.x_lo = xs.lo; p.y_hi = xs.hi; p.y_lo = xs.lo;
-    p.r_hi = rs.hi; p.r_lo = rs.lo;
-    if (!per_roi) {
-      p.partial += static_cast<size_t>(b0) * p.chunks * 32 * 3;
-      p.stats += static_cast<size_t>(b0) * 32 * 2;
-      p.counter += b0;
-    }
-    p.B = n;
-    return p;
-  };
-  G->p = params(0, buf.B);
-  c->gns.push_back(std::move(G));
-  // bytes: statistics read the view once; apply / per-ROI read it, write it and read the residual (a quarter of the view's
-  // size when it is upsampled)
-  const GnParams& p = c->gns.back()->p;
-  const double esz = c->split ? 4.0 : 2.0;
-  const double n = static_cast<double>(p.B) * p.H * p.W * p.C;
-  const double apply_bytes = 2.0 * n * esz + (p.r_hi ? n * esz / (p.res_shift ? 4.0 : 1.0) : 0.0);
-  const std::string dims = " [" + std::to_string(p.H) + "x" + std::to_string(p.W) + "x" + std::to_string(p.C);
-  const std::string epi = std::string(p.r_hi ? (p.res_shift ? " +up2" : " +res") : "") + (p.relu ? " relu" : "") + "]";
-  if (per_roi) {   // the box head's samples are ROIs, not images: always the whole buffer
-    add_batch_step(c, phase, 12, name + " per-roi" + dims + epi,
-                   [p](int, int, cudaStream_t st) { return gn_roi_launch(p, st); }).bytes = apply_bytes;
-  } else {
-    add_batch_step(c, phase, 10, name + " stats" + dims + "]",
-                   [params](int b0, int nb, cudaStream_t st) { return gn_stats_launch(params(b0, nb), st); }).bytes = n * esz;
-    add_batch_step(c, phase, 11, name + " apply" + dims + epi,
-                   [params](int b0, int nb, cudaStream_t st) { return gn_apply_launch(params(b0, nb), st); }).bytes = apply_bytes;
-  }
-  return 0;
-}
-
-// Squeeze-excite of the bottleneck `name` (nn.py:506-519) on its conv3 output `buf`, then relu(buf * gate + res) in place
-// (nn.py:520-521, 586-587): a squeeze step (per-image channel sums), an excite step (fc1 + ReLU, fc2 + sigmoid -> gate
-// [B][C]) and an apply step through GroupNorm's apply path.  Every image has its own scratch, so the per-part launches of
-// the forked phases never share a buffer and an image's gate does not depend on its batch.
-int add_se(b2_ctx* c, int phase, const std::string& name, const Planes& buf, const Planes& res) {
-  std::unique_ptr<SeOp> S(new SeOp());
-  S->name = name;
-  S->C = buf.C;
-  S->nr = buf.C / 16;                                 // ch_out // 4 with C = 4 * ch_out
-  const int B = buf.B, C = S->C, nr = S->nr, HW = buf.H * buf.W, nch = se_chunks(HW);
-  B2_CHECK(nr >= 1 && nr <= se_max_nr(), "b2_create: squeeze-excite width out of range (" + name + ")");
-  S->w1 = c->arena.alloc<float>(static_cast<size_t>(C) * nr);
-  S->b1 = c->arena.alloc<float>(nr);
-  S->w2 = c->arena.alloc<float>(static_cast<size_t>(nr) * C);
-  S->b2 = c->arena.alloc<float>(C);
-  float* partial = c->arena.alloc<float>(static_cast<size_t>(B) * nch * C);
-  float* r_part = c->arena.alloc<float>(static_cast<size_t>(B) * se_fc1_parts() * se_max_nr());
-  float* gate = c->arena.alloc<float>(static_cast<size_t>(B) * C);
-  B2_CHECK(S->w1 && S->b1 && S->w2 && S->b2 && partial && r_part && gate, "out of device memory (squeeze-excite " + name + ")");
-  GnParams base;
-  memset(&base, 0, sizeof(base));
-  base.H = buf.H; base.W = buf.W; base.C = C;
-  base.pitch_H = buf.H; base.pitch_W = buf.W; base.ld = C;
-  base.res_H = res.H; base.res_W = res.W; base.res_ld = res.C;
-  base.relu = 1;
-  base.chunks = gn_chunks(buf.H, buf.W, C);
-  base.range_flag = c->range_flag;
-  const SeOp* se = S.get();
-  c->ses.push_back(std::move(S));
-  const Planes x = buf, r = res;
-  const double esz = c->split ? 4.0 : 2.0;
-  const double n = static_cast<double>(B) * HW * C;
-  const std::string dims = " [" + std::to_string(buf.H) + "x" + std::to_string(buf.W) + "x" + std::to_string(C);
-  add_batch_step(c, phase, 13, name + "/se squeeze" + dims + "]", [x, partial, nch, C](int b0, int nb, cudaStream_t st) {
-    const Planes xs = x.images(b0, nb);
-    return se_squeeze_launch(xs.hi, xs.lo, nb, xs.H * xs.W, C, partial + static_cast<size_t>(b0) * nch * C, st);
-  }).bytes = n * esz;
-  c->steps.back().flops = n;
-  const size_t rp_img = static_cast<size_t>(se_fc1_parts()) * se_max_nr();
-  add_batch_step(c, phase, 14, name + "/se excite [" + std::to_string(C) + "->" + std::to_string(nr) + "->" +
-                                   std::to_string(C) + "]",
-                 [se, partial, r_part, gate, nch, HW, rp_img](int b0, int nb, cudaStream_t st) {
-                   return se_excite_launch(partial + static_cast<size_t>(b0) * nch * se->C, nb, HW, se->C, se->C, se->nr,
-                                           r_part + b0 * rp_img, se->w1, se->b1, se->w2, se->b2, 1,
-                                           gate + static_cast<size_t>(b0) * se->C, nullptr, 0, nullptr, nullptr, st);
-                 }, 2).bytes = B * (static_cast<double>(nch) * C + 2.0 * C * nr + C) * 4.0;
-  c->steps.back().flops = B * (static_cast<double>(nch) * C + 4.0 * C * nr);
-  add_batch_step(c, phase, 15, name + "/se apply" + dims + " +res relu]", [base, x, r, gate](int b0, int nb, cudaStream_t st) {
-    GnParams p = base;
-    const Planes xs = x.images(b0, nb), rs = r.images(b0, nb);
-    p.x_hi = xs.hi; p.x_lo = xs.lo; p.y_hi = xs.hi; p.y_lo = xs.lo;
-    p.r_hi = rs.hi; p.r_lo = rs.lo;
-    p.gate = gate + static_cast<size_t>(b0) * p.C;
-    p.B = nb;
-    return se_apply_launch(p, st);
-  }).bytes = 3.0 * n * esz;
-  c->steps.back().flops = 3.0 * n;
-  return 0;
-}
-
-// The relation module `name` (relation_network nn.py:115-190) over the M = B*K head rows h (image b's rows at b*K), with
-// out = h + output_linear(P . h) (models.py:1044-1054: the module's output plus its own input).  Steps:
-//   query_key          one N = 2D layer (query_linear | key_linear), fp32 output
-//   attend             per image: V^T into the image's P.V weights, then geometry + logits + masked softmax -> P
-//   attention_value    per image, one layer of 16K rows: P (rows i * 16 + g) times V^T, landing as the [K][16D] flatten
-//   output_linear      dense 16D -> D over the flatten, h added in the epilogue, no ReLU
-// An image's ROIs attend to its own proposals only (DESIGN 4, Relation head).
-int add_relation(b2_ctx* c, const std::string& name, const Planes& h, const Planes& out) {
-  const int B = c->cfg.batch, K = c->cfg.rpn_topk, D = c->cfg.fc_head_dim, M = B * K;
-  const int Kp = (K + 63) / 64 * 64, Mpad = (M + 127) / 128 * 128, G = kRelGroups;
-  if (!c->rel_qk) {
-    c->rel_qk = c->arena.alloc<float>(static_cast<size_t>(Mpad) * 2 * D);
-    B2_CHECK(c->rel_qk && c->alloc_planes(c->rel_p, B, 1, G * K, Kp) && c->alloc_planes(c->rel_o, 1, 1, Mpad, G * D),
-             "out of device memory (relation module scratch)");
-  }
-  std::unique_ptr<RelOp> R(new RelOp());
-  R->name = name;
-  R->geo = c->arena.alloc<float>(kRelGeoWeights);
-  __half** vt = c->arena.alloc<__half*>(2 * B);
-  B2_CHECK(R->geo && vt, "out of device memory (relation module " + name + ")");
-  add_conv(c, 5, name + "/query_key", h, 1, M, 1, 1, 1, 0, 0, 0, 0, 2 * D, false, false, false, Planes(), 0, 0, nullptr, 0,
-           c->rel_qk, 2 * D, kRelQK);
-  RelationParams p;
-  memset(&p, 0, sizeof(p));
-  p.boxes = c->rpn.prop_boxes; p.count = c->rpn.prop_count;
-  p.qk = c->rel_qk; p.ldqk = 2 * D; p.D = D; p.K = K; p.Kp = Kp;
-  p.rows = relation_rows_per_block(Kp, D);
-  p.geo = R->geo;
-  p.h_hi = h.hi; p.h_lo = h.lo;
-  p.p_hi = c->rel_p.hi; p.p_lo = c->rel_p.lo;
-  p.vt_hi = vt; p.vt_lo = c->split ? vt + B : nullptr;
-  c->rels.push_back(std::move(R));
-  const double esz = c->split ? 4.0 : 2.0;
-  Step& s = add_batch_step(c, 5, 16, name + "/attend [" + std::to_string(K) + "x" + std::to_string(K) + "x" +
-                                         std::to_string(G) + "]",
-                           [p](int b0, int nb, cudaStream_t st) { return relation_attend_launch(p, b0, nb, st); }, 2);
-  // at full K: per pair the 4 -> 64 -> 16 geometry net and 16 head dots; query / key read once, V^T and P written once
-  s.flops = 2.0 * B * K * K * (4.0 * kRelGeoDim + kRelGeoDim * G + D);
-  s.bytes = B * (static_cast<double>(K) * 2 * D * 4 + 2.0 * D * Kp * esz + static_cast<double>(G) * K * Kp * esz);
-  std::vector<__half*> tab(2 * B, nullptr);
-  for (int b = 0; b < B; ++b) {
-    Planes o = c->rel_o;   // image b's 16K rows of D: rows b*K .. b*K + K - 1 of the [Mpad][16D] operand
-    const size_t off = static_cast<size_t>(b) * G * K * D;
-    o.W = G * K; o.C = D;
-    o.hi += off;
-    if (o.lo) o.lo += off;
-    ConvLayer* L = add_conv(c, 5, name + "/attention_value [image " + std::to_string(b) + "]", c->rel_p.images(b, 1), 1,
-                            G * K, 1, 1, 1, 0, 0, 0, 0, D, false, false, false, o, 0, 0, nullptr, 0, nullptr, 0, kRuntime);
-    tab[b] = L->w.w_hi;
-    tab[B + b] = L->w.w_lo;
-  }
-  B2_CUDA(cudaMemcpy(vt, tab.data(), tab.size() * sizeof(__half*), cudaMemcpyHostToDevice));
-  Planes o = c->rel_o;
-  o.W = M;
-  add_conv(c, 5, name + "/output_linear", o, 1, M, 1, 1, 1, 0, 0, 0, 0, D, false, false, false, out, 0, 0, &h, 0, nullptr, 0,
-           kDense);
-  return 0;
-}
-
-// The deformable conv2 of block `name` (nn.py:470-486, deformable_conv2d nn.py:1642-1712) from conv1's output `in` into
-// `out`.  Steps:
-//   conv2_offset   the offsets, fp32 [B][Ho][Wo][kDeformOffsetLd]: the reference's 3x3 SAME stride-1 conv (bias, no norm,
-//                  no activation) is read at the even centres only, so it runs as a 3x3 stride-2 conv with pad 1 top / left
-//                  and 2 * Ho - H bottom (2 * Wo - W right): the same value at each centre, a quarter of the work
-//   conv2_sample   the bilinear sampler (deform.cu) -> the operand [B][Ho][Wo][9][C]
-//   conv2          a 1x1 conv with K = 9 * C over the operand: the [3,3,C,Cout] kernel packed as a 3x3 conv ([Cout][3][3][C])
-//                  lines tap k = ky * 3 + kx up with the operand's tap-major K; no bias, norm or ReLU (activation tf.identity)
-// Each image is sampled at its own offsets (DESIGN 4, Deformable conv).
-int add_deform(b2_ctx* c, const std::string& name, const Planes& in, const Planes& out) {
-  const int B = c->cfg.batch, H = in.H, W = in.W, C = in.C, Ho = (H + 1) / 2, Wo = (W + 1) / 2;
-  B2_CHECK(out.H == Ho && out.W == Wo && out.C == C, "b2_create: deformable conv2 output does not match its group");
-  float* off = c->arena.alloc<float>(static_cast<size_t>(B) * Ho * Wo * kDeformOffsetLd);
-  Planes smp;
-  B2_CHECK(off && c->alloc_planes(smp, B, Ho, Wo, 9 * C), "alloc deformable operand");
-  add_conv(c, 0, name + "/conv2_offset", in, H, W, 3, 2, 1, 1, 2 * Ho - H, 1, 2 * Wo - W, 18, false, true, false, Planes(),
-           0, 0, nullptr, 0, off, kDeformOffsetLd);
-  DeformParams dp;
-  dp.in_hi = in.hi; dp.in_lo = in.lo;
-  dp.offset = off; dp.ld_off = kDeformOffsetLd;
-  dp.H = H; dp.W = W; dp.C = C; dp.Ho = Ho; dp.Wo = Wo;
-  dp.out_hi = smp.hi; dp.out_lo = smp.lo;
-  const double esz = c->split ? 4.0 : 2.0;
-  const double taps = 9.0 * B * Ho * Wo;
-  Step& s = add_batch_step(c, 0, 17, name + "/conv2_sample [" + std::to_string(H) + "x" + std::to_string(W) + "x" +
-                                         std::to_string(C) + " ->" + std::to_string(Ho) + "x" + std::to_string(Wo) + "x9x" +
-                                         std::to_string(C) + "]",
-                           [dp](int b0, int n, cudaStream_t st) { return deform_sample_launch(dp, b0, n, st); });
-  // the input read once (the four corners of every sample are mostly L2 hits), the offsets once, the operand written once;
-  // three lerps of three operations per sample
-  s.bytes = static_cast<double>(B) * H * W * C * esz + B * static_cast<double>(Ho) * Wo * 18 * 4.0 + taps * C * esz;
-  s.flops = 9.0 * taps * C;
-  add_conv(c, 0, name + "/conv2", smp, Ho, Wo, 1, 1, 1, 0, 0, 0, 0, C, false, false, false, out, 0, 0, nullptr, 0);
-  c->stages.raw(name + "/conv2_offset", off, Stage::kF32, B, Ho, Wo, kDeformOffsetLd);
-  c->stages.planes(name + "/conv2_sample", smp);
-  return 0;
-}
-
-// TF padding SAME of a 3x3 conv (SURVEY Appendix B): pad[0..3] = top, bottom, left, right of an h x w input.  The total
-// (out - 1) * stride + 2 * dil + 1 - n puts its odd element at the bottom / right: at stride 2 on the even sizes of the
-// backbone 0 / 1, with dilation 2 then 1 / 2.
-void same_pads3(int h, int w, int stride, int dil, int pad[4]) {
-  for (int k = 0; k < 2; ++k) {
-    const int n = k == 0 ? h : w, o = (n + stride - 1) / stride;
-    const int total = std::max((o - 1) * stride + 2 * dil + 1 - n, 0);
-    pad[2 * k] = total / 2;
-    pad[2 * k + 1] = total - total / 2;
-  }
-}
-
-// The basic block `name` (resnet_basicblock nn.py:439-456, resnet_shortcut :551-566, the group's ReLU :586-587) from `x`
-// into `out` (feat channels): conv1 3x3 at `stride`, SAME, NormReLU into `t1`; the shortcut (`x` itself when it already
-// has feat channels, else convshortcut + norm into `sc`); conv2 3x3 stride 1 SAME, norm, + shortcut, ReLU.  With
-// BatchNorm the norm, shortcut and ReLU are conv epilogues; with GroupNorm the apply steps carry them.  The block has no
-// dilation, deformable or squeeze-excite branch.
-int add_basic_block(b2_ctx* c, const std::string& name, const Planes& x, int stride, const Planes& t1, const Planes& sc,
-                    const Planes& out, bool gn) {
-  const int feat = out.C;
-  int pad[4];
-  same_pads3(x.H, x.W, stride, 1, pad);
-  ConvLayer* L1 = add_conv(c, 0, name + "/conv1", x, x.H, x.W, 3, stride, 1, pad[0], pad[1], pad[2], pad[3], feat, !gn,
-                           false, !gn, t1, 0, 0, nullptr, 0);
-  B2_CHECK(L1->d.Ho() == t1.H && L1->d.Wo() == t1.W, "b2_create: basic-block conv1 output does not match its group");
-  if (gn && add_gn(c, 0, name + "/conv1/gn", t1, t1.H, t1.W, 0, 0, nullptr, 0, true)) return -1;
-  const Planes* resid = &x;
-  if (x.C != feat) {
-    // stride 2: drop the last row / column, 1x1 stride-2 VALID (nn.py:554-559)
-    ConvLayer* S = add_conv(c, 0, name + "/convshortcut", x, x.H, x.W, 1, stride, 1, 0, 1 - stride, 0, 1 - stride, feat,
-                            !gn, false, false, sc, 0, 0, nullptr, 0);
-    B2_CHECK(S->d.Ho() == sc.H && S->d.Wo() == sc.W, "b2_create: basic-block shortcut output does not match its group");
-    if (gn && add_gn(c, 0, name + "/convshortcut/gn", sc, sc.H, sc.W, 0, 0, nullptr, 0, false)) return -1;
-    resid = &sc;
-  }
-  add_conv(c, 0, name + "/conv2", t1, t1.H, t1.W, 3, 1, 1, 1, 1, 1, 1, feat, !gn, false, !gn, out, 0, 0,
-           gn ? nullptr : resid, 0);
-  if (gn && add_gn(c, 0, name + "/conv2/gn", out, out.H, out.W, 0, 0, resid, 0, true)) return -1;
-  return 0;
-}
 
 // generate_anchors.py:42-109 restated for one (stride, size): the 3 ratio anchors of a cell.
 void cell_anchors(float stride, float size, const float* ratios, float out[3][4]) {
@@ -577,13 +181,17 @@ int build_plan(b2_ctx* c) {
   B2_CHECK(B >= 1 && H >= 32 && W >= 32, "b2_create: bad frame geometry");
   B2_CHECK(cfg.fpn_num_channel == 256, "b2_create: fpn_num_channel must be 256");
   B2_CHECK(cfg.rpn_topk >= 1 && cfg.rpn_topk <= 1024, "b2_create: rpn_topk must be in [1,1024]");
+  DetPlan& P = c->plan;
+  P.batch = B;
+  P.conv_impl = cfg.conv_impl;
+  P.acc_kb = cfg.accum_chunk;
   // Images are independent through phases 0-2 (stem, ResNet, FPN, RPN head): their steps also get one launch per part of
   // the batch, each with its own plans (same tiles per image, so the results are bit-identical to the full-batch plan).
   if (cfg.conv_impl == 0) {
-    c->nsplit = 2;
-    if (const char* e = getenv("B2_SPLIT")) c->nsplit = atoi(e);   // experiment hook: 1, 2, 4, 8 batch parts
-    if (c->nsplit < 1 || c->nsplit > 8 || B % c->nsplit != 0) c->nsplit = 1;
-    c->dual = c->nsplit > 1;
+    P.nsplit = 2;
+    if (const char* e = getenv("B2_SPLIT")) P.nsplit = atoi(e);   // experiment hook: 1, 2, 4, 8 batch parts
+    if (P.nsplit < 1 || P.nsplit > 8 || B % P.nsplit != 0) P.nsplit = 1;
+    P.dual = P.nsplit > 1;
   }
   // ---- geometry (nn.py:843-944, tf_pad_reverse=True) ----
   const int PH = (H + 31) / 32 * 32, PW = (W + 31) / 32 * 32;
@@ -610,17 +218,17 @@ int build_plan(b2_ctx* c) {
 
   // ---- input + stem + pool (phase 0) ----
   c->img_bytes = static_cast<size_t>(B) * H * W * 3 * (cfg.input_dtype == 1 ? 1 : 4);
-  c->img = c->arena.alloc<uint8_t>(c->img_bytes);
-  c->range_flag = c->arena.alloc<unsigned int>(1);
-  B2_CHECK(c->range_flag != nullptr, "out of device memory (range flag)");
+  c->img = P.arena.alloc<uint8_t>(c->img_bytes);
+  P.range_flag = P.arena.alloc<unsigned int>(1);
+  B2_CHECK(P.range_flag != nullptr, "out of device memory (range flag)");
   B2_CUDA(cudaMallocHost(&c->h_range, 3 * sizeof(unsigned int)));
   c->h_range[0] = c->h_range[1] = c->h_range[2] = 0;
   // compact stem operand [B][c1h + 3][c1w + 3][16]; conv0 reads 64-channel pixels out of it with a pixel stride of 16 (stem.cu)
-  B2_CHECK(c->alloc_planes(c->stem_u, B, c->c1h + 3, c->c1w + 3, 16), "alloc stem operand");
-  B2_CHECK(c->alloc_planes(c->c1, B, c->c1h, c->c1w, 64), "alloc c1");
-  B2_CHECK(c->alloc_planes(c->pool, B, c->ch[0], c->cw[0], 64), "alloc pool");
-  const double esz = c->split ? 4.0 : 2.0;
-  add_batch_step(c, 0, 1, "", [c](int b0, int n, cudaStream_t st) {
+  B2_CHECK(P.alloc_planes(c->stem_u, B, c->c1h + 3, c->c1w + 3, 16), "alloc stem operand");
+  B2_CHECK(P.alloc_planes(c->c1, B, c->c1h, c->c1w, 64), "alloc c1");
+  B2_CHECK(P.alloc_planes(c->pool, B, c->ch[0], c->cw[0], 64), "alloc pool");
+  const double esz = P.split ? 4.0 : 2.0;
+  add_batch_step(P, 0, kStepStemPack, "", [c](int b0, int n, cudaStream_t st) {
     const Planes u = c->stem_u.images(b0, n);
     return stem_pack16_launch(static_cast<const uint8_t*>(c->img) + static_cast<size_t>(b0) * (c->img_bytes / c->cfg.batch),
                               c->cfg.input_dtype == 1, n, c->cfg.height, c->cfg.width, u.hi, u.lo, u.H, u.W, st);
@@ -635,20 +243,25 @@ int build_plan(b2_ctx* c) {
   // wins (nn.py:864-868)
   const bool basic = c->ext.use_basic_block != 0 && !rx;
   const bool se = cfg.use_se != 0 && !rx && !basic;   // squeeze-excite bottlenecks (nn.py:506-519)
+  const ConvAffine norm = gn ? kNoAffine : kBatchNorm;
   // conv0 as a 4x1 VALID conv over the packed operand (see stem.cu), BN + ReLU in the epilogue
   {
     Planes view = c->stem_u;
     view.C = 64;                       // one GEMM pixel = 4 consecutive operand pixels
-    add_conv(c, 0, "conv0", view, c->c1h + 3, c->c1w, 4, 1, 1, 0, 0, 0, 0, 64, !gn, false, !gn, c->c1, 0, 0, nullptr, 0,
-             nullptr, 0, kStem, 1, 16);
-    if (gn && add_gn(c, 0, "conv0/gn", c->c1, c->c1h, c->c1w, 0, 0, nullptr, 0, true)) return -1;
+    ConvDesc d = conv_desc(4, 64);
+    d.S = 1;
+    d.in_H = c->c1h + 3; d.in_W = c->c1w;
+    d.in_ld = 16;
+    d.relu = !gn;
+    add_conv(P, 0, "conv0", view, d, norm, c->c1, nullptr, kStem);
+    if (gn && add_gn(P, 0, "conv0/gn", c->c1, c->c1h, c->c1w, 0, 0, nullptr, 0, true)) return -1;
   }
-  add_batch_step(c, 0, 2, "", [c](int b0, int n, cudaStream_t st) {
+  add_batch_step(P, 0, kStepMaxpool, "", [c](int b0, int n, cudaStream_t st) {
     const Planes a = c->c1.images(b0, n), p = c->pool.images(b0, n);
     return maxpool_launch(a.hi, a.lo, n, c->c1h, c->c1w, 64, p.hi, p.lo, c->ch[0], c->cw[0], st);
   }).bytes = (static_cast<double>(c->c1.elems()) + c->pool.elems()) * esz;
-  c->stages.planes("c1", c->c1);
-  c->stages.planes("pool", c->pool);
+  P.stages.planes("c1", c->c1);
+  P.stages.planes("pool", c->pool);
 
   // ---- ResNet groups (nn.py:459-588) ----
   Planes cur = c->pool;
@@ -658,117 +271,66 @@ int build_plan(b2_ctx* c) {
     const int gh = c->ch[g], gw = c->cw[g];
     const int out_c = basic ? feat : feat * 4;   // the blocks' output width (resnet_shortcut's n_out)
     Planes pingpong[2];
-    B2_CHECK(c->alloc_planes(pingpong[0], B, gh, gw, out_c), "alloc group out");
-    B2_CHECK(c->alloc_planes(pingpong[1], B, gh, gw, out_c), "alloc group out");
+    B2_CHECK(P.alloc_planes(pingpong[0], B, gh, gw, out_c), "alloc group out");
+    B2_CHECK(P.alloc_planes(pingpong[1], B, gh, gw, out_c), "alloc group out");
+    // a bottleneck's conv1 writes t1_first in the first block (the previous group's size), conv2 writes t2_first where it
+    // changes the size (stride 2: with dilation its pad row / column must stay zero, which t2 does not keep)
     Planes t1_first, t1, t2, t2_first, sc;
-    if (!basic) B2_CHECK(c->alloc_planes(t1_first, B, cur.H, cur.W, mid), "alloc t1");
-    B2_CHECK(c->alloc_planes(t1, B, gh, gw, mid), "alloc t1");   // a basic block's conv1 output is gh x gw at any stride
+    if (!basic) B2_CHECK(P.alloc_planes(t1_first, B, cur.H, cur.W, mid), "alloc t1");
+    B2_CHECK(P.alloc_planes(t1, B, gh, gw, mid), "alloc t1");   // a basic block's conv1 output is gh x gw at any stride
     if (!basic) {
-      B2_CHECK(c->alloc_planes(t2, B, gh, gw, mid), "alloc t2");
-      B2_CHECK(c->alloc_planes(t2_first, B, gh, gw, mid), "alloc t2");
+      B2_CHECK(P.alloc_planes(t2, B, gh, gw, mid), "alloc t2");
+      B2_CHECK(P.alloc_planes(t2_first, B, gh, gw, mid), "alloc t2");
     }
-    B2_CHECK(c->alloc_planes(sc, B, gh, gw, out_c), "alloc shortcut");
+    B2_CHECK(P.alloc_planes(sc, B, gh, gw, out_c), "alloc shortcut");
     for (int i = 0; i < count; ++i) {
       const std::string p = "group" + std::to_string(g) + "/block" + std::to_string(i);
       const int stride = (g > 0 && i == 0) ? 2 : 1;
-      if (basic) {
-        if (add_basic_block(c, p, cur, stride, t1, sc, pingpong[i & 1], gn)) return -1;
-        cur = pingpong[i & 1];
-        continue;
-      }
-      const bool in_last3 = i >= count - 3;
-      const int dil = (g == 3 && cfg.use_dilations && in_last3) ? 2 : 1;
-      const Planes& x = cur;
-      const Planes& a1 = (i == 0) ? t1_first : t1;
-      add_conv(c, 0, p + "/conv1", x, x.H, x.W, 1, 1, 1, 0, 0, 0, 0, mid, !gn, false, !gn, a1, 0, 0, nullptr, 0);
-      if (gn && add_gn(c, 0, p + "/conv1/gn", a1, a1.H, a1.W, 0, 0, nullptr, 0, true)) return -1;
-      const Planes* a2 = &t2;
-      // use_deformable (nn.py:470-486, 577-581): a stride-2 block among the last 3 of its group; the ResNeXt block has no
-      // deformable branch
-      const bool deform = cfg.use_deformable != 0 && !rx && stride == 2 && in_last3;
-      if (deform) {
-        B2_CHECK(dil == 1, "b2_create: use_deformable cannot be combined with use_dilations: " + p + " pads its deformable "
-                           "conv2 output [1, 0] (nn.py:493-497), but that output is ceil(h/2), not the dilated conv's h/2 - 1, "
-                           "so the reference's residual sum fails (24x41 against 23x40 at 720x1280)");
-        a2 = &t2_first;
-        if (add_deform(c, p, a1, *a2)) return -1;
-      } else if (rx) {
-        // 3x3 split=32, padding SAME (nn.py:537-540): TF pads the total (out - 1) * stride + (3 - 1) * dil + 1 - in
-        // with the odd element at the bottom / right (SURVEY Appendix B) -- at stride 2 on the even sizes here 0 / 1,
-        // with dilation 2 then 1 / 2 -- and nothing follows the conv (no [1,0] pad, no output offset)
-        if (stride == 2) a2 = &t2_first;
-        int pad[4];   // top, bottom, left, right
-        same_pads3(a1.H, a1.W, stride, dil, pad);
-        ConvLayer* L2 = add_conv(c, 0, p + "/conv2", a1, a1.H, a1.W, 3, stride, dil, pad[0], pad[1], pad[2], pad[3], mid,
-                                 !gn, false, !gn, *a2, 0, 0, nullptr, 0, nullptr, 0, kGrouped, 0, 0, 32);
-        B2_CHECK(L2->d.Ho() == a2->H && L2->d.Wo() == a2->W, "b2_create: ResNeXt conv2 output does not match its group");
-        if (gn && add_gn(c, 0, p + "/conv2/gn", *a2, a2->H, a2->W, 0, 0, nullptr, 0, true)) return -1;
-      } else if (stride == 2) {
-        // pad [1,0] + 3x3 stride-2 VALID (nn.py:487-492); with dilation the output is padded [1,0] again
-        // (nn.py:493-497): written at offset (1,1) of a buffer whose first row/col stay zero.  GroupNorm + ReLU run
-        // before that pad (nn.py:490-497): their view is the conv output, so the pad row / column stay out of the
-        // statistics and stay 0.
-        a2 = &t2_first;
-        const int off = dil != 1 ? 1 : 0;
-        ConvLayer* L2 = add_conv(c, 0, p + "/conv2", a1, a1.H, a1.W, 3, 2, dil, 1, 0, 1, 0, mid, !gn, false, !gn, *a2, off,
-                             off, nullptr, 0);
-        if (gn && add_gn(c, 0, p + "/conv2/gn", *a2, L2->d.Ho(), L2->d.Wo(), off, off, nullptr, 0, true)) return -1;
-      } else {
-        add_conv(c, 0, p + "/conv2", a1, a1.H, a1.W, 3, 1, dil, dil, dil, dil, dil, mid, !gn, false, !gn, *a2, 0,
-                 0, nullptr, 0);
-        if (gn && add_gn(c, 0, p + "/conv2/gn", *a2, a2->H, a2->W, 0, 0, nullptr, 0, true)) return -1;
-      }
-      const Planes* resid = &x;
-      if (x.C != feat * 4) {
-        // resnet_shortcut (nn.py:551-566): stride 2 => drop last row/col, 1x1 stride-2 VALID
-        if (stride == 2)
-          add_conv(c, 0, p + "/convshortcut", x, x.H, x.W, 1, 2, 1, 0, -1, 0, -1, feat * 4, !gn, false, false, sc, 0,
-                   0, nullptr, 0);
-        else
-          add_conv(c, 0, p + "/convshortcut", x, x.H, x.W, 1, 1, 1, 0, 0, 0, 0, feat * 4, !gn, false, false, sc, 0,
-                   0, nullptr, 0);
-        if (gn && add_gn(c, 0, p + "/convshortcut/gn", sc, sc.H, sc.W, 0, 0, nullptr, 0, false)) return -1;
-        resid = &sc;
-      }
       const Planes& out = pingpong[i & 1];
-      // relu(norm(conv3) + shortcut) (nn.py:512-521, 586-587): with BatchNorm in the conv epilogue, with GroupNorm in its
-      // apply step; with use_se the norm alone, then the gate, the shortcut and the ReLU in the SE apply step
-      const bool epi = !gn && !se;
-      add_conv(c, 0, p + "/conv3", *a2, a2->H, a2->W, 1, 1, 1, 0, 0, 0, 0, feat * 4, !gn, false, epi, out, 0, 0,
-               epi ? resid : nullptr, 0);
-      if (gn && add_gn(c, 0, p + "/conv3/gn", out, out.H, out.W, 0, 0, se ? nullptr : resid, 0, !se)) return -1;
-      if (se && add_se(c, 0, p, out, *resid)) return -1;
+      if (basic) {
+        if (add_basic_block(P, p, cur, stride, BlockBufs{t1, Planes(), sc, out}, gn)) return -1;
+      } else {
+        const bool in_last3 = i >= count - 3;
+        const int dil = (g == 3 && cfg.use_dilations && in_last3) ? 2 : 1;
+        // use_deformable (nn.py:470-486, 577-581): a stride-2 block among the last 3 of its group; the ResNeXt block has
+        // no deformable branch
+        const bool deform = cfg.use_deformable != 0 && !rx && stride == 2 && in_last3;
+        const BlockBufs bufs{i == 0 ? t1_first : t1, stride == 2 ? t2_first : t2, sc, out};
+        if (add_bottleneck(P, p, cur, stride, dil, bufs, gn, se, rx, deform)) return -1;
+      }
       cur = out;
     }
     c->cfeat[g] = cur;
-    c->stages.planes("c" + std::to_string(g + 2), cur);
+    P.stages.planes("c" + std::to_string(g + 2), cur);
   }
 
   // ---- FPN (nn.py:947-1014), phase 1 ----
   const int nc = cfg.fpn_num_channel;
   for (int i = 3; i >= 0; --i) {
-    B2_CHECK(c->alloc_planes(c->lat[i], B, c->ch[i], c->cw[i], nc), "alloc lateral");
+    B2_CHECK(P.alloc_planes(c->lat[i], B, c->ch[i], c->cw[i], nc), "alloc lateral");
     const std::string nm = "fpn/lateral_1x1_c" + std::to_string(i + 2);
     // use_gn: GroupNorm of the lateral before the top-down sum (gn_c*, nn.py:987-990); its apply step does the
     // nearest-2x upsample-add that the conv epilogue does otherwise
     const Planes* up = i < 3 ? &c->lat[i + 1] : nullptr;
-    add_conv(c, 1, nm, c->cfeat[i], c->ch[i], c->cw[i], 1, 1, 1, 0, 0, 0, 0, nc, false, true, false, c->lat[i], 0, 0,
-             gn ? nullptr : up, 1);
-    if (gn && add_gn(c, 1, "fpn/gn_c" + std::to_string(i + 2), c->lat[i], c->ch[i], c->cw[i], 0, 0, up, 1, false))
+    ConvDesc d = conv_desc(1, nc);
+    d.res_shift = 1;
+    add_conv(P, 1, nm, c->cfeat[i], d, kBias, c->lat[i], gn ? nullptr : up);
+    if (gn && add_gn(P, 1, "fpn/gn_c" + std::to_string(i + 2), c->lat[i], c->ch[i], c->cw[i], 0, 0, up, 1, false))
       return -1;
   }
   for (int i = 0; i < 4; ++i) {
-    B2_CHECK(c->alloc_planes(c->pfeat[i], B, c->pfh[i], c->pfw[i], nc), "alloc p");
+    B2_CHECK(P.alloc_planes(c->pfeat[i], B, c->pfh[i], c->pfw[i], nc), "alloc p");
     const std::string nm = "fpn/posthoc_3x3_p" + std::to_string(i + 2);
-    add_conv(c, 1, nm, c->lat[i], c->ch[i], c->cw[i], 3, 1, 1, 1, 1, 1, 1, nc, false, true, false, c->pfeat[i], 0, 0,
-             nullptr, 0);
+    ConvDesc d = conv_desc(3, nc);
+    pad_all(d, 1);
+    add_conv(P, 1, nm, c->lat[i], d, kBias, c->pfeat[i]);
     // gn_p* (nn.py:1007-1009) over the whole, uncropped level; p6 below subsamples the normalised p5
-    if (gn && add_gn(c, 1, "fpn/gn_p" + std::to_string(i + 2), c->pfeat[i], c->pfh[i], c->pfw[i], 0, 0, nullptr, 0, false))
+    if (gn && add_gn(P, 1, "fpn/gn_p" + std::to_string(i + 2), c->pfeat[i], c->pfh[i], c->pfw[i], 0, 0, nullptr, 0, false))
       return -1;
-    c->stages.planes("p" + std::to_string(i + 2), c->pfeat[i]);
+    P.stages.planes("p" + std::to_string(i + 2), c->pfeat[i]);
   }
-  B2_CHECK(c->alloc_planes(c->pfeat[4], B, c->pfh[4], c->pfw[4], nc), "alloc p6");
-  add_batch_step(c, 1, 3, "", [c](int b0, int n, cudaStream_t st) {
+  B2_CHECK(P.alloc_planes(c->pfeat[4], B, c->pfh[4], c->pfw[4], nc), "alloc p6");
+  add_batch_step(P, 1, kStepP6Subsample, "", [c](int b0, int n, cudaStream_t st) {
     const Planes p5 = c->pfeat[3].images(b0, n), p6 = c->pfeat[4].images(b0, n);
     const size_t total = static_cast<size_t>(n) * p6.H * p6.W * (p6.C / 8);
     subsample2_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, st>>>(p5.hi, p5.lo, n, p5.H, p5.W, p5.C, p6.hi,
@@ -776,18 +338,19 @@ int build_plan(b2_ctx* c) {
     B2_CUDA(cudaGetLastError());
     return 0;
   });
-  c->stages.planes("p6", c->pfeat[4]);
+  P.stages.planes("p6", c->pfeat[4]);
 
   // ---- RPN head (models.py:979-1009), phase 2; class+box 1x1 fused into one N=15 GEMM ----
   for (int i = 0; i < 5; ++i) {
-    B2_CHECK(c->alloc_planes(c->rpn_h[i], B, c->ph[i], c->pw[i], nc), "alloc rpn hidden");
-    ConvLayer* L0 = add_conv(c, 2, "rpn/conv0", c->pfeat[i], c->ph[i], c->pw[i], 3, 1, 1, 1, 1, 1, 1, nc, false, true,
-                         true, c->rpn_h[i], 0, 0, nullptr, 0);
-    (void)L0;
-    c->rpn_out[i] = c->arena.alloc<float>(static_cast<size_t>(B) * c->ph[i] * c->pw[i] * 16 + 16 * 128);
-    add_conv(c, 2, "rpn/classbox", c->rpn_h[i], c->ph[i], c->pw[i], 1, 1, 1, 0, 0, 0, 0, 15, false, true, false,
-             Planes(), 0, 0, nullptr, 0, c->rpn_out[i], 16, kRpnOut);
-    c->stages.raw("rpn_l" + std::to_string(i), c->rpn_out[i], Stage::kF32, B, c->ph[i], c->pw[i], 16);
+    B2_CHECK(P.alloc_planes(c->rpn_h[i], B, c->ph[i], c->pw[i], nc), "alloc rpn hidden");
+    ConvDesc d = conv_desc(3, nc);
+    d.in_H = c->ph[i]; d.in_W = c->pw[i];   // the cropped level
+    pad_all(d, 1);
+    d.relu = 1;
+    add_conv(P, 2, "rpn/conv0", c->pfeat[i], d, kBias, c->rpn_h[i]);
+    c->rpn_out[i] = P.arena.alloc<float>(static_cast<size_t>(B) * c->ph[i] * c->pw[i] * 16 + 16 * 128);
+    add_conv_f32(P, 2, "rpn/classbox", c->rpn_h[i], conv_desc(1, 15), kBias, c->rpn_out[i], 16, kRpnOut);
+    P.stages.raw("rpn_l" + std::to_string(i), c->rpn_out[i], Stage::kF32, B, c->ph[i], c->pw[i], 16);
   }
 
   // ---- proposals (phase 3) ----
@@ -811,24 +374,24 @@ int build_plan(b2_ctx* c) {
   rp.min_size = cfg.rpn_min_size;
   rp.multi = cfg.multi_semantics;
   rp.nms_thr = cfg.rpn_nms_thres;
-  rp.lvl_boxes = c->arena.alloc<float>(static_cast<size_t>(B) * 5 * K * 4);
-  rp.lvl_scores = c->arena.alloc<float>(static_cast<size_t>(B) * 5 * K);
-  rp.lvl_count = c->arena.alloc<int>(B * 5);
-  rp.prop_boxes = c->arena.alloc<float>(static_cast<size_t>(B) * K * 4);
-  rp.prop_scores = c->arena.alloc<float>(static_cast<size_t>(B) * K);
-  rp.prop_count = c->arena.alloc<int>(B);
-  add_batch_step(c, 3, 4, "", [c](int, int, cudaStream_t st) { return rpn_proposals_launch(c->rpn, st); }, 2);
-  c->stages.raw("lvl_boxes", rp.lvl_boxes, Stage::kF32, B, 5, K, 4);
-  c->stages.raw("lvl_scores", rp.lvl_scores, Stage::kF32, B, 5, K, 1);
-  c->stages.raw("lvl_count", rp.lvl_count, Stage::kI32, B, 5, 1, 1);
-  c->stages.raw("proposal_boxes", rp.prop_boxes, Stage::kF32, B, K, 4, 1);
-  c->stages.raw("proposal_scores", rp.prop_scores, Stage::kF32, B, K, 1, 1);
-  c->stages.raw("proposal_count", rp.prop_count, Stage::kI32, B, 1, 1, 1);
+  rp.lvl_boxes = P.arena.alloc<float>(static_cast<size_t>(B) * 5 * K * 4);
+  rp.lvl_scores = P.arena.alloc<float>(static_cast<size_t>(B) * 5 * K);
+  rp.lvl_count = P.arena.alloc<int>(B * 5);
+  rp.prop_boxes = P.arena.alloc<float>(static_cast<size_t>(B) * K * 4);
+  rp.prop_scores = P.arena.alloc<float>(static_cast<size_t>(B) * K);
+  rp.prop_count = P.arena.alloc<int>(B);
+  add_batch_step(P, 3, kStepRpnProposals, "", [c](int, int, cudaStream_t st) { return rpn_proposals_launch(c->rpn, st); }, 2);
+  P.stages.raw("lvl_boxes", rp.lvl_boxes, Stage::kF32, B, 5, K, 4);
+  P.stages.raw("lvl_scores", rp.lvl_scores, Stage::kF32, B, 5, K, 1);
+  P.stages.raw("lvl_count", rp.lvl_count, Stage::kI32, B, 5, 1, 1);
+  P.stages.raw("proposal_boxes", rp.prop_boxes, Stage::kF32, B, K, 4, 1);
+  P.stages.raw("proposal_scores", rp.prop_scores, Stage::kF32, B, K, 1, 1);
+  P.stages.raw("proposal_count", rp.prop_count, Stage::kI32, B, 1, 1, 1);
 
   // ---- ROIAlign of the proposals (phase 4) ----
   const int M = B * K;
   const int Mpad = (M + 127) / 128 * 128;
-  B2_CHECK(c->alloc_planes(c->roi_feat, 1, 1, Mpad, 49 * nc), "alloc roi feat");
+  B2_CHECK(P.alloc_planes(c->roi_feat, 1, 1, Mpad, 49 * nc), "alloc roi feat");
   RoiAlignParams& r1 = c->roi1;
   memset(&r1, 0, sizeof(r1));
   for (int i = 0; i < 4; ++i) {
@@ -841,75 +404,73 @@ int build_plan(b2_ctx* c) {
   r1.C = nc; r1.B = B; r1.rois_per_image = K;
   r1.boxes = rp.prop_boxes; r1.count = rp.prop_count;
   r1.out_hi = c->roi_feat.hi; r1.out_lo = c->roi_feat.lo; r1.out_nchw = nullptr;
-  add_batch_step(c, 4, 5, "", [c](int, int, cudaStream_t st) { return roialign_launch(c->roi1, st); });
-  c->stages.planes("roi_feat", c->roi_feat);
+  add_batch_step(P, 4, kStepRoialignProposals, "", [c](int, int, cudaStream_t st) { return roialign_launch(c->roi1, st); });
+  P.stages.planes("roi_feat", c->roi_feat);
 
   // ---- box head (models.py:1030-1108), phase 5: fc6, fc7, class+box outputs fused (N = 5*num_class) ----
   const int dim = cfg.fc_head_dim;
   B2_CHECK(dim % 64 == 0, "b2_create: fc_head_dim must be a multiple of 64");
   const int hd = cfg.conv_head_dim;
   if (hd <= 0) {
-    B2_CHECK(c->alloc_planes(c->fc6, 1, 1, Mpad, dim), "alloc fc6");
-    B2_CHECK(c->alloc_planes(c->fc7, 1, 1, Mpad, dim), "alloc fc7");
+    B2_CHECK(P.alloc_rows(c->fc6, M, dim), "alloc fc6");
+    B2_CHECK(P.alloc_rows(c->fc7, M, dim), "alloc fc7");
   }
   const int nout = cfg.num_class + (cfg.class_agnostic ? 4 : cfg.num_class * 4);
   const int ldo = (nout + 15) / 16 * 16;
-  c->head_logits = c->arena.alloc<float>(static_cast<size_t>(Mpad) * ldo);
+  c->head_logits = P.arena.alloc<float>(static_cast<size_t>(Mpad) * ldo);
   Planes rf = c->roi_feat; rf.W = M;
+  ConvDesc fc = conv_desc(1, dim);   // fc6 / fc7 / the conv head's fc: dense + bias + ReLU
+  fc.relu = 1;
   if (hd > 0) {
     // conv_frcnn_head (models.py:1110-1125), use_conv_frcnn_head: 4 x [conv 3x3 SAME + bias + ReLU, then GroupNorm per ROI
     // if use_gn] on the [M][7][7] ROI maps (the ROIAlign rows are already (y*7+x)*256+c per ROI: M small images, as in the
     // mask head), then dense "fc" + ReLU over the NCHW flatten (fc6's row permutation with conv_head_dim channels)
     B2_CHECK(hd % 64 == 0 && hd <= 2048 && (!gn || 2048 % hd == 0),
              "b2_create: conv_head_dim must be a multiple of 64 (a power of two from 64 to 2048 with use_gn)");
-    B2_CHECK(c->alloc_planes(c->head_a, Mpad, 7, 7, hd) && c->alloc_planes(c->head_b, Mpad, 7, 7, hd), "alloc conv head");
-    B2_CHECK(c->alloc_planes(c->fc6, 1, 1, Mpad, dim), "alloc fc");
+    B2_CHECK(P.alloc_planes(c->head_a, Mpad, 7, 7, hd) && P.alloc_planes(c->head_b, Mpad, 7, 7, hd), "alloc conv head");
+    B2_CHECK(P.alloc_rows(c->fc6, M, dim), "alloc fc");
     Planes rf7 = c->roi_feat; rf7.B = M; rf7.H = 7; rf7.W = 7; rf7.C = nc;
     Planes ha = c->head_a; ha.B = M;
     Planes hb = c->head_b; hb.B = M;
     Planes cur_h = rf7;
+    ConvDesc d = conv_desc(3, hd);
+    pad_all(d, 1);
+    d.relu = 1;
     for (int k = 0; k < 4; ++k) {
       const Planes& o = (k & 1) ? hb : ha;
-      add_conv(c, 5, "fastrcnn/conv" + std::to_string(k), cur_h, 7, 7, 3, 1, 1, 1, 1, 1, 1, hd, false, true, true, o, 0, 0,
-               nullptr, 0);
-      if (gn && add_gn(c, 5, "fastrcnn/gn" + std::to_string(k), o, 7, 7, 0, 0, nullptr, 0, false, true)) return -1;
+      add_conv(P, 5, "fastrcnn/conv" + std::to_string(k), cur_h, d, kBias, o);
+      if (gn && add_gn(P, 5, "fastrcnn/gn" + std::to_string(k), o, 7, 7, 0, 0, nullptr, 0, false, true)) return -1;
       cur_h = o;
     }
     Planes flat = cur_h; flat.B = 1; flat.H = 1; flat.W = M; flat.C = 49 * hd;
-    Planes f = c->fc6; f.W = M;
-    add_conv(c, 5, "fastrcnn/fc", flat, 1, M, 1, 1, 1, 0, 0, 0, 0, dim, false, true, true, f, 0, 0, nullptr, 0, nullptr,
-             0, kFc6);
-    add_conv(c, 5, "fastrcnn/outputs", f, 1, M, 1, 1, 1, 0, 0, 0, 0, nout, false, true, false, Planes(), 0, 0, nullptr,
-             0, c->head_logits, ldo, kHeadOut);
-    c->stages.planes("fc", f);
+    const Planes& f = c->fc6;
+    add_conv(P, 5, "fastrcnn/fc", flat, fc, kBias, f, nullptr, kFc6);
+    add_conv_f32(P, 5, "fastrcnn/outputs", f, conv_desc(1, nout), kBias, c->head_logits, ldo, kHeadOut);
+    P.stages.planes("fc", f);
   } else {
-    Planes f6 = c->fc6; f6.W = M;
-    Planes f7 = c->fc7; f7.W = M;
+    const Planes &f6 = c->fc6, &f7 = c->fc7;
     // add_relation_nn (models.py:1044-1054): fc7 reads relu(fc6) + RM_r1, the outputs read relu(fc7) + RM_r2
     const bool rel = cfg.add_relation_nn != 0;
     Planes h1 = f6, h2 = f7;
     if (rel) {
       B2_CHECK(dim % 64 == 0, "b2_create: add_relation_nn needs fc_head_dim a multiple of 64");
-      B2_CHECK(c->alloc_planes(c->rm1, 1, 1, Mpad, dim) && c->alloc_planes(c->rm2, 1, 1, Mpad, dim), "alloc relation sums");
-      h1 = c->rm1; h1.W = M;
-      h2 = c->rm2; h2.W = M;
+      B2_CHECK(P.alloc_rows(c->rm1, M, dim) && P.alloc_rows(c->rm2, M, dim), "alloc relation sums");
+      h1 = c->rm1;
+      h2 = c->rm2;
     }
-    add_conv(c, 5, "fastrcnn/fc6", rf, 1, M, 1, 1, 1, 0, 0, 0, 0, dim, false, true, true, f6, 0, 0, nullptr, 0, nullptr,
-             0, kFc6);
-    if (rel && add_relation(c, "fastrcnn/RM_r1", f6, h1)) return -1;
-    add_conv(c, 5, "fastrcnn/fc7", h1, 1, M, 1, 1, 1, 0, 0, 0, 0, dim, false, true, true, f7, 0, 0, nullptr, 0, nullptr,
-             0, kDense);
-    if (rel && add_relation(c, "fastrcnn/RM_r2", f7, h2)) return -1;
-    add_conv(c, 5, "fastrcnn/outputs", h2, 1, M, 1, 1, 1, 0, 0, 0, 0, nout, false, true, false, Planes(), 0, 0, nullptr,
-             0, c->head_logits, ldo, kHeadOut);
-    c->stages.planes("fc6", f6);
-    c->stages.planes("fc7", f7);
+    add_conv(P, 5, "fastrcnn/fc6", rf, fc, kBias, f6, nullptr, kFc6);
+    if (rel && add_relation(P, "fastrcnn/RM_r1", B, K, dim, rp.prop_boxes, rp.prop_count, f6, h1)) return -1;
+    add_conv(P, 5, "fastrcnn/fc7", h1, fc, kBias, f7, nullptr, kDense);
+    if (rel && add_relation(P, "fastrcnn/RM_r2", B, K, dim, rp.prop_boxes, rp.prop_count, f7, h2)) return -1;
+    add_conv_f32(P, 5, "fastrcnn/outputs", h2, conv_desc(1, nout), kBias, c->head_logits, ldo, kHeadOut);
+    P.stages.planes("fc6", f6);
+    P.stages.planes("fc7", f7);
     if (rel) {
-      c->stages.planes("rm_r1", h1);
-      c->stages.planes("rm_r2", h2);
+      P.stages.planes("rm_r1", h1);
+      P.stages.planes("rm_r2", h2);
     }
   }
-  c->stages.raw("head_logits", c->head_logits, Stage::kF32, B, K, ldo, 1);
+  P.stages.raw("head_logits", c->head_logits, Stage::kF32, B, K, ldo, 1);
 
   // ---- post-processing (phase 6) ----
   HeadPostParams& hp = c->post;
@@ -925,31 +486,31 @@ int build_plan(b2_ctx* c) {
   hp.score_thresh = cfg.multi_semantics ? -INFINITY : cfg.result_score_thres;
   hp.nms_thr = cfg.fastrcnn_nms_iou_thres;
   hp.max_per_class = R; hp.max_total = R;
-  hp.probs = c->arena.alloc<float>(static_cast<size_t>(M) * cfg.num_class);
-  hp.dec_boxes = c->arena.alloc<float>(static_cast<size_t>(M) * nc1 * 4);
-  hp.cls_keep = c->arena.alloc<int>(static_cast<size_t>(B) * nc1 * R);
-  hp.cls_count = c->arena.alloc<int>(B * nc1);
-  hp.final_boxes = c->arena.alloc<float>(static_cast<size_t>(B) * R * 4);
-  hp.final_probs = c->arena.alloc<float>(static_cast<size_t>(B) * R);
-  hp.final_labels = c->arena.alloc<int>(static_cast<size_t>(B) * R);
-  hp.final_count = c->arena.alloc<int>(B);
-  add_batch_step(c, 6, 6, "", [c](int, int, cudaStream_t st) { return head_post_launch(c->post, st); }, 3);
-  c->stages.raw("probs", hp.probs, Stage::kF32, B, K, cfg.num_class, 1);
-  c->stages.raw("dec_boxes", hp.dec_boxes, Stage::kF32, B, K, nc1, 4);
-  c->stages.raw("final_boxes", hp.final_boxes, Stage::kF32, B, R, 4, 1);
-  c->stages.raw("final_probs", hp.final_probs, Stage::kF32, B, R, 1, 1);
-  c->stages.raw("final_labels", hp.final_labels, Stage::kI32, B, R, 1, 1);
-  c->stages.raw("final_count", hp.final_count, Stage::kI32, B, 1, 1, 1);
+  hp.probs = P.arena.alloc<float>(static_cast<size_t>(M) * cfg.num_class);
+  hp.dec_boxes = P.arena.alloc<float>(static_cast<size_t>(M) * nc1 * 4);
+  hp.cls_keep = P.arena.alloc<int>(static_cast<size_t>(B) * nc1 * R);
+  hp.cls_count = P.arena.alloc<int>(B * nc1);
+  hp.final_boxes = P.arena.alloc<float>(static_cast<size_t>(B) * R * 4);
+  hp.final_probs = P.arena.alloc<float>(static_cast<size_t>(B) * R);
+  hp.final_labels = P.arena.alloc<int>(static_cast<size_t>(B) * R);
+  hp.final_count = P.arena.alloc<int>(B);
+  add_batch_step(P, 6, kStepHeadPost, "", [c](int, int, cudaStream_t st) { return head_post_launch(c->post, st); }, 3);
+  P.stages.raw("probs", hp.probs, Stage::kF32, B, K, cfg.num_class, 1);
+  P.stages.raw("dec_boxes", hp.dec_boxes, Stage::kF32, B, K, nc1, 4);
+  P.stages.raw("final_boxes", hp.final_boxes, Stage::kF32, B, R, 4, 1);
+  P.stages.raw("final_probs", hp.final_probs, Stage::kF32, B, R, 1, 1);
+  P.stages.raw("final_labels", hp.final_labels, Stage::kI32, B, R, 1, 1);
+  P.stages.raw("final_count", hp.final_count, Stage::kI32, B, 1, 1, 1);
 
   // ---- fpn_box_feat: ROIAlign of the final boxes (models.py:972-973), phase 7 ----
-  c->box_feat = c->arena.alloc<float>(static_cast<size_t>(B) * R * nc * 49);
-  c->box_feat_pooled = c->arena.alloc<float>(static_cast<size_t>(B) * R * nc);
+  c->box_feat = P.arena.alloc<float>(static_cast<size_t>(B) * R * nc * 49);
+  c->box_feat_pooled = P.arena.alloc<float>(static_cast<size_t>(B) * R * nc);
   RoiAlignParams& r2 = c->roi2;
   r2 = r1;
   r2.rois_per_image = R;
   r2.boxes = hp.final_boxes; r2.count = hp.final_count;
   r2.out_hi = nullptr; r2.out_lo = nullptr; r2.out_nchw = c->box_feat;
-  add_batch_step(c, 7, 7, "", [c](int, int, cudaStream_t st) {
+  add_batch_step(P, 7, kStepRoialignFinal, "", [c](int, int, cudaStream_t st) {
     if (roialign_launch(c->roi2, st)) return -1;
     const int rows = c->cfg.batch * c->cfg.result_per_im;
     pool_feat_kernel<<<(rows * c->cfg.fpn_num_channel + 255) / 256, 256, 0, st>>>(c->box_feat, rows, c->cfg.fpn_num_channel,
@@ -957,38 +518,39 @@ int build_plan(b2_ctx* c) {
     B2_CUDA(cudaGetLastError());
     return 0;
   }, 2);
-  c->stages.raw("fpn_box_feat", c->box_feat, Stage::kF32, static_cast<int64_t>(B) * R, nc, 7, 7);
+  P.stages.raw("fpn_box_feat", c->box_feat, Stage::kF32, static_cast<int64_t>(B) * R, nc, 7, 7);
 
   // ---- mask head (models.py:934-961, 1173-1199), phase 7, only with cfg.add_mask ----
   if (cfg.add_mask) {
     B2_CHECK(cfg.num_class >= 2, "b2_create: add_mask needs at least one foreground class");
     const int MR = B * R, md = 256;                  // mrcnn_head_dim (obj_detect_tracking.py:324)
-    B2_CHECK(c->alloc_planes(c->mask_a, MR, 14, 14, md), "alloc mask head a");
-    B2_CHECK(c->alloc_planes(c->mask_b, MR, 14, 14, md), "alloc mask head b");
-    B2_CHECK(c->alloc_planes(c->mask_up, MR, 14, 14, 4 * md), "alloc mask head deconv");
+    B2_CHECK(P.alloc_planes(c->mask_a, MR, 14, 14, md), "alloc mask head a");
+    B2_CHECK(P.alloc_planes(c->mask_b, MR, 14, 14, md), "alloc mask head b");
+    B2_CHECK(P.alloc_planes(c->mask_up, MR, 14, 14, 4 * md), "alloc mask head deconv");
     RoiAlignParams& r3 = c->roi3;
     r3 = r1;
     r3.rois_per_image = R;
     r3.boxes = hp.final_boxes; r3.count = hp.final_count;
     r3.out_hi = c->mask_a.hi; r3.out_lo = c->mask_a.lo; r3.out_nchw = nullptr; r3.out_res = 14;
-    add_batch_step(c, 7, 8, "", [c](int, int, cudaStream_t st) { return roialign_launch(c->roi3, st); });
+    add_batch_step(P, 7, kStepRoialignMask, "", [c](int, int, cudaStream_t st) { return roialign_launch(c->roi3, st); });
     const Planes* pp[2] = {&c->mask_a, &c->mask_b};
-    for (int k = 0; k < 4; ++k)                      // conv2d 3x3 SAME + bias + ReLU
-      add_conv(c, 7, "maskrcnn/fcn" + std::to_string(k), *pp[k & 1], 14, 14, 3, 1, 1, 1, 1, 1, 1, md, false, true, true,
-               *pp[(k + 1) & 1], 0, 0, nullptr, 0);
+    ConvDesc fcn = conv_desc(3, md);                 // conv2d 3x3 SAME + bias + ReLU
+    pad_all(fcn, 1);
+    fcn.relu = 1;
+    for (int k = 0; k < 4; ++k) add_conv(P, 7, "maskrcnn/fcn" + std::to_string(k), *pp[k & 1], fcn, kBias, *pp[(k + 1) & 1]);
     // Conv2DTranspose 2x2 stride 2: no overlap between taps, so it is a 1x1 conv onto (tap, channel) outputs
-    add_conv(c, 7, "maskrcnn/deconv", c->mask_a, 14, 14, 1, 1, 1, 0, 0, 0, 0, 4 * md, false, true, true, c->mask_up, 0, 0,
-             nullptr, 0, nullptr, 0, kDeconv);
+    ConvDesc deconv = conv_desc(1, 4 * md);
+    deconv.relu = 1;
+    add_conv(P, 7, "maskrcnn/deconv", c->mask_a, deconv, kBias, c->mask_up, nullptr, kDeconv);
     // the 1x1 class conv commutes with the pixel shuffle: apply it to the (pixel, tap) rows directly
     const int rows = MR * 196 * 4, rows_pad = (rows + 127) / 128 * 128;
     c->mask_ld = (cfg.num_class - 1 + 15) / 16 * 16;
-    c->mask_logits = c->arena.alloc<float>(static_cast<size_t>(rows_pad) * c->mask_ld);
+    c->mask_logits = P.arena.alloc<float>(static_cast<size_t>(rows_pad) * c->mask_ld);
     Planes up_rows = c->mask_up;
     up_rows.B = 1; up_rows.H = 1; up_rows.W = rows; up_rows.C = md;
-    add_conv(c, 7, "maskrcnn/conv", up_rows, 1, rows, 1, 1, 1, 0, 0, 0, 0, cfg.num_class - 1, false, true, false, Planes(),
-             0, 0, nullptr, 0, c->mask_logits, c->mask_ld);
-    c->final_masks = c->arena.alloc<float>(static_cast<size_t>(MR) * 784);
-    add_batch_step(c, 7, 9, "", [c](int, int, cudaStream_t st) {
+    add_conv_f32(P, 7, "maskrcnn/conv", up_rows, conv_desc(1, cfg.num_class - 1), kBias, c->mask_logits, c->mask_ld);
+    c->final_masks = P.arena.alloc<float>(static_cast<size_t>(MR) * 784);
+    add_batch_step(P, 7, kStepMaskSelect, "", [c](int, int, cudaStream_t st) {
       const size_t total = static_cast<size_t>(c->cfg.batch) * c->cfg.result_per_im * 784;
       mask_select_kernel<<<static_cast<unsigned>(std::min<size_t>((total + 255) / 256, 132 * 32)), 256, 0, st>>>(
           c->mask_logits, c->mask_ld, c->post.final_labels, c->post.final_count, c->cfg.batch, c->cfg.result_per_im,
@@ -996,203 +558,44 @@ int build_plan(b2_ctx* c) {
       B2_CUDA(cudaGetLastError());
       return 0;
     });
-    c->stages.planes("mask_roi_feat", c->mask_a);       // valid right after step 8 only (ping-pong buffer)
-    c->stages.raw("mask_logits", c->mask_logits, Stage::kF32, MR, 196 * 4, c->mask_ld, 1);
-    c->stages.raw("final_masks", c->final_masks, Stage::kF32, B, R, 28, 28);
+    P.stages.planes("mask_roi_feat", c->mask_a);       // valid right after step 8 only (ping-pong buffer)
+    P.stages.raw("mask_logits", c->mask_logits, Stage::kF32, MR, 196 * 4, c->mask_ld, 1);
+    P.stages.raw("final_masks", c->final_masks, Stage::kF32, B, R, 28, 28);
   }
-
 
   // ---- tensor-core plans ----
-  if (cfg.conv_impl == 0) {
-    if (plan_convs(c->layers, c->split, c->num_sms)) return -1;
-    // the forked layers over each part of the batch: operands offset by whole images of their own buffers
-    for (ConvLayer* L : c->part_layers) {
-      if (!c->dual) break;
-      for (int h = 0; h < c->nsplit; ++h) {
-        ConvDesc d = L->d;
-        d.B = B / c->nsplit;
-        L->part_plan.emplace_back(conv_tc_plan_create(d, L->w, images(*L, h * d.B), c->split, c->num_sms));
-        if (!L->part_plan.back()) {
-          set_error(std::string("half-batch plan for ") + L->name + ": " + last_error());
-          return -1;
-        }
-      }
-    }
-  }
-  return 0;
+  return plan_layers(P, c->num_sms);
 }
 
 // The whole pass with phases 0-2 forked over nsplit streams (also valid inside a stream capture: the side streams join
 // the capture through the fork event and rejoin before the proposals).
 int enqueue_dual(b2_ctx* c) {
   B2_CUDA(cudaEventRecord(c->fork_ev, c->stream));
-  for (int h = 1; h < c->nsplit; ++h) B2_CUDA(cudaStreamWaitEvent(c->side_stream[h - 1], c->fork_ev, 0));
-  for (const Step& s : c->steps) {
+  for (int h = 1; h < c->plan.nsplit; ++h) B2_CUDA(cudaStreamWaitEvent(c->side_stream[h - 1], c->fork_ev, 0));
+  for (const Step& s : c->plan.steps) {
     if (s.phase > 2) continue;
-    for (int h = 0; h < c->nsplit; ++h)
+    for (int h = 0; h < c->plan.nsplit; ++h)
       if (s.parts[h](h == 0 ? c->stream : c->side_stream[h - 1])) return -1;
   }
-  for (int h = 1; h < c->nsplit; ++h) {
+  for (int h = 1; h < c->plan.nsplit; ++h) {
     B2_CUDA(cudaEventRecord(c->join_ev[h - 1], c->side_stream[h - 1]));
     B2_CUDA(cudaStreamWaitEvent(c->stream, c->join_ev[h - 1], 0));
   }
-  return run_steps(c->steps, ~0x7u, c->stream);
+  return run_steps(c->plan.steps, ~0x7u, c->stream);
 }
 
 int enqueue(b2_ctx* c, int mask, bool with_events) {
-  if (c->dual && !with_events && mask == B2_PHASE_ALL) return enqueue_dual(c);
-  if (!with_events) return run_steps(c->steps, mask, c->stream);
+  if (c->plan.dual && !with_events && mask == B2_PHASE_ALL) return enqueue_dual(c);
+  if (!with_events) return run_steps(c->plan.steps, mask, c->stream);
   B2_CUDA(cudaEventRecord(c->ev[0], c->stream));
   int last = -1;
-  for (const Step& s : c->steps) {
+  for (const Step& s : c->plan.steps) {
     if (!(mask & (1 << s.phase))) continue;
     if (last >= 0 && s.phase != last) B2_CUDA(cudaEventRecord(c->ev[last + 1], c->stream));
     if (s.run(c->stream)) return -1;
     last = s.phase;
   }
   if (last >= 0) B2_CUDA(cudaEventRecord(c->ev[last + 1], c->stream));
-  return 0;
-}
-
-// ---- weight loading -------------------------------------------------------------------------
-// geo_emb (dense 4 -> 64, nn.py:125-127) and geo_conv (1x1 conv 64 -> 16, nn.py:133-135) of a relation module
-int load_rel(b2_ctx* c, RelOp* R, const WeightSet& ws) {
-  const float* ew = ws.get(R->name + "/geo_emb/W", 4 * kRelGeoDim);
-  const float* eb = ws.get(R->name + "/geo_emb/b", kRelGeoDim);
-  const float* cw = ws.get(R->name + "/geo_conv/W", kRelGeoDim * kRelGroups);
-  const float* cb = ws.get(R->name + "/geo_conv/b", kRelGroups);
-  if (!ew || !eb || !cw || !cb) return -1;
-  return relation_upload_geo(ew, eb, cw, cb, R->geo, c->stream);
-}
-
-int load_layer(b2_ctx* c, const ConvLayer* L, const WeightSet& ws) {
-  if (L->layout == kRuntime) return 0;   // written by the pass itself
-  const int Cin = L->d.Cin, R = L->d.R, S = L->d.S, Cout = L->d.Cout, K = L->w.K, Cp = L->w.Cout_pad;
-  std::vector<float> packed(static_cast<size_t>(Cp) * K, 0.f);
-  std::vector<double> scale, shift;
-  // BatchNorm inference (nn.py:1771-1774, eps 1e-5)
-  if (fold_bn(ws, L->bn, kTensorpackBn, 1e-5, Cout, scale, shift)) return -1;
-  std::vector<float> b(Cout, 0.f);   // the layer's bias, when it has one
-  bool has_b = !L->bias.empty();
-  if (L->layout == kHwio) {
-    const float* w = ws.get(L->name + "/W", static_cast<int64_t>(R) * S * Cin * Cout);   // HWIO
-    if (!w) return -1;
-    for (int t = 0; t < R * S; ++t)
-      for (int ci = 0; ci < Cin; ++ci) {
-        const float* src = w + (static_cast<size_t>(t) * Cin + ci) * Cout;
-        for (int o = 0; o < Cout; ++o)
-          packed[static_cast<size_t>(o) * K + static_cast<size_t>(t) * Cin + ci] = static_cast<float>(src[o] * scale[o]);
-      }
-  } else if (L->layout == kGrouped) {
-    // ResNeXt conv2 (split=32): HWIO [R][S][Cin/groups][Cout], output o reading the input channels of its group
-    const float* w = ws.get(L->name + "/W", static_cast<int64_t>(R) * S * (Cin / L->d.groups) * Cout);
-    if (!w) return -1;
-    pack_grouped(w, R * S, Cin, Cout, L->d.groups, scale.data(), K, packed);
-  } else if (L->layout == kDeconv) {
-    // tf.layers.Conv2DTranspose kernel [kh=2, kw=2, out, in] (nn.py:402-412): output row (dy*2+dx)*out + o of the 1x1 conv
-    const int co = Cout / 4;
-    const float* w = ws.get(L->name + "/W", static_cast<int64_t>(4) * co * Cin);
-    const float* bb = ws.get(L->bias, co);
-    if (!w || !bb) return -1;
-    for (int t = 0; t < 4; ++t)
-      for (int o = 0; o < co; ++o) {
-        const float* src = w + (static_cast<size_t>(t) * co + o) * Cin;
-        for (int ci = 0; ci < Cin; ++ci) packed[static_cast<size_t>(t * co + o) * K + ci] = src[ci];
-        b[t * co + o] = bb[o];
-      }
-    has_b = false;
-  } else if (L->layout == kStem) {
-    // stem: reference HWIO [7,7,3,64] re-indexed for the packed operand (stem.cu):
-    // W'[o][r][s*16 + ry*6 + sx*3 + c] = W[2r+ry][2s+sx][c][o]   (12 real + 4 zero channels per width tap s)
-    const float* w = ws.get(L->name + "/W", 7 * 7 * 3 * 64);
-    if (!w) return -1;
-    for (int r = 0; r < 4; ++r)
-      for (int ch = 0; ch < 64; ++ch) {
-        const int s4 = ch / 16, r12 = ch % 16, ry = r12 / 6, sx = (r12 % 6) / 3, cc = r12 % 3;
-        const int rr = 2 * r + ry, ss = 2 * s4 + sx;
-        if (r12 >= 12 || rr >= 7 || ss >= 7) continue;
-        const float* src = w + (static_cast<size_t>(rr * 7 + ss) * 3 + cc) * 64;
-        for (int o = 0; o < Cout; ++o)
-          packed[static_cast<size_t>(o) * K + static_cast<size_t>(r) * Cin + ch] = static_cast<float>(src[o] * scale[o]);
-      }
-  } else if (L->layout == kFc6) {
-    // fc6 (and the conv head's fc): reference flattens NCHW (index c*49 + y*7 + x, models.py:1056 + nn.py:738-740);
-    // our ROI features are [y][x][c], so permute the rows of W [in, out].
-    const int C = Cin / 49;
-    const float* w = ws.get(L->name + "/W", static_cast<int64_t>(Cin) * Cout);
-    if (!w) return -1;
-    for (int ch = 0; ch < C; ++ch)
-      for (int s = 0; s < 49; ++s) {
-        const float* src = w + (static_cast<size_t>(ch) * 49 + s) * Cout;
-        const size_t k = static_cast<size_t>(s) * C + ch;
-        for (int o = 0; o < Cout; ++o) packed[static_cast<size_t>(o) * K + k] = src[o];
-      }
-  } else if (L->layout == kRelQK) {
-    // relation module query_linear / key_linear (nn.py:146-156): dense D -> D each, no bias, one N = 2D layer
-    const std::string scope = L->name.substr(0, L->name.rfind('/'));
-    const float* wq = ws.get(scope + "/query_linear/W", static_cast<int64_t>(Cin) * Cin);
-    const float* wk = ws.get(scope + "/key_linear/W", static_cast<int64_t>(Cin) * Cin);
-    if (!wq || !wk) return -1;
-    relation_pack_qk(wq, wk, Cin, packed);
-  } else if (L->layout == kDense) {
-    const float* w = ws.get(L->name + "/W", static_cast<int64_t>(Cin) * Cout);
-    if (!w) return -1;
-    for (int k = 0; k < Cin; ++k)
-      for (int o = 0; o < Cout; ++o) packed[static_cast<size_t>(o) * K + k] = w[static_cast<size_t>(k) * Cout + o];
-  } else {
-    // two reference layers fused along N: rpn/{class,box} or fastrcnn/outputs/{class,box}
-    const std::string base = L->layout == kRpnOut ? "rpn" : "fastrcnn/outputs";
-    const int n0 = L->layout == kRpnOut ? 3 : c->cfg.num_class;
-    const int n1 = Cout - n0;
-    const float* w0 = ws.get(base + "/class/W", static_cast<int64_t>(Cin) * n0);
-    const float* b0 = ws.get(base + "/class/b", n0);
-    const float* w1 = ws.get(base + "/box/W", static_cast<int64_t>(Cin) * n1);
-    const float* b1 = ws.get(base + "/box/b", n1);
-    if (!w0 || !b0 || !w1 || !b1) return -1;
-    for (int k = 0; k < Cin; ++k) {
-      for (int o = 0; o < n0; ++o) packed[static_cast<size_t>(o) * K + k] = w0[static_cast<size_t>(k) * n0 + o];
-      for (int o = 0; o < n1; ++o) packed[static_cast<size_t>(n0 + o) * K + k] = w1[static_cast<size_t>(k) * n1 + o];
-    }
-    for (int o = 0; o < n0; ++o) b[o] = b0[o];
-    for (int o = 0; o < n1; ++o) b[n0 + o] = b1[o];
-    has_b = false;
-  }
-  if (has_b) {
-    const float* bb = ws.get(L->bias, Cout);
-    if (!bb) return -1;
-    b.assign(bb, bb + Cout);
-  }
-  return upload_conv(*L, packed, fold_bias(scale, shift, L->bias.empty() ? nullptr : b.data(), Cout, Cp), c->stream);
-}
-
-// group_norm's "<scope>/gamma" and "<scope>/beta" (nn.py:97-102), [C] each
-int load_gn(b2_ctx* c, GnOp* G, const WeightSet& ws) {
-  const int C = G->p.C;
-  const float* g = ws.get(G->name + "/gamma", C);
-  const float* b = ws.get(G->name + "/beta", C);
-  if (!g || !b) return -1;
-  for (int i = 0; i < C; ++i)
-    B2_CHECK(std::isfinite(g[i]) && std::isfinite(b[i]), "GroupNorm " + G->name + ": gamma / beta not finite");
-  B2_CUDA(cudaMemcpyAsync(const_cast<float*>(G->p.gamma), g, C * sizeof(float), cudaMemcpyHostToDevice, c->stream));
-  B2_CUDA(cudaMemcpyAsync(const_cast<float*>(G->p.beta), b, C * sizeof(float), cudaMemcpyHostToDevice, c->stream));
-  B2_CUDA(cudaStreamSynchronize(c->stream));
-  return 0;
-}
-
-// dense "<block>/fc1" and "<block>/fc2" (nn.py:509-514, dense nn.py:730-774): W [in, out] row-contiguous, b [out]
-int load_se(b2_ctx* c, SeOp* S, const WeightSet& ws) {
-  const int C = S->C, nr = S->nr;
-  const struct { const char* suffix; int64_t n; float* dst; } parts[] = {
-      {"/fc1/W", static_cast<int64_t>(C) * nr, S->w1}, {"/fc1/b", nr, S->b1},
-      {"/fc2/W", static_cast<int64_t>(nr) * C, S->w2}, {"/fc2/b", C, S->b2}};
-  for (const auto& e : parts) {
-    const float* h = ws.get(S->name + e.suffix, e.n);
-    if (!h) return -1;
-    for (int64_t i = 0; i < e.n; ++i)
-      B2_CHECK(std::isfinite(h[i]), "squeeze-excite " + S->name + e.suffix + ": not finite");
-    B2_CUDA(cudaMemcpyAsync(e.dst, h, e.n * sizeof(float), cudaMemcpyHostToDevice, c->stream));
-  }
-  B2_CUDA(cudaStreamSynchronize(c->stream));
   return 0;
 }
 
@@ -1211,7 +614,7 @@ int b2_create_ex(b2_ctx** out, int device, const b2_config* cfg, const b2_config
   memset(&c->ext, 0, sizeof(c->ext));
   if (ext) c->ext = *ext;
   c->device = device;
-  c->split = cfg->precision == 1;
+  c->plan.split = cfg->precision == 1;
   if (open_device(device, "b2_create", &c->num_sms, &c->stream)) return -1;
   for (int i = 0; i <= NPHASE; ++i) B2_CUDA(cudaEventCreate(&c->ev[i]));
   memset(c->phase_ms, 0, sizeof(c->phase_ms));
@@ -1219,9 +622,9 @@ int b2_create_ex(b2_ctx** out, int device, const b2_config* cfg, const b2_config
     b2_destroy(c.release());
     return -1;
   }
-  if (c->dual) {
+  if (c->plan.dual) {
     B2_CUDA(cudaEventCreateWithFlags(&c->fork_ev, cudaEventDisableTiming));
-    for (int h = 1; h < c->nsplit; ++h) {
+    for (int h = 1; h < c->plan.nsplit; ++h) {
       B2_CUDA(cudaStreamCreateWithFlags(&c->side_stream[h - 1], cudaStreamNonBlocking));
       B2_CUDA(cudaEventCreateWithFlags(&c->join_ev[h - 1], cudaEventDisableTiming));
     }
@@ -1261,15 +664,7 @@ int b2_load_weights(b2_ctx* c, const char* const* names, const float* const* dat
   B2_CHECK(c && names && data && numel, "b2_load_weights: null argument");
   B2_CUDA(cudaSetDevice(c->device));
   const WeightSet ws(names, data, numel, n);
-  // shared RPN weights: packed once, every level's layer gets its own copy of the (small) operand
-  for (auto& L : c->layers)
-    if (load_layer(c, L.get(), ws)) return -1;
-  for (auto& G : c->gns)
-    if (load_gn(c, G.get(), ws)) return -1;
-  for (auto& S : c->ses)
-    if (load_se(c, S.get(), ws)) return -1;
-  for (auto& R : c->rels)
-    if (load_rel(c, R.get(), ws)) return -1;
+  if (load_weights(c->plan, ws, c->cfg.num_class, c->stream)) return -1;
   c->weights_loaded = true;
   return 0;
 }
@@ -1278,7 +673,7 @@ static int range_failed(b2_ctx* c, int idx);
 
 // Waits for the stream and fails when the pass left the fp16-plane range (synchronous calls).
 static int sync_range(b2_ctx* c) {
-  B2_CUDA(cudaMemcpyAsync(&c->h_range[2], c->range_flag, sizeof(unsigned int), cudaMemcpyDeviceToHost, c->stream));
+  B2_CUDA(cudaMemcpyAsync(&c->h_range[2], c->plan.range_flag, sizeof(unsigned int), cudaMemcpyDeviceToHost, c->stream));
   B2_CUDA(cudaStreamSynchronize(c->stream));
   return range_failed(c, 2);
 }
@@ -1293,7 +688,7 @@ int b2_run_phases(b2_ctx* c, int mask) {
     c->phase_ms[ph] = 0.f;
     if (!(mask & (1 << ph))) continue;
     bool any = false;
-    for (const auto& s : c->steps) any = any || s.phase == ph;
+    for (const auto& s : c->plan.steps) any = any || s.phase == ph;
     if (!any) continue;
     cudaEventElapsedTime(&c->phase_ms[ph], c->ev[last < 0 ? 0 : last + 1], c->ev[ph + 1]);
     last = ph;
@@ -1307,23 +702,23 @@ int b2_phase_times(b2_ctx* c, float ms[8]) {
   return 0;
 }
 
-int b2_kernel_launches(b2_ctx* c) { return c ? total_launches(c->steps) : -1; }
+int b2_kernel_launches(b2_ctx* c) { return c ? total_launches(c->plan.steps) : -1; }
 
 // Per-step device timing (CUDA events around every launch group, eager mode), averaged over `reps`.
 int b2_profile_steps(b2_ctx* c, int reps, float* ms_out, int cap, int* n_out) {
   B2_CHECK(c && ms_out && n_out, "b2_profile_steps: null argument");
   B2_CUDA(cudaSetDevice(c->device));
   B2_CHECK(c->weights_loaded, "b2_profile_steps: weights not loaded");
-  return profile_steps(c->steps, c->stream, reps, ms_out, cap, n_out);
+  return profile_steps(c->plan.steps, c->stream, reps, ms_out, cap, n_out);
 }
 
 // Describes step `idx`: name, kind (0 = tensor-core conv/dense), algorithmic FLOPs and HBM bytes
 // (each operand read once, output written once, at the stored precision).
 int b2_step_info(b2_ctx* c, int idx, char* name, int name_cap, double* flops, double* bytes, int* kind) {
   B2_CHECK(c, "b2_step_info: null argument");
-  return step_info(c->steps, idx, name, name_cap, flops, bytes, kind);
+  return step_info(c->plan.steps, idx, name, name_cap, flops, bytes, kind);
 }
-int b2_num_steps(b2_ctx* c) { return c ? static_cast<int>(c->steps.size()) : -1; }
+int b2_num_steps(b2_ctx* c) { return c ? static_cast<int>(c->plan.steps.size()) : -1; }
 
 static int ensure_graph(b2_ctx* c) {
   if (c->graph || !c->cfg.use_cuda_graph) return 0;
@@ -1344,7 +739,7 @@ static int run_all(b2_ctx* c) {
 static int range_failed(b2_ctx* c, int idx) {
   if (c->h_range[idx] == 0) return 0;
   c->h_range[idx] = 0;
-  cudaMemsetAsync(c->range_flag, 0, sizeof(unsigned int), c->stream);
+  cudaMemsetAsync(c->plan.range_flag, 0, sizeof(unsigned int), c->stream);
   set_error("activation outside the fp16-plane range (|x| > 65504 or NaN) in a convolution output: the weights / input are "
             "not conditioned for the (hi, lo) fp16 representation (DESIGN.md section 3)");
   return -1;
@@ -1365,7 +760,7 @@ static int copy_outputs(b2_ctx* c, float* boxes, float* probs, int32_t* labels, 
     } else if (feat_mode >= 2) {
       const int rows = B * R, n = feat_mode == 2 ? rows * C : rows * 49;
       if (!c->box_feat_agg) {
-        c->box_feat_agg = c->arena.alloc<float>(static_cast<size_t>(rows) * (C > 49 ? C : 49), /*zero=*/false);   // fully overwritten
+        c->box_feat_agg = c->plan.arena.alloc<float>(static_cast<size_t>(rows) * (C > 49 ? C : 49), /*zero=*/false);   // fully overwritten
         B2_CHECK(c->box_feat_agg != nullptr, "out of device memory (feature aggregation scratch)");
       }
       agg_feat_kernel<<<(n + 255) / 256, 256, 0, st>>>(c->box_feat, rows, C, feat_mode, c->box_feat_agg);
@@ -1451,8 +846,8 @@ static int submit_impl(b2_ctx* c, const void* frames_host, int src_h, int src_w,
     B2_CUDA(cudaStreamCreateWithFlags(&c->copy_stream, cudaStreamNonBlocking));
     B2_CUDA(cudaStreamCreateWithFlags(&c->down_stream, cudaStreamNonBlocking));
     for (int i = 0; i < 2; ++i) {
-      c->stage_in[i] = c->arena.alloc<uint8_t>(c->img_bytes, false);
-      c->stage_out[i] = c->arena.alloc<uint8_t>(nb_boxes + nb_probs + nb_labels + nb_valid + nb_feat, false);
+      c->stage_in[i] = c->plan.arena.alloc<uint8_t>(c->img_bytes, false);
+      c->stage_out[i] = c->plan.arena.alloc<uint8_t>(nb_boxes + nb_probs + nb_labels + nb_valid + nb_feat, false);
       B2_CHECK(c->stage_in[i] && c->stage_out[i], "out of device memory (submit staging buffers)");
       B2_CUDA(cudaEventCreateWithFlags(&c->h2d_done[i], cudaEventDisableTiming));
       B2_CUDA(cudaEventCreateWithFlags(&c->staged_free[i], cudaEventDisableTiming));
@@ -1488,7 +883,7 @@ static int submit_impl(b2_ctx* c, const void* frames_host, int src_h, int src_w,
   if (copy_outputs(c, boxes ? reinterpret_cast<float*>(d_boxes) : nullptr, probs ? reinterpret_cast<float*>(d_probs) : nullptr,
                    labels ? reinterpret_cast<int32_t*>(d_labels) : nullptr, valid ? reinterpret_cast<int32_t*>(d_valid) : nullptr,
                    box_feat ? reinterpret_cast<float*>(d_feat) : nullptr, feat_mode, cudaMemcpyDeviceToDevice)) return -1;
-  B2_CUDA(cudaMemcpyAsync(&c->h_range[slot], c->range_flag, sizeof(unsigned int), cudaMemcpyDeviceToHost, c->stream));
+  B2_CUDA(cudaMemcpyAsync(&c->h_range[slot], c->plan.range_flag, sizeof(unsigned int), cudaMemcpyDeviceToHost, c->stream));
   B2_CUDA(cudaEventRecord(c->pass_done[slot], c->stream));
   cudaStream_t ds = c->down_stream;
   B2_CUDA(cudaStreamWaitEvent(ds, c->pass_done[slot], 0));
@@ -1538,10 +933,10 @@ int b2_box_features(b2_ctx* c, const void* frame_host, const float* boxes_host, 
   B2_CHECK(c->weights_loaded, "b2_box_features: weights not loaded");
   const int R = c->cfg.result_per_im, C = c->cfg.fpn_num_channel;
   if (!c->given_boxes) {
-    c->given_boxes = c->arena.alloc<float>(static_cast<size_t>(R) * 4);
-    c->given_count = c->arena.alloc<int>(1);
-    c->given_feat = c->arena.alloc<float>(static_cast<size_t>(R) * C * 49);
-    c->given_pooled = c->arena.alloc<float>(static_cast<size_t>(R) * C);
+    c->given_boxes = c->plan.arena.alloc<float>(static_cast<size_t>(R) * 4);
+    c->given_count = c->plan.arena.alloc<int>(1);
+    c->given_feat = c->plan.arena.alloc<float>(static_cast<size_t>(R) * C * 49);
+    c->given_pooled = c->plan.arena.alloc<float>(static_cast<size_t>(R) * C);
     B2_CHECK(c->given_boxes && c->given_count && c->given_feat && c->given_pooled, "out of device memory (given-box buffers)");
     B2_CUDA(cudaDeviceSynchronize());   // the zero fills of alloc() run on the legacy stream
   }
@@ -1582,7 +977,7 @@ int b2_get_masks(b2_ctx* c, float* masks_host, int64_t capacity_bytes) {
 
 int b2_stage_shape(b2_ctx* c, const char* name, int64_t shape[4], int32_t* dtype) {
   B2_CHECK(c && name && shape, "b2_stage_shape: null argument");
-  const Stage* s = c->stages.find(name);
+  const Stage* s = c->plan.stages.find(name);
   if (!s) return -1;
   for (int i = 0; i < 4; ++i) shape[i] = s->shape[i];
   if (dtype) *dtype = s->kind == Stage::kI32 ? 1 : 0;
@@ -1592,7 +987,7 @@ int b2_stage_shape(b2_ctx* c, const char* name, int64_t shape[4], int32_t* dtype
 int b2_get_stage(b2_ctx* c, const char* name, void* dst, int64_t capacity) {
   B2_CHECK(c && name && dst, "b2_get_stage: null argument");
   B2_CUDA(cudaSetDevice(c->device));
-  const Stage* s = c->stages.find(name);
+  const Stage* s = c->plan.stages.find(name);
   if (!s) return -1;
   B2_CHECK(capacity >= s->numel() * 4, "b2_get_stage: buffer too small");
   return stage_read(*s, c->stream, dst);
@@ -1607,7 +1002,7 @@ int b2_set_stage(b2_ctx* c, const char* name, const void* src, int64_t bytes) {
     B2_CUDA(cudaStreamSynchronize(c->stream));
     return 0;
   }
-  const Stage* s = c->stages.find(name);
+  const Stage* s = c->plan.stages.find(name);
   if (!s) return -1;
   B2_CHECK(bytes == s->numel() * 4, "b2_set_stage: size mismatch");
   return stage_write(*s, c->stream, src);

@@ -87,7 +87,9 @@ int plan_convs(const std::vector<std::unique_ptr<ConvLayer>>& layers, bool split
 // A checkpoint as the caller passed it: name -> (data, element count).
 struct WeightSet {
   std::map<std::string, std::pair<const float*, int64_t>> m;
+  WeightSet() = default;
   WeightSet(const char* const* names, const float* const* data, const int64_t* numel, int n);
+  void add(const std::string& n, const float* data, int64_t numel) { m[n] = std::make_pair(data, numel); }
   const float* get(const std::string& n, int64_t expect) const;   // nullptr + error when missing or of another size
   bool has(const std::string& n) const { return m.count(n) != 0; }
 };

@@ -1,13 +1,13 @@
 // Single-kernel entry points for parity tests and host tools: one conv, one grouped conv, one GroupNorm, one squeeze-excite,
 // one relation module, the deformable sampler and conv, the frame resize.  Each call owns its device buffers in an Arena, so every return path frees them.
+// The squeeze-excite, relation and deformable-conv calls build a one-block plan with the detector's builders (detplan.h).
 #include <string.h>
 
 #include <algorithm>
 #include <vector>
 
 #include "../../include/b200det.h"
-#include "engine_core.h"
-#include "kernels.h"
+#include "detplan.h"
 
 using namespace b2;
 
@@ -68,6 +68,25 @@ int run_conv(int device, ConvDesc d, const float* x, const std::vector<float>& p
   if (download_planes(oh, split ? ol : nullptr, no, ho.data(), st)) return -1;
   for (size_t p = 0; p < static_cast<size_t>(d.B) * Ho * Wo; ++p)
     for (int o = 0; o < Cout; ++o) out[p * Cout + o] = ho[p * Cp + o];
+  return 0;
+}
+
+// A one-block plan over B images in the caller's precision and conv implementation, its outputs not range-monitored.
+void op_plan(DetPlan& p, int B, int split, int impl) {
+  p.batch = B;
+  p.split = split != 0;
+  p.conv_impl = impl;
+}
+
+// Plans the convs of `p`, loads its weights from `ws`, runs its steps on the legacy stream and waits for them.
+int run_plan(DetPlan& p, int device, const WeightSet& ws) {
+  cudaDeviceProp prop;
+  B2_CUDA(cudaGetDeviceProperties(&prop, device));
+  if (plan_layers(p, prop.multiProcessorCount) || load_weights(p, ws, 0, nullptr)) return -1;
+  const int rc = run_steps(p.steps, ~0u, nullptr);
+  const cudaError_t e = cudaDeviceSynchronize();   // the kernels are done before their plans go away
+  if (rc) return -1;
+  B2_CUDA(e);
   return 0;
 }
 
@@ -286,49 +305,28 @@ int b2_op_group_norm(int device, const float* x, const float* res, const float* 
 int b2_op_squeeze_excite(int device, const float* x, const float* res, const float* w1, const float* b1, const float* w2,
                          const float* b2, int B, int H, int W, int C, int nr, int split, float* out, float* gate_out) {
   B2_CHECK(x && w1 && b1 && w2 && b2 && out, "b2_op_squeeze_excite: null argument");
-  B2_CHECK(B >= 1 && H >= 1 && W >= 1 && nr >= 1 && nr <= se_max_nr() && C >= 64 && C <= 2048 && (C & (C - 1)) == 0,
-           "b2_op_squeeze_excite: C must be a power of two from 64 to 2048 and nr at most se_max_nr()");
+  B2_CHECK(B >= 1 && H >= 1 && W >= 1 && C >= 64 && C <= 2048 && (C & (C - 1)) == 0 && nr == C / 16,
+           "b2_op_squeeze_excite: C must be a power of two from 64 to 2048 and nr = C / 16 (the SE-ResNet bottleneck's)");
   B2_CUDA(cudaSetDevice(device));
-  const size_t n = static_cast<size_t>(B) * H * W * C;
-  Arena a;
-  const Planes xp = a.planes(B, H, W, C, split != 0);
-  const Planes rp = res ? a.planes(B, H, W, C, split != 0) : Planes();
-  float* partial = a.alloc<float>(static_cast<size_t>(B) * se_chunks(H * W) * C);
-  float* r_part = a.alloc<float>(static_cast<size_t>(B) * se_fc1_parts() * se_max_nr());
-  float* gate = a.alloc<float>(static_cast<size_t>(B) * C);
-  float* dw1 = a.alloc<float>(static_cast<size_t>(C) * nr);
-  float* db1 = a.alloc<float>(nr);
-  float* dw2 = a.alloc<float>(static_cast<size_t>(nr) * C);
-  float* db2 = a.alloc<float>(C);
-  B2_CHECK(xp.hi && (!res || rp.hi) && partial && r_part && gate && dw1 && db1 && dw2 && db2,
+  DetPlan p;
+  op_plan(p, B, split, 0);
+  Planes xp, rp;
+  B2_CHECK(p.alloc_planes(xp, B, H, W, C) && (!res || p.alloc_planes(rp, B, H, W, C)),
            "b2_op_squeeze_excite: out of device memory");
-  if (upload_planes(x, xp.hi, xp.lo, n, nullptr)) return -1;
-  if (res && upload_planes(res, rp.hi, rp.lo, n, nullptr)) return -1;
-  B2_CUDA(cudaMemcpy(dw1, w1, static_cast<size_t>(C) * nr * 4, cudaMemcpyHostToDevice));
-  B2_CUDA(cudaMemcpy(db1, b1, nr * 4, cudaMemcpyHostToDevice));
-  B2_CUDA(cudaMemcpy(dw2, w2, static_cast<size_t>(nr) * C * 4, cudaMemcpyHostToDevice));
-  B2_CUDA(cudaMemcpy(db2, b2, C * 4, cudaMemcpyHostToDevice));
-  GnParams p;
-  memset(&p, 0, sizeof(p));
-  p.x_hi = xp.hi; p.x_lo = xp.lo; p.y_hi = xp.hi; p.y_lo = xp.lo;
-  p.B = B; p.H = H; p.W = W; p.C = C;
-  p.pitch_H = H; p.pitch_W = W; p.ld = C;
-  if (res) { p.r_hi = rp.hi; p.r_lo = rp.lo; p.res_H = H; p.res_W = W; p.res_ld = C; }
-  p.relu = 1;
-  p.gate = gate;
-  p.chunks = gn_chunks(H, W, C);
-  if (se_squeeze_launch(xp.hi, xp.lo, B, H * W, C, partial, nullptr) ||
-      se_excite_launch(partial, B, H * W, C, C, nr, r_part, dw1, db1, dw2, db2, 1, gate, nullptr, 0, nullptr, nullptr,
-                       nullptr) ||
-      se_apply_launch(p, nullptr))
-    return -1;
-  B2_CUDA(cudaDeviceSynchronize());
-  if (gate_out) B2_CUDA(cudaMemcpy(gate_out, gate, static_cast<size_t>(B) * C * 4, cudaMemcpyDeviceToHost));
-  return download_planes(xp.hi, xp.lo, n, out, nullptr);
+  if (upload_planes(x, xp.hi, xp.lo, xp.elems(), nullptr)) return -1;
+  if (res && upload_planes(res, rp.hi, rp.lo, rp.elems(), nullptr)) return -1;
+  if (add_se(p, 0, "block", xp, res ? &rp : nullptr)) return -1;
+  WeightSet ws;
+  ws.add("block/fc1/W", w1, static_cast<int64_t>(C) * nr);
+  ws.add("block/fc1/b", b1, nr);
+  ws.add("block/fc2/W", w2, static_cast<int64_t>(nr) * C);
+  ws.add("block/fc2/b", b2, C);
+  if (run_plan(p, device, ws)) return -1;
+  if (gate_out) B2_CUDA(cudaMemcpy(gate_out, p.ses[0]->gate, static_cast<size_t>(B) * C * 4, cudaMemcpyDeviceToHost));
+  return download_planes(xp.hi, xp.lo, xp.elems(), out, nullptr);
 }
 
-// One relation module with the engine's steps and operands (engine.cu add_relation): query|key layer, V^T + attention,
-// one P.V layer per image, output_linear + h.
+// One relation module through the box head's builder (add_relation).
 int b2_op_relation(int device, const float* h, const float* boxes, const int32_t* count, const float* geo_emb_w,
                    const float* geo_emb_b, const float* geo_conv_w, const float* geo_conv_b, const float* query_w,
                    const float* key_w, const float* output_w, int B, int K, int D, int split, float* out) {
@@ -338,73 +336,26 @@ int b2_op_relation(int device, const float* h, const float* boxes, const int32_t
            "b2_op_relation: needs B >= 1, 1 <= K <= 1024 and D a multiple of 64");
   for (int b = 0; b < B; ++b) B2_CHECK(count[b] >= 0 && count[b] <= K, "b2_op_relation: count outside [0, K]");
   B2_CUDA(cudaSetDevice(device));
-  cudaDeviceProp prop;
-  B2_CUDA(cudaGetDeviceProperties(&prop, device));
-  const bool sp = split != 0;
-  const int G = kRelGroups, M = B * K, Mpad = (M + 127) / 128 * 128, Kp = (K + 63) / 64 * 64;
-  Arena a;
-  const Planes hp = a.planes(1, 1, Mpad, D, sp), op = a.planes(1, 1, Mpad, D, sp);
-  const Planes pp = a.planes(B, 1, G * K, Kp, sp), vp = a.planes(1, 1, Mpad, G * D, sp);
-  float* qk = a.alloc<float>(static_cast<size_t>(Mpad) * 2 * D);
-  float* dbox = a.alloc<float>(static_cast<size_t>(M) * 4);
-  int* dcount = a.alloc<int>(B);
-  float* geo = a.alloc<float>(kRelGeoWeights);
-  __half** vt = a.alloc<__half*>(2 * B);
-  B2_CHECK(hp.hi && op.hi && pp.hi && vp.hi && qk && dbox && dcount && geo && vt, "b2_op_relation: out of device memory");
+  const int M = B * K;
+  DetPlan p;
+  op_plan(p, B, split, 0);
+  Planes hp, op;
+  float* dbox = p.arena.alloc<float>(static_cast<size_t>(M) * 4);
+  int* dcount = p.arena.alloc<int>(B);
+  B2_CHECK(p.alloc_rows(hp, M, D) && p.alloc_rows(op, M, D) && dbox && dcount, "b2_op_relation: out of device memory");
   if (upload_planes(h, hp.hi, hp.lo, static_cast<size_t>(M) * D, nullptr)) return -1;
   B2_CUDA(cudaMemcpy(dbox, boxes, static_cast<size_t>(M) * 4 * sizeof(float), cudaMemcpyHostToDevice));
   B2_CUDA(cudaMemcpy(dcount, count, B * sizeof(int), cudaMemcpyHostToDevice));
-  if (relation_upload_geo(geo_emb_w, geo_emb_b, geo_conv_w, geo_conv_b, geo, nullptr)) return -1;
-
-  std::vector<std::unique_ptr<ConvLayer>> layers;
-  auto dense = [&](const char* name, const Planes& in, int rows, int Cout, const Planes& o, const Planes* res, float* f32,
-                   int ldc) {
-    ConvDesc d;
-    d.in_H = 1; d.in_W = rows; d.Cout = Cout;
-    layers.push_back(make_conv(a, sp, name, d, in, o, res, f32, ldc));
-    return layers.back().get();
-  };
-  Planes hv = hp, ov = op, vv = vp;
-  hv.W = M; ov.W = M; vv.W = M;
-  ConvLayer* Lqk = dense("query_key", hv, M, 2 * D, Planes(), nullptr, qk, 2 * D);
-  std::vector<__half*> tab(2 * B, nullptr);
-  for (int b = 0; b < B; ++b) {
-    Planes o = vp;
-    const size_t off = static_cast<size_t>(b) * G * K * D;
-    o.W = G * K; o.C = D;
-    o.hi += off;
-    if (o.lo) o.lo += off;
-    ConvLayer* L = dense("attention_value", pp.images(b, 1), G * K, D, o, nullptr, nullptr, 0);
-    tab[b] = L->w.w_hi;
-    tab[B + b] = L->w.w_lo;
-  }
-  ConvLayer* Lout = dense("output_linear", vv, M, D, ov, &hv, nullptr, 0);
-  B2_CUDA(cudaMemcpy(vt, tab.data(), tab.size() * sizeof(__half*), cudaMemcpyHostToDevice));
-  std::vector<float> packed;
-  relation_pack_qk(query_w, key_w, D, packed);
-  if (upload_conv(*Lqk, packed, std::vector<float>(2 * D, 0.f), nullptr)) return -1;
-  packed.assign(static_cast<size_t>(D) * G * D, 0.f);
-  for (size_t k = 0; k < static_cast<size_t>(G) * D; ++k)
-    for (int o = 0; o < D; ++o) packed[static_cast<size_t>(o) * G * D + k] = output_w[k * D + o];
-  if (upload_conv(*Lout, packed, std::vector<float>(D, 0.f), nullptr)) return -1;
-  if (plan_convs(layers, sp, prop.multiProcessorCount)) return -1;
-
-  RelationParams p;
-  memset(&p, 0, sizeof(p));
-  p.boxes = dbox; p.count = dcount;
-  p.qk = qk; p.ldqk = 2 * D; p.D = D; p.K = K; p.Kp = Kp;
-  p.rows = relation_rows_per_block(Kp, D);
-  p.geo = geo;
-  p.h_hi = hp.hi; p.h_lo = hp.lo;
-  p.p_hi = pp.hi; p.p_lo = pp.lo;
-  p.vt_hi = vt; p.vt_lo = sp ? vt + B : nullptr;
-  int rc = conv_tc_launch(Lqk->plan.get(), nullptr);
-  if (!rc) rc = relation_attend_launch(p, 0, B, nullptr);
-  for (size_t i = 1; i + 1 < layers.size() && !rc; ++i) rc = conv_tc_launch(layers[i]->plan.get(), nullptr);
-  if (!rc) rc = conv_tc_launch(Lout->plan.get(), nullptr);
-  const cudaError_t e = cudaDeviceSynchronize();   // the kernels are done before their plans go away
-  if (rc) return -1;
-  B2_CUDA(e);
+  if (add_relation(p, "rm", B, K, D, dbox, dcount, hp, op)) return -1;
+  WeightSet ws;
+  ws.add("rm/geo_emb/W", geo_emb_w, 4 * kRelGeoDim);
+  ws.add("rm/geo_emb/b", geo_emb_b, kRelGeoDim);
+  ws.add("rm/geo_conv/W", geo_conv_w, kRelGeoDim * kRelGroups);
+  ws.add("rm/geo_conv/b", geo_conv_b, kRelGroups);
+  ws.add("rm/query_linear/W", query_w, static_cast<int64_t>(D) * D);
+  ws.add("rm/key_linear/W", key_w, static_cast<int64_t>(D) * D);
+  ws.add("rm/output_linear/W", output_w, static_cast<int64_t>(kRelGroups) * D * D);
+  if (run_plan(p, device, ws)) return -1;
   return download_planes(op.hi, op.lo, static_cast<size_t>(M) * D, out, nullptr);
 }
 
@@ -432,66 +383,32 @@ int b2_op_deform_sample(int device, const float* x, const float* offsets, int B,
   return download_planes(op.hi, op.lo, op.elems(), out, nullptr);
 }
 
-// The deformable conv2 with the engine's steps and operands (engine.cu add_deform): offset conv, sampler, 1x1 conv over
-// the operand.
+// The deformable conv2 through the bottleneck's builder (add_deform).
 int b2_op_deform_conv2d(int device, const float* x, const float* offset_w, const float* offset_b, const float* w, int B,
                         int H, int W, int C, int Cout, int impl, int split, float* out, float* offsets_out) {
   B2_CHECK(x && offset_w && offset_b && w && out, "b2_op_deform_conv2d: null argument");
-  B2_CHECK(B >= 1 && H >= 2 && W >= 2 && C >= 64 && C % 64 == 0 && Cout >= 1,
+  B2_CHECK(B >= 1 && H >= 2 && W >= 2 && C >= 64 && C % 64 == 0,
            "b2_op_deform_conv2d: needs C a multiple of 64");
+  B2_CHECK(Cout == C, "b2_op_deform_conv2d: Cout must equal C (the bottleneck's deformable conv2 keeps its width)");
   B2_CUDA(cudaSetDevice(device));
-  cudaDeviceProp prop;
-  B2_CUDA(cudaGetDeviceProperties(&prop, device));
-  const bool sp = split != 0;
-  const int Ho = (H + 1) / 2, Wo = (W + 1) / 2, Cp = (Cout + 15) / 16 * 16;
-  const size_t npix = static_cast<size_t>(B) * Ho * Wo;
-  Arena a;
-  const Planes xp = a.planes(B, H, W, C, sp), smp = a.planes(B, Ho, Wo, 9 * C, sp), op = a.planes(B, Ho, Wo, Cp, sp);
-  float* off = a.alloc<float>(npix * kDeformOffsetLd);
-  B2_CHECK(xp.hi && smp.hi && op.hi && off, "b2_op_deform_conv2d: out of device memory");
+  DetPlan p;
+  op_plan(p, B, split, impl);
+  Planes xp, op;
+  B2_CHECK(p.alloc_planes(xp, B, H, W, C) && p.alloc_planes(op, B, (H + 1) / 2, (W + 1) / 2, C),
+           "b2_op_deform_conv2d: out of device memory");
   if (upload_planes(x, xp.hi, xp.lo, xp.elems(), nullptr)) return -1;
-  std::vector<std::unique_ptr<ConvLayer>> layers;
-  ConvDesc d;
-  d.R = 3; d.S = 3; d.stride = 2;
-  d.pad_t = 1; d.pad_b = 2 * Ho - H; d.pad_l = 1; d.pad_r = 2 * Wo - W;
-  d.Cout = 18;
-  layers.push_back(make_conv(a, sp, "conv2_offset", d, xp, Planes(), nullptr, off, kDeformOffsetLd));
-  ConvDesc d2;
-  d2.Cout = Cout;
-  layers.push_back(make_conv(a, sp, "conv2", d2, smp, op));
-  // HWIO -> [Cout_pad][K]: the offset conv's K = 9 * C, and conv2's [3,3,C,Cout] kernel as a 1x1 conv over 9 * C inputs
-  for (int l = 0; l < 2; ++l) {
-    const ConvLayer& L = *layers[l];
-    const int n = l == 0 ? 18 : Cout, K = L.w.K;
-    const float* src = l == 0 ? offset_w : w;
-    std::vector<float> packed(static_cast<size_t>(L.w.Cout_pad) * K, 0.f), bias(L.w.Cout_pad, 0.f);
-    for (int k = 0; k < K; ++k)
-      for (int o = 0; o < n; ++o) packed[static_cast<size_t>(o) * K + k] = src[static_cast<size_t>(k) * n + o];
-    if (l == 0) std::copy(offset_b, offset_b + 18, bias.begin());
-    if (upload_conv(L, packed, bias, nullptr)) return -1;
-  }
-  if (impl == 0 && plan_convs(layers, sp, prop.multiProcessorCount)) return -1;
-  auto conv = [&](const ConvLayer& L) {
-    return impl == 0 ? conv_tc_launch(L.plan.get(), nullptr) : conv_simt_launch(L.d, L.w, L.io, sp, nullptr);
-  };
-  DeformParams p;
-  p.in_hi = xp.hi; p.in_lo = xp.lo;
-  p.offset = off; p.ld_off = kDeformOffsetLd;
-  p.H = H; p.W = W; p.C = C; p.Ho = Ho; p.Wo = Wo;
-  p.out_hi = smp.hi; p.out_lo = smp.lo;
-  int rc = conv(*layers[0]);
-  if (!rc) rc = deform_sample_launch(p, 0, B, nullptr);
-  if (!rc) rc = conv(*layers[1]);
-  const cudaError_t e = cudaDeviceSynchronize();   // the kernels are done before their plans go away
-  if (rc) return -1;
-  B2_CUDA(e);
-  std::vector<float> o(npix * Cp);
-  if (download_planes(op.hi, op.lo, o.size(), o.data(), nullptr)) return -1;
-  for (size_t q = 0; q < npix; ++q) std::copy(&o[q * Cp], &o[q * Cp] + Cout, out + q * Cout);
-  if (offsets_out) {
-    std::vector<float> f(npix * kDeformOffsetLd);
-    B2_CUDA(cudaMemcpy(f.data(), off, f.size() * sizeof(float), cudaMemcpyDeviceToHost));
-    for (size_t q = 0; q < npix; ++q) std::copy(&f[q * kDeformOffsetLd], &f[q * kDeformOffsetLd] + 18, offsets_out + q * 18);
+  if (add_deform(p, "block", xp, op)) return -1;
+  WeightSet ws;
+  ws.add("block/conv2_offset/W", offset_w, static_cast<int64_t>(9) * C * 18);
+  ws.add("block/conv2_offset/b", offset_b, 18);
+  ws.add("block/conv2/W", w, static_cast<int64_t>(9) * C * C);
+  if (run_plan(p, device, ws)) return -1;
+  if (download_planes(op.hi, op.lo, op.elems(), out, nullptr)) return -1;
+  if (offsets_out) {   // the offset conv's 18 columns of each [kDeformOffsetLd] row
+    const Stage* s = p.stages.find("block/conv2_offset");
+    if (!s) return -1;
+    B2_CUDA(cudaMemcpy2D(offsets_out, 18 * sizeof(float), s->ptr, s->shape[3] * sizeof(float), 18 * sizeof(float),
+                         op.elems() / C, cudaMemcpyDeviceToHost));
   }
   return 0;
 }

@@ -4,9 +4,12 @@ compared byte for byte (a host-side refactor must leave all of them unchanged).
     python tools/engine_fingerprint.py --out a.npz [--root <tree>]
 
 --root selects the source tree whose package (and library, built in that tree) is exercised; default: this tree.
-Covers: the detector (BN R101 at batch 2 with multi semantics, GN with the conv box head at batch 2, add_mask), each in
-split and fp16 precision, CUDA graph and eager, B2_SPLIT=1 and 2, all four feat_modes, several stages, the step list and
-launch count; b2_box_features; OSNet and ResNet-101 ReID embeddings, activations and launch counts; EfficientDet-D0 with
+Covers: the detector (BN R101 at batch 2 with multi semantics, GN with the conv box head at batch 2, add_mask, and at
+192x256 with few blocks use_se (v6), use_resnext, add_relation_nn, use_deformable alone and with use_gn, use_basic_block
+alone and with use_gn + use_conv_frcnn_head), each in split and fp16 precision, CUDA graph and eager, B2_SPLIT=1 and 2,
+all four feat_modes, several stages, the step list and launch count; b2_box_features; op_relation, op_deform_conv2d
+(tensor and CUDA cores, with the offsets) and op_squeeze_excite (with and without a residual, with the gate) in both
+precisions; OSNet and ResNet-101 ReID embeddings, activations and launch counts; EfficientDet-D0 with
 an EfficientNet-b0 backbone (run_features, detect, stages, step list, launch count); b2_cosine_cost, b2_distance_matrix
 and b2_track_pair_cost over a growing-then-shrinking shape sequence."""
 import argparse
@@ -25,7 +28,8 @@ from object_detection_tracking_b200 import _lib  # noqa: E402
 from object_detection_tracking_b200.config import make_config  # noqa: E402
 from object_detection_tracking_b200.effdet import EffdetEngine  # noqa: E402
 from object_detection_tracking_b200.effdet_config import feat_sizes, make_effdet_config  # noqa: E402
-from object_detection_tracking_b200.engine import Detector, cosine_cost  # noqa: E402
+from object_detection_tracking_b200.engine import (Detector, cosine_cost, op_deform_conv2d, op_relation,  # noqa: E402
+                                                  op_squeeze_excite)
 from object_detection_tracking_b200.reid import ReidEngine, compute_distance_matrix  # noqa: E402
 from object_detection_tracking_b200.synth import (synth_effdet_weights, synth_efficientnet_weights, synth_frame,  # noqa: E402
                                                   synth_osnet_state, synth_resnet101_reid_state, synth_weights)
@@ -75,6 +79,55 @@ gn = make_config(resnet_num_block=(1, 1, 2, 2), max_size=W, short_edge_size=H, n
 detector("gn_head", gn, synth_weights(gn, 12), 2, True, ["fc"])
 mk = make_config(resnet_num_block=(1, 1, 2, 1), max_size=W, short_edge_size=H, add_mask=True)
 detector("mask", mk, synth_weights(mk, 13), 1, False, ["mask_logits", "final_masks"])
+# the detector variants at small geometry (as in their feature tests), batch 2 with multi semantics
+SMALL = dict(max_size=W, short_edge_size=H)
+DEFORM_BLOCKS = ["group%d/block0/conv2_%s" % (g, k) for g in (1, 2, 3) for k in ("offset", "sample")]
+for tag, kw, seed, extra in (
+        ("se_v6", dict(resnet_num_block=(1, 1, 2, 2), use_se=True, use_frcnn_class_agnostic=True, use_dilations=False,
+                       version=6), 14, ["c3", "c4"]),
+        ("resnext", dict(resnet_num_block=(1, 1, 2, 2), use_resnext=True), 15, ["c3", "c4"]),
+        ("relation", dict(resnet_num_block=(1, 1, 2, 2), add_relation_nn=True), 16, ["fc6", "fc7", "rm_r1", "rm_r2"]),
+        ("deform", dict(resnet_num_block=(1, 1, 2, 1), use_deformable=True, use_dilations=False), 17, DEFORM_BLOCKS),
+        ("deform_gn", dict(resnet_num_block=(1, 1, 2, 1), use_deformable=True, use_dilations=False, use_gn=True), 18,
+         DEFORM_BLOCKS),
+        ("basic", dict(resnet_num_block=(1, 2, 1, 1), use_basic_block=True), 19, ["c3", "c4"]),
+        ("basic_gn_head", dict(resnet_num_block=(1, 2, 1, 1), use_basic_block=True, use_gn=True, use_conv_frcnn_head=True),
+         20, ["c3", "c4", "fc"])):
+    cfg = make_config(**dict(SMALL, **kw))
+    detector(tag, cfg, synth_weights(cfg, seed), 2, True, extra)
+
+# the composite single-op entry points at fixed seeds
+orng = np.random.default_rng(21)
+for prec in ("split", "fp16"):
+    sp = prec == "split"
+    B, K, D = 2, 50, 256
+    h = np.maximum(orng.standard_normal((B, K, D)), 0).astype(np.float32)
+    xy = orng.uniform(0, 200, (B, K, 2))
+    boxes = np.concatenate([xy, xy + orng.uniform(8, 60, (B, K, 2))], -1).astype(np.float32)
+    rw = {k: (orng.standard_normal(s) * 0.1).astype(np.float32)
+          for k, s in (("geo_emb/W", (4, 64)), ("geo_emb/b", (64,)), ("geo_conv/W", (1, 1, 64, 16)), ("geo_conv/b", (16,)),
+                       ("query_linear/W", (D, D)), ("key_linear/W", (D, D)), ("output_linear/W", (16 * D, D)))}
+    out["op/relation/" + prec] = op_relation(h, boxes, np.array([K, 31], np.int32), rw, split=sp)
+    B, Hd, Wd, C = 2, 13, 19, 128
+    x = np.maximum(orng.standard_normal((B, Hd, Wd, C)), 0).astype(np.float32)
+    ow = (orng.standard_normal((3, 3, C, 18)) * 0.05).astype(np.float32)
+    ob = (orng.standard_normal(18) * 0.5).astype(np.float32)
+    w = (orng.standard_normal((3, 3, C, C)) / np.sqrt(9 * C)).astype(np.float32)
+    for impl in ("tcgen05", "simt"):
+        o, off = op_deform_conv2d(x, ow, ob, w, impl=impl, split=sp, return_offsets=True)
+        out["op/deform/%s/%s/out" % (impl, prec)] = o
+        out["op/deform/%s/%s/offsets" % (impl, prec)] = off
+    B, Hs, Ws, C = 2, 10, 12, 256
+    x = orng.standard_normal((B, Hs, Ws, C)).astype(np.float32)
+    w1 = (orng.standard_normal((C, C // 16)) * 0.2).astype(np.float32)
+    b1 = orng.uniform(0, 0.1, C // 16).astype(np.float32)
+    w2 = (orng.standard_normal((C // 16, C)) * 0.3).astype(np.float32)
+    b2 = (orng.standard_normal(C) * 0.4).astype(np.float32)
+    r = orng.standard_normal((B, Hs, Ws, C)).astype(np.float32)
+    for name, res in (("res", r), ("nores", None)):
+        o, g = op_squeeze_excite(x, w1, b1, w2, b2, res=res, split=sp)
+        out["op/se/%s/%s/out" % (name, prec)] = o
+        out["op/se/%s/%s/gate" % (name, prec)] = g
 
 # given-box features (batch-1 context, uncropped levels)
 det = Detector(bn, 1, H, W, precision="split")
