@@ -297,6 +297,15 @@ int b2_effdet_detect(b2_effdet* ctx, const uint8_t* frame_bgr, int h, int w, flo
                      int32_t* classes, int32_t* levels, float* box_feat, int32_t* count, float* image_scale_out);
 /* Stage tensors of the last pass (parity tests): "image", "stem", "block_<i>", "c3".."c5", "fpn3".."fpn7", "cls3".."cls7", "box3".."box7" as fp32 NHWC */
 int b2_effdet_get_stage(b2_effdet* ctx, const char* name, float* dst_host, int64_t capacity_bytes, int64_t shape[4]);
+/* Post-processing stages: "topk_boxes" [k][4] (ymin xmin ymax xmax, network pixels), "topk_scores" [k], "topk_classes"
+ * [k] (int32, 1-based), "topk_levels" [k] (int32), "topk_count" (int32): the candidates in top-k order (logit descending,
+ * then flat index); "final_boxes" [max][4] (x1 y1 x2 y2 * image_scale), "final_scores", "final_classes", "final_levels",
+ * "final_count" (int32) and "box_feat" [max][fpn_num_filters]: the outputs; "image_scale" (one float). */
+/* Writes a stage (bytes = its whole stored size) for b2_effdet_run_phases. */
+int b2_effdet_set_stage(b2_effdet* ctx, const char* name, const void* src_host, int64_t bytes);
+/* Run a subset of the pass eagerly: bit mask of B2_EFFDET_PHASE_*. */
+enum { B2_EFFDET_PHASE_BACKBONE = 1, B2_EFFDET_PHASE_FEATURES = 2, B2_EFFDET_PHASE_POST = 4, B2_EFFDET_PHASE_BOX_FEAT = 8 };
+int b2_effdet_run_phases(b2_effdet* ctx, int phase_mask);
 int b2_effdet_num_launches(b2_effdet* ctx);
 /* Per-step CUDA-event timing / description of the pass (same contract as b2_profile_steps / b2_step_info). */
 int b2_effdet_profile_steps(b2_effdet* ctx, int reps, float* ms_out, int cap, int* n_out);

@@ -112,6 +112,8 @@ SYMBOLS = [
     ("b2_effdet_run_features", c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_float] + [c_void_p] * 6),
     ("b2_effdet_detect", c_int, [c_void_p, c_void_p, c_int, c_int] + [c_void_p] * 7),
     ("b2_effdet_get_stage", c_int, [c_void_p, c_char_p, c_void_p, c_int64, POINTER(c_int64)]),
+    ("b2_effdet_set_stage", c_int, [c_void_p, c_char_p, c_void_p, c_int64]),
+    ("b2_effdet_run_phases", c_int, [c_void_p, c_int]),
     ("b2_effdet_num_launches", c_int, [c_void_p]),
     ("b2_effdet_profile_steps", c_int, [c_void_p, c_int, POINTER(c_float), c_int, POINTER(c_int)]),
     ("b2_effdet_step_info", c_int, [c_void_p, c_int, ctypes.c_char_p, c_int, POINTER(ctypes.c_double), POINTER(ctypes.c_double), POINTER(c_int)]),
@@ -135,6 +137,7 @@ SYMBOLS = [
 
 PHASES = dict(BACKBONE=1, FPN=2, RPN_HEAD=4, PROPOSALS=8, ROI=16, HEAD_FC=32, POST=64, BOX_FEAT=128, ALL=255)
 PHASE_NAMES = ["backbone", "fpn", "rpn_head", "proposals", "roi", "head_fc", "post", "box_feat"]
+EFFDET_PHASES = dict(BACKBONE=1, FEATURES=2, POST=4, BOX_FEAT=8)
 
 _lib = None
 

@@ -57,11 +57,24 @@ struct ESe {
   const ConvLayer* proj = nullptr;   // its w_master holds the BN-folded projection weights [Cout_pad][K] fp32
 };
 
-// Step phases: the backbone runs only in b2_effdet_detect's graph
-enum { kBackbone = 0, kFeatures = 1 };
+// Step phases (bit i of b2_effdet_run_phases' mask = phase i): the backbone runs only in b2_effdet_detect's graph; the
+// feature network + heads, the post-processing and the box feature run in both graphs
+enum { kBackbone = 0, kFeatures = 1, kPost = 2, kBoxFeat = 3 };
 
 int pad64(int c) { return (c + 63) / 64 * 64; }
 int pad16(int c) { return (c + 15) / 16 * 16; }
+
+// anchor_scale and the aspect ratios arrive as float32, but anchors.py builds the grid in float64 from the decimals the
+// configuration writes (1.4, 0.7): the shortest decimal that rounds to the float32 is that value.
+double config_double(float f) {
+  char buf[32];
+  for (int p = 1; p <= 9; ++p) {
+    snprintf(buf, sizeof(buf), "%.*g", p, static_cast<double>(f));
+    const double d = strtod(buf, nullptr);
+    if (static_cast<float>(d) == f) return d;
+  }
+  return f;
+}
 
 }  // namespace
 
@@ -427,10 +440,10 @@ int build(b2_effdet* c) {
     for (int o = 0; o < g.num_scales; ++o)
       for (int r = 0; r < g.num_aspects; ++r, ++a) {
         const double oct = pow(2.0, o / static_cast<double>(g.num_scales));
-        const double sx = static_cast<double>(g.anchor_scale) * p.stride_x[l] * oct;
-        const double sy = static_cast<double>(g.anchor_scale) * p.stride_y[l] * oct;
-        p.half_x[l][a] = sx * static_cast<double>(g.aspect_ratios[r][0]) / 2.0;
-        p.half_y[l][a] = sy * static_cast<double>(g.aspect_ratios[r][1]) / 2.0;
+        const double sx = config_double(g.anchor_scale) * p.stride_x[l] * oct;
+        const double sy = config_double(g.anchor_scale) * p.stride_y[l] * oct;
+        p.half_x[l][a] = sx * config_double(g.aspect_ratios[r][0]) / 2.0;
+        p.half_y[l][a] = sy * config_double(g.aspect_ratios[r][1]) / 2.0;
       }
   }
   p.level_off[5] = off; p.total = off;
@@ -467,11 +480,26 @@ int build(b2_effdet* c) {
   }
   r.C = c->Fp; r.Creal = c->F; r.min_level = 3; r.max_out = p.max_out;
   r.boxes = c->out_boxes; r.levels = c->out_levels; r.count = c->out_count; r.out = c->out_feat;
+  // the candidates in top-k order (boxes ymin xmin ymax xmax in network pixels, count = state[5]), the outputs, and the
+  // device copy of image_scale the NMS step multiplies the boxes by
+  const int k = p.k, m = p.max_out;
+  c->named.raw("topk_boxes", p.cand_box, Stage::kF32, 1, 1, k, 4);
+  c->named.raw("topk_scores", p.cand_score, Stage::kF32, 1, 1, k, 1);
+  c->named.raw("topk_classes", p.cand_cls, Stage::kI32, 1, 1, k, 1);
+  c->named.raw("topk_levels", p.cand_lvl, Stage::kI32, 1, 1, k, 1);
+  c->named.raw("topk_count", p.state + 5, Stage::kI32, 1, 1, 1, 1);
+  c->named.raw("final_boxes", c->out_boxes, Stage::kF32, 1, 1, m, 4);
+  c->named.raw("final_scores", c->out_scores, Stage::kF32, 1, 1, m, 1);
+  c->named.raw("final_classes", c->out_classes, Stage::kI32, 1, 1, m, 1);
+  c->named.raw("final_levels", c->out_levels, Stage::kI32, 1, 1, m, 1);
+  c->named.raw("final_count", c->out_count, Stage::kI32, 1, 1, 1, 1);
+  c->named.raw("box_feat", c->out_feat, Stage::kF32, 1, 1, m, c->F);
+  c->named.raw("image_scale", c->scale_dev, Stage::kF32, 1, 1, 1, 1);
   // 15 kernels (seed, 4 x (hist, pick), collect, tie scan, tie write, prepare, mask, scan), counted as the 14 that
   // b2_effdet_num_launches has always reported for them
-  add_step(c->steps, c->phase, 6, "post", [c](cudaStream_t st) { return effdet_post_launch(c->post, c->scale_dev, st); },
+  add_step(c->steps, kPost, 6, "post", [c](cudaStream_t st) { return effdet_post_launch(c->post, c->scale_dev, st); },
            static_cast<double>(p.total) * 4.0 * 6.0, 0.0, 14);
-  add_step(c->steps, c->phase, 7, "box_feat", [c](cudaStream_t st) { return level_roi_feat_launch(c->roi, st); }, 0.0);
+  add_step(c->steps, kBoxFeat, 7, "box_feat", [c](cudaStream_t st) { return level_roi_feat_launch(c->roi, st); }, 0.0);
   return plan_convs(c->convs, c->split, c->num_sms);
 }
 
@@ -651,6 +679,29 @@ int b2_effdet_get_stage(b2_effdet* c, const char* name, float* dst, int64_t capa
   B2_CHECK(c && name && dst && shape, "b2_effdet_get_stage: null argument");
   B2_CUDA(cudaSetDevice(c->device));
   return stage_get(c->named, name, c->stream, dst, capacity, shape, "b2_effdet_get_stage");
+}
+
+// Overwrites stage `name` with host data of its full stored shape (4 bytes per element), e.g. "cls3".."cls7" /
+// "box3".."box7" with their padding columns and "fpn3".."fpn7" with their padded channels, so that the phases after it can
+// run on chosen inputs.
+int b2_effdet_set_stage(b2_effdet* c, const char* name, const void* src, int64_t bytes) {
+  B2_CHECK(c && name && src, "b2_effdet_set_stage: null argument");
+  B2_CUDA(cudaSetDevice(c->device));
+  const Stage* s = c->named.find(name);
+  if (!s) return -1;
+  B2_CHECK(bytes == s->numel() * 4, "b2_effdet_set_stage: size mismatch");
+  return stage_write(*s, c->stream, src);
+}
+
+// Runs the steps of the phases in `mask` (B2_EFFDET_PHASE_*) eagerly on the stages as they stand, and waits for them.
+int b2_effdet_run_phases(b2_effdet* c, int mask) {
+  B2_CHECK(c, "b2_effdet_run_phases: null argument");
+  B2_CUDA(cudaSetDevice(c->device));
+  B2_CHECK(c->loaded, "b2_effdet_run_phases: weights not loaded");
+  B2_CHECK(!(mask & (1 << kBackbone)) || c->cfg.backbone >= 0, "b2_effdet_run_phases: the context has no backbone");
+  if (run_steps(c->steps, static_cast<unsigned>(mask), c->stream)) return -1;
+  B2_CUDA(cudaStreamSynchronize(c->stream));
+  return 0;
 }
 
 // Per-step CUDA-event timing of the whole pass (backbone when present, feature network, heads, post-processing, box

@@ -35,8 +35,10 @@ __device__ __forceinline__ Axis make_axis(float c0, float c1, int dim, int bin) 
   Axis a;
 #pragma unroll
   for (int t = 0; t < 2; ++t) {
-    const float in = __fadd_rn(base, __fmul_rn(static_cast<float>(2 * bin + t), scale));
-    a.ok[t] = !(in < 0.f || in > dm1);
+    // A 1-pixel axis samples its only pixel: the (dim - 1) normalisation makes every coordinate NaN there, which TF casts
+    // to an index (undefined).  A NaN coordinate on a longer axis (an infinite box side) is outside: extrapolation value.
+    const float in = dim == 1 ? 0.f : __fadd_rn(base, __fmul_rn(static_cast<float>(2 * bin + t), scale));
+    a.ok[t] = in >= 0.f && in <= dm1;
     const float inc = fminf(fmaxf(in, 0.f), dm1);
     const float fl = floorf(inc);
     a.lo[t] = static_cast<int>(fl);

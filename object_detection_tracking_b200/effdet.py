@@ -9,6 +9,11 @@ import numpy as np
 from . import _lib
 from .effdet_config import make_effdet_config  # noqa: F401  (re-export)
 
+# the post-processing's stages (include/b200det.h, b2_effdet_get_stage), and which of them hold int32
+POST_STAGES = ("topk_boxes", "topk_scores", "topk_classes", "topk_levels", "topk_count", "final_boxes", "final_scores",
+               "final_classes", "final_levels", "final_count", "box_feat", "image_scale")
+I32_STAGES = ("topk_classes", "topk_levels", "topk_count", "final_classes", "final_levels", "final_count")
+
 
 def _c_config(cfg, precision: str, backbone) -> _lib.B2EffdetConfig:
     c = _lib.B2EffdetConfig()
@@ -96,7 +101,10 @@ class EffdetEngine:
 
     def stage(self, name: str, real: int = None) -> np.ndarray:
         """'fpn3'..'fpn7' -> [H,W,F]; 'cls3'.. -> [H,W,A*num_classes]; 'box3'.. -> [H,W,A*4]; 'image' -> [H,W,3];
-        'stem' / 'block_<i>' / 'c3'..'c5' -> [h,w,C] (pass `real` to drop the operand channel padding)."""
+        'stem' / 'block_<i>' / 'c3'..'c5' -> [h,w,C] (pass `real` to drop the operand channel padding);
+        post-processing stages (POST_STAGES) -> [n,4] boxes, [n,F] box_feat, else [n] (int32 for I32_STAGES)."""
+        if name in POST_STAGES:
+            return self._post_stage(name)
         na = self.cfg.num_scales * len(self.cfg.aspect_ratios)
         if real is None:
             real = {"fpn": self.cfg.fpn_num_filters, "cls": na * self.cfg.num_classes, "box": na * 4,
@@ -113,6 +121,28 @@ class EffdetEngine:
         _, h, w, c = [int(v) for v in shape]
         out = buf[: h * w * c].reshape(h, w, c)
         return (out if real is None else out[:, :, :real]).copy()
+
+    def _post_stage(self, name: str) -> np.ndarray:
+        k, m = int(self.cfg.max_detection_topk), int(self.cfg.result_per_im)
+        buf = np.zeros(max(4 * k, m * max(4, int(self.cfg.fpn_num_filters))), np.float32)
+        shape = (ctypes.c_int64 * 4)()
+        _lib.check(self._lib.b2_effdet_get_stage(self._h, name.encode(), buf.ctypes.data, buf.nbytes, shape),
+                   "b2_effdet_get_stage")
+        n, c = int(shape[2]), int(shape[3])
+        out = buf[: n * c]
+        if name in I32_STAGES:
+            out = out.view(np.int32)
+        return (out.reshape(n, c) if c > 1 else out).copy()
+
+    def set_stage(self, name: str, value: np.ndarray) -> None:
+        """Overwrite a stage with its whole stored shape: 'cls3'.. [H,W,pad16(A*num_classes)], 'box3'.. [H,W,pad16(A*4)],
+        'fpn3'.. [H,W,pad64(F)] (float32), 'image_scale' [1], or a post-processing stage (int32 for I32_STAGES)."""
+        a = np.ascontiguousarray(value, np.int32 if name in I32_STAGES else np.float32)
+        _lib.check(self._lib.b2_effdet_set_stage(self._h, name.encode(), a.ctypes.data, a.nbytes), "b2_effdet_set_stage")
+
+    def run_phases(self, mask: int) -> None:
+        """Run the phases in `mask` (_lib.EFFDET_PHASES bits) eagerly on the current stages."""
+        _lib.check(self._lib.b2_effdet_run_phases(self._h, int(mask)), "b2_effdet_run_phases")
 
     def profile_steps(self, reps: int = 5):
         """[(name, kind, ms, flops, bytes)] per launch group of the last pass (CUDA events, eager launches)."""

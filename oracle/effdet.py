@@ -188,7 +188,13 @@ def postprocess(cls_out, box_out, cfg, fsizes, image_scale, partial_class_idxs=N
     """add_metric_fn_inputs (wrapper:367-474) + _generate_detections_tf (anchors.py:399-487).
     cls_out/box_out: {level: [H,W,A*C] / [H,W,A*4]} numpy.  Returns boxes x1y1x2y2 (scaled), scores, classes 1..90,
     level indexes -- canonical order = NMS selection order."""
-    f32 = np.float32
+    return nms_select(*topk_candidates(cls_out, box_out, cfg, fsizes, partial_class_idxs), cfg, image_scale)
+
+
+def topk_candidates(cls_out, box_out, cfg, fsizes, partial_class_idxs=None, top_k=tf_ops.top_k):
+    """add_metric_fn_inputs' global top-k over all class logits, then sigmoid and the anchor decode.  Returns the
+    candidates in top-k order (logit descending, then flat index): boxes [K,4] (ymin, xmin, ymax, xmax) in network
+    pixels, scores [K], classes [K] (1-based), levels [K].  top_k: any exact equivalent of tf_ops.top_k."""
     nc = cfg.num_classes
     na = cfg.num_scales * len(cfg.aspect_ratios)
     cls_all = np.concatenate([cls_out[l].reshape(-1, nc) for l in range(cfg.min_level, cfg.max_level + 1)], 0)
@@ -200,16 +206,24 @@ def postprocess(cls_out, box_out, cfg, fsizes, image_scale, partial_class_idxs=N
                               for l in range(cfg.min_level, cfg.max_level + 1)])
     flat = cls_all.reshape(-1)
     k = min(cfg.max_detection_topk, flat.shape[0])
-    _, ti = tf_ops.top_k(flat, k)
+    _, ti = top_k(flat, k)
     idx, cls = ti // nc, ti % nc
     logits = cls_all[idx, cls]
     anchors = anchor_boxes(cfg, fsizes)[idx]
     scores = sigmoid(logits)
-    boxes = decode_boxes(box_all[idx], anchors)
+    with np.errstate(over="ignore"):                                  # exp(th) may overflow to an infinite side
+        boxes = decode_boxes(box_all[idx], anchors)
+    return boxes, scores, (cls + 1).astype(np.int32), lvl_all[idx]
+
+
+def nms_select(boxes, scores, classes, levels, cfg, image_scale):
+    """_generate_detections_tf's class-agnostic non_max_suppression_with_scores over topk_candidates' output (visited by
+    score descending, then candidate rank).  Returns the kept boxes x1y1x2y2 * image_scale, scores, classes, levels."""
+    f32 = np.float32
     keep = tf_ops.non_max_suppression(boxes, scores, cfg.result_per_im, cfg.nms_iou_threshold,
                                       score_threshold=cfg.result_score_thres)
-    b = (boxes[keep] * f32(image_scale)).astype(f32)
-    return b[:, [1, 0, 3, 2]], scores[keep], (cls[keep] + 1).astype(np.int32), lvl_all[idx][keep]
+    b = (np.asarray(boxes, f32).reshape(-1, 4)[keep] * f32(image_scale)).astype(f32)
+    return b[:, [1, 0, 3, 2]], scores[keep], classes[keep], levels[keep]
 
 
 def box_features(fpn_feats, boxes, levels, cfg):

@@ -237,13 +237,15 @@ def roi_align(feat_chw: np.ndarray, boxes_fm: np.ndarray, out: int) -> np.ndarra
     C, H, W = feat_chw.shape
     crop = out * 2
     x0, y0, x1, y1 = [boxes_fm[:, i].astype(f32) for i in range(4)]
-    sw = ((x1 - x0) / f32(crop)).astype(f32)
-    sh = ((y1 - y0) / f32(crop)).astype(f32)
-    nx0 = ((x0 + sw / f32(2) - f32(0.5)) / f32(W - 1)).astype(f32)
-    ny0 = ((y0 + sh / f32(2) - f32(0.5)) / f32(H - 1)).astype(f32)
-    nw = (sw * f32(crop - 1) / f32(W - 1)).astype(f32)
-    nh = (sh * f32(crop - 1) / f32(H - 1)).astype(f32)
-    nb = np.stack([ny0, nx0, ny0 + nh, nx0 + nw], axis=1).astype(f32)
+    # a 1-pixel level divides by W - 1 = 0 here (NaN / inf box): tf_ops.crop_and_resize defines that axis
+    with np.errstate(divide="ignore", invalid="ignore", over="ignore"):
+        sw = ((x1 - x0) / f32(crop)).astype(f32)
+        sh = ((y1 - y0) / f32(crop)).astype(f32)
+        nx0 = ((x0 + sw / f32(2) - f32(0.5)) / f32(W - 1)).astype(f32)
+        ny0 = ((y0 + sh / f32(2) - f32(0.5)) / f32(H - 1)).astype(f32)
+        nw = (sw * f32(crop - 1) / f32(W - 1)).astype(f32)
+        nh = (sh * f32(crop - 1) / f32(H - 1)).astype(f32)
+        nb = np.stack([ny0, nx0, ny0 + nh, nx0 + nw], axis=1).astype(f32)
     r = tf_ops.crop_and_resize(np.ascontiguousarray(feat_chw.transpose(1, 2, 0)), nb, crop)
     r = r.reshape(r.shape[0], out, 2, out, 2, C)
     # tf.nn.avg_pool 2x2: sum of 4 * 0.25 (Eigen mean reducer: sum then divide)

@@ -89,13 +89,21 @@ def crop_and_resize(image_hwc: np.ndarray, boxes_norm: np.ndarray, crop: int) ->
     out = np.zeros((n, crop, crop, C), dtype=F32)
     for b in range(n):
         y1, x1, y2, x2 = [F32(v) for v in boxes_norm[b]]
-        hs = F32((y2 - y1) * F32(H - 1) / F32(crop - 1)) if crop > 1 else F32(0)
-        ws = F32((x2 - x1) * F32(W - 1) / F32(crop - 1)) if crop > 1 else F32(0)
-        ys = (F32(y1 * F32(H - 1)) + np.arange(crop, dtype=F32) * hs).astype(F32)
-        xs = (F32(x1 * F32(W - 1)) + np.arange(crop, dtype=F32) * ws).astype(F32)
+        with np.errstate(invalid="ignore", over="ignore"):
+            hs = F32((y2 - y1) * F32(H - 1) / F32(crop - 1)) if crop > 1 else F32(0)
+            ws = F32((x2 - x1) * F32(W - 1) / F32(crop - 1)) if crop > 1 else F32(0)
+            ys = (F32(y1 * F32(H - 1)) + np.arange(crop, dtype=F32) * hs).astype(F32)
+            xs = (F32(x1 * F32(W - 1)) + np.arange(crop, dtype=F32) * ws).astype(F32)
+        # A 1-pixel axis samples its only pixel.  Boxes normalised by (H - 1) = 0 give NaN coordinates there, which TF's
+        # kernel casts to an index (undefined behaviour); the GPU kernels define the case this way.  A NaN coordinate on a
+        # longer axis (an infinite box side) fails both range tests: extrapolation value, like any coordinate outside.
+        if H == 1:
+            ys = np.zeros(crop, F32)
+        if W == 1:
+            xs = np.zeros(crop, F32)
         yv = (ys >= 0) & (ys <= F32(H - 1))
         xv = (xs >= 0) & (xs <= F32(W - 1))
-        yc = np.clip(ys, 0, H - 1); xc = np.clip(xs, 0, W - 1)
+        yc = np.clip(np.where(yv, ys, F32(0)), 0, H - 1); xc = np.clip(np.where(xv, xs, F32(0)), 0, W - 1)
         t = np.floor(yc).astype(np.int64); bt = np.ceil(yc).astype(np.int64)
         l = np.floor(xc).astype(np.int64); r = np.ceil(xc).astype(np.int64)
         yl = (yc - t.astype(F32)).astype(F32)[:, None, None]
