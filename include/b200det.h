@@ -412,6 +412,52 @@ int b2_op_deform_sample(int device, const float* x, const float* offsets, int B,
 int b2_op_deform_conv2d(int device, const float* x, const float* offset_w, const float* offset_b, const float* w, int B,
                         int H, int W, int C, int Cout, int impl, int split, float* out, float* offsets_out);
 
+/* The element-wise and reduction kernels around the GEMMs, one at a time.  Activations are host fp32 converted to the
+ * engine's planes; a plane output is returned joined to fp32 in `out` and, where out_hi / out_lo are not NULL, as its raw
+ * fp16 planes (out_lo only in split precision).  Every size is checked before any device work.
+ *
+ * Depthwise conv of x [B][H][W][C] (C a multiple of 8) with w [K*K][C] (BatchNorm scale folded) and bias [C] into
+ * out [B][Ho][Wo][C].  impl 0, EfficientNet's strip kernel: B = 1, K 3 or 5, stride 1 or 2, output (y, x) reads input
+ * (y * stride - pad_t + r, x * stride - pad_l + s), zero outside the map; bias may be NULL; act 0 none, 2 swish.
+ * impl 1, OSNet's LightConv3x3 depthwise half: K = 3, stride 1, pad 1, Ho = H, Wo = W, bias given, act 1 (ReLU). */
+int b2_op_depthwise(int device, const float* x, const float* w, const float* bias, int B, int H, int W, int C, int K,
+                    int stride, int pad_t, int pad_l, int Ho, int Wo, int act, int impl, int split, float* out,
+                    uint16_t* out_hi, uint16_t* out_lo);
+/* A pool of x [B][H][W][C] (C a multiple of 8).  kind 0: the detector's and the ReID stems' 3x3 stride-2 max-pool, window
+ * rows 2y - 1 .. 2y + 1 (columns alike) clipped to the map, out [B][Ho][Wo][C] with the caller's Ho <= ceil(H / 2),
+ * Wo <= ceil(W / 2); the running maximum starts from 0, so it is the max-pool only of inputs >= 0 (every caller feeds it
+ * post-ReLU data), and it keeps the (hi, lo) pair of the element with the largest joined value.  kind 1: AvgPool2d(2),
+ * out [B][H / 2][W / 2][C].  kind 2: the global average pool, C a multiple of 64, out [B][out_ld] fp32 holding the
+ * buffer's content before the call (columns >= C keep it); out_hi / out_lo unused. */
+int b2_op_pool(int device, const float* x, int kind, int B, int H, int W, int C, int Ho, int Wo, int out_ld, int split,
+               float* out, uint16_t* out_hi, uint16_t* out_lo);
+/* One BiFPN node combine: n_in (1 to 3) inputs one after the other in x, input i [B][hw[2i]][hw[2i+1]][C], each resampled
+ * to Ho x Wo as the EfficientDet engine does (same size: read as is; 2x larger: 3x3 stride-2 max-pool with TF SAME
+ * padding; half the size: nearest 2x upsampling), then node = sum_i x_i * relu(w_i) / (sum_i relu(w_i) + 1e-4) with the
+ * raw fastattn weights (weights [n_in], or NULL for the plain sum), then x * sigmoid(x) when swish.  out [B][Ho][Wo][C];
+ * resample [n_in][3] (may be NULL) receives each input's (mode 0 / 1 / 2, pad_t, pad_l). */
+int b2_op_bifpn_combine(int device, const float* x, const int32_t* hw, const float* weights, int n_in, int B, int Ho,
+                        int Wo, int C, int swish, int split, float* out, uint16_t* out_hi, uint16_t* out_lo,
+                        int32_t* resample);
+/* MBConv's squeeze-excite: x [B][HW][Cpad] with channels [0, Creal) live, w1 [Creal][nr], b1 [nr], w2 [nr][Creal],
+ * b2 [Creal]; gate [B][Cpad] = sigmoid(swish(mean(x) @ w1 + b1) @ w2 + b2), 0 in columns >= Creal.  With w, the
+ * projection's fp32 master weight [rows][Cpad] (B = 1), the folded weight w[o][c] * gate[c] is returned as planes in
+ * w_hi / w_lo and joined in w_out (all [rows][Cpad]); with w NULL only the gate is computed. */
+int b2_op_mbconv_se(int device, const float* x, const float* w1, const float* b1, const float* w2, const float* b2,
+                    const float* w, int B, int HW, int Cpad, int Creal, int nr, int rows, int split, float* gate,
+                    float* w_out, uint16_t* w_hi, uint16_t* w_lo);
+/* OSNet's ChannelGate over an OSBlock's four streams and their gated sum: s [4][B][HW][C] (C a multiple of 64, channels
+ * [0, Creal) live), w1 [Cr][Creal], b1 [Cr], w2 [Creal][Cr], b2 [Creal]; gates [B][4][C] = sigmoid(relu(gap(s_k[b]) @ w1^T
+ * + b1) @ w2^T + b2), 0 in columns >= Creal; out [B][HW][C] = sum_k gates[b][k] * s_k[b].  gates_in [B][4][C] (may be
+ * NULL) replaces the computed gates, so that the gated sum runs alone; gates_out (may be NULL) receives the gates used. */
+int b2_op_channel_gate(int device, const float* s, const float* w1, const float* b1, const float* w2, const float* b2,
+                       const float* gates_in, int B, int HW, int C, int Creal, int Cr, int split, float* gates_out,
+                       float* out, uint16_t* out_hi, uint16_t* out_lo);
+/* EfficientNet's stem operand: img [H][W][3] fp32 -> out [Ho][Wo][64], column (r * 3 + s) * 3 + c of pixel (y, x) =
+ * img[2y - pad_t + r][2x - pad_l + s][c] (0 outside the image), columns 27..63 zero. */
+int b2_op_stem_im2col(int device, const float* img, int H, int W, int Ho, int Wo, int pad_t, int pad_l, int split,
+                      float* out, uint16_t* out_hi, uint16_t* out_lo);
+
 #ifdef __cplusplus
 }
 #endif

@@ -133,6 +133,12 @@ SYMBOLS = [
     ("b2_op_relation", c_int, [c_int] + [c_void_p] * 10 + [c_int] * 4 + [c_void_p]),
     ("b2_op_deform_sample", c_int, [c_int, c_void_p, c_void_p] + [c_int] * 5 + [c_void_p]),
     ("b2_op_deform_conv2d", c_int, [c_int] + [c_void_p] * 4 + [c_int] * 7 + [c_void_p, c_void_p]),
+    ("b2_op_depthwise", c_int, [c_int] + [c_void_p] * 3 + [c_int] * 13 + [c_void_p] * 3),
+    ("b2_op_pool", c_int, [c_int, c_void_p] + [c_int] * 9 + [c_void_p] * 3),
+    ("b2_op_bifpn_combine", c_int, [c_int] + [c_void_p] * 3 + [c_int] * 7 + [c_void_p] * 4),
+    ("b2_op_mbconv_se", c_int, [c_int] + [c_void_p] * 6 + [c_int] * 7 + [c_void_p] * 4),
+    ("b2_op_channel_gate", c_int, [c_int] + [c_void_p] * 6 + [c_int] * 6 + [c_void_p] * 4),
+    ("b2_op_stem_im2col", c_int, [c_int, c_void_p] + [c_int] * 7 + [c_void_p] * 3),
 ]
 
 PHASES = dict(BACKBONE=1, FPN=2, RPN_HEAD=4, PROPOSALS=8, ROI=16, HEAD_FC=32, POST=64, BOX_FEAT=128, ALL=255)

@@ -319,6 +319,33 @@ int next_pow2(int v) {
 
 }  // namespace
 
+int bifpn_set_input(BifpnInput& bi, const __half* hi, const __half* lo, int H, int W, int th, int tw) {
+  bi.hi = hi; bi.lo = lo; bi.H = H; bi.W = W; bi.pad_t = bi.pad_l = 0; bi.weight = 1.f;
+  if (H == th && W == tw) {
+    bi.mode = 0;
+  } else if (H > th && W > tw) {
+    B2_CHECK((H - 1) / th + 1 == 2 && (W - 1) / tw + 1 == 2, "effdet: only stride-2 downsampling between levels");
+    const int ph = (th - 1) * 2 + 3 - H, pw = (tw - 1) * 2 + 3 - W;
+    bi.mode = 1;
+    bi.pad_t = (ph > 0 ? ph : 0) / 2;
+    bi.pad_l = (pw > 0 ? pw : 0) / 2;
+  } else {
+    B2_CHECK(H * 2 == th && W * 2 == tw, "effdet: only exact 2x nearest upsampling between levels");
+    bi.mode = 2;
+  }
+  return 0;
+}
+
+void bifpn_set_weights(BifpnCombineParams& p, const float* raw) {
+  float tot32 = 0.f;
+  for (int i = 0; i < p.n_in; ++i) {
+    const float r = raw[i] > 0.f ? raw[i] : 0.f;          // tf.nn.relu
+    p.in[i].weight = r;
+    tot32 = i == 0 ? r : tot32 + r;                       // tf.add_n in float32
+  }
+  p.denom = tot32 + 0.0001f;
+}
+
 int bifpn_combine_launch(const BifpnCombineParams& p, cudaStream_t s) {
   B2_CHECK(p.C % 8 == 0 && p.n_in >= 1 && p.n_in <= 3, "bifpn_combine: bad parameters");
   const size_t total = static_cast<size_t>(p.B) * p.Ho * p.Wo * (p.C / 8);

@@ -175,20 +175,7 @@ void add_combine(b2_effdet* c, std::unique_ptr<ECombine> K) {
 }
 
 int set_input(BifpnInput& bi, const Planes& src, int th, int tw) {
-  bi.hi = src.hi; bi.lo = src.lo; bi.H = src.H; bi.W = src.W; bi.pad_t = bi.pad_l = 0; bi.weight = 1.f;
-  if (src.H == th && src.W == tw) {
-    bi.mode = 0;
-  } else if (src.H > th && src.W > tw) {
-    B2_CHECK((src.H - 1) / th + 1 == 2 && (src.W - 1) / tw + 1 == 2, "effdet: only stride-2 downsampling between levels");
-    const int ph = (th - 1) * 2 + 3 - src.H, pw = (tw - 1) * 2 + 3 - src.W;
-    bi.mode = 1;
-    bi.pad_t = (ph > 0 ? ph : 0) / 2;
-    bi.pad_l = (pw > 0 ? pw : 0) / 2;
-  } else {
-    B2_CHECK(src.H * 2 == th && src.W * 2 == tw, "effdet: only exact 2x nearest upsampling between levels");
-    bi.mode = 2;
-  }
-  return 0;
+  return bifpn_set_input(bi, src.hi, src.lo, src.H, src.W, th, tw);
 }
 
 // resample_feature_map's optional 1x1 conv + BN (at the source resolution), arch.py:131-146
@@ -606,15 +593,13 @@ int b2_effdet_load_weights(b2_effdet* c, const char* const* names, const float* 
   if (c->cfg.fpn_weight_method == 1) {
     for (auto& K : c->combines) {
       if (!K->p.weighted) continue;
-      float tot32 = 0.f;
+      float raw[3];
       for (int i = 0; i < K->p.n_in; ++i) {
         const float* w = ws.get(K->wnames[i], 1);
         if (!w) return -1;
-        const float r = w[0] > 0.f ? w[0] : 0.f;          // tf.nn.relu
-        K->p.in[i].weight = r;
-        tot32 = i == 0 ? r : tot32 + r;                    // tf.add_n in float32
+        raw[i] = w[0];
       }
-      K->p.denom = tot32 + 0.0001f;
+      bifpn_set_weights(K->p, raw);
     }
   }
   c->loaded = true;

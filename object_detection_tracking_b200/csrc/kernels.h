@@ -18,6 +18,9 @@ int stem_pack_launch(const void* img, int is_u8, int B, int H, int W, __half* ou
 // compact operand of the detector stem: [B][Hu][Wv = Wu + 3][16] (stem.cu)
 int stem_pack16_launch(const void* img, int is_u8, int B, int H, int W, __half* out_hi, __half* out_lo, int Hu, int Wv,
                        cudaStream_t s);
+// 3x3 stride-2 max-pool, window rows 2y - 1 .. 2y + 1 (columns alike) clipped to the map, Ho x Wo chosen by the caller;
+// C a multiple of 8.  The running maximum starts from 0, so this is the max-pool only of inputs >= 0: every caller feeds
+// it post-ReLU data.  The output is the (hi, lo) pair of the element with the largest joined value.
 int maxpool_launch(const __half* in_hi, const __half* in_lo, int B, int H, int W, int C, __half* out_hi,
                    __half* out_lo, int Ho, int Wo, cudaStream_t s);
 
@@ -138,6 +141,10 @@ struct BifpnCombineParams {
   __half* out_hi;
   __half* out_lo;
 };
+// Input i of a node of size th x tw from a source map H x W: the resampling mode from the two sizes, and mode 1's pads
+int bifpn_set_input(BifpnInput& bi, const __half* hi, const __half* lo, int H, int W, int th, int tw);
+// fastattn: weight_i = relu(raw_i), denom = add_n(weights) + 1e-4, in float32 as build_bifpn_layer computes them
+void bifpn_set_weights(BifpnCombineParams& p, const float* raw);
 int bifpn_combine_launch(const BifpnCombineParams& p, cudaStream_t s);
 int dw3x3_plain_launch(const __half* in_hi, const __half* in_lo, int B, int H, int W, int C, const float* w, __half* out_hi,
                        __half* out_lo, cudaStream_t s);

@@ -1,5 +1,7 @@
 // Single-kernel entry points for parity tests and host tools: one conv, one grouped conv, one GroupNorm, one squeeze-excite,
-// one relation module, the deformable sampler and conv, the frame resize.  Each call owns its device buffers in an Arena, so every return path frees them.
+// one relation module, the deformable sampler and conv, the frame resize, and the element-wise and reduction kernels around
+// the GEMMs (depthwise convs, pools, the BiFPN combine, MBConv's squeeze-excite, OSNet's channel gate, EfficientNet's stem
+// im2col).  Each call owns its device buffers in an Arena, so every return path frees them.
 // The squeeze-excite, relation and deformable-conv calls build a one-block plan with the detector's builders (detplan.h).
 #include <string.h>
 
@@ -87,6 +89,23 @@ int run_plan(DetPlan& p, int device, const WeightSet& ws) {
   const cudaError_t e = cudaDeviceSynchronize();   // the kernels are done before their plans go away
   if (rc) return -1;
   B2_CUDA(e);
+  return 0;
+}
+
+// A device copy of n host floats (16-byte aligned, as the kernels' float4 loads need); nullptr for a null host pointer,
+// when out of memory or when the copy fails.
+float* upload_f32(Arena& a, const float* host, size_t n) {
+  if (!host) return nullptr;
+  float* d = a.alloc<float>(n);
+  if (d && cudaMemcpy(d, host, n * sizeof(float), cudaMemcpyHostToDevice) != cudaSuccess) d = nullptr;
+  return d;
+}
+
+// The first n elements of the planes p joined to fp32 in out and, where given, raw into out_hi / out_lo.
+int return_planes(const Planes& p, size_t n, float* out, uint16_t* out_hi, uint16_t* out_lo) {
+  if (download_planes(p.hi, p.lo, n, out, nullptr)) return -1;
+  if (out_hi) B2_CUDA(cudaMemcpy(out_hi, p.hi, n * sizeof(__half), cudaMemcpyDeviceToHost));
+  if (out_lo && p.lo) B2_CUDA(cudaMemcpy(out_lo, p.lo, n * sizeof(__half), cudaMemcpyDeviceToHost));
   return 0;
 }
 
@@ -411,6 +430,212 @@ int b2_op_deform_conv2d(int device, const float* x, const float* offset_w, const
                          op.elems() / C, cudaMemcpyDeviceToHost));
   }
   return 0;
+}
+
+// One depthwise conv: EfficientNet's strip kernel (impl 0) or OSNet's 3x3 (impl 1).
+int b2_op_depthwise(int device, const float* x, const float* w, const float* bias, int B, int H, int W, int C, int K,
+                    int stride, int pad_t, int pad_l, int Ho, int Wo, int act, int impl, int split, float* out,
+                    uint16_t* out_hi, uint16_t* out_lo) {
+  B2_CHECK(x && w && out, "b2_op_depthwise: null argument");
+  B2_CHECK(B >= 1 && H >= 1 && W >= 1 && C >= 8 && C % 8 == 0,
+           "b2_op_depthwise: needs positive sizes and C a multiple of 8");
+  if (impl == 0) {
+    B2_CHECK(B == 1 && (K == 3 || K == 5) && (stride == 1 || stride == 2) && pad_t >= 0 && pad_t < K && pad_l >= 0 &&
+                 pad_l < K && Ho >= 1 && Wo >= 1 && (act == 0 || act == 2),
+             "b2_op_depthwise: the strip kernel takes one image, K 3 or 5, stride 1 or 2, pads in [0, K), act 0 or 2");
+  } else {
+    B2_CHECK(impl == 1 && K == 3 && stride == 1 && pad_t == 1 && pad_l == 1 && Ho == H && Wo == W && act == 1 && bias,
+             "b2_op_depthwise: OSNet's depthwise conv is 3x3, stride 1, pad 1, with a bias and ReLU");
+  }
+  B2_CUDA(cudaSetDevice(device));
+  const bool sp = split != 0;
+  Arena a;
+  const Planes xp = a.planes(B, H, W, C, sp), op = a.planes(B, Ho, Wo, C, sp);
+  float* dw = upload_f32(a, w, static_cast<size_t>(K) * K * C);
+  float* db = upload_f32(a, bias, C);
+  B2_CHECK(xp.hi && op.hi && dw && (!bias || db), "b2_op_depthwise: out of device memory");
+  if (upload_planes(x, xp.hi, xp.lo, xp.elems(), nullptr)) return -1;
+  if (impl == 0) {
+    const DwConvParams p{xp.hi, xp.lo, H, W, C, K, stride, pad_t, pad_l, Ho, Wo, dw, db, op.hi, op.lo};
+    if (dwconv_launch(p, act, nullptr)) return -1;
+  } else if (dwconv3x3_launch(xp.hi, xp.lo, B, H, W, C, dw, db, op.hi, op.lo, nullptr)) {
+    return -1;
+  }
+  B2_CUDA(cudaDeviceSynchronize());
+  return return_planes(op, op.elems(), out, out_hi, out_lo);
+}
+
+// One pool: the stems' 3x3/2 max-pool (kind 0), OSNet's AvgPool2d(2) (kind 1) or the global average pool (kind 2).
+int b2_op_pool(int device, const float* x, int kind, int B, int H, int W, int C, int Ho, int Wo, int out_ld, int split,
+               float* out, uint16_t* out_hi, uint16_t* out_lo) {
+  B2_CHECK(x && out, "b2_op_pool: null argument");
+  B2_CHECK(B >= 1 && H >= 1 && W >= 1 && C >= 8 && C % 8 == 0, "b2_op_pool: needs positive sizes and C a multiple of 8");
+  if (kind == 0) {
+    B2_CHECK(Ho >= 1 && Wo >= 1 && Ho <= (H + 1) / 2 && Wo <= (W + 1) / 2,
+             "b2_op_pool: the max-pool's output must be at least 1 x 1 and at most ceil(H / 2) x ceil(W / 2)");
+  } else if (kind == 1) {
+    B2_CHECK(H >= 2 && W >= 2, "b2_op_pool: AvgPool2d(2) needs H, W >= 2");
+    Ho = H / 2;
+    Wo = W / 2;
+  } else {
+    B2_CHECK(kind == 2 && C % 64 == 0 && out_ld >= C, "b2_op_pool: kind 0, 1 or 2; the global pool needs C % 64 == 0 "
+                                                      "and out_ld >= C");
+  }
+  B2_CUDA(cudaSetDevice(device));
+  const bool sp = split != 0;
+  Arena a;
+  const Planes xp = a.planes(B, H, W, C, sp);
+  const Planes op = kind == 2 ? Planes() : a.planes(B, Ho, Wo, C, sp);
+  float* g = kind == 2 ? upload_f32(a, out, static_cast<size_t>(B) * out_ld) : nullptr;
+  B2_CHECK(xp.hi && (kind == 2 ? g != nullptr : op.hi != nullptr), "b2_op_pool: out of device memory");
+  if (upload_planes(x, xp.hi, xp.lo, xp.elems(), nullptr)) return -1;
+  const int rc = kind == 0   ? maxpool_launch(xp.hi, xp.lo, B, H, W, C, op.hi, op.lo, Ho, Wo, nullptr)
+                 : kind == 1 ? avgpool2_launch(xp.hi, xp.lo, B, H, W, C, op.hi, op.lo, nullptr)
+                             : gap_launch(xp.hi, xp.lo, B, H * W, C, g, out_ld, nullptr);
+  if (rc) return -1;
+  B2_CUDA(cudaDeviceSynchronize());
+  if (kind == 2) {
+    B2_CUDA(cudaMemcpy(out, g, static_cast<size_t>(B) * out_ld * sizeof(float), cudaMemcpyDeviceToHost));
+    return 0;
+  }
+  return return_planes(op, op.elems(), out, out_hi, out_lo);
+}
+
+// One BiFPN node combine, its inputs resampled and weighted as the EfficientDet engine sets them up.
+int b2_op_bifpn_combine(int device, const float* x, const int32_t* hw, const float* weights, int n_in, int B, int Ho,
+                        int Wo, int C, int swish, int split, float* out, uint16_t* out_hi, uint16_t* out_lo,
+                        int32_t* resample) {
+  B2_CHECK(x && hw && out, "b2_op_bifpn_combine: null argument");
+  B2_CHECK(n_in >= 1 && n_in <= 3 && B >= 1 && Ho >= 1 && Wo >= 1 && C >= 8 && C % 8 == 0,
+           "b2_op_bifpn_combine: needs 1 to 3 inputs, positive sizes and C a multiple of 8");
+  BifpnCombineParams p;
+  memset(&p, 0, sizeof(p));
+  for (int i = 0; i < n_in; ++i) {
+    B2_CHECK(hw[2 * i] >= 1 && hw[2 * i + 1] >= 1, "b2_op_bifpn_combine: empty input map");
+    if (bifpn_set_input(p.in[i], nullptr, nullptr, hw[2 * i], hw[2 * i + 1], Ho, Wo)) return -1;
+  }
+  B2_CUDA(cudaSetDevice(device));
+  const bool sp = split != 0;
+  Arena a;
+  Planes ip[3];
+  const Planes op = a.planes(B, Ho, Wo, C, sp);
+  B2_CHECK(op.hi, "b2_op_bifpn_combine: out of device memory");
+  size_t at = 0;
+  for (int i = 0; i < n_in; ++i) {
+    ip[i] = a.planes(B, hw[2 * i], hw[2 * i + 1], C, sp);
+    B2_CHECK(ip[i].hi, "b2_op_bifpn_combine: out of device memory");
+    if (upload_planes(x + at, ip[i].hi, ip[i].lo, ip[i].elems(), nullptr)) return -1;
+    at += ip[i].elems();
+    p.in[i].hi = ip[i].hi;
+    p.in[i].lo = ip[i].lo;
+  }
+  p.n_in = n_in; p.B = B; p.Ho = Ho; p.Wo = Wo; p.C = C;
+  p.weighted = weights != nullptr; p.denom = 1.f; p.swish = swish != 0;
+  if (weights) bifpn_set_weights(p, weights);
+  p.out_hi = op.hi; p.out_lo = op.lo;
+  if (bifpn_combine_launch(p, nullptr)) return -1;
+  B2_CUDA(cudaDeviceSynchronize());
+  if (resample)
+    for (int i = 0; i < n_in; ++i) {
+      resample[3 * i] = p.in[i].mode;
+      resample[3 * i + 1] = p.in[i].pad_t;
+      resample[3 * i + 2] = p.in[i].pad_l;
+    }
+  return return_planes(op, op.elems(), out, out_hi, out_lo);
+}
+
+// MBConv's squeeze-excite: the gate, and with the projection's master weight the folded weight (se_gate_launch); without
+// it the gate of B images (se_squeeze_launch + se_excite_launch).
+int b2_op_mbconv_se(int device, const float* x, const float* w1, const float* b1, const float* w2, const float* b2,
+                    const float* w, int B, int HW, int Cpad, int Creal, int nr, int rows, int split, float* gate,
+                    float* w_out, uint16_t* w_hi, uint16_t* w_lo) {
+  B2_CHECK(x && w1 && b1 && w2 && b2 && gate && (!w || w_out), "b2_op_mbconv_se: null argument");
+  B2_CHECK(B >= 1 && HW >= 1 && Cpad >= 64 && Cpad % 64 == 0 && Creal >= 1 && Creal <= Cpad && nr >= 1 &&
+               nr <= se_max_nr(),
+           "b2_op_mbconv_se: needs Cpad a multiple of 64, 1 <= Creal <= Cpad and 1 <= nr <= se_max_nr()");
+  B2_CHECK(!w || (B == 1 && rows >= 1), "b2_op_mbconv_se: the weight fold takes one image and at least one row");
+  B2_CUDA(cudaSetDevice(device));
+  const bool sp = split != 0;
+  Arena a;
+  const Planes xp = a.planes(B, HW, 1, Cpad, sp);
+  const Planes wp = w ? a.planes(1, rows, 1, Cpad, sp) : Planes();
+  float* partial = a.alloc<float>(static_cast<size_t>(B) * se_chunks(HW) * Cpad);
+  float* r_part = a.alloc<float>(static_cast<size_t>(B) * se_fc1_parts() * se_max_nr());
+  float* g = a.alloc<float>(static_cast<size_t>(B) * Cpad);
+  float* d_w1 = upload_f32(a, w1, static_cast<size_t>(Creal) * nr);
+  float* d_b1 = upload_f32(a, b1, nr);
+  float* d_w2 = upload_f32(a, w2, static_cast<size_t>(nr) * Creal);
+  float* d_b2 = upload_f32(a, b2, Creal);
+  float* d_w = upload_f32(a, w, static_cast<size_t>(rows) * Cpad);
+  B2_CHECK(xp.hi && (!w || (wp.hi && d_w)) && partial && r_part && g && d_w1 && d_b1 && d_w2 && d_b2,
+           "b2_op_mbconv_se: out of device memory");
+  if (upload_planes(x, xp.hi, xp.lo, xp.elems(), nullptr)) return -1;
+  if (w) {
+    if (se_gate_launch(xp.hi, xp.lo, HW, Cpad, Creal, nr, partial, r_part, d_w1, d_b1, d_w2, d_b2, g, d_w, rows, wp.hi,
+                       wp.lo, nullptr))
+      return -1;
+  } else if (se_squeeze_launch(xp.hi, xp.lo, B, HW, Cpad, partial, nullptr) ||
+             se_excite_launch(partial, B, HW, Cpad, Creal, nr, r_part, d_w1, d_b1, d_w2, d_b2, 0, g, nullptr, 0, nullptr,
+                              nullptr, nullptr)) {
+    return -1;
+  }
+  B2_CUDA(cudaDeviceSynchronize());
+  B2_CUDA(cudaMemcpy(gate, g, static_cast<size_t>(B) * Cpad * sizeof(float), cudaMemcpyDeviceToHost));
+  return w ? return_planes(wp, wp.elems(), w_out, w_hi, w_lo) : 0;
+}
+
+// OSNet's ChannelGate over an OSBlock's four streams and their gated sum, as reid_engine.cu runs them.
+int b2_op_channel_gate(int device, const float* s, const float* w1, const float* b1, const float* w2, const float* b2,
+                       const float* gates_in, int B, int HW, int C, int Creal, int Cr, int split, float* gates_out,
+                       float* out, uint16_t* out_hi, uint16_t* out_lo) {
+  B2_CHECK(s && out && (gates_in || (w1 && b1 && w2 && b2)), "b2_op_channel_gate: null argument");
+  B2_CHECK(B >= 1 && HW >= 1 && C >= 64 && C % 64 == 0 && Creal >= 1 && Creal <= C && Creal <= 512 && Cr >= 1 && Cr <= 64,
+           "b2_op_channel_gate: needs C a multiple of 64, 1 <= Creal <= min(C, 512) and 1 <= Cr <= 64");
+  B2_CUDA(cudaSetDevice(device));
+  const bool sp = split != 0;
+  const size_t n = static_cast<size_t>(B) * HW * C, ng = static_cast<size_t>(B) * 4 * C;
+  Arena a;
+  Planes sp4[4];
+  for (int k = 0; k < 4; ++k) sp4[k] = a.planes(B, HW, 1, C, sp);
+  const Planes op = a.planes(B, HW, 1, C, sp);
+  float* pooled = a.alloc<float>(ng);
+  float* gates = gates_in ? upload_f32(a, gates_in, ng) : a.alloc<float>(ng);
+  float* d_w1 = upload_f32(a, w1, static_cast<size_t>(Cr) * Creal);
+  float* d_b1 = upload_f32(a, b1, Cr);
+  float* d_w2 = upload_f32(a, w2, static_cast<size_t>(Creal) * Cr);
+  float* d_b2 = upload_f32(a, b2, Creal);
+  B2_CHECK(sp4[0].hi && sp4[1].hi && sp4[2].hi && sp4[3].hi && op.hi && pooled && gates &&
+               (gates_in || (d_w1 && d_b1 && d_w2 && d_b2)),
+           "b2_op_channel_gate: out of device memory");
+  for (int k = 0; k < 4; ++k)
+    if (upload_planes(s + k * n, sp4[k].hi, sp4[k].lo, n, nullptr)) return -1;
+  if (!gates_in) {
+    for (int k = 0; k < 4; ++k)
+      if (gap_launch(sp4[k].hi, sp4[k].lo, B, HW, C, pooled + static_cast<size_t>(k) * C, 4 * C, nullptr)) return -1;
+    if (gate_mlp_launch(pooled, B * 4, C, Creal, Cr, d_w1, d_b1, d_w2, d_b2, gates, nullptr)) return -1;
+  }
+  const __half* hi[4] = {sp4[0].hi, sp4[1].hi, sp4[2].hi, sp4[3].hi};
+  const __half* lo[4] = {sp4[0].lo, sp4[1].lo, sp4[2].lo, sp4[3].lo};
+  if (gated_sum4_launch(hi, lo, gates, B, HW, C, op.hi, op.lo, nullptr)) return -1;
+  B2_CUDA(cudaDeviceSynchronize());
+  if (gates_out) B2_CUDA(cudaMemcpy(gates_out, gates, ng * sizeof(float), cudaMemcpyDeviceToHost));
+  return return_planes(op, n, out, out_hi, out_lo);
+}
+
+// EfficientNet's stem operand: 3x3/2 patches of the fp32 image as 64-channel pixels (stem_im2col_launch).
+int b2_op_stem_im2col(int device, const float* img, int H, int W, int Ho, int Wo, int pad_t, int pad_l, int split,
+                      float* out, uint16_t* out_hi, uint16_t* out_lo) {
+  B2_CHECK(img && out, "b2_op_stem_im2col: null argument");
+  B2_CHECK(H >= 1 && W >= 1 && Ho >= 1 && Wo >= 1 && pad_t >= 0 && pad_t < 3 && pad_l >= 0 && pad_l < 3,
+           "b2_op_stem_im2col: needs positive sizes and pads in [0, 3)");
+  B2_CUDA(cudaSetDevice(device));
+  Arena a;
+  const Planes op = a.planes(1, Ho, Wo, 64, split != 0);
+  float* d_img = upload_f32(a, img, static_cast<size_t>(H) * W * 3);
+  B2_CHECK(op.hi && d_img, "b2_op_stem_im2col: out of device memory");
+  if (stem_im2col_launch(d_img, H, W, Ho, Wo, pad_t, pad_l, op.hi, op.lo, nullptr)) return -1;
+  B2_CUDA(cudaDeviceSynchronize());
+  return return_planes(op, op.elems(), out, out_hi, out_lo);
 }
 
 // The resize alone (parity tests): host uint8 [n, src_h, src_w, 3] -> host float32 [n, dst_h, dst_w, 3].

@@ -118,9 +118,9 @@ Planes add_stem(b2_reid* c, const std::string& wname, const std::string& bn) {
   return c1;
 }
 
-// maxpool 3/2 pad 1
+// maxpool 3/2 pad 1: nn.MaxPool2d(3, 2, 1) gives (H - 1) / 2 + 1 rows, the last window cut by the border when H is odd
 Planes add_maxpool(b2_reid* c, const Planes& a) {
-  const Planes b = c->planes(a.B, a.H / 2, a.W / 2, a.C);
+  const Planes b = c->planes(a.B, (a.H - 1) / 2 + 1, (a.W - 1) / 2 + 1, a.C);
   add_step(c->steps, 0, 0, "", [a, b](cudaStream_t st) {
     return maxpool_launch(a.hi, a.lo, a.B, a.H, a.W, a.C, b.hi, b.lo, b.H, b.W, st);
   });

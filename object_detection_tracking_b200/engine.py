@@ -417,6 +417,141 @@ def op_deform_conv2d(x, offset_w, offset_b, w, impl="tcgen05", split=True, retur
     return (out, off) if return_offsets else out
 
 
+def _f32(a):
+    return None if a is None else np.ascontiguousarray(a, dtype=np.float32)
+
+
+def _plane_outputs(shape, split):
+    """fp32 output and its raw planes (uint16; lo None in fp16 precision) of a plane-output op."""
+    return (np.empty(shape, np.float32), np.empty(shape, np.uint16),
+            np.empty(shape, np.uint16) if split else None)
+
+
+def op_depthwise(x, w, bias=None, stride=1, pad=(0, 0), out_hw=None, act="none", impl="effnet", split=True, device=0):
+    """One depthwise conv through the C ABI -- used by the kernel tests: x [B, H, W, C] NHWC, w [K, K, C], bias [C].
+    impl "effnet": EfficientNet's strip kernel (B = 1; pad = (pad_t, pad_l), output size out_hw; act "none" / "swish");
+    impl "osnet": OSNet's 3x3 stride-1 pad-1 conv + bias + ReLU (act "relu").  Returns (out, hi, lo) as
+    op_conv2d_view does."""
+    lib = _lib.load()
+    x = _f32(x)
+    w = _f32(w)
+    B, H, W, C = x.shape
+    K = w.shape[0]
+    assert w.shape == (K, K, C), w.shape
+    Ho, Wo = out_hw if out_hw is not None else (H, W)
+    out, hi, lo = _plane_outputs((B, Ho, Wo, C), split)
+    _lib.check(lib.b2_op_depthwise(device, _lib.ptr(x), _lib.ptr(w), _lib.ptr(_f32(bias)), B, H, W, C, K, stride,
+                                   pad[0], pad[1], Ho, Wo, {"none": 0, "relu": 1, "swish": 2}[act],
+                                   {"effnet": 0, "osnet": 1}[impl], int(split), _lib.ptr(out), _lib.ptr(hi),
+                                   _lib.ptr(lo)),
+               "b2_op_depthwise")
+    return out, hi, lo
+
+
+def op_pool(x, kind, out_hw=None, out_ld=None, out_init=None, split=True, device=0):
+    """One pool through the C ABI -- used by the kernel tests: x [B, H, W, C] NHWC.  kind "max": the stems' 3x3/2
+    max-pool (inputs >= 0) with the caller's output size out_hw; "avg2": AvgPool2d(2); "gap": the global average pool
+    into a [B, out_ld] fp32 buffer that starts as out_init (default zeros).  Returns (out, hi, lo); hi, lo are None for
+    "gap"."""
+    lib = _lib.load()
+    x = _f32(x)
+    B, H, W, C = x.shape
+    k = {"max": 0, "avg2": 1, "gap": 2}[kind]
+    hi = lo = None
+    Ho = Wo = 0
+    if k == 2:
+        ld = out_ld or C
+        out = np.zeros((B, ld), np.float32) if out_init is None else np.array(out_init, np.float32, copy=True)
+        assert out.shape == (B, ld), out.shape
+    else:
+        ld = 0
+        Ho, Wo = out_hw if k == 0 else (H // 2, W // 2)
+        out, hi, lo = _plane_outputs((B, Ho, Wo, C), split)
+    _lib.check(lib.b2_op_pool(device, _lib.ptr(x), k, B, H, W, C, Ho, Wo, ld, int(split), _lib.ptr(out), _lib.ptr(hi),
+                              _lib.ptr(lo)),
+               "b2_op_pool")
+    return out, hi, lo
+
+
+def op_bifpn_combine(inputs, out_hw, weights=None, swish=False, split=True, device=0):
+    """One BiFPN node combine through the C ABI -- used by the kernel tests: inputs a list of 1 to 3 [B, H_i, W_i, C]
+    maps, each resampled to out_hw as the EfficientDet engine does; weights the raw fastattn weights (None: plain sum).
+    Returns (out, hi, lo, resample) with resample [n, 3] = (mode, pad_t, pad_l) per input."""
+    lib = _lib.load()
+    xs = [_f32(t) for t in inputs]
+    B, C = xs[0].shape[0], xs[0].shape[3]
+    assert all(t.shape[0] == B and t.shape[3] == C for t in xs), [t.shape for t in xs]
+    flat = np.ascontiguousarray(np.concatenate([t.ravel() for t in xs]))
+    hw = np.array([t.shape[1:3] for t in xs], np.int32)
+    wts = None if weights is None else _f32(np.asarray(weights, np.float32).reshape(len(xs)))
+    Ho, Wo = out_hw
+    out, hi, lo = _plane_outputs((B, Ho, Wo, C), split)
+    res = np.zeros((len(xs), 3), np.int32)
+    _lib.check(lib.b2_op_bifpn_combine(device, _lib.ptr(flat), _lib.ptr(hw), _lib.ptr(wts), len(xs), B, Ho, Wo, C,
+                                       int(bool(swish)), int(split), _lib.ptr(out), _lib.ptr(hi), _lib.ptr(lo),
+                                       _lib.ptr(res)),
+               "b2_op_bifpn_combine")
+    return out, hi, lo, res
+
+
+def op_mbconv_se(x, creal, w1, b1, w2, b2, w=None, split=True, device=0):
+    """MBConv's squeeze-excite through the C ABI -- used by the kernel tests: x [B, HW, Cpad] with channels [0, creal)
+    live, w1 [creal, nr], b1 [nr], w2 [nr, creal], b2 [creal]; w the projection's master weight [rows, Cpad] (B = 1) or
+    None.  Returns (gate [B, Cpad], folded, hi, lo): the folded weight joined and as raw planes (None without w)."""
+    lib = _lib.load()
+    x = _f32(x)
+    B, HW, Cp = x.shape
+    w1 = _f32(w1)
+    nr = w1.shape[1]
+    assert w1.shape == (creal, nr) and np.shape(w2) == (nr, creal), (w1.shape, np.shape(w2))
+    w = _f32(w)
+    rows = 0 if w is None else w.shape[0]
+    assert w is None or w.shape == (rows, Cp), w.shape
+    gate = np.empty((B, Cp), np.float32)
+    folded = hi = lo = None
+    if w is not None:
+        folded, hi, lo = _plane_outputs((rows, Cp), split)
+    _lib.check(lib.b2_op_mbconv_se(device, _lib.ptr(x), _lib.ptr(w1), _lib.ptr(_f32(b1)), _lib.ptr(_f32(w2)),
+                                   _lib.ptr(_f32(b2)), _lib.ptr(w), B, HW, Cp, creal, nr, rows, int(split),
+                                   _lib.ptr(gate), _lib.ptr(folded), _lib.ptr(hi), _lib.ptr(lo)),
+               "b2_op_mbconv_se")
+    return gate, folded, hi, lo
+
+
+def op_channel_gate(streams, creal, w1=None, b1=None, w2=None, b2=None, gates=None, split=True, device=0):
+    """OSNet's ChannelGate and 4-stream gated sum through the C ABI -- used by the kernel tests: streams [4, B, HW, C]
+    with channels [0, creal) live, w1 [Cr, creal], b1 [Cr], w2 [creal, Cr], b2 [creal]; gates [B, 4, C] given instead
+    runs the gated sum alone.  Returns (gates [B, 4, C], out, hi, lo) with out [B, HW, C]."""
+    lib = _lib.load()
+    s = _f32(streams)
+    _, B, HW, C = s.shape
+    assert s.shape[0] == 4, s.shape
+    cr = 1 if w1 is None else np.shape(w1)[0]
+    g_in = _f32(gates)
+    assert g_in is None or g_in.shape == (B, 4, C), g_in.shape
+    g_out = np.empty((B, 4, C), np.float32)
+    out, hi, lo = _plane_outputs((B, HW, C), split)
+    _lib.check(lib.b2_op_channel_gate(device, _lib.ptr(s), _lib.ptr(_f32(w1)), _lib.ptr(_f32(b1)), _lib.ptr(_f32(w2)),
+                                      _lib.ptr(_f32(b2)), _lib.ptr(g_in), B, HW, C, creal, cr, int(split),
+                                      _lib.ptr(g_out), _lib.ptr(out), _lib.ptr(hi), _lib.ptr(lo)),
+               "b2_op_channel_gate")
+    return g_out, out, hi, lo
+
+
+def op_stem_im2col(img, out_hw, pad, split=True, device=0):
+    """EfficientNet's stem im2col through the C ABI -- used by the kernel tests: img [H, W, 3] fp32, out_hw = (Ho, Wo),
+    pad = (pad_t, pad_l).  Returns (out, hi, lo) of the [Ho, Wo, 64] operand."""
+    lib = _lib.load()
+    img = _f32(img)
+    H, W, _ = img.shape
+    Ho, Wo = out_hw
+    out, hi, lo = _plane_outputs((Ho, Wo, 64), split)
+    _lib.check(lib.b2_op_stem_im2col(device, _lib.ptr(img), H, W, Ho, Wo, pad[0], pad[1], int(split), _lib.ptr(out),
+                                     _lib.ptr(hi), _lib.ptr(lo)),
+               "b2_op_stem_im2col")
+    return out, hi, lo
+
+
 def get_new_hw(h, w, size, max_size):
     """nn.py:1548-1560: (neww, newh) of resizeImage for an h x w frame."""
     scale = size * 1.0 / min(h, w)
