@@ -280,6 +280,8 @@ typedef struct b2_effdet_config {
   int precision;                   /* 0 fp16, 1 split (fp32-class) */
   int backbone;                    /* -1: none (b2_effdet_run_features only); 0..7: EfficientNet-b0..b7 trunk
                                     * (efficientdet_arch.py:396-437, backbone/efficientnet_model.py:504-704) */
+  int batch;                       /* images per call; 0 or 1: one (b2_effdet_detect / b2_effdet_run_features),
+                                    * > 1: b2_effdet_detect_batch, stages gain a leading [batch] */
 } b2_effdet_config;
 typedef struct b2_effdet b2_effdet;
 int b2_effdet_create(b2_effdet** out, const b2_effdet_config* cfg, int device);
@@ -295,12 +297,25 @@ int b2_effdet_run_features(b2_effdet* ctx, const float* c3, const float* c4, con
  * in frame pixels.  *image_scale_out = image_scale_to_original.  Needs cfg.backbone >= 0. */
 int b2_effdet_detect(b2_effdet* ctx, const uint8_t* frame_bgr, int h, int w, float* boxes, float* scores,
                      int32_t* classes, int32_t* levels, float* box_feat, int32_t* count, float* image_scale_out);
+/* The same for 1 <= n <= batch independent frames of any sizes (frames[i] is [h[i], w[i], 3]) in one pass of a context
+ * created with `batch` images; image i's outputs are bit-identical to b2_effdet_detect(frames[i]) on a batch-1 context.
+ * boxes [batch][max][4], scores / classes / levels [batch][max], box_feat [batch][max][fpn_num_filters], counts [batch],
+ * image_scales [batch]; rows past counts[i] are zero, blocks i >= n are not written (those images run on the last
+ * frame). */
+int b2_effdet_detect_batch(b2_effdet* ctx, const uint8_t* const* frames, const int32_t* h, const int32_t* w, int n,
+                           float* boxes, float* scores, int32_t* classes, int32_t* levels, float* box_feat, int32_t* counts,
+                           float* image_scales);
+/* Replays the whole-frame graph the last detect call captured `reps` times on the images as they stand (no host copies);
+ * *ms_out = mean milliseconds per replay. */
+int b2_effdet_replay(b2_effdet* ctx, int reps, float* ms_out);
 /* Stage tensors of the last pass (parity tests): "image", "stem", "block_<i>", "c3".."c5", "fpn3".."fpn7", "cls3".."cls7", "box3".."box7" as fp32 NHWC */
 int b2_effdet_get_stage(b2_effdet* ctx, const char* name, float* dst_host, int64_t capacity_bytes, int64_t shape[4]);
 /* Post-processing stages: "topk_boxes" [k][4] (ymin xmin ymax xmax, network pixels), "topk_scores" [k], "topk_classes"
  * [k] (int32, 1-based), "topk_levels" [k] (int32), "topk_count" (int32): the candidates in top-k order (logit descending,
  * then flat index); "final_boxes" [max][4] (x1 y1 x2 y2 * image_scale), "final_scores", "final_classes", "final_levels",
- * "final_count" (int32) and "box_feat" [max][fpn_num_filters]: the outputs; "image_scale" (one float). */
+ * "final_count" (int32) and "box_feat" [max][fpn_num_filters]: the outputs; "image_scale" (one float).
+ * On a context with batch > 1 every stage has shape[0] = batch (image-major), and "topk_count" is the [batch][8] top-k
+ * state with each image's count in column 5. */
 /* Writes a stage (bytes = its whole stored size) for b2_effdet_run_phases. */
 int b2_effdet_set_stage(b2_effdet* ctx, const char* name, const void* src_host, int64_t bytes);
 /* Run a subset of the pass eagerly: bit mask of B2_EFFDET_PHASE_*. */

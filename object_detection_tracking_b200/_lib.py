@@ -40,6 +40,7 @@ class B2EffdetConfig(ctypes.Structure):
         ("aspect_ratios", (c_float * 2) * 3), ("anchor_scale", c_float), ("fpn_weight_method", c_int32),
         ("backbone_channels", c_int32 * 3), ("max_detection_topk", c_int32), ("result_per_im", c_int32),
         ("nms_iou_threshold", c_float), ("result_score_thres", c_float), ("precision", c_int32), ("backbone", c_int32),
+        ("batch", c_int32),
     ]
 
 
@@ -111,6 +112,8 @@ SYMBOLS = [
     ("b2_effdet_load_weights", c_int, [c_void_p, POINTER(c_char_p), POINTER(c_void_p), POINTER(c_int64), c_int]),
     ("b2_effdet_run_features", c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_float] + [c_void_p] * 6),
     ("b2_effdet_detect", c_int, [c_void_p, c_void_p, c_int, c_int] + [c_void_p] * 7),
+    ("b2_effdet_detect_batch", c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_int] + [c_void_p] * 7),
+    ("b2_effdet_replay", c_int, [c_void_p, c_int, POINTER(c_float)]),
     ("b2_effdet_get_stage", c_int, [c_void_p, c_char_p, c_void_p, c_int64, POINTER(c_int64)]),
     ("b2_effdet_set_stage", c_int, [c_void_p, c_char_p, c_void_p, c_int64]),
     ("b2_effdet_run_phases", c_int, [c_void_p, c_int]),

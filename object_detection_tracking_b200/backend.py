@@ -309,6 +309,65 @@ class EfficientDet:
         return res
 
 
+class EfficientDet_multi(EfficientDet):
+    """Batch-mode EfficientDet model object for the reference's batch drivers (obj_detect_tracking_multi_queuer.py:472-515
+    with --is_efficientdet): `get_feed_dict_forward_multi(imgs)` and the `final_valid_indices` fetch.  The frames of a
+    batch may differ in size; each runs with the single-image semantics of `EfficientDet` (bit-identical outputs) in one
+    pass of a batch context, one context per batch size.  Outputs in the batch graph's layout: boxes [B, result_per_im, 4]
+    and probs [B, result_per_im] zero-padded, labels [B, result_per_im] float32 (1-based, 0 in the padding), valid [B]
+    int32, fpn_box_feat [sum(valid), fpn_num_filters] image by image."""
+
+    is_multi = True
+
+    def __init__(self, config, gpuid=0, precision="split"):
+        super().__init__(config, gpuid=gpuid, precision=precision)
+        self.final_valid_indices = TensorHandle(self, "final_valid_indices:0")
+        self._engines = {}
+
+    def set_weights(self, weights: dict):
+        super().set_weights(weights)
+        for e in self._engines.values():
+            e.load_weights(self._weights)
+
+    def get_feed_dict_forward_multi(self, imgdatas):
+        """models.py:3301-3310: the batch's frames, each [h, w, 3]."""
+        return {self.image: [np.asarray(im) for im in imgdatas]}
+
+    def _engine_for(self, batch: int):
+        from .effdet import EffdetEngine
+        eng = self._engines.get(batch)
+        if eng is None:
+            if self._weights is None:
+                raise RuntimeError("model has no weights: call set_weights()/load_npz() first")
+            eng = EffdetEngine(self.eff_config, self._weights, device=self.gpuid, precision=self.precision,
+                               backbone=self.backbone_name, batch=batch)
+            self._engines[batch] = eng
+        return eng
+
+    def _run(self, fetches, feed_dict):
+        imgs = feed_dict[self.image]
+        frames = [np.asarray(f) for f in (imgs if isinstance(imgs, (list, tuple)) else np.asarray(imgs))]
+        frames = [f if f.dtype == np.uint8 else f.astype(np.uint8) for f in frames]     # the placeholder is uint8
+        B, m = len(frames), int(self.eff_config.result_per_im)
+        outs = self._engine_for(B).detect_batch(frames)
+        boxes = np.zeros((B, m, 4), np.float32)
+        labels = np.zeros((B, m), np.float32)
+        probs = np.zeros((B, m), np.float32)
+        valid = np.zeros(B, np.int32)
+        for b, o in enumerate(outs):
+            r = len(o["final_probs"])
+            boxes[b, :r], labels[b, :r], probs[b, :r], valid[b] = o["final_boxes"], o["final_labels"], o["final_probs"], r
+        feat = np.concatenate([o["fpn_box_feat"] for o in outs], axis=0)
+        table = {id(self.final_boxes): boxes, id(self.final_labels): labels, id(self.final_probs): probs,
+                 id(self.final_valid_indices): valid, id(self.fpn_box_feat): feat}
+        res = []
+        for f in fetches:
+            if id(f) not in table:
+                raise KeyError("unknown fetch %r" % (f,))
+            res.append(table[id(f)].copy())
+        return res
+
+
 class Session:
     """`sess.run(fetches, feed_dict=...)` for fetches that all belong to one model object."""
 
@@ -333,7 +392,8 @@ def get_model(config, gpuid=0, task=0, controller="/cpu:0", is_multi=False, **kw
     """models.get_model (models.py:97-119).  `controller`/`task` are TF device-placement arguments with
     no meaning here; kept for signature compatibility."""
     if getattr(config, "is_efficientdet", False):
-        model = EfficientDet(config, gpuid=gpuid, **kw)                 # models.py:112-113
+        cls = EfficientDet_multi if is_multi else EfficientDet
+        model = cls(config, gpuid=gpuid, **kw)                          # models.py:112-113
         if getattr(config, "is_load_from_pb", False):                   # EfficientDet_frozen (models.py:103-104)
             model.load_pb(config.load_from)
         return model

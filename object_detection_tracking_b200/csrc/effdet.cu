@@ -73,52 +73,64 @@ __global__ void bifpn_combine_kernel(const __grid_constant__ BifpnCombineParams 
 }
 
 // ---- global top-k over all class logits: multi-block radix select on order-preserving keys ----------
+// Every kernel below works on image blockIdx.y (blockIdx.z for the NMS mask) and touches only that image's slices.
+constexpr unsigned kTopkMaxBlocks = 132 * 8;
+
 __device__ __forceinline__ int level_of(const EffdetPostParams& p, unsigned long long i) {
   int l = 0;
   while (l + 1 < p.n_levels && i >= p.level_off[l + 1]) ++l;
   return l;
 }
 
-__device__ __forceinline__ float logit_at(const EffdetPostParams& p, unsigned long long i) {
+__device__ __forceinline__ float logit_at(const EffdetPostParams& p, int b, unsigned long long i) {
   const int l = level_of(p, i);
   const unsigned long long r = i - p.level_off[l];
   const unsigned int per_pos = static_cast<unsigned int>(p.anchors * p.num_classes);
   const unsigned long long pos = r / per_pos;
   const unsigned int k = static_cast<unsigned int>(r - pos * per_pos);
-  return __ldg(p.logits[l] + pos * p.ld[l] + k);
+  return __ldg(p.logits[l] + b * p.logit_bstride[l] + pos * p.ld[l] + k);
 }
+
+__device__ __forceinline__ uint32_t* state_of(const EffdetPostParams& p, int b) { return p.state + 8 * b; }
+__device__ __forceinline__ unsigned int* hist_of(const EffdetPostParams& p, int b) { return p.hist + 256 * b; }
+__device__ __forceinline__ size_t kslice(const EffdetPostParams& p, int b) { return static_cast<size_t>(b) * p.k; }
 
 __global__ void topk_hist_kernel(const __grid_constant__ EffdetPostParams p, int pass) {
   __shared__ unsigned int h[256];
+  const int b = blockIdx.y;
   for (int i = threadIdx.x; i < 256; i += blockDim.x) h[i] = 0;
   __syncthreads();
   const int shift = 24 - 8 * pass;
-  const uint32_t prefix = p.state[0], pmask = p.state[1];
+  const uint32_t* state = state_of(p, b);
+  const uint32_t prefix = state[0], pmask = state[1];
   for (unsigned long long i = blockIdx.x * static_cast<unsigned long long>(blockDim.x) + threadIdx.x; i < p.total;
        i += static_cast<unsigned long long>(gridDim.x) * blockDim.x) {
-    const uint32_t key = float_key(logit_at(p, i));
+    const uint32_t key = float_key(logit_at(p, b, i));
     if ((key & pmask) == prefix) atomicAdd(&h[(key >> shift) & 255], 1u);
   }
   __syncthreads();
+  unsigned int* hist = hist_of(p, b);
   for (int i = threadIdx.x; i < 256; i += blockDim.x)
-    if (h[i]) atomicAdd(&p.hist[i], h[i]);
+    if (h[i]) atomicAdd(&hist[i], h[i]);
 }
 
 __global__ void topk_pick_kernel(const __grid_constant__ EffdetPostParams p, int pass) {
+  uint32_t* state = state_of(p, blockIdx.y);
+  unsigned int* hist = hist_of(p, blockIdx.y);
   if (threadIdx.x == 0) {
     const int shift = 24 - 8 * pass;
-    unsigned int need = p.state[2], cum = 0;
+    unsigned int need = state[2], cum = 0;
     int bsel = 0;
     for (int b = 255; b >= 0; --b) {
-      if (cum + p.hist[b] >= need) { bsel = b; break; }
-      cum += p.hist[b];
+      if (cum + hist[b] >= need) { bsel = b; break; }
+      cum += hist[b];
     }
-    p.state[2] = need - cum;
-    p.state[0] |= static_cast<uint32_t>(bsel) << shift;
-    p.state[1] |= 255u << shift;
+    state[2] = need - cum;
+    state[0] |= static_cast<uint32_t>(bsel) << shift;
+    state[1] |= 255u << shift;
   }
   __syncthreads();
-  for (int i = threadIdx.x; i < 256; i += blockDim.x) p.hist[i] = 0;
+  for (int i = threadIdx.x; i < 256; i += blockDim.x) hist[i] = 0;
 }
 
 // collect every key > kth (any order) and count the ties == kth per block (blocks own contiguous index ranges)
@@ -126,45 +138,53 @@ __global__ void topk_collect_kernel(const __grid_constant__ EffdetPostParams p, 
   __shared__ unsigned int s_ties;
   if (threadIdx.x == 0) s_ties = 0;
   __syncthreads();
-  const uint32_t kth = p.state[0];
+  const int b = blockIdx.y;
+  uint32_t* state = state_of(p, b);
+  unsigned long long* cand = p.cand + kslice(p, b);
+  const uint32_t kth = state[0];
   const unsigned long long lo = blockIdx.x * chunk;
   const unsigned long long hi = lo + chunk < p.total ? lo + chunk : p.total;
   unsigned int mine = 0;
   for (unsigned long long i = lo + threadIdx.x; i < hi; i += blockDim.x) {
-    const float v = logit_at(p, i);
+    const float v = logit_at(p, b, i);
     const uint32_t key = float_key(v);
     if (key > kth) {
-      const unsigned int slot = atomicAdd(&p.state[3], 1u);
-      if (slot < static_cast<unsigned int>(p.k)) p.cand[slot] = desc_key(v, static_cast<uint32_t>(i));
+      const unsigned int slot = atomicAdd(&state[3], 1u);
+      if (slot < static_cast<unsigned int>(p.k)) cand[slot] = desc_key(v, static_cast<uint32_t>(i));
     } else if (key == kth) {
       ++mine;
     }
   }
   if (mine) atomicAdd(&s_ties, mine);
   __syncthreads();
-  if (threadIdx.x == 0) p.tie_cnt[blockIdx.x] = s_ties;
+  if (threadIdx.x == 0) p.tie_cnt[static_cast<size_t>(b) * kTopkMaxBlocks + blockIdx.x] = s_ties;
 }
 
-// exclusive prefix of the per-block tie counts (one block; <= a few thousand entries)
+// exclusive prefix of the per-block tie counts (one block per image; <= a few thousand entries)
 __global__ void topk_tie_scan_kernel(const __grid_constant__ EffdetPostParams p, int nblocks) {
   if (threadIdx.x == 0) {
+    const size_t o = static_cast<size_t>(blockIdx.y) * kTopkMaxBlocks;
     unsigned int run = 0;
     for (int b = 0; b < nblocks; ++b) {
-      const unsigned int c = p.tie_cnt[b];
-      p.tie_off[b] = run;
+      const unsigned int c = p.tie_cnt[o + b];
+      p.tie_off[o + b] = run;
       run += c;
     }
-    p.state[4] = run;
+    state_of(p, blockIdx.y)[4] = run;
   }
 }
 
 // tf.nn.top_k keeps the lowest flat indices among equal values: write the first `need` ties in index order
 __global__ void __launch_bounds__(256) topk_tie_write_kernel(const __grid_constant__ EffdetPostParams p, unsigned long long chunk) {
-  const unsigned int need = p.state[2];
-  unsigned int base = p.tie_off[blockIdx.x];
-  if (p.tie_cnt[blockIdx.x] == 0 || base >= need) return;
+  const int img = blockIdx.y;
+  const uint32_t* state = state_of(p, img);
+  const size_t o = static_cast<size_t>(img) * kTopkMaxBlocks + blockIdx.x;
+  unsigned long long* ties = p.ties + kslice(p, img);
+  const unsigned int need = state[2];
+  unsigned int base = p.tie_off[o];
+  if (p.tie_cnt[o] == 0 || base >= need) return;
   __shared__ unsigned int warp_cnt[8];
-  const uint32_t kth = p.state[0];
+  const uint32_t kth = state[0];
   const unsigned long long lo = blockIdx.x * chunk;
   const unsigned long long hi = lo + chunk < p.total ? lo + chunk : p.total;
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
@@ -173,7 +193,7 @@ __global__ void __launch_bounds__(256) topk_tie_write_kernel(const __grid_consta
     float v = 0.f;
     bool tie = false;
     if (i < hi) {
-      v = logit_at(p, i);
+      v = logit_at(p, img, i);
       tie = float_key(v) == kth;
     }
     const unsigned int bal = __ballot_sync(0xffffffffu, tie);
@@ -188,23 +208,31 @@ __global__ void __launch_bounds__(256) topk_tie_write_kernel(const __grid_consta
     }
     if (tie) {
       const unsigned int rank = base + before + __popc(bal & ((1u << lane) - 1u));
-      if (rank < need) p.ties[rank] = desc_key(v, static_cast<uint32_t>(i));
+      if (rank < need) ties[rank] = desc_key(v, static_cast<uint32_t>(i));
     }
     base += tile;
     __syncthreads();
   }
 }
 
-// one block: (selected U lowest-index ties) sorted by (logit desc, index asc) = tf.nn.top_k order; then
+// one block per image: (selected U lowest-index ties) sorted by (logit desc, index asc) = tf.nn.top_k order; then
 // sigmoid + anchor decode per candidate
 __global__ void __launch_bounds__(1024, 1) det_prepare_kernel(const __grid_constant__ EffdetPostParams p, int KP) {
   extern __shared__ __align__(16) uint8_t sm[];
   uint64_t* keys = reinterpret_cast<uint64_t*>(sm);     // [KP]
-  const int tid = threadIdx.x;
-  const int n_gt = min(static_cast<int>(p.state[3]), p.k);
-  const int take = min(min(static_cast<int>(p.state[2]), static_cast<int>(p.state[4])), p.k - n_gt);
+  const int tid = threadIdx.x, img = blockIdx.y;
+  uint32_t* state = state_of(p, img);
+  const size_t ks = kslice(p, img);
+  const unsigned long long* cand = p.cand + ks;
+  const unsigned long long* ties = p.ties + ks;
+  float4* cand_box = p.cand_box + ks;
+  float* cand_score = p.cand_score + ks;
+  int* cand_cls = p.cand_cls + ks;
+  int* cand_lvl = p.cand_lvl + ks;
+  const int n_gt = min(static_cast<int>(state[3]), p.k);
+  const int take = min(min(static_cast<int>(state[2]), static_cast<int>(state[4])), p.k - n_gt);
   const int K = n_gt + take;
-  for (int i = tid; i < KP; i += blockDim.x) keys[i] = i < n_gt ? p.cand[i] : (i < K ? p.ties[i - n_gt] : ~0ull);
+  for (int i = tid; i < KP; i += blockDim.x) keys[i] = i < n_gt ? cand[i] : (i < K ? ties[i - n_gt] : ~0ull);
   block_bitonic_sort(keys, KP);
   const unsigned int per_pos = static_cast<unsigned int>(p.anchors * p.num_classes);
   for (int j = tid; j < K; j += blockDim.x) {
@@ -215,7 +243,7 @@ __global__ void __launch_bounds__(1024, 1) det_prepare_kernel(const __grid_const
     const int kk = static_cast<int>(r - pos * per_pos);
     const int a = kk / p.num_classes, cls = kk - a * p.num_classes;
     const int y = static_cast<int>(pos / p.w[l]), x = static_cast<int>(pos - static_cast<unsigned long long>(y) * p.w[l]);
-    const float logit = __ldg(p.logits[l] + pos * p.ld[l] + kk);
+    const float logit = __ldg(p.logits[l] + img * p.logit_bstride[l] + pos * p.ld[l] + kk);
     const float score = 1.f / (1.f + expf(-logit));
     // anchor (anchors.py:216-257), float64 grid like numpy, rounded once to float32
     const double yc_d = __dadd_rn(p.stride_y[l] / 2.0, __dmul_rn(static_cast<double>(y), p.stride_y[l]));
@@ -227,22 +255,26 @@ __global__ void __launch_bounds__(1024, 1) det_prepare_kernel(const __grid_const
     // decode_box_outputs_tf (anchors.py:369-396)
     const float yca = __fdiv_rn(__fadd_rn(ymin_a, ymax_a), 2.f), xca = __fdiv_rn(__fadd_rn(xmin_a, xmax_a), 2.f);
     const float ha = __fsub_rn(ymax_a, ymin_a), wa = __fsub_rn(xmax_a, xmin_a);
-    const float* t = p.boxes[l] + pos * p.ldb[l] + a * 4;
+    const float* t = p.boxes[l] + img * p.box_bstride[l] + pos * p.ldb[l] + a * 4;
     const float ty = __ldg(t), tx = __ldg(t + 1), th = __ldg(t + 2), tw = __ldg(t + 3);
     const float w = __fmul_rn(expf(tw), wa), h = __fmul_rn(expf(th), ha);
     const float yc = __fadd_rn(__fmul_rn(ty, ha), yca), xc = __fadd_rn(__fmul_rn(tx, wa), xca);
-    p.cand_box[j] = make_float4(__fsub_rn(yc, __fdiv_rn(h, 2.f)), __fsub_rn(xc, __fdiv_rn(w, 2.f)),
-                                __fadd_rn(yc, __fdiv_rn(h, 2.f)), __fadd_rn(xc, __fdiv_rn(w, 2.f)));
-    p.cand_score[j] = score;
-    p.cand_cls[j] = cls + 1;
-    p.cand_lvl[j] = l + p.min_level;
+    cand_box[j] = make_float4(__fsub_rn(yc, __fdiv_rn(h, 2.f)), __fsub_rn(xc, __fdiv_rn(w, 2.f)),
+                              __fadd_rn(yc, __fdiv_rn(h, 2.f)), __fadd_rn(xc, __fdiv_rn(w, 2.f)));
+    cand_score[j] = score;
+    cand_cls[j] = cls + 1;
+    cand_lvl[j] = l + p.min_level;
   }
-  if (tid == 0) p.state[5] = static_cast<uint32_t>(K);
+  if (tid == 0) state[5] = static_cast<uint32_t>(K);
 }
 
-// 64x64 tiles of the suppression bit matrix: mask[i][w] bit j = IoU(i, 64w + j) > thr, only j > i
-__global__ void nms_mask_kernel(const float4* __restrict__ boxes, const uint32_t* __restrict__ state, float thr,
+// 64x64 tiles of the suppression bit matrix: mask[i][w] bit j = IoU(i, 64w + j) > thr, only j > i; image blockIdx.z
+// (boxes [B][k], state [B][8], mask [B][k][words])
+__global__ void nms_mask_kernel(const float4* __restrict__ boxes, const uint32_t* __restrict__ state, float thr, int k,
                                 int words, unsigned long long* __restrict__ mask) {
+  boxes += static_cast<size_t>(blockIdx.z) * k;
+  state += 8 * blockIdx.z;
+  mask += static_cast<size_t>(blockIdx.z) * k * words;
   const int n = static_cast<int>(state[5]);
   const int row0 = blockIdx.y * 64, col0 = blockIdx.x * 64;
   if (row0 >= n || col0 >= n || col0 + 63 < row0) return;
@@ -261,18 +293,28 @@ __global__ void nms_mask_kernel(const float4* __restrict__ boxes, const uint32_t
   }
 }
 
-// one warp: greedy scan in score order (non_max_suppression_with_scores, hard NMS, score threshold), stops at
+// one warp per image: greedy scan in score order (non_max_suppression_with_scores, hard NMS, score threshold), stops at
 // max_out.  Lane l owns removed-words l, l+32, l+64, l+96 (k <= 8192).
 __global__ void __launch_bounds__(32, 1) nms_scan_kernel(const __grid_constant__ EffdetPostParams p, int words,
                                                         const float* __restrict__ scale_ptr) {
-  const int lane = threadIdx.x;
-  const float scale = __ldg(scale_ptr);
-  const int n = static_cast<int>(p.state[5]);
+  const int lane = threadIdx.x, img = blockIdx.y;
+  const float scale = __ldg(scale_ptr + img);
+  const size_t ks = kslice(p, img), os = static_cast<size_t>(img) * p.max_out;
+  const float4* cand_box = p.cand_box + ks;
+  const float* cand_score = p.cand_score + ks;
+  const int* cand_cls = p.cand_cls + ks;
+  const int* cand_lvl = p.cand_lvl + ks;
+  const unsigned long long* mask = p.mask + ks * words;
+  float4* out_boxes = p.out_boxes + os;
+  float* out_scores = p.out_scores + os;
+  int* out_classes = p.out_classes + os;
+  int* out_levels = p.out_levels + os;
+  const int n = static_cast<int>(state_of(p, img)[5]);
   unsigned long long rem[4] = {0ull, 0ull, 0ull, 0ull};
   int kept = 0;
   bool done = false;
   for (int base = 0; base < n && !done; base += 32) {
-    const float sc = base + lane < n ? p.cand_score[base + lane] : -1.f;
+    const float sc = base + lane < n ? cand_score[base + lane] : -1.f;
     for (int t = 0; t < 32; ++t) {
       const int i = base + t;
       if (i >= n || kept >= p.max_out) { done = true; break; }
@@ -285,31 +327,29 @@ __global__ void __launch_bounds__(32, 1) nms_scan_kernel(const __grid_constant__
 #pragma unroll
       for (int qq = 0; qq < 4; ++qq) {
         const int ww = lane + 32 * qq;
-        if (ww >= w && ww < words) rem[qq] |= p.mask[static_cast<size_t>(i) * words + ww];
+        if (ww >= w && ww < words) rem[qq] |= mask[static_cast<size_t>(i) * words + ww];
       }
       if (lane == 0) {
-        const float4 b = p.cand_box[i];                 // (ymin, xmin, ymax, xmax) * scale -> x1 y1 x2 y2
-        p.out_boxes[kept] = make_float4(__fmul_rn(b.y, scale), __fmul_rn(b.x, scale), __fmul_rn(b.w, scale),
-                                        __fmul_rn(b.z, scale));
-        p.out_scores[kept] = s;
-        p.out_classes[kept] = p.cand_cls[i];
-        p.out_levels[kept] = p.cand_lvl[i];
+        const float4 b = cand_box[i];                 // (ymin, xmin, ymax, xmax) * scale -> x1 y1 x2 y2
+        out_boxes[kept] = make_float4(__fmul_rn(b.y, scale), __fmul_rn(b.x, scale), __fmul_rn(b.w, scale),
+                                      __fmul_rn(b.z, scale));
+        out_scores[kept] = s;
+        out_classes[kept] = cand_cls[i];
+        out_levels[kept] = cand_lvl[i];
       }
       ++kept;
     }
   }
   for (int j = kept + lane; j < p.max_out; j += 32) {
-    p.out_boxes[j] = make_float4(0.f, 0.f, 0.f, 0.f);
-    p.out_scores[j] = 0.f;
-    p.out_classes[j] = 0;
-    p.out_levels[j] = p.min_level;
+    out_boxes[j] = make_float4(0.f, 0.f, 0.f, 0.f);
+    out_scores[j] = 0.f;
+    out_classes[j] = 0;
+    out_levels[j] = p.min_level;
   }
-  if (lane == 0) p.out_count[0] = kept;
+  if (lane == 0) p.out_count[img] = kept;
 }
 
-__global__ void topk_seed_kernel(uint32_t* state, uint32_t need) { state[2] = need; }
-
-constexpr unsigned kTopkMaxBlocks = 132 * 8;
+__global__ void topk_seed_kernel(uint32_t* state, uint32_t need) { state[8 * blockIdx.x + 2] = need; }
 
 int next_pow2(int v) {
   int p = 1;
@@ -356,37 +396,39 @@ int bifpn_combine_launch(const BifpnCombineParams& p, cudaStream_t s) {
 
 int dw3x3_plain_launch(const __half* in_hi, const __half* in_lo, int B, int H, int W, int C, const float* w, __half* out_hi,
                        __half* out_lo, cudaStream_t s) {
-  B2_CHECK(B == 1, "dw3x3_plain: batch 1 only");
-  DwConvParams p{in_hi, in_lo, H, W, C, 3, 1, 1, 1, H, W, w, nullptr, out_hi, out_lo};
+  DwConvParams p{in_hi, in_lo, B, H, W, C, 3, 1, 1, 1, H, W, w, nullptr, out_hi, out_lo};
   return dwconv_launch(p, 0, s);
 }
 
 int effdet_topk_blocks() { return static_cast<int>(kTopkMaxBlocks); }
 
-// top-k -> candidates -> sigmoid/decode -> class-agnostic NMS -> outputs; all on the stream, no host sync
+// top-k -> candidates -> sigmoid/decode -> class-agnostic NMS -> outputs for p.B images, each kernel once with the image
+// as a grid dimension; all on the stream, no host sync
 int effdet_post_launch(const EffdetPostParams& p, const float* image_scale_dev, cudaStream_t s) {
   B2_CHECK(p.k >= 1 && p.k <= 8192, "effdet post: max_detection_topk must be in [1, 8192]");
   B2_CHECK(p.total < (1ull << 32), "effdet post: more than 2^32 class logits");
   B2_CHECK(p.anchors <= 9 && p.n_levels <= 5, "effdet post: at most 9 anchors per cell and 5 levels");
-  B2_CUDA(cudaMemsetAsync(p.hist, 0, 256 * sizeof(unsigned int), s));
-  B2_CUDA(cudaMemsetAsync(p.state, 0, 8 * sizeof(uint32_t), s));
+  B2_CHECK(p.B >= 1 && p.B <= 1024, "effdet post: batch out of range");
+  const unsigned B = static_cast<unsigned>(p.B);
+  B2_CUDA(cudaMemsetAsync(p.hist, 0, B * 256 * sizeof(unsigned int), s));
+  B2_CUDA(cudaMemsetAsync(p.state, 0, B * 8 * sizeof(uint32_t), s));
   const uint32_t need = static_cast<uint32_t>(static_cast<unsigned long long>(p.k) < p.total ? p.k : p.total);
-  topk_seed_kernel<<<1, 1, 0, s>>>(p.state, need);
+  topk_seed_kernel<<<B, 1, 0, s>>>(p.state, need);
   const unsigned grid = grid_for(p.total, 256, kTopkMaxBlocks);
   for (int pass = 0; pass < 4; ++pass) {
-    topk_hist_kernel<<<grid, 256, 0, s>>>(p, pass);
-    topk_pick_kernel<<<1, 256, 0, s>>>(p, pass);
+    topk_hist_kernel<<<dim3(grid, B), 256, 0, s>>>(p, pass);
+    topk_pick_kernel<<<dim3(1, B), 256, 0, s>>>(p, pass);
   }
   const unsigned long long chunk = (p.total + grid - 1) / grid;
-  topk_collect_kernel<<<grid, 256, 0, s>>>(p, chunk);
-  topk_tie_scan_kernel<<<1, 32, 0, s>>>(p, static_cast<int>(grid));
-  topk_tie_write_kernel<<<grid, 256, 0, s>>>(p, chunk);
+  topk_collect_kernel<<<dim3(grid, B), 256, 0, s>>>(p, chunk);
+  topk_tie_scan_kernel<<<dim3(1, B), 32, 0, s>>>(p, static_cast<int>(grid));
+  topk_tie_write_kernel<<<dim3(grid, B), 256, 0, s>>>(p, chunk);
   const int KP = next_pow2(p.k);
   B2_CUDA(cudaFuncSetAttribute(det_prepare_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
-  det_prepare_kernel<<<1, 1024, static_cast<size_t>(KP) * 8, s>>>(p, KP);
+  det_prepare_kernel<<<dim3(1, B), 1024, static_cast<size_t>(KP) * 8, s>>>(p, KP);
   const int words = (p.k + 63) / 64;
-  nms_mask_kernel<<<dim3(words, words), 64, 0, s>>>(p.cand_box, p.state, p.nms_thr, words, p.mask);
-  nms_scan_kernel<<<1, 32, 0, s>>>(p, words, image_scale_dev);
+  nms_mask_kernel<<<dim3(words, words, B), 64, 0, s>>>(p.cand_box, p.state, p.nms_thr, p.k, words, p.mask);
+  nms_scan_kernel<<<dim3(1, B), 32, 0, s>>>(p, words, image_scale_dev);
   B2_CUDA(cudaGetLastError());
   return 0;
 }

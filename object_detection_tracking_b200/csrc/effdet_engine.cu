@@ -1,6 +1,10 @@
 // EfficientDet feature network (BiFPN), class/box nets and post-processing behind the C ABI.
-// One b2_effdet = one device = one fixed network input size; the pass is a fixed launch sequence replayed as a
-// CUDA graph.  Batch is 1 like the reference wrapper (efficientdet_wrapper.py:304-363 runs one frame per call).
+// One b2_effdet = one device = one fixed network input size and batch; the pass is a fixed launch sequence replayed as a
+// CUDA graph.  The reference wrapper runs one frame per call (efficientdet_wrapper.py:304-363); a context created with
+// batch B runs B independent frames per call, each with the batch-1 semantics and bit-identical to a batch-1 context:
+// every kernel takes the image from its grid or its row index, the squeeze-excite gate is folded into one copy of the
+// projection weights per image and each image's projection is its own conv layer, and the post-processing keeps one
+// slice of scratch and outputs per image.
 //
 // Reference graph: efficientdet_arch.py build_feature_network (:440-505) / build_bifpn_layer (:594-682) /
 // resample_feature_map (:105-200) / class_net (:227-282) / box_net (:285-340), then
@@ -48,13 +52,14 @@ struct EDwBn {
   int creal = 0;
 };
 
-// backbone: squeeze-excite whose gate is folded into the projection conv's weights every frame
+// backbone: squeeze-excite whose gate is folded into the projection conv's weights every frame, one copy per image
 struct ESe {
   std::string pre;          // ".../blocks_i/se"
   Planes x;
   int creal = 0, nr = 0;
   float *partial = nullptr, *r_part = nullptr, *gate = nullptr, *w1 = nullptr, *b1 = nullptr, *w2 = nullptr, *b2 = nullptr;
-  const ConvLayer* proj = nullptr;   // its w_master holds the BN-folded projection weights [Cout_pad][K] fp32
+  const ConvLayer* proj = nullptr;   // image 0's projection: its w_master holds the BN-folded weights [Cout_pad][K] fp32
+  __half *fold_hi = nullptr, *fold_lo = nullptr;   // [B][Cout_pad][K]: image b's projection layer reads slice b
 };
 
 // Step phases (bit i of b2_effdet_run_phases' mask = phase i): the backbone runs only in b2_effdet_detect's graph; the
@@ -95,9 +100,11 @@ struct b2_effdet {
   std::vector<Step> steps;           // backbone (when cfg.backbone >= 0), feature network, heads, post-processing
   int phase = kFeatures;             // phase of the steps being added
   std::string bb_name;
-  float* image = nullptr;            // [H][W][3] fp32, pre-processed network input
-  uint8_t* frame = nullptr;          // device copy of the caller's BGR frame
+  int B = 1;                         // images per call
+  float* image = nullptr;            // [B][H][W][3] fp32, pre-processed network input
+  uint8_t* frame = nullptr;          // device copy of the caller's BGR frames, back to back (grow-only)
   size_t frame_cap = 0;
+  EffnetFrame* frame_table = nullptr;   // [B] where each image's frame lies in `frame`, and its sizes
   Planes stem_cols;
   cudaGraphExec_t graph_full = nullptr;
   StageMap named;
@@ -105,15 +112,15 @@ struct b2_effdet {
   Planes fpn_out[5];
   EffdetPostParams post;
   LevelRoiFeatParams roi;
-  float* scale_dev = nullptr;
-  float4* out_boxes = nullptr;
+  float* scale_dev = nullptr;        // [B] image_scale of each image
+  float4* out_boxes = nullptr;       // outputs [B][max_out] (out_count [B], out_feat [B][max_out][F])
   float* out_scores = nullptr;
   int *out_classes = nullptr, *out_levels = nullptr, *out_count = nullptr;
   float* out_feat = nullptr;
   cudaGraphExec_t graph = nullptr;
   bool loaded = false;
 
-  Planes planes(int h, int w, int c, int creal) { return arena.planes(1, h, w, c, split, creal); }
+  Planes planes(int h, int w, int c, int creal) { return arena.planes(B, h, w, c, split, creal); }
   double esz() const { return split ? 4.0 : 2.0; }
 };
 
@@ -135,7 +142,7 @@ ConvLayer* add_pw(b2_effdet* c, const std::string& wname, const std::string& bia
   ConvLayer* raw = L.get();
   c->convs.push_back(std::move(L));
   const ConvDesc& e = raw->d;
-  const double M = static_cast<double>(e.in_H) * e.in_W, esz = c->esz();
+  const double M = static_cast<double>(e.B) * e.in_H * e.in_W, esz = c->esz();
   Step& s = add_conv_step(c->steps, c->phase, raw);
   s.name = wname + " [" + std::to_string(e.in_H) + "x" + std::to_string(e.in_W) + "x" + std::to_string(raw->cin_real) +
            "->" + std::to_string(cout_real) + "]";
@@ -157,8 +164,8 @@ void add_dw(b2_effdet* c, const std::string& wname, const Planes& in, const Plan
   }
   const EDw* e = D.get();
   add_step(c->steps, c->phase, 1, wname, [e](cudaStream_t st) {
-    return dw3x3_plain_launch(e->in.hi, e->in.lo, 1, e->in.H, e->in.W, e->in.C, e->w, e->out.hi, e->out.lo, st);
-  }, 2.0 * static_cast<double>(in.elems()) * c->esz(), 18.0 * static_cast<double>(in.H) * in.W * in.creal);
+    return dw3x3_plain_launch(e->in.hi, e->in.lo, e->in.B, e->in.H, e->in.W, e->in.C, e->w, e->out.hi, e->out.lo, st);
+  }, 2.0 * static_cast<double>(in.elems()) * c->esz(), 18.0 * static_cast<double>(in.B) * in.H * in.W * in.creal);
   c->dws.push_back(std::move(D));
 }
 
@@ -170,7 +177,7 @@ void add_combine(b2_effdet* c, std::unique_ptr<ECombine> K) {
   add_step(c->steps, c->phase, 2,
            "combine x" + std::to_string(p.n_in) + " [" + std::to_string(p.Ho) + "x" + std::to_string(p.Wo) + "]",
            [k](cudaStream_t st) { return bifpn_combine_launch(k->p, st); },
-           (in + static_cast<double>(p.Ho) * p.Wo * p.C) * c->esz());
+           p.B * (in + static_cast<double>(p.Ho) * p.Wo * p.C) * c->esz());
   c->combines.push_back(std::move(K));
 }
 
@@ -190,7 +197,7 @@ int add_pool(b2_effdet* c, const Planes& src, const Planes& dst) {
   std::unique_ptr<ECombine> K(new ECombine());
   memset(&K->p, 0, sizeof(K->p));
   if (set_input(K->p.in[0], src, dst.H, dst.W)) return -1;
-  K->p.n_in = 1; K->p.B = 1; K->p.Ho = dst.H; K->p.Wo = dst.W; K->p.C = dst.C;
+  K->p.n_in = 1; K->p.B = c->B; K->p.Ho = dst.H; K->p.Wo = dst.W; K->p.C = dst.C;
   K->p.weighted = 0; K->p.denom = 1.f; K->p.swish = 0;
   K->p.out_hi = dst.hi; K->p.out_lo = dst.lo;
   add_combine(c, std::move(K));
@@ -232,8 +239,9 @@ int build_backbone(b2_effdet* c) {
   }
   c->phase = kBackbone;
   const int H = g.image_h, W = g.image_w;
-  c->image = c->arena.alloc<float>(static_cast<size_t>(H) * W * 3);
-  c->named.raw("image", c->image, Stage::kF32, 1, H, W, 3);
+  c->image = c->arena.alloc<float>(static_cast<size_t>(c->B) * H * W * 3);
+  c->frame_table = c->arena.alloc<EffnetFrame>(c->B);
+  c->named.raw("image", c->image, Stage::kF32, c->B, H, W, 3);
   // stem: 3x3/2 SAME as a 1x1 conv over im2col-packed pixels (27 live of 64 operand channels)
   int h = 0, w = 0, pt = 0, pl = 0;
   same_pad(H, 3, 2, &h, &pt);
@@ -241,8 +249,8 @@ int build_backbone(b2_effdet* c) {
   c->stem_cols = c->planes(h, w, 64, 27);
   const Planes cols = c->stem_cols;
   add_step(c->steps, c->phase, 5, "stem_im2col", [c, cols, pt, pl](cudaStream_t st) {
-    return stem_im2col_launch(c->image, c->cfg.image_h, c->cfg.image_w, cols.H, cols.W, pt, pl, cols.hi, cols.lo, st);
-  }, static_cast<double>(H) * W * 3 * 4 + static_cast<double>(cols.elems()) * c->esz());
+    return stem_im2col_launch(c->image, cols.B, c->cfg.image_h, c->cfg.image_w, cols.H, cols.W, pt, pl, cols.hi, cols.lo, st);
+  }, static_cast<double>(c->B) * H * W * 3 * 4 + static_cast<double>(cols.elems()) * c->esz());
   const int stem_c = round_filters(32, width);
   Planes x = c->planes(h, w, pad64(stem_c), stem_c);
   add_pw(c, c->bb_name + "/stem/conv2d/kernel", "", c->bb_name + "/stem/tpu_batch_normalization", c->stem_cols, x, stem_c, 2);
@@ -268,39 +276,58 @@ int build_backbone(b2_effdet* c) {
     D->wname = pre + "/depthwise_conv2d/depthwise_kernel"; D->bnname = pre + "/tpu_batch_normalization_1"; D->creal = mid;
     D->w = c->arena.alloc<float>(static_cast<size_t>(b.kernel) * b.kernel * e.C);
     D->bias = c->arena.alloc<float>(e.C);
-    D->p = DwConvParams{e.hi, e.lo, e.H, e.W, e.C, b.kernel, b.stride, dpt, dpl, ho, wo, D->w, D->bias, d.hi, d.lo};
+    D->p = DwConvParams{e.hi, e.lo, c->B, e.H, e.W, e.C, b.kernel, b.stride, dpt, dpl, ho, wo, D->w, D->bias, d.hi, d.lo};
     const DwConvParams& dp = D->p;
     add_step(c->steps, c->phase, 3,
              D->wname + " [" + std::to_string(dp.H) + "x" + std::to_string(dp.W) + "x" + std::to_string(mid) + " k" +
                  std::to_string(dp.K) + "/" + std::to_string(dp.stride) + "]",
              [dp](cudaStream_t st) { return dwconv_bn_swish_launch(dp, st); },
-             (static_cast<double>(dp.H) * dp.W + static_cast<double>(dp.Ho) * dp.Wo) * dp.C * c->esz(),
-             2.0 * dp.K * dp.K * static_cast<double>(dp.Ho) * dp.Wo * mid);
+             dp.B * (static_cast<double>(dp.H) * dp.W + static_cast<double>(dp.Ho) * dp.Wo) * dp.C * c->esz(),
+             2.0 * dp.K * dp.K * dp.B * static_cast<double>(dp.Ho) * dp.Wo * mid);
     c->dwbns.push_back(std::move(D));
     // squeeze-excite (se_ratio 0.25 of the block's input filters)
     std::unique_ptr<ESe> S(new ESe());
     S->pre = pre + "/se"; S->x = d; S->creal = mid; S->nr = b.cin / 4 > 1 ? b.cin / 4 : 1;
-    S->partial = c->arena.alloc<float>(static_cast<size_t>(se_chunks(ho * wo)) * d.C);
-    S->gate = c->arena.alloc<float>(d.C);
-    S->r_part = c->arena.alloc<float>(static_cast<size_t>(se_fc1_parts()) * se_max_nr());
+    S->partial = c->arena.alloc<float>(static_cast<size_t>(c->B) * se_chunks(ho * wo) * d.C);
+    S->gate = c->arena.alloc<float>(static_cast<size_t>(c->B) * d.C);
+    S->r_part = c->arena.alloc<float>(static_cast<size_t>(c->B) * se_fc1_parts() * se_max_nr());
     S->w1 = c->arena.alloc<float>(static_cast<size_t>(mid) * S->nr); S->b1 = c->arena.alloc<float>(S->nr);
     S->w2 = c->arena.alloc<float>(static_cast<size_t>(S->nr) * mid); S->b2 = c->arena.alloc<float>(mid);
     const ESe* se = S.get();
     add_step(c->steps, c->phase, 4, S->pre, [se](cudaStream_t st) {   // pool + fc1 + fc2 / gate / weight rescale
       const ConvLayer* P = se->proj;
-      return se_gate_launch(se->x.hi, se->x.lo, se->x.H * se->x.W, se->x.C, se->creal, se->nr, se->partial, se->r_part,
-                            se->w1, se->b1, se->w2, se->b2, se->gate, P->w_master, P->w.Cout_pad, P->w.w_hi, P->w.w_lo, st);
+      return se_gate_launch(se->x.hi, se->x.lo, se->x.B, se->x.H * se->x.W, se->x.C, se->creal, se->nr, se->partial,
+                            se->r_part, se->w1, se->b1, se->w2, se->b2, se->gate, P->w_master, P->w.Cout_pad, se->fold_hi,
+                            se->fold_lo, st);
     }, 0.0, 0.0, 3);
     const size_t se_idx = c->steps.size() - 1;
     c->ses.push_back(std::move(S));
-    // projection (+ identity skip when the block keeps shape, efficientnet_model.py:381-390)
+    // projection (+ identity skip when the block keeps shape, efficientnet_model.py:381-390): one layer per image, on its
+    // slice of the depthwise output and skip, with its image's folded weights
     Planes y = c->planes(ho, wo, pad64(b.cout), b.cout);
     const bool skip = b.stride == 1 && b.cin == b.cout;
-    ConvLayer* P = add_pw(c, pre + "/" + proj + "/kernel", "", pre + "/tpu_batch_normalization_2", d, y, b.cout, 0,
-                          skip ? &x : nullptr);
-    P->w_master = c->arena.alloc<float>(static_cast<size_t>(P->w.Cout_pad) * P->w.K);
-    c->ses.back()->proj = P;
-    c->steps[se_idx].bytes = static_cast<double>(d.elems()) * c->esz() + 2.0 * P->w.Cout_pad * P->w.K * 4.0;
+    std::vector<ConvLayer*> P(c->B);
+    for (int im = 0; im < c->B; ++im) {
+      const Planes xi = x.images(im, 1);
+      P[im] = add_pw(c, pre + "/" + proj + "/kernel", "", pre + "/tpu_batch_normalization_2", d.images(im, 1),
+                     y.images(im, 1), b.cout, 0, skip ? &xi : nullptr);
+      if (c->B > 1) c->steps.back().name += " image " + std::to_string(im);
+    }
+    const size_t wsz = static_cast<size_t>(P[0]->w.Cout_pad) * P[0]->w.K;
+    P[0]->w_master = c->arena.alloc<float>(wsz);
+    ESe& se_b = *c->ses.back();
+    se_b.proj = P[0];
+    if (c->B == 1) {
+      se_b.fold_hi = P[0]->w.w_hi; se_b.fold_lo = P[0]->w.w_lo;
+    } else {
+      se_b.fold_hi = c->arena.alloc<__half>(c->B * wsz);
+      se_b.fold_lo = c->split ? c->arena.alloc<__half>(c->B * wsz) : nullptr;
+      for (int im = 0; im < c->B; ++im) {
+        P[im]->w.w_hi = se_b.fold_hi ? se_b.fold_hi + im * wsz : nullptr;
+        P[im]->w.w_lo = se_b.fold_lo ? se_b.fold_lo + im * wsz : nullptr;
+      }
+    }
+    c->steps[se_idx].bytes = static_cast<double>(d.elems()) * c->esz() + (1.0 + c->B) * wsz * 4.0;
     x = y;
     c->named.planes("block_" + std::to_string(i), x);
     if (i + 1 == blocks.size() || blocks[i + 1].stride > 1) {
@@ -364,7 +391,7 @@ int build(b2_effdet* c) {
         K->wnames[idx] = pre + "/WSM" + (idx == 0 ? std::string() : "_" + std::to_string(idx));
       }
       Planes comb = c->planes(th, tw, c->Fp, c->F);
-      K->p.n_in = n; K->p.B = 1; K->p.Ho = th; K->p.Wo = tw; K->p.C = c->Fp;
+      K->p.n_in = n; K->p.B = c->B; K->p.Ho = th; K->p.Wo = tw; K->p.C = c->Fp;
       K->p.weighted = g.fpn_weight_method == 1; K->p.denom = 1.f; K->p.swish = 1;
       K->p.out_hi = comb.hi; K->p.out_lo = comb.lo;
       add_combine(c, std::move(K));
@@ -406,11 +433,12 @@ int build(b2_effdet* c) {
       const std::string nm = kn + "_net/" + kn + "-predict";
       add_dw(c, nm + "/depthwise_kernel", x, t);
       const int creal = kind == 0 ? ncls : nbox, ld = pad16(creal);
-      float* o = c->arena.alloc<float>(static_cast<size_t>(h) * w * ld);
+      float* o = c->arena.alloc<float>(static_cast<size_t>(c->B) * h * w * ld);
       add_pw(c, nm + "/pointwise_kernel", nm + "/bias", "", t, Planes(), creal, 0, nullptr, o, ld);
       (kind == 0 ? p.logits[l] : p.boxes[l]) = o;
       (kind == 0 ? p.ld[l] : p.ldb[l]) = ld;
-      c->named.raw((kind == 0 ? "cls" : "box") + std::to_string(level), o, Stage::kF32, 1, h, w, ld);
+      (kind == 0 ? p.logit_bstride[l] : p.box_bstride[l]) = static_cast<unsigned long long>(h) * w * ld;
+      c->named.raw((kind == 0 ? "cls" : "box") + std::to_string(level), o, Stage::kF32, c->B, h, w, ld);
     }
   }
   // post-processing state
@@ -438,24 +466,27 @@ int build(b2_effdet* c) {
   p.k = g.max_detection_topk; p.max_out = g.result_per_im;
   B2_CHECK(p.k >= 1 && p.k <= 8192, "effdet: max_detection_topk must be in [1, 8192]");
   p.score_thresh = g.result_score_thres; p.nms_thr = g.nms_iou_threshold;
-  p.hist = c->arena.alloc<unsigned int>(256);
-  p.state = c->arena.alloc<uint32_t>(8);
-  p.cand = c->arena.alloc<unsigned long long>(p.k);
-  p.ties = c->arena.alloc<unsigned long long>(p.k);
-  p.tie_cnt = c->arena.alloc<unsigned int>(effdet_topk_blocks());
-  p.tie_off = c->arena.alloc<unsigned int>(effdet_topk_blocks());
-  p.cand_box = c->arena.alloc<float4>(p.k);
-  p.cand_score = c->arena.alloc<float>(p.k);
-  p.cand_cls = c->arena.alloc<int>(p.k);
-  p.cand_lvl = c->arena.alloc<int>(p.k);
-  p.mask = c->arena.alloc<unsigned long long>(static_cast<size_t>(p.k) * ((p.k + 63) / 64));
-  c->out_boxes = c->arena.alloc<float4>(p.max_out);
-  c->out_scores = c->arena.alloc<float>(p.max_out);
-  c->out_classes = c->arena.alloc<int>(p.max_out);
-  c->out_levels = c->arena.alloc<int>(p.max_out);
-  c->out_count = c->arena.alloc<int>(1);
-  c->out_feat = c->arena.alloc<float>(static_cast<size_t>(p.max_out) * c->F);
-  c->scale_dev = c->arena.alloc<float>(1);
+  // one slice per image of the scratch and the outputs
+  const size_t B = static_cast<size_t>(c->B), kb = B * p.k, mb = B * p.max_out;
+  p.B = c->B;
+  p.hist = c->arena.alloc<unsigned int>(B * 256);
+  p.state = c->arena.alloc<uint32_t>(B * 8);
+  p.cand = c->arena.alloc<unsigned long long>(kb);
+  p.ties = c->arena.alloc<unsigned long long>(kb);
+  p.tie_cnt = c->arena.alloc<unsigned int>(B * effdet_topk_blocks());
+  p.tie_off = c->arena.alloc<unsigned int>(B * effdet_topk_blocks());
+  p.cand_box = c->arena.alloc<float4>(kb);
+  p.cand_score = c->arena.alloc<float>(kb);
+  p.cand_cls = c->arena.alloc<int>(kb);
+  p.cand_lvl = c->arena.alloc<int>(kb);
+  p.mask = c->arena.alloc<unsigned long long>(kb * ((p.k + 63) / 64));
+  c->out_boxes = c->arena.alloc<float4>(mb);
+  c->out_scores = c->arena.alloc<float>(mb);
+  c->out_classes = c->arena.alloc<int>(mb);
+  c->out_levels = c->arena.alloc<int>(mb);
+  c->out_count = c->arena.alloc<int>(B);
+  c->out_feat = c->arena.alloc<float>(mb * c->F);
+  c->scale_dev = c->arena.alloc<float>(B);
   p.out_boxes = c->out_boxes; p.out_scores = c->out_scores; p.out_classes = c->out_classes;
   p.out_levels = c->out_levels; p.out_count = c->out_count;
   LevelRoiFeatParams& r = c->roi;
@@ -465,48 +496,104 @@ int build(b2_effdet* c) {
     r.H[l] = c->fpn_out[l].H; r.W[l] = c->fpn_out[l].W;
     r.inv_stride[l] = 1.0f / static_cast<float>(1 << (l + 3));
   }
-  r.C = c->Fp; r.Creal = c->F; r.min_level = 3; r.max_out = p.max_out;
+  r.B = c->B; r.C = c->Fp; r.Creal = c->F; r.min_level = 3; r.max_out = p.max_out;
   r.boxes = c->out_boxes; r.levels = c->out_levels; r.count = c->out_count; r.out = c->out_feat;
   // the candidates in top-k order (boxes ymin xmin ymax xmax in network pixels, count = state[5]), the outputs, and the
-  // device copy of image_scale the NMS step multiplies the boxes by
-  const int k = p.k, m = p.max_out;
-  c->named.raw("topk_boxes", p.cand_box, Stage::kF32, 1, 1, k, 4);
-  c->named.raw("topk_scores", p.cand_score, Stage::kF32, 1, 1, k, 1);
-  c->named.raw("topk_classes", p.cand_cls, Stage::kI32, 1, 1, k, 1);
-  c->named.raw("topk_levels", p.cand_lvl, Stage::kI32, 1, 1, k, 1);
-  c->named.raw("topk_count", p.state + 5, Stage::kI32, 1, 1, 1, 1);
-  c->named.raw("final_boxes", c->out_boxes, Stage::kF32, 1, 1, m, 4);
-  c->named.raw("final_scores", c->out_scores, Stage::kF32, 1, 1, m, 1);
-  c->named.raw("final_classes", c->out_classes, Stage::kI32, 1, 1, m, 1);
-  c->named.raw("final_levels", c->out_levels, Stage::kI32, 1, 1, m, 1);
-  c->named.raw("final_count", c->out_count, Stage::kI32, 1, 1, 1, 1);
-  c->named.raw("box_feat", c->out_feat, Stage::kF32, 1, 1, m, c->F);
-  c->named.raw("image_scale", c->scale_dev, Stage::kF32, 1, 1, 1, 1);
+  // device copy of image_scale the NMS step multiplies the boxes by; shape[0] = the batch
+  const int k = p.k, m = p.max_out, nb = c->B;
+  c->named.raw("topk_boxes", p.cand_box, Stage::kF32, nb, 1, k, 4);
+  c->named.raw("topk_scores", p.cand_score, Stage::kF32, nb, 1, k, 1);
+  c->named.raw("topk_classes", p.cand_cls, Stage::kI32, nb, 1, k, 1);
+  c->named.raw("topk_levels", p.cand_lvl, Stage::kI32, nb, 1, k, 1);
+  if (nb == 1) c->named.raw("topk_count", p.state + 5, Stage::kI32, 1, 1, 1, 1);
+  else c->named.raw("topk_count", p.state, Stage::kI32, nb, 1, 1, 8);   // [B][8]: the count is column 5
+  c->named.raw("final_boxes", c->out_boxes, Stage::kF32, nb, 1, m, 4);
+  c->named.raw("final_scores", c->out_scores, Stage::kF32, nb, 1, m, 1);
+  c->named.raw("final_classes", c->out_classes, Stage::kI32, nb, 1, m, 1);
+  c->named.raw("final_levels", c->out_levels, Stage::kI32, nb, 1, m, 1);
+  c->named.raw("final_count", c->out_count, Stage::kI32, nb, 1, 1, 1);
+  c->named.raw("box_feat", c->out_feat, Stage::kF32, nb, 1, m, c->F);
+  c->named.raw("image_scale", c->scale_dev, Stage::kF32, nb, 1, 1, 1);
   // 15 kernels (seed, 4 x (hist, pick), collect, tie scan, tie write, prepare, mask, scan), counted as the 14 that
-  // b2_effdet_num_launches has always reported for them
+  // b2_effdet_num_launches has always reported for them; every one covers all images
   add_step(c->steps, kPost, 6, "post", [c](cudaStream_t st) { return effdet_post_launch(c->post, c->scale_dev, st); },
-           static_cast<double>(p.total) * 4.0 * 6.0, 0.0, 14);
+           static_cast<double>(p.total) * 4.0 * 6.0 * c->B, 0.0, 14);
   add_step(c->steps, kBoxFeat, 7, "box_feat", [c](cudaStream_t st) { return level_roi_feat_launch(c->roi, st); }, 0.0);
+  B2_CHECK(c->arena.failed() == 0,
+           "b2_effdet_create: out of device memory: a batch-" + std::to_string(c->B) + " context needs " +
+               std::to_string(c->arena.requested()) + " bytes of device memory, and " + std::to_string(c->arena.failed()) +
+               " of them could not be allocated");
   return plan_convs(c->convs, c->split, c->num_sms);
 }
 
 
-int launch_and_fetch(b2_effdet* c, bool full, float image_scale, float* boxes, float* scores, int* classes, int* levels,
-                     float* box_feat, int* count) {
-  B2_CUDA(cudaMemcpyAsync(c->scale_dev, &image_scale, 4, cudaMemcpyHostToDevice, c->stream));
+// Runs the pass on the images as they stand (image_scale[B] of every image) and copies images [0, n) of the outputs.
+int launch_and_fetch(b2_effdet* c, bool full, const float* image_scale, int n, float* boxes, float* scores, int* classes,
+                     int* levels, float* box_feat, int* count) {
+  B2_CUDA(cudaMemcpyAsync(c->scale_dev, image_scale, sizeof(float) * c->B, cudaMemcpyHostToDevice, c->stream));
   cudaGraphExec_t& graph = full ? c->graph_full : c->graph;
   const unsigned mask = full ? ~0u : ~(1u << kBackbone);
   if (!graph && capture_graph(c->stream, [c, mask] { return run_steps(c->steps, mask, c->stream); }, &graph)) return -1;
   B2_CUDA(cudaGraphLaunch(graph, c->stream));
-  const int m = c->post.max_out;
+  const size_t m = static_cast<size_t>(n) * c->post.max_out;
   B2_CUDA(cudaMemcpyAsync(boxes, c->out_boxes, sizeof(float) * 4 * m, cudaMemcpyDeviceToHost, c->stream));
   B2_CUDA(cudaMemcpyAsync(scores, c->out_scores, sizeof(float) * m, cudaMemcpyDeviceToHost, c->stream));
   B2_CUDA(cudaMemcpyAsync(classes, c->out_classes, sizeof(int) * m, cudaMemcpyDeviceToHost, c->stream));
   if (levels) B2_CUDA(cudaMemcpyAsync(levels, c->out_levels, sizeof(int) * m, cudaMemcpyDeviceToHost, c->stream));
   if (box_feat) B2_CUDA(cudaMemcpyAsync(box_feat, c->out_feat, sizeof(float) * m * c->F, cudaMemcpyDeviceToHost, c->stream));
-  B2_CUDA(cudaMemcpyAsync(count, c->out_count, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
+  B2_CUDA(cudaMemcpyAsync(count, c->out_count, sizeof(int) * n, cudaMemcpyDeviceToHost, c->stream));
   B2_CUDA(cudaStreamSynchronize(c->stream));
   return 0;
+}
+
+// Uploads frames [0, n) back to back into the grow-only frame buffer, pre-processes them into images [0, n) and the last
+// frame again into images [n, B) (a short batch is padded as the reference's batch driver pads it, so one graph serves
+// every n), then runs the whole pass.  image_scale_out[i] = image_scale_to_original of frame i.
+int detect_frames(b2_effdet* c, const char* who, const uint8_t* const* frames, const int* h, const int* w, int n,
+                  float* boxes, float* scores, int* classes, int* levels, float* box_feat, int* count,
+                  float* image_scale_out) {
+  B2_CUDA(cudaSetDevice(c->device));
+  B2_CHECK(c->loaded, std::string(who) + ": weights not loaded");
+  B2_CHECK(c->cfg.backbone >= 0,
+           std::string(who) + ": the context was created without a backbone (use b2_effdet_run_features)");
+  std::vector<unsigned long long> off(n);
+  size_t bytes = 0;
+  for (int i = 0; i < n; ++i) {
+    B2_CHECK(frames[i], std::string(who) + ": null frame");
+    B2_CHECK(h[i] >= 1 && w[i] >= 1, std::string(who) + ": empty frame");
+    off[i] = bytes;
+    bytes += static_cast<size_t>(h[i]) * w[i] * 3;
+  }
+  if (bytes > c->frame_cap) {
+    if (c->frame) B2_CUDA(cudaFree(c->frame));
+    c->frame = nullptr; c->frame_cap = 0;
+    B2_CUDA(cudaMalloc(&c->frame, bytes));
+    c->frame_cap = bytes;
+  }
+  std::vector<EffnetFrame> table(c->B);
+  std::vector<float> scales(c->B);
+  for (int b = 0; b < c->B; ++b) {
+    const int i = b < n ? b : n - 1;
+    // set_scale_factors_to_output_size (dataloader.py:101-113), float32 like the TF graph
+    const float sy = static_cast<float>(c->cfg.image_h) / static_cast<float>(h[i]);
+    const float sx = static_cast<float>(c->cfg.image_w) / static_cast<float>(w[i]);
+    const float scale = sx < sy ? sx : sy;
+    int sh = static_cast<int>(static_cast<float>(h[i]) * scale), sw = static_cast<int>(static_cast<float>(w[i]) * scale);
+    if (sh > c->cfg.image_h) sh = c->cfg.image_h;
+    if (sw > c->cfg.image_w) sw = c->cfg.image_w;
+    B2_CHECK(sh >= 1 && sw >= 1, std::string(who) + ": frame " + std::to_string(i) + " resizes to an empty image");
+    table[b] = effnet_frame(off[i], h[i], w[i], sh, sw);
+    scales[b] = 1.0f / scale;
+  }
+  for (int i = 0; i < n; ++i) {
+    B2_CUDA(cudaMemcpyAsync(c->frame + off[i], frames[i], static_cast<size_t>(h[i]) * w[i] * 3, cudaMemcpyHostToDevice,
+                            c->stream));
+    if (image_scale_out) image_scale_out[i] = scales[i];
+  }
+  B2_CUDA(cudaMemcpyAsync(c->frame_table, table.data(), sizeof(EffnetFrame) * c->B, cudaMemcpyHostToDevice, c->stream));
+  if (effnet_preprocess_launch(c->frame, c->frame_table, c->B, c->image, c->cfg.image_h, c->cfg.image_w, c->stream))
+    return -1;
+  return launch_and_fetch(c, true, scales.data(), n, boxes, scores, classes, levels, box_feat, count);
 }
 
 }  // namespace
@@ -517,7 +604,9 @@ int b2_effdet_create(b2_effdet** out, const b2_effdet_config* cfg, int device) {
   B2_CHECK(out && cfg, "b2_effdet_create: null argument");
   *out = nullptr;
   std::unique_ptr<b2_effdet> c(new b2_effdet());
+  B2_CHECK(cfg->batch >= 0 && cfg->batch <= 1024, "b2_effdet_create: batch must be in [0, 1024] (0 means 1)");
   c->cfg = *cfg; c->device = device; c->split = cfg->precision == 1;
+  c->B = cfg->batch > 1 ? cfg->batch : 1;
   if (open_device(device, "b2_effdet_create", &c->num_sms, &c->stream)) return -1;
   if (build(c.get())) { b2_effdet_destroy(c.release()); return -1; }
   B2_CUDA(cudaDeviceSynchronize());
@@ -616,6 +705,8 @@ int b2_effdet_run_features(b2_effdet* c, const float* c3, const float* c4, const
   B2_CHECK(c && c3 && c4 && c5 && boxes && scores && classes && count, "b2_effdet_run_features: null argument");
   B2_CUDA(cudaSetDevice(c->device));
   B2_CHECK(c->loaded, "b2_effdet_run_features: weights not loaded");
+  B2_CHECK(c->B == 1, "b2_effdet_run_features: the context was created for a batch of " + std::to_string(c->B) +
+                          " images and this call takes one image's features; use a batch-1 context");
   const float* src[3] = {c3, c4, c5};
   for (int i = 0; i < 3; ++i) {
     const Planes& p = c->backbone[i];
@@ -624,7 +715,7 @@ int b2_effdet_run_features(b2_effdet* c, const float* c3, const float* c4, const
     for (size_t q = 0; q < px; ++q) memcpy(&padded[q * p.C], src[i] + q * p.creal, sizeof(float) * p.creal);
     if (upload_planes(padded.data(), p.hi, p.lo, padded.size(), c->stream)) return -1;
   }
-  return launch_and_fetch(c, false, image_scale, boxes, scores, classes, levels, box_feat, count);
+  return launch_and_fetch(c, false, &image_scale, 1, boxes, scores, classes, levels, box_feat, count);
 }
 
 // Full per-frame path of the reference wrapper (EfficientDet.build_preprocess + build_model): host BGR uint8 frame
@@ -634,28 +725,22 @@ int b2_effdet_detect(b2_effdet* c, const uint8_t* frame_bgr, int h, int w, float
                      int* levels, float* box_feat, int* count, float* image_scale_out) {
   B2_CHECK(c && frame_bgr && boxes && scores && classes && count, "b2_effdet_detect: null argument");
   B2_CHECK(h >= 1 && w >= 1, "b2_effdet_detect: empty frame");
-  B2_CUDA(cudaSetDevice(c->device));
-  B2_CHECK(c->loaded, "b2_effdet_detect: weights not loaded");
-  B2_CHECK(c->cfg.backbone >= 0, "b2_effdet_detect: the context was created without a backbone (use b2_effdet_run_features)");
-  const size_t bytes = static_cast<size_t>(h) * w * 3;
-  if (bytes > c->frame_cap) {
-    if (c->frame) B2_CUDA(cudaFree(c->frame));
-    c->frame = nullptr; c->frame_cap = 0;
-    B2_CUDA(cudaMalloc(&c->frame, bytes));
-    c->frame_cap = bytes;
-  }
-  // set_scale_factors_to_output_size (dataloader.py:101-113), float32 like the TF graph
-  const float sy = static_cast<float>(c->cfg.image_h) / static_cast<float>(h);
-  const float sx = static_cast<float>(c->cfg.image_w) / static_cast<float>(w);
-  const float scale = sx < sy ? sx : sy;
-  int sh = static_cast<int>(static_cast<float>(h) * scale), sw = static_cast<int>(static_cast<float>(w) * scale);
-  if (sh > c->cfg.image_h) sh = c->cfg.image_h;
-  if (sw > c->cfg.image_w) sw = c->cfg.image_w;
-  const float image_scale = 1.0f / scale;
-  if (image_scale_out) *image_scale_out = image_scale;
-  B2_CUDA(cudaMemcpyAsync(c->frame, frame_bgr, bytes, cudaMemcpyHostToDevice, c->stream));
-  if (effnet_preprocess_launch(c->frame, h, w, sh, sw, c->image, c->cfg.image_h, c->cfg.image_w, c->stream)) return -1;
-  return launch_and_fetch(c, true, image_scale, boxes, scores, classes, levels, box_feat, count);
+  B2_CHECK(c->B == 1, "b2_effdet_detect: the context was created for a batch of " + std::to_string(c->B) +
+                          " images; use b2_effdet_detect_batch");
+  return detect_frames(c, "b2_effdet_detect", &frame_bgr, &h, &w, 1, boxes, scores, classes, levels, box_feat, count,
+                       image_scale_out);
+}
+
+// The same for 1 <= n <= batch frames of any sizes in one pass: image i's outputs at row block i of boxes [batch][max][4],
+// scores / classes / levels [batch][max], box_feat [batch][max][F], counts [batch], image_scales [batch]; blocks i >= n
+// are not written.
+int b2_effdet_detect_batch(b2_effdet* c, const uint8_t* const* frames, const int* h, const int* w, int n, float* boxes,
+                           float* scores, int* classes, int* levels, float* box_feat, int* counts, float* image_scales) {
+  B2_CHECK(c && frames && h && w && boxes && scores && classes && counts, "b2_effdet_detect_batch: null argument");
+  B2_CHECK(n >= 1 && n <= c->B, "b2_effdet_detect_batch: n = " + std::to_string(n) + " frames, the context takes 1 to " +
+                                    std::to_string(c->B));
+  return detect_frames(c, "b2_effdet_detect_batch", frames, h, w, n, boxes, scores, classes, levels, box_feat, counts,
+                       image_scales);
 }
 
 // Stage-addressable tensors of the last pass as fp32 NHWC: "fpn3".."fpn7" (BiFPN outputs, channel-padded),
@@ -704,6 +789,31 @@ int b2_effdet_profile_steps(b2_effdet* c, int reps, float* ms_out, int cap, int*
 int b2_effdet_step_info(b2_effdet* c, int idx, char* name, int name_cap, double* flops, double* bytes, int* kind) {
   B2_CHECK(c, "b2_effdet_step_info: null argument");
   return step_info(c->steps, idx, name, name_cap, flops, bytes, kind);
+}
+
+// Replays the whole-frame graph that b2_effdet_detect / b2_effdet_detect_batch captured `reps` times on the images as
+// they stand, with no host copies; *ms_out = mean milliseconds per replay (CUDA events).
+int b2_effdet_replay(b2_effdet* c, int reps, float* ms_out) {
+  B2_CHECK(c && ms_out && reps >= 1, "b2_effdet_replay: bad argument");
+  B2_CUDA(cudaSetDevice(c->device));
+  B2_CHECK(c->graph_full, "b2_effdet_replay: no captured graph yet (run b2_effdet_detect or b2_effdet_detect_batch first)");
+  cudaEvent_t ev[2] = {nullptr, nullptr};
+  B2_CUDA(cudaEventCreate(&ev[0]));
+  if (cudaEventCreate(&ev[1]) != cudaSuccess) {
+    cudaEventDestroy(ev[0]);
+    B2_CHECK(false, "b2_effdet_replay: cudaEventCreate failed");
+  }
+  cudaError_t e = cudaEventRecord(ev[0], c->stream);
+  for (int r = 0; r < reps && e == cudaSuccess; ++r) e = cudaGraphLaunch(c->graph_full, c->stream);
+  if (e == cudaSuccess) e = cudaEventRecord(ev[1], c->stream);
+  if (e == cudaSuccess) e = cudaEventSynchronize(ev[1]);
+  float ms = 0.f;
+  if (e == cudaSuccess) e = cudaEventElapsedTime(&ms, ev[0], ev[1]);
+  cudaEventDestroy(ev[0]);
+  cudaEventDestroy(ev[1]);
+  B2_CUDA(e);
+  *ms_out = ms / reps;
+  return 0;
 }
 
 // Kernels of one b2_effdet_detect call (pre-processing + the whole pass); b2_effdet_run_features runs the steps after the

@@ -14,11 +14,17 @@ namespace {
 
 // uint8 BGR frame -> RGB, * 1/255, (x - mean) / std, legacy bilinear resize (align_corners=False, no half-pixel
 // centres) to (sh, sw), zero-padded bottom/right to [H, W, 3] fp32.  The reference normalises first and resizes the
-// float image; lerp of normalised corner values is done in the same order here.
-__global__ void effnet_preprocess_kernel(const uint8_t* __restrict__ img, int h, int w, int sh, int sw, float ys, float xs,
+// float image; lerp of normalised corner values is done in the same order here.  Image blockIdx.y reads its frame and
+// sizes from table[blockIdx.y] and writes out[blockIdx.y].
+__global__ void effnet_preprocess_kernel(const uint8_t* __restrict__ frames, const EffnetFrame* __restrict__ table,
                                          float* __restrict__ out, int H, int W) {
   const int idx = blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= H * W) return;
+  const EffnetFrame f = table[blockIdx.y];
+  const uint8_t* img = frames + f.src;
+  const int h = f.h, w = f.w, sh = f.sh, sw = f.sw;
+  const float ys = f.ys, xs = f.xs;
+  out += static_cast<size_t>(blockIdx.y) * H * W * 3;
   const int y = idx / W, x = idx - y * W;
   float r[3] = {0.f, 0.f, 0.f};
   if (y < sh && x < sw) {
@@ -45,14 +51,16 @@ __global__ void effnet_preprocess_kernel(const uint8_t* __restrict__ img, int h,
   o[0] = r[0]; o[1] = r[1]; o[2] = r[2];
 }
 
-// stem operand: 3x3/2 SAME patches of the fp32 image as one 64-channel pixel (k = (r*3 + s)*3 + c, 27 live)
-__global__ void stem_im2col_kernel(const float* __restrict__ img, int H, int W, int Ho, int Wo, int pad_t, int pad_l,
+// stem operand: 3x3/2 SAME patches of the fp32 images [B][H][W][3] as one 64-channel pixel (k = (r*3 + s)*3 + c, 27 live)
+__global__ void stem_im2col_kernel(const float* __restrict__ img, int B, int H, int W, int Ho, int Wo, int pad_t, int pad_l,
                                    __half* __restrict__ out_hi, __half* __restrict__ out_lo) {
-  const size_t idx = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x;   // (pixel, octet)
-  if (idx >= static_cast<size_t>(Ho) * Wo * 8) return;
+  const size_t idx = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x;   // (image, pixel, octet)
+  if (idx >= static_cast<size_t>(B) * Ho * Wo * 8) return;
   const int oct = static_cast<int>(idx & 7);
-  const size_t pix = idx >> 3;
-  const int y = static_cast<int>(pix / Wo), x = static_cast<int>(pix - static_cast<size_t>(y) * Wo);
+  const size_t pix = idx >> 3;                       // image-major: the output pixel of the [B][Ho][Wo] operand
+  const size_t b = pix / (static_cast<size_t>(Ho) * Wo), rem = pix - b * Ho * Wo;
+  img += b * H * W * 3;
+  const int y = static_cast<int>(rem / Wo), x = static_cast<int>(rem - static_cast<size_t>(y) * Wo);
   float v[8];
 #pragma unroll
   for (int j = 0; j < 8; ++j) {
@@ -77,12 +85,14 @@ __global__ void __launch_bounds__(128) dw_strip_kernel(const __grid_constant__ D
   constexpr int NC = (TX - 1) * S + K;
   const int cvec = p.C / 8;
   const int strips = (p.Wo + TX - 1) / TX;
-  const size_t total = static_cast<size_t>(p.Ho) * strips * cvec;
+  const size_t total = static_cast<size_t>(p.B) * p.Ho * strips * cvec;
   for (size_t idx = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; idx < total;
        idx += static_cast<size_t>(gridDim.x) * blockDim.x) {
     const int cv = static_cast<int>(idx % cvec);
     const size_t rest = idx / cvec;
-    const int sx = static_cast<int>(rest % strips), y = static_cast<int>(rest / strips);
+    const int sx = static_cast<int>(rest % strips), by = static_cast<int>(rest / strips);   // by = image * Ho + y
+    const int b = by / p.Ho, y = by - b * p.Ho;
+    const size_t in_img = static_cast<size_t>(b) * p.H;    // first input row of image b
     const int x0 = sx * TX;
     float acc[TX][8];
     {
@@ -109,7 +119,7 @@ __global__ void __launch_bounds__(128) dw_strip_kernel(const __grid_constant__ D
         const int ix = ix0 + i;
         const bool ok = oky && ix >= 0 && ix < p.W;
         const int cx = min(max(ix, 0), p.W - 1);
-        load8(p.in_hi, p.in_lo, (static_cast<size_t>(cy) * p.W + cx) * p.C + cv * 8, col[i]);
+        load8(p.in_hi, p.in_lo, ((in_img + cy) * p.W + cx) * p.C + cv * 8, col[i]);
         if (!ok) {
 #pragma unroll
           for (int j = 0; j < 8; ++j) col[i][j] = 0.f;
@@ -133,7 +143,7 @@ __global__ void __launch_bounds__(128) dw_strip_kernel(const __grid_constant__ D
 #pragma unroll
         for (int j = 0; j < 8; ++j) acc[t][j] = __fmul_rn(acc[t][j], 1.f / (1.f + expf(-acc[t][j])));
       }
-      store8(p.out_hi, p.out_lo, (static_cast<size_t>(y) * p.Wo + x0 + t) * p.C + cv * 8, acc[t]);
+      store8(p.out_hi, p.out_lo, (static_cast<size_t>(by) * p.Wo + x0 + t) * p.C + cv * 8, acc[t]);
     }
   }
 }
@@ -228,9 +238,9 @@ __global__ void __launch_bounds__(256) se_fc1_kernel(const float* __restrict__ p
 
 // excite, stage 2 + optional weight fold: each block owns 64 channels of one image: r = act(sum_b r_part + b1)
 // (recomputed per block, tiny; ACT = swish for MBConv, ReLU for the SE-ResNet bottleneck),
-// gate_c = sigmoid(b2[c] + sum_j r_j w2[j][c]) into gate_out [B][K]; then, when w is given (MBConv, batch 1),
-// w'[o][c] = w[o][c] * gate_c for every output row o of the projection conv, written as (hi, lo) operand planes.
-// grid (K/64, B)
+// gate_c = sigmoid(b2[c] + sum_j r_j w2[j][c]) into gate_out [B][K]; then, when w is given (MBConv),
+// w'[o][c] = w[o][c] * gate_c for every output row o of the projection conv, written as (hi, lo) operand planes: one
+// folded copy per image, [B][rows][K].  grid (K/64, B)
 enum class SeAct { kSwish, kRelu };
 
 template <SeAct ACT>
@@ -274,28 +284,37 @@ __global__ void __launch_bounds__(256) se_fc2_scale_kernel(const float* __restri
   }
   if (w == nullptr) return;   // gate only (uniform across the block)
   __syncthreads();
+  const size_t img = static_cast<size_t>(blockIdx.y) * rows * K;
   const int cc = threadIdx.x & 63;
   const float g = gate[cc];
   for (int o = threadIdx.x >> 6; o < rows; o += 4) {
     const size_t idx = static_cast<size_t>(o) * K + c0 + cc;
-    store1(hi, lo, idx, __fmul_rn(w[idx], g));
+    store1(hi, lo, img + idx, __fmul_rn(w[idx], g));
   }
 }
 
 }  // namespace
 
-int effnet_preprocess_launch(const uint8_t* img, int h, int w, int sh, int sw, float* out, int H, int W, cudaStream_t s) {
-  B2_CHECK(sh >= 1 && sw >= 1 && h >= 1 && w >= 1, "effnet preprocess: empty frame");
-  const float ys = static_cast<float>(h) / static_cast<float>(sh), xs = static_cast<float>(w) / static_cast<float>(sw);
-  effnet_preprocess_kernel<<<(H * W + 255) / 256, 256, 0, s>>>(img, h, w, sh, sw, ys, xs, out, H, W);
+EffnetFrame effnet_frame(unsigned long long src, int h, int w, int sh, int sw) {
+  EffnetFrame f;
+  f.src = src; f.h = h; f.w = w; f.sh = sh; f.sw = sw;
+  f.ys = static_cast<float>(h) / static_cast<float>(sh);
+  f.xs = static_cast<float>(w) / static_cast<float>(sw);
+  return f;
+}
+
+int effnet_preprocess_launch(const uint8_t* frames, const EffnetFrame* table, int B, float* out, int H, int W, cudaStream_t s) {
+  B2_CHECK(B >= 1 && B <= 65535, "effnet preprocess: batch out of range");
+  effnet_preprocess_kernel<<<dim3((H * W + 255) / 256, B), 256, 0, s>>>(frames, table, out, H, W);
   B2_CUDA(cudaGetLastError());
   return 0;
 }
 
-int stem_im2col_launch(const float* img, int H, int W, int Ho, int Wo, int pad_t, int pad_l, __half* out_hi, __half* out_lo,
-                       cudaStream_t s) {
-  const size_t total = static_cast<size_t>(Ho) * Wo * 8;
-  stem_im2col_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, s>>>(img, H, W, Ho, Wo, pad_t, pad_l, out_hi, out_lo);
+int stem_im2col_launch(const float* img, int B, int H, int W, int Ho, int Wo, int pad_t, int pad_l, __half* out_hi,
+                       __half* out_lo, cudaStream_t s) {
+  const size_t total = static_cast<size_t>(B) * Ho * Wo * 8;
+  stem_im2col_kernel<<<static_cast<unsigned>((total + 255) / 256), 256, 0, s>>>(img, B, H, W, Ho, Wo, pad_t, pad_l, out_hi,
+                                                                                 out_lo);
   B2_CUDA(cudaGetLastError());
   return 0;
 }
@@ -303,7 +322,7 @@ int stem_im2col_launch(const float* img, int H, int W, int Ho, int Wo, int pad_t
 template <int K, int S>
 int dw_strip_launch(const DwConvParams& p, bool act, cudaStream_t s) {
   constexpr int TX = S == 2 ? 2 : 4;
-  const size_t total = static_cast<size_t>(p.Ho) * ((p.Wo + TX - 1) / TX) * (p.C / 8);
+  const size_t total = static_cast<size_t>(p.B) * p.Ho * ((p.Wo + TX - 1) / TX) * (p.C / 8);
   const unsigned grid = grid_for(total, 128, 132 * 64);
   if (act) dw_strip_kernel<K, S, TX, true><<<grid, 128, 0, s>>>(p);
   else dw_strip_kernel<K, S, TX, false><<<grid, 128, 0, s>>>(p);
@@ -313,7 +332,8 @@ int dw_strip_launch(const DwConvParams& p, bool act, cudaStream_t s) {
 
 // act: 0 none, 2 swish.  p.bias may be null (plain depthwise half of a separable conv).
 int dwconv_launch(const DwConvParams& p, int act, cudaStream_t s) {
-  B2_CHECK(p.C % 8 == 0 && (p.K == 3 || p.K == 5) && (p.stride == 1 || p.stride == 2), "dwconv: unsupported geometry");
+  B2_CHECK(p.B >= 1 && p.C % 8 == 0 && (p.K == 3 || p.K == 5) && (p.stride == 1 || p.stride == 2),
+           "dwconv: unsupported geometry");
   const bool a = act != 0;
   if (p.K == 3 && p.stride == 1) return dw_strip_launch<3, 1>(p, a, s);
   if (p.K == 3 && p.stride == 2) return dw_strip_launch<3, 2>(p, a, s);
@@ -343,7 +363,6 @@ int se_excite_launch(const float* partial, int B, int HW, int Cpad, int C, int n
                      const float* b1, const float* w2, const float* b2, int relu, float* gate, const float* w, int rows,
                      __half* w_hi, __half* w_lo, cudaStream_t s) {
   B2_CHECK(Cpad % 64 == 0 && nr >= 1 && nr <= kSeMaxNr, "se excite: channel count out of range");
-  B2_CHECK(w == nullptr || B == 1, "se excite: the weight fold takes one image");
   se_fc1_kernel<<<dim3(kSeFc1Blocks, B), 256, 0, s>>>(partial, se_chunks(HW), Cpad, C, nr, 1.0f / static_cast<float>(HW),
                                                        w1, r_part);
   const dim3 grid(Cpad / 64, B);
@@ -357,12 +376,13 @@ int se_excite_launch(const float* partial, int B, int HW, int Cpad, int C, int n
   return 0;
 }
 
-// squeeze-excite of one MBConv block, gate folded into the projection weights (w [rows][K=Cpad] fp32 master copy)
-int se_gate_launch(const __half* in_hi, const __half* in_lo, int HW, int Cpad, int C, int nr, float* partial, float* r_part,
-                   const float* w1, const float* b1, const float* w2, const float* b2, float* gate, const float* w, int rows,
-                   __half* w_hi, __half* w_lo, cudaStream_t s) {
-  if (se_squeeze_launch(in_hi, in_lo, 1, HW, Cpad, partial, s)) return -1;
-  return se_excite_launch(partial, 1, HW, Cpad, C, nr, r_part, w1, b1, w2, b2, 0, gate, w, rows, w_hi, w_lo, s);
+// squeeze-excite of one MBConv block over B images, each gate folded into its image's copy of the projection weights
+// (w [rows][K=Cpad] fp32 master copy -> [B][rows][K] planes)
+int se_gate_launch(const __half* in_hi, const __half* in_lo, int B, int HW, int Cpad, int C, int nr, float* partial,
+                   float* r_part, const float* w1, const float* b1, const float* w2, const float* b2, float* gate,
+                   const float* w, int rows, __half* w_hi, __half* w_lo, cudaStream_t s) {
+  if (se_squeeze_launch(in_hi, in_lo, B, HW, Cpad, partial, s)) return -1;
+  return se_excite_launch(partial, B, HW, Cpad, C, nr, r_part, w1, b1, w2, b2, 0, gate, w, rows, w_hi, w_lo, s);
 }
 
 }  // namespace b2

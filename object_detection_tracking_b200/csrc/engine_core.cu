@@ -18,7 +18,12 @@ Arena::~Arena() {
 
 void* Arena::raw(size_t bytes, bool zero) {
   void* p = nullptr;
-  if (cudaMalloc(&p, bytes + 256) != cudaSuccess) return nullptr;
+  requested_ += bytes + 256;
+  if (cudaMalloc(&p, bytes + 256) != cudaSuccess) {
+    cudaGetLastError();   // an out-of-memory result is not sticky: keep it from surfacing at a later launch check
+    failed_ += bytes + 256;
+    return nullptr;
+  }
   if (zero) cudaMemset(p, 0, bytes + 256);
   ptrs_.push_back(p);
   return p;

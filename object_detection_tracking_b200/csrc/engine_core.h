@@ -48,10 +48,13 @@ class Arena {
   }
   // hi (+ lo in split precision) planes of B x H x W x C; hi == nullptr when out of memory
   Planes planes(int B, int H, int W, int C, bool split, int creal = 0);
+  size_t requested() const { return requested_; }   // bytes asked for so far, failed requests included
+  size_t failed() const { return failed_; }         // bytes of the requests that could not be allocated
 
  private:
   void* raw(size_t bytes, bool zero);
   std::vector<void*> ptrs_;
+  size_t requested_ = 0, failed_ = 0;
 };
 
 struct PlanDeleter {

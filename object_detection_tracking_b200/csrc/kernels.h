@@ -149,9 +149,13 @@ int bifpn_combine_launch(const BifpnCombineParams& p, cudaStream_t s);
 int dw3x3_plain_launch(const __half* in_hi, const __half* in_lo, int B, int H, int W, int C, const float* w, __half* out_hi,
                        __half* out_lo, cudaStream_t s);
 
+// Every buffer below holds one slice per image (B images; the image is a grid dimension of every kernel): head outputs
+// image b at logits[l] + b * logit_bstride[l] (boxes alike), the scratch and the outputs at b times their per-image size.
 struct EffdetPostParams {
-  const float* logits[5];   // per level [h*w][ld]: anchor-major, class-minor (A * num_classes real columns)
-  const float* boxes[5];    // per level [h*w][ldb]: A * 4 (ty, tx, th, tw)
+  const float* logits[5];   // per level [B][h*w][ld]: anchor-major, class-minor (A * num_classes real columns)
+  const float* boxes[5];    // per level [B][h*w][ldb]: A * 4 (ty, tx, th, tw)
+  unsigned long long logit_bstride[5], box_bstride[5];   // elements between consecutive images of logits[l] / boxes[l]
+  int B;
   int ld[5], ldb[5], w[5];
   unsigned long long level_off[6];   // flat logit index where each level starts
   unsigned long long total;
@@ -159,34 +163,44 @@ struct EffdetPostParams {
   double stride_y[5], stride_x[5], half_y[5][9], half_x[5][9];   // anchor grid (anchors.py:216-257), float64 like numpy
   int k, max_out;
   float score_thresh, nms_thr;
-  unsigned int* hist;       // [256]
-  uint32_t* state;          // [8]: prefix, mask, need, n_selected (> k-th), n_ties (== k-th), n_candidates
-  unsigned long long* cand; // [k]
-  unsigned long long* ties; // [k] lowest-index ties of the k-th value
-  unsigned int* tie_cnt;    // [effdet_topk_blocks()] ties per block (blocks own contiguous index ranges)
+  unsigned int* hist;       // [B][256]
+  uint32_t* state;          // [B][8]: prefix, mask, need, n_selected (> k-th), n_ties (== k-th), n_candidates
+  unsigned long long* cand; // [B][k]
+  unsigned long long* ties; // [B][k] lowest-index ties of the k-th value
+  unsigned int* tie_cnt;    // [B][effdet_topk_blocks()] ties per block (blocks own contiguous index ranges)
   unsigned int* tie_off;    // exclusive prefix of tie_cnt
-  float4* cand_box;         // [k] (ymin, xmin, ymax, xmax), score order
+  float4* cand_box;         // [B][k] (ymin, xmin, ymax, xmax), score order
   float* cand_score;
   int* cand_cls;
   int* cand_lvl;
-  unsigned long long* mask; // [k][ceil(k/64)]
-  float4* out_boxes;        // [max_out] x1 y1 x2 y2, scaled back to the original frame
+  unsigned long long* mask; // [B][k][ceil(k/64)]
+  float4* out_boxes;        // [B][max_out] x1 y1 x2 y2, scaled back to the original frame
   float* out_scores;
   int* out_classes;
   int* out_levels;
-  int* out_count;
+  int* out_count;           // [B]
 };
 int effdet_topk_blocks();
+// image_scale_dev [B]: image b's boxes are multiplied by image_scale_dev[b]
 int effdet_post_launch(const EffdetPostParams& p, const float* image_scale_dev, cudaStream_t s);
 
 // effnet.cu -- EfficientNet backbone pieces + EfficientDet input pre-processing
-int effnet_preprocess_launch(const uint8_t* img_bgr, int h, int w, int sh, int sw, float* out, int H, int W, cudaStream_t s);
-int stem_im2col_launch(const float* img, int H, int W, int Ho, int Wo, int pad_t, int pad_l, __half* out_hi, __half* out_lo,
-                       cudaStream_t s);
+// One image of a pre-processing launch: its BGR frame at byte `src` of the upload buffer, h x w, resized to sh x sw
+// (ys = h / sh, xs = w / sw in float32, as effnet_frame computes them)
+struct EffnetFrame {
+  unsigned long long src;
+  int h, w, sh, sw;
+  float ys, xs;
+};
+EffnetFrame effnet_frame(unsigned long long src, int h, int w, int sh, int sw);
+// frames (device table of B entries) -> out [B][H][W][3] fp32
+int effnet_preprocess_launch(const uint8_t* frames, const EffnetFrame* table, int B, float* out, int H, int W, cudaStream_t s);
+int stem_im2col_launch(const float* img, int B, int H, int W, int Ho, int Wo, int pad_t, int pad_l, __half* out_hi,
+                       __half* out_lo, cudaStream_t s);
 struct DwConvParams {
   const __half* in_hi;
   const __half* in_lo;
-  int H, W, C;              // input map (batch 1), C multiple of 8
+  int B, H, W, C;           // input map [B][H][W][C], C multiple of 8
   int K, stride, pad_t, pad_l;
   int Ho, Wo;
   const float* w;           // [K*K][C], BatchNorm scale folded in
@@ -199,12 +213,15 @@ int dwconv_launch(const DwConvParams& p, int act, cudaStream_t s);   // act 0 no
 int se_chunks(int HW);      // rows of the partial-sum buffer se_gate_launch needs
 int se_fc1_parts();         // rows of the r_part buffer (row stride se_max_nr())
 int se_max_nr();
-int se_gate_launch(const __half* in_hi, const __half* in_lo, int HW, int Cpad, int C, int nr, float* partial, float* r_part,
-                   const float* w1, const float* b1, const float* w2, const float* b2, float* gate, const float* w, int rows,
-                   __half* w_hi, __half* w_lo, cudaStream_t s);
+// MBConv's squeeze-excite over B images, each gate folded into its own copy of the projection weights: w [rows][Cpad]
+// fp32 -> (w_hi, w_lo) [B][rows][Cpad]
+int se_gate_launch(const __half* in_hi, const __half* in_lo, int B, int HW, int Cpad, int C, int nr, float* partial,
+                   float* r_part, const float* w1, const float* b1, const float* w2, const float* b2, float* gate,
+                   const float* w, int rows, __half* w_hi, __half* w_lo, cudaStream_t s);
 // The two halves of squeeze-excite over B images [B][HW][Cpad], every image with its own scratch: partial
 // [B][se_chunks(HW)][Cpad], r_part [B][se_fc1_parts()][se_max_nr()], gate [B][Cpad].  relu selects the hidden activation
-// (1 ReLU for the SE-ResNet bottleneck, 0 swish for MBConv); w == nullptr writes the gate only (no weight fold).
+// (1 ReLU for the SE-ResNet bottleneck, 0 swish for MBConv); w == nullptr writes the gate only (no weight fold), else
+// image b's folded weights go to w_hi / w_lo + b * rows * Cpad.
 int se_squeeze_launch(const __half* in_hi, const __half* in_lo, int B, int HW, int Cpad, float* partial, cudaStream_t s);
 int se_excite_launch(const float* partial, int B, int HW, int Cpad, int C, int nr, float* r_part, const float* w1,
                      const float* b1, const float* w2, const float* b2, int relu, float* gate, const float* w, int rows,
@@ -212,15 +229,15 @@ int se_excite_launch(const float* partial, int B, int HW, int Cpad, int C, int n
 
 // roialign.cu -- ROIAlign 7x7 on the detection's own level + mean over the 49 bins (efficientdet_wrapper.py:265-301)
 struct LevelRoiFeatParams {
-  const __half* feat_hi[5];
+  const __half* feat_hi[5]; // per level [B][H][W][C]
   const __half* feat_lo[5];
   int H[5], W[5];
   float inv_stride[5];
-  int C, Creal, min_level, max_out;
-  const float4* boxes;      // x1 y1 x2 y2
-  const int* levels;
-  const int* count;
-  float* out;               // [max_out][Creal]
+  int B, C, Creal, min_level, max_out;
+  const float4* boxes;      // [B][max_out] x1 y1 x2 y2
+  const int* levels;        // [B][max_out]
+  const int* count;         // [B]
+  float* out;               // [B][max_out][Creal]
 };
 int level_roi_feat_launch(const LevelRoiFeatParams& p, cudaStream_t s);
 

@@ -456,7 +456,7 @@ int b2_op_depthwise(int device, const float* x, const float* w, const float* bia
   B2_CHECK(xp.hi && op.hi && dw && (!bias || db), "b2_op_depthwise: out of device memory");
   if (upload_planes(x, xp.hi, xp.lo, xp.elems(), nullptr)) return -1;
   if (impl == 0) {
-    const DwConvParams p{xp.hi, xp.lo, H, W, C, K, stride, pad_t, pad_l, Ho, Wo, dw, db, op.hi, op.lo};
+    const DwConvParams p{xp.hi, xp.lo, 1, H, W, C, K, stride, pad_t, pad_l, Ho, Wo, dw, db, op.hi, op.lo};
     if (dwconv_launch(p, act, nullptr)) return -1;
   } else if (dwconv3x3_launch(xp.hi, xp.lo, B, H, W, C, dw, db, op.hi, op.lo, nullptr)) {
     return -1;
@@ -571,7 +571,7 @@ int b2_op_mbconv_se(int device, const float* x, const float* w1, const float* b1
            "b2_op_mbconv_se: out of device memory");
   if (upload_planes(x, xp.hi, xp.lo, xp.elems(), nullptr)) return -1;
   if (w) {
-    if (se_gate_launch(xp.hi, xp.lo, HW, Cpad, Creal, nr, partial, r_part, d_w1, d_b1, d_w2, d_b2, g, d_w, rows, wp.hi,
+    if (se_gate_launch(xp.hi, xp.lo, 1, HW, Cpad, Creal, nr, partial, r_part, d_w1, d_b1, d_w2, d_b2, g, d_w, rows, wp.hi,
                        wp.lo, nullptr))
       return -1;
   } else if (se_squeeze_launch(xp.hi, xp.lo, B, HW, Cpad, partial, nullptr) ||
@@ -633,7 +633,7 @@ int b2_op_stem_im2col(int device, const float* img, int H, int W, int Ho, int Wo
   const Planes op = a.planes(1, Ho, Wo, 64, split != 0);
   float* d_img = upload_f32(a, img, static_cast<size_t>(H) * W * 3);
   B2_CHECK(op.hi && d_img, "b2_op_stem_im2col: out of device memory");
-  if (stem_im2col_launch(d_img, H, W, Ho, Wo, pad_t, pad_l, op.hi, op.lo, nullptr)) return -1;
+  if (stem_im2col_launch(d_img, 1, H, W, Ho, Wo, pad_t, pad_l, op.hi, op.lo, nullptr)) return -1;
   B2_CUDA(cudaDeviceSynchronize());
   return return_planes(op, op.elems(), out, out_hi, out_lo);
 }

@@ -113,16 +113,17 @@ __global__ void __launch_bounds__(256) roialign_kernel(const __grid_constant__ R
 }
 
 // EfficientDet box feature: ROIAlign 7x7 on the detection's own pyramid level, then the mean of the 49 bins.
-// One block per detection, one thread per channel octet.
+// One block per detection (blockIdx.x) of image blockIdx.y, one thread per channel octet.
 __global__ void level_roi_feat_kernel(const __grid_constant__ LevelRoiFeatParams p) {
-  const int roi = blockIdx.x;
+  const int roi = blockIdx.x, img = blockIdx.y;
+  const size_t slot = static_cast<size_t>(img) * p.max_out + roi;
   const int cvec = p.C / 8;
-  const bool live = roi < p.count[0];
+  const bool live = roi < p.count[img];
   float4 bx = make_float4(0.f, 0.f, 0.f, 0.f);
   int lvl = 0;
   if (live) {
-    bx = __ldg(p.boxes + roi);
-    lvl = p.levels[roi] - p.min_level;
+    bx = __ldg(p.boxes + slot);
+    lvl = p.levels[slot] - p.min_level;
   }
   for (int cv = threadIdx.x; cv < cvec; cv += blockDim.x) {
     float sum[8];
@@ -131,8 +132,9 @@ __global__ void level_roi_feat_kernel(const __grid_constant__ LevelRoiFeatParams
     if (live) {
       const float is = p.inv_stride[lvl];
       const int H = p.H[lvl], W = p.W[lvl];
-      const __half* fh = p.feat_hi[lvl];
-      const __half* fl = p.feat_lo[lvl];
+      const size_t fimg = static_cast<size_t>(img) * H * W * p.C;
+      const __half* fh = p.feat_hi[lvl] + fimg;
+      const __half* fl = p.feat_lo[lvl] ? p.feat_lo[lvl] + fimg : nullptr;
       for (int bin = 0; bin < kOut * kOut; ++bin) {
         const int oy = bin / kOut, ox = bin % kOut;
         const Axis ay = make_axis(__fmul_rn(bx.y, is), __fmul_rn(bx.w, is), H, oy);
@@ -167,7 +169,7 @@ __global__ void level_roi_feat_kernel(const __grid_constant__ LevelRoiFeatParams
 #pragma unroll
     for (int t = 0; t < 8; ++t) {
       const int ch = cv * 8 + t;
-      if (ch < p.Creal) p.out[static_cast<size_t>(roi) * p.Creal + ch] = __fdiv_rn(sum[t], 49.f);
+      if (ch < p.Creal) p.out[slot * p.Creal + ch] = __fdiv_rn(sum[t], 49.f);
     }
   }
 }
@@ -175,8 +177,8 @@ __global__ void level_roi_feat_kernel(const __grid_constant__ LevelRoiFeatParams
 }  // namespace
 
 int level_roi_feat_launch(const LevelRoiFeatParams& p, cudaStream_t s) {
-  B2_CHECK(p.C % 8 == 0 && p.max_out >= 1, "level_roi_feat: bad parameters");
-  level_roi_feat_kernel<<<p.max_out, 64, 0, s>>>(p);
+  B2_CHECK(p.C % 8 == 0 && p.max_out >= 1 && p.B >= 1 && p.B <= 65535, "level_roi_feat: bad parameters");
+  level_roi_feat_kernel<<<dim3(p.max_out, p.B), 64, 0, s>>>(p);
   B2_CUDA(cudaGetLastError());
   return 0;
 }

@@ -15,7 +15,7 @@ POST_STAGES = ("topk_boxes", "topk_scores", "topk_classes", "topk_levels", "topk
 I32_STAGES = ("topk_classes", "topk_levels", "topk_count", "final_classes", "final_levels", "final_count")
 
 
-def _c_config(cfg, precision: str, backbone) -> _lib.B2EffdetConfig:
+def _c_config(cfg, precision: str, backbone, batch: int = 1) -> _lib.B2EffdetConfig:
     c = _lib.B2EffdetConfig()
     c.backbone = -1 if backbone is None else int(str(backbone)[-1])
     c.image_h, c.image_w = int(cfg.image_size[0]), int(cfg.image_size[1])
@@ -35,18 +35,24 @@ def _c_config(cfg, precision: str, backbone) -> _lib.B2EffdetConfig:
     c.max_detection_topk, c.result_per_im = int(cfg.max_detection_topk), int(cfg.result_per_im)
     c.nms_iou_threshold, c.result_score_thres = float(cfg.nms_iou_threshold), float(cfg.result_score_thres)
     c.precision = {"fp16": 0, "split": 1}[precision]
+    c.batch = int(batch)
     return c
 
 
 class EffdetEngine:
     """Feature network + heads + post-processing of one EfficientDet configuration on one GPU."""
 
-    def __init__(self, cfg, weights: dict, device: int = 0, precision: str = "split", backbone=None):
-        """backbone: None (features in, run_features only) or "efficientnet-b0".."efficientnet-b7" (detect())."""
+    def __init__(self, cfg, weights: dict, device: int = 0, precision: str = "split", backbone=None, batch: int = 1):
+        """backbone: None (features in, run_features only) or "efficientnet-b0".."efficientnet-b7" (detect()).
+        batch: images per call; with batch > 1 the context runs detect_batch() (up to `batch` frames of any sizes, each
+        bit-identical to detect() on a batch-1 context) and its stages carry every image."""
+        if int(batch) < 1:
+            raise ValueError("batch must be >= 1")
         self.cfg = cfg
+        self.batch = int(batch)
         self._lib = _lib.load()
         self._h = ctypes.c_void_p()
-        cc = _c_config(cfg, precision, backbone)
+        cc = _c_config(cfg, precision, backbone, self.batch)
         _lib.check(self._lib.b2_effdet_create(ctypes.byref(self._h), ctypes.byref(cc), int(device)), "b2_effdet_create")
         self.load_weights(weights)
 
@@ -99,12 +105,52 @@ class EffdetEngine:
         return dict(final_boxes=boxes[:n], final_probs=scores[:n], final_labels=classes[:n], levels=levels[:n],
                     fpn_box_feat=feat[:n], image_scale=float(scale[0]))
 
-    def stage(self, name: str, real: int = None) -> np.ndarray:
+    def detect_batch(self, frames) -> list:
+        """1..batch BGR uint8 frames [h,w,3] of any sizes -> one dict per frame with detect()'s keys, in one pass."""
+        frames = [np.ascontiguousarray(f, np.uint8) for f in frames]
+        if not 1 <= len(frames) <= self.batch:
+            raise ValueError("detect_batch takes 1 to %d frames, got %d" % (self.batch, len(frames)))
+        for f in frames:
+            if f.ndim != 3 or f.shape[2] != 3:
+                raise ValueError("frames must be [h, w, 3] uint8 BGR")
+        B, n = self.batch, len(frames)
+        m, f = int(self.cfg.result_per_im), int(self.cfg.fpn_num_filters)
+        boxes = np.zeros((B, m, 4), np.float32)
+        scores = np.zeros((B, m), np.float32)
+        classes = np.zeros((B, m), np.int32)
+        levels = np.zeros((B, m), np.int32)
+        feat = np.zeros((B, m, f), np.float32)
+        count = np.zeros(B, np.int32)
+        scale = np.zeros(B, np.float32)
+        ptrs = (ctypes.c_void_p * n)(*[fr.ctypes.data for fr in frames])
+        hs = np.array([fr.shape[0] for fr in frames], np.int32)
+        ws = np.array([fr.shape[1] for fr in frames], np.int32)
+        _lib.check(self._lib.b2_effdet_detect_batch(
+            self._h, ptrs, hs.ctypes.data, ws.ctypes.data, n, boxes.ctypes.data, scores.ctypes.data, classes.ctypes.data,
+            levels.ctypes.data, feat.ctypes.data, count.ctypes.data, scale.ctypes.data), "b2_effdet_detect_batch")
+        out = []
+        for b in range(n):
+            r = int(count[b])
+            out.append(dict(final_boxes=boxes[b, :r].copy(), final_probs=scores[b, :r].copy(),
+                            final_labels=classes[b, :r].copy(), levels=levels[b, :r].copy(),
+                            fpn_box_feat=feat[b, :r].copy(), image_scale=float(scale[b])))
+        return out
+
+    def replay_ms(self, reps: int = 10) -> float:
+        """Mean milliseconds of one replay of the whole-frame graph the last detect call captured (no host copies)."""
+        ms = ctypes.c_float()
+        _lib.check(self._lib.b2_effdet_replay(self._h, int(reps), ctypes.byref(ms)), "b2_effdet_replay")
+        return float(ms.value)
+
+    def stage(self, name: str, real: int = None, image: int = None) -> np.ndarray:
         """'fpn3'..'fpn7' -> [H,W,F]; 'cls3'.. -> [H,W,A*num_classes]; 'box3'.. -> [H,W,A*4]; 'image' -> [H,W,3];
         'stem' / 'block_<i>' / 'c3'..'c5' -> [h,w,C] (pass `real` to drop the operand channel padding);
-        post-processing stages (POST_STAGES) -> [n,4] boxes, [n,F] box_feat, else [n] (int32 for I32_STAGES)."""
+        post-processing stages (POST_STAGES) -> [n,4] boxes, [n,F] box_feat, else [n] (int32 for I32_STAGES).
+        On a batch context: image `image`'s slice, or with image=None every image's, stacked on a leading axis."""
+        if image is not None and not 0 <= int(image) < self.batch:
+            raise IndexError("image %d of a batch of %d" % (image, self.batch))
         if name in POST_STAGES:
-            return self._post_stage(name)
+            return self._pick(self._post_stage(name), image)
         na = self.cfg.num_scales * len(self.cfg.aspect_ratios)
         if real is None:
             real = {"fpn": self.cfg.fpn_num_filters, "cls": na * self.cfg.num_classes, "box": na * 4,
@@ -114,29 +160,40 @@ class EffdetEngine:
         cap = int(self.cfg.image_size[0]) * int(self.cfg.image_size[1]) * 64      # stride-2 maps have <= 64 channels
         if name[:3] in ("cls", "box", "fpn") or name in ("c3", "c4", "c5"):
             cap //= 4
-        buf = np.zeros(cap, np.float32)
+        buf = np.zeros(cap * self.batch, np.float32)
         shape = (ctypes.c_int64 * 4)()
         _lib.check(self._lib.b2_effdet_get_stage(self._h, name.encode(), buf.ctypes.data, buf.nbytes, shape),
                    "b2_effdet_get_stage")
-        _, h, w, c = [int(v) for v in shape]
-        out = buf[: h * w * c].reshape(h, w, c)
-        return (out if real is None else out[:, :, :real]).copy()
+        nb, h, w, c = [int(v) for v in shape]
+        out = buf[: nb * h * w * c].reshape(nb, h, w, c)
+        return self._pick(out if real is None else out[..., :real], image).copy()
+
+    def _pick(self, per_image: np.ndarray, image) -> np.ndarray:
+        """[batch, ...] -> one image's [...] (image 0 of a batch-1 context when `image` is None), or all of them."""
+        if image is None:
+            return per_image[0] if self.batch == 1 else per_image
+        return per_image[int(image)]
 
     def _post_stage(self, name: str) -> np.ndarray:
+        """[batch, n, c] ([batch, n] where c is 1)."""
         k, m = int(self.cfg.max_detection_topk), int(self.cfg.result_per_im)
-        buf = np.zeros(max(4 * k, m * max(4, int(self.cfg.fpn_num_filters))), np.float32)
+        buf = np.zeros(self.batch * max(4 * k, m * max(4, int(self.cfg.fpn_num_filters)), 8), np.float32)
         shape = (ctypes.c_int64 * 4)()
         _lib.check(self._lib.b2_effdet_get_stage(self._h, name.encode(), buf.ctypes.data, buf.nbytes, shape),
                    "b2_effdet_get_stage")
-        n, c = int(shape[2]), int(shape[3])
-        out = buf[: n * c]
+        nb, n, c = int(shape[0]), int(shape[2]), int(shape[3])
+        out = buf[: nb * n * c]
         if name in I32_STAGES:
             out = out.view(np.int32)
-        return (out.reshape(n, c) if c > 1 else out).copy()
+        out = out.reshape(nb, n, c)
+        if name == "topk_count" and c == 8:          # a batch context exposes each image's [8] top-k state: count at 5
+            out = out[:, :, 5:6]
+        return (out if out.shape[2] > 1 else out[:, :, 0]).copy()
 
     def set_stage(self, name: str, value: np.ndarray) -> None:
         """Overwrite a stage with its whole stored shape: 'cls3'.. [H,W,pad16(A*num_classes)], 'box3'.. [H,W,pad16(A*4)],
-        'fpn3'.. [H,W,pad64(F)] (float32), 'image_scale' [1], or a post-processing stage (int32 for I32_STAGES)."""
+        'fpn3'.. [H,W,pad64(F)] (float32), 'image_scale' [1], or a post-processing stage (int32 for I32_STAGES); on a
+        batch context every image's, stacked on a leading [batch] axis."""
         a = np.ascontiguousarray(value, np.int32 if name in I32_STAGES else np.float32)
         _lib.check(self._lib.b2_effdet_set_stage(self._h, name.encode(), a.ctypes.data, a.nbytes), "b2_effdet_set_stage")
 
