@@ -88,12 +88,29 @@ typedef struct b2_config_ext {
                                  use_se; use_resnext wins over it (nn.py:864-868) */
 } b2_config_ext;
 
+/* Graph options added after b2_config_ext's layout was fixed (one int32, use_basic_block, which callers built against
+ * that header pass).  b2_create_ex2 takes them; b2_create_ex builds the graph with every field 0. */
+typedef struct b2_config_ext2 {
+  int32_t num_partial_classes;     /* --use_partial_classes (models.py:807-828): 0 = off.  Otherwise the box head keeps
+                                      only the label logits [0] + partial_class_ids and the box logits of those classes,
+                                      in this order, and the post-processing runs over num_partial_classes + 1 classes:
+                                      final labels are 1..num_partial_classes, the index into partial_class_ids plus one,
+                                      with probabilities from that (num_partial_classes + 1)-way softmax.  The checkpoint
+                                      keeps its num_class columns.  The mask head keeps num_class - 1 channels and picks
+                                      channel (final label - 1) of them, as the reference does (models.py:934-961).
+                                      At most num_class - 1 */
+  int32_t partial_class_ids[80];   /* the checkpoint's class ids, each in 1..num_class - 1, no duplicates */
+} b2_config_ext2;
+
 const char* b2_last_error(void);
 int b2_version(void);
 
 int b2_create(b2_ctx** out, int device, const b2_config* cfg);
 /* b2_create with the options of b2_config_ext; ext may be NULL (all 0) */
 int b2_create_ex(b2_ctx** out, int device, const b2_config* cfg, const b2_config_ext* ext);
+/* b2_create_ex with the options of b2_config_ext2 as well; ext and ext2 may be NULL (all 0).  Refuses, with the reason,
+ * partial class ids outside 1..num_class - 1, duplicates and a count above num_class - 1, before touching the device */
+int b2_create_ex2(b2_ctx** out, int device, const b2_config* cfg, const b2_config_ext* ext, const b2_config_ext2* ext2);
 void b2_destroy(b2_ctx* ctx);
 
 /* Named fp32 host arrays in the reference's Tensorpack-npz naming ("conv0/W",

@@ -32,6 +32,10 @@ class B2ConfigExt(ctypes.Structure):
     _fields_ = [("use_basic_block", c_int32)]
 
 
+class B2ConfigExt2(ctypes.Structure):
+    _fields_ = [("num_partial_classes", c_int32), ("partial_class_ids", c_int32 * 80)]
+
+
 class B2EffdetConfig(ctypes.Structure):
     _fields_ = [
         ("image_h", c_int32), ("image_w", c_int32), ("min_level", c_int32), ("max_level", c_int32),
@@ -57,6 +61,7 @@ SYMBOLS = [
     ("b2_version", c_int, []),
     ("b2_create", c_int, [POINTER(c_void_p), c_int, POINTER(B2Config)]),
     ("b2_create_ex", c_int, [POINTER(c_void_p), c_int, POINTER(B2Config), POINTER(B2ConfigExt)]),
+    ("b2_create_ex2", c_int, [POINTER(c_void_p), c_int, POINTER(B2Config), POINTER(B2ConfigExt), POINTER(B2ConfigExt2)]),
     ("b2_destroy", None, [c_void_p]),
     ("b2_load_weights", c_int, [c_void_p, POINTER(c_char_p), POINTER(c_void_p), POINTER(c_int64), c_int]),
     ("b2_detect", c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int]),
@@ -232,4 +237,17 @@ def make_config_ext(cfg) -> B2ConfigExt:
     """The options of the namespace that b2_config_ext carries."""
     e = B2ConfigExt()
     e.use_basic_block = int(bool(getattr(cfg, "use_basic_block", False)))
+    return e
+
+
+def make_config_ext2(cfg) -> B2ConfigExt2:
+    """The options of the namespace that b2_config_ext2 carries: the partial class ids (config.normalize_config resolves
+    and checks them; () = off)."""
+    e = B2ConfigExt2()
+    ids = tuple(getattr(cfg, "partial_class_ids", ()))
+    if len(ids) > 80:
+        raise ValueError("at most 80 partial classes, got %d" % len(ids))
+    e.num_partial_classes = len(ids)
+    for i, v in enumerate(ids):
+        e.partial_class_ids[i] = int(v)
     return e

@@ -13,7 +13,9 @@ models.py:196-263).  This module provides the same surface on top of libb200det:
     sess = Session(); sess.run([model.final_boxes, ...], feed_dict=fd)
 
 Outputs follow the reference conventions: fresh, writable numpy arrays owned by the caller; boxes are
-x1,y1,x2,y2 in resized-image pixels; labels are 1-based (int64 single image, float32 batch).
+x1,y1,x2,y2 in resized-image pixels; labels are 1-based (int64 single image, float32 batch): class ids 1..num_class-1,
+or with config.use_partial_classes 1..len(partial_classes), the position in partial_classes plus one, with probabilities
+from the (len(partial_classes) + 1)-way softmax (models.py:807-843).
 There is no CPU fallback: without the CUDA library or an H100 the calls raise.
 """
 from __future__ import annotations
@@ -62,7 +64,10 @@ class TensorHandle:
 
 
 class Mask_RCNN_FPN:
-    """Single-image model object (reference: models.py:266-1813, inference surface only)."""
+    """Single-image model object (reference: models.py:266-1813, inference surface only).  With use_partial_classes the
+    checkpoint (or frozen graph) is the 81-class COCO model; the engine keeps the box-head columns of
+    config.partial_class_ids and final_labels are 1..len(partial_classes), as the driver's partial targetid2class reads
+    them (obj_detect_tracking.py:287-291).  final_masks keep the reference's channel choice (DESIGN.md section 4)."""
 
     is_multi = False
 
@@ -149,7 +154,7 @@ class Mask_RCNN_FPN:
                 if f is self.final_boxes:
                     res.append(out["boxes"][0, :r].copy())
                 elif f is self.final_labels:
-                    res.append(out["labels"][0, :r].astype(np.int64))          # models.py:932: int64, class+1
+                    res.append(out["labels"][0, :r].astype(np.int64))          # models.py:932: int64, class+1 (partial: 1..C)
                 elif f is self.final_probs:
                     res.append(out["probs"][0, :r].copy())
                 elif f is self.fpn_box_feat:

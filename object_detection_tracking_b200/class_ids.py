@@ -34,6 +34,16 @@ coco_obj_class_to_id = {n: i for i, n in enumerate(coco_obj_classes)}
 coco_obj_id_to_class = {i: n for n, i in coco_obj_class_to_id.items()}
 assert len(coco_obj_classes) == 81 and len(coco_ids) == 80
 
+# class_ids.py:551-558: the COCO classes the ActEV drivers track and the ActEV object each stands for.  Its keys, in this
+# order, are the default partial_classes of --use_partial_classes (obj_detect_tracking.py:237-239).
+coco_obj_to_actev_obj = {
+    "person": "Person",
+    "car": "Vehicle",
+    "bus": "Vehicle",
+    "truck": "Vehicle",
+    "bicycle": "Bike",
+}
+
 
 def effdet_labels_to_coco80(labels):
     """obj_detect_tracking.py:644-647: EfficientDet's 1..90 category ids -> the detector's dense 1..80 class ids."""

@@ -53,7 +53,9 @@ _DEFAULTS = dict(
     use_basic_block=False,             # set by --resnet34 / --resnet18 (obj_detect_tracking.py:349-359): resnet_basicblock
                                        # (nn.py:439-456) instead of the bottleneck; use_resnext wins (nn.py:864-868);
                                        # the block ignores use_dilations, use_deformable and use_se
-    use_partial_classes=False,
+    use_partial_classes=False,         # --use_partial_classes (obj_detect_tracking.py:233-239): a COCO-81 checkpoint whose
+                                       # box head keeps only partial_classes (models.py:807-828); labels become 1..C
+    partial_classes=None,              # class names, in output-label order; None = the keys of coco_obj_to_actev_obj
     is_efficientdet=False,
 )
 
@@ -87,7 +89,38 @@ def normalize_config(cfg):
     cfg.bbox_decode_clip = float(np.log(cfg.max_size / 16.0))        # :370
     cfg.result_score_thres = float(cfg.threshold_conf)               # :385
     cfg.num_anchors_per_loc = len(cfg.anchor_ratios)
+    cfg.partial_class_ids = _partial_class_ids(cfg)
     return cfg
+
+
+def _partial_class_ids(cfg) -> tuple:
+    """The COCO class ids the box head keeps with use_partial_classes, in partial_classes order (models.py:807-811); ()
+    when it is off.  EfficientDet resolves its own selection (backend.EfficientDet).
+
+    The ids are always coco_obj_class_to_id[name]: what the published frozen partial model computes (main.py:562-566
+    packed it with the COCO table).  config.classname2id is not read: the checkpoint driver overwrites it with the partial
+    table (obj_detect_tracking.py:287-300), under which the same gather would pick the first len(partial_classes) COCO
+    classes instead."""
+    from .class_ids import coco_obj_class_to_id, coco_obj_to_actev_obj
+    if not cfg.use_partial_classes or cfg.is_efficientdet:
+        return ()
+    if cfg.partial_classes is None:
+        cfg.partial_classes = list(coco_obj_to_actev_obj)
+    names = list(cfg.partial_classes)
+    if int(cfg.num_class) != 81:
+        raise ValueError("use_partial_classes selects classes of a COCO model: num_class must be 81, got %d"
+                         % int(cfg.num_class))
+    if not names:
+        raise ValueError("use_partial_classes: partial_classes is empty")
+    for n in names:
+        if n == "BG":
+            raise ValueError("use_partial_classes: 'BG' cannot be selected (the background column is always kept)")
+        if n not in coco_obj_class_to_id:
+            raise ValueError("use_partial_classes: %r is not a COCO class name" % (n,))
+    dup = sorted({n for n in names if names.count(n) > 1})
+    if dup:
+        raise ValueError("use_partial_classes: %s selected more than once" % ", ".join(repr(n) for n in dup))
+    return tuple(coco_obj_class_to_id[n] for n in names)
 
 
 def backbone_geometry(h: int, w: int, cfg):

@@ -471,7 +471,8 @@ int load_rel(const RelOp* R, const WeightSet& ws, cudaStream_t st) {
   return relation_upload_geo(ew, eb, cw, cb, R->geo, st);
 }
 
-int load_layer(const ConvLayer* L, const WeightSet& ws, int num_class, cudaStream_t st) {
+int load_layer(const ConvLayer* L, const WeightSet& ws, int num_class, const int* partial_ids, int num_partial,
+               cudaStream_t st) {
   if (L->layout == kRuntime) return 0;   // written by the pass itself
   const int Cin = L->d.Cin, R = L->d.R, S = L->d.S, Cout = L->d.Cout, K = L->w.K, Cp = L->w.Cout_pad;
   std::vector<float> packed(static_cast<size_t>(Cp) * K, 0.f);
@@ -546,21 +547,32 @@ int load_layer(const ConvLayer* L, const WeightSet& ws, int num_class, cudaStrea
     for (int k = 0; k < Cin; ++k)
       for (int o = 0; o < Cout; ++o) packed[static_cast<size_t>(o) * K + k] = w[static_cast<size_t>(k) * Cout + o];
   } else {
-    // two reference layers fused along N: rpn/{class,box} or fastrcnn/outputs/{class,box}
-    const std::string base = L->layout == kRpnOut ? "rpn" : "fastrcnn/outputs";
-    const int n0 = L->layout == kRpnOut ? 3 : num_class;
-    const int n1 = Cout - n0;
+    // two reference layers fused along N: rpn/{class,box} or fastrcnn/outputs/{class,box}.  col0 / col1 hold the
+    // checkpoint column of each packed class / box column.  use_partial_classes (models.py:807-828) keeps the class
+    // columns [0] + partial_ids and the 4 box columns of each kept class; class 0's box columns stay as a slot the decode
+    // never reads, so the packed layout is the full one's for num_partial + 1 classes.  A class-agnostic box output (4
+    // columns) is kept whole.
+    const bool head = L->layout == kHeadOut, part = head && num_partial > 0;
+    const std::string base = head ? "fastrcnn/outputs" : "rpn";
+    const int n0 = head ? num_class : 3;                        // checkpoint class columns
+    const int p0 = part ? num_partial + 1 : n0;                 // packed class columns
+    const int p1 = Cout - p0;                                   // packed box columns
+    const bool gather_box = part && p1 != 4;
+    const int n1 = gather_box ? 4 * num_class : p1;             // checkpoint box columns
+    std::vector<int> col0(p0), col1(p1);
+    for (int o = 0; o < p0; ++o) col0[o] = part && o > 0 ? partial_ids[o - 1] : o;
+    for (int o = 0; o < p1; ++o) col1[o] = gather_box ? col0[o / 4] * 4 + o % 4 : o;
     const float* w0 = ws.get(base + "/class/W", static_cast<int64_t>(Cin) * n0);
     const float* b0 = ws.get(base + "/class/b", n0);
     const float* w1 = ws.get(base + "/box/W", static_cast<int64_t>(Cin) * n1);
     const float* b1 = ws.get(base + "/box/b", n1);
     if (!w0 || !b0 || !w1 || !b1) return -1;
     for (int k = 0; k < Cin; ++k) {
-      for (int o = 0; o < n0; ++o) packed[static_cast<size_t>(o) * K + k] = w0[static_cast<size_t>(k) * n0 + o];
-      for (int o = 0; o < n1; ++o) packed[static_cast<size_t>(n0 + o) * K + k] = w1[static_cast<size_t>(k) * n1 + o];
+      for (int o = 0; o < p0; ++o) packed[static_cast<size_t>(o) * K + k] = w0[static_cast<size_t>(k) * n0 + col0[o]];
+      for (int o = 0; o < p1; ++o) packed[static_cast<size_t>(p0 + o) * K + k] = w1[static_cast<size_t>(k) * n1 + col1[o]];
     }
-    for (int o = 0; o < n0; ++o) b[o] = b0[o];
-    for (int o = 0; o < n1; ++o) b[n0 + o] = b1[o];
+    for (int o = 0; o < p0; ++o) b[o] = b0[col0[o]];
+    for (int o = 0; o < p1; ++o) b[p0 + o] = b1[col1[o]];
     has_b = false;
   }
   if (has_b) {
@@ -604,10 +616,11 @@ int load_se(const SeOp* S, const WeightSet& ws, cudaStream_t st) {
 
 }  // namespace
 
-int load_weights(const DetPlan& p, const WeightSet& ws, int num_class, cudaStream_t st) {
+int load_weights(const DetPlan& p, const WeightSet& ws, int num_class, cudaStream_t st, const int* partial_ids,
+                 int num_partial) {
   // shared RPN weights: packed once, every level's layer gets its own copy of the (small) operand
   for (auto& L : p.layers)
-    if (load_layer(L.get(), ws, num_class, st)) return -1;
+    if (load_layer(L.get(), ws, num_class, partial_ids, num_partial, st)) return -1;
   for (auto& G : p.gns)
     if (load_gn(G.get(), ws, st)) return -1;
   for (auto& S : p.ses)

@@ -156,8 +156,10 @@ int add_bottleneck(DetPlan& p, const std::string& name, const Planes& x, int str
 
 // The full-batch tensor-core plan of every layer and, with dual, each forked layer's per-part plans (conv_impl 0 only).
 int plan_layers(DetPlan& p, int num_sms);
-// Every layer, GroupNorm, squeeze-excite and relation module of the plan from the checkpoint `ws`; num_class sizes the
-// fused box-head outputs.
-int load_weights(const DetPlan& p, const WeightSet& ws, int num_class, cudaStream_t st);
+// Every layer, GroupNorm, squeeze-excite and relation module of the plan from the checkpoint `ws`; num_class is the
+// checkpoint's class count of the fused box-head outputs.  With num_partial > 0 those outputs keep the class-0 column and
+// the columns of partial_ids[0 .. num_partial), in that order (use_partial_classes).
+int load_weights(const DetPlan& p, const WeightSet& ws, int num_class, cudaStream_t st, const int* partial_ids = nullptr,
+                 int num_partial = 0);
 
 }  // namespace b2

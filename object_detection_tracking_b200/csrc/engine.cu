@@ -100,6 +100,7 @@ struct b2_ctx {
   DetPlan plan;            // first member: its arena is freed after everything that refers to it
   b2_config cfg;
   b2_config_ext ext;       // options appended after b2_config's layout was fixed (b2_create_ex)
+  b2_config_ext2 ext2;     // and after b2_config_ext's (b2_create_ex2)
   int device = 0, num_sms = 132;
   cudaStream_t stream = nullptr;
   // geometry
@@ -415,7 +416,10 @@ int build_plan(b2_ctx* c) {
     B2_CHECK(P.alloc_rows(c->fc6, M, dim), "alloc fc6");
     B2_CHECK(P.alloc_rows(c->fc7, M, dim), "alloc fc7");
   }
-  const int nout = cfg.num_class + (cfg.class_agnostic ? 4 : cfg.num_class * 4);
+  // the classes the box head outputs and the post-processing sees: with use_partial_classes the background and the
+  // selected classes (models.py:807-828, num_class = len(ids) + 1); cfg.num_class stays the checkpoint's
+  const int ncls = c->ext2.num_partial_classes > 0 ? c->ext2.num_partial_classes + 1 : cfg.num_class;
+  const int nout = ncls + (cfg.class_agnostic ? 4 : ncls * 4);
   const int ldo = (nout + 15) / 16 * 16;
   c->head_logits = P.arena.alloc<float>(static_cast<size_t>(Mpad) * ldo);
   Planes rf = c->roi_feat; rf.W = M;
@@ -475,8 +479,8 @@ int build_plan(b2_ctx* c) {
   // ---- post-processing (phase 6) ----
   HeadPostParams& hp = c->post;
   memset(&hp, 0, sizeof(hp));
-  const int nc1 = cfg.num_class - 1, R = cfg.result_per_im;
-  hp.logits = c->head_logits; hp.ld = ldo; hp.num_class = cfg.num_class; hp.B = B; hp.rois_per_image = K;
+  const int nc1 = ncls - 1, R = cfg.result_per_im;
+  hp.logits = c->head_logits; hp.ld = ldo; hp.num_class = ncls; hp.B = B; hp.rois_per_image = K;
   hp.class_agnostic = cfg.class_agnostic;
   hp.rois = rp.prop_boxes; hp.roi_count = rp.prop_count;
   for (int i = 0; i < 4; ++i) hp.reg_w[i] = cfg.bbox_reg_weights[i];
@@ -486,7 +490,7 @@ int build_plan(b2_ctx* c) {
   hp.score_thresh = cfg.multi_semantics ? -INFINITY : cfg.result_score_thres;
   hp.nms_thr = cfg.fastrcnn_nms_iou_thres;
   hp.max_per_class = R; hp.max_total = R;
-  hp.probs = P.arena.alloc<float>(static_cast<size_t>(M) * cfg.num_class);
+  hp.probs = P.arena.alloc<float>(static_cast<size_t>(M) * ncls);
   hp.dec_boxes = P.arena.alloc<float>(static_cast<size_t>(M) * nc1 * 4);
   hp.cls_keep = P.arena.alloc<int>(static_cast<size_t>(B) * nc1 * R);
   hp.cls_count = P.arena.alloc<int>(B * nc1);
@@ -495,7 +499,7 @@ int build_plan(b2_ctx* c) {
   hp.final_labels = P.arena.alloc<int>(static_cast<size_t>(B) * R);
   hp.final_count = P.arena.alloc<int>(B);
   add_batch_step(P, 6, kStepHeadPost, "", [c](int, int, cudaStream_t st) { return head_post_launch(c->post, st); }, 3);
-  P.stages.raw("probs", hp.probs, Stage::kF32, B, K, cfg.num_class, 1);
+  P.stages.raw("probs", hp.probs, Stage::kF32, B, K, ncls, 1);
   P.stages.raw("dec_boxes", hp.dec_boxes, Stage::kF32, B, K, nc1, 4);
   P.stages.raw("final_boxes", hp.final_boxes, Stage::kF32, B, R, 4, 1);
   P.stages.raw("final_probs", hp.final_probs, Stage::kF32, B, R, 1, 1);
@@ -521,6 +525,8 @@ int build_plan(b2_ctx* c) {
   P.stages.raw("fpn_box_feat", c->box_feat, Stage::kF32, static_cast<int64_t>(B) * R, nc, 7, 7);
 
   // ---- mask head (models.py:934-961, 1173-1199), phase 7, only with cfg.add_mask ----
+  // It keeps the checkpoint's num_class - 1 channels with use_partial_classes too, and mask_select_kernel reads channel
+  // (label - 1) for the partial label, as the reference's gather_nd on the full mask logits does (models.py:954-958)
   if (cfg.add_mask) {
     B2_CHECK(cfg.num_class >= 2, "b2_create: add_mask needs at least one foreground class");
     const int MR = B * R, md = 256;                  // mrcnn_head_dim (obj_detect_tracking.py:324)
@@ -607,12 +613,30 @@ extern "C" {
 int b2_create(b2_ctx** out, int device, const b2_config* cfg) { return b2_create_ex(out, device, cfg, nullptr); }
 
 int b2_create_ex(b2_ctx** out, int device, const b2_config* cfg, const b2_config_ext* ext) {
+  return b2_create_ex2(out, device, cfg, ext, nullptr);
+}
+
+int b2_create_ex2(b2_ctx** out, int device, const b2_config* cfg, const b2_config_ext* ext, const b2_config_ext2* ext2) {
   B2_CHECK(out && cfg, "b2_create: null argument");
   *out = nullptr;
   std::unique_ptr<b2_ctx> c(new b2_ctx());
   c->cfg = *cfg;
   memset(&c->ext, 0, sizeof(c->ext));
   if (ext) c->ext = *ext;
+  memset(&c->ext2, 0, sizeof(c->ext2));
+  if (ext2) c->ext2 = *ext2;
+  const int np = c->ext2.num_partial_classes;
+  B2_CHECK(np >= 0 && np <= cfg->num_class - 1 && np <= 80,
+           "b2_create: num_partial_classes must be 0 (off) or 1 .. min(num_class - 1, 80) (num_class " +
+               std::to_string(cfg->num_class) + "), got " + std::to_string(np));
+  for (int i = 0; i < np; ++i) {
+    const int id = c->ext2.partial_class_ids[i];
+    B2_CHECK(id >= 1 && id <= cfg->num_class - 1, "b2_create: partial_class_ids[" + std::to_string(i) + "] = " +
+                                                      std::to_string(id) + " is not a class id in 1 .. num_class - 1");
+    for (int j = 0; j < i; ++j)
+      B2_CHECK(c->ext2.partial_class_ids[j] != id, "b2_create: class id " + std::to_string(id) +
+                                                      " appears twice in partial_class_ids");
+  }
   c->device = device;
   c->plan.split = cfg->precision == 1;
   if (open_device(device, "b2_create", &c->num_sms, &c->stream)) return -1;
@@ -664,7 +688,8 @@ int b2_load_weights(b2_ctx* c, const char* const* names, const float* const* dat
   B2_CHECK(c && names && data && numel, "b2_load_weights: null argument");
   B2_CUDA(cudaSetDevice(c->device));
   const WeightSet ws(names, data, numel, n);
-  if (load_weights(c->plan, ws, c->cfg.num_class, c->stream)) return -1;
+  if (load_weights(c->plan, ws, c->cfg.num_class, c->stream, c->ext2.partial_class_ids, c->ext2.num_partial_classes))
+    return -1;
   c->weights_loaded = true;
   return 0;
 }

@@ -148,7 +148,9 @@ int head_post_launch(const HeadPostParams& p, cudaStream_t s) {
   // them at 8)
   const int KP = next_pow2(R) < 2 ? 2 : next_pow2(R);
   const size_t smem1 = static_cast<size_t>(KP) * (8 + 16 + 4 + 4) + static_cast<size_t>(R) * ((R + 31) / 32) * 4;
-  const int KP2 = next_pow2(nc1 * p.max_per_class);
+  // at least 2 keys here too: the sort's first __syncthreads is what publishes the keys and s_total, and a sort of one key
+  // (one class, e.g. a single partial class, with max_per_class 1) has none
+  const int KP2 = next_pow2(nc1 * p.max_per_class) < 2 ? 2 : next_pow2(nc1 * p.max_per_class);
   const size_t smem2 = static_cast<size_t>(KP2) * 8;
   static bool attr_set = false;
   if (!attr_set) {

@@ -24,9 +24,10 @@ class Detector:
         self._c = _lib.make_config(self.cfg, batch, height, width, input_dtype, precision, conv_impl, use_cuda_graph,
                                    multi_semantics, accum_chunk)
         self._ext = _lib.make_config_ext(self.cfg)
+        self._ext2 = _lib.make_config_ext2(self.cfg)
         self._ctx = c_void_p(0)
-        _lib.check(self.lib.b2_create_ex(ctypes.byref(self._ctx), self.device, ctypes.byref(self._c),
-                                         ctypes.byref(self._ext)), "b2_create")
+        _lib.check(self.lib.b2_create_ex2(ctypes.byref(self._ctx), self.device, ctypes.byref(self._c),
+                                          ctypes.byref(self._ext), ctypes.byref(self._ext2)), "b2_create")
         self.R = int(self.cfg.result_per_im)
         self.C = int(self.cfg.fpn_num_channel)
         self._pinned = None
