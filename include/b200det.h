@@ -182,7 +182,10 @@ int b2_profile_steps(b2_ctx* ctx, int reps, float* ms_out, int cap, int* n_out);
 int b2_step_info(b2_ctx* ctx, int idx, char* name, int name_cap, double* flops, double* bytes, int* kind);
 
 /* DeepSORT appearance cost: gallery [S,D] rows grouped per track by seg_offsets[T+1], dets [N,D];
- * cost[T,N] = min over the track's rows of (1 - cos).  Host pointers. */
+ * cost[T,N] = min over the track's rows of (1 - cos).  Host pointers.  Rows are divided by their norm without an eps, as
+ * nn_matching: a zero row, or a row with a NaN or inf component, gives NaN, and a NaN among a track's rows makes that
+ * track's cost NaN (np.min); the tracker's assignment then refuses the matrix, as the reference's does.  A track with an
+ * empty segment gets 3.4e38 for every detection. */
 int b2_cosine_cost(int device, const float* gallery, const int32_t* seg_offsets, int T, const float* dets, int N,
                    int D, int precision, float* cost);
 
@@ -226,7 +229,8 @@ int b2_track_nms(const double* tlwh, const double* scores, int n, double max_bbo
  * b2_tmot_fuse_motion   = matching.fuse_motion (:97-109): Kalman gate (chi2inv95 of 4 or 2 dof -> inf) and
  *                         cost = lambda * cost + (1 - lambda) * squared Mahalanobis distance, in place on cost [T,N].
  * b2_tmot_embedding_distance = matching.embedding_distance (:80-94): euclidean distance of track / detection embeddings,
- *                         one tensor-core GEMM on `device` (|a|^2 + |b|^2 - 2ab, then sqrt(max(0, .))), out float64 [T,N]. */
+ *                         one tensor-core GEMM on `device` (|a|^2 + |b|^2 - 2ab, then sqrt(max(0, .)) with NaN kept, as
+ *                         np.maximum), out float64 [T,N]; b2_distance_matrix's range check applies. */
 int b2_lapjv(const double* cost, int nr, int nc, double cost_limit, int32_t* x, int32_t* y, double* opt);
 int b2_tmot_iou_distance(const double* atlbr, int na, const double* btlbr, int nb, double* out);
 int b2_tmot_fuse_motion(const double* means, const double* covs, int T, const double* xyah, int N, double* cost,
@@ -344,7 +348,11 @@ int b2_effdet_profile_steps(b2_effdet* ctx, int reps, float* ms_out, int cap, in
 int b2_effdet_step_info(b2_effdet* ctx, int idx, char* name, int name_cap, double* flops, double* bytes, int* kind);
 
 /* Distance matrix of torchreid/distance.py:6-80 on the tensor cores: a [na,D], b [nb,D] (host) -> out [na,nb].
- * metric 0 = cosine (1 - a^.b^), 1 = squared euclidean (|a|^2 + |b|^2 - 2 a.b). */
+ * metric 0 = cosine (1 - a^.b^) with x^ = x / max(|x|, 1e-12) as F.normalize, so a zero row is at distance 1 from every
+ * row; 1 = squared euclidean (|a|^2 + |b|^2 - 2 a.b).  A NaN component makes every distance of its row NaN; so does a
+ * +-inf one in split precision (fp16 precision may give inf instead).  Metric 1 fails ("outside the fp16-plane range")
+ * when a finite component has |x| >= 65520: the fp16 operand plane would hold inf and turn a finite distance into NaN or
+ * inf. */
 int b2_distance_matrix(int device, const float* a, int na, const float* b, int nb, int D, int metric, int precision,
                        float* out);
 
@@ -353,6 +361,9 @@ int b2_distance_matrix(int device, const float* a, int na, const float* b, int n
  * seg_a[N+1], camera 2's b / seg_b[M+1] (host, float32); out[i][j] = min over the two tracks' crops of the squared
  * euclidean distance (clamped at 0, as sklearn.euclidean_distances) where gate[i][j] != 0 (gate NULL = all pairs), else
  * `fill` (999 in the reference).  One tensor-core GEMM over the concatenated galleries + one segmented-min kernel.
+ * A NaN distance in a gated pair's block makes out[i][j] NaN (np.clip and np.min keep NaN); a track with no crops gets
+ * `fill`.  A row with a NaN or +-inf component makes all its distances NaN in split precision; a finite component with
+ * |x| >= 65520 fails the call ("outside the fp16-plane range"), as in b2_distance_matrix.
  * b2_track_spatial_dist = compute_spatial_dist (:260-305) without the ignore-pairs reset: trajectories as (frame, x, y)
  * rows grouped per track, out[i][j] = mean point distance over common frames (camera-2 frames + frame_offset) if <= tol,
  * else 9999.  Host code, float64. */
@@ -489,6 +500,24 @@ int b2_op_channel_gate(int device, const float* s, const float* w1, const float*
  * img[2y - pad_t + r][2x - pad_l + s][c] (0 outside the image), columns 27..63 zero. */
 int b2_op_stem_im2col(int device, const float* img, int H, int W, int Ho, int Wo, int pad_t, int pad_l, int split,
                       float* out, uint16_t* out_hi, uint16_t* out_lo);
+
+/* The distance kernels of b2_cosine_cost, b2_distance_matrix, b2_track_pair_cost and b2_tmot_embedding_distance, one at a
+ * time.  b2_op_distance_operand converts x [rows][D] (host fp32) into the GEMM's operand planes out_hi / out_lo
+ * [rows][ld] (raw fp16, ld >= D, columns >= D zero): normalize != 0, cosine_normalize_rows, x / max(|x|, eps) with the
+ * norm summed in fp32; normalize == 0, rows_to_planes, x itself, with sqnorm [rows] = sum x^2 in fp32 and range_flag = 1
+ * when a finite component rounds to an fp16 inf (sqnorm and range_flag may be NULL, and are not written when
+ * normalize != 0). */
+int b2_op_distance_operand(int device, const float* x, int rows, int D, int ld, int normalize, float eps, uint16_t* out_hi,
+                           uint16_t* out_lo, float* sqnorm, uint32_t* range_flag);
+/* b2_op_distance_epilogue runs one epilogue on host products dots [rows][ld] (ld >= cols), every step one IEEE fp32 op:
+ * kind 0: out [rows][cols] = 1 - dots; kind 1: out = (na2[i] + nb2[j]) - 2 dots[i][j], na2 [rows], nb2 [cols];
+ * kind 2: out [n_a][cols] = min over rows s in [seg_a[t], seg_a[t+1]) of 1 - dots[s][n] (NaN if any is NaN, 3.4e38 for
+ * an empty segment); kind 3: out [n_a][n_b] = min over the block (rows of segment i of seg_a, columns of segment j of
+ * seg_b) of max(0, kind 1's value), NaN if any is NaN, `fill` where gate[i][j] == 0 (gate [n_a][n_b] may be NULL) or a
+ * segment is empty.  Offsets are checked against rows / cols before any device work. */
+int b2_op_distance_epilogue(int device, int kind, const float* dots, int rows, int cols, int ld, const float* na2,
+                            const float* nb2, const int32_t* seg_a, int n_a, const int32_t* seg_b, int n_b,
+                            const uint8_t* gate, float fill, float* out);
 
 #ifdef __cplusplus
 }

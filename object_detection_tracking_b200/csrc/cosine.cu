@@ -11,8 +11,22 @@
 namespace b2 {
 namespace {
 
-// one warp per row: x / ||x||  -> (hi, lo) planes, row stride ld (zero padded to ld)
-__global__ void cosine_normalize_kernel(const float* __restrict__ src, int rows, int D, __half* __restrict__ hi,
+// NaN-propagating min / max (PTX min.NaN / max.NaN, sm_80+): NaN if either operand is NaN, as np.minimum / np.maximum.
+// fminf / fmaxf return the other operand, so a NaN distance would vanish from a minimum.
+__device__ __forceinline__ float min_nan(float a, float b) {
+  float r;
+  asm("min.NaN.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));
+  return r;
+}
+__device__ __forceinline__ float max_nan(float a, float b) {
+  float r;
+  asm("max.NaN.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));
+  return r;
+}
+
+// one warp per row: x / max(||x||, eps) -> (hi, lo) planes, row stride ld (zero padded to ld).  eps 0: a zero row is 0/0 =
+// NaN (nn_matching); eps 1e-12: F.normalize.  A NaN norm stays NaN.
+__global__ void cosine_normalize_kernel(const float* __restrict__ src, int rows, int D, float eps, __half* __restrict__ hi,
                                         __half* __restrict__ lo, int ld) {
   const int row = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
@@ -22,38 +36,48 @@ __global__ void cosine_normalize_kernel(const float* __restrict__ src, int rows,
   for (int c = lane; c < D; c += 32) ss = fmaf(x[c], x[c], ss);
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, o);
-  const float nrm = sqrtf(ss);
+  float nrm = sqrtf(ss);
+  if (nrm < eps) nrm = eps;
   for (int c = lane; c < ld; c += 32)
     store1(hi, lo, static_cast<size_t>(row) * ld + c, c < D ? __fdiv_rn(x[c], nrm) : 0.f);
 }
 
-// cost[t][n] = min over gallery rows s in [off[t], off[t+1]) of (1 - dots[s][n])
+// cost[t][n] = min over gallery rows s in [off[t], off[t+1]) of (1 - dots[s][n]); NaN if any of them is NaN, 3.4e38 for an
+// empty segment
 __global__ void cosine_segmin_kernel(const float* __restrict__ dots, int ld, const int* __restrict__ off, int T, int N,
                                      float* __restrict__ cost) {
   const int idx = blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= T * N) return;
   const int t = idx / N, n = idx - t * N;
   float best = 3.4e38f;
-  for (int s = off[t]; s < off[t + 1]; ++s) best = fminf(best, __fsub_rn(1.f, dots[static_cast<size_t>(s) * ld + n]));
+  for (int s = off[t]; s < off[t + 1]; ++s) best = min_nan(best, __fsub_rn(1.f, dots[static_cast<size_t>(s) * ld + n]));
   cost[idx] = best;
 }
 
-// plain (un-normalised) rows -> (hi, lo) planes + squared norms
+// plain (un-normalised) rows -> (hi, lo) planes + squared norms.  ORs *range_flag (may be null) with 1 when a finite
+// component rounds to an fp16 inf (|x| >= 65520): its planes would turn a finite distance into NaN or inf.
 __global__ void rows_to_planes_kernel(const float* __restrict__ src, int rows, int D, __half* __restrict__ hi,
-                                      __half* __restrict__ lo, int ld, float* __restrict__ sqnorm) {
+                                      __half* __restrict__ lo, int ld, float* __restrict__ sqnorm,
+                                      unsigned int* __restrict__ range_flag) {
   const int row = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int lane = threadIdx.x & 31;
   if (row >= rows) return;
   const float* x = src + static_cast<size_t>(row) * D;
   float ss = 0.f;
+  bool out_of_range = false;
   for (int c = lane; c < ld; c += 32) {
     const float v = c < D ? x[c] : 0.f;
     ss = fmaf(v, v, ss);
+    out_of_range |= fabsf(v) >= 65520.f && fabsf(v) <= 3.402823466e38f;
     store1(hi, lo, static_cast<size_t>(row) * ld + c, v);
   }
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, o);
-  if (lane == 0) sqnorm[row] = ss;
+  out_of_range = __any_sync(0xffffffffu, out_of_range);
+  if (lane == 0) {
+    sqnorm[row] = ss;
+    if (out_of_range && range_flag != nullptr) atomicOr(range_flag, 1u);
+  }
 }
 
 // out[i][j] = metric 0: 1 - dots[i][j]   metric 1: na2[i] + nb2[j] - 2 dots[i][j]
@@ -69,7 +93,8 @@ __global__ void distance_finish_kernel(const float* __restrict__ dots, int ld, i
 
 // Multi-camera ReID pair cost (multi_video_reid.py:308-324 compute_feature_dist): one warp per (track i of camera 1,
 // track j of camera 2); out[i][j] = min over the tracks' crops of max(0, |a|^2 + |b|^2 - 2 a.b) where gate[i][j] != 0,
-// else `fill`.  Lanes stride over the columns of track j (coalesced reads of the dot-product rows).
+// else `fill`; NaN if any distance of the block is NaN (np.clip and np.min keep NaN), `fill` for an empty track.  Lanes
+// stride over the columns of track j (coalesced reads of the dot-product rows).
 __global__ void pair_segmin_kernel(const float* __restrict__ dots, int ld, const float* __restrict__ na2,
                                    const float* __restrict__ nb2, const int* __restrict__ seg_a, int N,
                                    const int* __restrict__ seg_b, int M, const unsigned char* __restrict__ gate, float fill,
@@ -89,19 +114,20 @@ __global__ void pair_segmin_kernel(const float* __restrict__ dots, int ld, const
     const float* row = dots + static_cast<size_t>(r) * ld;
     for (int c = c0 + lane; c < c1; c += 32) {
       const float d = __fsub_rn(__fadd_rn(a2, nb2[c]), __fmul_rn(2.f, row[c]));
-      best = fminf(best, fmaxf(d, 0.f));
+      best = min_nan(best, max_nan(d, 0.f));
     }
   }
 #pragma unroll
-  for (int o = 16; o > 0; o >>= 1) best = fminf(best, __shfl_xor_sync(0xffffffffu, best, o));
+  for (int o = 16; o > 0; o >>= 1) best = min_nan(best, __shfl_xor_sync(0xffffffffu, best, o));
   if (lane == 0) out[pair] = (r1 > r0 && c1 > c0) ? best : fill;
 }
 
 }  // namespace
 
-int rows_to_planes(const float* src, int rows, int D, __half* hi, __half* lo, int ld, float* sqnorm, cudaStream_t s) {
+int rows_to_planes(const float* src, int rows, int D, __half* hi, __half* lo, int ld, float* sqnorm,
+                   unsigned int* range_flag, cudaStream_t s) {
   if (rows <= 0) return 0;
-  rows_to_planes_kernel<<<(rows * 32 + 255) / 256, 256, 0, s>>>(src, rows, D, hi, lo, ld, sqnorm);
+  rows_to_planes_kernel<<<(rows * 32 + 255) / 256, 256, 0, s>>>(src, rows, D, hi, lo, ld, sqnorm, range_flag);
   B2_CUDA(cudaGetLastError());
   return 0;
 }
@@ -124,11 +150,11 @@ int pair_segmin(const float* dots, int ld, const float* na2, const float* nb2, c
   return 0;
 }
 
-int cosine_normalize_rows(const float* src, int rows, int D, __half* hi, __half* lo, int ld, cudaStream_t s) {
+int cosine_normalize_rows(const float* src, int rows, int D, float eps, __half* hi, __half* lo, int ld, cudaStream_t s) {
   if (rows <= 0) return 0;
   const int threads = 256;
   const int blocks = (rows * 32 + threads - 1) / threads;
-  cosine_normalize_kernel<<<blocks, threads, 0, s>>>(src, rows, D, hi, lo, ld);
+  cosine_normalize_kernel<<<blocks, threads, 0, s>>>(src, rows, D, eps, hi, lo, ld);
   B2_CUDA(cudaGetLastError());
   return 0;
 }

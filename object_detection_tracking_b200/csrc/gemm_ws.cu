@@ -19,11 +19,12 @@ GemmWs::~GemmWs() {
 
 void GemmWs::release() {
   plans.clear();
-  void* ptrs[] = {d_a, d_b, d_dots, d_out, d_bias, d_na2, d_nb2, d_int, d_gate, a_hi, a_lo, b_hi, b_lo};
+  void* ptrs[] = {d_a, d_b, d_dots, d_out, d_bias, d_na2, d_nb2, d_int, d_gate, d_range, a_hi, a_lo, b_hi, b_lo};
   for (void* q : ptrs) if (q) cudaFree(q);
   d_a = d_b = d_dots = d_out = d_bias = d_na2 = d_nb2 = nullptr;
   d_int = nullptr;
   d_gate = nullptr;
+  d_range = nullptr;
   a_hi = a_lo = b_hi = b_lo = nullptr;
 }
 
@@ -36,7 +37,10 @@ int GemmWs::reserve(int device, const GemmNeed& need) {
   const size_t n[] = {need.a, need.b, need.Sp, need.Np, need.Dp, need.out, need.ints, need.gate};
   bool fits = true;
   for (int i = 0; i < 8; ++i) fits = fits && n[i] <= *c[i];
-  if (fits) return 0;
+  if (fits) {
+    B2_CUDA(cudaMemsetAsync(d_range, 0, sizeof(unsigned int), stream));
+    return 0;
+  }
   B2_CUDA(cudaStreamSynchronize(stream));
   release();
   for (int i = 0; i < 8; ++i) *c[i] = std::max<size_t>(n[i] > *c[i] ? n[i] * (transient ? 1 : 2) : *c[i], 1);
@@ -49,6 +53,8 @@ int GemmWs::reserve(int device, const GemmNeed& need) {
   B2_CUDA(cudaMalloc(&d_nb2, cap.Np * 4));
   B2_CUDA(cudaMalloc(&d_int, cap.ints * 4));
   B2_CUDA(cudaMalloc(&d_gate, cap.gate));
+  B2_CUDA(cudaMalloc(&d_range, sizeof(unsigned int)));
+  B2_CUDA(cudaMemsetAsync(d_range, 0, sizeof(unsigned int), stream));
   B2_CUDA(cudaMalloc(&a_hi, cap.Sp * cap.Dp * 2));
   B2_CUDA(cudaMalloc(&a_lo, cap.Sp * cap.Dp * 2));
   B2_CUDA(cudaMalloc(&b_hi, cap.Np * cap.Dp * 2));
@@ -82,6 +88,16 @@ int GemmWs::gemm(int Sp, int Np, int Dp, bool split) {
   return conv_tc_launch(it->second.get(), stream);
 }
 
+int GemmWs::download(float* out, size_t n, const char* who) {
+  unsigned int range = 0;
+  B2_CUDA(cudaMemcpyAsync(out, d_out, sizeof(float) * n, cudaMemcpyDeviceToHost, stream));
+  B2_CUDA(cudaMemcpyAsync(&range, d_range, sizeof(unsigned int), cudaMemcpyDeviceToHost, stream));
+  B2_CUDA(cudaStreamSynchronize(stream));
+  B2_CHECK(range == 0, std::string(who) + ": input outside the fp16-plane range (a finite |x| >= 65520 rounds to inf in "
+                       "the GEMM operand's hi plane); scale the embeddings down");
+  return 0;
+}
+
 namespace {
 
 // b2_cosine_cost / b2_distance_matrix are called once per frame (per cascade level) by the trackers: a call is three
@@ -103,9 +119,10 @@ int on_dist_ws(int device, const std::function<int(GemmWs&)>& run) {
 }
 
 // a [na][D] x b [nb][D] on the workspace, metric 0 cosine / 1 squared euclidean: the distance matrix [na][nb], or with
-// `seg` ([T + 1] offsets of a's rows) the per-segment minimum of the cosine distance [T][nb]
-int distance_run(GemmWs& w, int device, const float* a, int na, const float* b, int nb, int D, int metric, bool split,
-                 const int32_t* seg, int T, float* out) {
+// `seg` ([T + 1] offsets of a's rows) the per-segment minimum of the cosine distance [T][nb].  Cosine rows are divided by
+// max(|x|, eps).
+int distance_run(GemmWs& w, int device, const float* a, int na, const float* b, int nb, int D, int metric, float eps,
+                 bool split, const int32_t* seg, int T, float* out, const char* who) {
   const int Dp = (D + 63) / 64 * 64, Np = (nb + 15) / 16 * 16, Sp = (na + 127) / 128 * 128, rows = seg ? T : na;
   GemmNeed need;
   need.a = static_cast<size_t>(na) * D; need.b = static_cast<size_t>(nb) * D;
@@ -117,19 +134,19 @@ int distance_run(GemmWs& w, int device, const float* a, int na, const float* b, 
   B2_CUDA(cudaMemcpyAsync(w.d_b, b, sizeof(float) * nb * D, cudaMemcpyHostToDevice, st));
   if (seg) B2_CUDA(cudaMemcpyAsync(w.d_int, seg, sizeof(int) * (T + 1), cudaMemcpyHostToDevice, st));
   if (metric == 0) {
-    if (cosine_normalize_rows(w.d_a, na, D, w.a_hi, w.a_lo, Dp, st) || cosine_normalize_rows(w.d_b, nb, D, w.b_hi, w.b_lo, Dp, st))
+    if (cosine_normalize_rows(w.d_a, na, D, eps, w.a_hi, w.a_lo, Dp, st) ||
+        cosine_normalize_rows(w.d_b, nb, D, eps, w.b_hi, w.b_lo, Dp, st))
       return -1;
   } else {
-    if (rows_to_planes(w.d_a, na, D, w.a_hi, w.a_lo, Dp, w.d_na2, st) || rows_to_planes(w.d_b, nb, D, w.b_hi, w.b_lo, Dp, w.d_nb2, st))
+    if (rows_to_planes(w.d_a, na, D, w.a_hi, w.a_lo, Dp, w.d_na2, w.d_range, st) ||
+        rows_to_planes(w.d_b, nb, D, w.b_hi, w.b_lo, Dp, w.d_nb2, w.d_range, st))
       return -1;
   }
   if (w.gemm(Sp, Np, Dp, split)) return -1;
   if (seg ? cosine_segmin(w.d_dots, Np, w.d_int, T, nb, w.d_out, st)
           : distance_finish(w.d_dots, Np, na, nb, metric, w.d_na2, w.d_nb2, w.d_out, st))
     return -1;
-  B2_CUDA(cudaMemcpyAsync(out, w.d_out, sizeof(float) * rows * nb, cudaMemcpyDeviceToHost, st));
-  B2_CUDA(cudaStreamSynchronize(st));
-  return 0;
+  return w.download(out, static_cast<size_t>(rows) * nb, who);
 }
 
 }  // namespace
@@ -151,7 +168,7 @@ int b2_cosine_cost(int device, const float* gallery, const int32_t* seg_offsets,
   B2_CUDA(cudaSetDevice(device));
   const bool split = precision == 1;
   return on_dist_ws(device, [&](GemmWs& w) {
-    return distance_run(w, device, gallery, seg_offsets[T], dets, N, D, 0, split, seg_offsets, T, cost);
+    return distance_run(w, device, gallery, seg_offsets[T], dets, N, D, 0, 0.f, split, seg_offsets, T, cost, "b2_cosine_cost");
   });
 }
 
@@ -164,7 +181,9 @@ int b2_distance_matrix(int device, const float* a, int na, const float* b, int n
   B2_CHECK(D > 0, "b2_distance_matrix: D must be positive");
   B2_CUDA(cudaSetDevice(device));
   const bool split = precision == 1;
-  return on_dist_ws(device, [&](GemmWs& w) { return distance_run(w, device, a, na, b, nb, D, metric, split, nullptr, 0, out); });
+  return on_dist_ws(device, [&](GemmWs& w) {
+    return distance_run(w, device, a, na, b, nb, D, metric, 1e-12f, split, nullptr, 0, out, "b2_distance_matrix");
+  });
 }
 
 }  // extern "C"

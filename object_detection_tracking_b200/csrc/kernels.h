@@ -284,8 +284,9 @@ struct DeformParams {
 int deform_sample_launch(const DeformParams& p, int b0, int n, cudaStream_t s);
 
 // cosine.cu
-int cosine_normalize_rows(const float* src, int rows, int D, __half* hi, __half* lo, int ld, cudaStream_t s);
-int rows_to_planes(const float* src, int rows, int D, __half* hi, __half* lo, int ld, float* sqnorm, cudaStream_t s);
+int cosine_normalize_rows(const float* src, int rows, int D, float eps, __half* hi, __half* lo, int ld, cudaStream_t s);
+int rows_to_planes(const float* src, int rows, int D, __half* hi, __half* lo, int ld, float* sqnorm,
+                   unsigned int* range_flag, cudaStream_t s);
 int distance_finish(const float* dots, int ld, int na, int nb, int metric, const float* na2, const float* nb2, float* out,
                     cudaStream_t s);
 int pair_segmin(const float* dots, int ld, const float* na2, const float* nb2, const int* seg_a, int N, const int* seg_b,

@@ -1,7 +1,8 @@
 // Single-kernel entry points for parity tests and host tools: one conv, one grouped conv, one GroupNorm, one squeeze-excite,
 // one relation module, the deformable sampler and conv, the frame resize, and the element-wise and reduction kernels around
 // the GEMMs (depthwise convs, pools, the BiFPN combine, MBConv's squeeze-excite, OSNet's channel gate, EfficientNet's stem
-// im2col).  Each call owns its device buffers in an Arena, so every return path frees them.
+// im2col), and the distance kernels around the tracker / ReID GEMMs.  Each call owns its device buffers in an Arena, so
+// every return path frees them.
 // The squeeze-excite, relation and deformable-conv calls build a one-block plan with the detector's builders (detplan.h).
 #include <string.h>
 
@@ -636,6 +637,74 @@ int b2_op_stem_im2col(int device, const float* img, int H, int W, int Ho, int Wo
   if (stem_im2col_launch(d_img, 1, H, W, Ho, Wo, pad_t, pad_l, op.hi, op.lo, nullptr)) return -1;
   B2_CUDA(cudaDeviceSynchronize());
   return return_planes(op, op.elems(), out, out_hi, out_lo);
+}
+
+// The distance GEMMs' operand conversion alone: cosine_normalize_rows (normalize != 0) or rows_to_planes.
+int b2_op_distance_operand(int device, const float* x, int rows, int D, int ld, int normalize, float eps, uint16_t* out_hi,
+                           uint16_t* out_lo, float* sqnorm, uint32_t* range_flag) {
+  B2_CHECK(x && out_hi && out_lo, "b2_op_distance_operand: null argument");
+  B2_CHECK(rows >= 1 && D >= 1 && ld >= D && eps >= 0.f, "b2_op_distance_operand: needs rows, D >= 1, ld >= D, eps >= 0");
+  B2_CUDA(cudaSetDevice(device));
+  const size_t n = static_cast<size_t>(rows) * ld;
+  Arena a;
+  __half *hi = a.alloc<__half>(n), *lo = a.alloc<__half>(n);
+  float* d_x = upload_f32(a, x, static_cast<size_t>(rows) * D);
+  float* d_sq = a.alloc<float>(rows);
+  unsigned int* flag = a.alloc<unsigned int>(1);
+  B2_CHECK(hi && lo && d_x && d_sq && flag, "b2_op_distance_operand: out of device memory");
+  if (normalize ? cosine_normalize_rows(d_x, rows, D, eps, hi, lo, ld, nullptr)
+                : rows_to_planes(d_x, rows, D, hi, lo, ld, d_sq, flag, nullptr))
+    return -1;
+  B2_CUDA(cudaDeviceSynchronize());
+  B2_CUDA(cudaMemcpy(out_hi, hi, n * sizeof(__half), cudaMemcpyDeviceToHost));
+  B2_CUDA(cudaMemcpy(out_lo, lo, n * sizeof(__half), cudaMemcpyDeviceToHost));
+  if (sqnorm && !normalize) B2_CUDA(cudaMemcpy(sqnorm, d_sq, rows * sizeof(float), cudaMemcpyDeviceToHost));
+  if (range_flag && !normalize) B2_CUDA(cudaMemcpy(range_flag, flag, sizeof(unsigned int), cudaMemcpyDeviceToHost));
+  return 0;
+}
+
+// The distance GEMMs' epilogues alone, on host-given products: distance_finish (kind 0 cosine, 1 squared euclidean),
+// cosine_segmin (kind 2) or pair_segmin (kind 3).
+int b2_op_distance_epilogue(int device, int kind, const float* dots, int rows, int cols, int ld, const float* na2,
+                            const float* nb2, const int32_t* seg_a, int n_a, const int32_t* seg_b, int n_b,
+                            const uint8_t* gate, float fill, float* out) {
+  B2_CHECK(dots && out, "b2_op_distance_epilogue: null argument");
+  B2_CHECK(kind >= 0 && kind <= 3 && rows >= 1 && cols >= 1 && ld >= cols,
+           "b2_op_distance_epilogue: needs kind 0..3, rows, cols >= 1 and ld >= cols");
+  B2_CHECK((kind != 1 && kind != 3) || (na2 && nb2), "b2_op_distance_epilogue: the euclidean kinds need na2 and nb2");
+  auto segs_ok = [](const int32_t* seg, int n, int limit) {
+    if (!seg || n < 1 || seg[0] < 0) return false;
+    for (int i = 0; i < n; ++i)
+      if (seg[i + 1] < seg[i]) return false;
+    return seg[n] <= limit;
+  };
+  B2_CHECK(kind < 2 || segs_ok(seg_a, n_a, rows), "b2_op_distance_epilogue: seg_a must be n_a + 1 non-decreasing row offsets "
+                                                  "in [0, rows]");
+  B2_CHECK(kind < 3 || segs_ok(seg_b, n_b, cols), "b2_op_distance_epilogue: seg_b must be n_b + 1 non-decreasing column "
+                                                  "offsets in [0, cols]");
+  B2_CUDA(cudaSetDevice(device));
+  const size_t n_out = kind < 2 ? static_cast<size_t>(rows) * cols
+                                : static_cast<size_t>(n_a) * (kind == 2 ? cols : n_b);
+  Arena a;
+  float* d_dots = upload_f32(a, dots, static_cast<size_t>(rows) * ld);
+  float* d_na2 = upload_f32(a, na2, rows);
+  float* d_nb2 = upload_f32(a, nb2, cols);
+  int* d_seg = a.alloc<int>(static_cast<size_t>(n_a) + n_b + 2);
+  uint8_t* d_gate = gate && kind == 3 ? a.alloc<uint8_t>(static_cast<size_t>(n_a) * n_b) : nullptr;
+  float* d_out = a.alloc<float>(n_out);
+  B2_CHECK(d_dots && (!na2 || d_na2) && (!nb2 || d_nb2) && d_seg && (!gate || kind != 3 || d_gate) && d_out,
+           "b2_op_distance_epilogue: out of device memory");
+  if (kind >= 2) B2_CUDA(cudaMemcpy(d_seg, seg_a, (n_a + 1) * sizeof(int), cudaMemcpyHostToDevice));
+  if (kind == 3) B2_CUDA(cudaMemcpy(d_seg + n_a + 1, seg_b, (n_b + 1) * sizeof(int), cudaMemcpyHostToDevice));
+  if (d_gate) B2_CUDA(cudaMemcpy(d_gate, gate, static_cast<size_t>(n_a) * n_b, cudaMemcpyHostToDevice));
+  const int rc = kind < 2    ? distance_finish(d_dots, ld, rows, cols, kind, d_na2, d_nb2, d_out, nullptr)
+                 : kind == 2 ? cosine_segmin(d_dots, ld, d_seg, n_a, cols, d_out, nullptr)
+                             : pair_segmin(d_dots, ld, d_na2, d_nb2, d_seg, n_a, d_seg + n_a + 1, n_b, d_gate, fill, d_out,
+                                           nullptr);
+  if (rc) return -1;
+  B2_CUDA(cudaDeviceSynchronize());
+  B2_CUDA(cudaMemcpy(out, d_out, n_out * sizeof(float), cudaMemcpyDeviceToHost));
+  return 0;
 }
 
 // The resize alone (parity tests): host uint8 [n, src_h, src_w, 3] -> host float32 [n, dst_h, dst_w, 3].

@@ -7,6 +7,7 @@
 // Here: ONE tensor-core GEMM over the concatenated galleries ([Sa,D] x [Sb,D]^T on conv_tc_kernel) and one segmented
 // min kernel; the trajectory distance is plain host code (float64, as the reference).
 #include <math.h>
+#include <stdlib.h>
 #include <string.h>
 
 #include <algorithm>
@@ -36,8 +37,8 @@ extern "C" {
 // Shared body: `a` / `b` are host pointers (a_dev == 0: uploaded first) or device pointers -- b may be PEER memory of
 // another GPU opened through b2_gallery_open: rows_to_planes then reads it over NVLink while converting to the fp16 operand
 // planes, i.e. the "exchange" is the operand load of the GEMM's first stage, no staged copy of the peer gallery exists.
-// Operand rows beyond Sa / Sb (padding up to the plan's shape) hold finite leftovers of earlier calls: they only produce
-// products nobody reads.
+// Operand rows beyond Sa / Sb (padding up to the plan's shape) hold leftovers of earlier calls, NaN or inf included: they
+// only produce products nobody reads.
 static int pair_cost_impl(int device, const float* a, bool a_dev, const int32_t* seg_a, int N, const float* b, bool b_dev,
                           const int32_t* seg_b, int M, int D, const uint8_t* gate, float fill, int precision, float* out) {
   B2_CHECK(N >= 0 && M >= 0 && D > 0, "b2_track_pair_cost: bad argument");
@@ -55,7 +56,9 @@ static int pair_cost_impl(int device, const float* a, bool a_dev, const int32_t*
   const bool split = precision == 1;
   const int Dp = (D + 63) / 64 * 64, Np = (Sb + 15) / 16 * 16, Sp = (Sa + 127) / 128 * 128;
   std::lock_guard<std::mutex> lock(g_pair_mutex);
-  GemmWs& w = g_pair_ws[device];
+  GemmWs own;   // B2_NO_WS=1 (test hook): a private workspace per call, as for b2_distance_matrix
+  own.transient = true;
+  GemmWs& w = getenv("B2_NO_WS") != nullptr ? own : g_pair_ws[device];
   GemmNeed need;
   need.a = a_dev ? 0 : static_cast<size_t>(Sa) * D;
   need.b = b_dev ? 0 : static_cast<size_t>(Sb) * D;
@@ -80,13 +83,12 @@ static int pair_cost_impl(int device, const float* a, bool a_dev, const int32_t*
   B2_CUDA(cudaMemcpyAsync(d_sa, seg_a, sizeof(int) * (N + 1), cudaMemcpyHostToDevice, st));
   B2_CUDA(cudaMemcpyAsync(d_sb, seg_b, sizeof(int) * (M + 1), cudaMemcpyHostToDevice, st));
   if (gate) B2_CUDA(cudaMemcpyAsync(w.d_gate, gate, static_cast<size_t>(N) * M, cudaMemcpyHostToDevice, st));
-  if (rows_to_planes(d_a, Sa, D, w.a_hi, w.a_lo, Dp, w.d_na2, st) || rows_to_planes(d_b, Sb, D, w.b_hi, w.b_lo, Dp, w.d_nb2, st))
+  if (rows_to_planes(d_a, Sa, D, w.a_hi, w.a_lo, Dp, w.d_na2, w.d_range, st) ||
+      rows_to_planes(d_b, Sb, D, w.b_hi, w.b_lo, Dp, w.d_nb2, w.d_range, st))
     return -1;
   if (w.gemm(Sp, Np, Dp, split)) return -1;
   if (pair_segmin(w.d_dots, Np, w.d_na2, w.d_nb2, d_sa, N, d_sb, M, gate ? w.d_gate : nullptr, fill, w.d_out, st)) return -1;
-  B2_CUDA(cudaMemcpyAsync(out, w.d_out, sizeof(float) * N * M, cudaMemcpyDeviceToHost, st));
-  B2_CUDA(cudaStreamSynchronize(st));
-  return 0;
+  return w.download(out, static_cast<size_t>(N) * M, a_dev ? "b2_track_pair_cost_dev" : "b2_track_pair_cost");
 }
 
 int b2_track_pair_cost(int device, const float* a, const int32_t* seg_a, int N, const float* b, const int32_t* seg_b,

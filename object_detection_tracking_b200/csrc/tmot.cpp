@@ -277,6 +277,9 @@ void iou_cost(const TrackList& a, const TrackList& b, std::vector<double>& cost)
   iou_distance(ba.data(), static_cast<int>(a.size()), bb.data(), static_cast<int>(b.size()), cost.data());
 }
 
+// np.maximum(0, d): a NaN distance stays NaN (std::max(0.0, NaN) is 0, a perfect match), and the assignment refuses it
+double clamp0(double d) { return d < 0.0 ? 0.0 : d; }
+
 int embedding_cost(b2_jde* t, const TrackList& pool, const TrackList& dets, std::vector<double>& cost) {   // matching.py:80-94
   const int T = static_cast<int>(pool.size()), N = static_cast<int>(dets.size()), D = t->feat_dim;
   cost.assign(static_cast<size_t>(T) * N, 0.0);
@@ -288,10 +291,10 @@ int embedding_cost(b2_jde* t, const TrackList& pool, const TrackList& dets, std:
     std::vector<int32_t> seg(T + 1);
     for (int r = 0; r <= T; ++r) seg[r] = r;
     if (t->cost_fn(t->cost_user, a.data(), seg.data(), T, b.data(), N, D, c32.data()) != 0) return -1;
-    for (size_t i = 0; i < c32.size(); ++i) cost[i] = std::max(0.0, static_cast<double>(c32[i]));
+    for (size_t i = 0; i < c32.size(); ++i) cost[i] = clamp0(static_cast<double>(c32[i]));
   } else {
     if (b2_distance_matrix(t->device, a.data(), T, b.data(), N, D, 1, t->precision, c32.data()) != 0) return -1;
-    for (size_t i = 0; i < c32.size(); ++i) cost[i] = sqrt(std::max(0.0, static_cast<double>(c32[i])));
+    for (size_t i = 0; i < c32.size(); ++i) cost[i] = sqrt(clamp0(static_cast<double>(c32[i])));
   }
   return 0;
 }
@@ -359,7 +362,7 @@ int b2_tmot_embedding_distance(int device, const float* track_feats, int T, cons
   B2_CHECK(track_feats && det_feats && out, "b2_tmot_embedding_distance: null argument");
   std::vector<float> c32(static_cast<size_t>(T) * N);
   if (b2_distance_matrix(device, track_feats, T, det_feats, N, D, 1, precision, c32.data()) != 0) return -1;
-  for (size_t i = 0; i < c32.size(); ++i) out[i] = sqrt(std::max(0.0, static_cast<double>(c32[i])));
+  for (size_t i = 0; i < c32.size(); ++i) out[i] = sqrt(clamp0(static_cast<double>(c32[i])));
   return 0;
 }
 

@@ -553,6 +553,50 @@ def op_stem_im2col(img, out_hw, pad, split=True, device=0):
     return out, hi, lo
 
 
+def op_distance_operand(x, ld=None, normalize=False, eps=0.0, device=0):
+    """The distance GEMMs' operand conversion through the C ABI -- used by the kernel tests: x [rows, D] fp32 to planes
+    [rows, ld] (ld default D), normalised rows x / max(|x|, eps) or x itself.  Returns (hi, lo, sqnorm, range_flag) with
+    raw uint16 planes; sqnorm and range_flag are None for normalised rows."""
+    lib = _lib.load()
+    x = _f32(x)
+    rows, D = x.shape
+    ld = D if ld is None else int(ld)
+    hi, lo = np.empty((rows, ld), np.uint16), np.empty((rows, ld), np.uint16)
+    sq = None if normalize else np.empty(rows, np.float32)
+    flag = np.zeros(1, np.uint32)
+    _lib.check(lib.b2_op_distance_operand(device, _lib.ptr(x), rows, D, ld, int(bool(normalize)), float(eps),
+                                          _lib.ptr(hi), _lib.ptr(lo), _lib.ptr(sq), _lib.ptr(flag)),
+               "b2_op_distance_operand")
+    return hi, lo, sq, None if normalize else int(flag[0])
+
+
+def op_distance_epilogue(kind, dots, cols=None, na2=None, nb2=None, seg_a=None, seg_b=None, gate=None, fill=0.0,
+                         device=0):
+    """One distance epilogue through the C ABI -- used by the kernel tests: dots [rows, ld] fp32 with the first `cols`
+    columns live (default ld).  kind "cosine" / "euclidean": the [rows, cols] matrix; "cosine_segmin": the [T, cols]
+    per-segment minimum over seg_a [T + 1]; "pair_segmin": the [N, M] block minimum over seg_a [N + 1] and seg_b [M + 1],
+    gate [N, M] (uint8, None = all pairs), fill."""
+    lib = _lib.load()
+    k = {"cosine": 0, "euclidean": 1, "cosine_segmin": 2, "pair_segmin": 3}[kind]
+    dots = _f32(dots)
+    rows, ld = dots.shape
+    cols = ld if cols is None else int(cols)
+    sa = None if seg_a is None else np.ascontiguousarray(seg_a, np.int32)
+    sb = None if seg_b is None else np.ascontiguousarray(seg_b, np.int32)
+    na, nb = (0 if sa is None else len(sa) - 1), (0 if sb is None else len(sb) - 1)
+    g = None if gate is None else np.ascontiguousarray(gate, np.uint8)
+    na2, nb2 = _f32(na2), _f32(nb2)
+    shape = (rows, cols) if k < 2 else (na, cols) if k == 2 else (na, nb)
+    if g is not None:
+        assert g.shape == shape, (g.shape, shape)
+    out = np.empty(shape, np.float32)
+    _lib.check(lib.b2_op_distance_epilogue(device, k, _lib.ptr(dots), rows, cols, ld, _lib.ptr(na2), _lib.ptr(nb2),
+                                           _lib.ptr(sa), na, _lib.ptr(sb), nb, _lib.ptr(g),
+                                           float(fill), _lib.ptr(out)),
+               "b2_op_distance_epilogue")
+    return out
+
+
 def get_new_hw(h, w, size, max_size):
     """nn.py:1548-1560: (neww, newh) of resizeImage for an h x w frame."""
     scale = size * 1.0 / min(h, w)
