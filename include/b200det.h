@@ -102,6 +102,22 @@ typedef struct b2_config_ext2 {
   int32_t partial_class_ids[80];   /* the checkpoint's class ids, each in 1..num_class - 1, no duplicates */
 } b2_config_ext2;
 
+/* Graph options added after b2_config_ext2's layout was fixed.  b2_create_ex3 takes them; b2_create_ex2 builds the graph
+ * with every field 0. */
+typedef struct b2_config_ext3 {
+  int32_t use_att_frcnn_head;      /* --use_att_frcnn_head: the attention branch of the class-specific box head
+                                      (fastrcnn_2fc_head models.py:1064-1089, batch graph :2682-2707), after fc7 / fc,
+                                      the relation modules or the conv head: hidden = hidden + relu(att_trans(sum over the
+                                      7x7 bins of the ROIAlign features)), "fastrcnn/att_trans/{W,b}" [256, fc_head_dim].
+                                      The reference's 3x3 "fastrcnn/attention" conv has one output channel and a softmax
+                                      over that length-1 axis, so its weight is exactly 1 for a finite logit and NaN
+                                      otherwise: an ROI with a non-finite feature gets a NaN sum.  The attention weights
+                                      are only checked at load (finite, 65536 * sum|W| + |b| below FLT_MAX, so a logit of
+                                      finite features stays finite).  Ignored with class_agnostic, whose heads
+                                      (models.py:1126-1170) have no attention branch.  Needs fc_head_dim a power of two
+                                      from 64 to 2048 */
+} b2_config_ext3;
+
 const char* b2_last_error(void);
 int b2_version(void);
 
@@ -111,6 +127,9 @@ int b2_create_ex(b2_ctx** out, int device, const b2_config* cfg, const b2_config
 /* b2_create_ex with the options of b2_config_ext2 as well; ext and ext2 may be NULL (all 0).  Refuses, with the reason,
  * partial class ids outside 1..num_class - 1, duplicates and a count above num_class - 1, before touching the device */
 int b2_create_ex2(b2_ctx** out, int device, const b2_config* cfg, const b2_config_ext* ext, const b2_config_ext2* ext2);
+/* b2_create_ex2 with the options of b2_config_ext3 as well; ext, ext2 and ext3 may be NULL (all 0) */
+int b2_create_ex3(b2_ctx** out, int device, const b2_config* cfg, const b2_config_ext* ext, const b2_config_ext2* ext2,
+                  const b2_config_ext3* ext3);
 void b2_destroy(b2_ctx* ctx);
 
 /* Named fp32 host arrays in the reference's Tensorpack-npz naming ("conv0/W",
@@ -442,6 +461,11 @@ int b2_op_group_conv2d(int device, const float* x, const float* w, const float* 
 int b2_op_relation(int device, const float* h, const float* boxes, const int32_t* count, const float* geo_emb_w,
                    const float* geo_emb_b, const float* geo_conv_w, const float* geo_conv_b, const float* query_w,
                    const float* key_w, const float* output_w, int B, int K, int D, int split, float* out);
+/* The attention box head's pool (use_att_frcnn_head) as the engine runs it: x [M][49][C] (host, fp32, converted to the
+ * engine's planes, the ROIAlign row order), out [M][C] fp32 = the sum over the 49 bins, in bin order, read back from its
+ * planes; a row whose 49 x C values are not all finite is all NaN.  C a multiple of 8 up to 8192; the planes hold sums up
+ * to 65504 in magnitude (the engine's pass fails beyond that, as for every plane output). */
+int b2_op_att_pool(int device, const float* x, int M, int C, int split, float* out);
 /* The deformable conv's bilinear sampler (deformable_conv2d nn.py:1642-1712, deformable_helper.py:42-137) as the engine runs
  * it: x [B][H][W][C] (host, fp32, converted to the engine's planes), offsets [B][ceil(H/2)][ceil(W/2)][18] (channel 2k the
  * y and 2k+1 the x offset of tap k, per image).  out [B][ceil(H/2)][ceil(W/2)][9][C]: the sampled operand read back from

@@ -36,6 +36,10 @@ class B2ConfigExt2(ctypes.Structure):
     _fields_ = [("num_partial_classes", c_int32), ("partial_class_ids", c_int32 * 80)]
 
 
+class B2ConfigExt3(ctypes.Structure):
+    _fields_ = [("use_att_frcnn_head", c_int32)]
+
+
 class B2EffdetConfig(ctypes.Structure):
     _fields_ = [
         ("image_h", c_int32), ("image_w", c_int32), ("min_level", c_int32), ("max_level", c_int32),
@@ -62,6 +66,8 @@ SYMBOLS = [
     ("b2_create", c_int, [POINTER(c_void_p), c_int, POINTER(B2Config)]),
     ("b2_create_ex", c_int, [POINTER(c_void_p), c_int, POINTER(B2Config), POINTER(B2ConfigExt)]),
     ("b2_create_ex2", c_int, [POINTER(c_void_p), c_int, POINTER(B2Config), POINTER(B2ConfigExt), POINTER(B2ConfigExt2)]),
+    ("b2_create_ex3", c_int, [POINTER(c_void_p), c_int, POINTER(B2Config), POINTER(B2ConfigExt), POINTER(B2ConfigExt2),
+                              POINTER(B2ConfigExt3)]),
     ("b2_destroy", None, [c_void_p]),
     ("b2_load_weights", c_int, [c_void_p, POINTER(c_char_p), POINTER(c_void_p), POINTER(c_int64), c_int]),
     ("b2_detect", c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int]),
@@ -139,6 +145,7 @@ SYMBOLS = [
     ("b2_op_squeeze_excite", c_int, [c_int] + [c_void_p] * 6 + [c_int] * 6 + [c_void_p, c_void_p]),
     ("b2_op_group_conv2d", c_int, [c_int, c_void_p, c_void_p, c_void_p, c_void_p] + [c_int] * 16 + [c_void_p]),
     ("b2_op_relation", c_int, [c_int] + [c_void_p] * 10 + [c_int] * 4 + [c_void_p]),
+    ("b2_op_att_pool", c_int, [c_int, c_void_p, c_int, c_int, c_int, c_void_p]),
     ("b2_op_deform_sample", c_int, [c_int, c_void_p, c_void_p] + [c_int] * 5 + [c_void_p]),
     ("b2_op_deform_conv2d", c_int, [c_int] + [c_void_p] * 4 + [c_int] * 7 + [c_void_p, c_void_p]),
     ("b2_op_depthwise", c_int, [c_int] + [c_void_p] * 3 + [c_int] * 13 + [c_void_p] * 3),
@@ -253,4 +260,11 @@ def make_config_ext2(cfg) -> B2ConfigExt2:
     e.num_partial_classes = len(ids)
     for i, v in enumerate(ids):
         e.partial_class_ids[i] = int(v)
+    return e
+
+
+def make_config_ext3(cfg) -> B2ConfigExt3:
+    """The options of the namespace that b2_config_ext3 carries."""
+    e = B2ConfigExt3()
+    e.use_att_frcnn_head = int(bool(getattr(cfg, "use_att_frcnn_head", False)))
     return e

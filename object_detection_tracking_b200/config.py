@@ -56,6 +56,9 @@ _DEFAULTS = dict(
     use_partial_classes=False,         # --use_partial_classes (obj_detect_tracking.py:233-239): a COCO-81 checkpoint whose
                                        # box head keeps only partial_classes (models.py:807-828); labels become 1..C
     partial_classes=None,              # class names, in output-label order; None = the keys of coco_obj_to_actev_obj
+    use_att_frcnn_head=False,          # --use_att_frcnn_head (obj_detect_tracking.py:197-199): hidden + relu(att_trans(sum
+                                       # of the ROI's 49 cells)) in the class-specific box head (models.py:1064-1089); the
+                                       # class-agnostic heads have no attention branch (models.py:1126-1170)
     is_efficientdet=False,
 )
 

@@ -1,4 +1,5 @@
 // The detector plan's builders and weight loader (see detplan.h).
+#include <float.h>
 #include <math.h>
 #include <string.h>
 
@@ -294,6 +295,57 @@ int add_relation(DetPlan& p, const std::string& name, int B, int K, int D, const
   return 0;
 }
 
+// The attention branch of fastrcnn_2fc_head (models.py:1064-1089).  Steps:
+//   att_pool    the sum over the 49 bins of each ROI's raw ROIAlign features (att_head.cu: why the 3x3 "attention" conv and
+//               its length-1 softmax reduce to that sum)
+//   att_trans   dense C -> D + bias + ReLU (a plain [C, D] kernel over the channel vector)
+//   att_sum     out = att * 1 + hidden through the squeeze-excite apply path with a [1][D] gate of ones and no ReLU: in
+//               fp32 exactly relu(att_trans) + hidden, the reference's order (ReLU before the sum), which conv_tc's
+//               epilogue (bias, residual, activation) does not have
+// Each row depends on its own ROI only, so a batch's rows are those of its images alone.
+int add_att_head(DetPlan& p, const Planes& roi, int C, const Planes& hidden, const Planes& pooled, const Planes& att,
+                 const Planes& out) {
+  const int M = hidden.W, D = hidden.C;
+  B2_CHECK(D >= 64 && D <= 2048 && (D & (D - 1)) == 0,
+           "b2_create: use_att_frcnn_head needs fc_head_dim a power of two from 64 to 2048");
+  B2_CHECK(pooled.W == M && pooled.C == C && att.W == M && att.C == D && out.W == M && out.C == D,
+           "b2_create: attention head rows do not match the box head");
+  float* ones = p.arena.alloc<float>(D);
+  B2_CHECK(ones, "out of device memory (attention head)");
+  const std::vector<float> h_ones(D, 1.f);
+  B2_CUDA(cudaMemcpy(ones, h_ones.data(), D * sizeof(float), cudaMemcpyHostToDevice));
+  p.att_channels = C;
+  const double esz = p.split ? 4.0 : 2.0;
+  const std::string rows = " [" + std::to_string(M) + "x";
+  Step& sp = add_batch_step(p, 5, kStepAttPool, "fastrcnn/att_pool" + rows + "49x" + std::to_string(C) + "]",
+                            [roi, M, C, pooled, flag = p.range_flag](int, int, cudaStream_t st) {
+                              return att_pool_launch(roi.hi, roi.lo, M, C, pooled.hi, pooled.lo, flag, st);
+                            });
+  sp.bytes = static_cast<double>(M) * 49 * C * esz + static_cast<double>(M) * C * esz;
+  sp.flops = static_cast<double>(M) * 48 * C;
+  ConvDesc d = conv_desc(1, D);
+  d.relu = 1;
+  add_conv(p, 5, "fastrcnn/att_trans", pooled, d, kBias, att, nullptr, kDense);
+  GnParams q;
+  memset(&q, 0, sizeof(q));
+  q.x_hi = att.hi; q.x_lo = att.lo; q.y_hi = out.hi; q.y_lo = out.lo;
+  q.r_hi = hidden.hi; q.r_lo = hidden.lo;
+  q.B = 1; q.H = 1; q.W = M; q.C = D;
+  q.pitch_H = 1; q.pitch_W = M; q.ld = D;
+  q.res_H = 1; q.res_W = M; q.res_ld = D;
+  q.gate = ones;
+  q.chunks = gn_chunks(1, M, D);
+  q.range_flag = p.range_flag;
+  Step& ss = add_batch_step(p, 5, kStepAttSum, "fastrcnn/att_sum" + rows + std::to_string(D) + " +res]",
+                            [q](int, int, cudaStream_t st) { return se_apply_launch(q, st); });
+  ss.bytes = 3.0 * M * D * esz;
+  ss.flops = static_cast<double>(M) * D;
+  p.stages.planes("att_pool", pooled);
+  p.stages.planes("att_trans", att);
+  p.stages.planes("att_sum", out);
+  return 0;
+}
+
 // The deformable conv2 (nn.py:470-486, deformable_conv2d nn.py:1642-1712).  Steps:
 //   conv2_offset   the offsets, fp32 [B][Ho][Wo][kDeformOffsetLd]: the reference's 3x3 SAME stride-1 conv (bias, no norm,
 //                  no activation) is read at the even centres only, so it runs as a 3x3 stride-2 conv with pad 1 top / left
@@ -471,6 +523,25 @@ int load_rel(const RelOp* R, const WeightSet& ws, cudaStream_t st) {
   return relation_upload_geo(ew, eb, cw, cb, R->geo, st);
 }
 
+// fastrcnn/attention/{W,b} [3,3,C,1], [1] (models.py:1075-1077) are never computed with (att_head.cu); their only use is
+// this check, the condition that keeps every logit of finite fp16-plane features (|x| < 65536) finite, and so its
+// length-1 softmax exactly 1
+int load_att(int C, const WeightSet& ws) {
+  const float* w = ws.get("fastrcnn/attention/W", 9 * static_cast<int64_t>(C));
+  const float* b = ws.get("fastrcnn/attention/b", 1);
+  if (!w || !b) return -1;
+  double s = 0.0;
+  for (int i = 0; i < 9 * C; ++i) {
+    B2_CHECK(std::isfinite(w[i]), "attention head: fastrcnn/attention/W not finite");
+    s += fabs(static_cast<double>(w[i]));
+  }
+  B2_CHECK(std::isfinite(b[0]), "attention head: fastrcnn/attention/b not finite");
+  B2_CHECK(65536.0 * s + fabs(static_cast<double>(b[0])) < static_cast<double>(FLT_MAX),
+           "attention head: fastrcnn/attention/W too large: 65536 * sum|W| + |b| reaches FLT_MAX, so a logit of finite "
+           "features could overflow");
+  return 0;
+}
+
 int load_layer(const ConvLayer* L, const WeightSet& ws, int num_class, const int* partial_ids, int num_partial,
                cudaStream_t st) {
   if (L->layout == kRuntime) return 0;   // written by the pass itself
@@ -627,6 +698,7 @@ int load_weights(const DetPlan& p, const WeightSet& ws, int num_class, cudaStrea
     if (load_se(S.get(), ws, st)) return -1;
   for (auto& R : p.rels)
     if (load_rel(R.get(), ws, st)) return -1;
+  if (p.att_channels > 0 && load_att(p.att_channels, ws)) return -1;
   return 0;
 }
 

@@ -60,7 +60,8 @@ enum ConvAffine { kNoAffine, kBatchNorm, kBias };
   X(kStepRoialignFinal, 7, "roialign_final") X(kStepRoialignMask, 8, "roialign_mask")                            \
   X(kStepMaskSelect, 9, "mask_select") X(kStepGnStats, 10, "gn_stats") X(kStepGnApply, 11, "gn_apply")            \
   X(kStepGnRoi, 12, "gn_roi") X(kStepSeSqueeze, 13, "se_squeeze") X(kStepSeExcite, 14, "se_excite")               \
-  X(kStepSeApply, 15, "se_apply") X(kStepRelationAttend, 16, "relation_attend") X(kStepDeformSample, 17, "deform_sample")
+  X(kStepSeApply, 15, "se_apply") X(kStepRelationAttend, 16, "relation_attend") X(kStepDeformSample, 17, "deform_sample") \
+  X(kStepAttPool, 18, "att_pool") X(kStepAttSum, 19, "att_sum")
 enum StepKind {
 #define B2_STEP_KIND_VALUE(e, v, n) e = v,
   B2_STEP_KINDS(B2_STEP_KIND_VALUE)
@@ -84,6 +85,7 @@ struct DetPlan {
   std::vector<std::unique_ptr<GnOp>> gns;
   std::vector<std::unique_ptr<SeOp>> ses;
   std::vector<std::unique_ptr<RelOp>> rels;
+  int att_channels = 0;    // ROI channels of the attention box head (add_att_head); 0 = none
   std::vector<Step> steps;
   StageMap stages;
   // the scratch all relation modules share: query|key [Mpad][2D] fp32, P [B][16K][Kp], P.V = the output_linear operand
@@ -139,6 +141,11 @@ int add_se(DetPlan& p, int phase, const std::string& name, const Planes& buf, co
 // [B][K][4] and `count` [B] on the device: out = h + output_linear(P . h).
 int add_relation(DetPlan& p, const std::string& name, int B, int K, int D, const float* boxes, const int* count,
                  const Planes& h, const Planes& out);
+// The attention branch of the class-specific box head (use_att_frcnn_head) over the head rows `hidden` ([M][D] rows):
+// out = hidden + relu(att_trans(sum over the 49 bins of roi)), roi the ROIAlign planes [M][49][C]; `pooled` ([M][C]) and
+// `att` ([M][D]) are its intermediate rows.
+int add_att_head(DetPlan& p, const Planes& roi, int C, const Planes& hidden, const Planes& pooled, const Planes& att,
+                 const Planes& out);
 // The deformable conv2 of block `name` from conv1's output `in` into `out` ([B][ceil(H/2)][ceil(W/2)][in.C]).
 int add_deform(DetPlan& p, const std::string& name, const Planes& in, const Planes& out);
 
@@ -156,7 +163,8 @@ int add_bottleneck(DetPlan& p, const std::string& name, const Planes& x, int str
 
 // The full-batch tensor-core plan of every layer and, with dual, each forked layer's per-part plans (conv_impl 0 only).
 int plan_layers(DetPlan& p, int num_sms);
-// Every layer, GroupNorm, squeeze-excite and relation module of the plan from the checkpoint `ws`; num_class is the
+// Every layer, GroupNorm, squeeze-excite and relation module of the plan from the checkpoint `ws`, and the attention head's
+// weight check; num_class is the
 // checkpoint's class count of the fused box-head outputs.  With num_partial > 0 those outputs keep the class-0 column and
 // the columns of partial_ids[0 .. num_partial), in that order (use_partial_classes).
 int load_weights(const DetPlan& p, const WeightSet& ws, int num_class, cudaStream_t st, const int* partial_ids = nullptr,

@@ -101,6 +101,7 @@ struct b2_ctx {
   b2_config cfg;
   b2_config_ext ext;       // options appended after b2_config's layout was fixed (b2_create_ex)
   b2_config_ext2 ext2;     // and after b2_config_ext's (b2_create_ex2)
+  b2_config_ext3 ext3;     // and after b2_config_ext2's (b2_create_ex3)
   int device = 0, num_sms = 132;
   cudaStream_t stream = nullptr;
   // geometry
@@ -128,6 +129,7 @@ struct b2_ctx {
   Planes roi_feat, fc6, fc7;        // fc6 / fc7: the M = B * rpn_topk head rows (DetPlan::alloc_rows)
   Planes head_a, head_b;           // conv box head (cfg.conv_head_dim > 0): [M][7][7][conv_head_dim] ping-pong
   Planes rm1, rm2;                 // relation modules (cfg.add_relation_nn): their sums
+  Planes att_pool, att, att_sum;   // attention head (ext3.use_att_frcnn_head): bin sums [M][256], relu(att_trans), the sum
   float* head_logits = nullptr;
   float* box_feat = nullptr;
   float* box_feat_pooled = nullptr;
@@ -425,6 +427,18 @@ int build_plan(b2_ctx* c) {
   Planes rf = c->roi_feat; rf.W = M;
   ConvDesc fc = conv_desc(1, dim);   // fc6 / fc7 / the conv head's fc: dense + bias + ReLU
   fc.relu = 1;
+  // use_att_frcnn_head (models.py:1064-1089): the outputs read hidden + relu(att_trans(the bin sums of the raw ROIAlign
+  // features)), after the conv head or the relation modules; the class-agnostic heads (models.py:1126-1170) have no
+  // attention branch
+  const bool att = c->ext3.use_att_frcnn_head != 0 && !cfg.class_agnostic;
+  if (att)
+    B2_CHECK(P.alloc_rows(c->att_pool, M, nc) && P.alloc_rows(c->att, M, dim) && P.alloc_rows(c->att_sum, M, dim),
+             "alloc attention head");
+  Planes head_in;   // the rows fastrcnn/outputs reads
+  auto attend = [&](const Planes& hidden) {
+    head_in = att ? c->att_sum : hidden;
+    return att ? add_att_head(P, c->roi_feat, nc, hidden, c->att_pool, c->att, c->att_sum) : 0;
+  };
   if (hd > 0) {
     // conv_frcnn_head (models.py:1110-1125), use_conv_frcnn_head: 4 x [conv 3x3 SAME + bias + ReLU, then GroupNorm per ROI
     // if use_gn] on the [M][7][7] ROI maps (the ROIAlign rows are already (y*7+x)*256+c per ROI: M small images, as in the
@@ -449,7 +463,8 @@ int build_plan(b2_ctx* c) {
     Planes flat = cur_h; flat.B = 1; flat.H = 1; flat.W = M; flat.C = 49 * hd;
     const Planes& f = c->fc6;
     add_conv(P, 5, "fastrcnn/fc", flat, fc, kBias, f, nullptr, kFc6);
-    add_conv_f32(P, 5, "fastrcnn/outputs", f, conv_desc(1, nout), kBias, c->head_logits, ldo, kHeadOut);
+    if (attend(f)) return -1;
+    add_conv_f32(P, 5, "fastrcnn/outputs", head_in, conv_desc(1, nout), kBias, c->head_logits, ldo, kHeadOut);
     P.stages.planes("fc", f);
   } else {
     const Planes &f6 = c->fc6, &f7 = c->fc7;
@@ -466,7 +481,8 @@ int build_plan(b2_ctx* c) {
     if (rel && add_relation(P, "fastrcnn/RM_r1", B, K, dim, rp.prop_boxes, rp.prop_count, f6, h1)) return -1;
     add_conv(P, 5, "fastrcnn/fc7", h1, fc, kBias, f7, nullptr, kDense);
     if (rel && add_relation(P, "fastrcnn/RM_r2", B, K, dim, rp.prop_boxes, rp.prop_count, f7, h2)) return -1;
-    add_conv_f32(P, 5, "fastrcnn/outputs", h2, conv_desc(1, nout), kBias, c->head_logits, ldo, kHeadOut);
+    if (attend(h2)) return -1;
+    add_conv_f32(P, 5, "fastrcnn/outputs", head_in, conv_desc(1, nout), kBias, c->head_logits, ldo, kHeadOut);
     P.stages.planes("fc6", f6);
     P.stages.planes("fc7", f7);
     if (rel) {
@@ -617,6 +633,11 @@ int b2_create_ex(b2_ctx** out, int device, const b2_config* cfg, const b2_config
 }
 
 int b2_create_ex2(b2_ctx** out, int device, const b2_config* cfg, const b2_config_ext* ext, const b2_config_ext2* ext2) {
+  return b2_create_ex3(out, device, cfg, ext, ext2, nullptr);
+}
+
+int b2_create_ex3(b2_ctx** out, int device, const b2_config* cfg, const b2_config_ext* ext, const b2_config_ext2* ext2,
+                  const b2_config_ext3* ext3) {
   B2_CHECK(out && cfg, "b2_create: null argument");
   *out = nullptr;
   std::unique_ptr<b2_ctx> c(new b2_ctx());
@@ -625,6 +646,8 @@ int b2_create_ex2(b2_ctx** out, int device, const b2_config* cfg, const b2_confi
   if (ext) c->ext = *ext;
   memset(&c->ext2, 0, sizeof(c->ext2));
   if (ext2) c->ext2 = *ext2;
+  memset(&c->ext3, 0, sizeof(c->ext3));
+  if (ext3) c->ext3 = *ext3;
   const int np = c->ext2.num_partial_classes;
   B2_CHECK(np >= 0 && np <= cfg->num_class - 1 && np <= 80,
            "b2_create: num_partial_classes must be 0 (off) or 1 .. min(num_class - 1, 80) (num_class " +

@@ -268,6 +268,12 @@ void relation_pack_qk(const float* wq, const float* wk, int D, std::vector<float
 int relation_upload_geo(const float* emb_w, const float* emb_b, const float* conv_w, const float* conv_b, float* dst,
                         cudaStream_t s);
 
+// att_head.cu -- the attention box head's pool (use_att_frcnn_head, models.py:1064-1089): ROIAlign rows [M][49][C] planes
+// -> [M][C] planes, the sum over the 49 bins in bin order; a ROI with a non-finite input gets an all-NaN row.  A finite
+// sum beyond +-65504 ORs *range_flag (nullptr = not monitored)
+int att_pool_launch(const __half* in_hi, const __half* in_lo, int M, int C, __half* out_hi, __half* out_lo,
+                    unsigned int* range_flag, cudaStream_t s);
+
 // deform.cu -- the bilinear sampler of a deformable conv2 (use_deformable, deformable_helper.py:42-137): conv1's output
 // sampled at tap k's base + offset around (2i, 2j), clamped to the map, into the operand of a 1x1 conv with K = 9 * C
 constexpr int kDeformOffsetLd = 32;   // row stride of the fp32 offsets: the offset conv's 18 outputs padded to Cout_pad

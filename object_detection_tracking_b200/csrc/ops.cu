@@ -1,7 +1,7 @@
 // Single-kernel entry points for parity tests and host tools: one conv, one grouped conv, one GroupNorm, one squeeze-excite,
-// one relation module, the deformable sampler and conv, the frame resize, and the element-wise and reduction kernels around
-// the GEMMs (depthwise convs, pools, the BiFPN combine, MBConv's squeeze-excite, OSNet's channel gate, EfficientNet's stem
-// im2col), and the distance kernels around the tracker / ReID GEMMs.  Each call owns its device buffers in an Arena, so
+// one relation module, the attention head's pool, the deformable sampler and conv, the frame resize, and the element-wise
+// and reduction kernels around the GEMMs (depthwise convs, pools, the BiFPN combine, MBConv's squeeze-excite, OSNet's
+// channel gate, EfficientNet's stem im2col), and the distance kernels around the tracker / ReID GEMMs.  Each call owns its device buffers in an Arena, so
 // every return path frees them.
 // The squeeze-excite, relation and deformable-conv calls build a one-block plan with the detector's builders (detplan.h).
 #include <string.h>
@@ -377,6 +377,21 @@ int b2_op_relation(int device, const float* h, const float* boxes, const int32_t
   ws.add("rm/output_linear/W", output_w, static_cast<int64_t>(kRelGroups) * D * D);
   if (run_plan(p, device, ws)) return -1;
   return download_planes(op.hi, op.lo, static_cast<size_t>(M) * D, out, nullptr);
+}
+
+// The attention head's pool alone (att_head.cu): fp32 [M][49][C] in, converted to the engine's planes; the pooled planes
+// joined to fp32 out.
+int b2_op_att_pool(int device, const float* x, int M, int C, int split, float* out) {
+  B2_CHECK(x && out, "b2_op_att_pool: null argument");
+  B2_CHECK(M >= 1 && C >= 8 && C % 8 == 0 && C <= 8192, "b2_op_att_pool: needs M >= 1 and C a multiple of 8 up to 8192");
+  B2_CUDA(cudaSetDevice(device));
+  Arena a;
+  const Planes in = a.planes(1, 1, M, 49 * C, split != 0), o = a.planes(1, 1, M, C, split != 0);
+  B2_CHECK(in.hi && o.hi, "b2_op_att_pool: out of device memory");
+  if (upload_planes(x, in.hi, in.lo, static_cast<size_t>(M) * 49 * C, nullptr)) return -1;
+  if (att_pool_launch(in.hi, in.lo, M, C, o.hi, o.lo, nullptr, nullptr)) return -1;
+  B2_CUDA(cudaDeviceSynchronize());
+  return download_planes(o.hi, o.lo, static_cast<size_t>(M) * C, out, nullptr);
 }
 
 // The deformable sampler alone: fp32 x and offsets in, the sampled operand's planes joined to fp32 out.

@@ -25,9 +25,11 @@ class Detector:
                                    multi_semantics, accum_chunk)
         self._ext = _lib.make_config_ext(self.cfg)
         self._ext2 = _lib.make_config_ext2(self.cfg)
+        self._ext3 = _lib.make_config_ext3(self.cfg)
         self._ctx = c_void_p(0)
-        _lib.check(self.lib.b2_create_ex2(ctypes.byref(self._ctx), self.device, ctypes.byref(self._c),
-                                          ctypes.byref(self._ext), ctypes.byref(self._ext2)), "b2_create")
+        _lib.check(self.lib.b2_create_ex3(ctypes.byref(self._ctx), self.device, ctypes.byref(self._c),
+                                          ctypes.byref(self._ext), ctypes.byref(self._ext2), ctypes.byref(self._ext3)),
+                   "b2_create")
         self.R = int(self.cfg.result_per_im)
         self.C = int(self.cfg.fpn_num_channel)
         self._pinned = None
@@ -594,6 +596,19 @@ def op_distance_epilogue(kind, dots, cols=None, na2=None, nb2=None, seg_a=None, 
                                            _lib.ptr(sa), na, _lib.ptr(sb), nb, _lib.ptr(g),
                                            float(fill), _lib.ptr(out)),
                "b2_op_distance_epilogue")
+    return out
+
+
+def op_att_pool(x, split=True, device=0) -> np.ndarray:
+    """The attention box head's pool (use_att_frcnn_head, models.py:1064-1089) through the C ABI -- used by the kernel
+    tests: x [M, 49, C] ROIAlign rows (bin-major, as the engine stores them), converted to the engine's planes.  Returns
+    [M, C] float32, the sum over the 49 bins read back from its planes; a row with a non-finite input is all NaN."""
+    lib = _lib.load()
+    x = np.ascontiguousarray(x, dtype=np.float32)
+    M, nb, C = x.shape
+    assert nb == 49, x.shape
+    out = np.empty((M, C), dtype=np.float32)
+    _lib.check(lib.b2_op_att_pool(device, _lib.ptr(x), M, C, int(split), _lib.ptr(out)), "b2_op_att_pool")
     return out
 
 

@@ -16,6 +16,7 @@ weights.  Names follow the Tensorpack-npz convention the reference loads
   use_se: group{0..3}/block{i}/fc1/{W,b}, fc2/{W,b} (squeeze-excite dense layers)
   use_resnext: conv1 / conv2 at twice the width, conv2/W [3, 3, 2*ch/32, 2*ch] (32 groups), no fc1 / fc2
   add_relation_nn: fastrcnn/RM_r{1,2}/{geo_emb/{W,b}, geo_conv/{W,b}, query_linear/W, key_linear/W, output_linear/W}
+  use_att_frcnn_head (class-specific head): fastrcnn/attention/{W,b} [3, 3, 256, 1], [1], fastrcnn/att_trans/{W,b} [256, dim]
   use_deformable: <deformable block>/conv2_offset/{W,b} [3, 3, C, 18], [18]; that block's conv2 has no bn / gn
   use_basic_block: conv1/W [3, 3, cin, ch], conv2/W [3, 3, ch, ch], no conv3; convshortcut [1, 1, cin, ch] where cin != ch;
                    laterals read 64 / 128 / 256 / 512 channels
@@ -162,6 +163,17 @@ def synth_weights(cfg, seed: int = 1234) -> dict:
         # taps clamped (test_deform_cpu states the thresholds)
         w[p + "/conv2_offset/W"] = _conv_w(rng, 3, c, 18)
         w[p + "/conv2_offset/b"] = (rng.standard_normal(18) * 0.5).astype(np.float32)
+    # The attention branch draws from a stream of its own, so every other array of a seed is the same with and without it.
+    if _use_att(cfg):                                # fastrcnn_2fc_head's attention branch (models.py:1064-1089)
+        arng = np.random.default_rng([seed, 0x617474])
+        nc = cfg.fpn_num_channel
+        # the attention conv's values never change a finite result (its softmax runs over one channel); they only have to
+        # pass the load check.  att_trans reads the sum of 49 cells: a fan-in gain of 1 over 49 * sqrt(256) makes its
+        # output about the size of one mean cell, about half of hidden's norm, with about half of its units active
+        w["fastrcnn/attention/W"] = (arng.standard_normal((3, 3, nc, 1)) * 0.05).astype(np.float32)
+        w["fastrcnn/attention/b"] = (arng.standard_normal(1) * 0.1).astype(np.float32)
+        w["fastrcnn/att_trans/W"] = (arng.standard_normal((nc, dim)) * (1.0 / (49.0 * np.sqrt(nc)))).astype(np.float32)
+        w["fastrcnn/att_trans/b"] = (arng.standard_normal(dim) * 0.1).astype(np.float32)
     return w
 
 
@@ -205,6 +217,20 @@ def _relation_shapes(cfg):
                    p + "geo_conv/b": (16,), p + "query_linear/W": (dim, dim), p + "key_linear/W": (dim, dim),
                    p + "output_linear/W": (16 * dim, dim)})
     return sh
+
+
+def _use_att(cfg):
+    """use_att_frcnn_head adds the attention branch to the class-specific heads only: fastrcnn_2fc_head_class_agnostic has
+    none (models.py:1126-1170)."""
+    return getattr(cfg, "use_att_frcnn_head", False) and not cfg.use_frcnn_class_agnostic
+
+
+def _att_shapes(cfg):
+    """Name -> shape of the attention branch's variables (models.py:1075-1088): the 3x3 one-channel conv and the dense
+    att_trans over the channel vector."""
+    nc, dim = cfg.fpn_num_channel, cfg.fpn_frcnn_fc_head_dim
+    return {"fastrcnn/attention/W": (3, 3, nc, 1), "fastrcnn/attention/b": (1,), "fastrcnn/att_trans/W": (nc, dim),
+            "fastrcnn/att_trans/b": (dim,)}
 
 
 def deformable_blocks(cfg):
@@ -328,6 +354,8 @@ def frcnn_weight_shapes(cfg) -> dict:
         sh[name + "/b"] = (fout,)
     if _use_relation(cfg):                           # fastrcnn_2fc_head(_class_agnostic) (models.py:1044-1054, 1139-1148)
         sh.update(_relation_shapes(cfg))
+    if _use_att(cfg):                                # fastrcnn_2fc_head (models.py:1064-1089), with either hidden variant
+        sh.update(_att_shapes(cfg))
     if getattr(cfg, "add_mask", False):              # models.py:1173-1199; Conv2DTranspose kernel is [kh, kw, out, in]
         md = getattr(cfg, "mrcnn_head_dim", 256)
         for k in range(4):
