@@ -524,6 +524,15 @@ int b2_op_channel_gate(int device, const float* s, const float* w1, const float*
  * img[2y - pad_t + r][2x - pad_l + s][c] (0 outside the image), columns 27..63 zero. */
 int b2_op_stem_im2col(int device, const float* img, int H, int W, int Ho, int Wo, int pad_t, int pad_l, int split,
                       float* out, uint16_t* out_hi, uint16_t* out_lo);
+/* The ResNet stems' operand packs: frames img [B][H][W][3] (uint8 when is_u8, else float32) normalised and packed into
+ * out [B][Hu][Wu][L] with P the normalised frame, zero outside it:
+ *   layout 0, the detector (L = 16, any float32 allowed): lane ry*6 + sx*3 + c of pixel (y, x) = P[2y + ry - 3][2x + sx - 3][c],
+ *     lanes 12..15 zero; P = (x * (1/255) - mean) / std with BGR constants;
+ *   layout 1, the ReID engines (L = 64, uint8 only): lane s*12 + ry*6 + sx*3 + c of pixel (y, q) =
+ *     P[2y + ry - 3][2(q + s) + sx - 3][c], lanes 48..63 zero; P = (x / 255 - mean) / std with RGB constants.
+ * out is the operand joined to fp32, out_hi / out_lo (may be NULL; out_lo unwritten in fp16 precision) its raw planes. */
+int b2_op_stem_pack(int device, const void* img, int is_u8, int B, int H, int W, int layout, int Hu, int Wu, int split,
+                    float* out, uint16_t* out_hi, uint16_t* out_lo);
 
 /* The distance kernels of b2_cosine_cost, b2_distance_matrix, b2_track_pair_cost and b2_tmot_embedding_distance, one at a
  * time.  b2_op_distance_operand converts x [rows][D] (host fp32) into the GEMM's operand planes out_hi / out_lo

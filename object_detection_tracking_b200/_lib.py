@@ -154,6 +154,7 @@ SYMBOLS = [
     ("b2_op_mbconv_se", c_int, [c_int] + [c_void_p] * 6 + [c_int] * 7 + [c_void_p] * 4),
     ("b2_op_channel_gate", c_int, [c_int] + [c_void_p] * 6 + [c_int] * 6 + [c_void_p] * 4),
     ("b2_op_stem_im2col", c_int, [c_int, c_void_p] + [c_int] * 7 + [c_void_p] * 3),
+    ("b2_op_stem_pack", c_int, [c_int, c_void_p] + [c_int] * 8 + [c_void_p] * 3),
     ("b2_op_distance_operand", c_int, [c_int, c_void_p] + [c_int] * 4 + [c_float] + [c_void_p] * 4),
     ("b2_op_distance_epilogue", c_int, [c_int, c_int, c_void_p] + [c_int] * 3 + [c_void_p] * 3 + [c_int, c_void_p, c_int,
                                                                                                 c_void_p, c_float, c_void_p]),

@@ -10,12 +10,13 @@ namespace b2 {
 // stem.cu
 int f32_to_planes(const float* src, __half* hi, __half* lo, size_t n, cudaStream_t s);
 int planes_to_f32(const __half* hi, const __half* lo, float* dst, size_t n, cudaStream_t s);
-// norm_mode 0: detector (x * (1/255) - mean) / std with BGR constants (models.py:345-355);
-// norm_mode 1: torchvision ToTensor + Normalize (x / 255 - mean) / std with RGB constants (feature_extractor.py:190-196)
 int resize_u8_launch(const uint8_t* src, int B, int sh, int sw, float* dst, int dh, int dw, cudaStream_t s);
-int stem_pack_launch(const void* img, int is_u8, int B, int H, int W, __half* out_hi, __half* out_lo, int Hu, int Wu,
-                     int norm_mode, cudaStream_t s);
-// compact operand of the detector stem: [B][Hu][Wv = Wu + 3][16] (stem.cu)
+// operand of the ReID stems: [B][Hu][Wu][64] from RGB uint8 crops, torchvision ToTensor + Normalize (x / 255 - mean) / std
+// with RGB constants (feature_extractor.py:190-196), pad 3 on every side (stem.cu)
+int stem_pack_launch(const uint8_t* img, int B, int H, int W, __half* out_hi, __half* out_lo, int Hu, int Wu,
+                     cudaStream_t s);
+// compact operand of the detector stem: [B][Hu][Wv = Wu + 3][16] from uint8 (is_u8) or float32 BGR frames,
+// (x * (1/255) - mean) / std with BGR constants (models.py:345-355), pad [3, 2 + pad-to-32] (stem.cu)
 int stem_pack16_launch(const void* img, int is_u8, int B, int H, int W, __half* out_hi, __half* out_lo, int Hu, int Wv,
                        cudaStream_t s);
 // 3x3 stride-2 max-pool, window rows 2y - 1 .. 2y + 1 (columns alike) clipped to the map, Ho x Wo chosen by the caller;

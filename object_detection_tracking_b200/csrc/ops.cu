@@ -1,9 +1,10 @@
 // Single-kernel entry points for parity tests and host tools: one conv, one grouped conv, one GroupNorm, one squeeze-excite,
 // one relation module, the attention head's pool, the deformable sampler and conv, the frame resize, and the element-wise
 // and reduction kernels around the GEMMs (depthwise convs, pools, the BiFPN combine, MBConv's squeeze-excite, OSNet's
-// channel gate, EfficientNet's stem im2col), and the distance kernels around the tracker / ReID GEMMs.  Each call owns its device buffers in an Arena, so
+// channel gate, EfficientNet's stem im2col, the ResNet stems' operand packs), and the distance kernels around the tracker / ReID GEMMs.  Each call owns its device buffers in an Arena, so
 // every return path frees them.
 // The squeeze-excite, relation and deformable-conv calls build a one-block plan with the detector's builders (detplan.h).
+#include <limits.h>
 #include <string.h>
 
 #include <algorithm>
@@ -650,6 +651,32 @@ int b2_op_stem_im2col(int device, const float* img, int H, int W, int Ho, int Wo
   float* d_img = upload_f32(a, img, static_cast<size_t>(H) * W * 3);
   B2_CHECK(op.hi && d_img, "b2_op_stem_im2col: out of device memory");
   if (stem_im2col_launch(d_img, 1, H, W, Ho, Wo, pad_t, pad_l, op.hi, op.lo, nullptr)) return -1;
+  B2_CUDA(cudaDeviceSynchronize());
+  return return_planes(op, op.elems(), out, out_hi, out_lo);
+}
+
+// The ResNet stems' operand packs: the detector's compact 16-lane operand (stem_pack16_launch, layout 0) or the ReID
+// engines' 64-lane operand (stem_pack_launch, layout 1).
+int b2_op_stem_pack(int device, const void* img, int is_u8, int B, int H, int W, int layout, int Hu, int Wu, int split,
+                    float* out, uint16_t* out_hi, uint16_t* out_lo) {
+  B2_CHECK(img && out, "b2_op_stem_pack: null argument");
+  B2_CHECK(layout == 0 || layout == 1, "b2_op_stem_pack: layout must be 0 (detector) or 1 (ReID)");
+  B2_CHECK(layout == 0 || is_u8, "b2_op_stem_pack: the ReID layout takes uint8 crops only");
+  B2_CHECK(B >= 1 && H >= 1 && W >= 1 && Hu >= 1 && Wu >= 1, "b2_op_stem_pack: needs positive sizes");
+  const int lanes = layout == 0 ? 16 : 64;
+  const size_t n_img = static_cast<size_t>(B) * H * W * 3;
+  // the kernels index an image's pixels and an operand image's pixels with int
+  B2_CHECK(static_cast<size_t>(H) * W <= INT_MAX && static_cast<size_t>(Hu) * Wu <= INT_MAX,
+           "b2_op_stem_pack: frame or operand too large");
+  B2_CUDA(cudaSetDevice(device));
+  Arena a;
+  const Planes op = a.planes(B, Hu, Wu, lanes, split != 0);
+  uint8_t* d_img = a.alloc<uint8_t>(n_img * (is_u8 ? 1 : sizeof(float)));
+  B2_CHECK(op.hi && d_img, "b2_op_stem_pack: out of device memory");
+  B2_CUDA(cudaMemcpy(d_img, img, n_img * (is_u8 ? 1 : sizeof(float)), cudaMemcpyHostToDevice));
+  const int rc = layout == 0 ? stem_pack16_launch(d_img, is_u8 != 0, B, H, W, op.hi, op.lo, Hu, Wu, nullptr)
+                             : stem_pack_launch(d_img, B, H, W, op.hi, op.lo, Hu, Wu, nullptr);
+  if (rc) return -1;
   B2_CUDA(cudaDeviceSynchronize());
   return return_planes(op, op.elems(), out, out_hi, out_lo);
 }

@@ -105,7 +105,7 @@ Planes add_stem(b2_reid* c, const std::string& wname, const std::string& bn) {
   c->stem_u = c->planes(B, h1 + 3, w1, 64);
   const Planes u = c->stem_u;
   add_step(c->steps, 0, 0, "", [c, u](cudaStream_t st) {
-    return stem_pack_launch(c->crops, 1, c->B, c->in_h, c->in_w, u.hi, u.lo, u.H, u.W, 1, st);
+    return stem_pack_launch(c->crops, c->B, c->in_h, c->in_w, u.hi, u.lo, u.H, u.W, st);
   });
   Planes c1 = c->planes(B, h1, w1, 64);
   ConvDesc d;
@@ -114,6 +114,7 @@ Planes add_stem(b2_reid* c, const std::string& wname, const std::string& bn) {
   L->bn = bn; L->cin_real = 64; L->layout = kStem;
   add_conv_step(c->steps, 0, L.get());
   c->convs.push_back(std::move(L));
+  c->named.planes("stem_u", c->stem_u);
   c->named.planes("conv1", c1);
   return c1;
 }
@@ -198,7 +199,6 @@ int build(b2_reid* c) {
   const int B = c->B;
   c->crops = c->arena.alloc<uint8_t>(static_cast<size_t>(B) * c->in_h * c->in_w * 3);
   const Planes c1 = add_stem(c, "conv1.conv.weight", "conv1.bn");   // osnet.py:307
-  c->named.planes("stem_u", c->stem_u);
   Planes x = add_maxpool(c, c1);                                       // :308
   const int chans[4] = {64, 256, 384, 512};
   for (int stage = 0; stage < 3; ++stage) {
@@ -417,7 +417,7 @@ int b2_reid_embed_dev(b2_reid* c, const uint8_t* crops_host, int n, float* feats
 
 int b2_reid_feat_dim(b2_reid* c) { return c ? c->feat_dim : -1; }
 
-// Stage-addressable activation of the last pass as fp32 NHWC (names: "conv1", "maxpool", "conv2.0", "conv2.0.x1",
+// Stage-addressable activation of the last pass as fp32 NHWC (names: "stem_u", "conv1", "maxpool", "conv2.0", "conv2.0.x1",
 // "conv2.0.s0".."s3", "conv2.0.x2", "conv2.1", "conv2", ..., "conv5").
 int b2_reid_get_activation(b2_reid* c, const char* name, float* dst, int64_t capacity, int64_t shape[4]) {
   B2_CHECK(c && name && dst && shape, "b2_reid_get_activation: null argument");

@@ -30,18 +30,16 @@ __global__ void planes_to_f32_kernel(const __half* __restrict__ hi, const __half
 // Stem operand pack.  The 7x7 stride-2 conv on 3 channels is not a tensor-core shape, so the frame is
 // re-laid out once per pass so that it becomes a 4x1 stride-1 conv on 64 channels (K = 256) that the
 // wgmma implicit-GEMM kernel takes unchanged:
-//   P  = normalised frame, zero padded [3 top/left, 2 + pad-to-32 bottom/right]        (nn.py:871-877)
+//   P  = normalised frame, zero padded [3 top/left, 3 bottom/right]        (torchvision conv1 7x7/2 pad 3)
 //   U[b][y][q][s*12 + ry*6 + sx*3 + c] = P[b][2y + ry][2(q + s) + sx][c]   s in 0..3, ry,sx in 0..1, c in 0..2
 //   conv0[p][q][o] = sum_{r<4} sum_{ch<64} U[p + r][q][ch] * W'[o][r][ch],  W'[o][r][ch] = W[2r+ry][2s+sx][c][o]
-// (taps with 2r+ry == 7 or 2s+sx == 7 and channels 48..63 carry zero weights).  Normalisation follows
-// models.py:345-355 op by op: x * (1/255), - mean, / std (BGR order), exact fp32, then the (hi, lo) split.
-template <typename TIn>
-__global__ void __launch_bounds__(256) stem_pack_kernel(const TIn* __restrict__ img, int B, int H, int W,
+// (taps with 2r+ry == 7 or 2s+sx == 7 and channels 48..63 carry zero weights).  This is the ReID stem: RGB uint8 crops,
+// torchvision ToTensor + Normalize op by op (x / 255, - mean, / std, RGB order), exact fp32, then the (hi, lo) split.
+__global__ void __launch_bounds__(256) stem_pack_kernel(const uint8_t* __restrict__ img, int B, int H, int W,
                                                         __half* __restrict__ out_hi, __half* __restrict__ out_lo,
-                                                        int Hu, int Wu, int norm_mode) {
-  // mode 0: BGR order (models.py:350-352); mode 1: RGB order (torchvision Normalize defaults of the extractor)
-  const float mean[3] = {norm_mode ? 0.485f : 0.406f, 0.456f, norm_mode ? 0.406f : 0.485f};
-  const float stdv[3] = {norm_mode ? 0.229f : 0.225f, 0.224f, norm_mode ? 0.225f : 0.229f};
+                                                        int Hu, int Wu) {
+  const float mean[3] = {0.485f, 0.456f, 0.406f};      // torchvision Normalize of the extractor (RGB order)
+  const float stdv[3] = {0.229f, 0.224f, 0.225f};
   const size_t total = static_cast<size_t>(B) * Hu * Wu * 8;
   for (size_t idx = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; idx < total;
        idx += static_cast<size_t>(gridDim.x) * blockDim.x) {
@@ -62,7 +60,7 @@ __global__ void __launch_bounds__(256) stem_pack_kernel(const TIn* __restrict__ 
         const int iy = 2 * y + ry - 3, ix = 2 * (q + s) + sx - 3;
         if (iy >= 0 && iy < H && ix >= 0 && ix < W) {
           float x = static_cast<float>(img[((static_cast<size_t>(b) * H + iy) * W + ix) * 3 + c]);
-          x = norm_mode ? __fdiv_rn(x, 255.0f) : __fmul_rn(x, 1.0f / 255);   // ToTensor divides, TF multiplies
+          x = __fdiv_rn(x, 255.0f);                    // ToTensor divides
           x = __fsub_rn(x, mean[c]);
           v = __fdiv_rn(x, stdv[c]);
         }
@@ -75,7 +73,8 @@ __global__ void __launch_bounds__(256) stem_pack_kernel(const TIn* __restrict__ 
 }
 
 // Compact form of the same operand (detector): V[b][y][x][ry*6 + sx*3 + c] = P[b][2y + ry][2x + sx][c], 12 real channels
-// padded to 16, x in [0, Wu + 3).  The 64-channel pixel U[b][y][q][:] of the packed form is then the 64 CONSECUTIVE halves
+// padded to 16, x in [0, Wu + 3).  P is the frame normalised as models.py:345-355 does it, op by op: x * (1/255), - mean,
+// / std (BGR order), exact fp32, zero padded [3 top/left, 2 + pad-to-32 bottom/right] (nn.py:871-877).  The 64-channel pixel U[b][y][q][:] of the packed form is then the 64 CONSECUTIVE halves
 // V[b][y][q .. q+3][0..15]: the conv's TMA map reads it with an element stride of 16 between pixels (overlapping
 // windows), so the 4x width unroll is never written to memory -- 1/4 of the bytes and of the normalisation work
 // (round 1: 454 MB written per batch-8 pass, 81 % issue-bound, 0.45 ms).
@@ -205,14 +204,10 @@ int planes_to_f32(const __half* hi, const __half* lo, float* dst, size_t n, cuda
   return 0;
 }
 
-int stem_pack_launch(const void* img, int is_u8, int B, int H, int W, __half* out_hi, __half* out_lo, int Hu, int Wu,
-                     int norm_mode, cudaStream_t s) {
+int stem_pack_launch(const uint8_t* img, int B, int H, int W, __half* out_hi, __half* out_lo, int Hu, int Wu,
+                     cudaStream_t s) {
   const size_t total = static_cast<size_t>(B) * Hu * Wu * 8;
-  const unsigned grid = grid_for(total, 256, 132 * 32);
-  if (is_u8)
-    stem_pack_kernel<uint8_t><<<grid, 256, 0, s>>>(static_cast<const uint8_t*>(img), B, H, W, out_hi, out_lo, Hu, Wu, norm_mode);
-  else
-    stem_pack_kernel<float><<<grid, 256, 0, s>>>(static_cast<const float*>(img), B, H, W, out_hi, out_lo, Hu, Wu, norm_mode);
+  stem_pack_kernel<<<grid_for(total, 256, 132 * 32), 256, 0, s>>>(img, B, H, W, out_hi, out_lo, Hu, Wu);
   B2_CUDA(cudaGetLastError());
   return 0;
 }

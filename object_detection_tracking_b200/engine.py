@@ -555,6 +555,26 @@ def op_stem_im2col(img, out_hw, pad, split=True, device=0):
     return out, hi, lo
 
 
+def op_stem_pack(frames, layout, out_hw, split=True, device=0):
+    """The ResNet stems' operand pack through the C ABI -- used by the kernel tests: frames [B, H, W, 3] uint8 or float32
+    (float32 for the detector only).  layout "detector": the compact [B, Hu, Wv, 16] operand of conv0 (BGR frames, the
+    detector's normalisation); "reid": the [B, Hu, Wu, 64] operand of the ReID engines' conv1 (RGB crops, torchvision
+    ToTensor + Normalize).  out_hw = (Hu, Wv) or (Hu, Wu).  Returns (out, hi, lo) as op_conv2d_view does."""
+    lib = _lib.load()
+    frames = np.ascontiguousarray(frames)
+    if frames.dtype != np.uint8:
+        frames = _f32(frames)
+    B, H, W, ch = frames.shape
+    assert ch == 3, frames.shape
+    k = {"detector": 0, "reid": 1}[layout]
+    Hu, Wu = out_hw
+    out, hi, lo = _plane_outputs((B, Hu, Wu, 16 if k == 0 else 64), split)
+    _lib.check(lib.b2_op_stem_pack(device, _lib.ptr(frames), int(frames.dtype == np.uint8), B, H, W, k, Hu, Wu,
+                                   int(split), _lib.ptr(out), _lib.ptr(hi), _lib.ptr(lo)),
+               "b2_op_stem_pack")
+    return out, hi, lo
+
+
 def op_distance_operand(x, ld=None, normalize=False, eps=0.0, device=0):
     """The distance GEMMs' operand conversion through the C ABI -- used by the kernel tests: x [rows, D] fp32 to planes
     [rows, ld] (ld default D), normalised rows x / max(|x|, eps) or x itself.  Returns (hi, lo, sqnorm, range_flag) with
