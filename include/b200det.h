@@ -296,6 +296,16 @@ int b2_reid_embed(b2_reid* ctx, const uint8_t* crops_host, int n, float* feats_h
 /* Same, with the [n, feat_dim] features left in device memory of the context's GPU (`feats_dev`: e.g. this camera's slice of
  * the gallery buffer the NCCL all-gather of config 5 sends, multi_video_reid.py:448-476) -- a gallery never crosses PCIe. */
 int b2_reid_embed_dev(b2_reid* ctx, const uint8_t* crops_host, int n, float* feats_dev);
+/* The drivers' whole ReID input step on the GPU (single_video_reid.py:211-227): frames_host is uint8 BGR [nf][h][w][3],
+ * boxes_host [n][5] int32 (frame index, x, y, w, h) with 1 <= n <= batch.  Each box is cut out of its frame, turned to RGB
+ * and resized to the model's crop size exactly as Pillow's Image.resize(BILINEAR) does, then embedded as b2_reid_embed
+ * would embed those crops.  Every box must lie inside its frame with w, h >= 1; a bad box fails the call (b2_last_error)
+ * before any device work.  The frames go through a grow-only device buffer the context owns. */
+int b2_reid_embed_boxes(b2_reid* ctx, const uint8_t* frames_host, int nf, int h, int w, const int32_t* boxes_host, int n,
+                        float* feats_host);
+/* Same, with the features left in device memory of the context's GPU, as b2_reid_embed_dev. */
+int b2_reid_embed_boxes_dev(b2_reid* ctx, const uint8_t* frames_host, int nf, int h, int w, const int32_t* boxes_host, int n,
+                            float* feats_dev);
 int b2_reid_feat_dim(b2_reid* ctx);   /* 512 (osnet_x1_0) / 2048 (resnet101) */
 int b2_reid_num_launches(b2_reid* ctx);
 /* Stage-addressable activation of the last pass as fp32 NHWC (parity tests): "conv1", "maxpool", "conv2.0", ... */
@@ -533,6 +543,11 @@ int b2_op_stem_im2col(int device, const float* img, int H, int W, int Ho, int Wo
  * out is the operand joined to fp32, out_hi / out_lo (may be NULL; out_lo unwritten in fp16 precision) its raw planes. */
 int b2_op_stem_pack(int device, const void* img, int is_u8, int B, int H, int W, int layout, int Hu, int Wu, int split,
                     float* out, uint16_t* out_hi, uint16_t* out_lo);
+/* The ReID crop resize of b2_reid_embed_boxes alone: frames [nf][h][w][3] uint8 BGR and boxes [n][5] int32 (frame, x, y,
+ * w, h; host memory, checked as there) -> out [n][out_h][out_w][3] uint8 RGB, each box resized as Pillow's
+ * Image.resize((out_w, out_h), BILINEAR); 1 <= out_w <= 256. */
+int b2_op_reid_crop_resize(int device, const uint8_t* frames, int nf, int h, int w, const int32_t* boxes, int n, int out_h,
+                           int out_w, uint8_t* out);
 
 /* The distance kernels of b2_cosine_cost, b2_distance_matrix, b2_track_pair_cost and b2_tmot_embedding_distance, one at a
  * time.  b2_op_distance_operand converts x [rows][D] (host fp32) into the GEMM's operand planes out_hi / out_lo

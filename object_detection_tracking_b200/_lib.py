@@ -115,6 +115,8 @@ SYMBOLS = [
     ("b2_reid_load_weights", c_int, [c_void_p, POINTER(c_char_p), POINTER(c_void_p), POINTER(c_int64), c_int]),
     ("b2_reid_embed", c_int, [c_void_p, c_void_p, c_int, c_void_p]),
     ("b2_reid_embed_dev", c_int, [c_void_p, c_void_p, c_int, c_void_p]),
+    ("b2_reid_embed_boxes", c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_void_p]),
+    ("b2_reid_embed_boxes_dev", c_int, [c_void_p, c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_void_p]),
     ("b2_reid_feat_dim", c_int, [c_void_p]),
     ("b2_reid_num_launches", c_int, [c_void_p]),
     ("b2_reid_get_activation", c_int, [c_void_p, c_char_p, c_void_p, c_int64, POINTER(c_int64)]),
@@ -155,6 +157,7 @@ SYMBOLS = [
     ("b2_op_channel_gate", c_int, [c_int] + [c_void_p] * 6 + [c_int] * 6 + [c_void_p] * 4),
     ("b2_op_stem_im2col", c_int, [c_int, c_void_p] + [c_int] * 7 + [c_void_p] * 3),
     ("b2_op_stem_pack", c_int, [c_int, c_void_p] + [c_int] * 8 + [c_void_p] * 3),
+    ("b2_op_reid_crop_resize", c_int, [c_int, c_void_p, c_int, c_int, c_int, c_void_p, c_int, c_int, c_int, c_void_p]),
     ("b2_op_distance_operand", c_int, [c_int, c_void_p] + [c_int] * 4 + [c_float] + [c_void_p] * 4),
     ("b2_op_distance_epilogue", c_int, [c_int, c_int, c_void_p] + [c_int] * 3 + [c_void_p] * 3 + [c_int, c_void_p, c_int,
                                                                                                 c_void_p, c_float, c_void_p]),

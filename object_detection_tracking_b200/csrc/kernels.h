@@ -19,6 +19,12 @@ int stem_pack_launch(const uint8_t* img, int B, int H, int W, __half* out_hi, __
 // (x * (1/255) - mean) / std with BGR constants (models.py:345-355), pad [3, 2 + pad-to-32] (stem.cu)
 int stem_pack16_launch(const void* img, int is_u8, int B, int H, int W, __half* out_hi, __half* out_lo, int Hu, int Wv,
                        cudaStream_t s);
+// reid_ingest.cu: track boxes [n][5] (frame, x, y, w, h; int32, device) of uint8 BGR frames [nf][H][W][3] -> RGB uint8
+// crops [n][out_h][out_w][3] resized as Pillow's Image.resize(BILINEAR) (pil_resize_math.h); out_w <= 256.  The boxes must
+// have passed reid_boxes_check (host copy of the same table): frame index in [0, nf), w, h >= 1, inside the frame.
+int reid_boxes_check(const int32_t* boxes_host, int n, int nf, int H, int W, const char* who);
+int reid_crop_resize_launch(const uint8_t* frames, int H, int W, const int32_t* boxes, int n, uint8_t* crops, int out_h,
+                            int out_w, cudaStream_t s);
 // 3x3 stride-2 max-pool, window rows 2y - 1 .. 2y + 1 (columns alike) clipped to the map, Ho x Wo chosen by the caller;
 // C a multiple of 8.  The running maximum starts from 0, so this is the max-pool only of inputs >= 0: every caller feeds
 // it post-ReLU data.  The output is the (hi, lo) pair of the element with the largest joined value.

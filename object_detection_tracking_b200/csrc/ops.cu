@@ -749,6 +749,27 @@ int b2_op_distance_epilogue(int device, int kind, const float* dots, int rows, i
   return 0;
 }
 
+// The ReID crop resize alone (reid_crop_resize_launch).
+int b2_op_reid_crop_resize(int device, const uint8_t* frames, int nf, int h, int w, const int32_t* boxes, int n, int out_h,
+                           int out_w, uint8_t* out) {
+  B2_CHECK(frames && boxes && out, "b2_op_reid_crop_resize: null argument");
+  B2_CHECK(nf >= 1 && h >= 1 && w >= 1 && n >= 1, "b2_op_reid_crop_resize: needs nf, h, w, n >= 1");
+  if (reid_boxes_check(boxes, n, nf, h, w, "b2_op_reid_crop_resize")) return -1;
+  B2_CUDA(cudaSetDevice(device));
+  const size_t nb_frames = static_cast<size_t>(nf) * h * w * 3, nb_out = static_cast<size_t>(n) * out_h * out_w * 3;
+  Arena a;
+  uint8_t* d_frames = a.alloc<uint8_t>(nb_frames, false);
+  int32_t* d_boxes = a.alloc<int32_t>(static_cast<size_t>(n) * 5, false);
+  uint8_t* d_out = a.alloc<uint8_t>(nb_out);
+  B2_CHECK(d_frames && d_boxes && d_out, "b2_op_reid_crop_resize: out of device memory");
+  B2_CUDA(cudaMemcpy(d_frames, frames, nb_frames, cudaMemcpyHostToDevice));
+  B2_CUDA(cudaMemcpy(d_boxes, boxes, sizeof(int32_t) * 5 * n, cudaMemcpyHostToDevice));
+  if (reid_crop_resize_launch(d_frames, h, w, d_boxes, n, d_out, out_h, out_w, nullptr)) return -1;
+  B2_CUDA(cudaDeviceSynchronize());
+  B2_CUDA(cudaMemcpy(out, d_out, nb_out, cudaMemcpyDeviceToHost));
+  return 0;
+}
+
 // The resize alone (parity tests): host uint8 [n, src_h, src_w, 3] -> host float32 [n, dst_h, dst_w, 3].
 int b2_resize_frames(int device, const uint8_t* frames_u8, int n, int src_h, int src_w, int dst_h, int dst_w,
                      float* out_host) {

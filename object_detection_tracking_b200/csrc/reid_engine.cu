@@ -6,7 +6,9 @@
 //   conv1 7x7/2 + BN + ReLU -> maxpool 3/2 -> [OSBlock x2 + Conv1x1 + AvgPool2] x2 -> OSBlock x2 -> conv5 1x1
 //   -> global avg-pool -> fc(512) + BatchNorm1d + ReLU  (eval mode returns this 512-d vector)
 // Input contract (torchreid/feature_extractor.py:190-196,209-252): RGB uint8 crops already resized to
-// 256x128 (the PIL resize stays on the host), ToTensor + Normalize happen in the stem pack kernel.
+// 256x128 (b2_reid_embed: the caller ran the PIL resize), or uint8 BGR frames plus a table of track boxes
+// (b2_reid_embed_boxes: reid_ingest.cu cuts and resizes them as Pillow does into the same crop buffer); ToTensor +
+// Normalize happen in the stem pack kernel.
 //
 // Second model (b2_reid_create_model(..., model = 1)): torchreid's resnet101 (torchreid/models/resnet.py:441-455 ->
 // ResNet(Bottleneck, [3, 4, 23, 3], last_stride=2, fc_dims=None), forward :342-366), the vehicle extractor of
@@ -63,7 +65,10 @@ struct b2_reid {
   std::vector<std::unique_ptr<RGate>> gates;
   std::vector<Step> steps;
   StageMap named;                    // stage-addressable activations (parity tests)
-  uint8_t* crops = nullptr;
+  uint8_t* crops = nullptr;          // [B][in_h][in_w][3] RGB, the stem pack's input
+  uint8_t* frames = nullptr;         // b2_reid_embed_boxes: uploaded frames, grow-only (cudaMalloc, freed on destroy)
+  size_t frames_cap = 0;
+  int32_t* boxes = nullptr;          // [B][5] box table of the last b2_reid_embed_boxes call
   Planes stem_u, gap_planes;
   float* gap_f32 = nullptr;
   float* feats = nullptr;      // [Bpad][512]
@@ -299,6 +304,8 @@ int b2_reid_create_model(b2_reid** out, int device, int batch, int precision, in
   if (model == 1) { c->in_h = 128; c->in_w = 256; c->feat_dim = 2048; }   // single_video_reid.py:410-415
   if (open_device(device, "b2_reid_create", &c->num_sms, &c->stream)) return -1;
   if ((model == 1 ? build_resnet101(c.get()) : build(c.get()))) { b2_reid_destroy(c.release()); return -1; }
+  c->boxes = c->arena.alloc<int32_t>(static_cast<size_t>(batch) * 5);
+  if (!c->boxes) { b2_reid_destroy(c.release()); return -1; }
   B2_CUDA(cudaDeviceSynchronize());
   *out = c.release();
   return 0;
@@ -310,6 +317,7 @@ void b2_reid_destroy(b2_reid* c) {
   cudaDeviceSynchronize();
   if (c->graph) cudaGraphExecDestroy(c->graph);
   if (c->stream) cudaStreamDestroy(c->stream);
+  if (c->frames) cudaFree(c->frames);
   delete c;   // plans, then the arena's device memory
 }
 
@@ -413,6 +421,47 @@ int b2_reid_embed(b2_reid* c, const uint8_t* crops_host, int n, float* feats_hos
 // buffer that the NCCL all-gather / the peer-memory pair cost of config 5 reads), so a gallery never crosses PCIe.
 int b2_reid_embed_dev(b2_reid* c, const uint8_t* crops_host, int n, float* feats_dev) {
   return reid_embed_impl(c, crops_host, n, feats_dev, true);
+}
+
+// frames_host: uint8 BGR [nf][h][w][3]; boxes_host: [n][5] int32 (frame, x, y, w, h).  Every box is checked before anything
+// is uploaded; the crop-resize kernel then fills the crop buffer the captured pass reads (rows n..B zeroed as above).
+static int reid_embed_boxes_impl(b2_reid* c, const uint8_t* frames_host, int nf, int h, int w, const int32_t* boxes_host,
+                                 int n, float* feats, bool to_device) {
+  B2_CHECK(c && frames_host && boxes_host && feats, "b2_reid_embed_boxes: null argument");
+  B2_CHECK(n >= 1 && n <= c->B, "b2_reid_embed_boxes: needs 1 <= n <= the batch the context was created for");
+  B2_CHECK(nf >= 1 && h >= 1 && w >= 1, "b2_reid_embed_boxes: needs at least one frame of positive size");
+  if (reid_boxes_check(boxes_host, n, nf, h, w, "b2_reid_embed_boxes")) return -1;
+  B2_CUDA(cudaSetDevice(c->device));
+  B2_CHECK(c->loaded, "b2_reid_embed_boxes: weights not loaded");
+  const size_t per = static_cast<size_t>(c->in_h) * c->in_w * 3, frame_bytes = static_cast<size_t>(nf) * h * w * 3;
+  if (frame_bytes > c->frames_cap) {
+    B2_CUDA(cudaStreamSynchronize(c->stream));
+    if (c->frames) B2_CUDA(cudaFree(c->frames));
+    c->frames = nullptr;
+    c->frames_cap = 0;
+    B2_CUDA(cudaMalloc(&c->frames, frame_bytes));
+    c->frames_cap = frame_bytes;
+  }
+  const cudaMemcpyKind out_kind = to_device ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
+  B2_CUDA(cudaMemcpyAsync(c->frames, frames_host, frame_bytes, cudaMemcpyHostToDevice, c->stream));
+  B2_CUDA(cudaMemcpyAsync(c->boxes, boxes_host, sizeof(int32_t) * 5 * n, cudaMemcpyHostToDevice, c->stream));
+  if (n < c->B) B2_CUDA(cudaMemsetAsync(c->crops + n * per, 0, (c->B - n) * per, c->stream));
+  if (reid_crop_resize_launch(c->frames, h, w, c->boxes, n, c->crops, c->in_h, c->in_w, c->stream)) return -1;
+  if (!c->graph && capture_graph(c->stream, [c] { return run_steps(c->steps, ~0u, c->stream); }, &c->graph)) return -1;
+  B2_CUDA(cudaGraphLaunch(c->graph, c->stream));
+  B2_CUDA(cudaMemcpyAsync(feats, c->feats, sizeof(float) * n * c->feat_dim, out_kind, c->stream));
+  B2_CUDA(cudaStreamSynchronize(c->stream));
+  return 0;
+}
+
+int b2_reid_embed_boxes(b2_reid* c, const uint8_t* frames_host, int nf, int h, int w, const int32_t* boxes_host, int n,
+                        float* feats_host) {
+  return reid_embed_boxes_impl(c, frames_host, nf, h, w, boxes_host, n, feats_host, false);
+}
+
+int b2_reid_embed_boxes_dev(b2_reid* c, const uint8_t* frames_host, int nf, int h, int w, const int32_t* boxes_host, int n,
+                            float* feats_dev) {
+  return reid_embed_boxes_impl(c, frames_host, nf, h, w, boxes_host, n, feats_dev, true);
 }
 
 int b2_reid_feat_dim(b2_reid* c) { return c ? c->feat_dim : -1; }

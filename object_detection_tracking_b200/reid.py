@@ -2,9 +2,11 @@
 
 `FeatureExtractor` mirrors torchreid.utils.FeatureExtractor (torchreid/feature_extractor.py:121-252): same
 constructor arguments, callable on a list of HWC RGB uint8 arrays / a single array / image paths, returns a
-`torch.Tensor [B, 512]`.  The PIL resize of the reference's transform pipeline stays on the host (it is the
+`torch.Tensor [B, 512]`.  `__call__` keeps the PIL resize of the reference's transform pipeline on the host (it is the
 reference's own library call); ToTensor + Normalize + the whole OSNet-x1.0 forward run in libb200det
-(b2_reid_embed).  `compute_distance_matrix` mirrors torchreid/distance.py:6-46.  No CPU fallback.
+(b2_reid_embed).  `extract_boxes` takes the frame and the track boxes instead and cuts, converts and resizes them on
+the GPU bit-exactly as Pillow does (b2_reid_embed_boxes).  `compute_distance_matrix` mirrors
+torchreid/distance.py:6-46.  No CPU fallback.
 """
 from __future__ import annotations
 
@@ -72,6 +74,46 @@ class ReidEngine:
         _lib.check(self.lib.b2_reid_embed_dev(self._ctx, _lib.ptr(crops_u8), n, c_void_p(out_dev.data_ptr())),
                    "b2_reid_embed_dev")
 
+    def _boxes_args(self, frames, boxes):
+        frames = np.asarray(frames)
+        if frames.dtype != np.uint8:
+            raise ValueError("frames must be uint8 BGR, got %s" % frames.dtype)
+        frames = np.ascontiguousarray(frames)
+        if frames.ndim == 3:
+            frames = frames[None]
+        if frames.ndim != 4 or frames.shape[3] != 3:
+            raise ValueError("frames must be [h, w, 3] or [F, h, w, 3] uint8 BGR, got shape %s" % (frames.shape,))
+        boxes = np.asarray(boxes)
+        if boxes.ndim != 2 or boxes.shape[1] != 5 or not np.issubdtype(boxes.dtype, np.integer):
+            raise ValueError("boxes must be an integer [n, 5] table (frame, x, y, w, h), got %s %s" % (boxes.dtype,
+                                                                                                      boxes.shape))
+        if boxes.size and (boxes.min() < np.iinfo(np.int32).min or boxes.max() > np.iinfo(np.int32).max):
+            raise ValueError("box coordinates do not fit int32")
+        return frames, np.ascontiguousarray(boxes, dtype=np.int32)
+
+    def embed_boxes(self, frames, boxes) -> np.ndarray:
+        """frames: [h, w, 3] or [F, h, w, 3] uint8 BGR; boxes: int [n, 5] rows (frame index, x, y, w, h), 1 <= n <= batch,
+        each inside its frame -> [n, feat_dim] float32, the features of
+        Image.fromarray(frame[y:y+h, x:x+w, ::-1]).resize(crop size, BILINEAR) for every box, cut out and resized on the
+        GPU (b2_reid_embed_boxes).  A bad box raises RuntimeError before anything is launched."""
+        frames, boxes = self._boxes_args(frames, boxes)
+        out = np.empty((boxes.shape[0], self.feat_dim), dtype=np.float32)
+        _lib.check(self.lib.b2_reid_embed_boxes(self._ctx, _lib.ptr(frames), frames.shape[0], frames.shape[1],
+                                                frames.shape[2], _lib.ptr(boxes), boxes.shape[0], _lib.ptr(out)),
+                   "b2_reid_embed_boxes")
+        return out
+
+    def embed_boxes_dev(self, frames, boxes, out_dev) -> None:
+        """embed_boxes with the [n, feat_dim] features written into `out_dev`, a contiguous float32 torch CUDA tensor on
+        this engine's GPU, as embed_dev (b2_reid_embed_boxes_dev)."""
+        frames, boxes = self._boxes_args(frames, boxes)
+        n = boxes.shape[0]
+        assert out_dev.is_cuda and out_dev.is_contiguous() and tuple(out_dev.shape) == (n, self.feat_dim), out_dev.shape
+        assert str(out_dev.dtype) == "torch.float32"
+        _lib.check(self.lib.b2_reid_embed_boxes_dev(self._ctx, _lib.ptr(frames), frames.shape[0], frames.shape[1],
+                                                    frames.shape[2], _lib.ptr(boxes), n, c_void_p(out_dev.data_ptr())),
+                   "b2_reid_embed_boxes_dev")
+
     def get_activation(self, name: str) -> np.ndarray:
         """fp32 NHWC copy of a named intermediate of the last pass (parity tests)."""
         shape = (c_int64 * 4)()
@@ -132,6 +174,29 @@ class FeatureExtractor(object):
         feats = []
         for i in range(0, len(crops), self.batch):
             feats.append(self.engine.embed(np.stack(crops[i:i + self.batch])))
+        return torch.from_numpy(np.concatenate(feats, 0) if feats else np.zeros((0, self.engine.feat_dim), np.float32))
+
+    def extract_boxes(self, frame_bgr, tlwhs):
+        """The drivers' ReID input step (single_video_reid.py:211-227, multi_video_reid.py:212-239) on the GPU: for each
+        box tlwh of the uint8 BGR frame [h, w, 3], int() each coordinate, cut image[y:y+h, x:x+w], turn it to RGB and
+        resize it as T.Resize does -> torch.Tensor [n, D], the same features as
+        self([cv2.cvtColor(crop, cv2.COLOR_BGR2RGB) for crop in crops]).  Boxes go to the engine `batch` at a time.
+        Raises ValueError for a box whose integer crop is empty or leaves the frame: callers keep filtering with
+        valid_box (utils.py:44-57) first, as the drivers do."""
+        import torch
+        frame = np.asarray(frame_bgr)
+        if frame.ndim != 3 or frame.shape[2] != 3 or frame.dtype != np.uint8:
+            raise ValueError("frame_bgr must be a [h, w, 3] uint8 BGR image")
+        H, W = frame.shape[:2]
+        boxes = np.zeros((len(tlwhs), 5), np.int64)
+        for i, tlwh in enumerate(tlwhs):
+            x, y, w, h = (int(v) for v in list(tlwh)[:4])
+            if w < 1 or h < 1 or x < 0 or y < 0 or x + w > W or y + h > H:
+                raise ValueError("box %d %r: the crop [%d:%d, %d:%d] is empty or leaves the %dx%d frame"
+                                 % (i, tuple(tlwh), y, y + h, x, x + w, W, H))
+            boxes[i, 1:] = (x, y, w, h)
+        frame = np.ascontiguousarray(frame)                 # once, not once per chunk
+        feats = [self.engine.embed_boxes(frame, boxes[i:i + self.batch]) for i in range(0, len(boxes), self.batch)]
         return torch.from_numpy(np.concatenate(feats, 0) if feats else np.zeros((0, self.engine.feat_dim), np.float32))
 
 
