@@ -118,6 +118,27 @@ typedef struct b2_config_ext3 {
                                       from 64 to 2048 */
 } b2_config_ext3;
 
+/* Graph options added after b2_config_ext3's layout was fixed.  b2_create_ex4 takes them; b2_create_ex3 builds the graph
+ * with every field 0. */
+typedef struct b2_config_ext4 {
+  int32_t use_small_object_head;   /* main.py --use_small_object_head: the small-object branch of the single-image graph
+                                      (models.py:590-692, 845-897), results through b2_get_small_objects.  Per small class:
+                                      NMS of its unclipped decoded boxes without a score threshold (at most result_per_im),
+                                      ROIAlign 7 -> the head's fc6 / fc7, [optionally + person_object_relation], a [D, 2]
+                                      classification; then the head's per-class NMS and top-k over the rebuilt
+                                      [K, C + 1] LOGITS.  Every small class must keep the same count K: otherwise the
+                                      reference's tf.map_fn fails, and here the status is 1 with K = 0.  Needs batch 1, the
+                                      single-image graph and the class-specific 2fc head (refused otherwise, with the
+                                      reason); the main outputs do not depend on it */
+  int32_t num_small_objects;       /* C, 1 .. min(num_class - 1, 80) */
+  int32_t small_object_class_ids[80];   /* the head's class id of each small class, in label order, no duplicates */
+  int32_t use_so_association;      /* --use_so_association: hidden += person_object_relation(hidden, boxes, person rows)
+                                      (nn.py:194-270), weights "fastrcnn/small_objects/person_object_relation/..." */
+  int32_t so_person_class_id;      /* the head's class id of "Person" (with use_so_association) */
+  int32_t so_person_topk;          /* --so_person_topk: person boxes kept by their NMS, 1 .. 1024 */
+  int32_t use_so_score_thres;      /* --use_so_score_thres: the final NMS keeps logit > result_score_thres only */
+} b2_config_ext4;
+
 const char* b2_last_error(void);
 int b2_version(void);
 
@@ -130,6 +151,10 @@ int b2_create_ex2(b2_ctx** out, int device, const b2_config* cfg, const b2_confi
 /* b2_create_ex2 with the options of b2_config_ext3 as well; ext, ext2 and ext3 may be NULL (all 0) */
 int b2_create_ex3(b2_ctx** out, int device, const b2_config* cfg, const b2_config_ext* ext, const b2_config_ext2* ext2,
                   const b2_config_ext3* ext3);
+/* b2_create_ex3 with the options of b2_config_ext4 as well; ext .. ext4 may be NULL (all 0).  Refuses, with the reason, a
+ * small-object configuration the reference cannot build or this engine does not run, before touching the device */
+int b2_create_ex4(b2_ctx** out, int device, const b2_config* cfg, const b2_config_ext* ext, const b2_config_ext2* ext2,
+                  const b2_config_ext3* ext3, const b2_config_ext4* ext4);
 void b2_destroy(b2_ctx* ctx);
 
 /* Named fp32 host arrays in the reference's Tensorpack-npz naming ("conv0/W",
@@ -180,6 +205,12 @@ int b2_box_features(b2_ctx* ctx, const void* frame_host, const float* boxes_host
 /* final_masks of the last pass (needs cfg.add_mask): [batch][result_per_im][28][28] float32 (models.py:958-961; the
  * drivers paste them into the frame with fill_full_mask, obj_detect_tracking.py:719); rows >= valid[b] are zero. */
 int b2_get_masks(b2_ctx* ctx, float* masks_host, int64_t capacity_bytes);
+/* The small-object branch's outputs of the last pass (use_small_object_head), host buffers: boxes [result_per_im][4]
+ * (clipped, resized-image pixels), probs [result_per_im] (the rebuilt LOGITS, models.py:880-897), labels [result_per_im]
+ * (1 .. C: index in the small classes + 1), count [1] rows valid, class_counts [C] boxes each small class kept by its
+ * NMS, status [1]: 0, or 1 when those counts differ (then count is 0: the reference's graph fails there). */
+int b2_get_small_objects(b2_ctx* ctx, float* boxes, float* probs, int32_t* labels, int32_t* count, int32_t* class_counts,
+                         int32_t* status);
 
 /* Stage-addressable access for parity tests.  Activations are returned as fp32. */
 int b2_stage_shape(b2_ctx* ctx, const char* name, int64_t shape[4], int32_t* dtype /*0 f32, 1 i32*/);
@@ -476,6 +507,14 @@ int b2_op_relation(int device, const float* h, const float* boxes, const int32_t
  * planes; a row whose 49 x C values are not all finite is all NaN.  C a multiple of 8 up to 8192; the planes hold sums up
  * to 65504 in magnitude (the engine's pass fails beyond that, as for every plane output). */
 int b2_op_att_pool(int device, const float* x, int M, int C, int split, float* out);
+/* person_object_relation (nn.py:194-270, use_so_association) as the engine runs it: query rows h [K][D] with boxes [K][4],
+ * key rows ref [R][D] with boxes ref_boxes [R][4] (host, fp32; the rows are converted to the engine's planes), the
+ * module's weights (geo_emb W [4][64], b [64], geo_conv W [64][16], b [16], query / key W [D][D], output W [16D][D]).
+ * out [K][D] = h + output_linear(P . ref), P the softmax over the R key rows; read back from its planes.  D a multiple of
+ * 64, 1 <= R <= 1024. */
+int b2_op_so_attend(int device, const float* h, const float* boxes, int K, const float* ref, const float* ref_boxes, int R,
+                    const float* geo_emb_w, const float* geo_emb_b, const float* geo_conv_w, const float* geo_conv_b,
+                    const float* query_w, const float* key_w, const float* output_w, int D, int split, float* out);
 /* The deformable conv's bilinear sampler (deformable_conv2d nn.py:1642-1712, deformable_helper.py:42-137) as the engine runs
  * it: x [B][H][W][C] (host, fp32, converted to the engine's planes), offsets [B][ceil(H/2)][ceil(W/2)][18] (channel 2k the
  * y and 2k+1 the x offset of tap k, per image).  out [B][ceil(H/2)][ceil(W/2)][9][C]: the sampled operand read back from

@@ -40,6 +40,12 @@ class B2ConfigExt3(ctypes.Structure):
     _fields_ = [("use_att_frcnn_head", c_int32)]
 
 
+class B2ConfigExt4(ctypes.Structure):
+    _fields_ = [("use_small_object_head", c_int32), ("num_small_objects", c_int32),
+                ("small_object_class_ids", c_int32 * 80), ("use_so_association", c_int32), ("so_person_class_id", c_int32),
+                ("so_person_topk", c_int32), ("use_so_score_thres", c_int32)]
+
+
 class B2EffdetConfig(ctypes.Structure):
     _fields_ = [
         ("image_h", c_int32), ("image_w", c_int32), ("min_level", c_int32), ("max_level", c_int32),
@@ -68,6 +74,9 @@ SYMBOLS = [
     ("b2_create_ex2", c_int, [POINTER(c_void_p), c_int, POINTER(B2Config), POINTER(B2ConfigExt), POINTER(B2ConfigExt2)]),
     ("b2_create_ex3", c_int, [POINTER(c_void_p), c_int, POINTER(B2Config), POINTER(B2ConfigExt), POINTER(B2ConfigExt2),
                               POINTER(B2ConfigExt3)]),
+    ("b2_create_ex4", c_int, [POINTER(c_void_p), c_int, POINTER(B2Config), POINTER(B2ConfigExt), POINTER(B2ConfigExt2),
+                              POINTER(B2ConfigExt3), POINTER(B2ConfigExt4)]),
+    ("b2_get_small_objects", c_int, [c_void_p] + [c_void_p] * 6),
     ("b2_destroy", None, [c_void_p]),
     ("b2_load_weights", c_int, [c_void_p, POINTER(c_char_p), POINTER(c_void_p), POINTER(c_int64), c_int]),
     ("b2_detect", c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int]),
@@ -147,6 +156,8 @@ SYMBOLS = [
     ("b2_op_squeeze_excite", c_int, [c_int] + [c_void_p] * 6 + [c_int] * 6 + [c_void_p, c_void_p]),
     ("b2_op_group_conv2d", c_int, [c_int, c_void_p, c_void_p, c_void_p, c_void_p] + [c_int] * 16 + [c_void_p]),
     ("b2_op_relation", c_int, [c_int] + [c_void_p] * 10 + [c_int] * 4 + [c_void_p]),
+    ("b2_op_so_attend", c_int, [c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int] + [c_void_p] * 7
+     + [c_int, c_int, c_void_p]),
     ("b2_op_att_pool", c_int, [c_int, c_void_p, c_int, c_int, c_int, c_void_p]),
     ("b2_op_deform_sample", c_int, [c_int, c_void_p, c_void_p] + [c_int] * 5 + [c_void_p]),
     ("b2_op_deform_conv2d", c_int, [c_int] + [c_void_p] * 4 + [c_int] * 7 + [c_void_p, c_void_p]),
@@ -271,4 +282,23 @@ def make_config_ext3(cfg) -> B2ConfigExt3:
     """The options of the namespace that b2_config_ext3 carries."""
     e = B2ConfigExt3()
     e.use_att_frcnn_head = int(bool(getattr(cfg, "use_att_frcnn_head", False)))
+    return e
+
+
+def make_config_ext4(cfg) -> B2ConfigExt4:
+    """The options of the namespace that b2_config_ext4 carries (the small-object branch; all 0 when it is off)."""
+    e = B2ConfigExt4()
+    if not getattr(cfg, "use_small_object_head", False):
+        return e
+    ids = tuple(cfg.small_object_class_ids)
+    if len(ids) > 80:
+        raise ValueError("use_small_object_head: at most 80 small objects, got %d" % len(ids))
+    e.use_small_object_head = 1
+    e.num_small_objects = len(ids)
+    for i, v in enumerate(ids):
+        e.small_object_class_ids[i] = int(v)
+    e.use_so_association = int(bool(cfg.use_so_association))
+    e.so_person_class_id = int(cfg.so_person_class_id)
+    e.so_person_topk = int(cfg.so_person_topk)
+    e.use_so_score_thres = int(bool(cfg.use_so_score_thres))
     return e

@@ -20,6 +20,8 @@ There is no CPU fallback: without the CUDA library or an H100 the calls raise.
 """
 from __future__ import annotations
 
+import copy
+
 import numpy as np
 
 from .config import normalize_config
@@ -73,6 +75,12 @@ class Mask_RCNN_FPN:
 
     def __init__(self, config, gpuid=0, precision="split", input_dtype="float32", feat_mode=0):
         self.config = normalize_config(config)
+        if self.config.use_small_object_head and (self.is_multi or getattr(self.config, "is_load_from_pb", False)):
+            # the batch graph has no small-object branch (models.py:1969-3487) and pack() exports the main outputs only
+            # (models.py:134-147): such a model runs without it
+            cfg = copy.copy(self.config)
+            cfg.use_small_object_head = False
+            self.config = normalize_config(cfg)
         self.gpuid = gpuid
         self.precision = precision
         self.input_dtype = input_dtype
@@ -88,6 +96,10 @@ class Mask_RCNN_FPN:
         self.fpn_box_feat = TensorHandle(self, "fpn_box_feat:0")
         self.final_valid_indices = TensorHandle(self, "final_valid_indices:0")
         self.final_masks = TensorHandle(self, "final_masks:0")          # with config.add_mask (models.py:143-146,958-961)
+        # with config.use_small_object_head (models.py:893-897); single-image graph only
+        self.so_final_boxes = TensorHandle(self, "so_final_boxes:0")
+        self.so_final_labels = TensorHandle(self, "so_final_labels:0")
+        self.so_final_probs = TensorHandle(self, "so_final_probs:0")
         self._weights = None
         self._detectors = {}
 
@@ -147,9 +159,27 @@ class Mask_RCNN_FPN:
         want_feat = any(f is self.fpn_box_feat for f in fetches)
         out = det.detect_host(frames, feat_mode=self.feat_mode, want_feat=want_feat)
         valid = out["valid"]
+        so = None
+        so_handles = (self.so_final_boxes, self.so_final_labels, self.so_final_probs)
+        if any(f is h for f in fetches for h in so_handles):
+            if not self.config.use_small_object_head:
+                raise KeyError("so_final_boxes / so_final_labels / so_final_probs need config.use_small_object_head in the "
+                               "single-image graph (models.py:590)")
+            so = det.get_small_objects()
+            if so["status"]:
+                raise RuntimeError("small-object head: the classes %s kept %s boxes in their NMS; the reference's tf.map_fn "
+                                   "needs equal counts and fails here (models.py:618-621)"
+                                   % (list(self.config.small_objects), so["class_counts"].tolist()))
         res = []
         for f in fetches:
-            if single:
+            if so is not None and any(f is h for h in so_handles):
+                if f is self.so_final_boxes:
+                    res.append(so["boxes"])
+                elif f is self.so_final_labels:
+                    res.append(so["labels"].astype(np.int64))                 # models.py:887-888: int64, 1..C
+                else:
+                    res.append(so["probs"])                                   # logits (models.py:884)
+            elif single:
                 r = int(valid[0])
                 if f is self.final_boxes:
                     res.append(out["boxes"][0, :r].copy())

@@ -45,6 +45,18 @@ coco_obj_to_actev_obj = {
 }
 
 
+# class_ids.py:99-117: the ActEV merge-prop model's 17 classes (main.py --merge_prop), the table the small-object head
+# resolves its class names through (main.py:506-521)
+MERGE_PROP_NAMES = (
+    "BG Vehicle Person Parking_Meter Tree Other Trees Construction_Barrier Door Dumpster Push_Pulled_Object "
+    "Construction_Vehicle Prop Bike Animal Articulated_Infrastructure Prop_plus_Push_Pulled_Object")
+targetClass2id_mergeProp = {n: i for i, n in enumerate(MERGE_PROP_NAMES.split())}
+assert len(targetClass2id_mergeProp) == 17
+
+# main.py:506-507: the default small_objects of --use_small_object_head
+SMALL_OBJECTS = ("Prop", "Push_Pulled_Object", "Prop_plus_Push_Pulled_Object", "Bike")
+
+
 def effdet_labels_to_coco80(labels):
     """obj_detect_tracking.py:644-647: EfficientDet's 1..90 category ids -> the detector's dense 1..80 class ids."""
     return [coco_obj_class_to_id[coco_id_mapping[int(l)]] for l in labels]

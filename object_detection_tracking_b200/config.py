@@ -59,6 +59,12 @@ _DEFAULTS = dict(
     use_att_frcnn_head=False,          # --use_att_frcnn_head (obj_detect_tracking.py:197-199): hidden + relu(att_trans(sum
                                        # of the ROI's 49 cells)) in the class-specific box head (models.py:1064-1089); the
                                        # class-agnostic heads have no attention branch (models.py:1126-1170)
+    use_small_object_head=False,       # main.py --use_small_object_head (:263): the per-class small-object branch of the
+                                       # single-image graph (models.py:590-692, 845-897), outputs so_final_*
+    use_so_association=False,          # --use_so_association (:273): person_object_relation on the branch's rows
+    use_so_score_thres=False,          # --use_so_score_thres (:264): the branch's final NMS filters logit > thres
+    so_person_topk=10,                 # --so_person_topk (:274): reference person boxes of the association
+    small_objects=None,                # class names, in so label order; None = class_ids.SMALL_OBJECTS (main.py:506-507)
     is_efficientdet=False,
 )
 
@@ -93,7 +99,54 @@ def normalize_config(cfg):
     cfg.result_score_thres = float(cfg.threshold_conf)               # :385
     cfg.num_anchors_per_loc = len(cfg.anchor_ratios)
     cfg.partial_class_ids = _partial_class_ids(cfg)
+    _small_object_ids(cfg)
     return cfg
+
+
+def _small_object_ids(cfg):
+    """With use_small_object_head: cfg.small_object_class_ids (the head's class ids of small_objects, in order) and, with
+    use_so_association, cfg.so_person_class_id.  Names resolve through config.classname2id when the caller set it, as the
+    reference does (models.py:604-605, 647), else through the merge-prop table the reference's main.py asserts
+    (main.py:508-521).  Off: () and 0."""
+    from .class_ids import SMALL_OBJECTS, targetClass2id_mergeProp
+    cfg.small_object_class_ids = ()
+    cfg.so_person_class_id = 0
+    if not cfg.use_small_object_head or cfg.is_efficientdet:
+        return
+    if cfg.small_objects is None:
+        cfg.small_objects = list(SMALL_OBJECTS)
+    table = getattr(cfg, "classname2id", None) or targetClass2id_mergeProp
+    names = list(cfg.small_objects)
+    nc = int(cfg.num_class)
+
+    def resolve(n):
+        if n == "BG":
+            raise ValueError("use_small_object_head: 'BG' cannot be a small object")
+        if n not in table:
+            raise ValueError("use_small_object_head: %r is not a class name of classname2id" % (n,))
+        i = int(table[n])
+        if not 1 <= i <= nc - 1:
+            raise ValueError("use_small_object_head: %r has id %d, outside 1..num_class-1 (num_class %d)" % (n, i, nc))
+        return i
+
+    if not names:
+        raise ValueError("use_small_object_head: small_objects is empty")
+    dup = sorted({n for n in names if names.count(n) > 1})
+    if dup:
+        raise ValueError("use_small_object_head: %s listed more than once" % ", ".join(repr(n) for n in dup))
+    for flag, why in (("use_frcnn_class_agnostic", "the reference's decode reshapes [N,1,4] box logits against "
+                       "[N,num_class-1,4] anchors and fails"),
+                      ("use_partial_classes", "the branch reads the full head's class columns"),
+                      ("use_conv_frcnn_head", "the branch would need its own fc6 / fc7 next to fastrcnn/fc")):
+        if getattr(cfg, flag, False):
+            raise ValueError("use_small_object_head cannot be combined with %s: %s" % (flag, why))
+    cfg.small_object_class_ids = tuple(resolve(n) for n in names)
+    if cfg.use_so_association:
+        if "Person" not in table:
+            raise ValueError("use_so_association needs a 'Person' class in classname2id (models.py:647)")
+        cfg.so_person_class_id = resolve("Person")
+        if int(cfg.so_person_topk) < 1:
+            raise ValueError("use_so_association: so_person_topk must be >= 1, got %d" % int(cfg.so_person_topk))
 
 
 def _partial_class_ids(cfg) -> tuple:

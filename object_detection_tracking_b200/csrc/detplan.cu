@@ -40,11 +40,13 @@ ConvIO images(const ConvLayer& L, int b0) {
 }
 
 ConvLayer* add_layer(DetPlan& p, int phase, const std::string& name, const Planes& in, ConvDesc d, ConvAffine affine,
-                     const Planes& out, const Planes* res, float* out_f32, int ldc_f32, Layout layout) {
+                     const Planes& out, const Planes* res, float* out_f32, int ldc_f32, Layout layout,
+                     const ConvLayer* shared = nullptr) {
   d.acc_kb = p.acc_kb;
   if (!res) d.res_shift = 0;
   // the CUDA-core kernel runs a grouped conv as the dense conv with block-diagonal weights
-  std::unique_ptr<ConvLayer> L = make_conv(p.arena, p.split, name, d, in, out, res, out_f32, ldc_f32, p.conv_impl != 0);
+  std::unique_ptr<ConvLayer> L = make_conv(p.arena, p.split, name, d, in, out, res, out_f32, ldc_f32, p.conv_impl != 0,
+                                           shared ? &shared->w : nullptr);
   L->bn = affine == kBatchNorm ? name + "/bn" : "";
   L->bias = affine == kBias ? name + "/b" : "";
   L->layout = layout;
@@ -107,6 +109,17 @@ void same_pads3(int h, int w, ConvDesc& d) {
 ConvLayer* add_conv(DetPlan& p, int phase, const std::string& name, const Planes& in, ConvDesc d, ConvAffine affine,
                     const Planes& out, const Planes* res, Layout layout) {
   return add_layer(p, phase, name, in, d, affine, out, res, nullptr, 0, layout);
+}
+
+ConvLayer* add_conv_shared(DetPlan& p, int phase, const std::string& name, const Planes& in, const ConvLayer& src,
+                           const Planes& out) {
+  if (src.d.R != 1 || src.d.S != 1 || in.C != src.d.Cin) {
+    set_error("b2_create: " + name + " does not match " + src.name);
+    return nullptr;
+  }
+  ConvDesc d = conv_desc(1, src.d.Cout);
+  d.relu = src.d.relu;
+  return add_layer(p, phase, name, in, d, kNoAffine, out, nullptr, nullptr, 0, kShared, &src);
 }
 
 ConvLayer* add_conv_f32(DetPlan& p, int phase, const std::string& name, const Planes& in, ConvDesc d, ConvAffine affine,
@@ -292,6 +305,53 @@ int add_relation(DetPlan& p, const std::string& name, int B, int K, int D, const
   Planes o = p.rel_o;
   o.W = M;
   add_conv(p, 5, name + "/output_linear", o, conv_desc(1, D), kNoAffine, out, &h, kDense);
+  return 0;
+}
+
+// person_object_relation (nn.py:194-270): the relation module's steps with the query rows of the C blocks attending to
+// the Tp key (person) rows, the value being the key rows themselves.  Steps:
+//   query_key          one N = 2D layer over all rows (query_linear | key_linear), fp32 output
+//   so_attend          V^T of the key rows into the P.V weights, then geometry + logits + softmax over the key rows -> P
+//   attention_value    one layer of 16 C Rq rows: P (rows q * 16 + g) times V^T, landing as the [C Rq][16D] flatten
+//   output_linear      dense 16D -> D over the flatten, the query rows added in the epilogue
+int add_so_association(DetPlan& p, int phase, const std::string& scope, int C, int Rq, int Tp, const float* boxes,
+                       const int* kq, const int* nref, const Planes& rows, const Planes& out) {
+  const int D = rows.C, Mq = C * Rq, M = Mq + Tp, G = kRelGroups;
+  const int Tpp = (Tp + 63) / 64 * 64, Mpad = (M + 127) / 128 * 128, Mqpad = (Mq + 127) / 128 * 128;
+  B2_CHECK(D % 64 == 0 && rows.W == M && out.W == Mq && out.C == D, "b2_create: person_object_relation rows do not match");
+  std::unique_ptr<RelOp> R(new RelOp());
+  R->name = scope;
+  R->geo = p.arena.alloc<float>(kRelGeoWeights);
+  float* qk = p.arena.alloc<float>(static_cast<size_t>(Mpad) * 2 * D);
+  Planes pp, o;
+  B2_CHECK(R->geo && qk && p.alloc_rows(pp, Mq * G, Tpp) && p.alloc_planes(o, 1, 1, Mqpad, G * D),
+           "out of device memory (person_object_relation)");
+  add_conv_f32(p, phase, scope + "/query_key", rows, conv_desc(1, 2 * D), kNoAffine, qk, 2 * D, kRelQK);
+  Planes ov = o;   // the P.V output: 16 rows of D per query row
+  ov.W = Mq * G; ov.C = D;
+  ConvLayer* pv = add_conv(p, phase, scope + "/attention_value", pp, conv_desc(1, D), kNoAffine, ov, nullptr, kRuntime);
+  SoAttendParams ap;
+  memset(&ap, 0, sizeof(ap));
+  ap.boxes = boxes; ap.kq = kq; ap.nref = nref;
+  ap.qk = qk; ap.ldqk = 2 * D; ap.D = D; ap.C = C; ap.Rq = Rq; ap.Tp = Tp; ap.Tpp = Tpp;
+  ap.rows = relation_rows_per_block(Tpp, D);
+  ap.geo = R->geo;
+  const size_t kv = static_cast<size_t>(Mq) * D;
+  ap.v_hi = rows.hi + kv; ap.v_lo = rows.lo ? rows.lo + kv : nullptr;
+  ap.p_hi = pp.hi; ap.p_lo = pp.lo;
+  ap.vt_hi = pv->w.w_hi; ap.vt_lo = pv->w.w_lo;
+  p.rels.push_back(std::move(R));
+  // the P.V layer was appended before the attend step it depends on: move the attend step in front of it
+  Step& s = add_batch_step(p, phase, kStepSoAttend, scope + "/attend [" + std::to_string(Mq) + "x" + std::to_string(Tp) + "x" +
+                                                       std::to_string(G) + "]",
+                           [ap](int, int, cudaStream_t st) { return so_attend_launch(ap, st); }, 2);
+  s.flops = 2.0 * Mq * Tp * (4.0 * kRelGeoDim + kRelGeoDim * G + D);
+  s.bytes = static_cast<double>(M) * 2 * D * 4 + (2.0 * D * Tpp + static_cast<double>(G) * Mq * Tpp) * (p.split ? 4.0 : 2.0);
+  std::rotate(p.steps.end() - 2, p.steps.end() - 1, p.steps.end());
+  o.W = Mq;
+  Planes hq = rows;
+  hq.W = Mq;
+  add_conv(p, phase, scope + "/output_linear", o, conv_desc(1, D), kNoAffine, out, &hq, kDense);
   return 0;
 }
 
@@ -544,7 +604,7 @@ int load_att(int C, const WeightSet& ws) {
 
 int load_layer(const ConvLayer* L, const WeightSet& ws, int num_class, const int* partial_ids, int num_partial,
                cudaStream_t st) {
-  if (L->layout == kRuntime) return 0;   // written by the pass itself
+  if (L->layout == kRuntime || L->layout == kShared) return 0;   // written by the pass itself / another layer's
   const int Cin = L->d.Cin, R = L->d.R, S = L->d.S, Cout = L->d.Cout, K = L->w.K, Cp = L->w.Cout_pad;
   std::vector<float> packed(static_cast<size_t>(Cp) * K, 0.f);
   std::vector<double> scale, shift;
@@ -612,6 +672,19 @@ int load_layer(const ConvLayer* L, const WeightSet& ws, int num_class, const int
     const float* wk = ws.get(scope + "/key_linear/W", static_cast<int64_t>(Cin) * Cin);
     if (!wq || !wk) return -1;
     relation_pack_qk(wq, wk, Cin, packed);
+  } else if (L->layout == kSoClass) {
+    // the per-class [D, 2] layers of the small-object branch (models.py:682-689): class i's columns at 2i, 2i + 1
+    for (int i = 0; i < Cout / 2; ++i) {
+      const std::string n = "fastrcnn/small_objects/small_object_classification_c" + std::to_string(i + 1);
+      const float* w = ws.get(n + "/W", static_cast<int64_t>(Cin) * 2);
+      const float* bb = ws.get(n + "/b", 2);
+      if (!w || !bb) return -1;
+      for (int o = 0; o < 2; ++o) {
+        for (int k = 0; k < Cin; ++k) packed[static_cast<size_t>(2 * i + o) * K + k] = w[static_cast<size_t>(k) * 2 + o];
+        b[2 * i + o] = bb[o];
+      }
+    }
+    has_b = false;
   } else if (L->layout == kDense) {
     const float* w = ws.get(L->name + "/W", static_cast<int64_t>(Cin) * Cout);
     if (!w) return -1;

@@ -45,6 +45,9 @@ enum Layout {
   kGrouped = 7,  // grouped conv HWIO [R][S][Cin/groups][Cout] (pack_grouped)
   kRelQK = 8,    // relation module: <scope>/query_linear/W | <scope>/key_linear/W fused along N (relation_pack_qk)
   kRuntime = 9,  // relation module P.V: the weights are the image's V^T, written by the attention step every pass
+  kShared = 10,  // another layer's packed weights (add_conv_shared): nothing of its own to load
+  kSoClass = 11, // small-object classification: fastrcnn/small_objects/small_object_classification_c{i+1}/{W,b}, [D, 2]
+                 // each, as columns 2i, 2i + 1
 };
 
 // The checkpoint's per-channel affine of a conv output, applied in the epilogue: none, the folded BatchNorm "<name>/bn"
@@ -61,7 +64,9 @@ enum ConvAffine { kNoAffine, kBatchNorm, kBias };
   X(kStepMaskSelect, 9, "mask_select") X(kStepGnStats, 10, "gn_stats") X(kStepGnApply, 11, "gn_apply")            \
   X(kStepGnRoi, 12, "gn_roi") X(kStepSeSqueeze, 13, "se_squeeze") X(kStepSeExcite, 14, "se_excite")               \
   X(kStepSeApply, 15, "se_apply") X(kStepRelationAttend, 16, "relation_attend") X(kStepDeformSample, 17, "deform_sample") \
-  X(kStepAttPool, 18, "att_pool") X(kStepAttSum, 19, "att_sum")
+  X(kStepAttPool, 18, "att_pool") X(kStepAttSum, 19, "att_sum") X(kStepSoSelect, 20, "so_select")             \
+  X(kStepSoGather, 21, "so_gather") X(kStepSoRoialign, 22, "so_roialign") X(kStepSoAttend, 23, "so_attend")       \
+  X(kStepSoFinish, 24, "so_finish")
 enum StepKind {
 #define B2_STEP_KIND_VALUE(e, v, n) e = v,
   B2_STEP_KINDS(B2_STEP_KIND_VALUE)
@@ -126,6 +131,10 @@ void same_pads3(int h, int w, ConvDesc& d);
 // writing the planes `out`, with `res` (read at (y >> d.res_shift, x >> d.res_shift)) added in the epilogue when given.
 ConvLayer* add_conv(DetPlan& p, int phase, const std::string& name, const Planes& in, ConvDesc d, ConvAffine affine,
                     const Planes& out, const Planes* res = nullptr, Layout layout = kHwio);
+// A dense layer that runs `src`'s packed weights and epilogue (bias, ReLU) over other rows: `in` has src's input width
+// (nullptr with the error set otherwise).
+ConvLayer* add_conv_shared(DetPlan& p, int phase, const std::string& name, const Planes& in, const ConvLayer& src,
+                           const Planes& out);
 // The same with an fp32 output: rows of stride `ldc` at `out_f32`.
 ConvLayer* add_conv_f32(DetPlan& p, int phase, const std::string& name, const Planes& in, ConvDesc d, ConvAffine affine,
                         float* out_f32, int ldc, Layout layout = kHwio);
@@ -141,6 +150,11 @@ int add_se(DetPlan& p, int phase, const std::string& name, const Planes& buf, co
 // [B][K][4] and `count` [B] on the device: out = h + output_linear(P . h).
 int add_relation(DetPlan& p, const std::string& name, int B, int K, int D, const float* boxes, const int* count,
                  const Planes& h, const Planes& out);
+// person_object_relation `scope` (nn.py:194-270, use_so_association) over `rows` ([C * Rq + Tp][D] planes: C blocks of Rq
+// query rows, then Tp key rows) with their boxes [C * Rq + Tp][4] on the device; *kq query rows of each block and *nref
+// key rows are valid (device ints).  out ([C * Rq][D]) = query rows + output_linear(P . key rows).
+int add_so_association(DetPlan& p, int phase, const std::string& scope, int C, int Rq, int Tp, const float* boxes,
+                       const int* kq, const int* nref, const Planes& rows, const Planes& out);
 // The attention branch of the class-specific box head (use_att_frcnn_head) over the head rows `hidden` ([M][D] rows):
 // out = hidden + relu(att_trans(sum over the 49 bins of roi)), roi the ROIAlign planes [M][49][C]; `pooled` ([M][C]) and
 // `att` ([M][D]) are its intermediate rows.

@@ -95,4 +95,24 @@ __device__ __forceinline__ int block_nms_sorted(const float4* boxes, int n, floa
   return *s_count;
 }
 
+// decode_bbox_target (nn.py:1518-1538) of the box logits t[0..3] (divided by the regression weights here) against the
+// ROI x1 y1 x2 y2: unclipped.  Explicit rounding intrinsics, so the box is the same in every kernel that inlines it.
+__device__ __forceinline__ float4 decode_box(const float* t, const float reg_w[4], float decode_clip, float4 roi) {
+  const float wa = __fsub_rn(roi.z, roi.x), ha = __fsub_rn(roi.w, roi.y);
+  const float xa = __fmul_rn(__fadd_rn(roi.z, roi.x), 0.5f), ya = __fmul_rn(__fadd_rn(roi.w, roi.y), 0.5f);
+  const float tx = __fdiv_rn(t[0], reg_w[0]), ty = __fdiv_rn(t[1], reg_w[1]);
+  const float tw = __fdiv_rn(t[2], reg_w[2]), th = __fdiv_rn(t[3], reg_w[3]);
+  const float wb = __fmul_rn(expf(fminf(tw, decode_clip)), wa);
+  const float hb = __fmul_rn(expf(fminf(th, decode_clip)), ha);
+  const float xb = __fadd_rn(__fmul_rn(tx, wa), xa), yb = __fadd_rn(__fmul_rn(ty, ha), ya);
+  return make_float4(__fsub_rn(xb, __fmul_rn(wb, 0.5f)), __fsub_rn(yb, __fmul_rn(hb, 0.5f)),
+                     __fadd_rn(xb, __fmul_rn(wb, 0.5f)), __fadd_rn(yb, __fmul_rn(hb, 0.5f)));
+}
+
+// clip_boxes (nn.py:1339-1346): max(., 0), then min(., [w, h, w, h])
+__device__ __forceinline__ float4 clip_box(float4 b, float img_w, float img_h) {
+  return make_float4(fminf(fmaxf(b.x, 0.f), img_w), fminf(fmaxf(b.y, 0.f), img_h), fminf(fmaxf(b.z, 0.f), img_w),
+                     fminf(fmaxf(b.w, 0.f), img_h));
+}
+
 }  // namespace b2

@@ -102,6 +102,7 @@ struct b2_ctx {
   b2_config_ext ext;       // options appended after b2_config's layout was fixed (b2_create_ex)
   b2_config_ext2 ext2;     // and after b2_config_ext's (b2_create_ex2)
   b2_config_ext3 ext3;     // and after b2_config_ext2's (b2_create_ex3)
+  b2_config_ext4 ext4;     // and after b2_config_ext3's (b2_create_ex4)
   int device = 0, num_sms = 132;
   cudaStream_t stream = nullptr;
   // geometry
@@ -130,6 +131,10 @@ struct b2_ctx {
   Planes head_a, head_b;           // conv box head (cfg.conv_head_dim > 0): [M][7][7][conv_head_dim] ping-pong
   Planes rm1, rm2;                 // relation modules (cfg.add_relation_nn): their sums
   Planes att_pool, att, att_sum;   // attention head (ext3.use_att_frcnn_head): bin sums [M][256], relu(att_trans), the sum
+  // small-object branch (ext4.use_small_object_head): its parameters, rows and final selection
+  SoParams so;
+  HeadPostParams so_fin;
+  Planes so_roi, so_fc6, so_fc7, so_asso;
   float* head_logits = nullptr;
   float* box_feat = nullptr;
   float* box_feat_pooled = nullptr;
@@ -176,6 +181,134 @@ void cell_anchors(float stride, float size, const float* ratios, float out[3][4]
     out[i][2] = static_cast<float>(cx + 0.5 * (W - 1));
     out[i][3] = static_cast<float>(cy + 0.5 * (H - 1));
   }
+}
+
+// The small-object branch (models.py:590-692, 845-897), phase 6 after the head's post-processing.  Rows: C blocks of
+// R = result_per_im rows (small class i's NMS selections, in selection order), then Tp = so_person_topk person rows with
+// use_so_association.  Steps:
+//   so_select     the C (+ Person) class columns of the head: probabilities and unclipped decoded boxes; per-class NMS
+//                 without a score threshold, at most R per small class and Tp for Person (head.cu's class_nms_kernel)
+//   so_gather     the rows' boxes; K = the small classes' common count, or 0 with status 1 when they differ
+//   so_roialign   ROIAlign 7 of the rows (unclipped boxes: samples outside the level read 0, as crop_and_resize)
+//   fc6, fc7      the head's own layers (same packed weights) over all rows
+//   association   person_object_relation of the C * R rows against the person rows (add_so_association)
+//   classification one N = 2C fp32 layer over the C * R rows; row block i keeps its columns 2i, 2i + 1
+//   so_finish     the [K][C + 1] logits and clipped [K][C][4] boxes, then the head's per-class NMS and top-k over them,
+//                 with the score threshold only with use_so_score_thres: the scores are logits, not probabilities
+int add_small_objects(b2_ctx* c, const ConvLayer* fc6, const ConvLayer* fc7) {
+  const b2_config& cfg = c->cfg;
+  const b2_config_ext4& e = c->ext4;
+  DetPlan& P = c->plan;
+  B2_CHECK(fc6 && fc7, "b2_create: use_small_object_head needs the 2fc box head");
+  const int C = e.num_small_objects, R = cfg.result_per_im, K = cfg.rpn_topk, nc = cfg.fpn_num_channel;
+  const int Tp = e.use_so_association ? e.so_person_topk : 0, SR = C * R + Tp, dim = cfg.fc_head_dim;
+  const HeadPostParams& hp = c->post;
+  SoParams& sp = c->so;
+  memset(&sp, 0, sizeof(sp));
+  sp.logits = hp.logits; sp.ld = hp.ld; sp.num_class = hp.num_class; sp.rois = K;
+  sp.roi_boxes = hp.rois; sp.roi_count = hp.roi_count; sp.probs = hp.probs;
+  for (int i = 0; i < 4; ++i) sp.reg_w[i] = hp.reg_w[i];
+  sp.decode_clip = hp.decode_clip; sp.img_w = hp.img_w; sp.img_h = hp.img_h;
+  sp.C = C; sp.R = R; sp.Tp = Tp;
+  for (int i = 0; i < C; ++i) sp.ids[i] = e.small_object_class_ids[i];
+  if (Tp) sp.ids[C] = e.so_person_class_id;
+  sp.sel_probs = P.arena.alloc<float>(static_cast<size_t>(K) * (C + 2));
+  sp.sel_boxes = P.arena.alloc<float>(static_cast<size_t>(K) * (C + 1) * 4);
+  int* keep = P.arena.alloc<int>(static_cast<size_t>(C + 1) * R);
+  int* pkeep = P.arena.alloc<int>(static_cast<size_t>(C + 1) * std::max(Tp, 1));
+  int* sel_count = P.arena.alloc<int>(C + 1);
+  sp.keep = keep; sp.person_keep = pkeep + static_cast<size_t>(C) * Tp; sp.sel_count = sel_count;
+  sp.rows_boxes = P.arena.alloc<float>(static_cast<size_t>(SR) * 4);
+  sp.row_count = P.arena.alloc<int>(C + 1);
+  sp.k = P.arena.alloc<int>(1);
+  sp.status = P.arena.alloc<int>(1);
+  B2_CHECK(sp.sel_probs && sp.sel_boxes && keep && pkeep && sel_count && sp.rows_boxes && sp.row_count && sp.k && sp.status,
+           "out of device memory (small-object selection)");
+  // the selection's NMS: head.cu's kernel over the gathered columns, class s at dec_boxes column s, probs column s + 1
+  HeadPostParams sel = hp;
+  sel.probs = sp.sel_probs; sel.dec_boxes = sp.sel_boxes; sel.num_class = C + 2;
+  sel.score_thresh = -INFINITY;   // nms_return_boxes / the person NMS have no score threshold (models.py:1240-1250, 654-656)
+  sel.max_per_class = R; sel.cls_keep = keep; sel.cls_count = sel_count;
+  HeadPostParams psel = sel;
+  psel.max_per_class = std::max(Tp, 1); psel.cls_keep = pkeep;
+  Step& s1 = add_batch_step(P, 6, kStepSoSelect, "", [c, sel, psel](int, int, cudaStream_t st) {
+    if (so_select_launch(c->so, st) || class_nms_launch(sel, 0, c->so.C, st)) return -1;
+    return c->so.Tp ? class_nms_launch(psel, c->so.C, 1, st) : 0;
+  }, Tp ? 3 : 2);
+  s1.bytes = static_cast<double>(K) * (hp.ld + 2.0 * (C + 2) + 8.0 * (C + 1)) * 4;
+  add_batch_step(P, 6, kStepSoGather, "", [c](int, int, cudaStream_t st) { return so_gather_launch(c->so, st); });
+  // ROIAlign of the rows: the C class blocks as C groups of R rows (of the one image), then the Tp person rows
+  B2_CHECK(P.alloc_rows(c->so_roi, SR, 49 * nc) && P.alloc_rows(c->so_fc6, SR, dim) && P.alloc_rows(c->so_fc7, SR, dim),
+           "alloc small-object rows");
+  RoiAlignParams ra = c->roi1;
+  ra.B = C; ra.rois_per_image = R; ra.one_image = 1;
+  ra.boxes = sp.rows_boxes; ra.count = sp.row_count;
+  ra.out_hi = c->so_roi.hi; ra.out_lo = c->so_roi.lo;
+  RoiAlignParams rb = ra;
+  const size_t off = static_cast<size_t>(C) * R * 49 * nc;
+  rb.B = 1; rb.rois_per_image = Tp;
+  rb.boxes = sp.rows_boxes + static_cast<size_t>(C) * R * 4; rb.count = sp.row_count + C;
+  rb.out_hi = c->so_roi.hi + off; rb.out_lo = c->so_roi.lo ? c->so_roi.lo + off : nullptr;
+  add_batch_step(P, 6, kStepSoRoialign, "", [ra, rb](int, int, cudaStream_t st) {
+    if (roialign_launch(ra, st)) return -1;
+    return rb.rois_per_image > 0 ? roialign_launch(rb, st) : 0;
+  }, Tp ? 2 : 1).bytes = static_cast<double>(SR) * 49 * nc * (P.split ? 4.0 : 2.0) * 2;
+  if (!add_conv_shared(P, 6, "fastrcnn/small_objects/fc6", c->so_roi, *fc6, c->so_fc6) ||
+      !add_conv_shared(P, 6, "fastrcnn/small_objects/fc7", c->so_fc6, *fc7, c->so_fc7))
+    return -1;
+  Planes hidden = c->so_fc7;
+  hidden.W = C * R;
+  if (Tp) {
+    B2_CHECK(P.alloc_rows(c->so_asso, C * R, dim), "alloc small-object association rows");
+    if (add_so_association(P, 6, "fastrcnn/small_objects/person_object_relation", C, R, Tp, sp.rows_boxes, sp.k,
+                           sp.row_count + C, c->so_fc7, c->so_asso))
+      return -1;
+    hidden = c->so_asso;
+  }
+  sp.ldl = (2 * C + 15) / 16 * 16;
+  float* cls = P.arena.alloc<float>(static_cast<size_t>((C * R + 127) / 128 * 128) * sp.ldl);
+  sp.fin_logits = P.arena.alloc<float>(static_cast<size_t>(R) * (C + 1));
+  sp.fin_boxes = P.arena.alloc<float>(static_cast<size_t>(R) * C * 4);
+  sp.cls_logits = cls;
+  add_conv_f32(P, 6, "fastrcnn/small_objects/classification", hidden, conv_desc(1, 2 * C), kBias, cls, sp.ldl, kSoClass);
+  HeadPostParams& fin = c->so_fin;
+  memset(&fin, 0, sizeof(fin));
+  fin.probs = sp.fin_logits; fin.dec_boxes = sp.fin_boxes; fin.num_class = C + 1; fin.B = 1; fin.rois_per_image = R;
+  fin.roi_count = sp.k;
+  fin.score_thresh = e.use_so_score_thres ? cfg.result_score_thres : -INFINITY;   // models.py:880-884
+  fin.nms_thr = cfg.fastrcnn_nms_iou_thres;
+  fin.max_per_class = R; fin.max_total = R;
+  fin.cls_keep = P.arena.alloc<int>(static_cast<size_t>(C) * R);
+  fin.cls_count = P.arena.alloc<int>(C);
+  fin.final_boxes = P.arena.alloc<float>(static_cast<size_t>(R) * 4);
+  fin.final_probs = P.arena.alloc<float>(R);
+  fin.final_labels = P.arena.alloc<int>(R);
+  fin.final_count = P.arena.alloc<int>(1);
+  B2_CHECK(cls && sp.fin_logits && sp.fin_boxes && fin.cls_keep && fin.cls_count && fin.final_boxes && fin.final_probs &&
+               fin.final_labels && fin.final_count, "out of device memory (small-object outputs)");
+  add_batch_step(P, 6, kStepSoFinish, "", [c](int, int, cudaStream_t st) {
+    if (so_finish_launch(c->so, st)) return -1;
+    return head_select_launch(c->so_fin, st);
+  }, 3);
+  P.stages.raw("so_sel_probs", sp.sel_probs, Stage::kF32, K, C + 2, 1, 1);
+  P.stages.raw("so_sel_boxes", sp.sel_boxes, Stage::kF32, K, C + 1, 4, 1);
+  P.stages.raw("so_sel_count", sel_count, Stage::kI32, C + 1, 1, 1, 1);
+  P.stages.raw("so_keep", keep, Stage::kI32, C, R, 1, 1);
+  P.stages.raw("so_person_keep", pkeep + static_cast<size_t>(C) * Tp, Stage::kI32, std::max(Tp, 1), 1, 1, 1);
+  P.stages.raw("so_status", sp.status, Stage::kI32, 1, 1, 1, 1);
+  P.stages.raw("so_k", sp.k, Stage::kI32, 1, 1, 1, 1);
+  P.stages.raw("so_boxes", sp.rows_boxes, Stage::kF32, SR, 4, 1, 1);
+  P.stages.planes("so_roi_feat", c->so_roi);
+  P.stages.planes("so_fc6", c->so_fc6);
+  P.stages.planes("so_fc7", c->so_fc7);
+  if (Tp) P.stages.planes("so_asso", c->so_asso);
+  P.stages.raw("so_cls_logits", cls, Stage::kF32, C * R, sp.ldl, 1, 1);
+  P.stages.raw("so_logits", sp.fin_logits, Stage::kF32, R, C + 1, 1, 1);
+  P.stages.raw("so_final_boxes", fin.final_boxes, Stage::kF32, R, 4, 1, 1);
+  P.stages.raw("so_final_probs", fin.final_probs, Stage::kF32, R, 1, 1, 1);
+  P.stages.raw("so_final_labels", fin.final_labels, Stage::kI32, R, 1, 1, 1);
+  P.stages.raw("so_final_count", fin.final_count, Stage::kI32, 1, 1, 1, 1);
+  return 0;
 }
 
 int build_plan(b2_ctx* c) {
@@ -435,6 +568,7 @@ int build_plan(b2_ctx* c) {
     B2_CHECK(P.alloc_rows(c->att_pool, M, nc) && P.alloc_rows(c->att, M, dim) && P.alloc_rows(c->att_sum, M, dim),
              "alloc attention head");
   Planes head_in;   // the rows fastrcnn/outputs reads
+  const ConvLayer *head_fc6 = nullptr, *head_fc7 = nullptr;   // the 2fc head's layers (the small-object branch runs them)
   auto attend = [&](const Planes& hidden) {
     head_in = att ? c->att_sum : hidden;
     return att ? add_att_head(P, c->roi_feat, nc, hidden, c->att_pool, c->att, c->att_sum) : 0;
@@ -477,9 +611,9 @@ int build_plan(b2_ctx* c) {
       h1 = c->rm1;
       h2 = c->rm2;
     }
-    add_conv(P, 5, "fastrcnn/fc6", rf, fc, kBias, f6, nullptr, kFc6);
+    head_fc6 = add_conv(P, 5, "fastrcnn/fc6", rf, fc, kBias, f6, nullptr, kFc6);
     if (rel && add_relation(P, "fastrcnn/RM_r1", B, K, dim, rp.prop_boxes, rp.prop_count, f6, h1)) return -1;
-    add_conv(P, 5, "fastrcnn/fc7", h1, fc, kBias, f7, nullptr, kDense);
+    head_fc7 = add_conv(P, 5, "fastrcnn/fc7", h1, fc, kBias, f7, nullptr, kDense);
     if (rel && add_relation(P, "fastrcnn/RM_r2", B, K, dim, rp.prop_boxes, rp.prop_count, f7, h2)) return -1;
     if (attend(h2)) return -1;
     add_conv_f32(P, 5, "fastrcnn/outputs", head_in, conv_desc(1, nout), kBias, c->head_logits, ldo, kHeadOut);
@@ -521,6 +655,7 @@ int build_plan(b2_ctx* c) {
   P.stages.raw("final_probs", hp.final_probs, Stage::kF32, B, R, 1, 1);
   P.stages.raw("final_labels", hp.final_labels, Stage::kI32, B, R, 1, 1);
   P.stages.raw("final_count", hp.final_count, Stage::kI32, B, 1, 1, 1);
+  if (c->ext4.use_small_object_head && add_small_objects(c, head_fc6, head_fc7)) return -1;
 
   // ---- fpn_box_feat: ROIAlign of the final boxes (models.py:972-973), phase 7 ----
   c->box_feat = P.arena.alloc<float>(static_cast<size_t>(B) * R * nc * 49);
@@ -638,6 +773,11 @@ int b2_create_ex2(b2_ctx** out, int device, const b2_config* cfg, const b2_confi
 
 int b2_create_ex3(b2_ctx** out, int device, const b2_config* cfg, const b2_config_ext* ext, const b2_config_ext2* ext2,
                   const b2_config_ext3* ext3) {
+  return b2_create_ex4(out, device, cfg, ext, ext2, ext3, nullptr);
+}
+
+int b2_create_ex4(b2_ctx** out, int device, const b2_config* cfg, const b2_config_ext* ext, const b2_config_ext2* ext2,
+                  const b2_config_ext3* ext3, const b2_config_ext4* ext4) {
   B2_CHECK(out && cfg, "b2_create: null argument");
   *out = nullptr;
   std::unique_ptr<b2_ctx> c(new b2_ctx());
@@ -648,6 +788,8 @@ int b2_create_ex3(b2_ctx** out, int device, const b2_config* cfg, const b2_confi
   if (ext2) c->ext2 = *ext2;
   memset(&c->ext3, 0, sizeof(c->ext3));
   if (ext3) c->ext3 = *ext3;
+  memset(&c->ext4, 0, sizeof(c->ext4));
+  if (ext4) c->ext4 = *ext4;
   const int np = c->ext2.num_partial_classes;
   B2_CHECK(np >= 0 && np <= cfg->num_class - 1 && np <= 80,
            "b2_create: num_partial_classes must be 0 (off) or 1 .. min(num_class - 1, 80) (num_class " +
@@ -659,6 +801,33 @@ int b2_create_ex3(b2_ctx** out, int device, const b2_config* cfg, const b2_confi
     for (int j = 0; j < i; ++j)
       B2_CHECK(c->ext2.partial_class_ids[j] != id, "b2_create: class id " + std::to_string(id) +
                                                       " appears twice in partial_class_ids");
+  }
+  const b2_config_ext4& so = c->ext4;
+  if (so.use_small_object_head) {
+    const std::string who = "b2_create: use_small_object_head ";
+    B2_CHECK(!cfg->class_agnostic, who + "cannot be combined with use_frcnn_class_agnostic: the reference's decode reshapes "
+                                         "[N,1,4] box logits against [N,num_class-1,4] anchors and fails");
+    B2_CHECK(np == 0, who + "cannot be combined with use_partial_classes: the branch reads the full head's class columns");
+    B2_CHECK(cfg->conv_head_dim <= 0, who + "cannot be combined with use_conv_frcnn_head: the branch would need its own "
+                                             "fc6 / fc7 next to fastrcnn/fc");
+    B2_CHECK(cfg->batch == 1 && !cfg->multi_semantics, who + "needs batch 1 and the single-image graph: the batch graph "
+                                                             "(Mask_RCNN_FPN_multi) has no small-object branch");
+    const int C = so.num_small_objects;
+    B2_CHECK(C >= 1 && C <= cfg->num_class - 1 && C <= 80, who + "num_small_objects must be 1 .. min(num_class - 1, 80), got " +
+                                                              std::to_string(C));
+    for (int i = 0; i < C; ++i) {
+      const int id = so.small_object_class_ids[i];
+      B2_CHECK(id >= 1 && id <= cfg->num_class - 1, who + "small_object_class_ids[" + std::to_string(i) + "] = " +
+                                                        std::to_string(id) + " is not a class id in 1 .. num_class - 1");
+      for (int j = 0; j < i; ++j)
+        B2_CHECK(so.small_object_class_ids[j] != id, who + "class id " + std::to_string(id) + " appears twice");
+    }
+    if (so.use_so_association) {
+      B2_CHECK(so.so_person_class_id >= 1 && so.so_person_class_id <= cfg->num_class - 1,
+               who + "so_person_class_id " + std::to_string(so.so_person_class_id) + " is not a class id in 1 .. num_class - 1");
+      B2_CHECK(so.so_person_topk >= 1 && so.so_person_topk <= 1024,
+               who + "so_person_topk must be 1 .. 1024, got " + std::to_string(so.so_person_topk));
+    }
   }
   c->device = device;
   c->plan.split = cfg->precision == 1;
@@ -1020,6 +1189,23 @@ int b2_get_masks(b2_ctx* c, float* masks_host, int64_t capacity_bytes) {
   B2_CHECK(capacity_bytes >= bytes, "b2_get_masks: buffer too small");
   B2_CUDA(cudaMemcpyAsync(masks_host, c->final_masks, bytes, cudaMemcpyDeviceToHost, c->stream));
   B2_CUDA(cudaStreamSynchronize(c->stream));
+  return 0;
+}
+
+int b2_get_small_objects(b2_ctx* c, float* boxes, float* probs, int32_t* labels, int32_t* count, int32_t* class_counts,
+                         int32_t* status) {
+  B2_CHECK(c && boxes && probs && labels && count && class_counts && status, "b2_get_small_objects: null argument");
+  B2_CHECK(c->ext4.use_small_object_head, "b2_get_small_objects: the context was created without use_small_object_head");
+  B2_CUDA(cudaSetDevice(c->device));
+  const int R = c->cfg.result_per_im, C = c->so.C;
+  cudaStream_t st = c->stream;
+  B2_CUDA(cudaMemcpyAsync(boxes, c->so_fin.final_boxes, sizeof(float) * R * 4, cudaMemcpyDeviceToHost, st));
+  B2_CUDA(cudaMemcpyAsync(probs, c->so_fin.final_probs, sizeof(float) * R, cudaMemcpyDeviceToHost, st));
+  B2_CUDA(cudaMemcpyAsync(labels, c->so_fin.final_labels, sizeof(int32_t) * R, cudaMemcpyDeviceToHost, st));
+  B2_CUDA(cudaMemcpyAsync(count, c->so_fin.final_count, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+  B2_CUDA(cudaMemcpyAsync(class_counts, c->so.sel_count, sizeof(int32_t) * C, cudaMemcpyDeviceToHost, st));
+  B2_CUDA(cudaMemcpyAsync(status, c->so.status, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+  B2_CUDA(cudaStreamSynchronize(st));
   return 0;
 }
 

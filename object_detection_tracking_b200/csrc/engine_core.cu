@@ -40,7 +40,7 @@ Planes Arena::planes(int B, int H, int W, int C, bool split, int creal) {
 
 std::unique_ptr<ConvLayer> make_conv(Arena& a, bool split, const std::string& name, ConvDesc d, const Planes& in,
                                      const Planes& out, const Planes* res, float* out_f32, int ldc_f32,
-                                     bool dense_groups) {
+                                     bool dense_groups, const ConvWeights* shared) {
   std::unique_ptr<ConvLayer> L(new ConvLayer());
   L->name = name;
   d.B = in.B; d.Cin = in.C;
@@ -56,9 +56,13 @@ std::unique_ptr<ConvLayer> make_conv(Arena& a, bool split, const std::string& na
   L->d = d;
   L->w.Cout_pad = (d.Cout + 15) / 16 * 16;
   L->w.K = d.R * d.S * (d.groups > 1 && !dense_groups ? kGroupWindow : in.C);
-  L->w.w_hi = a.alloc<__half>(static_cast<size_t>(L->w.Cout_pad) * L->w.K);
-  L->w.w_lo = split ? a.alloc<__half>(static_cast<size_t>(L->w.Cout_pad) * L->w.K) : nullptr;
-  L->w.bias = a.alloc<float>(L->w.Cout_pad);
+  if (shared && shared->K == L->w.K && shared->Cout_pad == L->w.Cout_pad) {
+    L->w = *shared;
+  } else if (!shared) {
+    L->w.w_hi = a.alloc<__half>(static_cast<size_t>(L->w.Cout_pad) * L->w.K);
+    L->w.w_lo = split ? a.alloc<__half>(static_cast<size_t>(L->w.Cout_pad) * L->w.K) : nullptr;
+    L->w.bias = a.alloc<float>(L->w.Cout_pad);
+  }   // a mismatched `shared` leaves the weights null: plan_convs refuses the layer
   L->io.in_hi = in.hi; L->io.in_lo = in.lo;
   L->io.out_hi = out.hi; L->io.out_lo = out.lo; L->io.out_f32 = out_f32;
   if (res) { L->io.res_hi = res->hi; L->io.res_lo = res->lo; }

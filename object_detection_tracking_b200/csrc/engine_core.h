@@ -81,9 +81,10 @@ struct ConvLayer {
 // weights [Cout_pad][R*S*Cin] (a grouped conv: [Cout_pad][R*S*kGroupWindow], or with `dense_groups` the dense
 // block-diagonal expansion the CUDA-core kernel reads).  Caller fills R, S, stride, dilation, pads, Cout, groups,
 // epilogue and placement in `d`.
+// With `shared` the layer runs those packed weights (another layer's, of the same K and Cout) and allocates none.
 std::unique_ptr<ConvLayer> make_conv(Arena& a, bool split, const std::string& name, ConvDesc d, const Planes& in,
                                      const Planes& out, const Planes* res = nullptr, float* out_f32 = nullptr,
-                                     int ldc_f32 = 0, bool dense_groups = false);
+                                     int ldc_f32 = 0, bool dense_groups = false, const ConvWeights* shared = nullptr);
 // Creates the full-batch plan of every layer.
 int plan_convs(const std::vector<std::unique_ptr<ConvLayer>>& layers, bool split, int num_sms);
 

@@ -30,30 +30,15 @@ __global__ void head_decode_kernel(const __grid_constant__ HeadPostParams p) {
   }
   for (int c = 0; c < nc; ++c) pr[c] = __fdiv_rn(pr[c], sum);
   const float4 roi = reinterpret_cast<const float4*>(p.rois)[r];
-  const float wa = __fsub_rn(roi.z, roi.x), ha = __fsub_rn(roi.w, roi.y);
-  const float xa = __fmul_rn(__fadd_rn(roi.z, roi.x), 0.5f), ya = __fmul_rn(__fadd_rn(roi.w, roi.y), 0.5f);
   float4* ob = reinterpret_cast<float4*>(p.dec_boxes) + static_cast<size_t>(r) * (nc - 1);
-  for (int c = 1; c < nc; ++c) {
-    const float* t = lg + nc + (p.class_agnostic ? 0 : c * 4);
-    const float tx = __fdiv_rn(t[0], p.reg_w[0]), ty = __fdiv_rn(t[1], p.reg_w[1]);
-    const float tw = __fdiv_rn(t[2], p.reg_w[2]), th = __fdiv_rn(t[3], p.reg_w[3]);
-    const float wb = __fmul_rn(expf(fminf(tw, p.decode_clip)), wa);
-    const float hb = __fmul_rn(expf(fminf(th, p.decode_clip)), ha);
-    const float xb = __fadd_rn(__fmul_rn(tx, wa), xa), yb = __fadd_rn(__fmul_rn(ty, ha), ya);
-    float x1 = __fsub_rn(xb, __fmul_rn(wb, 0.5f)), y1 = __fsub_rn(yb, __fmul_rn(hb, 0.5f));
-    float x2 = __fadd_rn(xb, __fmul_rn(wb, 0.5f)), y2 = __fadd_rn(yb, __fmul_rn(hb, 0.5f));
-    x1 = fminf(fmaxf(x1, 0.f), p.img_w);
-    y1 = fminf(fmaxf(y1, 0.f), p.img_h);
-    x2 = fminf(fmaxf(x2, 0.f), p.img_w);
-    y2 = fminf(fmaxf(y2, 0.f), p.img_h);
-    ob[c - 1] = make_float4(x1, y1, x2, y2);
-  }
+  for (int c = 1; c < nc; ++c)
+    ob[c - 1] = clip_box(decode_box(lg + nc + (p.class_agnostic ? 0 : c * 4), p.reg_w, p.decode_clip, roi), p.img_w, p.img_h);
 }
 
-// grid (num_class-1, B): per-class NMS over the ROIs of one image
-__global__ void __launch_bounds__(512) class_nms_kernel(const __grid_constant__ HeadPostParams p, int KP) {
+// grid (classes, B): per-class NMS over the ROIs of one image, classes c0, c0 + 1, ...
+__global__ void __launch_bounds__(512) class_nms_kernel(const __grid_constant__ HeadPostParams p, int KP, int c0) {
   extern __shared__ __align__(16) uint8_t sm[];
-  const int c = blockIdx.x, b = blockIdx.y, tid = threadIdx.x;
+  const int c = c0 + blockIdx.x, b = blockIdx.y, tid = threadIdx.x;
   const int nc = p.num_class, R = p.rois_per_image;
   uint64_t* keys = reinterpret_cast<uint64_t*>(sm);          // [KP]
   float4* boxes = reinterpret_cast<float4*>(keys + KP);      // [KP]
@@ -138,32 +123,49 @@ int next_pow2(int v) {
 
 }  // namespace
 
-int head_post_launch(const HeadPostParams& p, cudaStream_t s) {
-  const int R = p.rois_per_image, nc1 = p.num_class - 1;
+int class_nms_launch(const HeadPostParams& p, int c0, int n, cudaStream_t s) {
+  const int R = p.rois_per_image;
   B2_CHECK(R <= 1024, "head: at most 1024 ROIs per image");
-  const int total = p.B * R;
-  head_decode_kernel<<<(total + 127) / 128, 128, 0, s>>>(p);
-  B2_CUDA(cudaGetLastError());
+  B2_CHECK(c0 >= 0 && n >= 1 && c0 + n <= p.num_class - 1, "head: class range outside the classes");
   // at least 2 keys, so that the float4 boxes after the 8-byte keys start 16-byte aligned (one ROI per image would put
   // them at 8)
   const int KP = next_pow2(R) < 2 ? 2 : next_pow2(R);
   const size_t smem1 = static_cast<size_t>(KP) * (8 + 16 + 4 + 4) + static_cast<size_t>(R) * ((R + 31) / 32) * 4;
+  static bool attr_set = false;
+  if (!attr_set) {
+    B2_CUDA(cudaFuncSetAttribute(class_nms_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
+    attr_set = true;
+  }
+  B2_CHECK(smem1 <= 200 * 1024, "head: too many ROIs for shared memory");
+  class_nms_kernel<<<dim3(n, p.B), 512, smem1, s>>>(p, KP, c0);
+  B2_CUDA(cudaGetLastError());
+  return 0;
+}
+
+int head_select_launch(const HeadPostParams& p, cudaStream_t s) {
+  const int nc1 = p.num_class - 1;
   // at least 2 keys here too: the sort's first __syncthreads is what publishes the keys and s_total, and a sort of one key
   // (one class, e.g. a single partial class, with max_per_class 1) has none
   const int KP2 = next_pow2(nc1 * p.max_per_class) < 2 ? 2 : next_pow2(nc1 * p.max_per_class);
   const size_t smem2 = static_cast<size_t>(KP2) * 8;
   static bool attr_set = false;
   if (!attr_set) {
-    B2_CUDA(cudaFuncSetAttribute(class_nms_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
     B2_CUDA(cudaFuncSetAttribute(final_topk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024));
     attr_set = true;
   }
-  B2_CHECK(smem1 <= 200 * 1024 && smem2 <= 200 * 1024, "head: too many ROIs/classes for shared memory");
-  class_nms_kernel<<<dim3(nc1, p.B), 512, smem1, s>>>(p, KP);
-  B2_CUDA(cudaGetLastError());
+  B2_CHECK(smem2 <= 200 * 1024, "head: too many classes for shared memory");
+  if (class_nms_launch(p, 0, nc1, s)) return -1;
   final_topk_kernel<<<p.B, 1024, smem2, s>>>(p, KP2);
   B2_CUDA(cudaGetLastError());
   return 0;
+}
+
+int head_post_launch(const HeadPostParams& p, cudaStream_t s) {
+  B2_CHECK(p.rois_per_image <= 1024, "head: at most 1024 ROIs per image");
+  const int total = p.B * p.rois_per_image;
+  head_decode_kernel<<<(total + 127) / 128, 128, 0, s>>>(p);
+  B2_CUDA(cudaGetLastError());
+  return head_select_launch(p, s);
 }
 
 }  // namespace b2

@@ -65,6 +65,7 @@ struct RoiAlignParams {
   float* out_nchw;            // [B*rois][C][7][7]   fp32 (fpn_box_feat contract)
   int out_res;                // 0 / 7: 7x7 bins from a 14x14 crop; 14: 14x14 bins from a 28x28 crop (mask head,
                               // models.py:936-937), planes output [B*rois][14][14][C]
+  int one_image;              // 1: the B box groups are groups of one image, all read the features of image 0
 };
 int roialign_launch(const RoiAlignParams& p, cudaStream_t s);
 
@@ -88,6 +89,63 @@ struct HeadPostParams {
   int* final_count;           // [B]
 };
 int head_post_launch(const HeadPostParams& p, cudaStream_t s);
+// head_post_launch's selection alone, over p.probs and p.dec_boxes as they stand: per-class NMS, then the final top-k
+int head_select_launch(const HeadPostParams& p, cudaStream_t s);
+// the per-class NMS of classes c0 .. c0 + n - 1 (dec_boxes column c, probs column c + 1) alone
+int class_nms_launch(const HeadPostParams& p, int c0, int n, cudaStream_t s);
+
+// small_objects.cu -- the small-object branch of the single-image graph (use_small_object_head, models.py:590-692,
+// 845-897).  Rows of the branch: C blocks of R rows (small class i's boxes in NMS selection order) then Tp person rows.
+struct SoParams {
+  // so_select: the head's outputs for the B = 1 image
+  const float* logits;        // [rois][ld] head logits (HeadPostParams layout)
+  int ld, num_class, rois;
+  const float* roi_boxes;     // [rois][4] proposals
+  const int* roi_count;       // [1]
+  const float* probs;         // [rois][num_class] the head's softmax
+  float reg_w[4];
+  float decode_clip, img_w, img_h;
+  int C, R, Tp;               // small classes, rows per class block (result_per_im), person rows (0 = no association)
+  int ids[81];                // the head class ids of the C small classes, then Person's when Tp > 0
+  float* sel_probs;           // [rois][C + 2]: column s + 1 the probability of selected class s (Person last)
+  float* sel_boxes;           // [rois][C + 1][4] unclipped decoded boxes of the selected classes
+  // so_gather: the selections (HeadPostParams cls_keep / cls_count of the two NMS launches)
+  const int* keep;            // [C][R] small classes
+  const int* person_keep;     // [Tp] Person
+  const int* sel_count;       // [C + 1] kept per class, Person last
+  float* rows_boxes;          // [C * R + Tp][4] the branch's rows, unclipped, zero beyond the counts
+  int* row_count;             // [C + 1]: K for every small class block, then the person rows
+  int* k;                     // [1] K: the common count, 0 when the classes kept different counts
+  int* status;                // [1] 0, or 1 when the counts differed
+  // so_finish: the classification layer's fp32 output [C * R][ldl], row block i's columns 2i, 2i + 1
+  const float* cls_logits;
+  int ldl;
+  float* fin_logits;          // [R][C + 1] the rebuilt logits (models.py:675-681)
+  float* fin_boxes;           // [R][C][4] the rows' boxes clipped to the image
+};
+int so_select_launch(const SoParams& p, cudaStream_t s);
+int so_gather_launch(const SoParams& p, cudaStream_t s);
+int so_finish_launch(const SoParams& p, cudaStream_t s);
+
+// person_object_relation (nn.py:194-270) over C blocks of Rq query rows and Tp key (person) rows: P [C * Rq * 16][Tpp]
+// planes (row q * 16 + g) of softmax_j(log(max(wg, 1e-6)) + q_g . k_g / sqrt(D / 16)) over the first *nref key rows, and
+// the key rows' V^T [D][Tpp] (the P.V layer's weights).  Query rows at or beyond *kq of their block, and all rows when
+// *nref is 0, are zero.
+struct SoAttendParams {
+  const float* boxes;         // [C * Rq + Tp][4]: query boxes, then key boxes
+  const int* kq;              // [1] valid query rows per block
+  const int* nref;            // [1] valid key rows
+  const float* qk;            // [C * Rq + Tp][ldqk] fp32: query in columns [0, D), key in [D, 2D)
+  int ldqk, D, C, Rq, Tp, Tpp, rows;
+  const float* geo;           // kRelGeoWeights (relation_upload_geo)
+  const __half* v_hi;         // the key rows' features [Tp][D] planes: the value
+  const __half* v_lo;
+  __half* p_hi;
+  __half* p_lo;
+  __half* vt_hi;              // [D][Tpp]
+  __half* vt_lo;
+};
+int so_attend_launch(const SoAttendParams& p, cudaStream_t s);
 
 // groupnorm.cu -- GroupNorm of a conv output at run time (nn.py:81-108), 32 groups, eps 1e-5
 struct GnParams {

@@ -1,5 +1,5 @@
 // Single-kernel entry points for parity tests and host tools: one conv, one grouped conv, one GroupNorm, one squeeze-excite,
-// one relation module, the attention head's pool, the deformable sampler and conv, the frame resize, and the element-wise
+// one relation module, person_object_relation, the attention head's pool, the deformable sampler and conv, the frame resize, and the element-wise
 // and reduction kernels around the GEMMs (depthwise convs, pools, the BiFPN combine, MBConv's squeeze-excite, OSNet's
 // channel gate, EfficientNet's stem im2col, the ResNet stems' operand packs), and the distance kernels around the tracker / ReID GEMMs.  Each call owns its device buffers in an Arena, so
 // every return path frees them.
@@ -378,6 +378,43 @@ int b2_op_relation(int device, const float* h, const float* boxes, const int32_t
   ws.add("rm/output_linear/W", output_w, static_cast<int64_t>(kRelGroups) * D * D);
   if (run_plan(p, device, ws)) return -1;
   return download_planes(op.hi, op.lo, static_cast<size_t>(M) * D, out, nullptr);
+}
+
+// person_object_relation through the engine's builder (add_so_association): one block of K query rows, then R key rows.
+int b2_op_so_attend(int device, const float* h, const float* boxes, int K, const float* ref, const float* ref_boxes, int R,
+                    const float* geo_emb_w, const float* geo_emb_b, const float* geo_conv_w, const float* geo_conv_b,
+                    const float* query_w, const float* key_w, const float* output_w, int D, int split, float* out) {
+  B2_CHECK(h && boxes && ref && ref_boxes && geo_emb_w && geo_emb_b && geo_conv_w && geo_conv_b && query_w && key_w &&
+               output_w && out, "b2_op_so_attend: null argument");
+  B2_CHECK(K >= 1 && R >= 1 && R <= 1024 && D >= 64 && D % 64 == 0,
+           "b2_op_so_attend: needs K >= 1, 1 <= R <= 1024 and D a multiple of 64");
+  B2_CUDA(cudaSetDevice(device));
+  const int M = K + R;
+  DetPlan p;
+  op_plan(p, 1, split, 0);
+  Planes rows, op;
+  float* dbox = p.arena.alloc<float>(static_cast<size_t>(M) * 4);
+  int* dn = p.arena.alloc<int>(2);
+  B2_CHECK(p.alloc_rows(rows, M, D) && p.alloc_rows(op, K, D) && dbox && dn, "b2_op_so_attend: out of device memory");
+  if (upload_planes(h, rows.hi, rows.lo, static_cast<size_t>(K) * D, nullptr)) return -1;
+  const size_t kd = static_cast<size_t>(K) * D;
+  if (upload_planes(ref, rows.hi + kd, rows.lo ? rows.lo + kd : nullptr, static_cast<size_t>(R) * D, nullptr)) return -1;
+  B2_CUDA(cudaMemcpy(dbox, boxes, static_cast<size_t>(K) * 4 * sizeof(float), cudaMemcpyHostToDevice));
+  B2_CUDA(cudaMemcpy(dbox + static_cast<size_t>(K) * 4, ref_boxes, static_cast<size_t>(R) * 4 * sizeof(float),
+                     cudaMemcpyHostToDevice));
+  const int n[2] = {K, R};
+  B2_CUDA(cudaMemcpy(dn, n, sizeof(n), cudaMemcpyHostToDevice));
+  if (add_so_association(p, 5, "po", 1, K, R, dbox, dn, dn + 1, rows, op)) return -1;
+  WeightSet ws;
+  ws.add("po/geo_emb/W", geo_emb_w, 4 * kRelGeoDim);
+  ws.add("po/geo_emb/b", geo_emb_b, kRelGeoDim);
+  ws.add("po/geo_conv/W", geo_conv_w, kRelGeoDim * kRelGroups);
+  ws.add("po/geo_conv/b", geo_conv_b, kRelGroups);
+  ws.add("po/query_linear/W", query_w, static_cast<int64_t>(D) * D);
+  ws.add("po/key_linear/W", key_w, static_cast<int64_t>(D) * D);
+  ws.add("po/output_linear/W", output_w, static_cast<int64_t>(kRelGroups) * D * D);
+  if (run_plan(p, device, ws)) return -1;
+  return download_planes(op.hi, op.lo, kd, out, nullptr);
 }
 
 // The attention head's pool alone (att_head.cu): fp32 [M][49][C] in, converted to the engine's planes; the pooled planes

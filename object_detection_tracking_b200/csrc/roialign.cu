@@ -78,7 +78,7 @@ __global__ void __launch_bounds__(256) roialign_kernel(const __grid_constant__ R
     const Axis ax = make_axis<2 * kOut>(__fmul_rn(bx.x, is), __fmul_rn(bx.z, is), W, ox);
     const __half* fh = p.feat_hi[lvl];
     const __half* fl = p.feat_lo[lvl];
-    const size_t img_off = static_cast<size_t>(b) * p.pitch_H[lvl] * p.pitch_W[lvl];
+    const size_t img_off = static_cast<size_t>(p.one_image ? 0 : b) * p.pitch_H[lvl] * p.pitch_W[lvl];
     // avg-pool order: (dy,dx) = (0,0) + (0,1) + (1,0) + (1,1), then / 4
 #pragma unroll
     for (int dy = 0; dy < 2; ++dy) {

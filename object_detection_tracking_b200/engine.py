@@ -26,10 +26,11 @@ class Detector:
         self._ext = _lib.make_config_ext(self.cfg)
         self._ext2 = _lib.make_config_ext2(self.cfg)
         self._ext3 = _lib.make_config_ext3(self.cfg)
+        self._ext4 = _lib.make_config_ext4(self.cfg)
         self._ctx = c_void_p(0)
-        _lib.check(self.lib.b2_create_ex3(ctypes.byref(self._ctx), self.device, ctypes.byref(self._c),
-                                          ctypes.byref(self._ext), ctypes.byref(self._ext2), ctypes.byref(self._ext3)),
-                   "b2_create")
+        _lib.check(self.lib.b2_create_ex4(ctypes.byref(self._ctx), self.device, ctypes.byref(self._c),
+                                          ctypes.byref(self._ext), ctypes.byref(self._ext2), ctypes.byref(self._ext3),
+                                          ctypes.byref(self._ext4)), "b2_create")
         self.R = int(self.cfg.result_per_im)
         self.C = int(self.cfg.fpn_num_channel)
         self._pinned = None
@@ -116,6 +117,20 @@ class Detector:
         out = np.empty((self.batch, int(self.cfg.result_per_im), 28, 28), dtype=np.float32)
         _lib.check(self.lib.b2_get_masks(self._ctx, _lib.ptr(out), out.nbytes), "b2_get_masks")
         return out
+
+    def get_small_objects(self) -> dict:
+        """The small-object branch's outputs of the last pass (config.use_small_object_head, models.py:880-897): boxes
+        [n, 4] float32, probs [n] float32 (logits, models.py:884), labels [n] int32 in 1..C, plus class_counts [C] (boxes
+        each small class kept by its NMS) and status (0, or 1 when those counts differ: then n = 0)."""
+        R, C = self.R, len(self.cfg.small_object_class_ids)
+        boxes, probs = np.empty((R, 4), np.float32), np.empty((R,), np.float32)
+        labels, count = np.empty((R,), np.int32), np.empty((1,), np.int32)
+        counts, status = np.empty((C,), np.int32), np.empty((1,), np.int32)
+        _lib.check(self.lib.b2_get_small_objects(self._ctx, *[_lib.ptr(a) for a in (boxes, probs, labels, count, counts,
+                                                                                      status)]), "b2_get_small_objects")
+        n = int(count[0])
+        return dict(boxes=boxes[:n].copy(), probs=probs[:n].copy(), labels=labels[:n].copy(), class_counts=counts,
+                    status=int(status[0]))
 
     def submit_host(self, frames, out: dict, slot: int, feat_mode: int = 0, want_feat: bool = True):
         """Asynchronous detect_host: enqueue upload + pass + download for `slot` (0/1) and return; `frames` and the
@@ -629,6 +644,23 @@ def op_att_pool(x, split=True, device=0) -> np.ndarray:
     assert nb == 49, x.shape
     out = np.empty((M, C), dtype=np.float32)
     _lib.check(lib.b2_op_att_pool(device, _lib.ptr(x), M, C, int(split), _lib.ptr(out)), "b2_op_att_pool")
+    return out
+
+
+def op_so_attend(h, boxes, ref, ref_boxes, weights, split=True, device=0) -> np.ndarray:
+    """person_object_relation (nn.py:194-270) through the C ABI as the engine runs it -- used by the kernel tests: query
+    rows h [K, D] with boxes [K, 4], person rows ref [R, D] with boxes [R, 4]; `weights` maps geo_emb/W, geo_emb/b,
+    geo_conv/W, geo_conv/b, query_linear/W, key_linear/W, output_linear/W (any prefix) to arrays.  Returns [K, D] float32
+    = h + the module's output, read back from its planes."""
+    lib = _lib.load()
+    h, boxes, ref, ref_boxes = (np.ascontiguousarray(a, dtype=np.float32) for a in (h, boxes, ref, ref_boxes))
+    K, D = h.shape
+    R = ref.shape[0]
+    names = ("geo_emb/W", "geo_emb/b", "geo_conv/W", "geo_conv/b", "query_linear/W", "key_linear/W", "output_linear/W")
+    ws = [np.ascontiguousarray(next(v for k, v in weights.items() if k.endswith(n)), dtype=np.float32) for n in names]
+    out = np.empty((K, D), dtype=np.float32)
+    _lib.check(lib.b2_op_so_attend(device, _lib.ptr(h), _lib.ptr(boxes), K, _lib.ptr(ref), _lib.ptr(ref_boxes), R,
+                                   *[_lib.ptr(w) for w in ws], D, int(split), _lib.ptr(out)), "b2_op_so_attend")
     return out
 
 

@@ -17,6 +17,9 @@ weights.  Names follow the Tensorpack-npz convention the reference loads
   use_resnext: conv1 / conv2 at twice the width, conv2/W [3, 3, 2*ch/32, 2*ch] (32 groups), no fc1 / fc2
   add_relation_nn: fastrcnn/RM_r{1,2}/{geo_emb/{W,b}, geo_conv/{W,b}, query_linear/W, key_linear/W, output_linear/W}
   use_att_frcnn_head (class-specific head): fastrcnn/attention/{W,b} [3, 3, 256, 1], [1], fastrcnn/att_trans/{W,b} [256, dim]
+  use_small_object_head: fastrcnn/small_objects/small_object_classification_c{1..C}/{W,b} [dim, 2], [2]; with
+                         use_so_association fastrcnn/small_objects/person_object_relation/{geo_emb/{W,b}, geo_conv/{W,b},
+                         query_linear/W, key_linear/W, output_linear/W}
   use_deformable: <deformable block>/conv2_offset/{W,b} [3, 3, C, 18], [18]; that block's conv2 has no bn / gn
   use_basic_block: conv1/W [3, 3, cin, ch], conv2/W [3, 3, ch, ch], no conv3; convshortcut [1, 1, cin, ch] where cin != ch;
                    laterals read 64 / 128 / 256 / 512 channels
@@ -174,6 +177,19 @@ def synth_weights(cfg, seed: int = 1234) -> dict:
         w["fastrcnn/attention/b"] = (arng.standard_normal(1) * 0.1).astype(np.float32)
         w["fastrcnn/att_trans/W"] = (arng.standard_normal((nc, dim)) * (1.0 / (49.0 * np.sqrt(nc)))).astype(np.float32)
         w["fastrcnn/att_trans/b"] = (arng.standard_normal(dim) * 0.1).astype(np.float32)
+    # The small-object branch draws from a stream of its own too.
+    if getattr(cfg, "use_small_object_head", False):  # models.py:652-692
+        srng = np.random.default_rng([seed, 0x736f])
+        for name, shape in _so_shapes(cfg).items():
+            fan_in = int(np.prod(shape[:-1]))
+            # the classification layers: a unit fan-in gain gives logits of about one unit of either sign, so both the
+            # score filter and negative final "probs" are exercised; the association follows the relation modules' choice
+            rel = name.startswith(_SO_REL)
+            std = ({"geo_emb/W": 0.3, "geo_emb/b": 0.1, "geo_conv/W": np.sqrt(1.0 / 64), "geo_conv/b": 0.05,
+                    "query_linear/W": np.sqrt(2.0 / fan_in), "key_linear/W": np.sqrt(2.0 / fan_in),
+                    "output_linear/W": np.sqrt(1.0 / fan_in)}[name[len(_SO_REL):]] if rel else
+                   {"W": np.sqrt(1.0 / fan_in), "b": 0.5}[name.rsplit("/", 1)[1]])
+            w[name] = (srng.standard_normal(shape) * std).astype(np.float32)
     return w
 
 
@@ -231,6 +247,26 @@ def _att_shapes(cfg):
     nc, dim = cfg.fpn_num_channel, cfg.fpn_frcnn_fc_head_dim
     return {"fastrcnn/attention/W": (3, 3, nc, 1), "fastrcnn/attention/b": (1,), "fastrcnn/att_trans/W": (nc, dim),
             "fastrcnn/att_trans/b": (dim,)}
+
+
+_SO_REL = "fastrcnn/small_objects/person_object_relation/"
+
+
+def _so_shapes(cfg):
+    """Name -> shape of the small-object branch's own variables (models.py:652-692): one [D, 2] classification per class
+    of small_objects and, with use_so_association, the shared person_object_relation (nn.py:194-270).  fc6 / fc7 are the
+    box head's own (AUTO_REUSE)."""
+    dim = cfg.fpn_frcnn_fc_head_dim
+    sh = {}
+    for i in range(len(cfg.small_objects)):
+        p = "fastrcnn/small_objects/small_object_classification_c%d/" % (i + 1)
+        sh.update({p + "W": (dim, 2), p + "b": (2,)})
+    if cfg.use_so_association:
+        p = _SO_REL
+        sh.update({p + "geo_emb/W": (4, 64), p + "geo_emb/b": (64,), p + "geo_conv/W": (1, 1, 64, 16),
+                   p + "geo_conv/b": (16,), p + "query_linear/W": (dim, dim), p + "key_linear/W": (dim, dim),
+                   p + "output_linear/W": (16 * dim, dim)})
+    return sh
 
 
 def deformable_blocks(cfg):
@@ -356,6 +392,8 @@ def frcnn_weight_shapes(cfg) -> dict:
         sh.update(_relation_shapes(cfg))
     if _use_att(cfg):                                # fastrcnn_2fc_head (models.py:1064-1089), with either hidden variant
         sh.update(_att_shapes(cfg))
+    if getattr(cfg, "use_small_object_head", False):  # models.py:652-692
+        sh.update(_so_shapes(cfg))
     if getattr(cfg, "add_mask", False):              # models.py:1173-1199; Conv2DTranspose kernel is [kh, kw, out, in]
         md = getattr(cfg, "mrcnn_head_dim", 256)
         for k in range(4):
