@@ -515,6 +515,22 @@ int b2_op_att_pool(int device, const float* x, int M, int C, int split, float* o
 int b2_op_so_attend(int device, const float* h, const float* boxes, int K, const float* ref, const float* ref_boxes, int R,
                     const float* geo_emb_w, const float* geo_emb_b, const float* geo_conv_w, const float* geo_conv_b,
                     const float* query_w, const float* key_w, const float* output_w, int D, int split, float* out);
+/* The mask head (models.py:934-961, 1173-1199) as the engine runs it, each layer into its own buffer: feats p2..p5 one
+ * after the other, level l [B][pitch_H][pitch_W][C] (host, fp32, converted to the engine's planes) with level_hw[4 l ..
+ * 4 l + 3] = (pitch_H, pitch_W, H, W), (H, W) the crop ROIAlign sees, and strides[l]; boxes [B][R][4] (x1, y1, x2, y2),
+ * count [B] in [0, R] and labels [B][R] (1 .. num_class - 1 below the count); the weights maskrcnn/fcn0..3/{W,b},
+ * maskrcnn/deconv/{W,b} and maskrcnn/conv/{W,b} under their checkpoint names (as b2_load_weights).  Outputs (each may be
+ * NULL but masks): roi [M][14][14][C] (M = B R) the ROIAlign 14 rows, fcn [4][M][14][14][C], up [M][14][14][4C] the
+ * deconv's (tap, channel) rows, each joined to fp32 and as raw planes (the lo planes unwritten in fp16 precision);
+ * logits [M * 784][ld] (ld = num_class - 1 rounded up to 16) the class conv; masks [B][R][28][28], 0 beyond the count.
+ * With logits_in ([M * 784][ld]) the own-class sigmoid alone runs on it, and feats, level_hw, strides, boxes and the
+ * weights may be NULL.  C must be 256.  Sizes, counts and labels are checked before any device work. */
+int b2_op_mask_head(int device, const float* feats, const int32_t* level_hw, const float* strides, int C, int B, int R,
+                    const float* boxes, const int32_t* count, const int32_t* labels, int num_class,
+                    const char* const* names, const float* const* data, const int64_t* numel, int n,
+                    const float* logits_in, int split, float* roi, uint16_t* roi_hi, uint16_t* roi_lo, float* fcn,
+                    uint16_t* fcn_hi, uint16_t* fcn_lo, float* up, uint16_t* up_hi, uint16_t* up_lo, float* logits,
+                    float* masks);
 /* The deformable conv's bilinear sampler (deformable_conv2d nn.py:1642-1712, deformable_helper.py:42-137) as the engine runs
  * it: x [B][H][W][C] (host, fp32, converted to the engine's planes), offsets [B][ceil(H/2)][ceil(W/2)][18] (channel 2k the
  * y and 2k+1 the x offset of tap k, per image).  out [B][ceil(H/2)][ceil(W/2)][9][C]: the sampled operand read back from

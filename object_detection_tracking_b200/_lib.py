@@ -158,6 +158,8 @@ SYMBOLS = [
     ("b2_op_relation", c_int, [c_int] + [c_void_p] * 10 + [c_int] * 4 + [c_void_p]),
     ("b2_op_so_attend", c_int, [c_int, c_void_p, c_void_p, c_int, c_void_p, c_void_p, c_int] + [c_void_p] * 7
      + [c_int, c_int, c_void_p]),
+    ("b2_op_mask_head", c_int, [c_int, c_void_p, c_void_p, c_void_p] + [c_int] * 3 + [c_void_p] * 3
+     + [c_int, POINTER(c_char_p), POINTER(c_void_p), POINTER(c_int64), c_int, c_void_p, c_int] + [c_void_p] * 11),
     ("b2_op_att_pool", c_int, [c_int, c_void_p, c_int, c_int, c_int, c_void_p]),
     ("b2_op_deform_sample", c_int, [c_int, c_void_p, c_void_p] + [c_int] * 5 + [c_void_p]),
     ("b2_op_deform_conv2d", c_int, [c_int] + [c_void_p] * 4 + [c_int] * 7 + [c_void_p, c_void_p]),

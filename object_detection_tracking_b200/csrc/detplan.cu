@@ -445,6 +445,47 @@ int add_deform(DetPlan& p, const std::string& name, const Planes& in, const Plan
   return 0;
 }
 
+// The mask head.  Steps:
+//   roialign_mask    ROIAlign 14 (a 28 x 28 crop, 2 x 2 average, models.py:936-937) of the boxes into buf.roi
+//   fcn0..fcn3       conv 3x3 SAME + bias + ReLU on the [M][14][14][C] maps (M small images)
+//   deconv           Conv2DTranspose 2x2 stride 2 + bias + ReLU: no overlap between taps, so a 1x1 conv onto (tap,
+//                    channel) outputs (load_layer's kDeconv packing)
+//   conv             the 1x1 class conv commutes with the pixel shuffle: it runs on the (pixel, tap) rows directly,
+//                    fp32 output
+//   mask_select      the logits of each box's own class, sigmoid, un-shuffled to 28 x 28 (mask_head.cu)
+// It keeps the checkpoint's num_class - 1 channels with use_partial_classes too, and mask_select reads channel
+// (label - 1) for the partial label, as the reference's gather_nd on the full mask logits does (models.py:954-958).
+int add_mask_head(DetPlan& p, RoiAlignParams roi, int num_class, const MaskBufs& buf, const int* labels, float* logits,
+                  float* masks) {
+  const int M = roi.B * roi.rois_per_image, C = roi.C;
+  B2_CHECK(num_class >= 2, "b2_create: add_mask needs at least one foreground class");
+  const Planes* io[6] = {&buf.roi, &buf.fcn[0], &buf.fcn[1], &buf.fcn[2], &buf.fcn[3], &buf.up};
+  for (int k = 0; k < 6; ++k)
+    B2_CHECK(io[k]->B == M && io[k]->H == 14 && io[k]->W == 14 && io[k]->C == (k == 5 ? 4 * C : C),
+             "b2_create: mask head buffers do not match its boxes");
+  roi.out_hi = buf.roi.hi; roi.out_lo = buf.roi.lo; roi.out_nchw = nullptr; roi.out_res = 14;
+  add_batch_step(p, 7, kStepRoialignMask, "", [roi](int, int, cudaStream_t st) { return roialign_launch(roi, st); });
+  ConvDesc fcn = conv_desc(3, C);
+  pad_all(fcn, 1);
+  fcn.relu = 1;
+  for (int k = 0; k < 4; ++k)
+    add_conv(p, 7, "maskrcnn/fcn" + std::to_string(k), k ? buf.fcn[k - 1] : buf.roi, fcn, kBias, buf.fcn[k]);
+  ConvDesc deconv = conv_desc(1, 4 * C);
+  deconv.relu = 1;
+  add_conv(p, 7, "maskrcnn/deconv", buf.fcn[3], deconv, kBias, buf.up, nullptr, kDeconv);
+  const int rows = M * 196 * 4;
+  Planes up_rows = buf.up;
+  up_rows.B = 1; up_rows.H = 1; up_rows.W = rows; up_rows.C = C;
+  const int ld = mask_logits_ld(num_class);
+  add_conv_f32(p, 7, "maskrcnn/conv", up_rows, conv_desc(1, num_class - 1), kBias, logits, ld);
+  const int B = roi.B, R = roi.rois_per_image;
+  const int* count = roi.count;
+  add_batch_step(p, 7, kStepMaskSelect, "", [logits, ld, labels, count, B, R, masks](int, int, cudaStream_t st) {
+    return mask_select_launch(logits, ld, labels, count, B, R, masks, st);
+  });
+  return 0;
+}
+
 // The basic block (resnet_basicblock nn.py:439-456, resnet_shortcut :551-566, the group's ReLU :586-587) into buf.out
 // (feat channels): conv1 3x3 at `stride`, SAME, NormReLU into t1; the shortcut (`x` itself when it already has feat
 // channels, else convshortcut + norm into sc); conv2 3x3 stride 1 SAME, norm, + shortcut, ReLU.  With BatchNorm the

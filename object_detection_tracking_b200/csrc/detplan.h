@@ -163,6 +163,23 @@ int add_att_head(DetPlan& p, const Planes& roi, int C, const Planes& hidden, con
 // The deformable conv2 of block `name` from conv1's output `in` into `out` ([B][ceil(H/2)][ceil(W/2)][in.C]).
 int add_deform(DetPlan& p, const std::string& name, const Planes& in, const Planes& out);
 
+// The planes the mask head writes, [M][14][14][C] each (M = B * R boxes, C = 256) but up ([M][14][14][4C], the deconv's
+// (tap, channel) outputs).  The layers may share buffers as long as none reads the one it writes: the engine ping-pongs
+// two (roi = fcn[1] = fcn[3], fcn[0] = fcn[2]).
+struct MaskBufs {
+  Planes roi, fcn[4], up;
+};
+// The class conv's output of M boxes: 784 rows per box (196 pixels x 4 taps), padded to whole 128-row tiles, of
+// mask_logits_ld(num_class) fp32 columns.
+inline size_t mask_logits_rows(int M) { return (static_cast<size_t>(M) * 784 + 127) / 128 * 128; }
+inline int mask_logits_ld(int num_class) { return (num_class - 1 + 15) / 16 * 16; }
+// The mask head (models.py:934-961, 1173-1199), phase 7, over the B x R boxes of `roi` (its levels, boxes and count;
+// the outputs are set here): ROIAlign 14 into buf.roi, maskrcnn/fcn0..3 (3x3 SAME + bias + ReLU) into buf.fcn, the
+// transposed conv maskrcnn/deconv into buf.up, the class conv maskrcnn/conv into `logits` and the sigmoid of each box's
+// own class (labels [B][R], 1 .. num_class - 1 below the count) into masks [B][R][28][28].
+int add_mask_head(DetPlan& p, RoiAlignParams roi, int num_class, const MaskBufs& buf, const int* labels, float* logits,
+                  float* masks);
+
 // The planes a residual block writes: conv1's output, conv2's (bottleneck only), the projection shortcut's (used when
 // the input's width is not the block's) and the block output.
 struct BlockBufs {

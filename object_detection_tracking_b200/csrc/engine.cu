@@ -68,27 +68,6 @@ __global__ void agg_feat_kernel(const float* __restrict__ feat, int rows, int C,
   }
 }
 
-// Mask head output (models.py:950-958): per final detection the logits of its own class, sigmoid, and the un-shuffle of
-// the 2x2 transposed-conv taps.  logits rows are ((roi * 196 + y * 14 + x) * 4 + dy * 2 + dx); out [B*R][28][28].
-__global__ void mask_select_kernel(const float* __restrict__ logits, int ld, const int* __restrict__ labels,
-                                   const int* __restrict__ count, int B, int R, float* __restrict__ out) {
-  const size_t total = static_cast<size_t>(B) * R * 784;
-  for (size_t idx = blockIdx.x * static_cast<size_t>(blockDim.x) + threadIdx.x; idx < total;
-       idx += static_cast<size_t>(gridDim.x) * blockDim.x) {
-    const int px = static_cast<int>(idx % 784);
-    const size_t roi = idx / 784;
-    const int b = static_cast<int>(roi / R), j = static_cast<int>(roi % R);
-    float v = 0.f;
-    if (j < count[b]) {
-      const int Y = px / 28, X = px % 28;
-      const size_t row = (roi * 196 + static_cast<size_t>(Y >> 1) * 14 + (X >> 1)) * 4 + (Y & 1) * 2 + (X & 1);
-      const float z = logits[row * ld + (labels[roi] - 1)];
-      v = 1.f / (1.f + expf(-z));
-    }
-    out[idx] = v;
-  }
-}
-
 enum { NPHASE = 8 };
 
 }  // namespace
@@ -125,7 +104,7 @@ struct b2_ctx {
   Planes stem_u, c1, pool, cfeat[4], lat[4], pfeat[5], rpn_h[5];
   float* rpn_out[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};
   RpnParams rpn;
-  RoiAlignParams roi1, roi2, roi3;
+  RoiAlignParams roi1, roi2;
   HeadPostParams post;
   Planes roi_feat, fc6, fc7;        // fc6 / fc7: the M = B * rpn_topk head rows (DetPlan::alloc_rows)
   Planes head_a, head_b;           // conv box head (cfg.conv_head_dim > 0): [M][7][7][conv_head_dim] ping-pong
@@ -676,46 +655,21 @@ int build_plan(b2_ctx* c) {
   P.stages.raw("fpn_box_feat", c->box_feat, Stage::kF32, static_cast<int64_t>(B) * R, nc, 7, 7);
 
   // ---- mask head (models.py:934-961, 1173-1199), phase 7, only with cfg.add_mask ----
-  // It keeps the checkpoint's num_class - 1 channels with use_partial_classes too, and mask_select_kernel reads channel
-  // (label - 1) for the partial label, as the reference's gather_nd on the full mask logits does (models.py:954-958)
+  // ROIAlign 14 of the final boxes, fcn0..3, the deconv, the class conv and the own-class sigmoid (add_mask_head); the
+  // layers ping-pong between two buffers
   if (cfg.add_mask) {
-    B2_CHECK(cfg.num_class >= 2, "b2_create: add_mask needs at least one foreground class");
     const int MR = B * R, md = 256;                  // mrcnn_head_dim (obj_detect_tracking.py:324)
     B2_CHECK(P.alloc_planes(c->mask_a, MR, 14, 14, md), "alloc mask head a");
     B2_CHECK(P.alloc_planes(c->mask_b, MR, 14, 14, md), "alloc mask head b");
     B2_CHECK(P.alloc_planes(c->mask_up, MR, 14, 14, 4 * md), "alloc mask head deconv");
-    RoiAlignParams& r3 = c->roi3;
-    r3 = r1;
+    RoiAlignParams r3 = r1;
     r3.rois_per_image = R;
     r3.boxes = hp.final_boxes; r3.count = hp.final_count;
-    r3.out_hi = c->mask_a.hi; r3.out_lo = c->mask_a.lo; r3.out_nchw = nullptr; r3.out_res = 14;
-    add_batch_step(P, 7, kStepRoialignMask, "", [c](int, int, cudaStream_t st) { return roialign_launch(c->roi3, st); });
-    const Planes* pp[2] = {&c->mask_a, &c->mask_b};
-    ConvDesc fcn = conv_desc(3, md);                 // conv2d 3x3 SAME + bias + ReLU
-    pad_all(fcn, 1);
-    fcn.relu = 1;
-    for (int k = 0; k < 4; ++k) add_conv(P, 7, "maskrcnn/fcn" + std::to_string(k), *pp[k & 1], fcn, kBias, *pp[(k + 1) & 1]);
-    // Conv2DTranspose 2x2 stride 2: no overlap between taps, so it is a 1x1 conv onto (tap, channel) outputs
-    ConvDesc deconv = conv_desc(1, 4 * md);
-    deconv.relu = 1;
-    add_conv(P, 7, "maskrcnn/deconv", c->mask_a, deconv, kBias, c->mask_up, nullptr, kDeconv);
-    // the 1x1 class conv commutes with the pixel shuffle: apply it to the (pixel, tap) rows directly
-    const int rows = MR * 196 * 4, rows_pad = (rows + 127) / 128 * 128;
-    c->mask_ld = (cfg.num_class - 1 + 15) / 16 * 16;
-    c->mask_logits = P.arena.alloc<float>(static_cast<size_t>(rows_pad) * c->mask_ld);
-    Planes up_rows = c->mask_up;
-    up_rows.B = 1; up_rows.H = 1; up_rows.W = rows; up_rows.C = md;
-    add_conv_f32(P, 7, "maskrcnn/conv", up_rows, conv_desc(1, cfg.num_class - 1), kBias, c->mask_logits, c->mask_ld);
+    c->mask_ld = mask_logits_ld(cfg.num_class);
+    c->mask_logits = P.arena.alloc<float>(mask_logits_rows(MR) * c->mask_ld);
     c->final_masks = P.arena.alloc<float>(static_cast<size_t>(MR) * 784);
-    add_batch_step(P, 7, kStepMaskSelect, "", [c](int, int, cudaStream_t st) {
-      const size_t total = static_cast<size_t>(c->cfg.batch) * c->cfg.result_per_im * 784;
-      mask_select_kernel<<<static_cast<unsigned>(std::min<size_t>((total + 255) / 256, 132 * 32)), 256, 0, st>>>(
-          c->mask_logits, c->mask_ld, c->post.final_labels, c->post.final_count, c->cfg.batch, c->cfg.result_per_im,
-          c->final_masks);
-      B2_CUDA(cudaGetLastError());
-      return 0;
-    });
-    P.stages.planes("mask_roi_feat", c->mask_a);       // valid right after step 8 only (ping-pong buffer)
+    const MaskBufs mb = {c->mask_a, {c->mask_b, c->mask_a, c->mask_b, c->mask_a}, c->mask_up};
+    if (add_mask_head(P, r3, cfg.num_class, mb, hp.final_labels, c->mask_logits, c->final_masks)) return -1;
     P.stages.raw("mask_logits", c->mask_logits, Stage::kF32, MR, 196 * 4, c->mask_ld, 1);
     P.stages.raw("final_masks", c->final_masks, Stage::kF32, B, R, 28, 28);
   }

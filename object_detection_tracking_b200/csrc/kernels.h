@@ -69,6 +69,13 @@ struct RoiAlignParams {
 };
 int roialign_launch(const RoiAlignParams& p, cudaStream_t s);
 
+// mask_head.cu: the mask head's output (models.py:950-958).  out [B*R][28][28] = sigmoid of channel labels[roi] - 1 of
+// the class-conv logits ([B*R*196*4][ld] fp32, rows (roi * 196 + (Y >> 1) * 14 + (X >> 1)) * 4 + (Y & 1) * 2 + (X & 1)),
+// 0 for rows j >= count[b].  The labels below the count must lie in 1 .. Cout of the class conv: the device does not check
+// them.
+int mask_select_launch(const float* logits, int ld, const int* labels, const int* count, int B, int R, float* out,
+                       cudaStream_t s);
+
 // head.cu
 struct HeadPostParams {
   const float* logits;        // [B*rois][ld]: cols 0..nc-1 class logits, nc + c*4 .. box logits of class c

@@ -1,9 +1,9 @@
 // Single-kernel entry points for parity tests and host tools: one conv, one grouped conv, one GroupNorm, one squeeze-excite,
-// one relation module, person_object_relation, the attention head's pool, the deformable sampler and conv, the frame resize, and the element-wise
+// one relation module, person_object_relation, the attention head's pool, the deformable sampler and conv, the mask head, the frame resize, and the element-wise
 // and reduction kernels around the GEMMs (depthwise convs, pools, the BiFPN combine, MBConv's squeeze-excite, OSNet's
 // channel gate, EfficientNet's stem im2col, the ResNet stems' operand packs), and the distance kernels around the tracker / ReID GEMMs.  Each call owns its device buffers in an Arena, so
 // every return path frees them.
-// The squeeze-excite, relation and deformable-conv calls build a one-block plan with the detector's builders (detplan.h).
+// The squeeze-excite, relation, deformable-conv and mask-head calls build a one-block plan with the detector's builders (detplan.h).
 #include <limits.h>
 #include <string.h>
 
@@ -483,6 +483,89 @@ int b2_op_deform_conv2d(int device, const float* x, const float* offset_w, const
     B2_CUDA(cudaMemcpy2D(offsets_out, 18 * sizeof(float), s->ptr, s->shape[3] * sizeof(float), 18 * sizeof(float),
                          op.elems() / C, cudaMemcpyDeviceToHost));
   }
+  return 0;
+}
+
+// The mask head through the engine's builder (add_mask_head), every layer in its own buffer; with logits_in the
+// own-class sigmoid alone.
+int b2_op_mask_head(int device, const float* feats, const int32_t* level_hw, const float* strides, int C, int B, int R,
+                    const float* boxes, const int32_t* count, const int32_t* labels, int num_class,
+                    const char* const* names, const float* const* data, const int64_t* numel, int n,
+                    const float* logits_in, int split, float* roi, uint16_t* roi_hi, uint16_t* roi_lo, float* fcn,
+                    uint16_t* fcn_hi, uint16_t* fcn_lo, float* up, uint16_t* up_hi, uint16_t* up_lo, float* logits,
+                    float* masks) {
+  const char* who = "b2_op_mask_head: ";
+  B2_CHECK(count && labels && masks && (logits_in || (feats && level_hw && strides && boxes && names && data && numel)),
+           std::string(who) + "null argument");
+  B2_CHECK(C == 256 && B >= 1 && R >= 1 && num_class >= 2 && num_class <= 1024,
+           std::string(who) + "needs C = 256, B, R >= 1 and 2 <= num_class <= 1024");
+  B2_CHECK(static_cast<int64_t>(B) * R <= 65536, std::string(who) + "at most 65536 boxes (B * R)");
+  for (int b = 0; b < B; ++b) {
+    B2_CHECK(count[b] >= 0 && count[b] <= R, std::string(who) + "count[" + std::to_string(b) + "] outside [0, R]");
+    for (int j = 0; j < count[b]; ++j) {
+      const int l = labels[static_cast<size_t>(b) * R + j];
+      B2_CHECK(l >= 1 && l <= num_class - 1, std::string(who) + "labels[" + std::to_string(b) + "][" + std::to_string(j) +
+                                                 "] = " + std::to_string(l) + " is not a class in 1 .. num_class - 1");
+    }
+  }
+  if (!logits_in)
+    for (int l = 0; l < 4; ++l) {
+      const int32_t* g = level_hw + 4 * l;   // pitch_H, pitch_W, H, W
+      B2_CHECK(g[2] >= 1 && g[3] >= 1 && g[2] <= g[0] && g[3] <= g[1] && strides[l] > 0.f,
+               std::string(who) + "level " + std::to_string(l) + ": needs 1 <= H <= pitch_H, 1 <= W <= pitch_W and a "
+                                  "positive stride");
+    }
+  B2_CUDA(cudaSetDevice(device));
+  const int M = B * R, ld = mask_logits_ld(num_class);
+  const size_t n_map = static_cast<size_t>(M) * 196 * C, n_rows = static_cast<size_t>(M) * 784;
+  DetPlan p;
+  op_plan(p, B, split, 0);
+  int* d_count = p.arena.alloc<int>(B);
+  int* d_labels = p.arena.alloc<int>(M);
+  float* d_logits = p.arena.alloc<float>(mask_logits_rows(M) * ld);
+  float* d_masks = p.arena.alloc<float>(n_rows);
+  B2_CHECK(d_count && d_labels && d_logits && d_masks, std::string(who) + "out of device memory");
+  B2_CUDA(cudaMemcpy(d_count, count, B * sizeof(int), cudaMemcpyHostToDevice));
+  B2_CUDA(cudaMemcpy(d_labels, labels, M * sizeof(int), cudaMemcpyHostToDevice));
+  if (logits_in) {
+    B2_CUDA(cudaMemcpy(d_logits, logits_in, n_rows * ld * sizeof(float), cudaMemcpyHostToDevice));
+    if (mask_select_launch(d_logits, ld, d_labels, d_count, B, R, d_masks, nullptr)) return -1;
+    B2_CUDA(cudaDeviceSynchronize());
+  } else {
+    RoiAlignParams ra;
+    memset(&ra, 0, sizeof(ra));
+    MaskBufs mb;
+    Planes lv[4];
+    size_t at = 0;
+    for (int l = 0; l < 4; ++l) {
+      const int32_t* g = level_hw + 4 * l;
+      B2_CHECK(p.alloc_planes(lv[l], B, g[0], g[1], C), std::string(who) + "out of device memory");
+      if (upload_planes(feats + at, lv[l].hi, lv[l].lo, lv[l].elems(), nullptr)) return -1;
+      at += lv[l].elems();
+      ra.feat_hi[l] = lv[l].hi; ra.feat_lo[l] = lv[l].lo;
+      ra.H[l] = g[2]; ra.W[l] = g[3]; ra.pitch_H[l] = g[0]; ra.pitch_W[l] = g[1];
+      ra.inv_stride[l] = 1.0f / strides[l];
+    }
+    float* d_boxes = p.arena.alloc<float>(static_cast<size_t>(M) * 4);
+    B2_CHECK(d_boxes && p.alloc_planes(mb.roi, M, 14, 14, C) && p.alloc_planes(mb.fcn[0], M, 14, 14, C) &&
+                 p.alloc_planes(mb.fcn[1], M, 14, 14, C) && p.alloc_planes(mb.fcn[2], M, 14, 14, C) &&
+                 p.alloc_planes(mb.fcn[3], M, 14, 14, C) && p.alloc_planes(mb.up, M, 14, 14, 4 * C),
+             std::string(who) + "out of device memory");
+    B2_CUDA(cudaMemcpy(d_boxes, boxes, static_cast<size_t>(M) * 4 * sizeof(float), cudaMemcpyHostToDevice));
+    ra.C = C; ra.B = B; ra.rois_per_image = R;
+    ra.boxes = d_boxes; ra.count = d_count;
+    if (add_mask_head(p, ra, num_class, mb, d_labels, d_logits, d_masks)) return -1;
+    const WeightSet ws(names, data, numel, n);
+    if (run_plan(p, device, ws)) return -1;
+    if (roi && return_planes(mb.roi, n_map, roi, roi_hi, roi_lo)) return -1;
+    for (int k = 0; k < 4 && fcn; ++k)
+      if (return_planes(mb.fcn[k], n_map, fcn + k * n_map, fcn_hi ? fcn_hi + k * n_map : nullptr,
+                        fcn_lo ? fcn_lo + k * n_map : nullptr))
+        return -1;
+    if (up && return_planes(mb.up, 4 * n_map, up, up_hi, up_lo)) return -1;
+  }
+  if (logits) B2_CUDA(cudaMemcpy(logits, d_logits, n_rows * ld * sizeof(float), cudaMemcpyDeviceToHost));
+  B2_CUDA(cudaMemcpy(masks, d_masks, n_rows * sizeof(float), cudaMemcpyDeviceToHost));
   return 0;
 }
 

@@ -439,6 +439,56 @@ def _f32(a):
     return None if a is None else np.ascontiguousarray(a, dtype=np.float32)
 
 
+def op_mask_head(boxes, count, labels, num_class, feats=None, level_hw=None, strides=(4, 8, 16, 32), weights=None,
+                 logits=None, split=True, outputs=("roi", "fcn", "up", "logits"), device=0) -> dict:
+    """The mask head (models.py:934-961, 1173-1199) through the engine's builder -- used by the kernel tests: feats p2..p5
+    [B, pitch_H, pitch_W, 256] each, level_hw their cropped (H, W), boxes [B, R, 4], count [B], labels [B, R] (1 ..
+    num_class - 1 below the count), `weights` the maskrcnn/* arrays under their checkpoint names.  Returns a dict: roi
+    [M, 14, 14, 256] (M = B R), fcn [4, M, 14, 14, 256], up [M, 14, 14, 1024] (the deconv's (tap, channel) outputs), each
+    with its raw planes "<name>_hi" / "<name>_lo" (lo None in fp16 precision); logits [M * 784, ld]; masks [B, R, 28, 28].
+    `outputs` names the ones fetched besides masks.  logits given ([M * 784, ld]) runs the own-class sigmoid alone on them:
+    the dict then holds masks only."""
+    lib = _lib.load()
+    boxes = _f32(boxes)
+    B, R = boxes.shape[:2]
+    count = np.ascontiguousarray(count, dtype=np.int32)
+    labels = np.ascontiguousarray(labels, dtype=np.int32)
+    assert boxes.shape == (B, R, 4) and count.shape == (B,) and labels.shape == (B, R), (boxes.shape, count.shape,
+                                                                                         labels.shape)
+    M, C, ld = B * R, 256, (num_class - 1 + 15) // 16 * 16
+    out = dict(masks=np.empty((B, R, 28, 28), np.float32))
+    null = (c_void_p(0),) * 3
+    if logits is not None:
+        lg = _f32(logits)
+        assert lg.shape == (M * 784, ld), (lg.shape, (M * 784, ld))
+        _lib.check(lib.b2_op_mask_head(device, None, None, None, C, B, R, None, _lib.ptr(count), _lib.ptr(labels),
+                                       int(num_class), None, None, None, 0, _lib.ptr(lg), int(split), *null, *null, *null,
+                                       None, _lib.ptr(out["masks"])),
+                   "b2_op_mask_head")
+        return out
+    fs = [_f32(f) for f in feats]
+    assert len(fs) == 4 and all(f.shape[0] == B and f.shape[3] == C for f in fs), [f.shape for f in fs]
+    flat = np.ascontiguousarray(np.concatenate([f.ravel() for f in fs]))
+    hw = np.array([[f.shape[1], f.shape[2], h, w] for f, (h, w) in zip(fs, level_hw)], np.int32)
+    st = np.asarray(strides, np.float32)
+    names = sorted(weights)
+    arrs = [_f32(weights[k]) for k in names]
+    for k, shape in (("roi", (M, 14, 14, C)), ("fcn", (4, M, 14, 14, C)), ("up", (M, 14, 14, 4 * C))):
+        if k in outputs:
+            out[k], out[k + "_hi"], out[k + "_lo"] = _plane_outputs(shape, split)
+    if "logits" in outputs:
+        out["logits"] = np.empty((M * 784, ld), np.float32)
+    planes = [_lib.ptr(out.get(k + s)) for k in ("roi", "fcn", "up") for s in ("", "_hi", "_lo")]
+    _lib.check(lib.b2_op_mask_head(device, _lib.ptr(flat), _lib.ptr(hw), _lib.ptr(st), C, B, R, _lib.ptr(boxes),
+                                   _lib.ptr(count), _lib.ptr(labels), int(num_class),
+                                   (c_char_p * len(names))(*[k.encode() for k in names]),
+                                   (c_void_p * len(names))(*[a.ctypes.data for a in arrs]),
+                                   (c_int64 * len(names))(*[a.size for a in arrs]), len(names), None, int(split), *planes,
+                                   _lib.ptr(out.get("logits")), _lib.ptr(out["masks"])),
+               "b2_op_mask_head")
+    return out
+
+
 def _plane_outputs(shape, split):
     """fp32 output and its raw planes (uint16; lo None in fp16 precision) of a plane-output op."""
     return (np.empty(shape, np.float32), np.empty(shape, np.uint16),
