@@ -32,6 +32,7 @@
 // (nn.py:989-996) + dense (nn.py:730-774).
 #include <stdlib.h>
 
+#include <type_traits>
 #include <vector>
 
 #include "common.h"
@@ -98,12 +99,41 @@ __device__ __forceinline__ void activate(int relu, float& v0, float& v1) {
   }
 }
 
+// The arithmetic of every epilogue path, for two adjacent output channels (n, n + 1) of one pixel: bias, residual (hi,
+// then lo'), activation.  load_res(plane) returns the residual's hi (0) or lo' (1) pair.  The full-tile paths pass the
+// flags as constants, the general paths as run-time values; either way the expressions and their order are these.
+template <bool SWISH, class LoadRes>
+__device__ __forceinline__ void pair_math(float& v0, float& v1, float2 b, bool res, bool res_lo, int relu,
+                                          LoadRes&& load_res) {
+  v0 += b.x;
+  v1 += b.y;
+  if (res) {
+    const float2 r = __half22float2(load_res(0));
+    v0 += r.x;
+    v1 += r.y;
+    if (res_lo) {
+      const float2 s = join2(make_float2(v0, v1), load_res(1));
+      v0 = s.x;
+      v1 = s.y;
+    }
+  }
+  activate<SWISH>(relu, v0, v1);
+}
+
+// fp16 (hi, lo') planes of two adjacent outputs, and the range monitor's running maximum
+__device__ __forceinline__ void to_planes(float v0, float v1, __half2& hi, __half2& lo, float& amax) {
+  amax = fmaxf(amax, fmaxf(fabsf(v0), fabsf(v1)));
+  split2(v0, v1, hi, lo);
+}
+
+__device__ __forceinline__ uint32_t h2_bits(__half2 h) { return *reinterpret_cast<const uint32_t*>(&h); }
+__device__ __forceinline__ __half2 bits_h2(uint32_t u) { return *reinterpret_cast<const __half2*>(&u); }
+
 // fp16 (hi, lo') planes of two adjacent outputs; lo == nullptr stores the hi plane only
 template <bool SPLIT>
 __device__ __forceinline__ void store_planes(float v0, float v1, __half2* hi_dst, __half2* lo_dst, float& amax) {
-  amax = fmaxf(amax, fmaxf(fabsf(v0), fabsf(v1)));
   __half2 hi, lo;
-  split2(v0, v1, hi, lo);
+  to_planes(v0, v1, hi, lo, amax);
   *hi_dst = hi;
   if (SPLIT && lo_dst != nullptr) *lo_dst = lo;
 }
@@ -114,19 +144,9 @@ template <bool SPLIT, bool SWISH>
 __device__ __forceinline__ void epilogue_pair(const ConvTcParams& p, float v0, float v1, size_t opix, size_t rpix, int n,
                                               float& amax) {
   const float2 b = __ldg(reinterpret_cast<const float2*>(p.bias + n));
-  v0 += b.x;
-  v1 += b.y;
-  if (p.res_hi != nullptr) {
-    const float2 r = __half22float2(__ldg(reinterpret_cast<const __half2*>(p.res_hi + rpix * p.ldr + n)));
-    v0 += r.x;
-    v1 += r.y;
-    if (SPLIT && p.res_lo != nullptr) {
-      const float2 s = join2(make_float2(v0, v1), __ldg(reinterpret_cast<const __half2*>(p.res_lo + rpix * p.ldr + n)));
-      v0 = s.x;
-      v1 = s.y;
-    }
-  }
-  activate<SWISH>(p.relu, v0, v1);
+  pair_math<SWISH>(v0, v1, b, p.res_hi != nullptr, SPLIT && p.res_lo != nullptr, p.relu, [&](int plane) {
+    return __ldg(reinterpret_cast<const __half2*>((plane == 0 ? p.res_hi : p.res_lo) + rpix * p.ldr + n));
+  });
   if (p.out_f32 != nullptr) {
     *reinterpret_cast<float2*>(p.out_f32 + opix * p.ldc + n) = make_float2(v0, v1);
     return;
@@ -141,20 +161,28 @@ template <bool SPLIT, bool SWISH>
 __device__ __forceinline__ void epilogue_pair_slot(const ConvTcParams& p, float v0, float v1, int n, __half2* s_hi,
                                                    __half2* s_lo, float& amax) {
   const float2 b = __ldg(reinterpret_cast<const float2*>(p.bias + n));
-  v0 += b.x;
-  v1 += b.y;
-  if (p.res_hi != nullptr) {
-    const float2 r = __half22float2(*s_hi);
-    v0 += r.x;
-    v1 += r.y;
-    if (SPLIT && p.res_lo != nullptr) {
-      const float2 s = join2(make_float2(v0, v1), *s_lo);
-      v0 = s.x;
-      v1 = s.y;
-    }
-  }
-  activate<SWISH>(p.relu, v0, v1);
+  pair_math<SWISH>(v0, v1, b, p.res_hi != nullptr, SPLIT && p.res_lo != nullptr, p.relu,
+                   [&](int plane) { return plane == 0 ? *s_hi : *s_lo; });
   store_planes<SPLIT>(v0, v1, s_hi, p.out_lo != nullptr ? s_lo : nullptr, amax);
+}
+
+// Runs f(RES, ACT) with the layer's residual flag and activation as compile-time constants (std::bool_constant,
+// std::integral_constant).  A SWISH instantiation only runs swish layers (plan_build), and without SWISH, activate()
+// applies nothing but ReLU.
+template <bool SWISH, class F>
+__device__ __forceinline__ void with_layer_flags(bool res, int relu, F&& f) {
+  using Res = std::true_type;
+  using NoRes = std::false_type;
+  if constexpr (SWISH) {
+    if (res) f(Res{}, std::integral_constant<int, 2>{});
+    else f(NoRes{}, std::integral_constant<int, 2>{});
+  } else if (relu == 1) {
+    if (res) f(Res{}, std::integral_constant<int, 1>{});
+    else f(NoRes{}, std::integral_constant<int, 1>{});
+  } else {
+    if (res) f(Res{}, std::integral_constant<int, 0>{});
+    else f(NoRes{}, std::integral_constant<int, 0>{});
+  }
 }
 
 // ACC (split precision only): the tensor core adds into its fp32 accumulator with truncation (round
@@ -461,61 +489,141 @@ conv_tc_kernel(const __grid_constant__ CUtensorMap tmA_hi, const __grid_constant
 #pragma unroll
     for (int h = 0; h < 2; ++h) valid[h] = m_blk * kBlockM + row0 + 8 * h < p.M;
     float amax = 0.f;   // largest |output| this thread writes in this tile (range monitor)
+    // A full tile (every row below M, every column below Cout_pad) of a layer whose planes are the precision's (lo'
+    // planes in split precision) takes an epilogue with the layer's flags as compile-time constants: no per-pair row or
+    // column checks and no flag reloads.  Other tiles take the general path, which clips and reads the flags per pair.
+    const bool res = p.res_hi != nullptr;
+    const bool full = m_blk * kBlockM + kBlockM <= p.M && n0 + BN <= p.n_cols && (!SWISH || p.relu == 2) &&
+                      (!SPLIT || ((!res || p.res_lo != nullptr) && (p.out_f32 != nullptr || p.out_lo != nullptr)));
     if (p.epi_slots == 0) {
+      // output and residual pixel of this thread's two rows (rows past M: 0, never stored).  Each branch below computes
+      // them itself: computed once ahead of the branch, they spill in the 128-column split + ACC kernel's ragged path.
       size_t opix[2] = {0, 0}, rpix[2] = {0, 0};
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int m = m_blk * kBlockM + row0 + 8 * h;
-        if (valid[h]) {
-          const int img = m / p.HoWo;
-          const int rem = m - img * p.HoWo;
-          const int pp = rem / p.Wo + p.off_h;
-          const int qq = rem - (rem / p.Wo) * p.Wo + p.off_w;
-          opix[h] = (static_cast<size_t>(img) * p.out_H + pp) * p.out_W + qq;
-          rpix[h] = (static_cast<size_t>(img) * p.res_H + (pp >> p.res_shift)) * p.res_W + (qq >> p.res_shift);
-        }
-      }
-#pragma unroll
-      for (int j = 0; j < BN / 8; ++j) {
-        const int n = n0 + 8 * j + col0;
-        if (n >= p.n_cols) continue;
+      auto row_pixels = [&] {
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
-          if (!valid[h]) continue;
-          const int i = 4 * j + 2 * h;
-          epilogue_pair<SPLIT, SWISH>(p, out_value(i), out_value(i + 1), opix[h], rpix[h], n, amax);
+          const int m = m_blk * kBlockM + row0 + 8 * h;
+          if (valid[h]) {
+            const int img = m / p.HoWo;
+            const int rem = m - img * p.HoWo;
+            const int pp = rem / p.Wo + p.off_h;
+            const int qq = rem - (rem / p.Wo) * p.Wo + p.off_w;
+            opix[h] = (static_cast<size_t>(img) * p.out_H + pp) * p.out_W + qq;
+            rpix[h] = (static_cast<size_t>(img) * p.res_H + (pp >> p.res_shift)) * p.res_W + (qq >> p.res_shift);
+          }
         }
-      }
-    } else {
-      // staged: one 64-column chunk at a time through this warpgroup's slot ring.  Slot layout = the TMA box with
-      // 128-byte swizzle: row r at r * 128, 16-byte unit u at (u ^ (r % 8)) * 16.  The 8 rows a warp's lanes hold
-      // have distinct r % 8, so every 4-byte access of the warp hits 32 distinct banks.
+      };
+      if (full) {
+        row_pixels();
+        auto direct_full = [&](auto F32, auto RES, auto ACT) {
+          constexpr bool kF32 = decltype(F32)::value;
+          constexpr bool kRes = decltype(RES)::value;
+          const float2* bias = reinterpret_cast<const float2*>(p.bias + n0 + col0);
 #pragma unroll
-      for (int c = 0; c < BN / kChunkN; ++c) {
-        mbar_wait(&slot_full[cwg * kMaxSlots + eslot], ephase);
-        uint8_t* s_hi = slots + static_cast<size_t>(cwg * p.epi_slots + eslot) * p.slot_bytes;
+          for (int j = 0; j < BN / 8; ++j) {   // 8-column block j: pair 4 * j of the row's float2 / __half2 view
+            const float2 b = __ldg(bias + 4 * j);
 #pragma unroll
-        for (int u = 0; u < kChunkN / 8; ++u) {
-          const int j = c * (kChunkN / 8) + u;
+            for (int h = 0; h < 2; ++h) {
+              const int i = 4 * j + 2 * h;
+              const size_t o = opix[h] * p.ldc + n0 + col0;
+              const size_t r = rpix[h] * p.ldr + n0 + col0;
+              float v0 = out_value(i), v1 = out_value(i + 1);
+              pair_math<SWISH>(v0, v1, b, kRes, SPLIT && kRes, ACT, [&](int plane) {
+                return __ldg(reinterpret_cast<const __half2*>((plane == 0 ? p.res_hi : p.res_lo) + r) + 4 * j);
+              });
+              if constexpr (kF32) {
+                reinterpret_cast<float2*>(p.out_f32 + o)[4 * j] = make_float2(v0, v1);
+              } else {
+                __half2 hi, lo;
+                to_planes(v0, v1, hi, lo, amax);
+                reinterpret_cast<__half2*>(p.out_hi + o)[4 * j] = hi;
+                if (SPLIT) reinterpret_cast<__half2*>(p.out_lo + o)[4 * j] = lo;
+              }
+            }
+          }
+        };
+        if (p.out_f32 != nullptr)
+          with_layer_flags<SWISH>(res, p.relu, [&](auto RES, auto ACT) { direct_full(std::true_type{}, RES, ACT); });
+        else
+          with_layer_flags<SWISH>(res, p.relu, [&](auto RES, auto ACT) { direct_full(std::false_type{}, RES, ACT); });
+      } else {
+        row_pixels();
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
           const int n = n0 + 8 * j + col0;
           if (n >= p.n_cols) continue;
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
             if (!valid[h]) continue;
             const int i = 4 * j + 2 * h;
-            const uint32_t off = (wg_row + 8 * h) * 128 + ((u ^ (lane >> 2)) << 4) + col0 * 2;
-            epilogue_pair_slot<SPLIT, SWISH>(p, out_value(i), out_value(i + 1), n,
-                                             reinterpret_cast<__half2*>(s_hi + off),
-                                             reinterpret_cast<__half2*>(s_hi + kSlotPlaneBytes + off), amax);
+            epilogue_pair<SPLIT, SWISH>(p, out_value(i), out_value(i + 1), opix[h], rpix[h], n, amax);
           }
         }
-        fence_proxy_async_smem();   // the TMA store reads what this thread wrote
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&slot_written[cwg * kMaxSlots + eslot]);
-        if (++eslot == p.epi_slots) {
-          eslot = 0;
-          ephase ^= 1;
+      }
+    } else {
+      // staged: one 64-column chunk at a time through this warpgroup's slot ring.  Slot layout = the TMA box with
+      // 128-byte swizzle: row r at r * 128, 16-byte unit u at (u ^ (r % 8)) * 16.  The 8 rows a warp's lanes hold
+      // have distinct r % 8, so every 4-byte access of the warp hits 32 distinct banks.
+      auto run_chunks = [&](auto&& chunk) {   // chunk(c, byte offset of the slot from `slots`)
+#pragma unroll
+        for (int c = 0; c < BN / kChunkN; ++c) {
+          mbar_wait(&slot_full[cwg * kMaxSlots + eslot], ephase);
+          chunk(c, static_cast<uint32_t>(cwg * p.epi_slots + eslot) * p.slot_bytes);
+          fence_proxy_async_smem();   // the TMA store reads what this thread wrote
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&slot_written[cwg * kMaxSlots + eslot]);
+          if (++eslot == p.epi_slots) {
+            eslot = 0;
+            ephase ^= 1;
+          }
         }
+      };
+      if (full) {
+        with_layer_flags<SWISH>(res, p.relu, [&](auto RES, auto ACT) {
+          constexpr bool kRes = decltype(RES)::value;
+          run_chunks([&](int c, uint32_t slot_off) {
+            // The slot is 1024-byte aligned and r % 8 = lane / 4, so the swizzle phase sits alone in address bits 4-6:
+            // unit u of this thread's first row is at row ^ (u << 4), and its second row (r + 8) 1024 bytes on.
+            const uint32_t row = smem_u32(slots) + slot_off + wg_row * 128 + ((lane >> 2) << 4) + col0 * 2;
+            const float2* bias = reinterpret_cast<const float2*>(p.bias + n0 + col0);
+#pragma unroll
+            for (int u = 0; u < kChunkN / 8; ++u) {
+              const int j = c * (kChunkN / 8) + u;
+              const float2 b = __ldg(bias + 4 * j);
+#pragma unroll
+              for (int h = 0; h < 2; ++h) {
+                const int i = 4 * j + 2 * h;
+                const uint32_t a = (row ^ (u << 4)) + h * 1024;
+                float v0 = out_value(i), v1 = out_value(i + 1);
+                pair_math<SWISH>(v0, v1, b, kRes, SPLIT && kRes, ACT,
+                                 [&](int plane) { return bits_h2(ld_shared_b32(a + plane * kSlotPlaneBytes)); });
+                __half2 hi, lo;
+                to_planes(v0, v1, hi, lo, amax);
+                st_shared_b32(a, h2_bits(hi));
+                if (SPLIT) st_shared_b32(a + kSlotPlaneBytes, h2_bits(lo));
+              }
+            }
+          });
+        });
+      } else {
+        run_chunks([&](int c, uint32_t slot_off) {
+          uint8_t* s_hi = slots + slot_off;
+#pragma unroll
+          for (int u = 0; u < kChunkN / 8; ++u) {
+            const int j = c * (kChunkN / 8) + u;
+            const int n = n0 + 8 * j + col0;
+            if (n >= p.n_cols) continue;
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              if (!valid[h]) continue;
+              const int i = 4 * j + 2 * h;
+              const uint32_t off = (wg_row + 8 * h) * 128 + ((u ^ (lane >> 2)) << 4) + col0 * 2;
+              epilogue_pair_slot<SPLIT, SWISH>(p, out_value(i), out_value(i + 1), n,
+                                               reinterpret_cast<__half2*>(s_hi + off),
+                                               reinterpret_cast<__half2*>(s_hi + kSlotPlaneBytes + off), amax);
+            }
+          }
+        });
       }
     }
     // inf included; a NaN can only follow an inf, which an earlier launch has flagged

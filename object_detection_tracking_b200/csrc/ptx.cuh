@@ -90,6 +90,16 @@ __device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.w
 // all but the newest N bulk groups are complete (writes performed)
 template <int N>
 __device__ __forceinline__ void bulk_wait() { asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory"); }
+// 4-byte shared-memory access by 32-bit shared address.  volatile keeps each one on its side of the mbarrier waits and
+// proxy fences around it (which are volatile asm too).
+__device__ __forceinline__ uint32_t ld_shared_b32(uint32_t addr) {
+  uint32_t v;
+  asm volatile("ld.shared.b32 %0, [%1];" : "=r"(v) : "r"(addr));
+  return v;
+}
+__device__ __forceinline__ void st_shared_b32(uint32_t addr, uint32_t v) {
+  asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(v));
+}
 // orders this thread's generic-proxy shared-memory writes before later async-proxy (TMA) accesses
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
