@@ -212,6 +212,33 @@ int b2_get_masks(b2_ctx* ctx, float* masks_host, int64_t capacity_bytes);
 int b2_get_small_objects(b2_ctx* ctx, float* boxes, float* probs, int32_t* labels, int32_t* count, int32_t* class_counts,
                          int32_t* status);
 
+/* Mask paste and COCO RLE on the GPU: the drivers' post-processing of final_masks (obj_detect_tracking.py:716-739,
+ * obj_detect_imgs.py:501-527), fill_full_mask (nn.py:1565-1584) then pycocotools.mask.encode of the Fortran-ordered frame,
+ * bit-exact with cv2.resize (OpenCV 4.13, default dispatch) and pycocotools.  A b2_masks is an encoder bound to one device:
+ * its grow-only workspaces and its stream.  boxes_host [n][4] float32 are the final boxes already divided by the resize
+ * scale; masks [n][mask_h][mask_w] float32 are host memory, or device memory of the encoder's GPU when masks_on_device.
+ * Only 28x28 masks (the mask head's) are accepted.  Each box's patch is placed as fill_full_mask places it; a box whose
+ * corner int(box[:2] + 0.5) is below 0, or whose patch NumPy could not broadcast into the frame's slice (the frame edge
+ * cuts the slice short, e.g. y1 = H), refuses the call with -2 (message via b2_last_error) before any device work. */
+typedef struct b2_masks b2_masks;
+int b2_masks_create(b2_masks** out, int device);
+void b2_masks_destroy(b2_masks* enc);
+/* The full-frame masks fill_full_mask returns: out_host [n][im_h][im_w] uint8 (0 / 1), capacity >= n * im_h * im_w. */
+int b2_masks_paste(b2_masks* enc, const float* boxes_host, const float* masks, int masks_on_device, int n, int mask_h,
+                   int mask_w, int im_h, int im_w, uint8_t* out_host, int64_t capacity_bytes);
+/* The RLE strings pycocotools' rleToString writes (rle["counts"] of the drivers) of the n full-frame masks: offsets_host
+ * [n + 1] receives the byte offsets of each string (offsets_host[n] = total bytes, no terminators); the bytes go to
+ * bytes_host when capacity >= that total, and stay in the encoder for b2_masks_fetch otherwise. */
+int b2_masks_encode(b2_masks* enc, const float* boxes_host, const float* masks, int masks_on_device, int n, int mask_h,
+                    int mask_w, int im_h, int im_w, int64_t* offsets_host, char* bytes_host, int64_t capacity);
+/* The string bytes of the encoder's last encode (capacity >= its total). */
+int b2_masks_fetch(b2_masks* enc, char* bytes_host, int64_t capacity);
+/* b2_masks_encode of final_masks rows 0 .. n - 1 of image `image` of the context's last pass (needs cfg.add_mask), read in
+ * place on the context's stream: the masks never leave the GPU.  enc must be bound to the context's device; n <=
+ * result_per_im. */
+int b2_encode_masks(b2_ctx* ctx, b2_masks* enc, int image, const float* boxes_host, int n, int im_h, int im_w,
+                    int64_t* offsets_host, char* bytes_host, int64_t capacity);
+
 /* Stage-addressable access for parity tests.  Activations are returned as fp32. */
 int b2_stage_shape(b2_ctx* ctx, const char* name, int64_t shape[4], int32_t* dtype /*0 f32, 1 i32*/);
 int b2_get_stage(b2_ctx* ctx, const char* name, void* dst_host, int64_t capacity_bytes);

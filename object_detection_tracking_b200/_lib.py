@@ -77,6 +77,12 @@ SYMBOLS = [
     ("b2_create_ex4", c_int, [POINTER(c_void_p), c_int, POINTER(B2Config), POINTER(B2ConfigExt), POINTER(B2ConfigExt2),
                               POINTER(B2ConfigExt3), POINTER(B2ConfigExt4)]),
     ("b2_get_small_objects", c_int, [c_void_p] + [c_void_p] * 6),
+    ("b2_masks_create", c_int, [POINTER(c_void_p), c_int]),
+    ("b2_masks_destroy", None, [c_void_p]),
+    ("b2_masks_paste", c_int, [c_void_p, c_void_p, c_void_p] + [c_int] * 6 + [c_void_p, c_int64]),
+    ("b2_masks_encode", c_int, [c_void_p, c_void_p, c_void_p] + [c_int] * 6 + [c_void_p, c_void_p, c_int64]),
+    ("b2_masks_fetch", c_int, [c_void_p, c_void_p, c_int64]),
+    ("b2_encode_masks", c_int, [c_void_p, c_void_p, c_int, c_void_p] + [c_int] * 3 + [c_void_p, c_void_p, c_int64]),
     ("b2_destroy", None, [c_void_p]),
     ("b2_load_weights", c_int, [c_void_p, POINTER(c_char_p), POINTER(c_void_p), POINTER(c_int64), c_int]),
     ("b2_detect", c_int, [c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_void_p, c_int, c_int]),

@@ -156,6 +156,7 @@ class Mask_RCNN_FPN:
         frames = img[None] if single else img
         B, H, W, _ = frames.shape
         det = self._detector(B, H, W)
+        self._last_det = det
         want_feat = any(f is self.fpn_box_feat for f in fetches)
         out = det.detect_host(frames, feat_mode=self.feat_mode, want_feat=want_feat)
         valid = out["valid"]
@@ -217,6 +218,18 @@ class Mask_RCNN_FPN:
                 else:
                     raise KeyError("unknown fetch %r" % (f,))
         return res
+
+
+    def encode_masks(self, boxes_scaled, im_shape, image=0):
+        """The drivers' RLE dicts ({"size": [H, W], "counts": str}, obj_detect_tracking.py:716-739) of the final_masks of
+        image `image` of the last run, computed on the GPU where the masks are: boxes_scaled are that image's final_boxes
+        divided by the resize scale (float32), im_shape the source frame's (H, W)."""
+        if not getattr(self.config, "add_mask", False):
+            raise KeyError("encode_masks needs config.add_mask (models.py:934)")
+        det = getattr(self, "_last_det", None)
+        if det is None:
+            raise RuntimeError("encode_masks needs a run of the model first")
+        return det.encode_masks(boxes_scaled, im_shape, image)
 
 
 class RCNN_FPN_givenbox(Mask_RCNN_FPN):

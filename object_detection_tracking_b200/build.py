@@ -12,7 +12,8 @@ OUT = os.path.join(HERE, "libb200det.so")
 SOURCES = ["engine_core.cu", "detplan.cu", "engine.cu", "ops.cu", "gemm_ws.cu", "conv_tc.cu", "conv_simt.cu", "stem.cu", "rpn.cu",
            "roialign.cu", "head.cu", "cosine.cu", "reid.cu", "reid_engine.cu", "effdet.cu", "effnet.cu", "effdet_engine.cu",
            "tracker.cpp", "tmot.cpp", "pairmatch.cu", "groupnorm.cu", "relation.cu", "deform.cu",
-           "att_head.cu", "reid_ingest.cu", "small_objects.cu", "mask_head.cu"]
+           "att_head.cu", "reid_ingest.cu", "small_objects.cu", "mask_head.cu",
+           "mask_rle.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
               "--expt-relaxed-constexpr", "-Xcompiler", "-fPIC", "-Xcompiler", "-O2",
               "-Xcompiler", "-Wno-attributes"]

@@ -1146,6 +1146,23 @@ int b2_get_masks(b2_ctx* c, float* masks_host, int64_t capacity_bytes) {
   return 0;
 }
 
+// b2_masks_encode of final_masks rows [0, n) of `image`, read in place (mask_rle.cu) on the context's stream.
+int b2_encode_masks(b2_ctx* c, b2_masks* enc, int image, const float* boxes_host, int n, int im_h, int im_w,
+                    int64_t* offsets_host, char* bytes_host, int64_t capacity) {
+  B2_CHECK(c && enc, "b2_encode_masks: null argument");
+  B2_CHECK(c->cfg.add_mask && c->final_masks, "b2_encode_masks: the context was created without add_mask");
+  B2_CHECK(mask_encoder_device(enc) == c->device, "b2_encode_masks: the encoder is bound to another device");
+  B2_CHECK(image >= 0 && image < c->cfg.batch, "b2_encode_masks: image out of range");
+  if (n < 0 || n > c->cfg.result_per_im) {
+    set_error("b2_encode_masks: needs 0 <= n <= result_per_im");
+    return kMaskRefused;
+  }
+  B2_CUDA(cudaSetDevice(c->device));
+  const float* masks = c->final_masks + static_cast<size_t>(image) * c->cfg.result_per_im * 784;
+  return mask_encode(enc, boxes_host, masks, 1, n, 28, 28, im_h, im_w, offsets_host, bytes_host, capacity, c->stream,
+                     "b2_encode_masks");
+}
+
 int b2_get_small_objects(b2_ctx* c, float* boxes, float* probs, int32_t* labels, int32_t* count, int32_t* class_counts,
                          int32_t* status) {
   B2_CHECK(c && boxes && probs && labels && count && class_counts && status, "b2_get_small_objects: null argument");

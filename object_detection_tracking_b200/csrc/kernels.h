@@ -5,6 +5,8 @@
 
 #include "common.h"
 
+struct b2_masks;
+
 namespace b2 {
 
 // stem.cu
@@ -25,6 +27,25 @@ int stem_pack16_launch(const void* img, int is_u8, int B, int H, int W, __half* 
 int reid_boxes_check(const int32_t* boxes_host, int n, int nf, int H, int W, const char* who);
 int reid_crop_resize_launch(const uint8_t* frames, int H, int W, const int32_t* boxes, int n, uint8_t* crops, int out_h,
                             int out_w, cudaStream_t s);
+// mask_rle.cu: a grow-only device buffer (reserve() synchronises `s` before it replaces a smaller one), the workspaces of
+// a b2_masks encoder
+struct DevBuf {
+  void* p = nullptr;
+  size_t cap = 0;
+  DevBuf() = default;
+  DevBuf(const DevBuf&) = delete;
+  DevBuf& operator=(const DevBuf&) = delete;
+  ~DevBuf();
+  int reserve(size_t bytes, cudaStream_t s);
+};
+// Return code of the mask calls for a refused input (bad box, size or shape), checked on the host before any launch.
+constexpr int kMaskRefused = -2;
+// The RLE of b2_masks_encode on stream s: masks [n][28][28] float32 (device memory of the encoder's GPU when
+// masks_on_device, else host), boxes [n][4] host.  Fills offsets[n + 1], copies the strings into bytes when capacity
+// holds them and keeps them in the encoder for b2_masks_fetch.
+int mask_encode(b2_masks* e, const float* boxes, const float* masks, int masks_on_device, int n, int mask_h, int mask_w,
+                int H, int W, int64_t* offsets, char* bytes, int64_t capacity, cudaStream_t s, const char* who);
+int mask_encoder_device(const b2_masks* e);
 // 3x3 stride-2 max-pool, window rows 2y - 1 .. 2y + 1 (columns alike) clipped to the map, Ho x Wo chosen by the caller;
 // C a multiple of 8.  The running maximum starts from 0, so this is the max-pool only of inputs >= 0: every caller feeds
 // it post-ReLU data.  The output is the (hi, lo) pair of the element with the largest joined value.

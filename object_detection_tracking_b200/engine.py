@@ -9,6 +9,7 @@ import numpy as np
 
 from . import _lib
 from .config import normalize_config
+from .masks import MaskEncoder
 
 
 class Detector:
@@ -117,6 +118,14 @@ class Detector:
         out = np.empty((self.batch, int(self.cfg.result_per_im), 28, 28), dtype=np.float32)
         _lib.check(self.lib.b2_get_masks(self._ctx, _lib.ptr(out), out.nbytes), "b2_get_masks")
         return out
+
+    def encode_masks(self, boxes_scaled, im_shape, image: int = 0) -> list:
+        """COCO RLE of the final_masks of image `image` of the last pass (config.add_mask), pasted as fill_full_mask pastes
+        them: boxes_scaled float32 [n, 4] are that image's first n final boxes divided by the resize scale, im_shape the
+        source frame's (H, W).  The masks are read in place on the GPU (masks.py)."""
+        if getattr(self, "_mask_encoder", None) is None:
+            self._mask_encoder = MaskEncoder(self.device)
+        return self._mask_encoder.encode_engine(self._ctx, image, boxes_scaled, im_shape)
 
     def get_small_objects(self) -> dict:
         """The small-object branch's outputs of the last pass (config.use_small_object_head, models.py:880-897): boxes
