@@ -212,6 +212,28 @@ int b2_get_masks(b2_ctx* ctx, float* masks_host, int64_t capacity_bytes);
 int b2_get_small_objects(b2_ctx* ctx, float* boxes, float* probs, int32_t* labels, int32_t* count, int32_t* class_counts,
                          int32_t* status);
 
+/* The fetches of main.py --mode forward (main.py:1540-1870) beyond the detections. */
+/* fpn_feature (models.py:517-518; --extract_feat, --just_feat): p5 of each image resized to 7 x 7 by TF1's legacy bilinear
+ * (align_corners=False, half_pixel_centers=False), feat_host [batch][7][7][fpn_num_channel] float32 NHWC.  The resize
+ * samples the p5 of the padded image (23 x 40 at 720 x 1280, 34 x 60 at 1080 x 1920; below 7 it upsamples).
+ * frames_host NULL: resizes the p5 of the context's last pass.  Otherwise frames_host [batch][H][W][3] of the context's
+ * input dtype are uploaded and only the backbone and FPN run before the resize (with use_cuda_graph, as a graph of their
+ * own); such a feature-only pass leaves the detection results, b2_get_* and every stage after the FPN stale: they keep an
+ * earlier pass's values.  b2_fpn_feature_launches counts the kernels of that pass, resize included. */
+int b2_fpn_feature(b2_ctx* ctx, const void* frames_host, float* feat_host);
+int b2_fpn_feature_launches(b2_ctx* ctx);
+/* proposal_boxes / proposal_scores of the last pass (models.py:550-558; batch graph 2490-2521), host buffers boxes
+ * [batch][rpn_topk][4] x1 y1 x2 y2, scores [batch][rpn_topk], count [batch]: rows >= count[b] are not proposals.  Order:
+ * score descending, ties to the lower position in the levels' concatenation (TF's top_k(sorted=False) leaves it open).
+ * With multi_semantics zero-area boxes are already dropped (models.py:2516-2521). */
+int b2_get_proposals(b2_ctx* ctx, float* boxes, float* scores, int32_t* count);
+/* The use_cpu_nms outputs (--no_nms / --save_all_box, models.py:899-916) of image `image` of the last pass, K = its
+ * proposal count (*k_out): boxes [num_class - 1][K][4] the decoded, clipped boxes of every class (the class-agnostic
+ * head's are the same boxes in every row), probs [num_class - 1][K] the softmax without the background column, rois [K][4]
+ * the proposals.  Capacities: (num_class - 1) * rpn_topk * 4, (num_class - 1) * rpn_topk and rpn_topk * 4 floats (with
+ * partial classes, their count in place of num_class - 1). */
+int b2_get_all_boxes(b2_ctx* ctx, int image, float* boxes, float* probs, float* rois, int32_t* k_out);
+
 /* Mask paste and COCO RLE on the GPU: the drivers' post-processing of final_masks (obj_detect_tracking.py:716-739,
  * obj_detect_imgs.py:501-527), fill_full_mask (nn.py:1565-1584) then pycocotools.mask.encode of the Fortran-ordered frame,
  * bit-exact with cv2.resize (OpenCV 4.13, default dispatch) and pycocotools.  A b2_masks is an encoder bound to one device:

@@ -9,8 +9,9 @@ models.py:196-263).  This module provides the same surface on top of libb200det:
     model = get_model(config, gpuid=0, controller="/cpu:0", is_multi=False)     # models.py:97-119
     model.image, model.final_boxes, model.final_labels, model.final_probs, model.fpn_box_feat,
     model.final_valid_indices (batch mode)
+    model.proposal_boxes, model.proposal_scores, model.fpn_feature          # main.py --mode forward (:1540-1870)
     model.get_feed_dict_forward(img) / model.get_feed_dict_forward_multi(imgs)  # models.py:1629,3301
-    sess = Session(); sess.run([model.final_boxes, ...], feed_dict=fd)
+    sess = Session(); sess.run([model.final_boxes, ...], feed_dict=fd)     # fetches of one or several models
 
 Outputs follow the reference conventions: fresh, writable numpy arrays owned by the caller; boxes are
 x1,y1,x2,y2 in resized-image pixels; labels are 1-based (int64 single image, float32 batch): class ids 1..num_class-1,
@@ -54,6 +55,22 @@ def check_weights(config, weights: dict) -> dict:
     return got
 
 
+def batch_proposals(boxes, scores, count):
+    """The batch graph's proposal_boxes and proposal_scores (models.py:2490-2521) from the engine's per-image proposals
+    (boxes [B, K, 4], scores [B, K], count [B]; zero-area rows are already dropped): [M, 5] rows of (image index as float32,
+    x1, y1, x2, y2) and [M], image by image.  When exactly one row survives, the reference's tf.squeeze(tf.where(area > 0))
+    makes a scalar index, so its outputs have shapes (5,) and (); this returns the same."""
+    boxes = np.asarray(boxes, np.float32)
+    scores = np.asarray(scores, np.float32)
+    n = [int(c) for c in count]
+    pb = np.concatenate([np.zeros((0, 5), np.float32)] +
+                        [np.concatenate([np.full((k, 1), b, np.float32), boxes[b, :k]], axis=1) for b, k in enumerate(n)])
+    ps = np.concatenate([np.zeros((0,), np.float32)] + [scores[b, :k] for b, k in enumerate(n)])
+    if len(ps) == 1:
+        return pb[0].copy(), ps.reshape(())
+    return pb, ps
+
+
 class TensorHandle:
     """Stands in for a tf.Tensor / placeholder: only identity and a name matter to the drivers."""
 
@@ -81,6 +98,20 @@ class Mask_RCNN_FPN:
             cfg = copy.copy(self.config)
             cfg.use_small_object_head = False
             self.config = normalize_config(cfg)
+        # use_cpu_nms (main.py --no_nms / --save_all_box, :493-497): the single-image graph returns every proposal's boxes
+        # and probabilities of every class before its NMS, box features and mask head (models.py:899-916).  The batch graph
+        # has no such branch and pack() exports the NMS outputs (models.py:134-147): those models ignore the flag
+        self.use_cpu_nms = (bool(getattr(self.config, "use_cpu_nms", False)) and not self.is_multi
+                            and not getattr(self.config, "is_load_from_pb", False))
+        if self.use_cpu_nms:
+            if self.config.use_partial_classes and len(self.config.partial_classes) != self.config.num_class - 1:
+                raise ValueError("use_cpu_nms with use_partial_classes needs all num_class - 1 = %d classes, got %d: the "
+                                 "reference asserts boxes.shape[1] == num_class - 1 (models.py:902-903)"
+                                 % (self.config.num_class - 1, len(self.config.partial_classes)))
+            if self.config.add_mask:
+                cfg = copy.copy(self.config)
+                cfg.add_mask = False
+                self.config = normalize_config(cfg)
         self.gpuid = gpuid
         self.precision = precision
         self.input_dtype = input_dtype
@@ -100,6 +131,10 @@ class Mask_RCNN_FPN:
         self.so_final_boxes = TensorHandle(self, "so_final_boxes:0")
         self.so_final_labels = TensorHandle(self, "so_final_labels:0")
         self.so_final_probs = TensorHandle(self, "so_final_probs:0")
+        # main.py --mode forward: --get_rpn_out (models.py:550-558) and --extract_feat / --just_feat (models.py:517-518)
+        self.proposal_boxes = TensorHandle(self, "proposal_boxes:0")
+        self.proposal_scores = TensorHandle(self, "proposal_scores:0")
+        self.fpn_feature = TensorHandle(self, "fpn_feature:0")
         self._weights = None
         self._detectors = {}
 
@@ -155,11 +190,33 @@ class Mask_RCNN_FPN:
         single = img.ndim == 3
         frames = img[None] if single else img
         B, H, W, _ = frames.shape
+        if self.is_multi and any(f is self.fpn_feature for f in fetches):
+            raise KeyError("fpn_feature is not built by the batch graph (commented out at models.py:2085)")
+        if self.use_cpu_nms:
+            if not single:
+                raise ValueError("use_cpu_nms: the single-image graph takes one [H, W, 3] frame")
+            for f in fetches:
+                if f is self.fpn_box_feat or f is self.final_masks:
+                    raise KeyError("%s is not built with use_cpu_nms: the graph returns before it (models.py:916)" % f.name)
         det = self._detector(B, H, W)
         self._last_det = det
+        if fetches and all(f is self.fpn_feature for f in fetches):
+            # main.py --just_feat: with nothing else fetched, the graph runs the backbone and FPN only
+            feat = det.fpn_feature(frames)
+            return [feat.copy() for _ in fetches]
         want_feat = any(f is self.fpn_box_feat for f in fetches)
         out = det.detect_host(frames, feat_mode=self.feat_mode, want_feat=want_feat)
         valid = out["valid"]
+        feat = det.fpn_feature() if any(f is self.fpn_feature for f in fetches) else None
+        props = None
+        if any(f is self.proposal_boxes or f is self.proposal_scores for f in fetches):
+            p = det.get_proposals()
+            if single:
+                n = int(p["count"][0])
+                props = (p["boxes"][0, :n], p["scores"][0, :n])
+            else:
+                props = batch_proposals(p["boxes"], p["scores"], p["count"])
+        allb = det.get_all_boxes(0) if self.use_cpu_nms else None
         so = None
         so_handles = (self.so_final_boxes, self.so_final_labels, self.so_final_probs)
         if any(f is h for f in fetches for h in so_handles):
@@ -180,6 +237,18 @@ class Mask_RCNN_FPN:
                     res.append(so["labels"].astype(np.int64))                 # models.py:887-888: int64, 1..C
                 else:
                     res.append(so["probs"])                                   # logits (models.py:884)
+            elif f is self.fpn_feature:
+                res.append(feat.copy())                                       # [B, 7, 7, C]
+            elif f is self.proposal_boxes:
+                res.append(props[0].copy())
+            elif f is self.proposal_scores:
+                res.append(props[1].copy())
+            elif allb is not None and f is self.final_boxes:
+                res.append(allb["boxes"].copy())                              # [C-1, K, 4]
+            elif allb is not None and f is self.final_probs:
+                res.append(allb["probs"].copy())                              # [C-1, K]
+            elif allb is not None and f is self.final_labels:
+                res.append(allb["rois"].copy())                               # the ROIs [K, 4] (models.py:914)
             elif single:
                 r = int(valid[0])
                 if f is self.final_boxes:
@@ -417,13 +486,20 @@ class EfficientDet_multi(EfficientDet):
 
 
 class Session:
-    """`sess.run(fetches, feed_dict=...)` for fetches that all belong to one model object."""
+    """`sess.run(fetches, feed_dict=...)`.  The fetches may belong to several model objects, as main.py --gpu N fetches
+    those of one model per GPU in one call (main.py:1698-1728): each model runs once, on its own image of the shared
+    feed_dict and with its own fetches only, one model after the other; the results come back in fetch order."""
 
     def run(self, fetches, feed_dict=None):
         single = not isinstance(fetches, (list, tuple))
         flist = [fetches] if single else list(fetches)
-        model = flist[0].model
-        out = model._run(flist, feed_dict or {})
+        groups = {}                                   # id(model) -> (model, positions of its fetches), in first-fetch order
+        for i, f in enumerate(flist):
+            groups.setdefault(id(f.model), (f.model, []))[1].append(i)
+        out = [None] * len(flist)
+        for model, pos in groups.values():
+            for i, r in zip(pos, model._run([flist[i] for i in pos], feed_dict or {})):
+                out[i] = r
         return out[0] if single else out
 
     def close(self):

@@ -8,14 +8,15 @@
 #include "common.h"
 #include "kernels.h"
 #include "planes.cuh"
+#include "tf_resize_math.h"
 
 namespace b2 {
 namespace {
 
-// uint8 BGR frame -> RGB, * 1/255, (x - mean) / std, legacy bilinear resize (align_corners=False, no half-pixel
-// centres) to (sh, sw), zero-padded bottom/right to [H, W, 3] fp32.  The reference normalises first and resizes the
-// float image; lerp of normalised corner values is done in the same order here.  Image blockIdx.y reads its frame and
-// sizes from table[blockIdx.y] and writes out[blockIdx.y].
+// uint8 BGR frame -> RGB, * 1/255, (x - mean) / std, TF1's legacy bilinear resize (tf_resize_math.h) to (sh, sw),
+// zero-padded bottom/right to [H, W, 3] fp32.  The reference normalises first and resizes the float image; lerp of
+// normalised corner values is done in the same order here.  Image blockIdx.y reads its frame and sizes from
+// table[blockIdx.y] and writes out[blockIdx.y].
 __global__ void effnet_preprocess_kernel(const uint8_t* __restrict__ frames, const EffnetFrame* __restrict__ table,
                                          float* __restrict__ out, int H, int W) {
   const int idx = blockIdx.x * blockDim.x + threadIdx.x;
@@ -28,11 +29,7 @@ __global__ void effnet_preprocess_kernel(const uint8_t* __restrict__ frames, con
   const int y = idx / W, x = idx - y * W;
   float r[3] = {0.f, 0.f, 0.f};
   if (y < sh && x < sw) {
-    const float in_y = __fmul_rn(static_cast<float>(y), ys), in_x = __fmul_rn(static_cast<float>(x), xs);
-    const float fy = floorf(in_y), fx = floorf(in_x);
-    const int y0 = static_cast<int>(fy), x0 = static_cast<int>(fx);
-    const int y1 = min(static_cast<int>(ceilf(in_y)), h - 1), x1 = min(static_cast<int>(ceilf(in_x)), w - 1);
-    const float ly = __fsub_rn(in_y, fy), lx = __fsub_rn(in_x, fx);
+    const TfResizeTap ty = tf_resize_tap(y, ys, h), tx = tf_resize_tap(x, xs, w);
     const float mean[3] = {0.485f, 0.456f, 0.406f}, stdv[3] = {0.229f, 0.224f, 0.225f};
 #pragma unroll
     for (int c = 0; c < 3; ++c) {
@@ -41,10 +38,7 @@ __global__ void effnet_preprocess_kernel(const uint8_t* __restrict__ frames, con
         const float v = __fmul_rn(static_cast<float>(img[(static_cast<size_t>(yy) * w + xx) * 3 + sc]), 1.0f / 255.0f);
         return __fdiv_rn(__fsub_rn(v, mean[c]), stdv[c]);
       };
-      const float tl = px(y0, x0), tr = px(y0, x1), bl = px(y1, x0), br = px(y1, x1);
-      const float top = __fadd_rn(tl, __fmul_rn(__fsub_rn(tr, tl), lx));
-      const float bot = __fadd_rn(bl, __fmul_rn(__fsub_rn(br, bl), lx));
-      r[c] = __fadd_rn(top, __fmul_rn(__fsub_rn(bot, top), ly));
+      r[c] = tf_resize_lerp(px(ty.lo, tx.lo), px(ty.lo, tx.hi), px(ty.hi, tx.lo), px(ty.hi, tx.hi), tx.lerp, ty.lerp);
     }
   }
   float* o = out + static_cast<size_t>(idx) * 3;
@@ -298,8 +292,8 @@ __global__ void __launch_bounds__(256) se_fc2_scale_kernel(const float* __restri
 EffnetFrame effnet_frame(unsigned long long src, int h, int w, int sh, int sw) {
   EffnetFrame f;
   f.src = src; f.h = h; f.w = w; f.sh = sh; f.sw = sw;
-  f.ys = static_cast<float>(h) / static_cast<float>(sh);
-  f.xs = static_cast<float>(w) / static_cast<float>(sw);
+  f.ys = tf_resize_scale(h, sh);
+  f.xs = tf_resize_scale(w, sw);
   return f;
 }
 

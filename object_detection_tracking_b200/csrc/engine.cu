@@ -16,6 +16,8 @@
 
 #include "../../include/b200det.h"
 #include "detplan.h"
+#include "planes.cuh"
+#include "tf_resize_math.h"
 
 namespace b2 {
 namespace {
@@ -66,6 +68,45 @@ __global__ void agg_feat_kernel(const float* __restrict__ feat, int rows, int C,
     for (int ch = 0; ch < C; ++ch) s += f[static_cast<size_t>(ch) * 49];
     out[idx] = s / static_cast<float>(C);
   }
+}
+
+// The scene feature fpn_feature (models.py:517-518): p5 resized to 7 x 7 with TF1's legacy bilinear (tf_resize_math.h),
+// float32 NHWC [B][7][7][C].  Samples the p5 of the padded image, ph x pw, out of planes of pitch pitch_h x pitch_w; below
+// 7 px the resize upsamples and the clamp of the upper tap to ph - 1 / pw - 1 applies.  One thread = 8 channels of one
+// output pixel.
+__global__ void fpn_feature_kernel(const __half* __restrict__ hi, const __half* __restrict__ lo, int B, int pitch_h,
+                                   int pitch_w, int C, int ph, int pw, float sy, float sx, float* __restrict__ out) {
+  const int cvec = C / 8;
+  const int idx = blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= B * 49 * cvec) return;
+  const int cv = idx % cvec, pix = idx / cvec;   // pix = (b * 7 + oy) * 7 + ox
+  const int ox = pix % 7, oy = (pix / 7) % 7, b = pix / 49;
+  const TfResizeTap ty = tf_resize_tap(oy, sy, ph), tx = tf_resize_tap(ox, sx, pw);
+  const size_t img = static_cast<size_t>(b) * pitch_h * pitch_w;
+  auto at = [&](int y, int x) { return (img + static_cast<size_t>(y) * pitch_w + x) * C + cv * 8; };
+  float tl[8], tr[8], bl[8], br[8], r[8];
+  load8(hi, lo, at(ty.lo, tx.lo), tl);
+  load8(hi, lo, at(ty.lo, tx.hi), tr);
+  load8(hi, lo, at(ty.hi, tx.lo), bl);
+  load8(hi, lo, at(ty.hi, tx.hi), br);
+#pragma unroll
+  for (int j = 0; j < 8; ++j) r[j] = tf_resize_lerp(tl[j], tr[j], bl[j], br[j], tx.lerp, ty.lerp);
+  float4* o = reinterpret_cast<float4*>(out + static_cast<size_t>(pix) * C + cv * 8);
+  o[0] = make_float4(r[0], r[1], r[2], r[3]);
+  o[1] = make_float4(r[4], r[5], r[6], r[7]);
+}
+
+// The use_cpu_nms outputs of one image (models.py:899-912): the decoded, clipped boxes [K][nc1][4] transposed to
+// [nc1][n][4] and the probabilities' class columns [K][1 + nc1] to [nc1][n], n = *count proposals.
+__global__ void all_boxes_kernel(const float4* __restrict__ dec, const float* __restrict__ probs,
+                                 const int* __restrict__ count, int K, int nc1, int ncls, float4* __restrict__ out_boxes,
+                                 float* __restrict__ out_probs) {
+  const int idx = blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= nc1 * K) return;
+  const int n = *count, c = idx / K, k = idx - c * K;
+  if (k >= n) return;
+  out_boxes[static_cast<size_t>(c) * n + k] = dec[static_cast<size_t>(k) * nc1 + c];
+  out_probs[static_cast<size_t>(c) * n + k] = probs[static_cast<size_t>(k) * ncls + c + 1];
 }
 
 enum { NPHASE = 8 };
@@ -128,6 +169,12 @@ struct b2_ctx {
   int mask_ld = 0;
   float* final_masks = nullptr;    // [B][R][28][28]
   cudaGraphExec_t graph = nullptr;
+  // b2_fpn_feature: the resized p5 [B][7][7][C], and the graph of the backbone-only pass
+  float* fpn_feat = nullptr;
+  cudaGraphExec_t feat_graph = nullptr;
+  // b2_get_all_boxes: one image's re-laid-out boxes [nc1][K][4] and probabilities [nc1][K], allocated on first use
+  float* all_boxes = nullptr;
+  float* all_probs = nullptr;
   // dual-stream pass (plan.dual): the backbone / FPN / RPN-head phases run as plan.nsplit batch parts on as many streams,
   // so that the tail of one layer's persistent kernel (tiles % SMs != 0, no SM busy in the last round) overlaps the other
   // parts' kernels
@@ -674,17 +721,21 @@ int build_plan(b2_ctx* c) {
     P.stages.raw("final_masks", c->final_masks, Stage::kF32, B, R, 28, 28);
   }
 
+  // ---- fpn_feature (models.py:517-518): b2_fpn_feature's output, outside the per-frame plan ----
+  c->fpn_feat = P.arena.alloc<float>(static_cast<size_t>(B) * 49 * nc);
+  B2_CHECK(c->fpn_feat != nullptr, "out of device memory (fpn_feature)");
+
   // ---- tensor-core plans ----
   return plan_layers(P, c->num_sms);
 }
 
-// The whole pass with phases 0-2 forked over nsplit streams (also valid inside a stream capture: the side streams join
-// the capture through the fork event and rejoin before the proposals).
-int enqueue_dual(b2_ctx* c) {
+// The phases of `mask` with phases 0-2 forked over nsplit streams (also valid inside a stream capture: the side streams
+// join the capture through the fork event and rejoin before the proposals).
+int enqueue_dual(b2_ctx* c, unsigned mask) {
   B2_CUDA(cudaEventRecord(c->fork_ev, c->stream));
   for (int h = 1; h < c->plan.nsplit; ++h) B2_CUDA(cudaStreamWaitEvent(c->side_stream[h - 1], c->fork_ev, 0));
   for (const Step& s : c->plan.steps) {
-    if (s.phase > 2) continue;
+    if (s.phase > 2 || !((mask >> s.phase) & 1u)) continue;
     for (int h = 0; h < c->plan.nsplit; ++h)
       if (s.parts[h](h == 0 ? c->stream : c->side_stream[h - 1])) return -1;
   }
@@ -692,11 +743,11 @@ int enqueue_dual(b2_ctx* c) {
     B2_CUDA(cudaEventRecord(c->join_ev[h - 1], c->side_stream[h - 1]));
     B2_CUDA(cudaStreamWaitEvent(c->stream, c->join_ev[h - 1], 0));
   }
-  return run_steps(c->plan.steps, ~0x7u, c->stream);
+  return run_steps(c->plan.steps, mask & ~0x7u, c->stream);
 }
 
 int enqueue(b2_ctx* c, int mask, bool with_events) {
-  if (c->plan.dual && !with_events && mask == B2_PHASE_ALL) return enqueue_dual(c);
+  if (c->plan.dual && !with_events && mask == B2_PHASE_ALL) return enqueue_dual(c, B2_PHASE_ALL);
   if (!with_events) return run_steps(c->plan.steps, mask, c->stream);
   B2_CUDA(cudaEventRecord(c->ev[0], c->stream));
   int last = -1;
@@ -708,6 +759,23 @@ int enqueue(b2_ctx* c, int mask, bool with_events) {
   }
   if (last >= 0) B2_CUDA(cudaEventRecord(c->ev[last + 1], c->stream));
   return 0;
+}
+
+int fpn_feature_launch(b2_ctx* c) {
+  const Planes& p5 = c->pfeat[3];
+  const int total = p5.B * 49 * (p5.C / 8);
+  fpn_feature_kernel<<<(total + 255) / 256, 256, 0, c->stream>>>(p5.hi, p5.lo, p5.B, p5.H, p5.W, p5.C, c->pfh[3], c->pfw[3],
+                                                                  tf_resize_scale(c->pfh[3], 7), tf_resize_scale(c->pfw[3], 7),
+                                                                  c->fpn_feat);
+  B2_CUDA(cudaGetLastError());
+  return 0;
+}
+
+// The backbone-only pass of b2_fpn_feature: phases 0-1, forked over the batch parts as in a full pass, then the resize.
+int enqueue_feature(b2_ctx* c) {
+  const unsigned mask = B2_PHASE_BACKBONE | B2_PHASE_FPN;
+  if (c->plan.dual ? enqueue_dual(c, mask) : run_steps(c->plan.steps, mask, c->stream)) return -1;
+  return fpn_feature_launch(c);
 }
 
 }  // namespace
@@ -809,6 +877,7 @@ void b2_destroy(b2_ctx* c) {
   cudaSetDevice(c->device);
   cudaDeviceSynchronize();
   if (c->graph) cudaGraphExecDestroy(c->graph);
+  if (c->feat_graph) cudaGraphExecDestroy(c->feat_graph);
   if (c->fork_ev) cudaEventDestroy(c->fork_ev);
   for (int h = 0; h < 7; ++h) {
     if (c->join_ev[h]) cudaEventDestroy(c->join_ev[h]);
@@ -874,6 +943,14 @@ int b2_phase_times(b2_ctx* c, float ms[8]) {
 }
 
 int b2_kernel_launches(b2_ctx* c) { return c ? total_launches(c->plan.steps) : -1; }
+
+int b2_fpn_feature_launches(b2_ctx* c) {
+  if (!c) return -1;
+  std::vector<Step> steps;
+  for (const Step& s : c->plan.steps)
+    if (s.phase <= 1) steps.push_back(s);
+  return total_launches(steps) + 1;
+}
 
 // Per-step device timing (CUDA events around every launch group, eager mode), averaged over `reps`.
 int b2_profile_steps(b2_ctx* c, int reps, float* ms_out, int cap, int* n_out) {
@@ -1161,6 +1238,70 @@ int b2_encode_masks(b2_ctx* c, b2_masks* enc, int image, const float* boxes_host
   const float* masks = c->final_masks + static_cast<size_t>(image) * c->cfg.result_per_im * 784;
   return mask_encode(enc, boxes_host, masks, 1, n, 28, 28, im_h, im_w, offsets_host, bytes_host, capacity, c->stream,
                      "b2_encode_masks");
+}
+
+// models.py:517-518, main.py --extract_feat / --just_feat.  With frames the backbone-only pass (main.py's just_feat graph
+// stops after the FPN): the detection results and every stage past the FPN still hold an earlier pass's values.
+int b2_fpn_feature(b2_ctx* c, const void* frames_host, float* feat_host) {
+  B2_CHECK(c && feat_host, "b2_fpn_feature: null argument");
+  B2_CUDA(cudaSetDevice(c->device));
+  B2_CHECK(c->weights_loaded, "b2_fpn_feature: weights not loaded");
+  if (frames_host) {
+    B2_CUDA(cudaMemcpyAsync(c->img, frames_host, c->img_bytes, cudaMemcpyHostToDevice, c->stream));
+    if (c->cfg.use_cuda_graph) {
+      if (!c->feat_graph && capture_graph(c->stream, [c] { return enqueue_feature(c); }, &c->feat_graph)) return -1;
+      B2_CUDA(cudaGraphLaunch(c->feat_graph, c->stream));
+    } else if (enqueue_feature(c)) {
+      return -1;
+    }
+  } else if (fpn_feature_launch(c)) {
+    return -1;
+  }
+  const size_t bytes = sizeof(float) * c->cfg.batch * 49 * c->cfg.fpn_num_channel;
+  B2_CUDA(cudaMemcpyAsync(feat_host, c->fpn_feat, bytes, cudaMemcpyDeviceToHost, c->stream));
+  return sync_range(c);
+}
+
+// proposal_boxes / proposal_scores of the last pass (models.py:550-558, 2490-2521), as the merge kernel left them.
+int b2_get_proposals(b2_ctx* c, float* boxes, float* scores, int32_t* count) {
+  B2_CHECK(c && boxes && scores && count, "b2_get_proposals: null argument");
+  B2_CUDA(cudaSetDevice(c->device));
+  const size_t n = static_cast<size_t>(c->cfg.batch) * c->cfg.rpn_topk;
+  cudaStream_t st = c->stream;
+  B2_CUDA(cudaMemcpyAsync(boxes, c->rpn.prop_boxes, sizeof(float) * n * 4, cudaMemcpyDeviceToHost, st));
+  B2_CUDA(cudaMemcpyAsync(scores, c->rpn.prop_scores, sizeof(float) * n, cudaMemcpyDeviceToHost, st));
+  B2_CUDA(cudaMemcpyAsync(count, c->rpn.prop_count, sizeof(int32_t) * c->cfg.batch, cudaMemcpyDeviceToHost, st));
+  B2_CUDA(cudaStreamSynchronize(st));
+  return 0;
+}
+
+// The use_cpu_nms outputs (models.py:899-916) of image `image` of the last pass: the K proposals' boxes of every class, their
+// probabilities and the proposals themselves, laid out on the device and copied once K is known.
+int b2_get_all_boxes(b2_ctx* c, int image, float* boxes, float* probs, float* rois, int32_t* k_out) {
+  B2_CHECK(c && boxes && probs && rois && k_out, "b2_get_all_boxes: null argument");
+  B2_CHECK(image >= 0 && image < c->cfg.batch, "b2_get_all_boxes: image out of range");
+  B2_CUDA(cudaSetDevice(c->device));
+  const int K = c->cfg.rpn_topk, ncls = c->post.num_class, nc1 = ncls - 1;
+  cudaStream_t st = c->stream;
+  if (!c->all_boxes) {
+    c->all_boxes = c->plan.arena.alloc<float>(static_cast<size_t>(nc1) * K * 4, /*zero=*/false);   // written before read
+    c->all_probs = c->plan.arena.alloc<float>(static_cast<size_t>(nc1) * K, /*zero=*/false);
+    B2_CHECK(c->all_boxes && c->all_probs, "out of device memory (b2_get_all_boxes)");
+  }
+  const size_t m = static_cast<size_t>(image) * K;
+  all_boxes_kernel<<<(nc1 * K + 255) / 256, 256, 0, st>>>(reinterpret_cast<const float4*>(c->post.dec_boxes) + m * nc1,
+                                                          c->post.probs + m * ncls, c->rpn.prop_count + image, K, nc1, ncls,
+                                                          reinterpret_cast<float4*>(c->all_boxes), c->all_probs);
+  B2_CUDA(cudaGetLastError());
+  B2_CUDA(cudaMemcpyAsync(k_out, c->rpn.prop_count + image, sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+  B2_CUDA(cudaStreamSynchronize(st));
+  const size_t n = static_cast<size_t>(*k_out);
+  B2_CHECK(*k_out >= 0 && *k_out <= K, "b2_get_all_boxes: proposal count out of range");
+  B2_CUDA(cudaMemcpyAsync(boxes, c->all_boxes, sizeof(float) * nc1 * n * 4, cudaMemcpyDeviceToHost, st));
+  B2_CUDA(cudaMemcpyAsync(probs, c->all_probs, sizeof(float) * nc1 * n, cudaMemcpyDeviceToHost, st));
+  B2_CUDA(cudaMemcpyAsync(rois, c->rpn.prop_boxes + m * 4, sizeof(float) * n * 4, cudaMemcpyDeviceToHost, st));
+  B2_CUDA(cudaStreamSynchronize(st));
+  return 0;
 }
 
 int b2_get_small_objects(b2_ctx* c, float* boxes, float* probs, int32_t* labels, int32_t* count, int32_t* class_counts,

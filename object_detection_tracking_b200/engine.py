@@ -141,6 +141,44 @@ class Detector:
         return dict(boxes=boxes[:n].copy(), probs=probs[:n].copy(), labels=labels[:n].copy(), class_counts=counts,
                     status=int(status[0]))
 
+    def fpn_feature(self, frames=None) -> np.ndarray:
+        """fpn_feature (models.py:517-518): p5 resized to 7 x 7 by TF1's legacy bilinear, [B, 7, 7, C] float32.  frames None:
+        of the last pass.  frames [B, H, W, 3] of the configured dtype: a backbone-only pass over them first, after which
+        the detection results and the stages past the FPN are stale (main.py --just_feat)."""
+        if frames is not None:
+            frames = np.ascontiguousarray(frames, dtype=self._np_dtype())
+            assert frames.shape == (self.batch, self.height, self.width, 3), frames.shape
+        out = np.empty((self.batch, 7, 7, self.C), dtype=np.float32)
+        _lib.check(self.lib.b2_fpn_feature(self._ctx, _lib.ptr(frames), _lib.ptr(out)), "b2_fpn_feature")
+        return out
+
+    def fpn_feature_launches(self) -> int:
+        return int(self.lib.b2_fpn_feature_launches(self._ctx))
+
+    def get_proposals(self) -> dict:
+        """proposal_boxes [B, rpn_topk, 4], proposal_scores [B, rpn_topk] and count [B] of the last pass: score descending,
+        ties to the lower position in the levels' concatenation; rows >= count[b] are not proposals."""
+        B, K = self.batch, int(self.cfg.rpn_test_post_nms_topk)
+        boxes, scores = np.empty((B, K, 4), np.float32), np.empty((B, K), np.float32)
+        count = np.empty((B,), np.int32)
+        _lib.check(self.lib.b2_get_proposals(self._ctx, _lib.ptr(boxes), _lib.ptr(scores), _lib.ptr(count)),
+                   "b2_get_proposals")
+        return dict(boxes=boxes, scores=scores, count=count)
+
+    def get_all_boxes(self, image: int = 0) -> dict:
+        """The use_cpu_nms outputs of image `image` of the last pass (models.py:899-916), K = its proposal count: boxes
+        [C - 1, K, 4] of every class, probs [C - 1, K] (softmax without the background), rois [K, 4] the proposals; C is
+        the box head's class count."""
+        K = int(self.cfg.rpn_test_post_nms_topk)
+        nc1 = (len(self.cfg.partial_class_ids) or int(self.cfg.num_class) - 1)
+        boxes, probs = np.empty(nc1 * K * 4, np.float32), np.empty(nc1 * K, np.float32)
+        rois, k = np.empty(K * 4, np.float32), np.empty((1,), np.int32)
+        _lib.check(self.lib.b2_get_all_boxes(self._ctx, int(image), _lib.ptr(boxes), _lib.ptr(probs), _lib.ptr(rois),
+                                             _lib.ptr(k)), "b2_get_all_boxes")
+        n = int(k[0])
+        return dict(boxes=boxes[:nc1 * n * 4].reshape(nc1, n, 4), probs=probs[:nc1 * n].reshape(nc1, n),
+                    rois=rois[:n * 4].reshape(n, 4))
+
     def submit_host(self, frames, out: dict, slot: int, feat_mode: int = 0, want_feat: bool = True):
         """Asynchronous detect_host: enqueue upload + pass + download for `slot` (0/1) and return; `frames` and the
         arrays of `out` must stay alive (pinned for real overlap) until wait(slot).  Streaming drivers alternate slots
