@@ -139,6 +139,22 @@ typedef struct b2_config_ext4 {
   int32_t use_so_score_thres;      /* --use_so_score_thres: the final NMS keeps logit > result_score_thres only */
 } b2_config_ext4;
 
+/* Graph options added after b2_config_ext4's layout was fixed.  b2_create_ex5 takes them; b2_create_ex4 builds the graph
+ * with every field 0. */
+typedef struct b2_config_ext5 {
+  int32_t use_bg_score;            /* main.py --use_bg_score: fastrcnn_predictions (models.py:1263-1270) first drops every
+                                      ROI whose argmax over the class probabilities is column 0 (background; ties go to
+                                      the lowest column, a NaN never wins), then runs the per-class NMS and top-k over the
+                                      kept rows.  As in the reference, a detection's box is then its class's decoded box
+                                      of ROI j, j = the selected ROI's rank among the kept rows, not of the selected ROI
+                                      itself (models.py:925-930: gather_nd on the unfiltered boxes); its label and
+                                      probability are the selected ROI's, and fpn_box_feat / final_masks follow the box.
+                                      The small-object branch's final selection filters the same way over its rebuilt
+                                      logits (models.py:885-889).  Stages "bg_rank" [B][rpn_topk] and, with the branch,
+                                      "so_bg_rank" [result_per_im] hold each row's rank, -1 when dropped.  Ignored with
+                                      multi_semantics: the batch graph has no filter (models.py:2924-2976) */
+} b2_config_ext5;
+
 const char* b2_last_error(void);
 int b2_version(void);
 
@@ -155,6 +171,9 @@ int b2_create_ex3(b2_ctx** out, int device, const b2_config* cfg, const b2_confi
  * small-object configuration the reference cannot build or this engine does not run, before touching the device */
 int b2_create_ex4(b2_ctx** out, int device, const b2_config* cfg, const b2_config_ext* ext, const b2_config_ext2* ext2,
                   const b2_config_ext3* ext3, const b2_config_ext4* ext4);
+/* b2_create_ex4 with the options of b2_config_ext5 as well; ext .. ext5 may be NULL (all 0) */
+int b2_create_ex5(b2_ctx** out, int device, const b2_config* cfg, const b2_config_ext* ext, const b2_config_ext2* ext2,
+                  const b2_config_ext3* ext3, const b2_config_ext4* ext4, const b2_config_ext5* ext5);
 void b2_destroy(b2_ctx* ctx);
 
 /* Named fp32 host arrays in the reference's Tensorpack-npz naming ("conv0/W",

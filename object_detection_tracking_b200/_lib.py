@@ -46,6 +46,10 @@ class B2ConfigExt4(ctypes.Structure):
                 ("so_person_topk", c_int32), ("use_so_score_thres", c_int32)]
 
 
+class B2ConfigExt5(ctypes.Structure):
+    _fields_ = [("use_bg_score", c_int32)]
+
+
 class B2EffdetConfig(ctypes.Structure):
     _fields_ = [
         ("image_h", c_int32), ("image_w", c_int32), ("min_level", c_int32), ("max_level", c_int32),
@@ -76,6 +80,8 @@ SYMBOLS = [
                               POINTER(B2ConfigExt3)]),
     ("b2_create_ex4", c_int, [POINTER(c_void_p), c_int, POINTER(B2Config), POINTER(B2ConfigExt), POINTER(B2ConfigExt2),
                               POINTER(B2ConfigExt3), POINTER(B2ConfigExt4)]),
+    ("b2_create_ex5", c_int, [POINTER(c_void_p), c_int, POINTER(B2Config), POINTER(B2ConfigExt), POINTER(B2ConfigExt2),
+                              POINTER(B2ConfigExt3), POINTER(B2ConfigExt4), POINTER(B2ConfigExt5)]),
     ("b2_get_small_objects", c_int, [c_void_p] + [c_void_p] * 6),
     ("b2_fpn_feature", c_int, [c_void_p, c_void_p, c_void_p]),
     ("b2_fpn_feature_launches", c_int, [c_void_p]),
@@ -313,4 +319,11 @@ def make_config_ext4(cfg) -> B2ConfigExt4:
     e.so_person_class_id = int(cfg.so_person_class_id)
     e.so_person_topk = int(cfg.so_person_topk)
     e.use_so_score_thres = int(bool(cfg.use_so_score_thres))
+    return e
+
+
+def make_config_ext5(cfg) -> B2ConfigExt5:
+    """The options of the namespace that b2_config_ext5 carries."""
+    e = B2ConfigExt5()
+    e.use_bg_score = int(bool(getattr(cfg, "use_bg_score", False)))
     return e

@@ -86,7 +86,13 @@ class Mask_RCNN_FPN:
     """Single-image model object (reference: models.py:266-1813, inference surface only).  With use_partial_classes the
     checkpoint (or frozen graph) is the 81-class COCO model; the engine keeps the box-head columns of
     config.partial_class_ids and final_labels are 1..len(partial_classes), as the driver's partial targetid2class reads
-    them (obj_detect_tracking.py:287-291).  final_masks keep the reference's channel choice (DESIGN.md section 4)."""
+    them (obj_detect_tracking.py:287-291).  final_masks keep the reference's channel choice (DESIGN.md section 4).
+
+    With config.use_bg_score (main.py --use_bg_score) the box selection and the small-object branch's drop the ROIs whose
+    argmax is background first, and keep the reference's gather of the unfiltered boxes at the filtered index (DESIGN.md
+    section 4).  A model loaded from a frozen graph follows the caller's config here too: the .pb reader reads only the
+    weights, so it cannot tell whether the graph was exported with the flag.  Mask_RCNN_FPN_multi ignores the flag, as the
+    batch graph does (models.py:2924-2976)."""
 
     is_multi = False
 

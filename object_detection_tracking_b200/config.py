@@ -65,6 +65,9 @@ _DEFAULTS = dict(
     use_so_score_thres=False,          # --use_so_score_thres (:264): the branch's final NMS filters logit > thres
     so_person_topk=10,                 # --so_person_topk (:274): reference person boxes of the association
     small_objects=None,                # class names, in so label order; None = class_ids.SMALL_OBJECTS (main.py:506-507)
+    use_bg_score=False,                # main.py --use_bg_score (:171): the single-image graph's fastrcnn_predictions drops the
+                                       # ROIs whose argmax is background before its NMS (models.py:1263-1270); the batch
+                                       # graph ignores it
     use_cpu_nms=False,                 # main.py --use_cpu_nms, set by --no_nms / --save_all_box (:493-497): the single-image
                                        # graph returns every proposal's boxes and probabilities of every class instead of
                                        # the NMS outputs (models.py:899-916)

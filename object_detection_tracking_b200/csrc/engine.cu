@@ -123,6 +123,7 @@ struct b2_ctx {
   b2_config_ext2 ext2;     // and after b2_config_ext's (b2_create_ex2)
   b2_config_ext3 ext3;     // and after b2_config_ext2's (b2_create_ex3)
   b2_config_ext4 ext4;     // and after b2_config_ext3's (b2_create_ex4)
+  b2_config_ext5 ext5;     // and after b2_config_ext4's (b2_create_ex5)
   int device = 0, num_sms = 132;
   cudaStream_t stream = nullptr;
   // geometry
@@ -255,6 +256,7 @@ int add_small_objects(b2_ctx* c, const ConvLayer* fc6, const ConvLayer* fc7) {
   sel.probs = sp.sel_probs; sel.dec_boxes = sp.sel_boxes; sel.num_class = C + 2;
   sel.score_thresh = -INFINITY;   // nms_return_boxes / the person NMS have no score threshold (models.py:1240-1250, 654-656)
   sel.max_per_class = R; sel.cls_keep = keep; sel.cls_count = sel_count;
+  sel.bg_rank = nullptr;          // nms_return_boxes has no background filter (models.py:1240-1250)
   HeadPostParams psel = sel;
   psel.max_per_class = std::max(Tp, 1); psel.cls_keep = pkeep;
   Step& s1 = add_batch_step(P, 6, kStepSoSelect, "", [c, sel, psel](int, int, cudaStream_t st) {
@@ -312,10 +314,16 @@ int add_small_objects(b2_ctx* c, const ConvLayer* fc6, const ConvLayer* fc7) {
   fin.final_count = P.arena.alloc<int>(1);
   B2_CHECK(cls && sp.fin_logits && sp.fin_boxes && fin.cls_keep && fin.cls_count && fin.final_boxes && fin.final_probs &&
                fin.final_labels && fin.final_count, "out of device memory (small-object outputs)");
+  // use_bg_score: the branch's fastrcnn_predictions filters too, on the argmax of the rebuilt logits (models.py:885-889)
+  if (c->post.bg_rank) {
+    fin.bg_rank = P.arena.alloc<int>(R);
+    B2_CHECK(fin.bg_rank, "out of device memory (small-object background filter)");
+    P.stages.raw("so_bg_rank", fin.bg_rank, Stage::kI32, R, 1, 1, 1);
+  }
   add_batch_step(P, 6, kStepSoFinish, "", [c](int, int, cudaStream_t st) {
     if (so_finish_launch(c->so, st)) return -1;
     return head_select_launch(c->so_fin, st);
-  }, 3);
+  }, fin.bg_rank ? 4 : 3);
   P.stages.raw("so_sel_probs", sp.sel_probs, Stage::kF32, K, C + 2, 1, 1);
   P.stages.raw("so_sel_boxes", sp.sel_boxes, Stage::kF32, K, C + 1, 4, 1);
   P.stages.raw("so_sel_count", sel_count, Stage::kI32, C + 1, 1, 1, 1);
@@ -674,7 +682,15 @@ int build_plan(b2_ctx* c) {
   hp.final_probs = P.arena.alloc<float>(static_cast<size_t>(B) * R);
   hp.final_labels = P.arena.alloc<int>(static_cast<size_t>(B) * R);
   hp.final_count = P.arena.alloc<int>(B);
-  add_batch_step(P, 6, kStepHeadPost, "", [c](int, int, cudaStream_t st) { return head_post_launch(c->post, st); }, 3);
+  // use_bg_score (models.py:1263-1270): the single-image graph's fastrcnn_predictions drops background-argmax rows; the
+  // batch graph's combined NMS (models.py:2924-2976) has no such filter
+  if (c->ext5.use_bg_score && !cfg.multi_semantics) {
+    hp.bg_rank = P.arena.alloc<int>(static_cast<size_t>(M));
+    B2_CHECK(hp.bg_rank, "out of device memory (background filter)");
+    P.stages.raw("bg_rank", hp.bg_rank, Stage::kI32, B, K, 1, 1);
+  }
+  add_batch_step(P, 6, kStepHeadPost, "", [c](int, int, cudaStream_t st) { return head_post_launch(c->post, st); },
+                 hp.bg_rank ? 4 : 3);
   P.stages.raw("probs", hp.probs, Stage::kF32, B, K, ncls, 1);
   P.stages.raw("dec_boxes", hp.dec_boxes, Stage::kF32, B, K, nc1, 4);
   P.stages.raw("final_boxes", hp.final_boxes, Stage::kF32, B, R, 4, 1);
@@ -800,6 +816,11 @@ int b2_create_ex3(b2_ctx** out, int device, const b2_config* cfg, const b2_confi
 
 int b2_create_ex4(b2_ctx** out, int device, const b2_config* cfg, const b2_config_ext* ext, const b2_config_ext2* ext2,
                   const b2_config_ext3* ext3, const b2_config_ext4* ext4) {
+  return b2_create_ex5(out, device, cfg, ext, ext2, ext3, ext4, nullptr);
+}
+
+int b2_create_ex5(b2_ctx** out, int device, const b2_config* cfg, const b2_config_ext* ext, const b2_config_ext2* ext2,
+                  const b2_config_ext3* ext3, const b2_config_ext4* ext4, const b2_config_ext5* ext5) {
   B2_CHECK(out && cfg, "b2_create: null argument");
   *out = nullptr;
   std::unique_ptr<b2_ctx> c(new b2_ctx());
@@ -812,6 +833,8 @@ int b2_create_ex4(b2_ctx** out, int device, const b2_config* cfg, const b2_confi
   if (ext3) c->ext3 = *ext3;
   memset(&c->ext4, 0, sizeof(c->ext4));
   if (ext4) c->ext4 = *ext4;
+  memset(&c->ext5, 0, sizeof(c->ext5));
+  if (ext5) c->ext5 = *ext5;
   const int np = c->ext2.num_partial_classes;
   B2_CHECK(np >= 0 && np <= cfg->num_class - 1 && np <= 80,
            "b2_create: num_partial_classes must be 0 (off) or 1 .. min(num_class - 1, 80) (num_class " +

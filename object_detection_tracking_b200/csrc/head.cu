@@ -1,5 +1,5 @@
-// Detection post-processing on device: softmax + per-class box decode + clip, per-class NMS,
-// global top-k.  Three small kernels, no host round trip.
+// Detection post-processing on device: softmax + per-class box decode + clip, [use_bg_score's background filter,]
+// per-class NMS, global top-k.  Three (four) small kernels, no host round trip.
 //
 // Reference ops replaced: inference decode (models.py:830-843: decode_bbox_target with
 // fastrcnn_bbox_reg_weights, clip_boxes, tf.nn.softmax), fastrcnn_predictions (models.py:1258-1304)
@@ -35,6 +35,36 @@ __global__ void head_decode_kernel(const __grid_constant__ HeadPostParams p) {
     ob[c - 1] = clip_box(decode_box(lg + nc + (p.class_agnostic ? 0 : c * 4), p.reg_w, p.decode_clip, roi), p.img_w, p.img_h);
 }
 
+// grid (B), one thread per ROI: use_bg_score's filter (models.py:1263-1270).  tf.argmax over the row's num_class values,
+// restated as a scan that moves only on a strictly greater value: ties go to the lowest column, so a background value
+// equal to the best class drops the row, and a NaN never wins (an all-NaN row has argmax 0).  Kept rows get their rank
+// among the image's kept rows, in ROI order (tf.where + tf.gather); dropped rows and rows beyond the count get -1.
+__global__ void __launch_bounds__(1024) bg_filter_kernel(const __grid_constant__ HeadPostParams p) {
+  __shared__ int warp_kept[32];
+  const int b = blockIdx.x, i = threadIdx.x, lane = i & 31, w = i >> 5;
+  const int nc = p.num_class, R = p.rois_per_image;
+  bool keep = false;
+  if (i < R && i < p.roi_count[b]) {
+    const float* pr = p.probs + (static_cast<size_t>(b) * R + i) * nc;
+    float best = pr[0];
+    int arg = 0;
+    for (int c = 1; c < nc; ++c) {
+      const float v = pr[c];
+      if (v > best) {
+        best = v;
+        arg = c;
+      }
+    }
+    keep = arg != 0;
+  }
+  const uint32_t bal = __ballot_sync(0xffffffffu, keep);
+  if (lane == 0) warp_kept[w] = __popc(bal);
+  __syncthreads();
+  int rank = __popc(bal & ((1u << lane) - 1u));
+  for (int k = 0; k < w; ++k) rank += warp_kept[k];
+  if (i < R) p.bg_rank[static_cast<size_t>(b) * R + i] = keep ? rank : -1;
+}
+
 // grid (classes, B): per-class NMS over the ROIs of one image, classes c0, c0 + 1, ...
 __global__ void __launch_bounds__(512) class_nms_kernel(const __grid_constant__ HeadPostParams p, int KP, int c0) {
   extern __shared__ __align__(16) uint8_t sm[];
@@ -51,7 +81,7 @@ __global__ void __launch_bounds__(512) class_nms_kernel(const __grid_constant__ 
   __syncthreads();
   for (int i = tid; i < KP; i += blockDim.x) {
     uint64_t k = ~0ull;
-    if (i < cnt) {
+    if (i < cnt && (!p.bg_rank || p.bg_rank[static_cast<size_t>(b) * R + i] >= 0)) {
       const float pr = p.probs[(static_cast<size_t>(b) * R + i) * nc + c + 1];
       if (pr > p.score_thresh) {
         k = desc_key(pr, static_cast<uint32_t>(i));
@@ -102,8 +132,11 @@ __global__ void __launch_bounds__(1024) final_topk_kernel(const __grid_constant_
     if (j < K) {
       const uint32_t ci = static_cast<uint32_t>(keys[j] & 0xffffffffu);
       const int c = ci / R, i = ci - c * R;
+      // with the background filter the box is ROI j's, j = i's rank among the kept rows: the reference gathers the
+      // unfiltered boxes at the filtered index (models.py:925-930).  The key (c, i) sorts as (c, j) would
+      const int row = p.bg_rank ? p.bg_rank[static_cast<size_t>(b) * R + i] : i;
       reinterpret_cast<float4*>(p.final_boxes)[o] =
-          reinterpret_cast<const float4*>(p.dec_boxes)[(static_cast<size_t>(b) * R + i) * nc1 + c];
+          reinterpret_cast<const float4*>(p.dec_boxes)[(static_cast<size_t>(b) * R + row) * nc1 + c];
       p.final_probs[o] = p.probs[(static_cast<size_t>(b) * R + i) * p.num_class + c + 1];
       p.final_labels[o] = c + 1;
     } else {
@@ -154,6 +187,11 @@ int head_select_launch(const HeadPostParams& p, cudaStream_t s) {
     attr_set = true;
   }
   B2_CHECK(smem2 <= 200 * 1024, "head: too many classes for shared memory");
+  if (p.bg_rank) {
+    B2_CHECK(p.rois_per_image <= 1024, "head: at most 1024 ROIs per image");
+    bg_filter_kernel<<<p.B, (p.rois_per_image + 31) / 32 * 32, 0, s>>>(p);
+    B2_CUDA(cudaGetLastError());
+  }
   if (class_nms_launch(p, 0, nc1, s)) return -1;
   final_topk_kernel<<<p.B, 1024, smem2, s>>>(p, KP2);
   B2_CUDA(cudaGetLastError());

@@ -115,9 +115,15 @@ struct HeadPostParams {
   float* final_probs;         // [B][max_total]
   int* final_labels;          // [B][max_total]
   int* final_count;           // [B]
+  // use_bg_score (models.py:1263-1270): null = no filter.  Else [B][rois]: row i's rank j among the image's rows below
+  // roi_count[b] whose argmax over probs is not column 0, or -1 for a dropped row.  The per-class NMS skips the dropped
+  // rows, and the final top-k gathers dec_boxes at row j instead of i, as the reference's gather_nd on the unfiltered
+  // boxes does (models.py:925-930)
+  int* bg_rank;
 };
 int head_post_launch(const HeadPostParams& p, cudaStream_t s);
-// head_post_launch's selection alone, over p.probs and p.dec_boxes as they stand: per-class NMS, then the final top-k
+// head_post_launch's selection alone, over p.probs and p.dec_boxes as they stand: with p.bg_rank the background filter,
+// then per-class NMS, then the final top-k
 int head_select_launch(const HeadPostParams& p, cudaStream_t s);
 // the per-class NMS of classes c0 .. c0 + n - 1 (dec_boxes column c, probs column c + 1) alone
 int class_nms_launch(const HeadPostParams& p, int c0, int n, cudaStream_t s);

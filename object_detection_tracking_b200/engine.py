@@ -28,10 +28,11 @@ class Detector:
         self._ext2 = _lib.make_config_ext2(self.cfg)
         self._ext3 = _lib.make_config_ext3(self.cfg)
         self._ext4 = _lib.make_config_ext4(self.cfg)
+        self._ext5 = _lib.make_config_ext5(self.cfg)
         self._ctx = c_void_p(0)
-        _lib.check(self.lib.b2_create_ex4(ctypes.byref(self._ctx), self.device, ctypes.byref(self._c),
+        _lib.check(self.lib.b2_create_ex5(ctypes.byref(self._ctx), self.device, ctypes.byref(self._c),
                                           ctypes.byref(self._ext), ctypes.byref(self._ext2), ctypes.byref(self._ext3),
-                                          ctypes.byref(self._ext4)), "b2_create")
+                                          ctypes.byref(self._ext4), ctypes.byref(self._ext5)), "b2_create")
         self.R = int(self.cfg.result_per_im)
         self.C = int(self.cfg.fpn_num_channel)
         self._pinned = None
