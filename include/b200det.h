@@ -515,6 +515,24 @@ int b2_gallery_free(int device, float* dev);
 int b2_track_spatial_dist(const int32_t* frames1, const double* pts1, const int32_t* seg1, int N, const int32_t* frames2,
                           const double* pts2, const int32_t* seg2, int M, int frame_offset, double tol, double* out);
 
+/* ---- Tracklet re-linking within one video (single_video_reid.py:233-306, object_detection_tracking_b200/relink.py).
+ * q_dev [seg_q[NQ], D]: the query tracklets' crop features grouped by seg_q[NQ+1]; g_dev / seg_g[NG+1] the gallery
+ * tracklets'; both in device memory of `device`.  pairs [P][2] (host) lists (query segment, gallery segment) pairs, in any
+ * order and with repeats.  out [P] (host):
+ *   method 0 (min_all, :291-299): min over the pair's query rows a and gallery rows b of (|a|^2 + |b|^2) - 2 a.b --
+ *     torchreid's squared euclidean, NOT clamped at 0 (b2_track_pair_cost clamps, as sklearn); NaN if any distance of
+ *     the block is NaN, as torch.min;
+ *   method 1 (avg, :279-290): the same formula on the two segments' float32 means (sum in row order / count).
+ * One GEMM of all query rows x all gallery rows (split or fp16 precision, as b2_distance_matrix) and one kernel that
+ * reads each pair's block of the products only.  Refused (b2_last_error): offsets that do not start at 0 or decrease, an
+ * empty segment (the reference removes tracklets without crops before comparing, :242-261), a pair index outside
+ * [0, NQ) x [0, NG), a method other than 0 / 1, and a finite component with |x| >= 65520 ("outside the fp16-plane
+ * range").  Runs on a private non-blocking stream and returns when `out` is complete: the device inputs must be complete
+ * when it is entered. */
+int b2_tracklet_dist_dev(int device, const float* q_dev, const int32_t* seg_q, int NQ, const float* g_dev,
+                         const int32_t* seg_g, int NG, int D, const int32_t* pairs, int P, int method, int precision,
+                         float* out);
+
 /* Single-op entry used by the kernel parity tests (host pointers, NHWC activations, HWIO kernel). */
 int b2_op_conv2d(int device, const float* x, const float* w, const float* bias, const float* res, int B, int H, int W,
                  int Cin, int R, int S, int Cout, int stride, int dil, int pad_t, int pad_b, int pad_l, int pad_r,

@@ -122,6 +122,44 @@ __global__ void pair_segmin_kernel(const float* __restrict__ dots, int ld, const
   if (lane == 0) out[pair] = (r1 > r0 && c1 > c0) ? best : fill;
 }
 
+// Tracklet re-linking distance (single_video_reid.py:291-299, torchreid's unclamped squared euclidean): one warp per entry
+// p of the explicit pair list; out[p] = min over query rows r of segment pairs[p][0] and gallery columns c of segment
+// pairs[p][1] of (|a|^2 + |b|^2) - 2 a.b.  No clamp at 0, no gate, no fill (the caller refuses empty segments); NaN if any
+// distance of the block is NaN, as torch.min.  Only the pair's own block of the products is read.
+__global__ void tracklet_pair_min_kernel(const float* __restrict__ dots, int ld, const float* __restrict__ na2,
+                                         const float* __restrict__ nb2, const int* __restrict__ seg_q,
+                                         const int* __restrict__ seg_g, const int* __restrict__ pairs, int P,
+                                         float* __restrict__ out) {
+  const int p = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int lane = threadIdx.x & 31;
+  if (p >= P) return;
+  const int qi = pairs[2 * p], gi = pairs[2 * p + 1];
+  const int r0 = seg_q[qi], r1 = seg_q[qi + 1], c0 = seg_g[gi], c1 = seg_g[gi + 1];
+  float best = INFINITY;
+  for (int r = r0; r < r1; ++r) {
+    const float a2 = na2[r];
+    const float* row = dots + static_cast<size_t>(r) * ld;
+    for (int c = c0 + lane; c < c1; c += 32)
+      best = min_nan(best, __fsub_rn(__fadd_rn(a2, nb2[c]), __fmul_rn(2.f, row[c])));
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) best = min_nan(best, __shfl_xor_sync(0xffffffffu, best, o));
+  if (lane == 0) out[p] = best;
+}
+
+// torch.mean(x, 0) of each segment, restated as the float32 sum in row order divided by the row count: one thread per
+// (segment, column), mean[s][d] of rows [seg[s], seg[s+1]).  Segments are not empty (the caller refuses them).
+__global__ void segment_mean_kernel(const float* __restrict__ src, const int* __restrict__ seg, int D,
+                                    float* __restrict__ mean) {
+  const int d = blockIdx.y * blockDim.x + threadIdx.x;
+  const int s = blockIdx.x;
+  if (d >= D) return;
+  const int r0 = seg[s], r1 = seg[s + 1];
+  float sum = 0.f;
+  for (int r = r0; r < r1; ++r) sum = __fadd_rn(sum, src[static_cast<size_t>(r) * D + d]);
+  mean[static_cast<size_t>(s) * D + d] = __fdiv_rn(sum, static_cast<float>(r1 - r0));
+}
+
 }  // namespace
 
 int rows_to_planes(const float* src, int rows, int D, __half* hi, __half* lo, int ld, float* sqnorm,
@@ -146,6 +184,23 @@ int pair_segmin(const float* dots, int ld, const float* na2, const float* nb2, c
   const long long threads = static_cast<long long>(N) * M * 32;
   pair_segmin_kernel<<<static_cast<unsigned>((threads + 255) / 256), 256, 0, s>>>(dots, ld, na2, nb2, seg_a, N, seg_b, M,
                                                                                   gate, fill, out);
+  B2_CUDA(cudaGetLastError());
+  return 0;
+}
+
+int tracklet_pair_min(const float* dots, int ld, const float* na2, const float* nb2, const int* seg_q, const int* seg_g,
+                      const int* pairs, int P, float* out, cudaStream_t s) {
+  if (P <= 0) return 0;
+  const long long threads = static_cast<long long>(P) * 32;
+  tracklet_pair_min_kernel<<<static_cast<unsigned>((threads + 255) / 256), 256, 0, s>>>(dots, ld, na2, nb2, seg_q, seg_g,
+                                                                                        pairs, P, out);
+  B2_CUDA(cudaGetLastError());
+  return 0;
+}
+
+int segment_mean(const float* src, const int* seg, int S, int D, float* mean, cudaStream_t s) {
+  if (S <= 0 || D <= 0) return 0;
+  segment_mean_kernel<<<dim3(S, (D + 255) / 256), 256, 0, s>>>(src, seg, D, mean);
   B2_CUDA(cudaGetLastError());
   return 0;
 }

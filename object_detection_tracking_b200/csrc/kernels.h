@@ -397,5 +397,10 @@ int distance_finish(const float* dots, int ld, int na, int nb, int metric, const
 int pair_segmin(const float* dots, int ld, const float* na2, const float* nb2, const int* seg_a, int N, const int* seg_b,
                 int M, const unsigned char* gate, float fill, float* out, cudaStream_t s);
 int cosine_segmin(const float* dots, int ld, const int* seg_offsets, int T, int N, float* cost, cudaStream_t s);
+// out[p] = min over the block (query segment pairs[2p], gallery segment pairs[2p+1]) of (na2 + nb2) - 2 dots, unclamped
+int tracklet_pair_min(const float* dots, int ld, const float* na2, const float* nb2, const int* seg_q, const int* seg_g,
+                      const int* pairs, int P, float* out, cudaStream_t s);
+// mean [S][D] of the rows of src [seg[S]][D] per segment: float32 sum in row order / count
+int segment_mean(const float* src, const int* seg, int S, int D, float* mean, cudaStream_t s);
 
 }  // namespace b2

@@ -26,6 +26,9 @@ namespace {
 // trackers' so that the two kinds of callers do not wait on each other.
 std::map<int, GemmWs> g_pair_ws;
 std::mutex g_pair_mutex;
+// The tracklet re-linking distances' own workspaces (b2_tracklet_dist_dev), one per device.
+std::map<int, GemmWs> g_tracklet_ws;
+std::mutex g_tracklet_mutex;
 
 }  // namespace
 }  // namespace b2
@@ -99,6 +102,78 @@ int b2_track_pair_cost(int device, const float* a, const int32_t* seg_a, int N, 
 int b2_track_pair_cost_dev(int device, const float* a_dev, const int32_t* seg_a, int N, const float* b_dev,
                            const int32_t* seg_b, int M, int D, const uint8_t* gate, float fill, int precision, float* out) {
   return pair_cost_impl(device, a_dev, true, seg_a, N, b_dev, true, seg_b, M, D, gate, fill, precision, out);
+}
+
+// ---- tracklet re-linking within one video (single_video_reid.py:233-306) ----
+// Query tracklets' rows q [seg_q[NQ], D] x gallery tracklets' rows g [seg_g[NG], D], both in device memory: one GEMM of
+// all query rows against all gallery rows, then one warp per listed (query, gallery) pair reads that pair's block only.
+// method 1 first replaces every segment by its mean row (segment_mean_kernel into the workspace's fp32 buffers) and runs the
+// same path on segments of one row each.
+int b2_tracklet_dist_dev(int device, const float* q_dev, const int32_t* seg_q, int NQ, const float* g_dev,
+                         const int32_t* seg_g, int NG, int D, const int32_t* pairs, int P, int method, int precision,
+                         float* out) {
+  B2_CHECK(NQ >= 0 && NG >= 0 && P >= 0 && D > 0, "b2_tracklet_dist_dev: bad argument");
+  B2_CHECK(method == 0 || method == 1, "b2_tracklet_dist_dev: method must be 0 (min_all) or 1 (avg)");
+  if (P == 0) return 0;
+  B2_CHECK(q_dev && seg_q && g_dev && seg_g && pairs && out, "b2_tracklet_dist_dev: null argument");
+  B2_CHECK(seg_q[0] == 0 && seg_g[0] == 0, "b2_tracklet_dist_dev: segment offsets must start at 0");
+  for (int i = 0; i < NQ; ++i) {
+    B2_CHECK(seg_q[i + 1] >= seg_q[i], "b2_tracklet_dist_dev: seg_q not monotone");
+    B2_CHECK(seg_q[i + 1] > seg_q[i], "b2_tracklet_dist_dev: empty query segment " + std::to_string(i));
+  }
+  for (int j = 0; j < NG; ++j) {
+    B2_CHECK(seg_g[j + 1] >= seg_g[j], "b2_tracklet_dist_dev: seg_g not monotone");
+    B2_CHECK(seg_g[j + 1] > seg_g[j], "b2_tracklet_dist_dev: empty gallery segment " + std::to_string(j));
+  }
+  for (int p = 0; p < P; ++p)
+    B2_CHECK(pairs[2 * p] >= 0 && pairs[2 * p] < NQ && pairs[2 * p + 1] >= 0 && pairs[2 * p + 1] < NG,
+             "b2_tracklet_dist_dev: pair " + std::to_string(p) + " out of range");
+  B2_CUDA(cudaSetDevice(device));
+  const bool split = precision == 1, avg = method == 1;
+  const int Sa = avg ? NQ : seg_q[NQ], Sb = avg ? NG : seg_g[NG];
+  const int Dp = (D + 63) / 64 * 64, Np = (Sb + 15) / 16 * 16, Sp = (Sa + 127) / 128 * 128;
+  std::lock_guard<std::mutex> lock(g_tracklet_mutex);
+  GemmWs own;   // B2_NO_WS=1 (test hook): a private workspace per call
+  own.transient = true;
+  GemmWs& w = getenv("B2_NO_WS") != nullptr ? own : g_tracklet_ws[device];
+  GemmNeed need;
+  need.a = avg ? static_cast<size_t>(NQ) * D : 0;   // the mean rows
+  need.b = avg ? static_cast<size_t>(NG) * D : 0;
+  need.Sp = Sp; need.Np = Np; need.Dp = Dp;
+  need.out = P;
+  need.ints = static_cast<size_t>(NQ) + NG + 2 + (avg ? static_cast<size_t>(NQ) + NG + 2 : 0) + 2 * static_cast<size_t>(P);
+  if (w.reserve(device, need)) return -1;
+  cudaStream_t st = w.stream;
+  int* d_sq = w.d_int;
+  int* d_sg = d_sq + NQ + 1;
+  int* d_pairs = d_sg + NG + 1;
+  B2_CUDA(cudaMemcpyAsync(d_sq, seg_q, sizeof(int) * (NQ + 1), cudaMemcpyHostToDevice, st));
+  B2_CUDA(cudaMemcpyAsync(d_sg, seg_g, sizeof(int) * (NG + 1), cudaMemcpyHostToDevice, st));
+  B2_CUDA(cudaMemcpyAsync(d_pairs, pairs, sizeof(int) * 2 * P, cudaMemcpyHostToDevice, st));
+  const float* d_q = q_dev;
+  const float* d_g = g_dev;
+  const int* d_rq = d_sq;   // the segments the pair kernel reads
+  const int* d_rg = d_sg;
+  std::vector<int32_t> one_row;   // kept alive until the stream is synchronised (download)
+  if (avg) {
+    if (segment_mean(q_dev, d_sq, NQ, D, w.d_a, st) || segment_mean(g_dev, d_sg, NG, D, w.d_b, st)) return -1;
+    d_q = w.d_a;
+    d_g = w.d_b;
+    one_row.resize(std::max(NQ, NG) + 1);
+    for (size_t k = 0; k < one_row.size(); ++k) one_row[k] = static_cast<int32_t>(k);
+    int* d_iq = d_pairs + 2 * P;
+    int* d_ig = d_iq + NQ + 1;
+    B2_CUDA(cudaMemcpyAsync(d_iq, one_row.data(), sizeof(int) * (NQ + 1), cudaMemcpyHostToDevice, st));
+    B2_CUDA(cudaMemcpyAsync(d_ig, one_row.data(), sizeof(int) * (NG + 1), cudaMemcpyHostToDevice, st));
+    d_rq = d_iq;
+    d_rg = d_ig;
+  }
+  if (rows_to_planes(d_q, Sa, D, w.a_hi, w.a_lo, Dp, w.d_na2, w.d_range, st) ||
+      rows_to_planes(d_g, Sb, D, w.b_hi, w.b_lo, Dp, w.d_nb2, w.d_range, st))
+    return -1;
+  if (w.gemm(Sp, Np, Dp, split)) return -1;
+  if (tracklet_pair_min(w.d_dots, Np, w.d_na2, w.d_nb2, d_rq, d_rg, d_pairs, P, w.d_out, st)) return -1;
+  return w.download(out, static_cast<size_t>(P), "b2_tracklet_dist_dev");
 }
 
 // ---- galleries in device memory that other processes of the node can map (one process per GPU, SURVEY 8e) ----

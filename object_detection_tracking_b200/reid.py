@@ -28,6 +28,7 @@ class ReidEngine:
         self.lib = _lib.load()
         self.batch = int(batch)
         self.model = model
+        self.device = int(device)
         self.model_id, self.image_size, self.feat_dim = self.MODELS[model]
         self._ctx = c_void_p(0)
         _lib.check(self.lib.b2_reid_create_model(ctypes.byref(self._ctx), int(device), self.batch,
