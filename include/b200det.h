@@ -387,7 +387,13 @@ int b2_reid_create(b2_reid** out, int device, int batch, int precision);
 /* model 0 = osnet_x1_0 as above; model 1 = torchreid's resnet101 (torchreid/models/resnet.py:441-455, the vehicle extractor
  * of single_video_reid.py:410-415): b2_reid_embed then takes crops resized to 128x256 ([n,128,256,3] RGB uint8) and
  * returns [n,2048] (global average pool of layer4, eval mode); state_dict names "conv1.weight", "bn1.*",
- * "layer3.22.conv2.weight", "layer2.0.downsample.0.weight", ... */
+ * "layer3.22.conv2.weight", "layer2.0.downsample.0.weight", ...
+ * Models 2-6 are the rest of torchreid's OSNet family, all at 256x128 with 512-d features like model 0, each loading its
+ * own torchreid state_dict: 2 = osnet_x0_75, 3 = osnet_x0_5, 4 = osnet_x0_25 (osnet.py:537-579, channels
+ * [48,192,288,384] / [32,128,192,256] / [16,64,96,128]), 5 = osnet_ibn_x1_0 (osnet.py:582-598, InstanceNorm in conv1 and
+ * after the residual of conv2's blocks), 6 = osnet_ain_x1_0 (osnet_ain.py:524-541, InstanceNorm in conv1 and inside the
+ * residual of the OSBlockINin blocks; streams "conv2.0.conv2.3.layers.2.*", transitions "pool2.0.*" / "pool3.0.*").
+ * InstanceNorm layers load ".weight" and ".bias" only.  Any other model id fails. */
 int b2_reid_create_model(b2_reid** out, int device, int batch, int precision, int model);
 void b2_reid_destroy(b2_reid* ctx);
 int b2_reid_load_weights(b2_reid* ctx, const char* const* names, const float* const* data, const int64_t* numel, int n);
@@ -405,9 +411,10 @@ int b2_reid_embed_boxes(b2_reid* ctx, const uint8_t* frames_host, int nf, int h,
 /* Same, with the features left in device memory of the context's GPU, as b2_reid_embed_dev. */
 int b2_reid_embed_boxes_dev(b2_reid* ctx, const uint8_t* frames_host, int nf, int h, int w, const int32_t* boxes_host, int n,
                             float* feats_dev);
-int b2_reid_feat_dim(b2_reid* ctx);   /* 512 (osnet_x1_0) / 2048 (resnet101) */
+int b2_reid_feat_dim(b2_reid* ctx);   /* 512 (the OSNet models) / 2048 (resnet101) */
 int b2_reid_num_launches(b2_reid* ctx);
-/* Stage-addressable activation of the last pass as fp32 NHWC (parity tests): "conv1", "maxpool", "conv2.0", ... */
+/* Stage-addressable activation of the last pass as fp32 NHWC (parity tests): "conv1", "maxpool", "conv2.0", ...; models with
+ * InstanceNorm add "<stage>.pre_in", the IN's input, for each IN ("conv1.pre_in", "conv2.0.pre_in", ...). */
 int b2_reid_get_activation(b2_reid* ctx, const char* name, float* dst_host, int64_t capacity_bytes, int64_t shape[4]);
 
 /* ---- EfficientDet (config 3): BiFPN feature network + class/box nets + detection post-processing.
@@ -569,6 +576,10 @@ int b2_op_conv2d_view(int device, const b2_conv_view* a, const float* x, const f
 int b2_op_group_norm(int device, const float* x, const float* res, const float* gamma, const float* beta, int B,
                      int pitch_H, int pitch_W, int C, int H, int W, int off_h, int off_w, int res_H, int res_W, int res_shift,
                      int relu, int per_roi, int split, int in_place, float* out);
+/* The ReID engine's InstanceNorm2d(affine, eps 1e-5, per-image statistics) of x [B][H][W][C] (host, fp32, converted to the
+ * engine's planes; C a multiple of 64), then + res [B][H][W][C] (may be NULL), then ReLU when relu -> out [B][H][W][C]. */
+int b2_op_instance_norm(int device, const float* x, const float* res, const float* gamma, const float* beta, int B, int H,
+                        int W, int C, int relu, int split, float* out);
 /* The SE-ResNet bottleneck's squeeze-excite (nn.py:506-519) as the engine runs it: x [B][H][W][C] (host, fp32, converted to
  * the engine's planes), gate[b] = sigmoid(relu(mean_hw(x[b]) @ w1 + b1) @ w2 + b2) with w1 [C][nr], w2 [nr][C] (nr = C / 16),
  * then out = relu(x * gate[b][c] + res) in place (res [B][H][W][C], may be NULL).  gate_out [B][C] may be NULL. */

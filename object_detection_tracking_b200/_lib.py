@@ -170,6 +170,7 @@ SYMBOLS = [
     ("b2_op_conv2d", c_int, [c_int, c_void_p, c_void_p, c_void_p, c_void_p] + [c_int] * 18 + [c_void_p]),
     ("b2_op_conv2d_view", c_int, [c_int, POINTER(B2ConvView)] + [c_void_p] * 9),
     ("b2_op_group_norm", c_int, [c_int, c_void_p, c_void_p, c_void_p, c_void_p] + [c_int] * 15 + [c_void_p]),
+    ("b2_op_instance_norm", c_int, [c_int, c_void_p, c_void_p, c_void_p, c_void_p] + [c_int] * 6 + [c_void_p]),
     ("b2_op_squeeze_excite", c_int, [c_int] + [c_void_p] * 6 + [c_int] * 6 + [c_void_p, c_void_p]),
     ("b2_op_group_conv2d", c_int, [c_int, c_void_p, c_void_p, c_void_p, c_void_p] + [c_int] * 16 + [c_void_p]),
     ("b2_op_relation", c_int, [c_int] + [c_void_p] * 10 + [c_int] * 4 + [c_void_p]),

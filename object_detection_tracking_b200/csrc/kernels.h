@@ -220,6 +220,10 @@ int gated_sum4_launch(const __half* const hi[4], const __half* const lo[4], cons
                       __half* out_hi, __half* out_lo, cudaStream_t s);
 int avgpool2_launch(const __half* in_hi, const __half* in_lo, int B, int H, int W, int C, __half* out_hi,
                     __half* out_lo, cudaStream_t s);
+// InstanceNorm2d (affine, per-image statistics, eps 1e-5) of x [B][HW][C] (C a multiple of 64), then + r when r_hi is set,
+// then ReLU when relu, into y (which may not alias x or r).  gamma / beta [C] are 0 on padded channels, which stay 0.
+int instnorm_launch(const __half* x_hi, const __half* x_lo, const __half* r_hi, const __half* r_lo, int B, int HW, int C,
+                    const float* gamma, const float* beta, int relu, __half* y_hi, __half* y_lo, cudaStream_t s);
 
 // effdet.cu -- EfficientDet feature network, heads' depthwise halves, post-processing
 struct BifpnInput {

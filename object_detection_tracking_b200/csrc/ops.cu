@@ -323,6 +323,28 @@ int b2_op_group_norm(int device, const float* x, const float* res, const float* 
   return download_planes(yp.hi, yp.lo, n, out, nullptr);
 }
 
+// The ReID engine's InstanceNorm step alone (instnorm_launch): x, res, out [B][H][W][C] fp32 host, C a multiple of 64.
+int b2_op_instance_norm(int device, const float* x, const float* res, const float* gamma, const float* beta, int B, int H,
+                        int W, int C, int relu, int split, float* out) {
+  B2_CHECK(x && gamma && beta && out, "b2_op_instance_norm: null argument");
+  B2_CHECK(B >= 1 && H >= 1 && W >= 1 && C >= 64 && C % 64 == 0,
+           "b2_op_instance_norm: needs B, H, W >= 1 and C a positive multiple of 64");
+  B2_CUDA(cudaSetDevice(device));
+  const size_t n = static_cast<size_t>(B) * H * W * C;
+  Arena a;
+  const Planes xp = a.planes(B, H, W, C, split != 0);
+  const Planes yp = a.planes(B, H, W, C, split != 0);
+  const Planes rp = res ? a.planes(B, H, W, C, split != 0) : Planes();
+  float* g = upload_f32(a, gamma, C);
+  float* b = upload_f32(a, beta, C);
+  B2_CHECK(xp.hi && yp.hi && (!res || rp.hi) && g && b, "b2_op_instance_norm: out of device memory");
+  if (upload_planes(x, xp.hi, xp.lo, n, nullptr)) return -1;
+  if (res && upload_planes(res, rp.hi, rp.lo, n, nullptr)) return -1;
+  if (instnorm_launch(xp.hi, xp.lo, rp.hi, rp.lo, B, H * W, C, g, b, relu, yp.hi, yp.lo, nullptr)) return -1;
+  B2_CUDA(cudaDeviceSynchronize());
+  return download_planes(yp.hi, yp.lo, n, out, nullptr);
+}
+
 int b2_op_squeeze_excite(int device, const float* x, const float* res, const float* w1, const float* b1, const float* w2,
                          const float* b2, int B, int H, int W, int C, int nr, int split, float* out, float* gate_out) {
   B2_CHECK(x && w1 && b1 && w2 && b2 && out, "b2_op_squeeze_excite: null argument");

@@ -3,7 +3,8 @@
 //
 // Reference ops replaced (torchreid/models/osnet.py): LightConv3x3's depthwise 3x3 + BN + ReLU (:128-156),
 // ChannelGate (:162-220: global avg-pool -> fc1 -> ReLU -> fc2 -> sigmoid -> scale), the 4-stream gated sum
-// of OSBlock.forward (:262-268), AvgPool2d(2) of the transitions (:375-381), AdaptiveAvgPool2d(1) (:428).
+// of OSBlock.forward (:262-268), AvgPool2d(2) of the transitions (:375-381), AdaptiveAvgPool2d(1) (:428), and the
+// InstanceNorm2d of the IBN / AIN variants (:52,260; osnet_ain.py:42,281).
 #include "common.h"
 #include "kernels.h"
 #include "planes.cuh"
@@ -169,7 +170,107 @@ __global__ void avgpool2_kernel(const __half* __restrict__ in_hi, const __half* 
   }
 }
 
+// InstanceNorm2d(affine=True, track_running_stats=False) of osnet_ibn / osnet_ain (osnet.py:52,260; osnet_ain.py:42,281):
+// y = (x - mean_hw) / sqrt(var_hw + 1e-5) * gamma + beta per (image, channel), biased variance, then optionally + res and
+// ReLU.  One block per (image, 64-channel slab): 8 channel vectors x 64 pixel lanes.  Three passes over the slab (at most
+// 8192 pixels x 64 channels, 2 MB of planes, so passes 2 and 3 read L2): the shifted mean (each channel's first pixel
+// taken off, so a large mean loses no bits of a small spread), the squared deviations from that mean, then the apply.
+// Every sum runs in one fixed order that depends on HW alone -- the same bits for an image at any slot of any batch.
+constexpr int kInLanes = 64;
+
+__global__ void __launch_bounds__(512) instnorm_kernel(const __half* __restrict__ x_hi, const __half* __restrict__ x_lo,
+                                                       const __half* __restrict__ r_hi, const __half* __restrict__ r_lo,
+                                                       int HW, int C, const float* __restrict__ gamma,
+                                                       const float* __restrict__ beta, int relu, __half* __restrict__ y_hi,
+                                                       __half* __restrict__ y_lo) {
+  const int b = blockIdx.y, c0 = blockIdx.x * 64;
+  const int cv = threadIdx.x & 7, pl = threadIdx.x >> 3;
+  const size_t base = static_cast<size_t>(b) * HW * C + c0 + cv * 8;
+  __shared__ float red[kInLanes][65];
+  __shared__ float s_mean[64], s_scale[64];
+  float k[8], acc[8];
+  load8_early(x_hi, x_lo, base, k);   // the shift: pixel 0 of each channel
+#pragma unroll
+  for (int j = 0; j < 8; ++j) acc[j] = 0.f;
+  for (int p = pl; p < HW; p += kInLanes) {
+    float v[8];
+    load8_early(x_hi, x_lo, base + static_cast<size_t>(p) * C, v);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) acc[j] += v[j] - k[j];
+  }
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    red[pl][cv * 8 + j] = acc[j];
+    if (pl == 0) s_mean[cv * 8 + j] = k[j];
+  }
+  __syncthreads();
+  if (threadIdx.x < 64) {
+    float s = 0.f;
+    for (int i = 0; i < kInLanes; ++i) s += red[i][threadIdx.x];
+    s_mean[threadIdx.x] += s / static_cast<float>(HW);
+  }
+  __syncthreads();
+  float m[8];
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    m[j] = s_mean[cv * 8 + j];
+    acc[j] = 0.f;
+  }
+  for (int p = pl; p < HW; p += kInLanes) {
+    float v[8];
+    load8_early(x_hi, x_lo, base + static_cast<size_t>(p) * C, v);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const float d = v[j] - m[j];
+      acc[j] = fmaf(d, d, acc[j]);
+    }
+  }
+#pragma unroll
+  for (int j = 0; j < 8; ++j) red[pl][cv * 8 + j] = acc[j];
+  __syncthreads();
+  if (threadIdx.x < 64) {
+    float s = 0.f;
+    for (int i = 0; i < kInLanes; ++i) s += red[i][threadIdx.x];
+    const float var = s / static_cast<float>(HW);
+    s_scale[threadIdx.x] = gamma[c0 + threadIdx.x] / sqrtf(var + 1e-5f);
+  }
+  __syncthreads();
+  float sc[8], bt[8];
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    sc[j] = s_scale[cv * 8 + j];
+    bt[j] = __ldg(beta + c0 + cv * 8 + j);
+  }
+  for (int p = pl; p < HW; p += kInLanes) {
+    const size_t off = base + static_cast<size_t>(p) * C;
+    float v[8];
+    load8_early(x_hi, x_lo, off, v);
+#pragma unroll
+    for (int j = 0; j < 8; ++j) v[j] = fmaf(v[j] - m[j], sc[j], bt[j]);
+    if (r_hi) {
+      float r[8];
+      load8_early(r_hi, r_lo, off, r);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) v[j] += r[j];
+    }
+    if (relu) {
+#pragma unroll
+      for (int j = 0; j < 8; ++j) v[j] = fmaxf(v[j], 0.f);
+    }
+    store8(y_hi, y_lo, off, v);
+  }
+}
+
 }  // namespace
+
+int instnorm_launch(const __half* x_hi, const __half* x_lo, const __half* r_hi, const __half* r_lo, int B, int HW, int C,
+                    const float* gamma, const float* beta, int relu, __half* y_hi, __half* y_lo, cudaStream_t s) {
+  B2_CHECK(B >= 1 && HW >= 1 && C >= 64 && C % 64 == 0, "instnorm: needs B, HW >= 1 and C a multiple of 64");
+  B2_CHECK(x_hi != y_hi && (r_hi == nullptr || r_hi != y_hi), "instnorm: the output may not alias the input or residual");
+  instnorm_kernel<<<dim3(C / 64, B), 512, 0, s>>>(x_hi, x_lo, r_hi, r_lo, HW, C, gamma, beta, relu, y_hi, y_lo);
+  B2_CUDA(cudaGetLastError());
+  return 0;
+}
 
 int dwconv3x3_launch(const __half* in_hi, const __half* in_lo, int B, int H, int W, int C, const float* w,
                      const float* bias, __half* out_hi, __half* out_lo, cudaStream_t s) {

@@ -16,6 +16,11 @@
 // layer1..4 of Bottleneck blocks (1x1 -> 3x3 carrying the stride -> 1x1, BN folded, ReLU / residual in the epilogue,
 // 1x1 strided downsample on the first block of a layer) -> global avg-pool = the 2048-d feature (eval mode).
 // Every conv runs on conv_tc_kernel (wgmma); max-pool / global-average kernels are shared with OSNet.
+//
+// The rest of torchreid's OSNet family (models 2-6) builds from the same blocks through a per-model table (kOsnet):
+// the x0.75 / x0.5 / x0.25 widths (osnet.py:537-579) carry channel counts that are not multiples of 64 as zero-padded
+// planes, and osnet_ibn_x1_0 (osnet.py:582-598) / osnet_ain_x1_0 (osnet_ain.py:524-541) add InstanceNorm2d steps
+// (instnorm_launch, reid.cu) on the stem and on the blocks the table marks.
 #include <math.h>
 #include <stdlib.h>
 #include <string.h>
@@ -47,15 +52,47 @@ struct RGate {
   int creal = 0, cr = 0;
 };
 
+// InstanceNorm2d(affine) of x, then + res (when res.hi) and ReLU, into y
+struct RIn {
+  std::string prefix;      // "...IN" / "conv1.bn": .weight / .bias in the state_dict
+  Planes x, res, y;
+  float *gamma = nullptr, *beta = nullptr;   // [C], zero on padded channels
+  int creal = 0;
+  bool relu = true;
+};
+
 // ConvLayer::layout: how the torch weight is packed
 enum { kOI = 0, kStem = 1, kOIHW = 2 };   // [O][I] (1x1 OIHW or Linear), packed 7x7 stem, RxS conv OIHW
+
+// OSNet block kinds: OSBlock; OSBlock with IN after the residual add (osnet.py:270-276, IN=True); OSBlockINin, IN on
+// the bare conv3 inside the residual (osnet_ain.py:263-295)
+enum { kPlainBlock = 0, kIbnBlock = 1, kINinBlock = 2 };
+
+struct OsnetSpec {
+  const char* name;
+  int ch[4];                 // channels (osnet.py:310-334): stem, conv2, conv3, conv4 outputs
+  bool stem_in;              // conv1 is conv -> IN -> ReLU
+  int kind[3][2];            // block kind of convN.0 / convN.1
+  bool ain_names;            // osnet_ain.py's module names: convN.M.conv2.{t}.layers.{j} streams, poolN.0 transitions
+};
+
+// indexed by model id; id 1 is resnet101
+const OsnetSpec kOsnet[7] = {
+    {"osnet_x1_0", {64, 256, 384, 512}, false, {{0, 0}, {0, 0}, {0, 0}}, false},
+    {nullptr, {0, 0, 0, 0}, false, {{0, 0}, {0, 0}, {0, 0}}, false},
+    {"osnet_x0_75", {48, 192, 288, 384}, false, {{0, 0}, {0, 0}, {0, 0}}, false},
+    {"osnet_x0_5", {32, 128, 192, 256}, false, {{0, 0}, {0, 0}, {0, 0}}, false},
+    {"osnet_x0_25", {16, 64, 96, 128}, false, {{0, 0}, {0, 0}, {0, 0}}, false},
+    {"osnet_ibn_x1_0", {64, 256, 384, 512}, true, {{1, 1}, {0, 0}, {0, 0}}, false},
+    {"osnet_ain_x1_0", {64, 256, 384, 512}, true, {{2, 2}, {0, 2}, {2, 0}}, true},
+};
 
 }  // namespace
 
 struct b2_reid {
   Arena arena;                       // first member: freed after everything that refers to it
   int device = 0, num_sms = 132, B = 0;
-  int model = 0;                     // 0 osnet_x1_0, 1 resnet101
+  int model = 0;                     // 0 osnet_x1_0, 1 resnet101, 2-6 the OSNet family of kOsnet
   int in_h = 256, in_w = 128;        // crop size (h, w) the extractor resizes to
   int feat_dim = 512;
   bool split = true;
@@ -63,6 +100,7 @@ struct b2_reid {
   std::vector<std::unique_ptr<ConvLayer>> convs;
   std::vector<std::unique_ptr<RDw>> dws;
   std::vector<std::unique_ptr<RGate>> gates;
+  std::vector<std::unique_ptr<RIn>> ins;
   std::vector<Step> steps;
   StageMap named;                    // stage-addressable activations (parity tests)
   uint8_t* crops = nullptr;          // [B][in_h][in_w][3] RGB, the stem pack's input
@@ -71,7 +109,7 @@ struct b2_reid {
   int32_t* boxes = nullptr;          // [B][5] box table of the last b2_reid_embed_boxes call
   Planes stem_u, gap_planes;
   float* gap_f32 = nullptr;
-  float* feats = nullptr;      // [Bpad][512]
+  float* feats = nullptr;      // [Bpad][feat_dim]
   cudaGraphExec_t graph = nullptr;
   bool loaded = false;
 
@@ -104,17 +142,18 @@ ConvLayer* add_conv(b2_reid* c, const std::string& wname, const std::string& bn,
   return raw;
 }
 
-// conv1 7x7/2 pad 3 through the packed-operand trick of stem.cu: a 4x1 VALID conv over the packed operand
-Planes add_stem(b2_reid* c, const std::string& wname, const std::string& bn) {
+// conv1 7x7/2 pad 3 through the packed-operand trick of stem.cu: a 4x1 VALID conv over the packed operand, with `cout`
+// outputs padded to 64; BN + ReLU in the epilogue, or (bn empty, relu false) the bare conv an InstanceNorm follows
+Planes add_stem(b2_reid* c, const std::string& wname, const std::string& bn, int cout = 64, bool relu = true) {
   const int B = c->B, h1 = (c->in_h + 6 - 7) / 2 + 1, w1 = (c->in_w + 6 - 7) / 2 + 1;
   c->stem_u = c->planes(B, h1 + 3, w1, 64);
   const Planes u = c->stem_u;
   add_step(c->steps, 0, 0, "", [c, u](cudaStream_t st) {
     return stem_pack_launch(c->crops, c->B, c->in_h, c->in_w, u.hi, u.lo, u.H, u.W, st);
   });
-  Planes c1 = c->planes(B, h1, w1, 64);
+  Planes c1 = c->planes(B, h1, w1, pad64(cout));
   ConvDesc d;
-  d.R = 4; d.S = 1; d.Cout = 64; d.relu = 1;
+  d.R = 4; d.S = 1; d.Cout = cout; d.relu = relu ? 1 : 0;
   std::unique_ptr<ConvLayer> L = make_conv(c->arena, c->split, wname, d, c->stem_u, c1);
   L->bn = bn; L->cin_real = 64; L->layout = kStem;
   add_conv_step(c->steps, 0, L.get());
@@ -122,6 +161,22 @@ Planes add_stem(b2_reid* c, const std::string& wname, const std::string& bn) {
   c->named.planes("stem_u", c->stem_u);
   c->named.planes("conv1", c1);
   return c1;
+}
+
+// InstanceNorm2d(creal, affine=True) `prefix` of x, then + res (may be null) and ReLU, into new planes
+Planes add_instnorm(b2_reid* c, const std::string& prefix, const Planes& x, const Planes* res, int creal) {
+  std::unique_ptr<RIn> N(new RIn());
+  N->prefix = prefix; N->x = x; N->creal = creal;
+  if (res) N->res = *res;
+  N->y = c->planes(x.B, x.H, x.W, x.C);
+  N->gamma = c->arena.alloc<float>(x.C); N->beta = c->arena.alloc<float>(x.C);
+  const RIn* n = N.get();
+  add_step(c->steps, 0, 0, prefix, [n](cudaStream_t st) {
+    return instnorm_launch(n->x.hi, n->x.lo, n->res.hi, n->res.lo, n->x.B, n->x.H * n->x.W, n->x.C, n->gamma, n->beta,
+                           n->relu ? 1 : 0, n->y.hi, n->y.lo, st);
+  });
+  c->ins.push_back(std::move(N));
+  return n->y;
 }
 
 // maxpool 3/2 pad 1: nn.MaxPool2d(3, 2, 1) gives (H - 1) / 2 + 1 rows, the last window cut by the border when H is odd
@@ -152,8 +207,10 @@ Planes add_light(b2_reid* c, const std::string& pre, const Planes& in, int creal
   return dw->out;
 }
 
-Planes add_osblock(b2_reid* c, const std::string& pre, const Planes& x, int cin, int cout) {
-  // OSBlock (osnet.py:223-276)
+// OSBlock (osnet.py:223-276, osnet_ain.py:230-260) or OSBlockINin (osnet_ain.py:263-295) by `kind`; cin / cout are the
+// model's channel counts, the planes carry them padded to 64
+Planes add_osblock(b2_reid* c, const std::string& pre, const Planes& x, int cin, int cout, int kind = kPlainBlock,
+                   bool ain_names = false) {
   const int mid = cout / 4, midp = pad64(mid);
   Planes x1 = c->planes(x.B, x.H, x.W, midp);
   add_conv(c, pre + ".conv1.conv.weight", pre + ".conv1.bn", "", x, cin, x1, mid, true, nullptr);
@@ -161,7 +218,9 @@ Planes add_osblock(b2_reid* c, const std::string& pre, const Planes& x, int cin,
   const char* names[4] = {".conv2a", ".conv2b", ".conv2c", ".conv2d"};
   for (int k = 0; k < 4; ++k) {
     Planes t = x1;
-    if (k == 0) t = add_light(c, pre + names[k], t, mid);
+    if (ain_names)   // LightConvStream of depth k + 1 (osnet_ain.py:148-163)
+      for (int j = 0; j <= k; ++j) t = add_light(c, pre + ".conv2." + std::to_string(k) + ".layers." + std::to_string(j), t, mid);
+    else if (k == 0) t = add_light(c, pre + names[k], t, mid);
     else
       for (int j = 0; j <= k; ++j) t = add_light(c, pre + names[k] + "." + std::to_string(j), t, mid);
     s[k] = t;
@@ -192,29 +251,51 @@ Planes add_osblock(b2_reid* c, const std::string& pre, const Planes& x, int cin,
   c->gates.push_back(std::move(G));
   Planes identity = x;
   if (cin != cout) {
-    identity = c->planes(x.B, x.H, x.W, cout);
+    identity = c->planes(x.B, x.H, x.W, pad64(cout));
     add_conv(c, pre + ".downsample.conv.weight", pre + ".downsample.bn", "", x, cin, identity, cout, false, nullptr);
   }
-  Planes out = c->planes(x.B, x.H, x.W, cout);
-  add_conv(c, pre + ".conv3.conv.weight", pre + ".conv3.bn", "", x2, mid, out, cout, true, &identity);   // relu(x3 + identity)
-  return out;
+  Planes out = c->planes(x.B, x.H, x.W, pad64(cout));
+  if (kind == kPlainBlock) {
+    add_conv(c, pre + ".conv3.conv.weight", pre + ".conv3.bn", "", x2, mid, out, cout, true, &identity);   // relu(x3 + identity)
+    return out;
+  }
+  if (kind == kIbnBlock) {   // relu(IN(x3 + identity))
+    add_conv(c, pre + ".conv3.conv.weight", pre + ".conv3.bn", "", x2, mid, out, cout, false, &identity);
+    c->named.planes(pre + ".pre_in", out);
+    return add_instnorm(c, pre + ".IN", out, nullptr, cout);
+  }
+  // relu(IN(conv3(x2)) + identity), conv3 without BN or bias
+  add_conv(c, pre + ".conv3.conv.weight", "", "", x2, mid, out, cout, false, nullptr);
+  c->named.planes(pre + ".pre_in", out);
+  return add_instnorm(c, pre + ".IN", out, &identity, cout);
 }
 
 int build(b2_reid* c) {
   const int B = c->B;
+  const OsnetSpec& m = kOsnet[c->model];
   c->crops = c->arena.alloc<uint8_t>(static_cast<size_t>(B) * c->in_h * c->in_w * 3);
-  const Planes c1 = add_stem(c, "conv1.conv.weight", "conv1.bn");   // osnet.py:307
+  Planes c1;
+  if (m.stem_in) {   // ConvLayer(IN=True): conv -> InstanceNorm2d -> ReLU (osnet.py:28-61)
+    const Planes pre = add_stem(c, "conv1.conv.weight", "", m.ch[0], false);
+    c1 = add_instnorm(c, "conv1.bn", pre, nullptr, m.ch[0]);
+    c->named.planes("conv1.pre_in", pre);
+    c->named.planes("conv1", c1);
+  } else {
+    c1 = add_stem(c, "conv1.conv.weight", "conv1.bn", m.ch[0]);     // osnet.py:307
+  }
   Planes x = add_maxpool(c, c1);                                       // :308
-  const int chans[4] = {64, 256, 384, 512};
+  const int* chans = m.ch;
   for (int stage = 0; stage < 3; ++stage) {
     const std::string sn = "conv" + std::to_string(stage + 2);
-    x = add_osblock(c, sn + ".0", x, chans[stage], chans[stage + 1]);
+    x = add_osblock(c, sn + ".0", x, chans[stage], chans[stage + 1], m.kind[stage][0], m.ain_names);
     c->named.planes(sn + ".0", x);
-    x = add_osblock(c, sn + ".1", x, chans[stage + 1], chans[stage + 1]);
+    x = add_osblock(c, sn + ".1", x, chans[stage + 1], chans[stage + 1], m.kind[stage][1], m.ain_names);
     c->named.planes(sn + ".1", x);
-    if (stage < 2) {   // transition: Conv1x1 + AvgPool2d(2) (:375-381)
+    if (stage < 2) {   // transition: Conv1x1 + AvgPool2d(2) (:375-381; osnet_ain.py:336-344 names it poolN.0)
+      const std::string tn = m.ain_names ? "pool" + std::to_string(stage + 2) + ".0" : sn + ".2.0";
+      const int cr = chans[stage + 1];
       Planes t = c->planes(B, x.H, x.W, x.C);
-      add_conv(c, sn + ".2.0.conv.weight", sn + ".2.0.bn", "", x, x.C, t, x.C, true, nullptr);
+      add_conv(c, tn + ".conv.weight", tn + ".bn", "", x, cr, t, cr, true, nullptr);
       Planes q = c->planes(B, x.H / 2, x.W / 2, x.C);
       add_step(c->steps, 0, 0, "", [t, q](cudaStream_t st) {
         return avgpool2_launch(t.hi, t.lo, t.B, t.H, t.W, t.C, q.hi, q.lo, st);
@@ -224,13 +305,14 @@ int build(b2_reid* c) {
       c->named.planes(sn, x);
     }
   }
-  Planes x5 = c->planes(B, x.H, x.W, 512);
-  add_conv(c, "conv5.conv.weight", "conv5.bn", "", x, 512, x5, 512, true, nullptr);
+  const int c5 = chans[3];   // conv5 and the fc input are channels[3] wide (osnet.py:334-339); the feature stays 512
+  Planes x5 = c->planes(B, x.H, x.W, pad64(c5));
+  add_conv(c, "conv5.conv.weight", "conv5.bn", "", x, c5, x5, c5, true, nullptr);
   c->named.planes("conv5", x5);
   // global average pool -> fc + BN1d + ReLU (:428-431, fc built by _construct_fc_layer :386-405)
   const int Bp = (B + 127) / 128 * 128;
-  c->gap_f32 = c->arena.alloc<float>(static_cast<size_t>(Bp) * 512);
-  c->gap_planes = c->planes(1, 1, Bp, 512);
+  c->gap_f32 = c->arena.alloc<float>(static_cast<size_t>(Bp) * x5.C);
+  c->gap_planes = c->planes(1, 1, Bp, x5.C);
   const Planes gp = c->gap_planes;
   float* gap_f32 = c->gap_f32;
   add_step(c->steps, 0, 0, "", [x5, gp, gap_f32](cudaStream_t st) {
@@ -239,7 +321,7 @@ int build(b2_reid* c) {
   }, 0, 0, 2);
   c->feats = c->arena.alloc<float>(static_cast<size_t>(Bp) * 512);
   Planes rows = c->gap_planes; rows.W = B;
-  add_conv(c, "fc.0.weight", "fc.1", "fc.0.bias", rows, 512, Planes(), 512, true, nullptr, 1, 1, 0, c->feats, 512);
+  add_conv(c, "fc.0.weight", "fc.1", "fc.0.bias", rows, c5, Planes(), 512, true, nullptr, 1, 1, 0, c->feats, 512);
   return plan_convs(c->convs, c->split, c->num_sms);
 }
 
@@ -297,7 +379,9 @@ int b2_reid_create(b2_reid** out, int device, int batch, int precision) {
 int b2_reid_create_model(b2_reid** out, int device, int batch, int precision, int model) {
   B2_CHECK(out && batch >= 1, "b2_reid_create: bad argument");
   *out = nullptr;
-  B2_CHECK(model == 0 || model == 1, "b2_reid_create_model: model must be 0 (osnet_x1_0) or 1 (resnet101)");
+  B2_CHECK(model >= 0 && model <= 6,
+           "b2_reid_create_model: model must be 0 (osnet_x1_0), 1 (resnet101), 2 (osnet_x0_75), 3 (osnet_x0_5), "
+           "4 (osnet_x0_25), 5 (osnet_ibn_x1_0) or 6 (osnet_ain_x1_0)");
   std::unique_ptr<b2_reid> c(new b2_reid());
   c->device = device; c->B = batch; c->split = precision == 1;
   c->model = model;
@@ -321,7 +405,7 @@ void b2_reid_destroy(b2_reid* c) {
   delete c;   // plans, then the arena's device memory
 }
 
-// state_dict of torchreid's osnet_x1_0 (names as model.state_dict(): "conv2.0.conv2b.1.conv1.weight", ...)
+// state_dict of the context's torchreid model (names as model.state_dict(): "conv2.0.conv2b.1.conv1.weight", ...)
 int b2_reid_load_weights(b2_reid* c, const char* const* names, const float* const* data, const int64_t* numel, int n) {
   B2_CHECK(c && names && data && numel, "b2_reid_load_weights: null argument");
   B2_CUDA(cudaSetDevice(c->device));
@@ -332,10 +416,10 @@ int b2_reid_load_weights(b2_reid* c, const char* const* names, const float* cons
     std::vector<double> scale, shift;
     if (fold_bn(ws, L->bn, kTorchBn, 1e-5, co, scale, shift)) return -1;   // torch BatchNorm eps
     if (L->layout == kStem) {
-      // torch OIHW [64,3,7,7] -> packed stem operand order (stem.cu): k = r*64 + s*12 + ry*6 + sx*3 + c
-      const float* w = ws.get(L->name, 64 * 3 * 49);
+      // torch OIHW [co,3,7,7] -> packed stem operand order (stem.cu): k = r*64 + s*12 + ry*6 + sx*3 + c
+      const float* w = ws.get(L->name, static_cast<int64_t>(co) * 3 * 49);
       if (!w) return -1;
-      for (int o = 0; o < 64; ++o)
+      for (int o = 0; o < co; ++o)
         for (int r = 0; r < 4; ++r)
           for (int ch = 0; ch < 48; ++ch) {
             const int s4 = ch / 12, r12 = ch % 12, ry = r12 / 6, sx = (r12 % 6) / 3, cc = r12 % 3;
@@ -389,6 +473,20 @@ int b2_reid_load_weights(b2_reid* c, const char* const* names, const float* cons
     B2_CUDA(cudaMemcpyAsync(G->b1, b1, sizeof(float) * r, cudaMemcpyHostToDevice, c->stream));
     B2_CUDA(cudaMemcpyAsync(G->w2, w2, sizeof(float) * m * r, cudaMemcpyHostToDevice, c->stream));
     B2_CUDA(cudaMemcpyAsync(G->b2, b2, sizeof(float) * m, cudaMemcpyHostToDevice, c->stream));
+    B2_CUDA(cudaStreamSynchronize(c->stream));
+  }
+  for (auto& N : c->ins) {   // InstanceNorm2d affine: weight / bias only (track_running_stats=False)
+    const int C = N->x.C, cr = N->creal;
+    const float* g = ws.get(N->prefix + ".weight", cr);
+    const float* b = ws.get(N->prefix + ".bias", cr);
+    if (!g || !b) return -1;
+    std::vector<float> pg(C, 0.f), pb(C, 0.f);
+    for (int ch = 0; ch < cr; ++ch) {
+      pg[ch] = g[ch];
+      pb[ch] = b[ch];
+    }
+    B2_CUDA(cudaMemcpyAsync(N->gamma, pg.data(), sizeof(float) * C, cudaMemcpyHostToDevice, c->stream));
+    B2_CUDA(cudaMemcpyAsync(N->beta, pb.data(), sizeof(float) * C, cudaMemcpyHostToDevice, c->stream));
     B2_CUDA(cudaStreamSynchronize(c->stream));
   }
   c->loaded = true;

@@ -3,8 +3,9 @@
 `FeatureExtractor` mirrors torchreid.utils.FeatureExtractor (torchreid/feature_extractor.py:121-252): same
 constructor arguments, callable on a list of HWC RGB uint8 arrays / a single array / image paths, returns a
 `torch.Tensor [B, 512]`.  `__call__` keeps the PIL resize of the reference's transform pipeline on the host (it is the
-reference's own library call); ToTensor + Normalize + the whole OSNet-x1.0 forward run in libb200det
-(b2_reid_embed).  `extract_boxes` takes the frame and the track boxes instead and cuts, converts and resizes them on
+reference's own library call); ToTensor + Normalize + the whole network's forward run in libb200det (b2_reid_embed):
+torchreid's six OSNet person models (osnet_x1_0 / x0_75 / x0_5 / x0_25, osnet_ibn_x1_0, osnet_ain_x1_0) and the
+resnet101 vehicle model.  `extract_boxes` takes the frame and the track boxes instead and cuts, converts and resizes them on
 the GPU bit-exactly as Pillow does (b2_reid_embed_boxes).  `compute_distance_matrix` mirrors
 torchreid/distance.py:6-46.  No CPU fallback.
 """
@@ -22,7 +23,9 @@ from . import _lib
 class ReidEngine:
     """Owner of a b2_reid context for one crop batch size."""
 
-    MODELS = {"osnet_x1_0": (0, (256, 128), 512), "resnet101": (1, (128, 256), 2048)}   # id, crop (h, w), feature width
+    MODELS = {"osnet_x1_0": (0, (256, 128), 512), "resnet101": (1, (128, 256), 2048),   # id, crop (h, w), feature width
+              "osnet_x0_75": (2, (256, 128), 512), "osnet_x0_5": (3, (256, 128), 512), "osnet_x0_25": (4, (256, 128), 512),
+              "osnet_ibn_x1_0": (5, (256, 128), 512), "osnet_ain_x1_0": (6, (256, 128), 512)}
 
     def __init__(self, batch: int, device: int = 0, precision: str = "split", model: str = "osnet_x1_0"):
         self.lib = _lib.load()
@@ -54,8 +57,8 @@ class ReidEngine:
                                                  (c_int64 * n)(*[a.size for a in arrs]), n), "b2_reid_load_weights")
 
     def embed(self, crops_u8: np.ndarray) -> np.ndarray:
-        """crops_u8: [n, h, w, 3] RGB uint8 already resized to the model's crop size (256x128 osnet_x1_0, 128x256
-        resnet101), n <= batch -> [n, 512 | 2048] float32."""
+        """crops_u8: [n, h, w, 3] RGB uint8 already resized to the model's crop size (256x128 for the OSNet models,
+        128x256 resnet101), n <= batch -> [n, 512 | 2048] float32."""
         crops_u8 = np.ascontiguousarray(crops_u8, dtype=np.uint8)
         n = crops_u8.shape[0]
         assert crops_u8.shape[1:] == self.image_size + (3,), crops_u8.shape
@@ -130,18 +133,19 @@ class ReidEngine:
 
 
 class FeatureExtractor(object):
-    """torchreid/feature_extractor.py:121-252 with model_name='osnet_x1_0' (person, image_size (256, 128)) or 'resnet101'
-    (vehicle, image_size (128, 256): single_video_reid.py:404-415)."""
+    """torchreid/feature_extractor.py:121-252 with model_name one of torchreid's OSNet person models (osnet_x1_0,
+    osnet_x0_75, osnet_x0_5, osnet_x0_25, osnet_ibn_x1_0, osnet_ain_x1_0; image_size (256, 128)) or 'resnet101' (vehicle,
+    image_size (128, 256): single_video_reid.py:404-415).  Weights come from `model_path` (a torchreid checkpoint, its
+    "module." prefixes stripped) or `state_dict`."""
 
     def __init__(self, model_name="osnet_x1_0", model_path="", image_size=(256, 128),
                  pixel_mean=(0.485, 0.456, 0.406), pixel_std=(0.229, 0.224, 0.225), pixel_norm=True,
                  device="cuda", verbose=False, batch=32, precision="split", state_dict=None):
         if model_name not in ReidEngine.MODELS:
-            raise NotImplementedError("the GPU path implements osnet_x1_0 (person) and resnet101 (vehicle), the two "
-                                      "extractors the drivers build (single_video_reid.py:404-415)")
+            raise NotImplementedError("the GPU path implements %s" % ", ".join(sorted(ReidEngine.MODELS)))
         if tuple(image_size) != ReidEngine.MODELS[model_name][1] or not pixel_norm \
                 or tuple(pixel_mean) != (0.485, 0.456, 0.406) or tuple(pixel_std) != (0.229, 0.224, 0.225):
-            raise NotImplementedError("only the drivers' settings are built: 256x128 for osnet_x1_0, 128x256 for "
+            raise NotImplementedError("only the drivers' settings are built: 256x128 for the OSNet models, 128x256 for "
                                       "resnet101, ImageNet mean/std")
         dev = 0
         if isinstance(device, str) and ":" in device:

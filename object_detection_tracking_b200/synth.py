@@ -504,6 +504,123 @@ def synth_osnet_state(seed: int = 4321) -> dict:
     return out
 
 
+# torchreid's OSNet family (osnet.py:522-598, osnet_ain.py:524-541): channels, stem InstanceNorm, block kind of each
+# stage's two blocks ("plain" OSBlock, "ibn" = OSBlock with IN after the residual, "inin" = OSBlockINin) and whether the
+# module names are osnet_ain.py's (conv2.{t}.layers.{j} streams, poolN.0 transitions)
+OSNET_FAMILY = {
+    "osnet_x1_0": dict(ch=(64, 256, 384, 512), stem_in=False, kinds=(("plain",) * 2,) * 3, ain=False),
+    "osnet_x0_75": dict(ch=(48, 192, 288, 384), stem_in=False, kinds=(("plain",) * 2,) * 3, ain=False),
+    "osnet_x0_5": dict(ch=(32, 128, 192, 256), stem_in=False, kinds=(("plain",) * 2,) * 3, ain=False),
+    "osnet_x0_25": dict(ch=(16, 64, 96, 128), stem_in=False, kinds=(("plain",) * 2,) * 3, ain=False),
+    "osnet_ibn_x1_0": dict(ch=(64, 256, 384, 512), stem_in=True,
+                           kinds=(("ibn", "ibn"), ("plain", "plain"), ("plain", "plain")), ain=False),
+    "osnet_ain_x1_0": dict(ch=(64, 256, 384, 512), stem_in=True,
+                           kinds=(("inin", "inin"), ("plain", "inin"), ("inin", "plain")), ain=True),
+}
+
+
+def osnet_family_param_shapes(name: str) -> dict:
+    """Parameter / buffer names and shapes of torchreid's `name` state_dict (one of OSNET_FAMILY), minus the unused
+    classifier.  InstanceNorm2d(affine=True) layers hold only .weight and .bias."""
+    spec = OSNET_FAMILY[name]
+    ch, ain = spec["ch"], spec["ain"]
+    shapes = {}
+
+    def bn(prefix, c):
+        for k in ("weight", "bias", "running_mean", "running_var"):
+            shapes[prefix + "." + k] = (c,)
+
+    def inorm(prefix, c):
+        shapes[prefix + ".weight"] = (c,)
+        shapes[prefix + ".bias"] = (c,)
+
+    def light(prefix, c):
+        shapes[prefix + ".conv1.weight"] = (c, c, 1, 1)
+        shapes[prefix + ".conv2.weight"] = (c, 1, 3, 3)
+        bn(prefix + ".bn", c)
+
+    def osblock(prefix, cin, cout, kind):
+        mid = cout // 4
+        shapes[prefix + ".conv1.conv.weight"] = (mid, cin, 1, 1)
+        bn(prefix + ".conv1.bn", mid)
+        for t in range(4):
+            for j in range(t + 1):
+                if ain:
+                    light("%s.conv2.%d.layers.%d" % (prefix, t, j), mid)
+                else:
+                    light("%s.conv2%s" % (prefix, "abcd"[t]) + ("" if t == 0 else ".%d" % j), mid)
+        shapes[prefix + ".gate.fc1.weight"] = (mid // 16, mid, 1, 1)
+        shapes[prefix + ".gate.fc1.bias"] = (mid // 16,)
+        shapes[prefix + ".gate.fc2.weight"] = (mid, mid // 16, 1, 1)
+        shapes[prefix + ".gate.fc2.bias"] = (mid,)
+        shapes[prefix + ".conv3.conv.weight"] = (cout, mid, 1, 1)
+        if kind != "inin":
+            bn(prefix + ".conv3.bn", cout)
+        if cin != cout:
+            shapes[prefix + ".downsample.conv.weight"] = (cout, cin, 1, 1)
+            bn(prefix + ".downsample.bn", cout)
+        if kind != "plain":
+            inorm(prefix + ".IN", cout)
+
+    shapes["conv1.conv.weight"] = (ch[0], 3, 7, 7)
+    (inorm if spec["stem_in"] else bn)("conv1.bn", ch[0])
+    for s in range(3):
+        name_s = "conv%d" % (s + 2)
+        osblock(name_s + ".0", ch[s], ch[s + 1], spec["kinds"][s][0])
+        osblock(name_s + ".1", ch[s + 1], ch[s + 1], spec["kinds"][s][1])
+        if s < 2:
+            t = "pool%d.0" % (s + 2) if ain else name_s + ".2.0"
+            shapes[t + ".conv.weight"] = (ch[s + 1], ch[s + 1], 1, 1)
+            bn(t + ".bn", ch[s + 1])
+    shapes["conv5.conv.weight"] = (ch[3], ch[3], 1, 1)
+    bn("conv5.bn", ch[3])
+    shapes["fc.0.weight"] = (512, ch[3])
+    shapes["fc.0.bias"] = (512,)
+    bn("fc.1", 512)
+    return shapes
+
+
+def osnet_family_in_layers(name: str) -> list:
+    """The InstanceNorm2d scopes of `name`, in forward order: the norm layers without running statistics."""
+    shapes = osnet_family_param_shapes(name)
+    return [k[:-7] for k, s in shapes.items()
+            if k.endswith(".weight") and len(s) == 1 and k[:-7] + ".running_mean" not in shapes]
+
+
+def synth_osnet_family_state(name: str, seed: int = 4321) -> dict:
+    """Seeded float32 state_dict for `name` (one of OSNET_FAMILY), drawn as synth_osnet_state draws osnet_x1_0's, with
+    InstanceNorm gamma ~ U(0.8, 1.2) and beta ~ N(0, 0.05)."""
+    rng = np.random.default_rng(seed)
+    shapes = osnet_family_param_shapes(name)
+    in_scopes = set(osnet_family_in_layers(name))
+    out = {}
+    for k, shp in shapes.items():
+        scope = k.rsplit(".", 1)[0]
+        if scope in in_scopes:
+            v = rng.uniform(0.8, 1.2, shp) if k.endswith(".weight") else rng.standard_normal(shp) * 0.05
+        elif k.endswith("running_var"):
+            v = rng.uniform(0.6, 1.4, shp)
+        elif k.endswith("running_mean"):
+            v = rng.standard_normal(shp) * 0.1
+        elif k.endswith("conv3.bn.weight"):              # residual-branch BN: small gamma keeps the sum bounded
+            v = rng.uniform(0.1, 0.3, shp)
+        elif k.endswith("bn.weight") or k == "fc.1.weight":
+            v = rng.uniform(0.7, 1.3, shp)
+        elif k.endswith("bias"):
+            v = rng.standard_normal(shp) * 0.05
+        elif len(shp) == 4 and shp[1] == 1:              # depthwise 3x3: fan_in 9
+            v = rng.standard_normal(shp) * np.sqrt(1.0 / 9)
+        elif len(shp) >= 2:
+            fan_in = int(np.prod(shp[1:]))
+            relu_follows = k.endswith("conv1.conv.weight") or k.endswith(".2.0.conv.weight") \
+                or (k.startswith("pool") and k.endswith(".0.conv.weight")) or k in ("conv5.conv.weight", "fc.0.weight")
+            v = rng.standard_normal(shp) * np.sqrt((2.0 if relu_follows else 1.0) / fan_in)
+        else:
+            v = rng.standard_normal(shp) * 0.05
+        out[k] = v.astype(np.float32)
+    return out
+
+
 def resnet101_reid_param_shapes() -> dict:
     """Parameter / buffer names and shapes of torchreid's resnet101 state_dict (torchreid/models/resnet.py:157-290,
     441-455: Bottleneck [3, 4, 23, 3], last_stride 2), minus the unused classifier."""
