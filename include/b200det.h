@@ -395,6 +395,18 @@ int b2_reid_create(b2_reid** out, int device, int batch, int precision);
  * residual of the OSBlockINin blocks; streams "conv2.0.conv2.3.layers.2.*", transitions "pool2.0.*" / "pool3.0.*").
  * InstanceNorm layers load ".weight" and ".bias" only.  Any other model id fails. */
 int b2_reid_create_model(b2_reid** out, int device, int batch, int precision, int model);
+/* Any model the engine builds, by torchreid's model name (torchreid/models/__init__.py), at crop size in_h x in_w:
+ *  - the OSNet models above at 256x128;
+ *  - resnet101 at 128x256 only;
+ *  - torchreid's other ResNets at 256x128 (torchreid's default) or 128x256 (the drivers' vehicle size): resnet18 and
+ *    resnet34 (512-d features), resnet50, resnet152, resnext50_32x4d, resnext101_32x8d, resnet50_ibn_a and
+ *    resnet50_ibn_b (2048-d), resnet50_fc512 (512-d, after fc.0 / fc.1 / ReLU).  Their state_dict names are torchreid's:
+ *    "layer1.0.conv2.weight" ([C][C/32][3][3] for the ResNeXts), "layer2.0.downsample.0.weight", IBN-a's
+ *    "layer1.0.bn1.IN.weight" / "layer1.0.bn1.BN.running_mean", IBN-b's stem "bn1.weight" / "bn1.bias" and
+ *    "layer1.2.IN.weight".
+ * Any other name or size fails, and the error lists what is built.  b2_reid_create_model(id) is this call with id's name
+ * and its size above. */
+int b2_reid_create_named(b2_reid** out, int device, int batch, int precision, const char* model, int in_h, int in_w);
 void b2_reid_destroy(b2_reid* ctx);
 int b2_reid_load_weights(b2_reid* ctx, const char* const* names, const float* const* data, const int64_t* numel, int n);
 int b2_reid_embed(b2_reid* ctx, const uint8_t* crops_host, int n, float* feats_host);
@@ -411,7 +423,7 @@ int b2_reid_embed_boxes(b2_reid* ctx, const uint8_t* frames_host, int nf, int h,
 /* Same, with the features left in device memory of the context's GPU, as b2_reid_embed_dev. */
 int b2_reid_embed_boxes_dev(b2_reid* ctx, const uint8_t* frames_host, int nf, int h, int w, const int32_t* boxes_host, int n,
                             float* feats_dev);
-int b2_reid_feat_dim(b2_reid* ctx);   /* 512 (the OSNet models) / 2048 (resnet101) */
+int b2_reid_feat_dim(b2_reid* ctx);   /* 512 (the OSNet models, resnet18 / 34, resnet50_fc512) / 2048 (the other ResNets) */
 int b2_reid_num_launches(b2_reid* ctx);
 /* Stage-addressable activation of the last pass as fp32 NHWC (parity tests): "conv1", "maxpool", "conv2.0", ...; models with
  * InstanceNorm add "<stage>.pre_in", the IN's input, for each IN ("conv1.pre_in", "conv2.0.pre_in", ...). */
@@ -580,6 +592,11 @@ int b2_op_group_norm(int device, const float* x, const float* res, const float* 
  * engine's planes; C a multiple of 64), then + res [B][H][W][C] (may be NULL), then ReLU when relu -> out [B][H][W][C]. */
 int b2_op_instance_norm(int device, const float* x, const float* res, const float* gamma, const float* beta, int B, int H,
                         int W, int C, int relu, int split, float* out);
+/* IBN-a's split norm (torchreid resnet_ibn_a.py:63-79, then the block's ReLU) as the ReID engine runs it: the InstanceNorm
+ * above of channels [0, c_norm) of x [B][H][W][C] with gamma / beta [c_norm], channels [c_norm, C) passed through, then
+ * ReLU on every channel -> out [B][H][W][C].  C a multiple of 64, c_norm a multiple of 8 in [8, C]. */
+int b2_op_instance_norm_split(int device, const float* x, const float* gamma, const float* beta, int B, int H, int W, int C,
+                              int c_norm, int split, float* out);
 /* The SE-ResNet bottleneck's squeeze-excite (nn.py:506-519) as the engine runs it: x [B][H][W][C] (host, fp32, converted to
  * the engine's planes), gate[b] = sigmoid(relu(mean_hw(x[b]) @ w1 + b1) @ w2 + b2) with w1 [C][nr], w2 [nr][C] (nr = C / 16),
  * then out = relu(x * gate[b][c] + res) in place (res [B][H][W][C], may be NULL).  gate_out [B][C] may be NULL. */

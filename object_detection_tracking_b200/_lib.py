@@ -136,6 +136,7 @@ SYMBOLS = [
     ("b2_jde_get_tracks", c_int, [c_void_p, c_int, c_int] + [c_void_p] * 12),
     ("b2_reid_create", c_int, [POINTER(c_void_p), c_int, c_int, c_int]),
     ("b2_reid_create_model", c_int, [POINTER(c_void_p), c_int, c_int, c_int, c_int]),
+    ("b2_reid_create_named", c_int, [POINTER(c_void_p), c_int, c_int, c_int, c_char_p, c_int, c_int]),
     ("b2_reid_destroy", None, [c_void_p]),
     ("b2_reid_load_weights", c_int, [c_void_p, POINTER(c_char_p), POINTER(c_void_p), POINTER(c_int64), c_int]),
     ("b2_reid_embed", c_int, [c_void_p, c_void_p, c_int, c_void_p]),
@@ -171,6 +172,7 @@ SYMBOLS = [
     ("b2_op_conv2d_view", c_int, [c_int, POINTER(B2ConvView)] + [c_void_p] * 9),
     ("b2_op_group_norm", c_int, [c_int, c_void_p, c_void_p, c_void_p, c_void_p] + [c_int] * 15 + [c_void_p]),
     ("b2_op_instance_norm", c_int, [c_int, c_void_p, c_void_p, c_void_p, c_void_p] + [c_int] * 6 + [c_void_p]),
+    ("b2_op_instance_norm_split", c_int, [c_int, c_void_p, c_void_p, c_void_p] + [c_int] * 6 + [c_void_p]),
     ("b2_op_squeeze_excite", c_int, [c_int] + [c_void_p] * 6 + [c_int] * 6 + [c_void_p, c_void_p]),
     ("b2_op_group_conv2d", c_int, [c_int, c_void_p, c_void_p, c_void_p, c_void_p] + [c_int] * 16 + [c_void_p]),
     ("b2_op_relation", c_int, [c_int] + [c_void_p] * 10 + [c_int] * 4 + [c_void_p]),

@@ -224,6 +224,10 @@ int avgpool2_launch(const __half* in_hi, const __half* in_lo, int B, int H, int 
 // then ReLU when relu, into y (which may not alias x or r).  gamma / beta [C] are 0 on padded channels, which stay 0.
 int instnorm_launch(const __half* x_hi, const __half* x_lo, const __half* r_hi, const __half* r_lo, int B, int HW, int C,
                     const float* gamma, const float* beta, int relu, __half* y_hi, __half* y_lo, cudaStream_t s);
+// IBN-a's split norm (resnet_ibn_a.py:63-79, then the block's ReLU): the same InstanceNorm of channels [0, c_norm) with
+// gamma / beta [c_norm], channels [c_norm, C) passed through, then ReLU on every channel.  c_norm a multiple of 8.
+int instnorm_split_launch(const __half* x_hi, const __half* x_lo, int B, int HW, int C, int c_norm, const float* gamma,
+                          const float* beta, __half* y_hi, __half* y_lo, cudaStream_t s);
 
 // effdet.cu -- EfficientDet feature network, heads' depthwise halves, post-processing
 struct BifpnInput {

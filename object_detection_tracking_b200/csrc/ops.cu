@@ -345,6 +345,26 @@ int b2_op_instance_norm(int device, const float* x, const float* res, const floa
   return download_planes(yp.hi, yp.lo, n, out, nullptr);
 }
 
+// IBN-a's split norm step alone (instnorm_split_launch): x, out [B][H][W][C] fp32 host, gamma / beta [c_norm].
+int b2_op_instance_norm_split(int device, const float* x, const float* gamma, const float* beta, int B, int H, int W, int C,
+                              int c_norm, int split, float* out) {
+  B2_CHECK(x && gamma && beta && out, "b2_op_instance_norm_split: null argument");
+  B2_CHECK(B >= 1 && H >= 1 && W >= 1 && C >= 64 && C % 64 == 0 && c_norm >= 8 && c_norm <= C && c_norm % 8 == 0,
+           "b2_op_instance_norm_split: needs B, H, W >= 1, C a positive multiple of 64 and c_norm a multiple of 8 in [8, C]");
+  B2_CUDA(cudaSetDevice(device));
+  const size_t n = static_cast<size_t>(B) * H * W * C;
+  Arena a;
+  const Planes xp = a.planes(B, H, W, C, split != 0);
+  const Planes yp = a.planes(B, H, W, C, split != 0);
+  float* g = upload_f32(a, gamma, c_norm);
+  float* b = upload_f32(a, beta, c_norm);
+  B2_CHECK(xp.hi && yp.hi && g && b, "b2_op_instance_norm_split: out of device memory");
+  if (upload_planes(x, xp.hi, xp.lo, n, nullptr)) return -1;
+  if (instnorm_split_launch(xp.hi, xp.lo, B, H * W, C, c_norm, g, b, yp.hi, yp.lo, nullptr)) return -1;
+  B2_CUDA(cudaDeviceSynchronize());
+  return download_planes(yp.hi, yp.lo, n, out, nullptr);
+}
+
 int b2_op_squeeze_excite(int device, const float* x, const float* res, const float* w1, const float* b1, const float* w2,
                          const float* b2, int B, int H, int W, int C, int nr, int split, float* out, float* gate_out) {
   B2_CHECK(x && w1 && b1 && w2 && b2 && out, "b2_op_squeeze_excite: null argument");

@@ -176,15 +176,19 @@ __global__ void avgpool2_kernel(const __half* __restrict__ in_hi, const __half* 
 // 8192 pixels x 64 channels, 2 MB of planes, so passes 2 and 3 read L2): the shifted mean (each channel's first pixel
 // taken off, so a large mean loses no bits of a small spread), the squared deviations from that mean, then the apply.
 // Every sum runs in one fixed order that depends on HW alone -- the same bits for an image at any slot of any batch.
+// Only channels [0, c_norm) are normalised (IBN-a's split, resnet_ibn_a.py:63-79; c_norm a multiple of 8, C for a plain
+// InstanceNorm): the others skip the statistics and pass through unchanged, then take the residual and ReLU like the rest.
 constexpr int kInLanes = 64;
 
 __global__ void __launch_bounds__(512) instnorm_kernel(const __half* __restrict__ x_hi, const __half* __restrict__ x_lo,
                                                        const __half* __restrict__ r_hi, const __half* __restrict__ r_lo,
-                                                       int HW, int C, const float* __restrict__ gamma,
+                                                       int HW, int C, int c_norm, const float* __restrict__ gamma,
                                                        const float* __restrict__ beta, int relu, __half* __restrict__ y_hi,
                                                        __half* __restrict__ y_lo) {
   const int b = blockIdx.y, c0 = blockIdx.x * 64;
   const int cv = threadIdx.x & 7, pl = threadIdx.x >> 3;
+  const bool norm = c0 + cv * 8 < c_norm;   // this thread's 8 channels are normalised
+  const int hw_norm = norm ? HW : 0;        // pixels the statistics passes read
   const size_t base = static_cast<size_t>(b) * HW * C + c0 + cv * 8;
   __shared__ float red[kInLanes][65];
   __shared__ float s_mean[64], s_scale[64];
@@ -192,7 +196,7 @@ __global__ void __launch_bounds__(512) instnorm_kernel(const __half* __restrict_
   load8_early(x_hi, x_lo, base, k);   // the shift: pixel 0 of each channel
 #pragma unroll
   for (int j = 0; j < 8; ++j) acc[j] = 0.f;
-  for (int p = pl; p < HW; p += kInLanes) {
+  for (int p = pl; p < hw_norm; p += kInLanes) {
     float v[8];
     load8_early(x_hi, x_lo, base + static_cast<size_t>(p) * C, v);
 #pragma unroll
@@ -216,7 +220,7 @@ __global__ void __launch_bounds__(512) instnorm_kernel(const __half* __restrict_
     m[j] = s_mean[cv * 8 + j];
     acc[j] = 0.f;
   }
-  for (int p = pl; p < HW; p += kInLanes) {
+  for (int p = pl; p < hw_norm; p += kInLanes) {
     float v[8];
     load8_early(x_hi, x_lo, base + static_cast<size_t>(p) * C, v);
 #pragma unroll
@@ -232,21 +236,23 @@ __global__ void __launch_bounds__(512) instnorm_kernel(const __half* __restrict_
     float s = 0.f;
     for (int i = 0; i < kInLanes; ++i) s += red[i][threadIdx.x];
     const float var = s / static_cast<float>(HW);
-    s_scale[threadIdx.x] = gamma[c0 + threadIdx.x] / sqrtf(var + 1e-5f);
+    s_scale[threadIdx.x] = c0 + static_cast<int>(threadIdx.x) < c_norm ? gamma[c0 + threadIdx.x] / sqrtf(var + 1e-5f) : 0.f;
   }
   __syncthreads();
   float sc[8], bt[8];
 #pragma unroll
   for (int j = 0; j < 8; ++j) {
     sc[j] = s_scale[cv * 8 + j];
-    bt[j] = __ldg(beta + c0 + cv * 8 + j);
+    bt[j] = norm ? __ldg(beta + c0 + cv * 8 + j) : 0.f;
   }
   for (int p = pl; p < HW; p += kInLanes) {
     const size_t off = base + static_cast<size_t>(p) * C;
     float v[8];
     load8_early(x_hi, x_lo, off, v);
+    if (norm) {
 #pragma unroll
-    for (int j = 0; j < 8; ++j) v[j] = fmaf(v[j] - m[j], sc[j], bt[j]);
+      for (int j = 0; j < 8; ++j) v[j] = fmaf(v[j] - m[j], sc[j], bt[j]);
+    }
     if (r_hi) {
       float r[8];
       load8_early(r_hi, r_lo, off, r);
@@ -267,7 +273,17 @@ int instnorm_launch(const __half* x_hi, const __half* x_lo, const __half* r_hi, 
                     const float* gamma, const float* beta, int relu, __half* y_hi, __half* y_lo, cudaStream_t s) {
   B2_CHECK(B >= 1 && HW >= 1 && C >= 64 && C % 64 == 0, "instnorm: needs B, HW >= 1 and C a multiple of 64");
   B2_CHECK(x_hi != y_hi && (r_hi == nullptr || r_hi != y_hi), "instnorm: the output may not alias the input or residual");
-  instnorm_kernel<<<dim3(C / 64, B), 512, 0, s>>>(x_hi, x_lo, r_hi, r_lo, HW, C, gamma, beta, relu, y_hi, y_lo);
+  instnorm_kernel<<<dim3(C / 64, B), 512, 0, s>>>(x_hi, x_lo, r_hi, r_lo, HW, C, C, gamma, beta, relu, y_hi, y_lo);
+  B2_CUDA(cudaGetLastError());
+  return 0;
+}
+
+int instnorm_split_launch(const __half* x_hi, const __half* x_lo, int B, int HW, int C, int c_norm, const float* gamma,
+                          const float* beta, __half* y_hi, __half* y_lo, cudaStream_t s) {
+  B2_CHECK(B >= 1 && HW >= 1 && C >= 64 && C % 64 == 0 && c_norm >= 8 && c_norm <= C && c_norm % 8 == 0,
+           "instnorm_split: needs B, HW >= 1, C a multiple of 64 and c_norm a multiple of 8 in [8, C]");
+  B2_CHECK(x_hi != y_hi, "instnorm_split: the output may not alias the input");
+  instnorm_kernel<<<dim3(C / 64, B), 512, 0, s>>>(x_hi, x_lo, nullptr, nullptr, HW, C, c_norm, gamma, beta, 1, y_hi, y_lo);
   B2_CUDA(cudaGetLastError());
   return 0;
 }

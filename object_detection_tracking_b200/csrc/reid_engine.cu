@@ -17,6 +17,12 @@
 // 1x1 strided downsample on the first block of a layer) -> global avg-pool = the 2048-d feature (eval mode).
 // Every conv runs on conv_tc_kernel (wgmma); max-pool / global-average kernels are shared with OSNet.
 //
+// resnet101 is one row of the ResNet family table (kResnet, b2_reid_create_named): resnet18 / resnet34 (BasicBlock,
+// resnet.py:52-102), resnet50 / resnet152, resnext50_32x4d / resnext101_32x8d (conv2 grouped 32 ways, on the conv kernel's
+// block-diagonal 64-channel windows), resnet50_fc512 (last stride 1, then fc 2048 -> 512 + BN1d + ReLU), resnet50_ibn_a
+// (resnet_ibn_a.py: bn1 of layer1-3 = IN of the first planes/2 channels beside BN of the rest, instnorm_split_launch) and
+// resnet50_ibn_b (resnet_ibn_b.py: IN stem, IN after the residual of layer1.2 and layer2.3).
+//
 // The rest of torchreid's OSNet family (models 2-6) builds from the same blocks through a per-model table (kOsnet):
 // the x0.75 / x0.5 / x0.25 widths (osnet.py:537-579) carry channel counts that are not multiples of 64 as zero-padded
 // planes, and osnet_ibn_x1_0 (osnet.py:582-598) / osnet_ain_x1_0 (osnet_ain.py:524-541) add InstanceNorm2d steps
@@ -25,6 +31,7 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <map>
 #include <memory>
 #include <string>
 #include <vector>
@@ -52,17 +59,20 @@ struct RGate {
   int creal = 0, cr = 0;
 };
 
-// InstanceNorm2d(affine) of x, then + res (when res.hi) and ReLU, into y
+// InstanceNorm2d(affine) of x, then + res (when res.hi) and ReLU, into y; with c_norm, IBN-a's split (channels
+// [0, c_norm) normalised, the rest passed through)
 struct RIn {
   std::string prefix;      // "...IN" / "conv1.bn": .weight / .bias in the state_dict
   Planes x, res, y;
   float *gamma = nullptr, *beta = nullptr;   // [C], zero on padded channels
-  int creal = 0;
+  int creal = 0;           // channels with a gamma / beta
+  int c_norm = 0;          // 0: every channel (instnorm_launch); else instnorm_split_launch
   bool relu = true;
 };
 
 // ConvLayer::layout: how the torch weight is packed
-enum { kOI = 0, kStem = 1, kOIHW = 2 };   // [O][I] (1x1 OIHW or Linear), packed 7x7 stem, RxS conv OIHW
+// [O][I] (1x1 OIHW or Linear), packed 7x7 stem, RxS conv OIHW, grouped RxS conv OIHW [O][I/groups][R][S]
+enum { kOI = 0, kStem = 1, kOIHW = 2, kGroupedOIHW = 3 };
 
 // OSNet block kinds: OSBlock; OSBlock with IN after the residual add (osnet.py:270-276, IN=True); OSBlockINin, IN on
 // the bare conv3 inside the residual (osnet_ain.py:263-295)
@@ -76,10 +86,8 @@ struct OsnetSpec {
   bool ain_names;            // osnet_ain.py's module names: convN.M.conv2.{t}.layers.{j} streams, poolN.0 transitions
 };
 
-// indexed by model id; id 1 is resnet101
-const OsnetSpec kOsnet[7] = {
+const OsnetSpec kOsnet[] = {
     {"osnet_x1_0", {64, 256, 384, 512}, false, {{0, 0}, {0, 0}, {0, 0}}, false},
-    {nullptr, {0, 0, 0, 0}, false, {{0, 0}, {0, 0}, {0, 0}}, false},
     {"osnet_x0_75", {48, 192, 288, 384}, false, {{0, 0}, {0, 0}, {0, 0}}, false},
     {"osnet_x0_5", {32, 128, 192, 256}, false, {{0, 0}, {0, 0}, {0, 0}}, false},
     {"osnet_x0_25", {16, 64, 96, 128}, false, {{0, 0}, {0, 0}, {0, 0}}, false},
@@ -87,12 +95,41 @@ const OsnetSpec kOsnet[7] = {
     {"osnet_ain_x1_0", {64, 256, 384, 512}, true, {{2, 2}, {0, 2}, {2, 0}}, true},
 };
 
+// torchreid's ResNet family (resnet.py:157-530, resnet_ibn_a.py:131-289, resnet_ibn_b.py:114-274)
+enum { kBasic = 0, kBottleneck = 1 };
+enum { kNoIbn = 0, kIbnA = 1, kIbnB = 2 };
+
+struct ResnetSpec {
+  const char* name;
+  int block;               // kBasic (expansion 1) or kBottleneck (expansion 4)
+  int layers[4];           // blocks of layer1..4
+  int groups, width;       // conv2's groups and width per group: a Bottleneck's conv2 is planes * width / 64 * groups wide
+  int last_stride;         // layer4's stride
+  int fc;                  // fc_dims = [fc]: Linear + BatchNorm1d + ReLU after the pool; 0 = none
+  int ibn;                 // kIbnA: bn1 of layer1-3 is IBN; kIbnB: IN stem, IN after layer1 / layer2's last residual
+  bool person;             // built at 256x128 (torchreid's default) as well as at 128x256
+};
+
+const ResnetSpec kResnet[] = {
+    {"resnet101", kBottleneck, {3, 4, 23, 3}, 1, 64, 2, 0, kNoIbn, false},
+    {"resnet18", kBasic, {2, 2, 2, 2}, 1, 64, 2, 0, kNoIbn, true},
+    {"resnet34", kBasic, {3, 4, 6, 3}, 1, 64, 2, 0, kNoIbn, true},
+    {"resnet50", kBottleneck, {3, 4, 6, 3}, 1, 64, 2, 0, kNoIbn, true},
+    {"resnet152", kBottleneck, {3, 8, 36, 3}, 1, 64, 2, 0, kNoIbn, true},
+    {"resnext50_32x4d", kBottleneck, {3, 4, 6, 3}, 32, 4, 2, 0, kNoIbn, true},
+    {"resnext101_32x8d", kBottleneck, {3, 4, 23, 3}, 32, 8, 2, 0, kNoIbn, true},
+    {"resnet50_fc512", kBottleneck, {3, 4, 6, 3}, 1, 64, 1, 512, kNoIbn, true},
+    {"resnet50_ibn_a", kBottleneck, {3, 4, 6, 3}, 1, 64, 2, 0, kIbnA, true},
+    {"resnet50_ibn_b", kBottleneck, {3, 4, 6, 3}, 1, 64, 2, 0, kIbnB, true},
+};
+
 }  // namespace
 
 struct b2_reid {
   Arena arena;                       // first member: freed after everything that refers to it
   int device = 0, num_sms = 132, B = 0;
-  int model = 0;                     // 0 osnet_x1_0, 1 resnet101, 2-6 the OSNet family of kOsnet
+  const OsnetSpec* osnet = nullptr;  // the model: a row of kOsnet or of kResnet
+  const ResnetSpec* resnet = nullptr;
   int in_h = 256, in_w = 128;        // crop size (h, w) the extractor resizes to
   int feat_dim = 512;
   bool split = true;
@@ -101,6 +138,7 @@ struct b2_reid {
   std::vector<std::unique_ptr<RDw>> dws;
   std::vector<std::unique_ptr<RGate>> gates;
   std::vector<std::unique_ptr<RIn>> ins;
+  std::map<const ConvLayer*, int> bn_from;   // IBN-a conv1: its BN covers output channels [bn_from, Cout) only
   std::vector<Step> steps;
   StageMap named;                    // stage-addressable activations (parity tests)
   uint8_t* crops = nullptr;          // [B][in_h][in_w][3] RGB, the stem pack's input
@@ -124,9 +162,9 @@ int pad64(int c) { return (c + 63) / 64 * 64; }
 // with optional BN / bias / ReLU / residual
 ConvLayer* add_conv(b2_reid* c, const std::string& wname, const std::string& bn, const std::string& bias, const Planes& in,
                     int cin_real, const Planes& out, int cout_real, bool relu, const Planes* res, int k = 1, int stride = 1,
-                    int pad = 0, float* out_f32 = nullptr, int ldc32 = 0) {
+                    int pad = 0, float* out_f32 = nullptr, int ldc32 = 0, int groups = 1) {
   ConvDesc d;
-  d.R = d.S = k; d.stride = stride;
+  d.R = d.S = k; d.stride = stride; d.groups = groups;
   d.pad_t = d.pad_l = pad;
   // stride 2 on even extents: the last window ends one row / column before torch's bottom / right padding, so
   // (pad, pad - 1) is the same convolution -- and exactly the geometry the detector's strided layers use
@@ -135,7 +173,7 @@ ConvLayer* add_conv(b2_reid* c, const std::string& wname, const std::string& bn,
   d.Cout = cout_real; d.relu = relu ? 1 : 0;
   std::unique_ptr<ConvLayer> L = make_conv(c->arena, c->split, wname, d, in, out, res, out_f32, ldc32);
   L->bn = bn; L->bias = bias; L->cin_real = cin_real;
-  L->layout = (k != 1 || stride != 1) ? kOIHW : kOI;
+  L->layout = groups > 1 ? kGroupedOIHW : (k != 1 || stride != 1) ? kOIHW : kOI;
   ConvLayer* raw = L.get();
   add_conv_step(c->steps, 0, raw);
   c->convs.push_back(std::move(L));
@@ -163,15 +201,19 @@ Planes add_stem(b2_reid* c, const std::string& wname, const std::string& bn, int
   return c1;
 }
 
-// InstanceNorm2d(creal, affine=True) `prefix` of x, then + res (may be null) and ReLU, into new planes
-Planes add_instnorm(b2_reid* c, const std::string& prefix, const Planes& x, const Planes* res, int creal) {
+// InstanceNorm2d(creal, affine=True) `prefix` of x, then + res (may be null) and ReLU, into new planes.  With c_norm:
+// IBN-a's split, the IN of channels [0, c_norm) only (creal == c_norm), the others passed through to the ReLU.
+Planes add_instnorm(b2_reid* c, const std::string& prefix, const Planes& x, const Planes* res, int creal, int c_norm = 0) {
   std::unique_ptr<RIn> N(new RIn());
-  N->prefix = prefix; N->x = x; N->creal = creal;
+  N->prefix = prefix; N->x = x; N->creal = creal; N->c_norm = c_norm;
   if (res) N->res = *res;
   N->y = c->planes(x.B, x.H, x.W, x.C);
   N->gamma = c->arena.alloc<float>(x.C); N->beta = c->arena.alloc<float>(x.C);
   const RIn* n = N.get();
   add_step(c->steps, 0, 0, prefix, [n](cudaStream_t st) {
+    if (n->c_norm)
+      return instnorm_split_launch(n->x.hi, n->x.lo, n->x.B, n->x.H * n->x.W, n->x.C, n->c_norm, n->gamma, n->beta, n->y.hi,
+                                   n->y.lo, st);
     return instnorm_launch(n->x.hi, n->x.lo, n->res.hi, n->res.lo, n->x.B, n->x.H * n->x.W, n->x.C, n->gamma, n->beta,
                            n->relu ? 1 : 0, n->y.hi, n->y.lo, st);
   });
@@ -270,9 +312,26 @@ Planes add_osblock(b2_reid* c, const std::string& pre, const Planes& x, int cin,
   return add_instnorm(c, pre + ".IN", out, &identity, cout);
 }
 
-int build(b2_reid* c) {
+// global average pool of x -> fp32 rows -> fc.0 (Linear cin_real -> dim) + fc.1 (BatchNorm1d) + ReLU into c->feats
+// (osnet.py:386-405, 428-431; resnet.py:292-320, 353-362)
+void add_gap_fc(b2_reid* c, const Planes& x5, int cin_real, int dim) {
+  const int B = c->B, Bp = (B + 127) / 128 * 128;
+  c->gap_f32 = c->arena.alloc<float>(static_cast<size_t>(Bp) * x5.C);
+  c->gap_planes = c->planes(1, 1, Bp, x5.C);
+  const Planes gp = c->gap_planes;
+  float* gap_f32 = c->gap_f32;
+  add_step(c->steps, 0, 0, "", [x5, gp, gap_f32](cudaStream_t st) {
+    if (gap_launch(x5.hi, x5.lo, x5.B, x5.H * x5.W, x5.C, gap_f32, x5.C, st)) return -1;
+    return f32_to_planes(gap_f32, gp.hi, gp.lo, static_cast<size_t>(x5.B) * x5.C, st);
+  }, 0, 0, 2);
+  c->feats = c->arena.alloc<float>(static_cast<size_t>(Bp) * dim);
+  Planes rows = c->gap_planes; rows.W = B;
+  add_conv(c, "fc.0.weight", "fc.1", "fc.0.bias", rows, cin_real, Planes(), dim, true, nullptr, 1, 1, 0, c->feats, dim);
+}
+
+int build_osnet(b2_reid* c) {
   const int B = c->B;
-  const OsnetSpec& m = kOsnet[c->model];
+  const OsnetSpec& m = *c->osnet;
   c->crops = c->arena.alloc<uint8_t>(static_cast<size_t>(B) * c->in_h * c->in_w * 3);
   Planes c1;
   if (m.stem_in) {   // ConvLayer(IN=True): conv -> InstanceNorm2d -> ReLU (osnet.py:28-61)
@@ -309,63 +368,105 @@ int build(b2_reid* c) {
   Planes x5 = c->planes(B, x.H, x.W, pad64(c5));
   add_conv(c, "conv5.conv.weight", "conv5.bn", "", x, c5, x5, c5, true, nullptr);
   c->named.planes("conv5", x5);
-  // global average pool -> fc + BN1d + ReLU (:428-431, fc built by _construct_fc_layer :386-405)
-  const int Bp = (B + 127) / 128 * 128;
-  c->gap_f32 = c->arena.alloc<float>(static_cast<size_t>(Bp) * x5.C);
-  c->gap_planes = c->planes(1, 1, Bp, x5.C);
-  const Planes gp = c->gap_planes;
-  float* gap_f32 = c->gap_f32;
-  add_step(c->steps, 0, 0, "", [x5, gp, gap_f32](cudaStream_t st) {
-    if (gap_launch(x5.hi, x5.lo, x5.B, x5.H * x5.W, x5.C, gap_f32, x5.C, st)) return -1;
-    return f32_to_planes(gap_f32, gp.hi, gp.lo, static_cast<size_t>(x5.B) * x5.C, st);
-  }, 0, 0, 2);
-  c->feats = c->arena.alloc<float>(static_cast<size_t>(Bp) * 512);
-  Planes rows = c->gap_planes; rows.W = B;
-  add_conv(c, "fc.0.weight", "fc.1", "fc.0.bias", rows, c5, Planes(), 512, true, nullptr, 1, 1, 0, c->feats, 512);
+  add_gap_fc(c, x5, c5, 512);   // global average pool -> fc + BN1d + ReLU
   return plan_convs(c->convs, c->split, c->num_sms);
 }
 
-// torchreid resnet101 (resnet.py:157-366): see the header comment.
-int build_resnet101(b2_reid* c) {
+// torchreid's ResNet family by its kResnet row (resnet.py:157-366; see the header comment).  Stage names: "conv1",
+// "maxpool", "layerN.M", "layerN", and for each InstanceNorm "<stage>.pre_in" for its input ("conv1.pre_in",
+// "layer1.2.pre_in"; IBN-a: "layerN.M.bn1.pre_in" and "layerN.M.bn1").
+int build_resnet(b2_reid* c) {
+  const ResnetSpec& m = *c->resnet;
   const int B = c->B;
   c->crops = c->arena.alloc<uint8_t>(static_cast<size_t>(B) * c->in_h * c->in_w * 3);
-  const Planes c1 = add_stem(c, "conv1.weight", "bn1");                // conv1 7x7/2 pad 3 (:211-213)
-  Planes x = add_maxpool(c, c1);                                       // maxpool 3/2 pad 1 (:216)
-  const int blocks[4] = {3, 4, 23, 3}, planes[4] = {64, 128, 256, 512};
+  Planes c1;
+  if (m.ibn == kIbnB) {   // bn1 = InstanceNorm2d(64, affine) (resnet_ibn_b.py:142)
+    const Planes pre = add_stem(c, "conv1.weight", "", 64, false);
+    c1 = add_instnorm(c, "bn1", pre, nullptr, 64);
+    c->named.planes("conv1.pre_in", pre);
+    c->named.planes("conv1", c1);
+  } else {
+    c1 = add_stem(c, "conv1.weight", "bn1");                         // conv1 7x7/2 pad 3 (:211-213)
+  }
+  Planes x = add_maxpool(c, c1);                                     // maxpool 3/2 pad 1 (:216)
+  int cin = 64;
   for (int li = 0; li < 4; ++li) {
     const std::string ln = "layer" + std::to_string(li + 1);
-    for (int bi = 0; bi < blocks[li]; ++bi) {
+    const int planes = 64 << li;
+    const int cout = m.block == kBasic ? planes : planes * 4;
+    const int width = m.block == kBasic ? planes : planes * m.width / 64 * m.groups;   // Bottleneck :122
+    for (int bi = 0; bi < m.layers[li]; ++bi) {
       const std::string pre = ln + "." + std::to_string(bi);
-      const int stride = (bi == 0 && li > 0) ? 2 : 1;                 // _make_layer :246-290 (last_stride = 2)
-      const int width = planes[li], cout = width * 4;
+      const int stride = bi > 0 || li == 0 ? 1 : li == 3 ? m.last_stride : 2;       // _make_layer :257-290
       if (stride == 2 && ((x.H | x.W) & 1)) {
-        set_error("resnet101 reid: odd feature-map extent before a stride-2 layer");
+        set_error(std::string(m.name) + " reid: odd feature-map extent before a stride-2 layer");
         return -1;
       }
       const int ho = x.H / stride, wo = x.W / stride;
-      Planes t1 = c->planes(B, x.H, x.W, width);
-      add_conv(c, pre + ".conv1.weight", pre + ".bn1", "", x, x.C, t1, t1.C, true, nullptr);
-      Planes t2 = c->planes(B, ho, wo, width);
-      add_conv(c, pre + ".conv2.weight", pre + ".bn2", "", t1, t1.C, t2, t2.C, true, nullptr, 3, stride, 1);   // stride on the 3x3 (:126)
-      Planes identity = x;
-      if (bi == 0) {                                                   // downsample: conv1x1(stride) + BN (:262-268)
-        identity = c->planes(B, ho, wo, cout);
-        add_conv(c, pre + ".downsample.0.weight", pre + ".downsample.1", "", x, x.C, identity, cout, false, nullptr, 1, stride);
-      }
+      const bool down = bi == 0 && (stride != 1 || cin != cout);    // downsample: conv1x1(stride) + BN (:264-268)
+      auto add_downsample = [&]() {
+        Planes identity = x;
+        if (down) {
+          identity = c->planes(B, ho, wo, cout);
+          add_conv(c, pre + ".downsample.0.weight", pre + ".downsample.1", "", x, x.C, identity, cout, false, nullptr, 1,
+                   stride);
+        }
+        return identity;
+      };
       Planes out = c->planes(B, ho, wo, cout);
-      add_conv(c, pre + ".conv3.weight", pre + ".bn3", "", t2, t2.C, out, cout, true, &identity);   // relu(bn3 + identity)
+      if (m.block == kBasic) {   // BasicBlock (:52-102): 3x3 carrying the stride, 3x3 with the residual
+        Planes t1 = c->planes(B, ho, wo, width);
+        add_conv(c, pre + ".conv1.weight", pre + ".bn1", "", x, x.C, t1, width, true, nullptr, 3, stride, 1);
+        const Planes identity = add_downsample();
+        add_conv(c, pre + ".conv2.weight", pre + ".bn2", "", t1, width, out, cout, true, &identity, 3, 1, 1);
+      } else {
+        Planes t1 = c->planes(B, x.H, x.W, width);
+        const bool ibn_a = m.ibn == kIbnA && li < 3;                 // resnet_ibn_a.py:198-200
+        ConvLayer* conv1 = add_conv(c, pre + ".conv1.weight", pre + (ibn_a ? ".bn1.BN" : ".bn1"), "", x, x.C, t1, width,
+                                    !ibn_a, nullptr);
+        if (ibn_a) {   // IBN (resnet_ibn_a.py:63-79): conv1's epilogue ran BN on channels [width / 2, width) only
+          c->bn_from[conv1] = width / 2;
+          c->named.planes(pre + ".bn1.pre_in", t1);
+          t1 = add_instnorm(c, pre + ".bn1.IN", t1, nullptr, width / 2, width / 2);
+          c->named.planes(pre + ".bn1", t1);
+        }
+        Planes t2 = c->planes(B, ho, wo, width);
+        add_conv(c, pre + ".conv2.weight", pre + ".bn2", "", t1, t1.C, t2, t2.C, true, nullptr, 3, stride, 1, nullptr, 0,
+                 m.groups);                                          // stride on the 3x3 (:126)
+        const Planes identity = add_downsample();
+        // resnet_ibn_b.py:106-109, 184-189: relu(IN(bn3 + identity)) in the last block of layer1 and layer2
+        const bool ibn_b = m.ibn == kIbnB && li < 2 && bi == m.layers[li] - 1;
+        add_conv(c, pre + ".conv3.weight", pre + ".bn3", "", t2, t2.C, out, cout, !ibn_b, &identity);   // relu(bn3 + identity)
+        if (ibn_b) {
+          c->named.planes(pre + ".pre_in", out);
+          out = add_instnorm(c, pre + ".IN", out, nullptr, cout);
+        }
+      }
       x = out;
+      cin = cout;
       c->named.planes(pre, x);
     }
     c->named.planes(ln, x);
   }
-  const int Bp = (B + 127) / 128 * 128;
-  c->feats = c->arena.alloc<float>(static_cast<size_t>(Bp) * c->feat_dim);
-  float* feats = c->feats;
-  add_step(c->steps, 0, 0, "", [x, feats](cudaStream_t st) {   // global_avgpool -> v (:355-359)
-    return gap_launch(x.hi, x.lo, x.B, x.H * x.W, x.C, feats, x.C, st);
-  });
+  if (m.fc) {
+    add_gap_fc(c, x, cin, m.fc);
+  } else {
+    const int Bp = (B + 127) / 128 * 128;
+    c->feats = c->arena.alloc<float>(static_cast<size_t>(Bp) * c->feat_dim);
+    float* feats = c->feats;
+    add_step(c->steps, 0, 0, "", [x, feats](cudaStream_t st) {   // global_avgpool -> v (:355-359)
+      return gap_launch(x.hi, x.lo, x.B, x.H * x.W, x.C, feats, x.C, st);
+    });
+  }
   return plan_convs(c->convs, c->split, c->num_sms);
+}
+
+// "name at HxW, ..." for every model and crop size b2_reid_create_named builds
+std::string built_models() {
+  std::string s;
+  for (const OsnetSpec& m : kOsnet) s += std::string(s.empty() ? "" : ", ") + m.name + " at 256x128";
+  for (const ResnetSpec& m : kResnet) s += std::string(", ") + m.name + (m.person ? " at 256x128 or 128x256" : " at 128x256");
+  return s;
 }
 
 }  // namespace
@@ -382,12 +483,29 @@ int b2_reid_create_model(b2_reid** out, int device, int batch, int precision, in
   B2_CHECK(model >= 0 && model <= 6,
            "b2_reid_create_model: model must be 0 (osnet_x1_0), 1 (resnet101), 2 (osnet_x0_75), 3 (osnet_x0_5), "
            "4 (osnet_x0_25), 5 (osnet_ibn_x1_0) or 6 (osnet_ain_x1_0)");
+  static const char* const kIds[7] = {"osnet_x1_0", "resnet101", "osnet_x0_75", "osnet_x0_5", "osnet_x0_25",
+                                      "osnet_ibn_x1_0", "osnet_ain_x1_0"};
+  const bool vehicle = model == 1;   // single_video_reid.py:410-415
+  return b2_reid_create_named(out, device, batch, precision, kIds[model], vehicle ? 128 : 256, vehicle ? 256 : 128);
+}
+
+int b2_reid_create_named(b2_reid** out, int device, int batch, int precision, const char* model, int in_h, int in_w) {
+  B2_CHECK(out && batch >= 1 && model, "b2_reid_create_named: bad argument");
+  *out = nullptr;
   std::unique_ptr<b2_reid> c(new b2_reid());
+  for (const OsnetSpec& m : kOsnet)
+    if (!strcmp(m.name, model)) c->osnet = &m;
+  for (const ResnetSpec& m : kResnet)
+    if (!strcmp(m.name, model)) c->resnet = &m;
+  const bool person = in_h == 256 && in_w == 128, vehicle = in_h == 128 && in_w == 256;
+  B2_CHECK(c->osnet ? person : c->resnet && (vehicle || (person && c->resnet->person)),
+           std::string("b2_reid_create_named: ") + model + " at " + std::to_string(in_h) + "x" + std::to_string(in_w) +
+               " is not built; the models are " + built_models());
   c->device = device; c->B = batch; c->split = precision == 1;
-  c->model = model;
-  if (model == 1) { c->in_h = 128; c->in_w = 256; c->feat_dim = 2048; }   // single_video_reid.py:410-415
+  c->in_h = in_h; c->in_w = in_w;
+  if (c->resnet) c->feat_dim = c->resnet->fc ? c->resnet->fc : c->resnet->block == kBasic ? 512 : 2048;
   if (open_device(device, "b2_reid_create", &c->num_sms, &c->stream)) return -1;
-  if ((model == 1 ? build_resnet101(c.get()) : build(c.get()))) { b2_reid_destroy(c.release()); return -1; }
+  if ((c->resnet ? build_resnet(c.get()) : build_osnet(c.get()))) { b2_reid_destroy(c.release()); return -1; }
   c->boxes = c->arena.alloc<int32_t>(static_cast<size_t>(batch) * 5);
   if (!c->boxes) { b2_reid_destroy(c.release()); return -1; }
   B2_CUDA(cudaDeviceSynchronize());
@@ -414,7 +532,11 @@ int b2_reid_load_weights(b2_reid* c, const char* const* names, const float* cons
     const int K = L->w.K, Cp = L->w.Cout_pad, co = L->d.Cout, ci = L->cin_real;
     std::vector<float> packed(static_cast<size_t>(Cp) * K, 0.f);
     std::vector<double> scale, shift;
-    if (fold_bn(ws, L->bn, kTorchBn, 1e-5, co, scale, shift)) return -1;   // torch BatchNorm eps
+    const auto split = c->bn_from.find(L.get());   // IBN-a: channels [0, c_bn) leave conv1 raw for the InstanceNorm
+    const int c_bn = split == c->bn_from.end() ? 0 : split->second;
+    if (fold_bn(ws, L->bn, kTorchBn, 1e-5, co - c_bn, scale, shift)) return -1;   // torch BatchNorm eps
+    scale.insert(scale.begin(), c_bn, 1.0);
+    shift.insert(shift.begin(), c_bn, 0.0);
     if (L->layout == kStem) {
       // torch OIHW [co,3,7,7] -> packed stem operand order (stem.cu): k = r*64 + s*12 + ry*6 + sx*3 + c
       const float* w = ws.get(L->name, static_cast<int64_t>(co) * 3 * 49);
@@ -427,6 +549,17 @@ int b2_reid_load_weights(b2_reid* c, const char* const* names, const float* cons
             if (rr >= 7 || ss >= 7) continue;
             packed[static_cast<size_t>(o) * K + r * 64 + ch] = static_cast<float>(w[((o * 3 + cc) * 7 + rr) * 7 + ss] * scale[o]);
           }
+    } else if (L->layout == kGroupedOIHW) {
+      // torch OIHW [co][ci/groups][R][S] -> HWIO [r*S+s][ci/groups][co] -> the conv kernel's block-diagonal windows
+      const int RS = L->d.R * L->d.S, cg = ci / L->d.groups;
+      const float* w = ws.get(L->name, static_cast<int64_t>(co) * cg * RS);
+      if (!w) return -1;
+      std::vector<float> hwio(static_cast<size_t>(RS) * cg * co);
+      for (int o = 0; o < co; ++o)
+        for (int i = 0; i < cg; ++i)
+          for (int t = 0; t < RS; ++t)
+            hwio[(static_cast<size_t>(t) * cg + i) * co + o] = w[(static_cast<size_t>(o) * cg + i) * RS + t];
+      pack_grouped(hwio.data(), RS, ci, co, L->d.groups, scale.data(), K, packed);
     } else if (L->layout == kOIHW) {
       // torch OIHW [co][ci][R][S] -> K-major [o][r][s][ci]
       const int R = L->d.R, S = L->d.S;

@@ -4,8 +4,9 @@
 constructor arguments, callable on a list of HWC RGB uint8 arrays / a single array / image paths, returns a
 `torch.Tensor [B, 512]`.  `__call__` keeps the PIL resize of the reference's transform pipeline on the host (it is the
 reference's own library call); ToTensor + Normalize + the whole network's forward run in libb200det (b2_reid_embed):
-torchreid's six OSNet person models (osnet_x1_0 / x0_75 / x0_5 / x0_25, osnet_ibn_x1_0, osnet_ain_x1_0) and the
-resnet101 vehicle model.  `extract_boxes` takes the frame and the track boxes instead and cuts, converts and resizes them on
+torchreid's six OSNet person models (osnet_x1_0 / x0_75 / x0_5 / x0_25, osnet_ibn_x1_0, osnet_ain_x1_0), the
+resnet101 vehicle model and torchreid's other ResNets (resnet18 / 34 / 50 / 152, resnext50_32x4d, resnext101_32x8d,
+resnet50_fc512, resnet50_ibn_a, resnet50_ibn_b) at 256x128 or 128x256.  `extract_boxes` takes the frame and the track boxes instead and cuts, converts and resizes them on
 the GPU bit-exactly as Pillow does (b2_reid_embed_boxes).  `compute_distance_matrix` mirrors
 torchreid/distance.py:6-46.  No CPU fallback.
 """
@@ -21,21 +22,30 @@ from . import _lib
 
 
 class ReidEngine:
-    """Owner of a b2_reid context for one crop batch size."""
+    """Owner of a b2_reid context for one crop batch size, model and crop size (`image_size` (h, w), default the model's
+    first size in MODELS)."""
 
-    MODELS = {"osnet_x1_0": (0, (256, 128), 512), "resnet101": (1, (128, 256), 2048),   # id, crop (h, w), feature width
-              "osnet_x0_75": (2, (256, 128), 512), "osnet_x0_5": (3, (256, 128), 512), "osnet_x0_25": (4, (256, 128), 512),
-              "osnet_ibn_x1_0": (5, (256, 128), 512), "osnet_ain_x1_0": (6, (256, 128), 512)}
+    _PERSON, _VEHICLE, _BOTH = ((256, 128),), ((128, 256),), ((256, 128), (128, 256))
+    MODELS = {   # torchreid model name -> (crop sizes (h, w) built, feature width)
+        "osnet_x1_0": (_PERSON, 512), "osnet_x0_75": (_PERSON, 512), "osnet_x0_5": (_PERSON, 512),
+        "osnet_x0_25": (_PERSON, 512), "osnet_ibn_x1_0": (_PERSON, 512), "osnet_ain_x1_0": (_PERSON, 512),
+        "resnet101": (_VEHICLE, 2048),
+        "resnet18": (_BOTH, 512), "resnet34": (_BOTH, 512), "resnet50": (_BOTH, 2048), "resnet152": (_BOTH, 2048),
+        "resnext50_32x4d": (_BOTH, 2048), "resnext101_32x8d": (_BOTH, 2048), "resnet50_fc512": (_BOTH, 512),
+        "resnet50_ibn_a": (_BOTH, 2048), "resnet50_ibn_b": (_BOTH, 2048)}
 
-    def __init__(self, batch: int, device: int = 0, precision: str = "split", model: str = "osnet_x1_0"):
+    def __init__(self, batch: int, device: int = 0, precision: str = "split", model: str = "osnet_x1_0",
+                 image_size=None):
         self.lib = _lib.load()
         self.batch = int(batch)
         self.model = model
         self.device = int(device)
-        self.model_id, self.image_size, self.feat_dim = self.MODELS[model]
+        sizes, self.feat_dim = self.MODELS[model]
+        self.image_size = sizes[0] if image_size is None else tuple(int(v) for v in image_size)
         self._ctx = c_void_p(0)
-        _lib.check(self.lib.b2_reid_create_model(ctypes.byref(self._ctx), int(device), self.batch,
-                                                 {"fp16": 0, "split": 1}[precision], self.model_id), "b2_reid_create_model")
+        _lib.check(self.lib.b2_reid_create_named(ctypes.byref(self._ctx), int(device), self.batch,
+                                                 {"fp16": 0, "split": 1}[precision], model.encode(), *self.image_size),
+                   "b2_reid_create_named")
 
     def close(self):
         if getattr(self, "_ctx", None) is not None and self._ctx.value:
@@ -57,8 +67,8 @@ class ReidEngine:
                                                  (c_int64 * n)(*[a.size for a in arrs]), n), "b2_reid_load_weights")
 
     def embed(self, crops_u8: np.ndarray) -> np.ndarray:
-        """crops_u8: [n, h, w, 3] RGB uint8 already resized to the model's crop size (256x128 for the OSNet models,
-        128x256 resnet101), n <= batch -> [n, 512 | 2048] float32."""
+        """crops_u8: [n, h, w, 3] RGB uint8 already resized to the engine's crop size (image_size), n <= batch ->
+        [n, feat_dim] float32."""
         crops_u8 = np.ascontiguousarray(crops_u8, dtype=np.uint8)
         n = crops_u8.shape[0]
         assert crops_u8.shape[1:] == self.image_size + (3,), crops_u8.shape
@@ -121,7 +131,8 @@ class ReidEngine:
     def get_activation(self, name: str) -> np.ndarray:
         """fp32 NHWC copy of a named intermediate of the last pass (parity tests)."""
         shape = (c_int64 * 4)()
-        cap = self.batch * 131 * 64 * 64 * 4 * (4 if self.model_id == 1 else 1) + 1024
+        h, w = self.image_size
+        cap = self.batch * (h // 2 + 3) * (w // 2) * 64 * 4 + 1024     # the stem's packed operand is the largest stage
         buf = np.empty(cap // 4, dtype=np.float32)
         _lib.check(self.lib.b2_reid_get_activation(self._ctx, name.encode(), _lib.ptr(buf), buf.nbytes, shape),
                    "b2_reid_get_activation")
@@ -134,24 +145,26 @@ class ReidEngine:
 
 class FeatureExtractor(object):
     """torchreid/feature_extractor.py:121-252 with model_name one of torchreid's OSNet person models (osnet_x1_0,
-    osnet_x0_75, osnet_x0_5, osnet_x0_25, osnet_ibn_x1_0, osnet_ain_x1_0; image_size (256, 128)) or 'resnet101' (vehicle,
-    image_size (128, 256): single_video_reid.py:404-415).  Weights come from `model_path` (a torchreid checkpoint, its
-    "module." prefixes stripped) or `state_dict`."""
+    osnet_x0_75, osnet_x0_5, osnet_x0_25, osnet_ibn_x1_0, osnet_ain_x1_0; image_size (256, 128)), 'resnet101' (vehicle,
+    image_size (128, 256): single_video_reid.py:404-415) or one of torchreid's other ResNets (resnet18, resnet34,
+    resnet50, resnet152, resnext50_32x4d, resnext101_32x8d, resnet50_fc512, resnet50_ibn_a, resnet50_ibn_b; image_size
+    (256, 128) or (128, 256)).  Weights come from `model_path` (a torchreid checkpoint, its "module." prefixes stripped)
+    or `state_dict`."""
 
     def __init__(self, model_name="osnet_x1_0", model_path="", image_size=(256, 128),
                  pixel_mean=(0.485, 0.456, 0.406), pixel_std=(0.229, 0.224, 0.225), pixel_norm=True,
                  device="cuda", verbose=False, batch=32, precision="split", state_dict=None):
         if model_name not in ReidEngine.MODELS:
             raise NotImplementedError("the GPU path implements %s" % ", ".join(sorted(ReidEngine.MODELS)))
-        if tuple(image_size) != ReidEngine.MODELS[model_name][1] or not pixel_norm \
+        if tuple(image_size) not in ReidEngine.MODELS[model_name][0] or not pixel_norm \
                 or tuple(pixel_mean) != (0.485, 0.456, 0.406) or tuple(pixel_std) != (0.229, 0.224, 0.225):
-            raise NotImplementedError("only the drivers' settings are built: 256x128 for the OSNet models, 128x256 for "
-                                      "resnet101, ImageNet mean/std")
+            raise NotImplementedError("only these settings are built: 256x128 for the OSNet models, 128x256 for "
+                                      "resnet101, 256x128 or 128x256 for torchreid's other ResNets; ImageNet mean/std")
         dev = 0
         if isinstance(device, str) and ":" in device:
             dev = int(device.split(":")[1])
         self.image_size = tuple(image_size)
-        self.engine = ReidEngine(batch, dev, precision, model_name)
+        self.engine = ReidEngine(batch, dev, precision, model_name, self.image_size)
         self.batch = batch
         if state_dict is None and model_path and os.path.isfile(model_path):
             import torch

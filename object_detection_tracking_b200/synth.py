@@ -672,6 +672,126 @@ def synth_resnet101_reid_state(seed: int = 2468) -> dict:
     return out
 
 
+# torchreid's ResNet family (resnet.py:393-530, resnet_ibn_a.py:283-289, resnet_ibn_b.py:268-274): block ("basic" /
+# "bottleneck"), blocks per layer, conv2 groups and width per group, layer4's stride, fc_dims[0] (0 = none) and the IBN
+# kind ("a": bn1 of layer1-3 is IN of the first half beside BN of the rest; "b": IN stem, IN after the residual of the
+# last block of layer1 and layer2)
+RESNET_FAMILY = {
+    "resnet18": dict(block="basic", layers=(2, 2, 2, 2), groups=1, width=64, last_stride=2, fc=0, ibn=None),
+    "resnet34": dict(block="basic", layers=(3, 4, 6, 3), groups=1, width=64, last_stride=2, fc=0, ibn=None),
+    "resnet50": dict(block="bottleneck", layers=(3, 4, 6, 3), groups=1, width=64, last_stride=2, fc=0, ibn=None),
+    "resnet101": dict(block="bottleneck", layers=(3, 4, 23, 3), groups=1, width=64, last_stride=2, fc=0, ibn=None),
+    "resnet152": dict(block="bottleneck", layers=(3, 8, 36, 3), groups=1, width=64, last_stride=2, fc=0, ibn=None),
+    "resnext50_32x4d": dict(block="bottleneck", layers=(3, 4, 6, 3), groups=32, width=4, last_stride=2, fc=0, ibn=None),
+    "resnext101_32x8d": dict(block="bottleneck", layers=(3, 4, 23, 3), groups=32, width=8, last_stride=2, fc=0,
+                             ibn=None),
+    "resnet50_fc512": dict(block="bottleneck", layers=(3, 4, 6, 3), groups=1, width=64, last_stride=1, fc=512, ibn=None),
+    "resnet50_ibn_a": dict(block="bottleneck", layers=(3, 4, 6, 3), groups=1, width=64, last_stride=2, fc=0, ibn="a"),
+    "resnet50_ibn_b": dict(block="bottleneck", layers=(3, 4, 6, 3), groups=1, width=64, last_stride=2, fc=0, ibn="b"),
+}
+
+
+def resnet_family_blocks(name: str):
+    """[(prefix, stride, cin, width, cout, downsample)] of every residual block of `name`, in forward order
+    (_make_layer, resnet.py:257-290)."""
+    spec = RESNET_FAMILY[name]
+    basic = spec["block"] == "basic"
+    out, cin = [], 64
+    for li, (n, planes) in enumerate(zip(spec["layers"], (64, 128, 256, 512))):
+        cout = planes if basic else planes * 4
+        width = planes if basic else planes * spec["width"] // 64 * spec["groups"]
+        for bi in range(n):
+            stride = 1 if bi > 0 or li == 0 else (spec["last_stride"] if li == 3 else 2)
+            out.append(("layer%d.%d" % (li + 1, bi), stride, cin, width, cout, bi == 0 and (stride != 1 or cin != cout)))
+            cin = cout
+    return out
+
+
+def resnet_family_param_shapes(name: str) -> dict:
+    """Parameter / buffer names and shapes of torchreid's `name` state_dict (one of RESNET_FAMILY), minus the unused
+    classifier.  InstanceNorm2d(affine=True) layers hold only .weight and .bias."""
+    spec = RESNET_FAMILY[name]
+    shapes = {"conv1.weight": (64, 3, 7, 7)}
+
+    def bn(prefix, c):
+        for k in ("weight", "bias", "running_mean", "running_var"):
+            shapes[prefix + "." + k] = (c,)
+
+    def inorm(prefix, c):
+        shapes[prefix + ".weight"] = (c,)
+        shapes[prefix + ".bias"] = (c,)
+
+    (inorm if spec["ibn"] == "b" else bn)("bn1", 64)
+    last = {"layer%d.%d" % (li + 1, n - 1) for li, n in enumerate(spec["layers"])}
+    for p, _, cin, width, cout, down in resnet_family_blocks(name):
+        li = int(p[5]) - 1
+        if spec["block"] == "basic":
+            shapes[p + ".conv1.weight"] = (width, cin, 3, 3)
+            bn(p + ".bn1", width)
+            shapes[p + ".conv2.weight"] = (cout, width, 3, 3)
+            bn(p + ".bn2", cout)
+        else:
+            shapes[p + ".conv1.weight"] = (width, cin, 1, 1)
+            if spec["ibn"] == "a" and li < 3:                  # IBN(planes): IN of planes // 2, BN of the rest
+                inorm(p + ".bn1.IN", width // 2)
+                bn(p + ".bn1.BN", width - width // 2)
+            else:
+                bn(p + ".bn1", width)
+            shapes[p + ".conv2.weight"] = (width, width // spec["groups"], 3, 3)
+            bn(p + ".bn2", width)
+            shapes[p + ".conv3.weight"] = (cout, width, 1, 1)
+            bn(p + ".bn3", cout)
+        if spec["ibn"] == "b" and li < 2 and p in last:
+            inorm(p + ".IN", cout)
+        if down:
+            shapes[p + ".downsample.0.weight"] = (cout, cin, 1, 1)
+            bn(p + ".downsample.1", cout)
+    if spec["fc"]:
+        cin = resnet_family_blocks(name)[-1][4]
+        shapes["fc.0.weight"] = (spec["fc"], cin)
+        shapes["fc.0.bias"] = (spec["fc"],)
+        bn("fc.1", spec["fc"])
+    return shapes
+
+
+def resnet_family_in_layers(name: str) -> list:
+    """The InstanceNorm2d scopes of `name`, in forward order: the norm layers without running statistics."""
+    shapes = resnet_family_param_shapes(name)
+    return [k[:-7] for k, s in shapes.items()
+            if k.endswith(".weight") and len(s) == 1 and k[:-7] + ".running_mean" not in shapes]
+
+
+def synth_resnet_family_state(name: str, seed: int = 2468) -> dict:
+    """Seeded float32 state_dict for `name` (one of RESNET_FAMILY), drawn as synth_resnet101_reid_state draws: the last BN
+    of every residual branch (bn3, a BasicBlock's bn2) gets a small gamma so that 36 stacked blocks keep activations O(1)
+    (fp16-plane range); InstanceNorm gamma ~ U(0.8, 1.2), beta ~ N(0, 0.05)."""
+    rng = np.random.default_rng(seed)
+    shapes = resnet_family_param_shapes(name)
+    in_scopes = set(resnet_family_in_layers(name))
+    last_bn = "bn2.weight" if RESNET_FAMILY[name]["block"] == "basic" else "bn3.weight"
+    out = {}
+    for k, shp in shapes.items():
+        if k.rsplit(".", 1)[0] in in_scopes:
+            v = rng.uniform(0.8, 1.2, shp) if k.endswith(".weight") else rng.standard_normal(shp) * 0.05
+        elif k.endswith("running_var"):
+            v = rng.uniform(0.6, 1.4, shp)
+        elif k.endswith("running_mean"):
+            v = rng.standard_normal(shp) * 0.1
+        elif k.endswith(last_bn):
+            v = rng.uniform(0.1, 0.3, shp)
+        elif k.endswith(".weight") and len(shp) == 1:
+            v = rng.uniform(0.7, 1.3, shp)
+        elif k.endswith("bias"):
+            v = rng.standard_normal(shp) * 0.05
+        else:
+            fan_in = int(np.prod(shp[1:]))
+            residual = k.endswith("conv3.weight") or "downsample" in k or (last_bn == "bn2.weight"
+                                                                           and k.endswith("conv2.weight"))
+            v = rng.standard_normal(shp) * np.sqrt((1.0 if residual else 2.0) / fan_in)
+        out[k] = v.astype(np.float32)
+    return out
+
+
 def synth_effdet_weights(cfg, seed: int = 99) -> dict:
     """Seeded weights of the EfficientDet feature network + class/box nets in the TF variable naming of
     efficientdet_arch.py (kernels HWIO, depthwise [3,3,C,1]); BN statistics non-trivial; predict biases spread
